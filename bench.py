@@ -7,11 +7,12 @@ deepvoice3_ljspeech preset on synthetic data, plus the fused-ConvBlock roofline 
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...      # the CPU arm: the UNMODIFIED reference package + the reference's own
                                               # train.py loop (oracle/_ref), on the host cores
+    python bench.py ... --dump-outputs DIR    # also write the last timed step's results to DIR/*.npy
 
 One step = zero_grad -> forward -> the reference's losses (train.py:704-740) -> backward -> (NCCL gradient
 all-reduce) -> clip_grad_norm(0.1) -> Adam.  Timed with CUDA events on the launching stream, barrier +
 synchronize on both sides, max over ranks.  A step touches > 1.5 GB of weights, optimizer state and
-activations, i.e. far more than the 126 MB L2 ("inputs larger than L2").
+activations, i.e. far more than the H100's 50 MB L2 ("inputs larger than L2").
 """
 import argparse
 import json
@@ -57,19 +58,19 @@ PRESETS = {
 B, T_TEXT, T_MEL = 16, 128, 800
 METRIC = "mel-frames/sec training step (B=16,T_mel=800)"
 WORKLOAD = "%s training step, B=16/GPU, T_text=128, T_mel=800 (T_dec=200)"
-NCU_TRAFFIC_GATED_512_800 = 90.40e6   # dram__bytes_read.sum + dram__bytes_write.sum (58.82 + 31.58 MB) of the (16,512,800)
-                                      # gated forward, profiles/r02_ncu_full_conv.csv (`ncu --set full` of this kernel)
+DUMP_SAMPLE = 1 << 20                 # elements of the fixed, seeded sample of the parameters / gradients --dump-outputs writes
 
 
 def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "datasheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -132,7 +133,7 @@ def cpu_model():
 # The reference itself: oracle/_ref (an unmodified copy of the reference package + train.py, oracle/make_ref.py) driven
 # through the reference's own train() loop (train.py:604-785) on reference collate_fn batches.  Used for
 #   * the CPU arm (`--impl reference`, `cpu_baseline`): device = cpu, all the host threads oneDNN scales to;
-#   * `gpu_eager_baseline`: the same modules in PyTorch eager on the B200 (cuDNN / cuBLAS), TF32 off and on -- the
+#   * `gpu_eager_baseline`: the same modules in PyTorch eager on the GPU (cuDNN / cuBLAS), TF32 off and on -- the
 #     honest GPU competitor of SURVEY.md section 8(d).
 # -------------------------------------------------------------------------------------------------
 class _TimedLoader:
@@ -165,7 +166,7 @@ def reference_train_throughput(preset, device, steps, warmup, threads=None, tf32
     import tempfile
     if device.type == "cpu":
         # oneDNN's small convolutions stop scaling (and on shared 100+-core hosts collapse) beyond a few dozen
-        # threads: use at most 32 (measured: 128 threads on the B200 host = 134 s/step vs ~1-6 s/step at 8-32).
+        # threads: use at most 32.
         torch.set_num_threads(threads or min(os.cpu_count() or 8, 32))
     old = (torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32)
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = bool(tf32)
@@ -310,8 +311,8 @@ def _time_launch(launch, flush, reps=10):
 
 
 def convblock_roofline(dev, pk, pk_kind):
-    """The time-dominant kernel FAMILY of the step: tc_conv_kernel (tcgen05 gated forward / conv / data-gradient GEMM;
-    42 % of the GPU time of a step, profiles/r02_step_profile.txt).  Every ConvBlock shape of the ljspeech model is
+    """The time-dominant kernel FAMILY of the step: tc_conv_kernel (wgmma gated forward / conv / data-gradient GEMM).
+    Every ConvBlock shape of the ljspeech model is
     timed -- gated forward and data gradient, operands prepared outside, CUDA events on the launching stream, L2
     flushed between launches -- and aggregated with the number of such launches per training step:
         achieved = sum_i n_i * flops_i / sum_i n_i * t_i      (ALGORITHMIC flops: 2*B*T*2C*C*k per launch)
@@ -363,16 +364,13 @@ def convblock_roofline(dev, pk, pk_kind):
     tf, flops, alg_bytes = big
     return {
         "bound": "tensor",
-        "kernel": "tc_conv_kernel family (persistent tcgen05 gated-forward / data-gradient GEMMs of all 25 ConvBlocks "
+        "kernel": "tc_conv_kernel family (persistent wgmma gated-forward / data-gradient GEMMs of all 25 ConvBlocks "
                   "of the step: 50 launches, time-weighted) via dv3_tc_convblock_fwd / dv3_tc_conv",
         "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"],
         "issued_tflops": 3 * ach, "issued_frac": 3 * ach / pk["bf16_tflops"],
         "note": "achieved counts ALGORITHMIC flops (one fp32 multiply-add per term); the kernels issue 3 fp16 MMA "
                 "passes per term (hi*hi, hi*lo, lo*hi of fp16 operand pairs) for fp32-class results",
         "family_us_per_step": tot_t * 1e6, "shapes": rows, "peak_source": pk_kind,
-        # dram__bytes_read.sum + dram__bytes_write.sum of the (16,512,800) gated forward from the committed
-        # `ncu --set full` capture of THIS kernel (profiles/r02_ncu_full_conv.csv)
-        "traffic": NCU_TRAFFIC_GATED_512_800,
         "largest_member": {"shape": "(B=16,C=512,T=800,k=3) gated forward", "launch_us": tf * 1e6,
                            "achieved": flops / tf / 1e12, "frac": flops / tf / 1e12 / pk["bf16_tflops"],
                            "alg_flops": flops},
@@ -510,6 +508,7 @@ def run_gpu_arm(args):
         dist.all_reduce(t_loc, op=dist.ReduceOp.MAX)
     t_e2e = float(t_loc.item())
     assert len(sink) - n_before >= args.steps and all(np.isfinite(v) for v in sink), "e2e: every step's loss is read"
+    dump = step_outputs(step, sink[-1]) if args.dump_outputs and rank == 0 else None
     t_extra = time.perf_counter()
     while len(clocks.rows) < 3 and time.perf_counter() - t_extra < 3.0:      # keep the load on until sampled
         step.step(resident)
@@ -521,15 +520,15 @@ def run_gpu_arm(args):
         "metric": METRIC, "value": frames * args.steps / t_res, "unit": "mel-frames/s", "n_gpus": world,
         "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": t_res / args.steps * 1e3,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": {"tc": "f32 via split 16-bit pairs (fp16 pairs forward, bf16 pairs for gradients; 3 tcgen05 MMA passes per product, fp32 accumulate)",
+        "dtype": {"tc": "f32 via split 16-bit pairs (fp16 pairs forward, bf16 pairs for gradients; 3 wgmma passes per product, fp32 accumulate)",
                   "bf16x3": "as tc", "fp32": "f32"}[args.math], "data": "synthetic",
         "config": {"workload": WORKLOAD % args.preset + ", random-init weights, fwd+losses+bwd+clip+Adam",
                    "global_batch": B * world, "parallelism": "dp%d" % world,
                    "l2": "inputs larger than L2 (>1.5 GB touched per step)",
                    "cuda_graph": not args.no_graph, "conv_math": args.math,
-                   "conv_math_note": {"tc": "tcgen05: forward operands as fp16 (hi, lo*2^11) pairs = 22-bit operands, "
+                   "conv_math_note": {"tc": "wgmma: forward operands as fp16 (hi, lo*2^11) pairs = 22-bit operands, "
                                             "gradient GEMMs on bf16 pairs (16 bits, full fp32 range), hi*hi + hi*lo + lo*hi "
-                                            "with fp32 accumulation in TMEM; all three presets within rtol 1e-3 / atol 1e-4 of the "
+                                            "with fp32 accumulation in registers; all three presets within rtol 1e-3 / atol 1e-4 of the "
                                             "fp32 oracle at B=16, full depth (tests/test_gpu_models.py)",
                                       "bf16x3": "alias of tc",
                                       "fp32": "exact fp32 FMA on CUDA cores"}[args.math]},
@@ -573,7 +572,7 @@ def run_gpu_arm(args):
             del st, rb
             torch.cuda.empty_cache()
             ops.conv_math = args.math
-            # the GPU competitor: the UNMODIFIED reference modules + train.py loop in PyTorch eager on this B200
+            # the GPU competitor: the UNMODIFIED reference modules + train.py loop in PyTorch eager on this GPU
             eager = {}
             for tf32 in (False, True):
                 try:
@@ -596,10 +595,34 @@ def run_gpu_arm(args):
                                                  c["n"], c["sec"], c["cores"],
                                                  "reference package + train.py loop (oracle/_ref)"
                                                  if c["kind"] == "reference" else "oracle port")}
+        if dump is not None:
+            write_outputs(args.dump_outputs, dump)
         print(json.dumps(out))
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def step_outputs(step, loss):
+    """What a caller of the training step holds after its last step: the loss, and the updated parameters and their
+    gradients (the flat arenas), as a fixed seeded sample of DUMP_SAMPLE elements when they are larger."""
+    flat, grad = step.arena.flat, step.arena.grad
+    idx = None
+    if flat.numel() > DUMP_SAMPLE:
+        gen = torch.Generator().manual_seed(0)
+        idx = torch.randperm(flat.numel(), generator=gen)[:DUMP_SAMPLE].sort().values.to(flat.device)
+    pick = (lambda t: t) if idx is None else (lambda t: t[idx])
+    out = {"loss": np.array(loss, dtype=np.float64),
+           "params": pick(flat).float().cpu().numpy(), "grads": pick(grad).float().cpu().numpy()}
+    if idx is not None:
+        out["sample_index"] = idx.cpu().numpy().astype(np.float64)
+    return out
+
+
+def write_outputs(path, arrays):
+    os.makedirs(path, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def stft_throughput(dev, world, rank, timed):
@@ -646,10 +669,13 @@ def main():
     ap.add_argument("--preset", default="deepvoice3_ljspeech", choices=sorted(PRESETS))
     ap.add_argument("--no-graph", action="store_true", help="run the step eagerly instead of replaying a CUDA graph")
     ap.add_argument("--math", default=os.environ.get("DV3_CONV_MATH", "tc"), choices=["tc", "fp32", "bf16x3"],
-                    help="contraction arithmetic: tc = tcgen05 split 16-bit pairs (fp32-class, default), fp32 = CUDA cores")
+                    help="contraction arithmetic: tc = wgmma split 16-bit pairs (fp32-class, default), fp32 = CUDA cores")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true",
                     help="skip the sub-benchmarks (other presets, STFT, exact-fp32 mode, reference-in-eager competitor)")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the last timed step's loss and a fixed sample of the updated parameters and their "
+                         "gradients to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference_arm(args)

@@ -1,4 +1,4 @@
-"""In-tree nvcc build of the C-ABI library (sm_100a only).  Used by ``__graft_entry__.build()``.
+"""In-tree nvcc build of the C-ABI library (sm_90a only).  Used by ``__graft_entry__.build()``.
 
     python -m deepvoice3_pytorch_b200._build
 """
@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libdv3b200.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--use_fast_math=false"]
 
 
@@ -46,7 +46,7 @@ def build(force=False, verbose=False):
             raise RuntimeError("nvcc failed on %s:\n%s" % (src, out))
         if verbose and out.strip():
             print(out)
-    subprocess.check_call([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs)
+    subprocess.check_call([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + objs)
     return LIB
 
 

@@ -22,8 +22,9 @@ const Config& config() {
         int dev = 0, sms = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-        v.sms = sms > 0 ? sms : 148;
-        // measured on B200 (tools/trunc_bias.py): the main accumulator (fp16 x fp16 products) loses 0.56 * 2^-25 of its value per MMA
+        v.sms = sms > 0 ? sms : 132;
+        // relative loss of the main accumulator (fp16 x fp16 products) per MMA, in units of 2^-25: 0.56 measured on an
+        // H100 SXM with tools/trunc_bias.py
         e = getenv("DV3_TC_GAMMA");               // override, in units of 2^-25 per MMA
         v.tc_gamma = (e ? (float)atof(e) : 0.56f) * 2.98023224e-8f;
         return v;

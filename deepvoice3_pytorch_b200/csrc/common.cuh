@@ -1,4 +1,4 @@
-// Shared device/host helpers for the dv3b200 C-ABI library (sm_100a only).
+// Shared device/host helpers for the dv3b200 C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -24,13 +24,13 @@ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 struct Config {
     int pdl;            // DV3_PDL=0 disables programmatic dependent launch (default on)
     int sms;            // multiprocessor count of the current device at first use
-    float tc_gamma;     // per-MMA truncation compensation of the tcgen05 accumulators (tc_gemm.cu TcParams::gmain)
+    float tc_gamma;     // per-MMA truncation compensation of the tensor-core accumulators (tc_gemm.cu TcParams::gmain)
 };
 const Config& config();
 
 // ---- programmatic dependent launch -------------------------------------------------------------------------
 // Every kernel of this library begins with pdl_trigger() -- the next kernel on the stream may be scheduled onto SMs as
-// they free up and run its own set-up (barrier init, TMEM allocation, descriptor prefetch) under this kernel's tail --
+// they free up and run its own set-up (barrier init, descriptor prefetch) under this kernel's tail --
 // and calls pdl_wait() before its first access to global memory, which blocks until the preceding kernel has completed
 // and its writes are visible.  Launches go through launch_k(), which sets the programmatic-serialisation attribute
 // (a plain full dependency when the predecessor is not a kernel of ours, or when DV3_PDL=0).  A captured CUDA graph

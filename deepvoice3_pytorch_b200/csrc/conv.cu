@@ -369,7 +369,7 @@ static int num_sms() {
         int dev = 0;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-        if (g_num_sms <= 0) g_num_sms = 148;
+        if (g_num_sms <= 0) g_num_sms = 132;
     }
     return g_num_sms;
 }
@@ -454,7 +454,7 @@ int dv3_conv1d_dgrad(const float* dab, const float* w_b, float* dx, int B, int M
 int dv3_conv1d_wgrad_nsplit(int B, int M, int Cin, int T, int k) {
     const int tiles = ceil_div(M, GEMM_BM) * ceil_div(Cin, 64) * k;
     const int chunks = ceil_div(B * T, GEMM_BK);
-    int want = ceil_div(4 * 148, tiles);
+    int want = ceil_div(4 * num_sms(), tiles);
     int maxs = chunks / 8 > 0 ? chunks / 8 : 1;           // at least 8 chunks (128 samples) per split
     if (want > maxs) want = maxs;
     if (want < 1) want = 1;

@@ -217,7 +217,7 @@ using namespace dv3;
 
 static inline int ew_blocks(long long n, int threads) {
     long long b = (n + threads - 1) / threads;
-    return (int)(b > 148 * 16 ? 148 * 16 : (b < 1 ? 1 : b));
+    return (int)(b > 132 * 16 ? 132 * 16 : (b < 1 ? 1 : b));
 }
 
 extern "C" {

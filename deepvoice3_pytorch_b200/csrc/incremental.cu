@@ -3,8 +3,8 @@
 // modules.py:145-167 / 200-226 (gate epilogues on a (B,1,C) slice), deepvoice3.py:132-176 (attention with the
 // monotonic window) and the decoder loops deepvoice3.py:367-485 / nyanko.py:250-338.
 //
-// B200 design: a decoder step is ~40 dependent matrix-VECTOR products (B is 1..16, M = 1), i.e. pure weight
-// streaming out of L2 (the 10-25 MB of decoder weights stay resident in the 126 MB L2) and launch latency.  So the
+// Design: a decoder step is ~40 dependent matrix-VECTOR products (B is 1..16, M = 1), i.e. pure weight
+// streaming out of L2 (the 10-25 MB of decoder weights stay resident in the 50 MB L2) and launch latency.  So the
 // step is a fixed sequence of small kernels with ALL loop state in device memory -- the step counter t, the ring
 // buffers, the monotonic-attention cursor, the output arrays indexed by t -- which makes the sequence identical
 // from step to step: the host captures it once in a CUDA graph and replays it, checking the done flags only every

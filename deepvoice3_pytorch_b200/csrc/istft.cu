@@ -164,7 +164,7 @@ extern "C" {
 int dv3_spec_to_amp(const float* spec_norm, float* amp, long long n, float min_level_db, float ref_level_db,
                     float power, void* stream) {
     long long blocks = (n + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     launch_k(spec_to_amp_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, spec_norm, amp, n, min_level_db, ref_level_db,
              power);

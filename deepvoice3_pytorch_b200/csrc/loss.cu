@@ -135,7 +135,7 @@ int dv3_spec_loss(const float* y_hat, const float* y, const long long* lengths, 
     DV3_REQUIRE(priority_bin >= 0 && priority_bin <= D && priority_weight >= 0.f && priority_weight <= 1.f,
                 "spec_loss: priority_bin=%d (D=%d) priority_weight=%g out of range", priority_bin, D, priority_weight);
     long long blocks = ((long long)B * T * D + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     launch_k(spec_loss_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, grad, loss, B, T, D, r,
                                                                    masked_loss_weight, binary_divergence_weight, 1e-8f,
                                                                    priority_bin, priority_weight);
@@ -145,7 +145,7 @@ int dv3_spec_loss(const float* y_hat, const float* y, const long long* lengths, 
 int dv3_aux_loss(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
                  float* d_attn, const long long* in_len, const long long* dec_len, int A, int B, int Td, int Ts,
                  float sigma, int use_attn, float* loss, void* stream) {
-    launch_k(aux_loss_kernel, 148 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done, attn, d_attn, in_len,
+    launch_k(aux_loss_kernel, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done, attn, d_attn, in_len,
                                                               dec_len, A, B, Td, Ts, sigma, use_attn, loss);
     return check_launch("aux_loss");
 }

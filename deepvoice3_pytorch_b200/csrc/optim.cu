@@ -12,7 +12,7 @@ namespace dv3 {
 // data-parallel replicas (which hold bit-identical all-reduced gradients) get the same clip coefficient.
 // scratch: >= DV3_SUMSQ_SCRATCH floats; scratch[DV3_SUMSQ_SCRATCH-1] is the ticket counter (zero before first use;
 // the kernel leaves it zero).
-constexpr int SUMSQ_MAX_BLOCKS = 148 * 8;
+constexpr int SUMSQ_MAX_BLOCKS = 132 * 8;
 constexpr int SUMSQ_SCRATCH = 2048;
 __global__ void sumsq_kernel(const float* __restrict__ x, long long n, float* __restrict__ out,
                              float* __restrict__ scratch) {
@@ -107,7 +107,7 @@ int dv3_sumsq(const float* x, long long n, float* out, float* scratch, void* str
 int dv3_adam_clip(float* p, const float* g, float* m, float* v, long long n, const float* hyper,
                   const float* sumsq, float beta1, float beta2, float eps, float max_norm, void* stream) {
     long long blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
     launch_k(adam_clip_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, p, g, m, v, n, hyper, sumsq, beta1, beta2,
                                                                    eps, max_norm);

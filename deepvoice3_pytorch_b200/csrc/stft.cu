@@ -8,7 +8,7 @@
 //   * the 11*256 raw samples the 8 frames overlap on are staged once in shared memory by 16-byte cp.async (zero-filled
 //     outside the clip), the copy for the next 8 frames in flight while the mel rows of the current ones are formed;
 //   * each warp runs the register-resident radix-8 transform of stft_core.cuh: two butterflies per lane held as
-//     register PAIRS, all arithmetic as packed f32x2 instructions (FADD2 / FMUL2 / FFMA2), pre-emphasis and window
+//     register PAIRS, all arithmetic pair-wise (stft_core.cuh), pre-emphasis and window
 //     applied as the points are read, two exchanges through its private work area (__syncwarp only), then the split
 //     into the 513-bin half spectrum four bins at a time; the normalised dB row goes straight to global memory
 //     (coalesced) and the magnitudes stay in shared memory;

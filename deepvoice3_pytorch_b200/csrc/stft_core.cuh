@@ -3,8 +3,8 @@
 //
 // One warp transforms one frame.  1024 real samples are packed as 512 complex points z[n] = x[2n] + i*x[2n+1];
 // the 512-point transform is three radix-8 passes (512 = 8*8*8).  Every lane runs TWO butterflies per pass ("virtual
-// threads" a and b) and keeps their data as PAIRS pr = (value of a, value of b): all arithmetic is pair-wise, which
-// on sm_100 is one FADD2 / FMUL2 / FFMA2 (add/mul/fma.f32x2) per pair -- half the issue slots of scalar code.  The
+// threads" a and b) and keeps their data as PAIRS pr = (value of a, value of b): all arithmetic is pair-wise (two independent
+// scalar instructions per pair, which keeps the issue of a lane dense).  The
 // pairing of every pass is chosen so that the loads deliver pairs in adjacent registers (64/128-bit shared-memory
 // accesses) with no register shuffling.  With n = 64*n2 + 8*n1 + n0 and k = k0 + 8*k1 + 64*k2:
 //   pass 1  lane l: a,b = points t = 2l, 2l+1   A[k0]  = W512^(t*k0) * sum_n2 z[64*n2 + t]      * W8^(n2*k0)
@@ -39,29 +39,13 @@ constexpr int PITCH2 = 34;       // exchange 2: pairs per n0 row
 
 // ---- pair arithmetic: one instruction per pair on the device ----------------------------------------------------
 #if defined(__CUDA_ARCH__)
-__device__ __forceinline__ unsigned long long pk_(pr a) {
-    unsigned long long r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y)); return r;
-}
-__device__ __forceinline__ pr upk_(unsigned long long v) {
-    pr a; asm("mov.b64 {%0, %1}, %2;" : "=f"(a.x), "=f"(a.y) : "l"(v)); return a;
-}
-__device__ __forceinline__ pr padd(pr a, pr b) {
-    unsigned long long r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(pk_(a)), "l"(pk_(b))); return upk_(r);
-}
-__device__ __forceinline__ pr psub(pr a, pr b) {
-    unsigned long long r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(pk_(a)), "l"(pk_(b))); return upk_(r);
-}
-__device__ __forceinline__ pr pmul(pr a, pr b) {
-    unsigned long long r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(pk_(a)), "l"(pk_(b))); return upk_(r);
-}
-__device__ __forceinline__ pr pfma(pr a, pr b, pr c) {          // a*b + c
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(pk_(a)), "l"(pk_(b)), "l"(pk_(c)));
-    return upk_(r);
-}
-__device__ __forceinline__ pr pfnma(pr a, pr b, pr c) {         // c - a*b  (the negation folds into the FFMA2 operand)
-    return pfma(pr{-a.x, -a.y}, b, c);
-}
+// sm_90 has no packed f32x2 arithmetic: two scalar instructions per pair.  The _rn intrinsics keep nvcc from fusing a
+// separate multiply and add into one FMA, so the device rounds exactly like the host build of this header.
+__device__ __forceinline__ pr padd(pr a, pr b) { return {__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+__device__ __forceinline__ pr psub(pr a, pr b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)}; }
+__device__ __forceinline__ pr pmul(pr a, pr b) { return {__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
+__device__ __forceinline__ pr pfma(pr a, pr b, pr c) { return {__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)}; }
+__device__ __forceinline__ pr pfnma(pr a, pr b, pr c) { return {__fmaf_rn(-a.x, b.x, c.x), __fmaf_rn(-a.y, b.y, c.y)}; }
 #else
 STFT_HD pr padd(pr a, pr b) { return {a.x + b.x, a.y + b.y}; }
 STFT_HD pr psub(pr a, pr b) { return {a.x - b.x, a.y - b.y}; }

@@ -1,13 +1,13 @@
-// Fused dot-product attention of the teacher-forced decoder on tcgen05 tensor cores -- reference
+// Fused dot-product attention of the teacher-forced decoder on wgmma tensor cores -- reference
 // deepvoice3.py:132-176 (AttentionLayer.forward between the projections):
 //     S = Q.K^T (no 1/sqrt(d)) -> mask padded keys with -inf -> softmax over keys -> [return P] -> dropout
 //       -> O = scale * Pd.V                                                     (scale = Ts * sqrt(1/Ts))
 // and its backward.  Layouts are the channel-major ones the decoder already holds: q (B,E,Td), k, v (B,E,Ts),
 // out (B,E,Td), probabilities (B,Td,Ts) (materialised: the guided-attention loss reads them, train.py:734-738).
 //
-// Arithmetic: fp32-equivalent split-bf16 (hi*hi in one TMEM accumulator, hi*lo + lo*hi in a second one, summed in
-// fp32 by the epilogue -- same scheme as tc_gemm.cu).  The fp32 operands are split INSIDE the kernel while they are
-// staged into shared memory in the UMMA canonical layouts (there is no pre-pass and nothing but q/k/v/probs ever
+// Arithmetic: fp32-equivalent split-bf16 (hi*hi in one register accumulator, hi*lo + lo*hi in a second one, summed
+// in fp32 by the epilogue -- same scheme as tc_gemm.cu).  The fp32 operands are split INSIDE the kernel while they are
+// staged into shared memory in the wgmma canonical layouts (there is no pre-pass and nothing but q/k/v/probs ever
 // touches HBM):
 //   * operands whose contraction index is the ROW of the global tensor (q, k, dO, v in the score GEMMs; P, dS in the
 //     key/value-gradient GEMMs) are written MN-major: [contraction row][64 elements = 128 B], 16-byte chunk c of row
@@ -21,9 +21,10 @@
 //                            dropout(P) as the A operand of the second GEMM) -> O GEMM -> store.
 //   attn_rows_kernel<BWD=1>  same skeleton for the backward: dPd = dO^T.V -> softmax backward epilogue (writes dS)
 //                            -> dQ = dS.K^T.
-//   attn_cols_kernel         one CTA per (128 channels, utterance): dV = scale * dO.Pd and dK = Q.dS, contraction over
-//                            the query axis (which spans the CTAs of attn_rows_kernel, hence a second launch).
-// 256 threads: all stage operands; thread 0 issues the MMAs; warps 0-3 (TMEM lane quarter = warp) run the epilogues.
+//   attn_cols_kernel         one CTA per (128 channels, utterance): dV = scale * dO.Pd, then dK = Q.dS, contraction
+//                            over the query axis (which spans the CTAs of attn_rows_kernel, hence a second launch).
+// 256 threads = two warpgroups: all stage operands; warpgroup w accumulates output rows [64 w, 64 w + 64) of the
+// 128-row tile in registers; the softmax epilogues run on warps 0-3 from the scores gathered in shared memory.
 #include "tc_common.cuh"
 
 namespace dv3 {
@@ -47,24 +48,6 @@ struct AttnParams {
     const unsigned long long* seed_ptr;
     uint32_t salt;
 };
-
-__device__ __forceinline__ uint64_t desc_kmajor(uint32_t saddr) {            // [row][64 k] 128-byte rows, SWIZZLE_128B
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr, uint32_t lbo) {   // [k row][64 mn], chunk stride lbo
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
 
 // 8 fp32 -> 8 bf16 hi (16 bytes) + 8 bf16 lo
 __device__ __forceinline__ void split8(const float* x, uint4& hi, uint4& lo) {
@@ -156,32 +139,33 @@ __device__ __forceinline__ void stage_k(uint8_t* dst, uint32_t plane_bytes, cons
     }
 }
 
-__device__ __forceinline__ void tmem_ld_sum(uint32_t taddr, int cross_off, float* v) {
-    float c[32];
-    tmem_ld_32x32(taddr, v);
-    tmem_ld_32x32(taddr + cross_off, c);
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] += c[i];
+__device__ __forceinline__ uint64_t desc_kmajor(uint32_t saddr) {            // [row][64 k] 128-byte rows, SWIZZLE_128B
+    return make_wgmma_desc(saddr, 16, 1024, WG_SW128);
+}
+__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t saddr, uint32_t lbo) {   // [k row][64 mn], chunk stride lbo
+    return make_wgmma_desc(saddr, lbo, 1024, WG_SW128);
 }
 
-// main (+)= Ahi*Bhi ; cross (+)= Ahi*Blo + Alo*Bhi
-__device__ __forceinline__ void mma3(uint32_t tmain, uint32_t tcross, uint64_t ahi, uint64_t alo, uint64_t bhi,
-                                     uint64_t blo, uint32_t idesc, bool first) {
-    umma_bf16(tmain, ahi, bhi, idesc, first ? 0u : 1u);
-    umma_bf16(tcross, ahi, blo, idesc, first ? 0u : 1u);
-    umma_bf16(tcross, alo, bhi, idesc, 1u);
+// 64 x 128 tile of one warpgroup: main (acc[0, 64)) (+)= Ahi*Bhi ; cross (acc[64, 128)) (+)= Ahi*Blo + Alo*Bhi
+template <int TA, int TB>
+__device__ __forceinline__ void mma3(float* acc, uint64_t ahi, uint64_t alo, uint64_t bhi, uint64_t blo) {
+    wgmma_mma<AT_NS, TA, TB>(true, acc, ahi, bhi, 1);
+    wgmma_mma<AT_NS, TA, TB>(true, acc + 64, ahi, blo, 1);
+    wgmma_mma<AT_NS, TA, TB>(true, acc + 64, alo, bhi, 1);
 }
 
 // Shared-memory map of attn_rows_kernel (bytes, after 1024-byte alignment):
-//   phase 1 (two stages of 64 KB):  stage s at s*65536: A hi 16 KB | A lo 16 KB | B hi 16 KB | B lo 16 KB
-//   phase 2 (aliases phase 1):      A2 hi 32 KB | A2 lo 32 KB  (2 key slabs x 128 rows x 128 B)
-//                                   B2 at 65536: per key slab [hi E*128 | lo E*128]  (<= 2 x 64 KB)
-// Epilogue warps exchange 32 x 32 tiles with global memory through a per-warp transposing buffer: the thread of TMEM
-// lane r owns ROW r of the score tile, and a row of the (B,Td,Ts) probability tensors is contiguous along the keys -- a
-// direct per-thread access touches 32 different 128-byte lines per warp instruction (ncu: the softmax epilogues were
-// bound by those LSU transactions).  Through the buffer every global access is one full 128-byte line per instruction.
+//   GEMM 1 (two stages of 64 KB):   stage s at s*65536: A hi 16 KB | A lo 16 KB | B hi 16 KB | B lo 16 KB
+//   epilogue 1 (aliases GEMM 1):    A2 hi 32 KB | A2 lo 32 KB  (2 key slabs x 128 rows x 128 B) ; scores at 65536
+//                                   ([128][SC_PITCH] fp32, summed accumulators of both warpgroups)
+//   GEMM 2 (aliases the scores):    B2 at 65536: per key slab [hi E*128 | lo E*128]  (<= 2 x 64 KB)
+// The epilogue warps exchange 32 x 32 tiles with global memory through a per-warp transposing buffer: the thread of
+// warp w, lane l owns ROW 32 w + l of the score tile, and a row of the (B,Td,Ts) probability tensors is contiguous
+// along the keys -- a direct per-thread access touches 32 different 128-byte lines per warp instruction.  Through the
+// buffer every global access is one full 128-byte line per instruction.
 constexpr int TILE_PITCH = 33;
 constexpr int TILE_FLOATS = 32 * TILE_PITCH;
+constexpr int SC_PITCH = AT_NS + 1;
 constexpr int ROWS_SMEM = 65536 + 2 * 65536 + 1024 + 256 + 4 * TILE_FLOATS * 4;
 
 // global rows [0, rows_valid) x columns [c0, c0+32) of a row-major matrix (row stride ld) starting at src -> tile
@@ -210,65 +194,54 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 3 * 65536);        // [0,1]: stage free, [2]: GEMM1 done, [3]: GEMM2 done
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 4);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
     const int b = blockIdx.y, t0 = blockIdx.x * 128;
     const int E = p.E, Td = p.Td, Ts = p.Ts;
     const float* A1 = p.a1 + (size_t)b * E * Td;
     const float* B1 = p.b1 + (size_t)b * E * Ts;
     const float* B2 = p.b2 + (size_t)b * E * Ts;
     const bool vec_td = (Td & 3) == 0, vec_ts = (Ts & 3) == 0;
-
-    if (tid == 0) {
-        for (int i = 0; i < 4; ++i) mbar_init(&bars[i], 1);
-        fence_barrier_init();
-    }
-    if (warp == 0) tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_ptr;
-    pdl_wait();                 // set-up above overlaps the previous kernel's tail; global memory from here on
+    float* sc = reinterpret_cast<float*>(smem + 65536);
+    pdl_wait();                 // global memory from here on
 
     // ---------------- GEMM 1: D1[t][s] = sum_e A1[e][t0+t] * B1[e][s] -----------------------------------
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
     const int kchunks = (E + 63) / 64;
-    constexpr uint32_t idesc_mn = make_idesc_bf16(128, AT_NS) | (1u << 15) | (1u << 16);
     for (int kc = 0; kc < kchunks; ++kc) {
         const int s = kc & 1;
-        if (kc >= 2) mbar_wait(&bars[s], ((kc >> 1) - 1) & 1);          // the MMAs that read this stage retired
+        if (kc >= 2) __syncthreads();                       // both warpgroups retired the MMAs that read this stage
         uint8_t* st = smem + s * 65536;
         stage_mn<2>(st, 16384, A1, Td, kc * 64, E, t0, Td, vec_td, tid, AT_THREADS);
         stage_mn<2>(st + 32768, 16384, B1, Ts, kc * 64, E, 0, Ts, vec_ts, tid, AT_THREADS);
         fence_proxy_async();
         __syncthreads();
-        if (tid == 0) {
-            tc_fence_after();
-            const uint32_t sa = smem_u32(st);
+        const uint32_t sa = smem_u32(st);
+        wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const uint32_t ko = kk * 2048;
-                mma3(tmem, tmem + AT_NS, desc_mnmajor(sa + ko, 8192), desc_mnmajor(sa + 16384 + ko, 8192),
-                     desc_mnmajor(sa + 32768 + ko, 8192), desc_mnmajor(sa + 49152 + ko, 8192), idesc_mn,
-                     kc == 0 && kk == 0);
-            }
-            umma_commit(&bars[s]);
-            if (kc == kchunks - 1) umma_commit(&bars[2]);
+        for (int kk = 0; kk < 4; ++kk) {
+            const uint32_t ko = kk * 2048, ao = sa + wg * 8192 + ko;
+            mma3<1, 1>(acc, desc_mnmajor(ao, 8192), desc_mnmajor(ao + 16384, 8192), desc_mnmajor(sa + 32768 + ko, 8192),
+                       desc_mnmajor(sa + 49152 + ko, 8192));
         }
+        wgmma_commit();
+        wgmma_wait<1>();
     }
-    mbar_wait(&bars[2], 0);
-    tc_fence_after();
+    wgmma_wait<0>();
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < 64; ++i)
+        sc[(64 * wg + frag_row(i, wq, lane)) * SC_PITCH + frag_col(i, lane)] = acc[i] + acc[64 + i];
+    __syncthreads();
 
-    // ---------------- epilogue 1 (warps 0-3) || stage B2 (warps 4-7) -------------------------------------
+    // ---------------- epilogue 1 (warps 0-3, thread = score row) -------------------------------------------
     const int nslab = (Ts + 63) / 64;                       // 64-key slabs of the second contraction
     const uint32_t b2_plane = (uint32_t)E * 128u;           // one plane of one slab: E rows x 128 B
-    if (warp >= 4) {
-        for (int sl = 0; sl < nslab; ++sl)
-            stage_k(smem + 65536 + sl * 2 * b2_plane, b2_plane, B2, Ts, 0, E, E, sl * 64, Ts, vec_ts, tid - 128, 128);
-    } else {
+    if (warp < 4) {
         const int row = warp * 32 + lane, t = t0 + row;
         const bool tv = t < Td;
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
+        const float* srow = sc + row * SC_PITCH;
         const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
         const size_t rbase = ((size_t)b * Td + (tv ? t : 0)) * Ts;
         const unsigned char* mrow = p.mask ? p.mask + (size_t)b * Ts : nullptr;
@@ -288,25 +261,20 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
             float mx = -INFINITY;
 #pragma unroll
             for (int c32 = 0; c32 < AT_NS; c32 += 32) {
-                float v[32];
-                tmem_ld_sum(taddr + c32, AT_NS, v);
 #pragma unroll
-                for (int i = 0; i < 32; ++i) mx = fmaxf(mx, ((mb[c32 >> 5] >> i) & 1u) ? -INFINITY : v[i]);
+                for (int i = 0; i < 32; ++i) mx = fmaxf(mx, ((mb[c32 >> 5] >> i) & 1u) ? -INFINITY : srow[c32 + i]);
             }
             float sum = 0.f;
 #pragma unroll
             for (int c32 = 0; c32 < AT_NS; c32 += 32) {
-                float v[32];
-                tmem_ld_sum(taddr + c32, AT_NS, v);
 #pragma unroll
-                for (int i = 0; i < 32; ++i) sum += ((mb[c32 >> 5] >> i) & 1u) ? 0.f : expf(v[i] - mx);
+                for (int i = 0; i < 32; ++i) sum += ((mb[c32 >> 5] >> i) & 1u) ? 0.f : expf(srow[c32 + i] - mx);
             }
             r0v = mx; r1v = 1.f / sum;
         } else {
             float dot = 0.f;
             for (int c32 = 0; c32 < AT_NS; c32 += 32) {
-                float v[32], pv[32];
-                tmem_ld_sum(taddr + c32, AT_NS, v);
+                float pv[32];
                 if (c32 >= Ts) continue;                          // uniform
                 tile_load(tile, p.probs + wbase, Ts, rows_valid, c32, Ts, lane);
 #pragma unroll
@@ -316,7 +284,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
                 for (int i = 0; i < 32; ++i) {
                     const int s = c32 + i;
                     if (tv && s < Ts) {
-                        float g = p.scale * v[i] * drop_scale(drop, (uint32_t)(rbase + s));
+                        float g = p.scale * srow[s] * drop_scale(drop, (uint32_t)(rbase + s));
                         if (p.dprobs) g += tile[lane * TILE_PITCH + i];
                         dot = fmaf(g, pv[i], dot);
                     }
@@ -326,8 +294,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
         }
         // final pass: produce the row of the second GEMM's A operand (dropout(P) or dS), write P / dS to HBM
         for (int c32 = 0; c32 < AT_NS; c32 += 32) {
-            float v[32], o[32];
-            tmem_ld_sum(taddr + c32, AT_NS, v);
+            float o[32];
             const bool live = c32 < Ts;                           // uniform: chunks past the last key hold nothing
             const uint32_t mbc = c32 == 0 ? mb[0] : (c32 == 32 ? mb[1] : (c32 == 64 ? mb[2] : mb[3]));
             float pv[32];
@@ -343,13 +310,14 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
                 const int s = c32 + i;
                 float a2 = 0.f, wr = 0.f;
                 if (tv && s < Ts) {
+                    const float v = srow[s];
                     if (BWD == 0) {
                         const bool ok = !((mbc >> i) & 1u);
-                        const float pr = ok ? expf(v[i] - r0v) * r1v : 0.f;
+                        const float pr = ok ? expf(v - r0v) * r1v : 0.f;
                         wr = pr;
                         a2 = pr * drop_scale(drop, (uint32_t)(rbase + s));
                     } else {
-                        float g = p.scale * v[i] * drop_scale(drop, (uint32_t)(rbase + s));
+                        float g = p.scale * v * drop_scale(drop, (uint32_t)(rbase + s));
                         if (p.dprobs) g += tile[lane * TILE_PITCH + i];
                         a2 = pv[i] * (g - r0v);
                         wr = a2;
@@ -376,51 +344,42 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
                 }
             }
         }
-        tc_fence_before();
     }
+    __syncthreads();                                        // the scores are consumed: B2 takes their place
+    for (int sl = 0; sl < nslab; ++sl)
+        stage_k(smem + 65536 + sl * 2 * b2_plane, b2_plane, B2, Ts, 0, E, E, sl * 64, Ts, vec_ts, tid, AT_THREADS);
     fence_proxy_async();
     __syncthreads();
 
-    // ---------------- GEMM 2: D2[t][e] = sum_s A2[t][s] * B2[e][s] ---------------------------------------
-    if (tid == 0) {
-        tc_fence_after();
-        const uint32_t idesc_k = make_idesc_bf16(128, E);
-        const uint32_t sa = smem_u32(smem), sb = smem_u32(smem + 65536);
+    // ---------------- GEMM 2: D2[t][e] = sum_s A2[t][s] * B2[e][s], 128 channels at a time -------------------------
+    const float scl = BWD == 0 ? p.scale : 1.f;
+    float* __restrict__ out = p.out + (size_t)b * E * Td;
+    const uint32_t sa = smem_u32(smem) + wg * 8192, sb = smem_u32(smem + 65536);
+    for (int e0 = 0; e0 < E; e0 += AT_NS) {               // rows of B2 past E are never stored
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        wgmma_fence();
         for (int sl = 0; sl < nslab; ++sl) {
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {
-                const uint32_t a_hi = sa + sl * 16384 + kk * 32, b_hi = sb + sl * 2 * b2_plane + kk * 32;
-                mma3(tmem, tmem + 256, desc_kmajor(a_hi), desc_kmajor(a_hi + 32768), desc_kmajor(b_hi),
-                     desc_kmajor(b_hi + b2_plane), idesc_k, sl == 0 && kk == 0);
+                const uint32_t a_hi = sa + sl * 16384 + kk * 32, b_hi = sb + sl * 2 * b2_plane + e0 * 128 + kk * 32;
+                mma3<0, 0>(acc, desc_kmajor(a_hi), desc_kmajor(a_hi + 32768), desc_kmajor(b_hi),
+                           desc_kmajor(b_hi + b2_plane));
             }
         }
-        umma_commit(&bars[3]);
-    }
-    mbar_wait(&bars[3], 0);
-    tc_fence_after();
-    if (warp < 4) {
-        const int row = warp * 32 + lane, t = t0 + row;
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-        const float sc = BWD == 0 ? p.scale : 1.f;
-        float* __restrict__ out = p.out + (size_t)b * E * Td;
-        for (int c32 = 0; c32 < E; c32 += 32) {             // E % 16 == 0: the last chunk may be half used
-            float v[32];
-            tmem_ld_sum(taddr + c32, 256, v);
-            if (t < Td) {
+        wgmma_commit();
+        wgmma_wait<0>();
 #pragma unroll
-                for (int i = 0; i < 32; ++i)
-                    if (c32 + i < E) out[(size_t)(c32 + i) * Td + t] = sc * v[i];
-            }
+        for (int i = 0; i < 64; ++i) {
+            const int t = t0 + 64 * wg + frag_row(i, wq, lane), e = e0 + frag_col(i, lane);
+            if (t < Td && e < E) out[(size_t)e * Td + t] = scl * (acc[i] + acc[64 + i]);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<512>(tmem);
 }
 
-// dV[e][s] = scale * sum_t dO[e][t] * Pd[t][s] ;  dK[e][s] = sum_t Q[e][t] * dS[t][s]
-// smem per 64-query chunk: A(dO) hi 16 KB | lo 16 KB | A(q) hi | lo | B(Pd) hi 16 KB | lo | B(dS) hi | lo  = 128 KB
-constexpr int COLS_SMEM = 131072 + 1024 + 256;
+// dV[e][s] = scale * sum_t dO[e][t] * Pd[t][s] ;  dK[e][s] = sum_t Q[e][t] * dS[t][s], one after the other
+// smem per 64-query chunk: A (dO or q) hi 16 KB | lo 16 KB | B (Pd or dS) hi 16 KB | lo 16 KB
+constexpr int COLS_SMEM = 65536 + 1024;
 
 struct AttnColsParams {
     const float* dout; const float* q; const float* probs; const float* ds;
@@ -435,49 +394,39 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_cols_kernel(const __grid_c
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 131072);            // [0]: chunk MMAs retired
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2, wq = warp & 3;
     const int b = blockIdx.y, e0 = blockIdx.x * 128;
     const int E = p.E, Td = p.Td, Ts = p.Ts;
-    const float* dO = p.dout + (size_t)b * E * Td;
-    const float* Q = p.q + (size_t)b * E * Td;
-    const float* P = p.probs + (size_t)b * Td * Ts;
-    const float* dS = p.ds + (size_t)b * Td * Ts;
     const bool vec_td = (Td & 3) == 0, vec_ts = (Ts & 3) == 0;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
-
-    if (tid == 0) { mbar_init(&bars[0], 1); fence_barrier_init(); }
-    if (warp == 0) tmem_alloc<512>(tmem_ptr);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_ptr;
-    pdl_wait();                 // set-up above overlaps the previous kernel's tail; global memory from here on
+    pdl_wait();                 // global memory from here on
 
     const int kchunks = (Td + 63) / 64;
-    constexpr uint32_t idesc = make_idesc_bf16(128, AT_NS) | (1u << 16);      // A K-major, B MN-major
-    for (int kc = 0; kc < kchunks; ++kc) {
-        if (kc >= 1) mbar_wait(&bars[0], (kc - 1) & 1);
-        // A operands: rows e0.. of (E,Td), 64 query columns
-        stage_k(smem, 16384, dO, Td, e0, E, 128, kc * 64, Td, vec_td, tid, AT_THREADS);
-        stage_k(smem + 32768, 16384, Q, Td, e0, E, 128, kc * 64, Td, vec_td, tid, AT_THREADS);
-        // B operands: 64 query rows of (Td,Ts); Pd = P * dropout mask regenerated from the element index
-        {
-            uint8_t* dst = smem + 65536;
+    const uint32_t sa = smem_u32(smem);
+    float acc[128];
+    for (int pass = 0; pass < 2; ++pass) {                  // 0: dV (A = dO, B = Pd), 1: dK (A = q, B = dS)
+        const float* A = (pass == 0 ? p.dout : p.q) + (size_t)b * E * Td;
+        const float* Bm = (pass == 0 ? p.probs : p.ds) + (size_t)b * Td * Ts;
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        for (int kc = 0; kc < kchunks; ++kc) {
+            __syncthreads();                                // the previous chunk's MMAs have retired (wait below)
+            // A operand: rows e0.. of (E,Td), 64 query columns
+            stage_k(smem, 16384, A, Td, e0, E, 128, kc * 64, Td, vec_td, tid, AT_THREADS);
+            // B operand: 64 query rows of (Td,Ts); Pd = P * dropout mask regenerated from the element index
+            uint8_t* dst = smem + 32768;
             for (int g0 = tid; g0 < 64 * 16; g0 += AT_THREADS * 2) {
-                float x[2][8], y[2][8];
+                float x[2][8];
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
                     const int g = g0 + u * AT_THREADS, r = g >> 4, cg = g & 15, t = kc * 64 + r;
-                    load8(P + (long long)t * Ts, cg * 8, Ts, t < Td, vec_ts, x[u]);
-                    load8(dS + (long long)t * Ts, cg * 8, Ts, t < Td, vec_ts, y[u]);
+                    load8(Bm + (long long)t * Ts, cg * 8, Ts, t < Td, vec_ts, x[u]);
                 }
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
                     const int g = g0 + u * AT_THREADS, r = g >> 4, cg = g & 15, h = cg >> 3, c = cg & 7;
                     const int t = kc * 64 + r;
-                    if (drop.on) {
+                    if (pass == 0 && drop.on) {
                         const size_t idx0 = ((size_t)b * Td + t) * Ts + cg * 8;
 #pragma unroll
                         for (int i = 0; i < 8; ++i) x[u][i] *= drop_scale(drop, (uint32_t)(idx0 + i));
@@ -487,56 +436,29 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_cols_kernel(const __grid_c
                     split8(x[u], hi, lo);
                     *reinterpret_cast<uint4*>(dst + off) = hi;
                     *reinterpret_cast<uint4*>(dst + 16384 + off) = lo;
-                    split8(y[u], hi, lo);
-                    *reinterpret_cast<uint4*>(dst + 32768 + off) = hi;
-                    *reinterpret_cast<uint4*>(dst + 49152 + off) = lo;
                 }
             }
-        }
-        fence_proxy_async();
-        __syncthreads();
-        if (tid == 0) {
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem);
+            fence_proxy_async();
+            __syncthreads();
+            wgmma_fence();
 #pragma unroll
             for (int kk = 0; kk < 4; ++kk) {
-                const uint32_t ak = kk * 32, bk = kk * 2048;
-                // dV: A = dO, B = Pd
-                mma3(tmem, tmem + 128, desc_kmajor(sa + ak), desc_kmajor(sa + 16384 + ak),
-                     desc_mnmajor(sa + 65536 + bk, 8192), desc_mnmajor(sa + 81920 + bk, 8192), idesc, kc == 0 && kk == 0);
-                // dK: A = q, B = dS
-                mma3(tmem + 256, tmem + 384, desc_kmajor(sa + 32768 + ak), desc_kmajor(sa + 49152 + ak),
-                     desc_mnmajor(sa + 98304 + bk, 8192), desc_mnmajor(sa + 114688 + bk, 8192), idesc,
-                     kc == 0 && kk == 0);
+                const uint32_t ak = sa + wg * 8192 + kk * 32, bk = sa + 32768 + kk * 2048;
+                mma3<0, 1>(acc, desc_kmajor(ak), desc_kmajor(ak + 16384), desc_mnmajor(bk, 8192),
+                           desc_mnmajor(bk + 16384, 8192));
             }
-            umma_commit(&bars[0]);
+            wgmma_commit();
+            wgmma_wait<0>();
+        }
+        // rows e of dV / dK are contiguous along the keys
+        float* __restrict__ dst = (pass == 0 ? p.dv : p.dk) + (size_t)b * E * Ts;
+        const float scl = pass == 0 ? p.scale : 1.f;
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+            const int e = e0 + 64 * wg + frag_row(i, wq, lane), s = frag_col(i, lane);
+            if (e < E && s < Ts) dst[(size_t)e * Ts + s] = scl * (acc[i] + acc[64 + i]);
         }
     }
-    mbar_wait(&bars[0], (kchunks - 1) & 1);
-    tc_fence_after();
-    if (warp < 4) {
-        // rows e of dV / dK are contiguous along the keys: through the transposing tile (the operand buffers are free)
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16);
-        float* tile = reinterpret_cast<float*>(smem) + warp * TILE_FLOATS;
-        const int ew0 = e0 + warp * 32, rows_valid = min(max(E - ew0, 0), 32);
-        const size_t wbase = ((size_t)b * E + min(ew0, E - 1)) * Ts;
-        for (int c32 = 0; c32 < AT_NS; c32 += 32) {
-            float v[32], w[32];
-            tmem_ld_sum(taddr + c32, 128, v);
-            tmem_ld_sum(taddr + 256 + c32, 128, w);
-            if (c32 >= Ts) continue;                              // uniform
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) tile[lane * TILE_PITCH + i] = p.scale * v[i];
-            tile_store(tile, p.dv + wbase, Ts, rows_valid, c32, Ts, lane);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) tile[lane * TILE_PITCH + i] = w[i];
-            tile_store(tile, p.dk + wbase, Ts, rows_valid, c32, Ts, lane);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc<512>(tmem);
 }
 
 template <typename K>

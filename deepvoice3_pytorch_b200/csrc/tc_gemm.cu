@@ -1,10 +1,10 @@
-// tcgen05 tensor-core path of the ConvBlock and of the plain (1x1 / k-tap) weight-normed convolutions: forward,
+// wgmma tensor-core path of the ConvBlock and of the plain (1x1 / k-tap) weight-normed convolutions: forward,
 // data-gradient and weight-gradient as implicit GEMMs with fp32-equivalent accuracy from split-bf16 operands.
 // Every fp32 operand is split into bf16 planes p0 = bf16(x), p1 = bf16(x - p0) and each K-step issues
 // p0*p0 + p0*p1 + p1*p0 (operand error ~2^-17; single-pass TF32 would miss the rtol=1e-3/atol=1e-4 parity bar after
 // ~30 blocks).  The tensor core adds each MMA into the fp32 accumulator with truncation (bias ~N_mma x 2^-25), so the
-// main term p0*p0 and the 2^-8-smaller cross terms accumulate in two separate TMEM accumulators that the epilogue
-// adds in fp32 (tools/precision_report.py).
+// main term p0*p0 and the 2^-8-smaller cross terms accumulate in two separate register accumulators that the
+// epilogue adds in fp32 (tools/precision_report.py).
 //
 //   GATED : D[t, (a|b) c] = sum_{j,ci} Xd[b, t+off_j, ci] * W[j, (a|b) c, ci]    M = 128 time steps, N = 64 a | 64 b
 //   CONV  : D[t, n]       = sum_{j,kc} A[b, t+off_j, kc]  * W[j, n, kc]           M = 128 time steps, N = 64 or 128
@@ -17,10 +17,11 @@
 // back to back in a stage, so p0(A) x [p0(W) ; p1(W)] is ONE N = 2*NCOLS MMA filling the main | cross accumulators,
 // followed by p1(A) x p0(W) into the cross accumulator.
 //
-// tc_conv_kernel is PERSISTENT: one CTA per SM walks a static round-robin list of output tiles; TMEM holds two
-// accumulator sets, so the epilogue warps drain tile n while the MMA thread accumulates tile n+1 and the TMA ring
-// streams across tile boundaries.  Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer,
-// warps 2-5 = epilogue (TMEM -> registers -> fused math -> stores coalesced along T).
+// tc_conv_kernel is PERSISTENT: one CTA per SM walks a static round-robin list of output tiles and the TMA ring
+// streams across tile boundaries, so the loads of tile n+1 overlap the epilogue of tile n.  Warp roles (288 threads):
+// warps 0-3 and 4-7 = two consumer warpgroups, each accumulating 64 of the 128 tile rows in registers (wgmma), then
+// handing the accumulators over 32 columns at a time through a shared-memory tile to warpgroup 0, whose thread r owns
+// row r (time step) in the epilogue (fused math -> stores coalesced along T); warp 8 = TMA producer.
 //
 // What the epilogues fuse besides the block's own math (Dv3TcFuse, include/dv3b200.h):
 //   * forward: the bf16 hi/lo planes -- with the CONSUMER's input dropout applied -- that the next convolution reads,
@@ -34,11 +35,13 @@ namespace dv3 {
 
 using namespace tc;
 
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 288;
 constexpr int MAX_TAPS_TC = 8;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memory per CTA
 constexpr int EPI_BUF = 16384;              // epilogue -> TMA-store staging buffer: hi 8 KB | lo 8 KB
 constexpr int EPI_STAGING = 2 * EPI_BUF;
+constexpr int ACC_PITCH = 33;               // accumulator hand-over tile: [128 rows][32 columns], padded rows
+constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
 
 enum { TC_GATED = 0, TC_CONV = 1 };
 enum { POST_NONE = 0, POST_GLU = 1, POST_HIGHWAY = 2, POST_RELU = 3, POST_IDENT = 4 };
@@ -67,27 +70,22 @@ struct TcParams {
     int post_kind, post_residual, post_pitch;
     const float* post_a; const float* post_s; const float* post_x;
     __nv_bfloat16* post_planes; long long post_plane; float* post_dbias;
-    // Compensation of the tensor core's truncating accumulation: every tcgen05.mma adds its K = 16 partial product
-    // into the fp32 accumulator rounding TOWARD ZERO, an expected relative loss of ~0.35 * 2^-23 per event on the
-    // running sum; over the n_mma events of one output that is a systematic shrink of ~gcoef * n_mma (measured,
-    // tools/precision_presets.py).  The epilogue multiplies the main accumulator by gmain = 1 + gcoef * n_mma (the
-    // cross-term accumulator is 2^-8 smaller: its loss is below fp32 resolution).
+    // Compensation of the tensor core's truncating accumulation: every MMA adds its K = 16 partial product into the
+    // fp32 accumulator rounding TOWARD ZERO, a small expected relative loss per event on the running sum; over the
+    // n_mma events of one output that is a systematic shrink of ~gcoef * n_mma (tools/trunc_bias.py measures gcoef).
+    // The epilogue multiplies the main accumulator by gmain = 1 + gcoef * n_mma (the cross-term accumulator is 2^-8
+    // smaller: its loss is below fp32 resolution).
     float gmain;
-    uint32_t idesc_fmt;        // a_format / b_format bits of the instruction descriptor (fp16 forward, bf16 gradients)
+    int operand_bf16;          // operand format of the MMAs: 0 = fp16 planes (forward), 1 = bf16 planes (gradients)
 };
 
 template <int BK> struct SwizzleOf;
-template <> struct SwizzleOf<64> { static constexpr uint32_t layout = 2, sbo = 1024; };   // SWIZZLE_128B
-template <> struct SwizzleOf<32> { static constexpr uint32_t layout = 4, sbo = 512; };    // SWIZZLE_64B
+template <> struct SwizzleOf<64> { static constexpr uint32_t layout = WG_SW128, sbo = 1024; };
+template <> struct SwizzleOf<32> { static constexpr uint32_t layout = WG_SW64, sbo = 512; };
 
 template <int BK>
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                 // start address / 16
-    d |= (uint64_t)(SwizzleOf<BK>::sbo >> 4) << 32;          // stride between 8-row swizzle atoms
-    d |= (uint64_t)1 << 46;                                  // sm_100 descriptor version
-    d |= (uint64_t)SwizzleOf<BK>::layout << 61;
-    return d;
+    return make_wgmma_desc(saddr, 16, SwizzleOf<BK>::sbo, SwizzleOf<BK>::layout);
 }
 
 // BR = rows of one B-operand box (128, or 64 for problems too small to fill the machine with 128-wide tiles)
@@ -96,20 +94,29 @@ struct TcCfg {
     static constexpr int TILE = 128 * BK * 2;            // A tile (128 rows)
     static constexpr int TILE_B = BR * BK * 2;           // one B box
     static constexpr int STAGE = 2 * (TILE + NBOX * TILE_B);
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_STAGING) / STAGE;
+    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_STAGING - ACC_TILE) / STAGE;
     static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-    static constexpr int SMEM = STAGES * STAGE + EPI_STAGING + 1024 + 512;   // + alignment slack + barriers
-    static constexpr int NCOLS = BR * NBOX;              // columns per accumulator; (main, cross) x two sets
+    static constexpr int SMEM = STAGES * STAGE + EPI_STAGING + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
+    static constexpr int NCOLS = BR * NBOX;              // columns per accumulator (main, cross)
 };
 
-// main + cross accumulator -> registers, summed in fp32 (round-to-nearest)
-// gmain = 1 + (expected relative truncation loss of the main accumulator), see TcParams::gmain
-__device__ __forceinline__ void tmem_ld_add(uint32_t taddr, int cross_off, float* v, float gmain) {
-    float c[32];
-    tmem_ld_32x32(taddr, v);
-    tmem_ld_32x32(taddr + cross_off, c);
+__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
+
+// Columns [c0, c0 + 32) of the summed accumulator (registers [0, NR) of both consumer warpgroups) -> row threadIdx.x
+// of that column chunk in v, for the threads of warpgroup 0.  Every consumer thread calls it with the same c0.
+template <int NR>
+__device__ __forceinline__ void acc_chunk(const float* acc, int c0, float* tile, int wg, int wq, int lane, float* v) {
+    consumer_bar();                                      // the previous chunk has been read
 #pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = fmaf(c[i], LO_INV, v[i] * gmain);       // lo planes carry a 2^11 scale
+    for (int i = 0; i < NR; ++i) {
+        const int c = frag_col(i, lane) - c0;
+        if (c >= 0 && c < 32) tile[(64 * wg + frag_row(i, wq, lane)) * ACC_PITCH + c] = acc[i];
+    }
+    consumer_bar();
+    if (wg == 0) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = tile[threadIdx.x * ACC_PITCH + i];
+    }
 }
 
 // ---- operand planes written by the epilogues: registers -> shared-memory staging -> TMA tensor store ---------------
@@ -193,8 +200,9 @@ __device__ __forceinline__ float warp_colsum32(float* v, int lane) {
 // must order every load after the previous iteration's stores (possible aliasing), which serialised 128
 // global-memory round trips per thread (ncu: 40 % of the stall samples sat on the first use of these loads).
 template <int BR, int NCOLS>
-__device__ __forceinline__ void epilogue_gated(const TcParams& p, uint32_t taddr, int a_row0, int a_z, int b_row0,
-                                               int row, EpiStage& es) {
+__device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* acc, float* tile, int wg, int wq,
+                                               int lane, int a_row0, int a_z, int b_row0, EpiStage& es) {
+    const int row = threadIdx.x & 127;
     const int t = a_row0 + row, b = a_z, C = p.Nc;
     const bool tv = t < p.T;
     const float* __restrict__ bias = p.bias;
@@ -206,10 +214,12 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, uint32_t taddr
     const bool need_res = (p.gate_mode != 0) || p.residual;
     const size_t base = ((size_t)b * C + b_row0) * p.T + (tv ? t : 0);
     const DropCfg nd = make_drop(p.np ? p.np_p : 0.f, p.np_seed, p.np_salt);
+#pragma unroll
     for (int c32 = 0; c32 < BR; c32 += 32) {
         float va[32], vb[32], rr[32];
-        tmem_ld_add(taddr + c32, NCOLS, va, p.gmain);
-        tmem_ld_add(taddr + BR + c32, NCOLS, vb, p.gmain);
+        acc_chunk<NCOLS / 2>(acc, c32, tile, wg, wq, lane, va);
+        acc_chunk<NCOLS / 2>(acc, BR + c32, tile, wg, wq, lane, vb);
+        if (wg != 0) continue;
         if (tv) {
             const size_t cb = base + (size_t)c32 * p.T;
 #pragma unroll
@@ -246,8 +256,9 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, uint32_t taddr
 }
 
 template <int NCOLS>
-__device__ __forceinline__ void epilogue_conv(const TcParams& p, uint32_t taddr, int a_row0, int a_z, int b_row0,
-                                              int row, int lane, EpiStage& es) {
+__device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* acc, float* tile, int wg, int wq,
+                                              int lane, int a_row0, int a_z, int b_row0, EpiStage& es) {
+    const int row = threadIdx.x & 127;
     const int t = a_row0 + row, b = a_z;
     const bool tv = t < p.T;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
@@ -261,9 +272,11 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, uint32_t taddr,
     float* __restrict__ out = p.out;
     const int kind = p.post_kind;
     const float gs = (kind == POST_GLU && p.post_residual) ? 0.70710678118654752f : 1.f;
+#pragma unroll
     for (int c32 = 0; c32 < NCOLS; c32 += 32) {
         float v[32], x1[32], x2[32];
-        tmem_ld_add(taddr + c32, NCOLS, v, p.gmain);
+        acc_chunk<NCOLS / 2>(acc, c32, tile, wg, wq, lane, v);
+        if (wg != 0) continue;
         const int n0 = b_row0 + c32;
         const size_t cb = ((size_t)b * p.Nc + n0) * p.T + (tv ? t : 0);
         if (tv) {
@@ -342,9 +355,10 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, uint32_t taddr,
 }
 
 // ------------------------------------------------------------------------------------------------
-// GATED / CONV kernel (persistent, see file header).  N per tile is limited to 128 columns (4 x 128 = 512 TMEM columns).
+// GATED / CONV kernel (persistent, see file header).  N per tile is limited to 128 columns: the main and cross
+// accumulators of a consumer warpgroup take 2 x 64 registers per thread.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int NBOX, int BR, int BK>
+template <int MODE, int NBOX, int BR, int BK, bool BF16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int tiles_x, int tiles_y,
                int num_tiles) {
@@ -352,16 +366,16 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     using Cfg = TcCfg<NBOX, BK, BR>;
     constexpr int TILE = Cfg::TILE, TILE_B = Cfg::TILE_B, STAGE = Cfg::STAGE, STAGES = Cfg::STAGES, NCOLS = Cfg::NCOLS;
     constexpr int B_OFF = 2 * TILE;
-    static_assert(4 * NCOLS <= 512, "two accumulator sets of (main + cross) must fit in TMEM");
+    constexpr int NR = NCOLS / 2;                            // registers per accumulator per thread
+    constexpr int A_HALF = 64 * BK * 2;                      // rows [64 wg, 64 wg + 64) of the A tile
+    static_assert(NCOLS <= 128, "main + cross accumulators must fit in the registers of a consumer thread");
     static_assert(STAGES >= 2, "pipeline needs at least two stages");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* staging = smem + STAGES * STAGE;                // epilogue -> TMA store tiles (1024-aligned: STAGE % 1024 == 0)
-    uint64_t* full = reinterpret_cast<uint64_t*>(staging + EPI_STAGING);
+    float* acc_tile = reinterpret_cast<float*>(staging + EPI_STAGING);
+    uint64_t* full = reinterpret_cast<uint64_t*>(staging + EPI_STAGING + ACC_TILE);
     uint64_t* empty = full + STAGES;
-    uint64_t* tfull = empty + STAGES;          // [2] accumulator set ready for the epilogue
-    uint64_t* tempty = tfull + 2;              // [2] accumulator set drained
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tempty + 2);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_iters = p.k * p.kb_n;
 
@@ -369,15 +383,10 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         prefetch_tmap(&maps.a[0]); prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.b[0]); prefetch_tmap(&maps.b[1]);
         if (p.np || p.post_kind) { prefetch_tmap(&maps.st[0]); prefetch_tmap(&maps.st[1]); }
         if (p.np_wg) { prefetch_tmap(&maps.st[2]); prefetch_tmap(&maps.st[3]); }
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], 128); }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<4 * NCOLS>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     pdl_wait();                    // everything above overlapped the previous kernel's tail; global memory from here
 
     // tile id -> (time tile, channel tile, batch); channel tiles vary fastest so that concurrently running CTAs share
@@ -391,85 +400,77 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         else { b_row0 = ty * BR * NBOX; b_row1 = b_row0 + BR; }
     };
 
-    if (warp == 0 && lane == 0) {
+    if (warp == 8) {
+        if (lane == 0) {
+            int it = 0;
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                int a_row0, a_z, b_row0, b_row1;
+                decode(tile, a_row0, a_z, b_row0, b_row1);
+                for (int kit = 0; kit < n_iters; ++kit, ++it) {
+                    const int s = it % STAGES, ph = (it / STAGES) & 1;
+                    mbar_wait(&empty[s], ph ^ 1);
+                    uint8_t* st = smem + s * STAGE;
+                    const int j = kit / p.kb_n, kb = kit - j * p.kb_n;
+                    const int ax = kb * BK, ay = a_row0 + p.tap_off[j];
+                    const int by0 = j * p.rows_per_tap + b_row0, by1 = j * p.rows_per_tap + b_row1;
+                    mbar_arrive_expect_tx(&full[s], STAGE);
+#pragma unroll
+                    for (int pl = 0; pl < 2; ++pl) {
+                        tma_load_3d(st + pl * TILE, &maps.a[pl], &full[s], ax, ay, a_z);
+                        uint8_t* bdst = st + B_OFF + pl * NBOX * TILE_B;
+                        tma_load_3d(bdst, &maps.b[pl], &full[s], ax, by0, 0);
+                        if (NBOX == 2) tma_load_3d(bdst + TILE_B, &maps.b[pl], &full[s], ax, by1, 0);
+                    }
+                }
+            }
+        }
+    } else {
+        const int wg = warp >> 2, wq = warp & 3;
+        EpiStage es;
+        es.base = staging; es.map = maps.st; es.uses = 0; es.issuer = (threadIdx.x == 0);
+        float acc[2 * NR];                                   // [0, NR): main, [NR, 2 NR): cross
         int it = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int a_row0, a_z, b_row0, b_row1;
             decode(tile, a_row0, a_z, b_row0, b_row1);
-            for (int kit = 0; kit < n_iters; ++kit, ++it) {
-                const int s = it % STAGES, ph = (it / STAGES) & 1;
-                mbar_wait(&empty[s], ph ^ 1);
-                uint8_t* st = smem + s * STAGE;
-                const int j = kit / p.kb_n, kb = kit - j * p.kb_n;
-                const int ax = kb * BK, ay = a_row0 + p.tap_off[j];
-                const int by0 = j * p.rows_per_tap + b_row0, by1 = j * p.rows_per_tap + b_row1;
-                mbar_arrive_expect_tx(&full[s], STAGE);
 #pragma unroll
-                for (int pl = 0; pl < 2; ++pl) {
-                    tma_load_3d(st + pl * TILE, &maps.a[pl], &full[s], ax, ay, a_z);
-                    uint8_t* bdst = st + B_OFF + pl * NBOX * TILE_B;
-                    tma_load_3d(bdst, &maps.b[pl], &full[s], ax, by0, 0);
-                    if (NBOX == 2) tma_load_3d(bdst + TILE_B, &maps.b[pl], &full[s], ax, by1, 0);
-                }
-            }
-        }
-    } else if (warp == 1 && lane == 0) {
-        const uint32_t idesc = make_idesc_mn(128, NCOLS) | p.idesc_fmt, idesc2 = make_idesc_mn(128, 2 * NCOLS) | p.idesc_fmt;
-        int it = 0, tcount = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
-            const int a = tcount & 1, aph = (tcount >> 1) & 1;
-            mbar_wait(&tempty[a], aph ^ 1);                         // the epilogue has drained this accumulator set
-            tc_fence_after();
-            const uint32_t acc = tmem_base + a * 2 * NCOLS;
+            for (int i = 0; i < 2 * NR; ++i) acc[i] = 0.f;
             for (int kit = 0; kit < n_iters; ++kit, ++it) {
                 const int s = it % STAGES, ph = (it / STAGES) & 1;
                 mbar_wait(&full[s], ph);
-                tc_fence_after();
-                const uint32_t sa = smem_u32(smem + s * STAGE);
-                const uint64_t da0 = make_desc<BK>(sa), da1 = make_desc<BK>(sa + TILE);
-                const uint64_t db0 = make_desc<BK>(sa + B_OFF);         // plane 1 follows plane 0: rows [NCOLS, 2 NCOLS)
+                const uint32_t sa = smem_u32(smem + s * STAGE) + wg * A_HALF;
+                const uint32_t sb = smem_u32(smem + s * STAGE + B_OFF);   // plane 1 follows plane 0: rows [NCOLS, 2 NCOLS)
+                wgmma_fence();
 #pragma unroll
                 for (int kk = 0; kk < BK / 16; ++kk) {
-                    const uint64_t adv = (uint64_t)(kk * 2);
-                    umma_bf16(acc, da0 + adv, db0 + adv, idesc2, (kit | kk) != 0);     // p0 x [p0 ; p1] -> main | cross
-                    umma_bf16(acc + NCOLS, da1 + adv, db0 + adv, idesc, 1);
+                    const uint32_t ko = kk * 32;
+                    wgmma_mma<2 * NCOLS, 0, 0>(BF16, acc, make_desc<BK>(sa + ko), make_desc<BK>(sb + ko), 1);  // p0 x [p0 ; p1]
+                    wgmma_mma<NCOLS, 0, 0>(BF16, acc + NR, make_desc<BK>(sa + TILE + ko), make_desc<BK>(sb + ko), 1);
                 }
-                umma_commit(&empty[s]);
+                wgmma_commit();
+                wgmma_wait<1>();                                  // the previous stage's MMAs have retired
+                if (kit > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
             }
-            umma_commit(&tfull[a]);
-        }
-    } else if (warp >= 2) {
-        const int q = warp & 3, row = q * 32 + lane;
-        EpiStage es;
-        es.base = staging; es.map = maps.st; es.uses = 0; es.issuer = (warp == 2 && lane == 0);
-        int tcount = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++tcount) {
-            int a_row0, a_z, b_row0, b_row1;
-            decode(tile, a_row0, a_z, b_row0, b_row1);
-            const int a = tcount & 1, aph = (tcount >> 1) & 1;
-            mbar_wait(&tfull[a], aph);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + a * 2 * NCOLS + ((uint32_t)(q * 32) << 16);
-            if (MODE == TC_GATED) epilogue_gated<BR, NCOLS>(p, taddr, a_row0, a_z, b_row0, row, es);
-            else epilogue_conv<NCOLS>(p, taddr, a_row0, a_z, b_row0, row, lane, es);
-            tc_fence_before();
-            mbar_arrive(&tempty[a]);                                // 128 arrivals release the set to the MMA thread
+            wgmma_wait<0>();
+            if (n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+#pragma unroll
+            for (int i = 0; i < NR; ++i) acc[i] = fmaf(acc[NR + i], LO_INV, acc[i] * p.gmain);   // lo planes carry 2^11
+            if (MODE == TC_GATED) epilogue_gated<BR, NCOLS>(p, acc, acc_tile, wg, wq, lane, a_row0, a_z, b_row0, es);
+            else epilogue_conv<NCOLS>(p, acc, acc_tile, wg, wq, lane, a_row0, a_z, b_row0, es);
         }
         if (es.issuer) bulk_wait_all();                             // plane stores complete before the CTA exits
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<4 * NCOLS>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Weight gradient straight from the (B,T,C) planes the forward / data-gradient GEMMs already use:
 //     D[m, n] (tap j) = sum_{b,t} dY[b, t, m] * Xd[b, t + off_j, n]
 // Both operands are "MN-major" here (channels contiguous, the contraction index t is the row): 64-channel x 32-row
-// TMA boxes (128-byte rows, SWIZZLE_128B), UMMA descriptors with the MN-major canonical layout
-// ((64 channels contiguous, chunk stride LBO), (8 rows x 128 B, group stride SBO)) and a_major = b_major = 1 in the
-// instruction descriptor.  The tap shift is a ROW coordinate of the TMA box (any alignment, out-of-bounds rows are
-// zero = the conv padding), so no time-shifted copies of the input are needed.
+// TMA boxes (128-byte rows, SWIZZLE_128B), wgmma descriptors with the MN-major canonical layout
+// ((64 channels contiguous, chunk stride LBO), (8 rows x 128 B, group stride SBO)) and both operands transposed in the
+// instruction.  The tap shift is a ROW coordinate of the TMA box (any alignment, out-of-bounds rows are zero = the
+// conv padding), so no time-shifted copies of the input are needed.  Tile 128 (m) x 128 (n); each consumer warpgroup
+// owns 64 rows of m and writes its partials straight from the accumulator registers.
 // ------------------------------------------------------------------------------------------------
 struct TcMnParams {
     int T, B, Mw, Nw, k;
@@ -480,128 +481,95 @@ struct TcMnParams {
     float gcoef;                              // see TcParams::gmain (n_mma = 2 per 32-row time chunk)
 };
 
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;                    // SWIZZLE_128B
-    return d;
-}
+constexpr int WG_BOX = 64 * 32 * 2;                      // 64 channels x 32 time steps of bf16 = 4 KB
+constexpr int WG_STAGE = 2 * (2 * WG_BOX + 2 * WG_BOX);  // per plane: 128 channels of m, 128 channels of n
+constexpr int WG_STAGES = ((SMEM_LIMIT - 2048) / WG_STAGE) > 6 ? 6 : ((SMEM_LIMIT - 2048) / WG_STAGE);
+constexpr int WG_SMEM = WG_STAGES * WG_STAGE + 1024 + 512;
 
-template <int NBOX>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcMnParams p) {
     pdl_trigger();
-    constexpr int BOX = 64 * 32 * 2;                     // 64 channels x 32 time steps of bf16 = 4 KB
-    constexpr int A_PL = 2 * BOX, B_PL = 2 * NBOX * BOX; // per plane: 128 rows of M, 128*NBOX columns of N
-    constexpr int STAGE = 2 * (A_PL + B_PL);
-    constexpr int STAGES = ((SMEM_LIMIT - 2048) / STAGE) > 6 ? 6 : ((SMEM_LIMIT - 2048) / STAGE);
-    constexpr int NCOLS = 128 * NBOX;
+    constexpr int A_PL = 2 * WG_BOX, B_PL = 2 * WG_BOX;
     constexpr uint32_t LBO = 4096, SBO = 1024;           // 64-channel chunks one TMA box apart; 8-row groups 1 KB apart
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE);
-    uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE);
+    uint64_t* empty = full + WG_STAGES;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     const int wg_j = blockIdx.z % p.k, wg_split = blockIdx.z / p.k;
-    const int m0 = blockIdx.y * 128, n0 = blockIdx.x * 128 * NBOX;
+    const int m0 = blockIdx.y * 128, n0 = blockIdx.x * 128;
     const int b_beg = wg_split * p.batches_per_split;
     int b_end = b_beg + p.batches_per_split; if (b_end > p.B) b_end = p.B;
     const int n_iters = (b_end > b_beg ? b_end - b_beg : 0) * p.kb_n;
 
     if (threadIdx.x == 0) {
         prefetch_tmap(&maps.a[0]); prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.b[0]); prefetch_tmap(&maps.b[1]);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(tmem_full, 1);
+        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<2 * NCOLS>(tmem_ptr);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr;
     pdl_wait();
 
-    if (warp == 0 && lane == 0) {
-        for (int it = 0; it < n_iters; ++it) {
-            const int s = it % STAGES, ph = (it / STAGES) & 1;
-            mbar_wait(&empty[s], ph ^ 1);
-            uint8_t* st = smem + s * STAGE;
-            const int bi = it / p.kb_n, tc_ = it - bi * p.kb_n;
-            const int b = b_beg + bi, t0 = tc_ * 32;
-            mbar_arrive_expect_tx(&full[s], STAGE);
+    if (warp == 8) {
+        if (lane == 0) {
+            for (int it = 0; it < n_iters; ++it) {
+                const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
+                mbar_wait(&empty[s], ph ^ 1);
+                uint8_t* st = smem + s * WG_STAGE;
+                const int bi = it / p.kb_n, tc_ = it - bi * p.kb_n;
+                const int b = b_beg + bi, t0 = tc_ * 32;
+                mbar_arrive_expect_tx(&full[s], WG_STAGE);
 #pragma unroll
-            for (int pl = 0; pl < 2; ++pl) {
+                for (int pl = 0; pl < 2; ++pl) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    tma_load_3d(st + pl * A_PL + h * BOX, &maps.a[pl], &full[s], m0 + h * 64, t0, b);
+                    for (int h = 0; h < 2; ++h)
+                        tma_load_3d(st + pl * A_PL + h * WG_BOX, &maps.a[pl], &full[s], m0 + h * 64, t0, b);
 #pragma unroll
-                for (int q = 0; q < 2 * NBOX; ++q)
-                    tma_load_3d(st + 2 * A_PL + pl * B_PL + q * BOX, &maps.b[pl], &full[s], n0 + q * 64,
-                                t0 + p.tap_off[wg_j], b);
+                    for (int q = 0; q < 2; ++q)
+                        tma_load_3d(st + 2 * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], &full[s], n0 + q * 64,
+                                    t0 + p.tap_off[wg_j], b);
+                }
             }
         }
-    } else if (warp == 1 && lane == 0) {
+    } else {
         // A = gradient planes, B = the bf16 copy of the forward operand planes; both MN-major
-        constexpr uint32_t idesc = make_idesc_bf16(128, NCOLS) | (1u << 15) | (1u << 16);
+        const int wg = warp >> 2, wq = warp & 3;
+        float acc[128];                                      // [0, 64): main, [64, 128): cross
+#pragma unroll
+        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
         for (int it = 0; it < n_iters; ++it) {
-            const int s = it % STAGES, ph = (it / STAGES) & 1;
+            const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
             mbar_wait(&full[s], ph);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + s * STAGE);
+            const uint32_t sa = smem_u32(smem + s * WG_STAGE);
+            wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {                        // 2 x UMMA_K(16 rows of 128 B)
+            for (int kk = 0; kk < 2; ++kk) {                        // 2 x K = 16 rows of 128 B
                 const uint32_t ko = kk * 16 * 128;
-                const uint64_t a0 = make_desc_mn(sa + ko, LBO, SBO);
-                const uint64_t a1 = make_desc_mn(sa + A_PL + ko, LBO, SBO);
-                const uint64_t b0 = make_desc_mn(sa + 2 * A_PL + ko, LBO, SBO);
-                const uint64_t b1 = make_desc_mn(sa + 2 * A_PL + B_PL + ko, LBO, SBO);
-                umma_bf16(tmem_base, a0, b0, idesc, (it | kk) != 0);
-                umma_bf16(tmem_base + NCOLS, a0, b1, idesc, (it | kk) != 0);
-                umma_bf16(tmem_base + NCOLS, a1, b0, idesc, 1);
+                const uint64_t a0 = make_wgmma_desc(sa + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+                const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+                const uint64_t b0 = make_wgmma_desc(sa + 2 * A_PL + ko, LBO, SBO, WG_SW128);
+                const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
+                wgmma_mma<128, 1, 1>(true, acc, a0, b0, 1);
+                wgmma_mma<128, 1, 1>(true, acc + 64, a0, b1, 1);
+                wgmma_mma<128, 1, 1>(true, acc + 64, a1, b0, 1);
             }
-            umma_commit(&empty[s]);
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (it > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
         }
-        umma_commit(tmem_full);
-    } else if (warp >= 2) {
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
-        const int q = warp & 3, row = q * 32 + lane;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16);
-        const int m = m0 + row;
+        wgmma_wait<0>();
         float* __restrict__ out = p.dw + (size_t)wg_split * p.split_stride + (size_t)wg_j * p.s_j;
-        const size_t ma = (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh;
-        // partials with unit stride along n ([split][j][m][n]): each thread owns a contiguous run -> float4 stores
-        const bool vec = (p.s_n == 1) && ((p.Nw & 3) == 0) &&
-                         (((ma + (size_t)wg_j * p.s_j + (size_t)wg_split * p.split_stride) & 3) == 0);
-        for (int c32 = 0; c32 < NCOLS; c32 += 32) {
-            float v[32];
-            tmem_ld_add(taddr + c32, NCOLS, v, 1.f + p.gcoef * (float)(2 * n_iters));
-            if (m >= p.Mw) continue;
-            const int nn = n0 + c32;
-            if (n_iters == 0) {
+        const float gmain = 1.f + p.gcoef * (float)(2 * n_iters);
 #pragma unroll
-                for (int i = 0; i < 32; ++i) v[i] = 0.f;
-            }
-            if (vec && nn + 32 <= p.Nw) {
-#pragma unroll
-                for (int i = 0; i < 32; i += 4)
-                    *reinterpret_cast<float4*>(&out[ma + nn + i]) = make_float4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-            } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i)
-                    if (nn + i < p.Nw) out[ma + (size_t)(nn + i) * p.s_n] = v[i];
+        for (int i = 0; i < 64; ++i) {
+            const int m = m0 + 64 * wg + frag_row(i, wq, lane), n = n0 + frag_col(i, lane);
+            if (m < p.Mw && n < p.Nw) {
+                const size_t ma = (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh;
+                out[ma + (size_t)n * p.s_n] = fmaf(acc[64 + i], LO_INV, acc[i] * gmain);
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<2 * NCOLS>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -650,11 +618,11 @@ static int ensure_smem(K kern, int bytes, const char* what) {
     return 0;
 }
 
-template <int MODE, int NBOX, int BR, int BK>
-static int launch_conv(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
+template <int MODE, int NBOX, int BR, int BK, bool BF16>
+static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
                        const char* what) {
     using Cfg = TcCfg<NBOX, BK, BR>;
-    auto kern = tc_conv_kernel<MODE, NBOX, BR, BK>;
+    auto kern = tc_conv_kernel<MODE, NBOX, BR, BK, BF16>;
     static const int configured = ensure_smem(kern, Cfg::SMEM, what);       // once per instantiation, thread-safe
     if (configured) return 1;
     const int sms = config().sms;
@@ -664,6 +632,13 @@ static int launch_conv(const TcMaps& maps, const TcParams& p, int tiles_x, int t
                              num_tiles);
     if (e != cudaSuccess) { set_error("%s: launch failed: %s", what, cudaGetErrorString(e)); return 1; }
     return check_launch(what);
+}
+
+template <int MODE, int NBOX, int BR, int BK>
+static int launch_conv(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
+                       const char* what) {
+    if (p.operand_bf16) return launch_conv_fmt<MODE, NBOX, BR, BK, true>(maps, p, tiles_x, tiles_y, batch, st, what);
+    return launch_conv_fmt<MODE, NBOX, BR, BK, false>(maps, p, tiles_x, tiles_y, batch, st, what);
 }
 
 static void fill_taps_tc(int* tap_off, int k, int dilation, int causal, bool transpose) {
@@ -755,7 +730,7 @@ int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bi
     p.bias = bias; p.spk = spk; p.res = res; p.y = y; p.save_a = save_a; p.save_s = save_s;
     p.gate_mode = mode; p.residual = residual;
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * 4);
-    p.idesc_fmt = IDESC_A_F16 | IDESC_B_F16;                     // forward operands: fp16 hi/lo planes
+    p.operand_bf16 = 0;                                          // forward operands: fp16 hi/lo planes
     if (apply_fuse(p, maps, fuse, B, T, C, "tc_convblock_fwd")) return 1;
     DV3_REQUIRE(p.post_kind == POST_NONE, "tc_convblock_fwd: post_kind is a data-gradient option");
     return launch_conv<TC_GATED, 2, 64, 64>(maps, p, t_tiles, C / 64, B, (cudaStream_t)stream, "tc_convblock_fwd");
@@ -794,7 +769,7 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     p.p_drop = p_drop; p.seed_ptr = seed_ptr; p.salt = salt;
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (bk / 16));
     // forward conv: fp16 activation x fp16 weight planes; data gradient: bf16 gradient x bf16 weight planes
-    p.idesc_fmt = transpose_taps ? (IDESC_A_BF16 | IDESC_B_BF16) : (IDESC_A_F16 | IDESC_B_F16);
+    p.operand_bf16 = transpose_taps ? 1 : 0;
     if (apply_fuse(p, maps, fuse, B, T, Nc, "tc_conv")) return 1;
     const int tiles_y = (Nc + br - 1) / br;
     if (narrow) {
@@ -806,14 +781,12 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
 }
 
 int dv3_tc_wgrad_nsplit(int B, int Mw, int Nw, int T, int k) {
-    const int nt = Nw > 128 ? (Nw + 255) / 256 : 1;
-    const int tiles = ((Mw + 127) / 128) * nt * k;
+    const int tiles = ((Mw + 127) / 128) * ((Nw + 127) / 128) * k;
     // split (b,t) over enough CTAs for two waves, unless that leaves each CTA fewer than ~64 K-iterations (then the
     // per-CTA prologue/epilogue and the extra partial traffic cost more than the parallelism buys: one wave).
-    // Measured on the preset shapes (tools/tc_time.py): (512,800) prefers 296, (256,800)/(512,128)/(256,200) prefer 148.
-    const int kb_n = (T + 31) / 32;
+    const int kb_n = (T + 31) / 32, sms = config().sms;
     int best = 1;
-    for (int target = 2 * 148; target >= 148; target -= 148) {
+    for (int target = 2 * sms; target >= sms; target -= sms) {
         int want = (target + tiles - 1) / tiles;
         if (want > B) want = B;
         if (want < 1) want = 1;
@@ -848,19 +821,10 @@ int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long lon
     p.gcoef = config().tc_gamma;
     cudaStream_t st = (cudaStream_t)stream;
     const int m_tiles = (Mw + 127) / 128;
-    cudaError_t e;
-    if (Nw > 128) {
-        constexpr int SMEM = 4 * 2 * (2 * 4096 + 4 * 4096) + 1024 + 512;
-        static const int configured = ensure_smem(tc_wgrad_mn_kernel<2>, SMEM, "tc_wgrad_mn");
-        if (configured) return 1;
-        e = launch_k(tc_wgrad_mn_kernel<2>, dim3((Nw + 255) / 256, m_tiles, p.nsplit * k), dim3(TC_THREADS), (size_t)SMEM,
-                     st, maps, p);
-    } else {
-        constexpr int SMEM = 6 * 2 * (2 * 4096 + 2 * 4096) + 1024 + 512;
-        static const int configured = ensure_smem(tc_wgrad_mn_kernel<1>, SMEM, "tc_wgrad_mn");
-        if (configured) return 1;
-        e = launch_k(tc_wgrad_mn_kernel<1>, dim3(1, m_tiles, p.nsplit * k), dim3(TC_THREADS), (size_t)SMEM, st, maps, p);
-    }
+    static const int configured = ensure_smem(tc_wgrad_mn_kernel, WG_SMEM, "tc_wgrad_mn");
+    if (configured) return 1;
+    const cudaError_t e = launch_k(tc_wgrad_mn_kernel, dim3((Nw + 127) / 128, m_tiles, p.nsplit * k), dim3(TC_THREADS),
+                                   (size_t)WG_SMEM, st, maps, p);
     if (e != cudaSuccess) { set_error("tc_wgrad_mn: launch failed: %s", cudaGetErrorString(e)); return 1; }
     return check_launch("tc_wgrad_mn");
 }

@@ -14,7 +14,7 @@ namespace dv3 {
 // ---- activation-side operand preparation: ONE kernel template, three uses ------------------------------------
 //   SPLIT_INPUT  x (B,C,T) -> conv-input dropout -> fp16 planes (B,T,Cp) [forward operand] and, when wg != NULL, the same
 //                values as a bf16 pair [operand of the weight gradient, which multiplies them with bf16 gradient
-//                planes: tcgen05 kind::f16 cannot mix fp16 and bf16 operands in one MMA]
+//                planes: a wgmma cannot mix fp16 and bf16 operands]
 //   SPLIT_GATE   gate backward (conv.cu gate_bwd_kernel) of dy with the saved a, s (, x) -> dAB = [da | db] as bf16
 //                planes (B,T,2C); dbias[2C] += sums over (b,t)                           [data-/weight-gradient operand]
 //   SPLIT_GRAD   g = dy * (relu ? y > 0 : 1) -> bf16 planes (B,T,Cp); dbias[C] += sums

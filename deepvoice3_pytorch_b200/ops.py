@@ -14,12 +14,12 @@ from ._lib import lib, Dv3Error
 MODE_GLU, MODE_HIGHWAY = 0, 1
 
 # Arithmetic of the ConvBlock / conv / attention contractions:
-#   "tc"     (default) tcgen05 tensor cores, every fp32 operand split into a 16-bit (hi, lo) pair, hi*hi + hi*lo + lo*hi
-#            with fp32 accumulation in TMEM (csrc/tc_gemm.cu, tc_attn.cu): fp16 pairs (22-bit operands) in the forward
+#   "tc"     (default) wgmma tensor cores, every fp32 operand split into a 16-bit (hi, lo) pair, hi*hi + hi*lo + lo*hi
+#            with fp32 accumulation in registers (csrc/tc_gemm.cu, tc_attn.cu): fp16 pairs (22-bit operands) in the forward
 #            GEMMs, bf16 pairs in the gradient GEMMs.  Full-depth preset models match the fp32 oracle at rtol 1e-3 /
 #            atol 1e-4 (tests/test_gpu_models.py).  Shapes the tensor-core kernels do not cover (C % 128 != 0, tiny
 #            GEMMs) run on the exact-fp32 kernels automatically.  ("bf16x3" is accepted as an alias.)
-#   "fp32"   exact-fp32 CUDA-core kernels everywhere (csrc/conv.cu, bgemm.cu): ~7x slower, the strict reference mode.
+#   "fp32"   exact-fp32 CUDA-core kernels everywhere (csrc/conv.cu, bgemm.cu): much slower, the strict reference mode.
 conv_math = os.environ.get("DV3_CONV_MATH", "tc")
 
 
@@ -271,7 +271,7 @@ class _ConvBlockFn(torch.autograd.Function):
 
 
 # The weight-gradient GEMM (+ the weight-norm backward that consumes it) and the data-gradient GEMM of a block are
-# independent: run the former on a side stream so the two overlap -- most layers launch only 32-128 CTAs on 148 SMs.
+# independent: run the former on a side stream so the two overlap -- most layers launch only 32-128 CTAs on 132 SMs.
 # Fork/join with stream waits, which a CUDA-graph capture records as graph edges.
 overlap_wgrad = os.environ.get("DV3_OVERLAP_WGRAD", "1") == "1"
 _side_streams = {}
@@ -317,8 +317,7 @@ def _pad8(n):
 # fuse_bwd: the data-gradient GEMM of the consumer applies the producer's backward (gate / ReLU) in its epilogue and
 #           emits the producer's gradient planes + bias-gradient sums -> no dv3_tc_gate_bwd_split / dv3_tc_grad_split.
 # Both need the caller (modules.run_conv_stack) to state that the tensor has exactly ONE consumer.
-# Both are OFF by default: measured on the B200 (profiles/r02_fusion_ab.txt) the fused step is SLOWER (7.26 vs 6.34 ms,
-# forward fusion alone 6.45): the separate split / gate-backward kernels stream at HBM speed with full occupancy, while
+# Both are OFF by default: the separate split / gate-backward kernels stream at HBM speed with full occupancy, while
 # inside the GEMM the same work is done by the 4 epilogue warps of each SM (latency bound), and at C = 256 the fused
 # data-gradient epilogue of a 128x128 tile takes longer than the tile's MMAs.  Kept opt-in because the arithmetic is
 # bit-identical (tests/test_gpu_fusion.py) and the trade flips for wider layers.
@@ -418,7 +417,7 @@ def _rec_sink_bias(rec):
 
 
 class _ConvBlockTCFn(torch.autograd.Function):
-    """Same contract as _ConvBlockFn on the tcgen05 path: operands are bf16 hi/lo planes.
+    """Same contract as _ConvBlockFn on the tensor-core path: operands are bf16 hi/lo planes.
     xh: Planes of x written by the producer (or None -> split here); emit_p: input dropout of the single consumer
     (None: no planes emitted); link: ProducerRec of x's producer when this block is its only consumer."""
 
@@ -555,7 +554,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
 
 
 class _Conv1dTCFn(torch.autograd.Function):
-    """Plain weight-normed conv (+ReLU) on the tcgen05 path (1x1 convs, projections)."""
+    """Plain weight-normed conv (+ReLU) on the tensor-core path (1x1 convs, projections)."""
 
     @staticmethod
     def forward(ctx, x, v, g, bias, k, dilation, causal, relu, xh, emit_p, training, link, want_rec, box):
@@ -666,7 +665,7 @@ class _Conv1dTCFn(torch.autograd.Function):
 
 
 class _ConvT2TCFn(torch.autograd.Function):
-    """ConvTranspose1d(k=2,s=2) on the tcgen05 path: a 1x1 conv with 2*Cout rows (j,co) + the time interleave."""
+    """ConvTranspose1d(k=2,s=2) on the tensor-core path: a 1x1 conv with 2*Cout rows (j,co) + the time interleave."""
 
     @staticmethod
     def forward(ctx, x, v, g, bias, xh, link):
@@ -1124,7 +1123,7 @@ tc_attention = os.environ.get("DV3_TC_ATTN", "1") == "1"      # 0: attention on 
 
 
 class _AttentionTCFn(torch.autograd.Function):
-    """The same contract on the fused tcgen05 kernels (csrc/tc_attn.cu): one launch forward, two backward."""
+    """The same contract on the fused tensor-core kernels (csrc/tc_attn.cu): one launch forward, two backward."""
 
     @staticmethod
     def forward(ctx, q, k, v, mask, p_drop, training):

@@ -1,4 +1,4 @@
-"""One data-parallel training step of the hot path, B200-first.
+"""One data-parallel training step of the hot path.
 
 What the reference does per step (train.py:621-779) -- H2D of the batch, model forward, the four losses,
 backward, ``clip_grad_norm_``, ``Adam.step`` -- restated around three ideas:

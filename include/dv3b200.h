@@ -1,4 +1,4 @@
-/* dv3b200 -- C ABI of the B200-native hot path of r9y9/deepvoice3_pytorch.
+/* dv3b200 -- C ABI of the H100-native hot path of r9y9/deepvoice3_pytorch.
  *
  * The reference has no FFI of its own (it is pure Python on ATen): the seam it offers is the Python
  * module API (deepvoice3_pytorch.builder.* -> nn.Module, SURVEY.md section 8b).  This header is the
@@ -122,7 +122,7 @@ int dv3_bgemm(const float* A, long long sAb, long long sAm, long long sAk, const
               long long sBk, long long sBn, float* C, long long sCb, int ldc, int batch, int M, int N, int K,
               float alpha, int accumulate, void* stream);
 
-/* ---- fused tensor-core attention (tcgen05, split-bf16 operands staged and split in-kernel): reference
+/* ---- fused tensor-core attention (wgmma, split-bf16 operands staged and split in-kernel): reference
  * deepvoice3.py:132-176 between the projections.  q (B,E,Td), k / v (B,E,Ts), mask (B,Ts) bytes (1 = padding) or
  * null -> probs (B,Td,Ts) = softmax(q^T k) (pre-dropout, returned as the alignment), out (B,E,Td) =
  * scale * v . dropout(probs)^T.  Backward: dout (B,E,Td), dprobs (B,Td,Ts) gradient arriving at the returned
@@ -174,7 +174,7 @@ int dv3_stft_complex(const float* wav, int n_samples, const float* mag, float* s
 int dv3_istft(const float* spec, float* wav, int n_samples, int nframes, void* stream);
 int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long long stride, float coef, void* stream);
 
-/* ================= tensor-core ConvBlock / conv path: tcgen05 + TMA, split-bf16 operands =================
+/* ================= tensor-core ConvBlock / conv path: wgmma + TMA, split-bf16 operands =================
  * Same reference code as dv3_convblock_fwd / dv3_conv1d_fwd / dv3_conv1d_dgrad / dv3_conv1d_wgrad (modules.py:94-100,
  * 145-164, 200-226 and their autograd).  fp32 operands are split into bf16 planes p0 = bf16(x), p1 = bf16(x-p0)
  * [, p2 = bf16(x-p0-p1)]; npl = 2 issues p0*p0 + p0*p1 + p1*p0 ("x3", ~2^-17/operand), npl = 3 adds
@@ -185,7 +185,7 @@ int dv3_tc_conv_supported(int B, int Cin, int Cout, int T, int k);   /* plain co
 /* Operand planes: every fp32 operand x travels as hi = rn16(x), lo = rn16((x - hi) * 2^11) (csrc/common.cuh).
  * Forward GEMMs multiply fp16 pairs (22-bit operands: fp32-class results; activations and normalised weights are O(1),
  * values are clamped to +-65504); gradient GEMMs multiply bf16 pairs (gradients need the fp32 exponent range for any
- * loss scale) -- tcgen05 kind::f16 does not mix formats in one MMA, so a conv input is split into both.
+ * loss scale) -- a wgmma does not mix operand formats, so a conv input is split into both.
  * x (B,C,T) fp32 -> conv-input dropout -> btc: [2][B][T][Cp] fp16 pair (forward operand, Cp = pad8(C)) and
  * bct (may be NULL): [2][B][T][Cp] bf16 pair of the same values (operand of the weight gradient). npl must be 2. */
 int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, int k, int dilation,

@@ -25,6 +25,8 @@ import torch
 warnings.filterwarnings("ignore")
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF = "/root/reference"
+sys.path.insert(0, os.path.dirname(HERE))
+import golden_util as G  # noqa: E402
 
 
 def import_reference():
@@ -49,9 +51,8 @@ class Fixture:
         self.d["%s|%s|%s" % (case, group, name)] = t2n(value) if torch.is_tensor(value) else np.asarray(value)
 
     def save(self, fname):
-        path = os.path.join(HERE, fname)
-        np.savez_compressed(path, **self.d)
-        print("wrote %s: %d arrays, %.1f KB" % (fname, len(self.d), os.path.getsize(path) / 1024))
+        G.save(fname, self.d)
+        print("wrote %s: %d arrays" % (fname, len(self.d)))
 
 
 def loss_weights(shape, i):

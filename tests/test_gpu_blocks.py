@@ -146,7 +146,7 @@ def test_plain_conv_canonical_vs_oracle(Cin, Cout, T, kind, math, monkeypatch):
 ])
 @pytest.mark.parametrize("math", ["fp32", "tc"])
 def test_convblock_canonical_vs_oracle(B, C, T, k, d, causal, residual, mode, math, monkeypatch):
-    """Both arithmetic modes of the ConvBlock -- exact-fp32 CUDA cores and the tcgen05 split-bf16 path --
+    """Both arithmetic modes of the ConvBlock -- exact-fp32 CUDA cores and the wgmma split-bf16 path --
     must meet the same parity bar against the CPU oracle."""
     from deepvoice3_pytorch_b200 import ops
     from oracle import dv3_oracle as O

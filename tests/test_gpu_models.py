@@ -135,7 +135,7 @@ _FP32_MODE_ERR = {}        # (preset, parameter) -> relative L2 gradient error o
 @pytest.mark.parametrize("preset", ["deepvoice3_ljspeech", "nyanko_ljspeech", "deepvoice3_vctk"])
 def test_preset_model_vs_oracle(preset, math, monkeypatch):
     """The three BASELINE.json presets at the benchmark size -- B=16, T_text=128, T_mel=800 (T_dec=200) -- forward +
-    every parameter gradient, in both ConvBlock arithmetic modes (tcgen05 fp16/bf16 operand pairs = the benched mode;
+    every parameter gradient, in both ConvBlock arithmetic modes (wgmma fp16/bf16 operand pairs = the benched mode;
     exact-fp32 CUDA cores), at north_star's tolerance: rtol=1e-3 / atol=1e-4 on every output."""
     from deepvoice3_pytorch_b200 import builder, ops
     monkeypatch.setattr(ops, "conv_math", math)

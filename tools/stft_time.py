@@ -21,4 +21,4 @@ b = 4.0 * nb * (n + frames * 513 + frames * 80)
 pk = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json"))) if os.path.exists(
     os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")) else {}
 print("stft_mel: %.3f ms / %d clips  -> %.0f clips/s, %.1f GB/s algorithmic, %.0f clk/frame/SM" % (
-    ms, nb, nb / ms * 1e3, b / ms / 1e6, ms * 1e-3 * 1.965e9 * 148 / (nb * frames)))
+    ms, nb, nb / ms * 1e3, b / ms / 1e6, ms * 1e-3 * 1.98e9 * 132 / (nb * frames)))

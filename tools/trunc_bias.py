@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Systematic (scale) error of the tcgen05 split-bf16 convolution against float64: the tensor core accumulates with
+"""Systematic (scale) error of the tensor-core split-bf16 convolution against float64: the tensor core accumulates with
 truncation, which shrinks every output by ~n_mma * 2^-25.  Prints, for a plain k-tap conv at a few contraction
 lengths, bias = <(y - y64), y64> / <y64, y64> and the relative rms error.  DV3_TC_GAMMA (units of 2^-25 per MMA) sets the
 epilogue compensation (read once per process)."""
