@@ -53,6 +53,14 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
+// ---- per-warpgroup register budget ---------------------------------------------------------------
+// Executed by every thread of a warpgroup: hand registers back to the SM (producer) or claim them (consumers) so that
+// warp-specialised kernels can give their MMA warpgroups more than the launch's uniform per-thread share.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- wgmma ---------------------------------------------------------------------------------------
 // D (64 x N fp32, registers of the 128 threads of a warpgroup) (+)= A (64 x 16, shared memory) * B (N x 16)^T.
 // Register i of thread (warp w of the warpgroup, lane l) holds row 16*w + l/4 + 8*((i/2)&1), column

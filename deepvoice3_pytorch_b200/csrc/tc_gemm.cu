@@ -12,16 +12,19 @@
 //   WGRAD : D[m, n] (j)   = sum_{b,t}  dY[b, t, m] * Xd[b, t+off_j, n]            MN-major operands, M = 128, N <= 256
 //
 // Operands are bf16 (B,T,C) planes fetched by TMA as K-major tiles of 128 rows x BK (BK = 64: 128-byte rows,
-// SWIZZLE_128B -- wherever the channel count is a multiple of 64; BK = 32: 64-byte rows, SWIZZLE_64B); the conv's zero
-// padding, the causal shift, ragged T / channel tails are TMA out-of-bounds zero fill.  The hi and lo weight planes sit
-// back to back in a stage, so p0(A) x [p0(W) ; p1(W)] is ONE N = 2*NCOLS MMA filling the main | cross accumulators,
-// followed by p1(A) x p0(W) into the cross accumulator.
+// SWIZZLE_128B; BK = 32: 64-byte rows, SWIZZLE_64B; the host launchers pick BK per configuration); the conv's zero
+// padding, the causal shift, ragged T / channel tails are TMA out-of-bounds zero fill.  Each K = 16 step issues three
+// N = NCOLS MMAs: p0(A) x p0(W) into the main accumulator, then p0(A) x p1(W) and p1(A) x p0(W) into the cross
+// accumulator.  Main and cross are two disjoint register tuples: when an in-flight MMA's accumulator partially overlaps
+// the next one's, ptxas serialises the whole wgmma chain (C7511), whatever the register budget.
 //
 // tc_conv_kernel is PERSISTENT: one CTA per SM walks a static round-robin list of output tiles and the TMA ring
-// streams across tile boundaries, so the loads of tile n+1 overlap the epilogue of tile n.  Warp roles (288 threads):
-// warps 0-3 and 4-7 = two consumer warpgroups, each accumulating 64 of the 128 tile rows in registers (wgmma), then
-// handing the accumulators over 32 columns at a time through a shared-memory tile to warpgroup 0, whose thread r owns
-// row r (time step) in the epilogue (fused math -> stores coalesced along T); warp 8 = TMA producer.
+// streams across tile boundaries, so the loads of tile n+1 overlap the epilogue of tile n.  Warp roles (384 threads):
+// warpgroups 0 and 1 = consumers (setmaxnreg 232), each accumulating 64 of the 128 tile rows in registers (wgmma),
+// then handing the accumulators over 32 columns at a time through a shared-memory tile to warpgroup 0, whose thread r
+// owns row r (time step) in the epilogue (fused math -> stores coalesced along T); warpgroup 2 = producer
+// (setmaxnreg 40), one thread of which issues the TMA loads.  The registers the producer gives back let the consumers
+// hold both accumulators (up to 2 x 64 per thread) without spills; at a uniform 168 per thread they spilled.
 //
 // What the epilogues fuse besides the block's own math (Dv3TcFuse, include/dv3b200.h):
 //   * forward: the bf16 hi/lo planes -- with the CONSUMER's input dropout applied -- that the next convolution reads,
@@ -35,7 +38,10 @@ namespace dv3 {
 
 using namespace tc;
 
-constexpr int TC_THREADS = 288;
+constexpr int TC_CONV_THREADS = 384;        // tc_conv_kernel: consumer warpgroups 0-1, producer warpgroup 2
+constexpr int TC_PRODUCER_REGS = 40;        // setmaxnreg budgets: 128 x 40 + 256 x 232 = 64 512 <= 65 536 registers
+constexpr int TC_CONSUMER_REGS = 232;
+constexpr int TC_WGRAD_THREADS = 288;       // tc_wgrad_mn_kernel: consumer warpgroups 0-1, producer warp 8
 constexpr int MAX_TAPS_TC = 8;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memory per CTA
 constexpr int EPI_BUF = 16384;              // epilogue -> TMA-store staging buffer: hi 8 KB | lo 8 KB
@@ -359,7 +365,7 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ac
 // accumulators of a consumer warpgroup take 2 x 64 registers per thread.
 // ------------------------------------------------------------------------------------------------
 template <int MODE, int NBOX, int BR, int BK, bool BF16>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(TC_CONV_THREADS, 1)
 tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int tiles_x, int tiles_y,
                int num_tiles) {
     pdl_trigger();
@@ -400,8 +406,9 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         else { b_row0 = ty * BR * NBOX; b_row1 = b_row0 + BR; }
     };
 
-    if (warp == 8) {
-        if (lane == 0) {
+    if (warp >= 8) {
+        setmaxnreg_dec<TC_PRODUCER_REGS>();
+        if (warp == 8 && lane == 0) {
             int it = 0;
             for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
                 int a_row0, a_z, b_row0, b_row1;
@@ -425,27 +432,33 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
             }
         }
     } else {
+        setmaxnreg_inc<TC_CONSUMER_REGS>();
         const int wg = warp >> 2, wq = warp & 3;
         EpiStage es;
         es.base = staging; es.map = maps.st; es.uses = 0; es.issuer = (threadIdx.x == 0);
-        float acc[2 * NR];                                   // [0, NR): main, [NR, 2 NR): cross
+        // Two disjoint register tuples: an MMA in flight may not share accumulator registers with the next one, or
+        // ptxas serialises every wgmma of the chain.
+        float acc[NR], xacc[NR];                             // main (p0 x p0), cross (p0 x p1 + p1 x p0)
         int it = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
             int a_row0, a_z, b_row0, b_row1;
             decode(tile, a_row0, a_z, b_row0, b_row1);
 #pragma unroll
-            for (int i = 0; i < 2 * NR; ++i) acc[i] = 0.f;
+            for (int i = 0; i < NR; ++i) { acc[i] = 0.f; xacc[i] = 0.f; }
             for (int kit = 0; kit < n_iters; ++kit, ++it) {
                 const int s = it % STAGES, ph = (it / STAGES) & 1;
                 mbar_wait(&full[s], ph);
                 const uint32_t sa = smem_u32(smem + s * STAGE) + wg * A_HALF;
-                const uint32_t sb = smem_u32(smem + s * STAGE + B_OFF);   // plane 1 follows plane 0: rows [NCOLS, 2 NCOLS)
+                const uint32_t sb = smem_u32(smem + s * STAGE + B_OFF);
                 wgmma_fence();
 #pragma unroll
                 for (int kk = 0; kk < BK / 16; ++kk) {
                     const uint32_t ko = kk * 32;
-                    wgmma_mma<2 * NCOLS, 0, 0>(BF16, acc, make_desc<BK>(sa + ko), make_desc<BK>(sb + ko), 1);  // p0 x [p0 ; p1]
-                    wgmma_mma<NCOLS, 0, 0>(BF16, acc + NR, make_desc<BK>(sa + TILE + ko), make_desc<BK>(sb + ko), 1);
+                    const uint64_t a0 = make_desc<BK>(sa + ko), a1 = make_desc<BK>(sa + TILE + ko);
+                    const uint64_t b0 = make_desc<BK>(sb + ko), b1 = make_desc<BK>(sb + NBOX * TILE_B + ko);
+                    wgmma_mma<NCOLS, 0, 0>(BF16, acc, a0, b0, 1);
+                    wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a0, b1, 1);
+                    wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a1, b0, 1);
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                                  // the previous stage's MMAs have retired
@@ -454,7 +467,7 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
             wgmma_wait<0>();
             if (n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
 #pragma unroll
-            for (int i = 0; i < NR; ++i) acc[i] = fmaf(acc[NR + i], LO_INV, acc[i] * p.gmain);   // lo planes carry 2^11
+            for (int i = 0; i < NR; ++i) acc[i] = fmaf(xacc[i], LO_INV, acc[i] * p.gmain);   // lo planes carry 2^11
             if (MODE == TC_GATED) epilogue_gated<BR, NCOLS>(p, acc, acc_tile, wg, wq, lane, a_row0, a_z, b_row0, es);
             else epilogue_conv<NCOLS>(p, acc, acc_tile, wg, wq, lane, a_row0, a_z, b_row0, es);
         }
@@ -486,7 +499,7 @@ constexpr int WG_STAGE = 2 * (2 * WG_BOX + 2 * WG_BOX);  // per plane: 128 chann
 constexpr int WG_STAGES = ((SMEM_LIMIT - 2048) / WG_STAGE) > 6 ? 6 : ((SMEM_LIMIT - 2048) / WG_STAGE);
 constexpr int WG_SMEM = WG_STAGES * WG_STAGE + 1024 + 512;
 
-__global__ void __launch_bounds__(TC_THREADS, 1)
+__global__ void __launch_bounds__(TC_WGRAD_THREADS, 1)
 tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcMnParams p) {
     pdl_trigger();
     constexpr int A_PL = 2 * WG_BOX, B_PL = 2 * WG_BOX;
@@ -628,7 +641,7 @@ static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, i
     const int sms = config().sms;
     const int num_tiles = tiles_x * tiles_y * batch;
     const int grid = num_tiles < sms ? num_tiles : sms;
-    cudaError_t e = launch_k(kern, dim3(grid), dim3(TC_THREADS), (size_t)Cfg::SMEM, st, maps, p, tiles_x, tiles_y,
+    cudaError_t e = launch_k(kern, dim3(grid), dim3(TC_CONV_THREADS), (size_t)Cfg::SMEM, st, maps, p, tiles_x, tiles_y,
                              num_tiles);
     if (e != cudaSuccess) { set_error("%s: launch failed: %s", what, cudaGetErrorString(e)); return 1; }
     return check_launch(what);
@@ -710,7 +723,8 @@ static int apply_fuse(TcParams& p, TcMaps& maps, const Dv3TcFuse* f, int B, int 
 }
 
 // Gated forward.  xd: [2][B][T][C] bf16 planes of the (dropped-out) input; w: [2][k][2C][C] bf16 planes of the
-// normalised weight; the rest as dv3_convblock_fwd.  64-channel tiles (64 a | 64 b columns), BK = 64.
+// normalised weight; the rest as dv3_convblock_fwd.  64-channel tiles (64 a | 64 b columns), BK = 32: a BK = 64
+// stage (64 KB) leaves room for only two ring stages, BK = 32 for five (H100: 1.45x faster at C=512, T=800).
 int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bias, const float* spk,
                          const float* res, float* y, float* save_a, float* save_s, int B, int C, int T, int k,
                          int dilation, int causal, int mode, int residual, const Dv3TcFuse* fuse, void* stream) {
@@ -718,29 +732,31 @@ int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bi
     DV3_REQUIRE(npl == 2, "tc_convblock_fwd: npl must be 2");
     TcMaps maps;
     const int t_tiles = (T + 127) / 128;
+    constexpr int BK = 32;
     for (int pl = 0; pl < 2; ++pl) {
         if (encode_tmap_bf16_3d(&maps.a[pl], plane(xd, pl, (long long)B * T * C), C, T, B, (uint64_t)C * 2,
-                                (uint64_t)T * C * 2, 64, 128)) return 1;
+                                (uint64_t)T * C * 2, BK, 128)) return 1;
         if (encode_tmap_bf16_3d(&maps.b[pl], plane(w, pl, (long long)k * 2 * C * C), C, (uint64_t)k * 2 * C, 1,
-                                (uint64_t)C * 2, (uint64_t)k * 2 * C * C * 2, 64, 64)) return 1;
+                                (uint64_t)C * 2, (uint64_t)k * 2 * C * C * 2, BK, 64)) return 1;
     }
     TcParams p = {};
-    p.T = T; p.B = B; p.Kc = C; p.Nc = C; p.rows_per_tap = 2 * C; p.k = k; p.kb_n = C / 64;
+    p.T = T; p.B = B; p.Kc = C; p.Nc = C; p.rows_per_tap = 2 * C; p.k = k; p.kb_n = C / BK;
     fill_taps_tc(p.tap_off, k, dilation, causal, false);
     p.bias = bias; p.spk = spk; p.res = res; p.y = y; p.save_a = save_a; p.save_s = save_s;
     p.gate_mode = mode; p.residual = residual;
-    p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * 4);
+    p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (BK / 16));
     p.operand_bf16 = 0;                                          // forward operands: fp16 hi/lo planes
     if (apply_fuse(p, maps, fuse, B, T, C, "tc_convblock_fwd")) return 1;
     DV3_REQUIRE(p.post_kind == POST_NONE, "tc_convblock_fwd: post_kind is a data-gradient option");
-    return launch_conv<TC_GATED, 2, 64, 64>(maps, p, t_tiles, C / 64, B, (cudaStream_t)stream, "tc_convblock_fwd");
+    return launch_conv<TC_GATED, 2, 64, BK>(maps, p, t_tiles, C / 64, B, (cudaStream_t)stream, "tc_convblock_fwd");
 }
 
 // Generic conv / data-gradient:  out (B, Nc, T) fp32 = sum_j A[b, t+off_j, :] . W[j, n, :]  (+ epilogue)
 //   a: [2][B][T][Kp] bf16 planes, Kp = Kc rounded up to 8;  w: [2][k][Nc][Kp] bf16 planes.
 //   transpose_taps = 1 for a data gradient (offsets padl - j*d), 0 for a forward conv.
-// Tile width: 128 output channels, or 64 when 128-wide tiles would leave most of the SMs idle.  BK = 64 needs
-// Kc % 64 == 0 (else BK = 32: the 80-channel mel input, the 513-wide linear output, the 16-wide speaker embedding).
+// Tile width: 128 output channels, or 64 when 128-wide tiles would leave most of the SMs idle.  BK: 32 for 128-wide
+// tiles (a 64 KB BK = 64 stage would leave two ring stages, BK = 32 gives five); 64 for 64-wide tiles when
+// Kc % 64 == 0 (else 32: the 80-channel mel input, the 513-wide linear output, the 16-wide speaker embedding).
 int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc, int Nc, int T, int k, int dilation,
                 int causal, int transpose_taps, const float* bias, int relu, float p_drop,
                 const unsigned long long* seed_ptr, unsigned salt, int addmode, const float* e1, const float* e2,
@@ -754,7 +770,7 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     const long long tiles128 = (long long)t_tiles * ((Nc + 127) / 128) * B;
     const bool narrow = Nc > 64 && (k == 1 || Nc % 64 == 0) && tiles128 < 100;
     const bool k64 = Kc % 64 == 0;
-    const int bk = k64 ? 64 : 32, br = narrow ? 64 : 128;
+    const int bk = (narrow && k64) ? 64 : 32, br = narrow ? 64 : 128;
     TcMaps maps;
     for (int pl = 0; pl < 2; ++pl) {
         if (encode_tmap_bf16_3d(&maps.a[pl], plane(a, pl, (long long)B * T * Kp), Kc, T, B, (uint64_t)Kp * 2,
@@ -776,8 +792,7 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
         if (k64) return launch_conv<TC_CONV, 1, 64, 64>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
         return launch_conv<TC_CONV, 1, 64, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
     }
-    if (k64) return launch_conv<TC_CONV, 1, 128, 64>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
-    return launch_conv<TC_CONV, 1, 128, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128,bk32)");
+    return launch_conv<TC_CONV, 1, 128, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
 }
 
 int dv3_tc_wgrad_nsplit(int B, int Mw, int Nw, int T, int k) {
@@ -823,7 +838,7 @@ int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long lon
     const int m_tiles = (Mw + 127) / 128;
     static const int configured = ensure_smem(tc_wgrad_mn_kernel, WG_SMEM, "tc_wgrad_mn");
     if (configured) return 1;
-    const cudaError_t e = launch_k(tc_wgrad_mn_kernel, dim3((Nw + 127) / 128, m_tiles, p.nsplit * k), dim3(TC_THREADS),
+    const cudaError_t e = launch_k(tc_wgrad_mn_kernel, dim3((Nw + 127) / 128, m_tiles, p.nsplit * k), dim3(TC_WGRAD_THREADS),
                                    (size_t)WG_SMEM, st, maps, p);
     if (e != cudaSuccess) { set_error("tc_wgrad_mn: launch failed: %s", cudaGetErrorString(e)); return 1; }
     return check_launch("tc_wgrad_mn");
