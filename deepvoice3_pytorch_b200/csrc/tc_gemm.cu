@@ -19,12 +19,15 @@
 // the next one's, ptxas serialises the whole wgmma chain (C7511), whatever the register budget.
 //
 // tc_conv_kernel is PERSISTENT: one CTA per SM walks a static round-robin list of output tiles and the TMA ring
-// streams across tile boundaries, so the loads of tile n+1 overlap the epilogue of tile n.  Warp roles (384 threads):
-// warpgroups 0 and 1 = consumers (setmaxnreg 232), each accumulating 64 of the 128 tile rows in registers (wgmma),
-// then handing the accumulators over 32 columns at a time through a shared-memory tile to warpgroup 0, whose thread r
-// owns row r (time step) in the epilogue (fused math -> stores coalesced along T); warpgroup 2 = producer
-// (setmaxnreg 40), one thread of which issues the TMA loads.  The registers the producer gives back let the consumers
-// hold both accumulators (up to 2 x 64 per thread) without spills; at a uniform 168 per thread they spilled.
+// streams across tile boundaries.  Warp roles (512 threads, one setmaxnreg budget per warpgroup):
+//   * warpgroups 0 and 1 = consumers (176 registers): each accumulates 64 of the 128 tile rows in registers (wgmma),
+//     then writes the summed accumulators into a full-tile fp32 shared-memory hand-off tile (acc_tile) and goes
+//     straight on to the next tile's MMAs;
+//   * warpgroup 2 = producer (24 registers): one thread issues the TMA loads;
+//   * warpgroup 3 = epilogue (136 registers): thread r owns row r (time step) of acc_tile and runs the fused math and
+//     the stores (coalesced along T) and the TMA plane stores.
+// Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (all
+// 128 epilogue threads have read it).  So the epilogue of tile n runs while the consumers issue the MMAs of tile n+1.
 //
 // What the epilogues fuse besides the block's own math (Dv3TcFuse, include/dv3b200.h):
 //   * forward: the bf16 hi/lo planes -- with the CONSUMER's input dropout applied -- that the next convolution reads,
@@ -38,16 +41,18 @@ namespace dv3 {
 
 using namespace tc;
 
-constexpr int TC_CONV_THREADS = 384;        // tc_conv_kernel: consumer warpgroups 0-1, producer warpgroup 2
-constexpr int TC_PRODUCER_REGS = 40;        // setmaxnreg budgets: 128 x 40 + 256 x 232 = 64 512 <= 65 536 registers
-constexpr int TC_CONSUMER_REGS = 232;
+constexpr int TC_CONV_THREADS = 512;        // tc_conv_kernel: consumers 0-1, producer 2, epilogue 3 (warpgroups)
+constexpr int TC_PRODUCER_REGS = 24;        // setmaxnreg budgets: 128 x 24 + 256 x 176 + 128 x 136 = 65 536 registers
+constexpr int TC_CONSUMER_REGS = 176;
+constexpr int TC_EPILOGUE_REGS = 136;       // > 65 536 / 512: claimed with setmaxnreg.inc (.dec may not raise it)
+static_assert(TC_PRODUCER_REGS <= 65536 / TC_CONV_THREADS && TC_CONSUMER_REGS >= 65536 / TC_CONV_THREADS &&
+              TC_EPILOGUE_REGS >= 65536 / TC_CONV_THREADS, "setmaxnreg direction of each warpgroup");
+static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS + 128 * TC_EPILOGUE_REGS <= 65536, "register file");
 constexpr int TC_WGRAD_THREADS = 288;       // tc_wgrad_mn_kernel: consumer warpgroups 0-1, producer warp 8
 constexpr int MAX_TAPS_TC = 8;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memory per CTA
 constexpr int EPI_BUF = 16384;              // epilogue -> TMA-store staging buffer: hi 8 KB | lo 8 KB
 constexpr int EPI_STAGING = 2 * EPI_BUF;
-constexpr int ACC_PITCH = 33;               // accumulator hand-over tile: [128 rows][32 columns], padded rows
-constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
 
 enum { TC_GATED = 0, TC_CONV = 1 };
 enum { POST_NONE = 0, POST_GLU = 1, POST_HIGHWAY = 2, POST_RELU = 3, POST_IDENT = 4 };
@@ -100,30 +105,17 @@ struct TcCfg {
     static constexpr int TILE = 128 * BK * 2;            // A tile (128 rows)
     static constexpr int TILE_B = BR * BK * 2;           // one B box
     static constexpr int STAGE = 2 * (TILE + NBOX * TILE_B);
+    static constexpr int NCOLS = BR * NBOX;              // columns per accumulator (main, cross)
+    // consumer -> epilogue hand-off: the whole fp32 output tile, [128 rows][NCOLS + 1].  The odd pitch keeps the
+    // epilogue's column reads (a warp reads one column of 32 consecutive rows) conflict-free; every access is a row
+    // base plus an immediate offset, which the register budgets of both sides need (an XOR swizzle that also makes
+    // the consumers' fragment-order writes 2-way instead of 4-way conflicted spilled in both warpgroups).
+    static constexpr int ACC_PITCH = NCOLS + 1;
+    static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
     static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_STAGING - ACC_TILE) / STAGE;
     static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
     static constexpr int SMEM = STAGES * STAGE + EPI_STAGING + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
-    static constexpr int NCOLS = BR * NBOX;              // columns per accumulator (main, cross)
 };
-
-__device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 2, 256;" ::: "memory"); }
-
-// Columns [c0, c0 + 32) of the summed accumulator (registers [0, NR) of both consumer warpgroups) -> row threadIdx.x
-// of that column chunk in v, for the threads of warpgroup 0.  Every consumer thread calls it with the same c0.
-template <int NR>
-__device__ __forceinline__ void acc_chunk(const float* acc, int c0, float* tile, int wg, int wq, int lane, float* v) {
-    consumer_bar();                                      // the previous chunk has been read
-#pragma unroll
-    for (int i = 0; i < NR; ++i) {
-        const int c = frag_col(i, lane) - c0;
-        if (c >= 0 && c < 32) tile[(64 * wg + frag_row(i, wq, lane)) * ACC_PITCH + c] = acc[i];
-    }
-    consumer_bar();
-    if (wg == 0) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = tile[threadIdx.x * ACC_PITCH + i];
-    }
-}
 
 // ---- operand planes written by the epilogues: registers -> shared-memory staging -> TMA tensor store ---------------
 // The epilogue thread of accumulator row r (time step) holds 32 consecutive channels; the planes are (B,T,C) with C
@@ -205,9 +197,12 @@ __device__ __forceinline__ float warp_colsum32(float* v, int lane) {
 // batch of 32 independent loads BEFORE the dependent math and stores of the chunk.  With plain loads the compiler
 // must order every load after the previous iteration's stores (possible aliasing), which serialised 128
 // global-memory round trips per thread (ncu: 40 % of the stall samples sat on the first use of these loads).
-template <int BR, int NCOLS>
-__device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* acc, float* tile, int wg, int wq,
-                                               int lane, int a_row0, int a_z, int b_row0, EpiStage& es) {
+// The accumulator values are read from the hand-off tile where they are used rather than staged in registers: the
+// epilogue warpgroup runs on TC_EPILOGUE_REGS.  Each epilogue thread arrives on acc_empty right after its last read of
+// the tile, so the consumers can overwrite it while the last stores and plane emissions are still under way.
+template <int BR>
+__device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
+                                               int a_z, int b_row0, EpiStage& es) {
     const int row = threadIdx.x & 127;
     const int t = a_row0 + row, b = a_z, C = p.Nc;
     const bool tv = t < p.T;
@@ -222,24 +217,23 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* a
     const DropCfg nd = make_drop(p.np ? p.np_p : 0.f, p.np_seed, p.np_salt);
 #pragma unroll
     for (int c32 = 0; c32 < BR; c32 += 32) {
-        float va[32], vb[32], rr[32];
-        acc_chunk<NCOLS / 2>(acc, c32, tile, wg, wq, lane, va);
-        acc_chunk<NCOLS / 2>(acc, BR + c32, tile, wg, wq, lane, vb);
-        if (wg != 0) continue;
+        float rr[32], sp[32];                               // rr: residual in, then the emitted plane values
         if (tv) {
             const size_t cb = base + (size_t)c32 * p.T;
 #pragma unroll
             for (int i = 0; i < 32; ++i) rr[i] = need_res ? __ldg(&res[cb + (size_t)i * p.T]) : 0.f;
             if (spk) {
 #pragma unroll
-                for (int i = 0; i < 32; ++i) va[i] += __ldg(&spk[cb + (size_t)i * p.T]);
+                for (int i = 0; i < 32; ++i) sp[i] = __ldg(&spk[cb + (size_t)i * p.T]);
             }
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
                 const int c = b_row0 + c32 + i;
                 const size_t idx = cb + (size_t)i * p.T;
-                const float a = va[i] + __ldg(&bias[c]);
-                const float s = sigmoidf_(vb[i] + __ldg(&bias[C + c]));
+                float va = arow[c32 + i];
+                if (spk) va += sp[i];
+                const float a = va + __ldg(&bias[c]);
+                const float s = sigmoidf_(arow[BR + c32 + i] + __ldg(&bias[C + c]));
                 float y;
                 if (p.gate_mode == 0) {
                     y = a * s;
@@ -250,21 +244,22 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* a
                 yo[idx] = y;
                 if (ao) ao[idx] = a;
                 if (so) so[idx] = s;
-                va[i] = y * drop_scale(nd, (uint32_t)idx);          // the consumer's conv-input dropout
+                rr[i] = y * drop_scale(nd, (uint32_t)idx);          // the consumer's conv-input dropout
             }
         }
+        if (c32 + 32 == BR) mbar_arrive(acc_empty);
         // all 128 epilogue threads reach the emission together (named barriers inside); rows >= T are clipped by TMA
         if (p.np) {
-            epi_emit<FMT_F16>(es, row, va, b_row0 + c32, a_row0, b);
-            if (p.np_wg) epi_emit<FMT_BF16>(es, row, va, b_row0 + c32, a_row0, b, 2);
+            epi_emit<FMT_F16>(es, row, rr, b_row0 + c32, a_row0, b);
+            if (p.np_wg) epi_emit<FMT_BF16>(es, row, rr, b_row0 + c32, a_row0, b, 2);
         }
     }
 }
 
 template <int NCOLS>
-__device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* acc, float* tile, int wg, int wq,
-                                              int lane, int a_row0, int a_z, int b_row0, EpiStage& es) {
-    const int row = threadIdx.x & 127;
+__device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
+                                              int a_z, int b_row0, EpiStage& es) {
+    const int row = threadIdx.x & 127, lane = threadIdx.x & 31;
     const int t = a_row0 + row, b = a_z;
     const bool tv = t < p.T;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
@@ -278,18 +273,16 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ac
     float* __restrict__ out = p.out;
     const int kind = p.post_kind;
     const float gs = (kind == POST_GLU && p.post_residual) ? 0.70710678118654752f : 1.f;
-#pragma unroll
-    for (int c32 = 0; c32 < NCOLS; c32 += 32) {
-        float v[32], x1[32], x2[32];
-        acc_chunk<NCOLS / 2>(acc, c32, tile, wg, wq, lane, v);
-        if (wg != 0) continue;
+#pragma unroll 1
+    for (int c32 = 0; c32 < NCOLS; c32 += 32) {             // not unrolled: interleaving the chunks spilled
+        float v[32], x2[32];                                // v: addend e1 in, then this chunk's outputs
         const int n0 = b_row0 + c32;
         const size_t cb = ((size_t)b * p.Nc + n0) * p.T + (tv ? t : 0);
         if (tv) {
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
                 const bool ok = n0 + i < p.Nc;
-                x1[i] = (p.addmode != 0 && ok) ? __ldg(&e1[cb + (size_t)i * p.T]) : 0.f;
+                v[i] = (p.addmode != 0 && ok) ? __ldg(&e1[cb + (size_t)i * p.T]) : 0.f;
                 x2[i] = (p.addmode == 2 && ok) ? __ldg(&e2[cb + (size_t)i * p.T]) : 0.f;
             }
 #pragma unroll
@@ -298,10 +291,10 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ac
                 float g = 0.f;
                 if (n < p.Nc) {
                     const size_t idx = cb + (size_t)i * p.T;
-                    g = v[i] * drop_scale(drop, (uint32_t)idx);
+                    g = arow[c32 + i] * drop_scale(drop, (uint32_t)idx);
                     if (bias) g += __ldg(&bias[n]);
-                    if (p.addmode == 1) g += p.alpha * x1[i];
-                    else if (p.addmode == 2) g += x1[i] * (1.f - x2[i]);
+                    if (p.addmode == 1) g += p.alpha * v[i];
+                    else if (p.addmode == 2) g += v[i] * (1.f - x2[i]);
                     if (p.relu) g = fmaxf(g, 0.f);
                     out[idx] = g;
                 }
@@ -311,6 +304,7 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ac
 #pragma unroll
             for (int i = 0; i < 32; ++i) v[i] = 0.f;
         }
+        if (c32 + 32 == NCOLS) mbar_arrive(acc_empty);
         if (p.np) {                                         // forward: operand planes of the consumer
             float w[32];
 #pragma unroll
@@ -380,8 +374,10 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint8_t* staging = smem + STAGES * STAGE;                // epilogue -> TMA store tiles (1024-aligned: STAGE % 1024 == 0)
     float* acc_tile = reinterpret_cast<float*>(staging + EPI_STAGING);
-    uint64_t* full = reinterpret_cast<uint64_t*>(staging + EPI_STAGING + ACC_TILE);
+    uint64_t* full = reinterpret_cast<uint64_t*>(staging + EPI_STAGING + Cfg::ACC_TILE);
     uint64_t* empty = full + STAGES;
+    uint64_t* acc_full = empty + STAGES;                     // the consumers have written acc_tile (256 arrivals)
+    uint64_t* acc_empty = acc_full + 1;                      // the epilogue has read acc_tile (128 arrivals)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_iters = p.k * p.kb_n;
 
@@ -390,6 +386,8 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         if (p.np || p.post_kind) { prefetch_tmap(&maps.st[0]); prefetch_tmap(&maps.st[1]); }
         if (p.np_wg) { prefetch_tmap(&maps.st[2]); prefetch_tmap(&maps.st[3]); }
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+        mbar_init(acc_full, 256);
+        mbar_init(acc_empty, 128);
         fence_barrier_init();
     }
     __syncthreads();
@@ -406,7 +404,21 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         else { b_row0 = ty * BR * NBOX; b_row1 = b_row0 + BR; }
     };
 
-    if (warp >= 8) {
+    if (warp >= 12) {
+        setmaxnreg_inc<TC_EPILOGUE_REGS>();                  // up from the launch's 65 536 / 512 = 128 per thread
+        EpiStage es;
+        es.base = staging; es.map = maps.st; es.uses = 0; es.issuer = (threadIdx.x == 384);
+        const float* arow = acc_tile + (threadIdx.x & 127) * Cfg::ACC_PITCH;   // this thread's time step
+        int n = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
+            int a_row0, a_z, b_row0, b_row1;
+            decode(tile, a_row0, a_z, b_row0, b_row1);
+            mbar_wait(acc_full, n & 1);
+            if (MODE == TC_GATED) epilogue_gated<BR>(p, arow, acc_empty, a_row0, a_z, b_row0, es);
+            else epilogue_conv<NCOLS>(p, arow, acc_empty, a_row0, a_z, b_row0, es);
+        }
+        if (es.issuer) bulk_wait_all();                             // plane stores complete before the CTA exits
+    } else if (warp >= 8) {
         setmaxnreg_dec<TC_PRODUCER_REGS>();
         if (warp == 8 && lane == 0) {
             int it = 0;
@@ -434,13 +446,11 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     } else {
         setmaxnreg_inc<TC_CONSUMER_REGS>();
         const int wg = warp >> 2, wq = warp & 3;
-        EpiStage es;
-        es.base = staging; es.map = maps.st; es.uses = 0; es.issuer = (threadIdx.x == 0);
         // Two disjoint register tuples: an MMA in flight may not share accumulator registers with the next one, or
         // ptxas serialises every wgmma of the chain.
         float acc[NR], xacc[NR];                             // main (p0 x p0), cross (p0 x p1 + p1 x p0)
-        int it = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        int it = 0, n = 0;
+        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
             int a_row0, a_z, b_row0, b_row1;
             decode(tile, a_row0, a_z, b_row0, b_row1);
 #pragma unroll
@@ -466,12 +476,13 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
             }
             wgmma_wait<0>();
             if (n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous tile
 #pragma unroll
-            for (int i = 0; i < NR; ++i) acc[i] = fmaf(xacc[i], LO_INV, acc[i] * p.gmain);   // lo planes carry 2^11
-            if (MODE == TC_GATED) epilogue_gated<BR, NCOLS>(p, acc, acc_tile, wg, wq, lane, a_row0, a_z, b_row0, es);
-            else epilogue_conv<NCOLS>(p, acc, acc_tile, wg, wq, lane, a_row0, a_z, b_row0, es);
+            for (int i = 0; i < NR; ++i)                              // lo planes carry 2^11
+                acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)] =
+                    fmaf(xacc[i], LO_INV, acc[i] * p.gmain);
+            mbar_arrive(acc_full);
         }
-        if (es.issuer) bulk_wait_all();                             // plane stores complete before the CTA exits
     }
 }
 

@@ -317,10 +317,11 @@ def _pad8(n):
 # fuse_bwd: the data-gradient GEMM of the consumer applies the producer's backward (gate / ReLU) in its epilogue and
 #           emits the producer's gradient planes + bias-gradient sums -> no dv3_tc_gate_bwd_split / dv3_tc_grad_split.
 # Both need the caller (modules.run_conv_stack) to state that the tensor has exactly ONE consumer.
-# Both are OFF by default: the separate split / gate-backward kernels stream at HBM speed with full occupancy, while
-# inside the GEMM the same work is done by the 4 epilogue warps of each SM (latency bound), and at C = 256 the fused
-# data-gradient epilogue of a 128x128 tile takes longer than the tile's MMAs.  Kept opt-in because the arithmetic is
-# bit-identical (tests/test_gpu_fusion.py) and the trade flips for wider layers.
+# Both are OFF by default.  Inside the GEMM the work runs on the kernel's epilogue warpgroup (4 warps per SM, latency
+# bound), which now overlaps the next tile's MMAs; even so, the deepvoice3_ljspeech step with fuse_fwd measured no
+# faster than with the separate full-occupancy split kernels (H100 SXM, 400 W: 10.77 ms against 10.65-10.73 ms).
+# fuse_bwd is not bit-identical (its bias gradients are atomic sums) and was not re-measured.  Kept opt-in because the
+# fuse_fwd arithmetic is bit-identical (tests/test_gpu_fusion.py) and the trade may flip for wider layers.
 fuse_fwd = os.environ.get("DV3_FUSE_FWD", "0") == "1"
 fuse_bwd = os.environ.get("DV3_FUSE_BWD", "0") == "1"
 
