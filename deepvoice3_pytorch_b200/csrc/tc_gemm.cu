@@ -1,17 +1,18 @@
 // wgmma tensor-core path of the ConvBlock and of the plain (1x1 / k-tap) weight-normed convolutions: forward,
-// data-gradient and weight-gradient as implicit GEMMs with fp32-equivalent accuracy from split-bf16 operands.
-// Every fp32 operand is split into bf16 planes p0 = bf16(x), p1 = bf16(x - p0) and each K-step issues
-// p0*p0 + p0*p1 + p1*p0 (operand error ~2^-17; single-pass TF32 would miss the rtol=1e-3/atol=1e-4 parity bar after
-// ~30 blocks).  The tensor core adds each MMA into the fp32 accumulator with truncation (bias ~N_mma x 2^-25), so the
-// main term p0*p0 and the 2^-8-smaller cross terms accumulate in two separate register accumulators that the
-// epilogue adds in fp32 (tools/precision_report.py).
+// data-gradient and weight-gradient as implicit GEMMs with fp32-class accuracy from split 16-bit operands.
+// Every fp32 operand travels as a pair of planes p0 = rn16(x), p1 = rn16((x - p0) * 2^11) (common.cuh): fp16 pairs in
+// the forward GEMMs, bf16 pairs in the gradient GEMMs.  Each K-step issues p0*p0 + p0*p1 + p1*p0 (single-pass TF32
+// would miss the rtol=1e-3/atol=1e-4 parity bar after ~30 blocks).  The tensor core adds each MMA into the fp32
+// accumulator with truncation (bias ~N_mma x 2^-25), so the main term p0*p0 and the cross terms (2^-11 smaller in
+// effect with fp16 pairs, 2^-8 with bf16 pairs) accumulate in two separate register accumulators that the epilogue
+// adds in fp32 as main + cross * 2^-11 (tools/precision_report.py).
 //
 //   GATED : D[t, (a|b) c] = sum_{j,ci} Xd[b, t+off_j, ci] * W[j, (a|b) c, ci]    M = 128 time steps, N = 64 a | 64 b
 //   CONV  : D[t, n]       = sum_{j,kc} A[b, t+off_j, kc]  * W[j, n, kc]           M = 128 time steps, N = 64 or 128
 //           (plain conv forward with bias/ReLU, and every data gradient: A = dY or dAB, W = transposed weight)
 //   WGRAD : D[m, n] (j)   = sum_{b,t}  dY[b, t, m] * Xd[b, t+off_j, n]            MN-major operands, M = 128, N <= 256
 //
-// Operands are bf16 (B,T,C) planes fetched by TMA as K-major tiles of 128 rows x BK (BK = 64: 128-byte rows,
+// Operands are 16-bit (B,T,C) planes fetched by TMA as K-major tiles of 128 rows x BK (BK = 64: 128-byte rows,
 // SWIZZLE_128B; BK = 32: 64-byte rows, SWIZZLE_64B; the host launchers pick BK per configuration); the conv's zero
 // padding, the causal shift, ragged T / channel tails are TMA out-of-bounds zero fill.  Each K = 16 step issues three
 // N = NCOLS MMAs: p0(A) x p0(W) into the main accumulator, then p0(A) x p1(W) and p1(A) x p0(W) into the cross
@@ -25,15 +26,13 @@
 //     straight on to the next tile's MMAs;
 //   * warpgroup 2 = producer (24 registers): one thread issues the TMA loads;
 //   * warpgroup 3 = epilogue (136 registers): thread r owns row r (time step) of acc_tile and runs the fused math and
-//     the stores (coalesced along T) and the TMA plane stores.
+//     the stores (coalesced along T).
 // Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (all
 // 128 epilogue threads have read it).  So the epilogue of tile n runs while the consumers issue the MMAs of tile n+1.
 //
-// What the epilogues fuse besides the block's own math (Dv3TcFuse, include/dv3b200.h):
-//   * forward: the bf16 hi/lo planes -- with the CONSUMER's input dropout applied -- that the next convolution reads,
-//     so chained blocks need no operand-split pass;
-//   * data gradient: the backward of the PRODUCER of the tensor whose gradient this call computes (GLU / highway gate,
-//     ReLU or identity), emitted as that producer's dAB planes + bias-gradient sums, so no gate-backward pass.
+// The epilogues fuse the launch's own math only (gate, bias, speaker bias, residual, dropout mask, addend, ReLU) and
+// write fp32 (B,C,T) outputs.  The operand planes of the next GEMM come from the split kernels of tc_split.cu, which
+// run at full occupancy rather than on one warpgroup per SM.
 #include "tc_common.cuh"
 #include "../../include/dv3b200.h"
 
@@ -51,14 +50,13 @@ static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS + 128 * TC_EPILOGU
 constexpr int TC_WGRAD_THREADS = 288;       // tc_wgrad_mn_kernel: consumer warpgroups 0-1, producer warp 8
 constexpr int MAX_TAPS_TC = 8;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memory per CTA
-constexpr int EPI_BUF = 16384;              // epilogue -> TMA-store staging buffer: hi 8 KB | lo 8 KB
-constexpr int EPI_STAGING = 2 * EPI_BUF;
+// Shared memory tc_conv_kernel leaves unused, so that every configuration keeps the ring depth it was measured with
+// (static_asserts after TcCfg).  Claiming it for a deeper ring is a performance change of its own.
+constexpr int RING_RESERVE = 32768;
 
 enum { TC_GATED = 0, TC_CONV = 1 };
-enum { POST_NONE = 0, POST_GLU = 1, POST_HIGHWAY = 2, POST_RELU = 3, POST_IDENT = 4 };
 
-struct TcMaps { CUtensorMap a[2]; CUtensorMap b[2]; CUtensorMap st[4]; };   // st: planes written by the epilogue
-                                                                            // (hi, lo) [+ (hi, lo) of the bf16 copy]
+struct TcMaps { CUtensorMap a[2]; CUtensorMap b[2]; };
 
 struct TcParams {
     int T, B;
@@ -74,18 +72,11 @@ struct TcParams {
     // conv epilogue: out = acc*dropmask + bias + addend ; relu
     float* out; const float* e1; const float* e2; float alpha; int addmode, relu;
     float p_drop; const unsigned long long* seed_ptr; uint32_t salt;
-    // forward fusion: planes of (output * next dropout mask) for the consumer conv, [2][B][T][np_pitch]
-    __nv_bfloat16* np; int np_pitch; long long np_plane; int np_wg;    // np_wg: also emit the bf16 pair (maps.st[2..3])
-    float np_p; const unsigned long long* np_seed; uint32_t np_salt;
-    // backward fusion: producer backward applied to the data gradient this launch computes
-    int post_kind, post_residual, post_pitch;
-    const float* post_a; const float* post_s; const float* post_x;
-    __nv_bfloat16* post_planes; long long post_plane; float* post_dbias;
     // Compensation of the tensor core's truncating accumulation: every MMA adds its K = 16 partial product into the
     // fp32 accumulator rounding TOWARD ZERO, a small expected relative loss per event on the running sum; over the
     // n_mma events of one output that is a systematic shrink of ~gcoef * n_mma (tools/trunc_bias.py measures gcoef).
-    // The epilogue multiplies the main accumulator by gmain = 1 + gcoef * n_mma (the cross-term accumulator is 2^-8
-    // smaller: its loss is below fp32 resolution).
+    // The epilogue multiplies the main accumulator by gmain = 1 + gcoef * n_mma (the cross terms are 2^-8 or more
+    // smaller in effect: their loss is below fp32 resolution).
     float gmain;
     int operand_bf16;          // operand format of the MMAs: 0 = fp16 planes (forward), 1 = bf16 planes (gradients)
 };
@@ -112,85 +103,14 @@ struct TcCfg {
     // the consumers' fragment-order writes 2-way instead of 4-way conflicted spilled in both warpgroups).
     static constexpr int ACC_PITCH = NCOLS + 1;
     static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - EPI_STAGING - ACC_TILE) / STAGE;
+    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - RING_RESERVE - ACC_TILE) / STAGE;
     static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-    static constexpr int SMEM = STAGES * STAGE + EPI_STAGING + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
+    static constexpr int SMEM = STAGES * STAGE + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
 };
-
-// ---- operand planes written by the epilogues: registers -> shared-memory staging -> TMA tensor store ---------------
-// The epilogue thread of accumulator row r (time step) holds 32 consecutive channels; the planes are (B,T,C) with C
-// contiguous, so direct stores would be 16-byte pieces 1-2 KB apart (32 LSU wavefronts per instruction: measured 2.3x
-// slower data-gradient kernels).  Instead the 128 epilogue threads write their rows into a [128][64 B] staging tile
-// (SWIZZLE_64B: conflict-free) and one thread hands the tile to the TMA unit (cp.async.bulk.tensor store), which
-// also clips rows >= T and pad channels.  Two staging buffers alternate; a buffer is rewritten once the bulk group
-// that read it has drained (cp.async.bulk.wait_group.read 1).
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(map), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-struct EpiStage {
-    uint8_t* base;             // EPI_STAGING bytes, 1024-aligned
-    const CUtensorMap* map;    // [2]: hi, lo
-    int uses;                  // buffer = uses & 1
-    bool issuer;
-};
-
-// One use = one [128 rows][32 channels] tile of one output tensor: FMT_F16 (forward operand) or FMT_BF16 (gradient).
-template <int FMT>
-__device__ __forceinline__ void epi_emit(EpiStage& es, int row, const float* v, int c0, int t0, int b, int map0 = 0) {
-    uint8_t* buf = es.base + (es.uses & 1) * EPI_BUF;
-    __syncwarp();                                        // bar.sync needs converged warps
-    if (es.issuer) bulk_wait_read<1>();                  // the group that last read this buffer has drained
-    __syncwarp();
-    epi_bar();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        uint32_t h[4], l[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            uint16_t h0, l0, h1, l1;
-            split_pair<FMT>(v[j * 8 + 2 * i], h0, l0);
-            split_pair<FMT>(v[j * 8 + 2 * i + 1], h1, l1);
-            h[i] = (uint32_t)h0 | ((uint32_t)h1 << 16);
-            l[i] = (uint32_t)l0 | ((uint32_t)l1 << 16);
-        }
-        const uint32_t off = (uint32_t)row * 64u + (uint32_t)((j ^ ((row >> 1) & 3)) << 4);   // SWIZZLE_64B
-        *reinterpret_cast<uint4*>(buf + off) = make_uint4(h[0], h[1], h[2], h[3]);
-        *reinterpret_cast<uint4*>(buf + 8192 + off) = make_uint4(l[0], l[1], l[2], l[3]);
-    }
-    fence_proxy_async();
-    __syncwarp();
-    epi_bar();
-    if (es.issuer) {
-        tma_store_3d(&es.map[map0], buf, c0, t0, b);
-        tma_store_3d(&es.map[map0 + 1], buf + 8192, c0, t0, b);
-        bulk_commit();
-    }
-    ++es.uses;
-}
-
-// Column sums over the 32 rows held by the lanes of a warp: after the call lane i holds sum_rows v[i].
-// Butterfly "transpose-reduce": 31 shuffles instead of 32 x 5.
-__device__ __forceinline__ float warp_colsum32(float* v, int lane) {
-#pragma unroll
-    for (int half = 16; half >= 1; half >>= 1) {
-        const bool upper = (lane & half) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            // lanes with the bit set keep columns [half, 2*half), the others [0, half); exchange the other part
-            const float send = upper ? v[i] : v[i + half];
-            const float recv = __shfl_xor_sync(0xffffffffu, send, half);
-            v[i] = (upper ? v[i + half] : v[i]) + recv;
-        }
-    }
-    return v[0];
-}
+static_assert(TcCfg<2, 32, 64>::STAGES == 4, "gated forward: 4-stage ring");
+static_assert(TcCfg<1, 32, 128>::STAGES == 4, "128-column conv: 4-stage ring");
+static_assert(TcCfg<1, 64, 64>::STAGES == 3, "64-column conv at BK = 64: 3-stage ring");
+static_assert(TcCfg<1, 32, 64>::STAGES == 6, "64-column conv at BK = 32: 6-stage ring");
 
 // ---- epilogues -----------------------------------------------------------------------------------------------
 // NOTE on the epilogue loads: residual / addend / bias reads go through __ldg (ld.global.nc) and are issued as a
@@ -199,12 +119,11 @@ __device__ __forceinline__ float warp_colsum32(float* v, int lane) {
 // global-memory round trips per thread (ncu: 40 % of the stall samples sat on the first use of these loads).
 // The accumulator values are read from the hand-off tile where they are used rather than staged in registers: the
 // epilogue warpgroup runs on TC_EPILOGUE_REGS.  Each epilogue thread arrives on acc_empty right after its last read of
-// the tile, so the consumers can overwrite it while the last stores and plane emissions are still under way.
+// the tile, so the consumers can overwrite it while the last stores are still under way.
 template <int BR>
 __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
-                                               int a_z, int b_row0, EpiStage& es) {
-    const int row = threadIdx.x & 127;
-    const int t = a_row0 + row, b = a_z, C = p.Nc;
+                                               int a_z, int b_row0) {
+    const int t = a_row0 + (threadIdx.x & 127), b = a_z, C = p.Nc;
     const bool tv = t < p.T;
     const float* __restrict__ bias = p.bias;
     const float* __restrict__ res = p.res;
@@ -214,10 +133,9 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* a
     float* __restrict__ so = p.save_s;
     const bool need_res = (p.gate_mode != 0) || p.residual;
     const size_t base = ((size_t)b * C + b_row0) * p.T + (tv ? t : 0);
-    const DropCfg nd = make_drop(p.np ? p.np_p : 0.f, p.np_seed, p.np_salt);
 #pragma unroll
     for (int c32 = 0; c32 < BR; c32 += 32) {
-        float rr[32], sp[32];                               // rr: residual in, then the emitted plane values
+        float rr[32], sp[32];                               // rr: residual
         if (tv) {
             const size_t cb = base + (size_t)c32 * p.T;
 #pragma unroll
@@ -244,38 +162,25 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* a
                 yo[idx] = y;
                 if (ao) ao[idx] = a;
                 if (so) so[idx] = s;
-                rr[i] = y * drop_scale(nd, (uint32_t)idx);          // the consumer's conv-input dropout
             }
         }
         if (c32 + 32 == BR) mbar_arrive(acc_empty);
-        // all 128 epilogue threads reach the emission together (named barriers inside); rows >= T are clipped by TMA
-        if (p.np) {
-            epi_emit<FMT_F16>(es, row, rr, b_row0 + c32, a_row0, b);
-            if (p.np_wg) epi_emit<FMT_BF16>(es, row, rr, b_row0 + c32, a_row0, b, 2);
-        }
     }
 }
 
 template <int NCOLS>
 __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
-                                              int a_z, int b_row0, EpiStage& es) {
-    const int row = threadIdx.x & 127, lane = threadIdx.x & 31;
-    const int t = a_row0 + row, b = a_z;
+                                              int a_z, int b_row0) {
+    const int t = a_row0 + (threadIdx.x & 127), b = a_z;
     const bool tv = t < p.T;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
-    const DropCfg nd = make_drop(p.np ? p.np_p : 0.f, p.np_seed, p.np_salt);
     const float* __restrict__ bias = p.bias;
     const float* __restrict__ e1 = p.e1;
     const float* __restrict__ e2 = p.e2;
-    const float* __restrict__ pa = p.post_a;
-    const float* __restrict__ ps = p.post_s;
-    const float* __restrict__ px = p.post_x;
     float* __restrict__ out = p.out;
-    const int kind = p.post_kind;
-    const float gs = (kind == POST_GLU && p.post_residual) ? 0.70710678118654752f : 1.f;
 #pragma unroll 1
     for (int c32 = 0; c32 < NCOLS; c32 += 32) {             // not unrolled: interleaving the chunks spilled
-        float v[32], x2[32];                                // v: addend e1 in, then this chunk's outputs
+        float v[32], x2[32];                                // addends e1, e2
         const int n0 = b_row0 + c32;
         const size_t cb = ((size_t)b * p.Nc + n0) * p.T + (tv ? t : 0);
         if (tv) {
@@ -288,69 +193,18 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
 #pragma unroll
             for (int i = 0; i < 32; ++i) {
                 const int n = n0 + i;
-                float g = 0.f;
                 if (n < p.Nc) {
                     const size_t idx = cb + (size_t)i * p.T;
-                    g = arow[c32 + i] * drop_scale(drop, (uint32_t)idx);
+                    float g = arow[c32 + i] * drop_scale(drop, (uint32_t)idx);
                     if (bias) g += __ldg(&bias[n]);
                     if (p.addmode == 1) g += p.alpha * v[i];
                     else if (p.addmode == 2) g += v[i] * (1.f - x2[i]);
                     if (p.relu) g = fmaxf(g, 0.f);
                     out[idx] = g;
                 }
-                v[i] = g;
             }
-        } else {
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = 0.f;
         }
         if (c32 + 32 == NCOLS) mbar_arrive(acc_empty);
-        if (p.np) {                                         // forward: operand planes of the consumer
-            float w[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) w[i] = v[i] * drop_scale(nd, (uint32_t)(cb + (size_t)i * p.T));
-            epi_emit<FMT_F16>(es, row, w, n0, a_row0, b);
-            if (p.np_wg) epi_emit<FMT_BF16>(es, row, w, n0, a_row0, b, 2);
-        }
-        if (kind != POST_NONE) {                            // backward of the producer of this gradient's tensor
-            // v[i] = dL/d(producer output) at (b, n0+i, t) (0 outside the tile).  Gate kinds emit [da | db] planes of
-            // width 2*Nc, the others a single gradient plane of width post_pitch.
-            float da[32], db[32];
-            if (kind == POST_GLU || kind == POST_HIGHWAY) {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float av = 0.f, sv = 0.f, xv = 0.f;
-                    if (tv && n0 + i < p.Nc) {
-                        const size_t idx = cb + (size_t)i * p.T;
-                        av = __ldg(&pa[idx]); sv = __ldg(&ps[idx]);
-                        if (kind == POST_HIGHWAY) xv = __ldg(&px[idx]);
-                    }
-                    const float g = v[i] * gs;
-                    da[i] = g * sv;
-                    db[i] = g * (kind == POST_GLU ? av : (av - xv)) * sv * (1.f - sv);
-                }
-                epi_emit<FMT_BF16>(es, row, da, n0, a_row0, b);
-                epi_emit<FMT_BF16>(es, row, db, p.Nc + n0, a_row0, b);
-                const float sa = warp_colsum32(da, lane), sb = warp_colsum32(db, lane);
-                if (p.post_dbias && n0 + lane < p.Nc) {
-                    atomicAdd(&p.post_dbias[n0 + lane], sa);
-                    atomicAdd(&p.post_dbias[p.Nc + n0 + lane], sb);
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    float g = v[i];
-                    if (kind == POST_RELU) {
-                        const bool on = tv && n0 + i < p.Nc && __ldg(&pa[cb + (size_t)i * p.T]) > 0.f;
-                        g = on ? g : 0.f;
-                    }
-                    da[i] = g;
-                }
-                epi_emit<FMT_BF16>(es, row, da, n0, a_row0, b);
-                const float sa = warp_colsum32(da, lane);
-                if (p.post_dbias && n0 + lane < p.Nc) atomicAdd(&p.post_dbias[n0 + lane], sa);
-            }
-        }
     }
 }
 
@@ -372,9 +226,8 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     static_assert(STAGES >= 2, "pipeline needs at least two stages");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint8_t* staging = smem + STAGES * STAGE;                // epilogue -> TMA store tiles (1024-aligned: STAGE % 1024 == 0)
-    float* acc_tile = reinterpret_cast<float*>(staging + EPI_STAGING);
-    uint64_t* full = reinterpret_cast<uint64_t*>(staging + EPI_STAGING + Cfg::ACC_TILE);
+    float* acc_tile = reinterpret_cast<float*>(smem + STAGES * STAGE);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE + Cfg::ACC_TILE);
     uint64_t* empty = full + STAGES;
     uint64_t* acc_full = empty + STAGES;                     // the consumers have written acc_tile (256 arrivals)
     uint64_t* acc_empty = acc_full + 1;                      // the epilogue has read acc_tile (128 arrivals)
@@ -383,8 +236,6 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
 
     if (threadIdx.x == 0) {
         prefetch_tmap(&maps.a[0]); prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.b[0]); prefetch_tmap(&maps.b[1]);
-        if (p.np || p.post_kind) { prefetch_tmap(&maps.st[0]); prefetch_tmap(&maps.st[1]); }
-        if (p.np_wg) { prefetch_tmap(&maps.st[2]); prefetch_tmap(&maps.st[3]); }
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         mbar_init(acc_full, 256);
         mbar_init(acc_empty, 128);
@@ -406,18 +257,15 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
 
     if (warp >= 12) {
         setmaxnreg_inc<TC_EPILOGUE_REGS>();                  // up from the launch's 65 536 / 512 = 128 per thread
-        EpiStage es;
-        es.base = staging; es.map = maps.st; es.uses = 0; es.issuer = (threadIdx.x == 384);
         const float* arow = acc_tile + (threadIdx.x & 127) * Cfg::ACC_PITCH;   // this thread's time step
         int n = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
             int a_row0, a_z, b_row0, b_row1;
             decode(tile, a_row0, a_z, b_row0, b_row1);
             mbar_wait(acc_full, n & 1);
-            if (MODE == TC_GATED) epilogue_gated<BR>(p, arow, acc_empty, a_row0, a_z, b_row0, es);
-            else epilogue_conv<NCOLS>(p, arow, acc_empty, a_row0, a_z, b_row0, es);
+            if (MODE == TC_GATED) epilogue_gated<BR>(p, arow, acc_empty, a_row0, a_z, b_row0);
+            else epilogue_conv<NCOLS>(p, arow, acc_empty, a_row0, a_z, b_row0);
         }
-        if (es.issuer) bulk_wait_all();                             // plane stores complete before the CTA exits
     } else if (warp >= 8) {
         setmaxnreg_dec<TC_PRODUCER_REGS>();
         if (warp == 8 && lane == 0) {
@@ -693,54 +541,16 @@ int dv3_tc_conv_supported(int B, int Cin, int Cout, int T, int k) {
            Cout >= 1;
 }
 
-// planes written by the epilogue: [2][B][T][pitch], stored as [128 rows][32 channels] boxes (SWIZZLE_64B staging)
-static int encode_store_maps(TcMaps& maps, int first, void* planes, int pitch, int B, int T) {
-    for (int pl = 0; pl < 2; ++pl)
-        if (encode_tmap_bf16_3d(&maps.st[first + pl], plane(planes, pl, (long long)B * T * pitch), pitch, T, B,
-                                (uint64_t)pitch * 2, (uint64_t)T * pitch * 2, 32, 128)) return 1;
-    return 0;
-}
-
-static int apply_fuse(TcParams& p, TcMaps& maps, const Dv3TcFuse* f, int B, int T, int out_channels, const char* what) {
-    if (!f) return 0;
-    DV3_REQUIRE(!(f->np && f->post_kind != POST_NONE), "%s: np and post_kind are exclusive (forward vs data gradient)", what);
-    if (f->np) {
-        DV3_REQUIRE(f->np_pitch >= out_channels && f->np_pitch % 8 == 0, "%s: np_pitch %d must be pad8 of %d channels",
-                    what, f->np_pitch, out_channels);
-        p.np = (__nv_bfloat16*)f->np; p.np_pitch = f->np_pitch; p.np_plane = (long long)B * T * f->np_pitch;
-        p.np_p = f->np_p; p.np_seed = f->np_seed; p.np_salt = f->np_salt;
-        if (encode_store_maps(maps, 0, f->np, f->np_pitch, B, T)) return 1;
-        if (f->np_wg) {
-            p.np_wg = 1;
-            if (encode_store_maps(maps, 2, f->np_wg, f->np_pitch, B, T)) return 1;
-        }
-    }
-    if (f->post_kind != POST_NONE) {
-        DV3_REQUIRE(f->post_kind >= POST_GLU && f->post_kind <= POST_IDENT && f->post_planes, "%s: bad post_kind %d",
-                    what, f->post_kind);
-        const bool gate = f->post_kind == POST_GLU || f->post_kind == POST_HIGHWAY;
-        DV3_REQUIRE(!gate || (f->post_a && f->post_s && out_channels % 8 == 0), "%s: gate backward needs saved a, s", what);
-        DV3_REQUIRE(f->post_kind != POST_HIGHWAY || f->post_x, "%s: highway backward needs the block input", what);
-        DV3_REQUIRE(f->post_kind != POST_RELU || f->post_a, "%s: ReLU backward needs the producer output", what);
-        p.post_kind = f->post_kind; p.post_residual = f->post_residual;
-        p.post_a = f->post_a; p.post_s = f->post_s; p.post_x = f->post_x;
-        p.post_planes = (__nv_bfloat16*)f->post_planes;
-        p.post_pitch = gate ? 2 * out_channels : (out_channels + 7) / 8 * 8;
-        p.post_plane = (long long)B * T * p.post_pitch;
-        p.post_dbias = f->post_dbias;
-        if (encode_store_maps(maps, 0, f->post_planes, p.post_pitch, B, T)) return 1;
-    }
-    return 0;
-}
-
-// Gated forward.  xd: [2][B][T][C] bf16 planes of the (dropped-out) input; w: [2][k][2C][C] bf16 planes of the
+// Gated forward.  xd: [2][B][T][C] fp16 planes of the (dropped-out) input; w: [2][k][2C][C] fp16 planes of the
 // normalised weight; the rest as dv3_convblock_fwd.  64-channel tiles (64 a | 64 b columns), BK = 32: a BK = 64
-// stage (64 KB) leaves room for only two ring stages, BK = 32 for five (H100: 1.45x faster at C=512, T=800).
+// stage (64 KB) leaves room for only two ring stages, BK = 32 for four (with five, H100: 1.45x faster at C=512,
+// T=800).
 int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bias, const float* spk,
                          const float* res, float* y, float* save_a, float* save_s, int B, int C, int T, int k,
-                         int dilation, int causal, int mode, int residual, const Dv3TcFuse* fuse, void* stream) {
+                         int dilation, int causal, int mode, int residual, const void* fuse, void* stream) {
     DV3_REQUIRE(dv3_tc_supported(B, C, T, k), "tc_convblock_fwd: unsupported shape B=%d C=%d T=%d k=%d", B, C, T, k);
     DV3_REQUIRE(npl == 2, "tc_convblock_fwd: npl must be 2");
+    DV3_REQUIRE(fuse == nullptr, "tc_convblock_fwd: fuse must be NULL");
     TcMaps maps;
     const int t_tiles = (T + 127) / 128;
     constexpr int BK = 32;
@@ -757,24 +567,23 @@ int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bi
     p.gate_mode = mode; p.residual = residual;
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (BK / 16));
     p.operand_bf16 = 0;                                          // forward operands: fp16 hi/lo planes
-    if (apply_fuse(p, maps, fuse, B, T, C, "tc_convblock_fwd")) return 1;
-    DV3_REQUIRE(p.post_kind == POST_NONE, "tc_convblock_fwd: post_kind is a data-gradient option");
     return launch_conv<TC_GATED, 2, 64, BK>(maps, p, t_tiles, C / 64, B, (cudaStream_t)stream, "tc_convblock_fwd");
 }
 
 // Generic conv / data-gradient:  out (B, Nc, T) fp32 = sum_j A[b, t+off_j, :] . W[j, n, :]  (+ epilogue)
-//   a: [2][B][T][Kp] bf16 planes, Kp = Kc rounded up to 8;  w: [2][k][Nc][Kp] bf16 planes.
-//   transpose_taps = 1 for a data gradient (offsets padl - j*d), 0 for a forward conv.
+//   a: [2][B][T][Kp] planes, Kp = Kc rounded up to 8;  w: [2][k][Nc][Kp] planes (fp16 pairs for a forward conv, bf16
+//   pairs for a data gradient).  transpose_taps = 1 for a data gradient (offsets padl - j*d), 0 for a forward conv.
 // Tile width: 128 output channels, or 64 when 128-wide tiles would leave most of the SMs idle.  BK: 32 for 128-wide
-// tiles (a 64 KB BK = 64 stage would leave two ring stages, BK = 32 gives five); 64 for 64-wide tiles when
+// tiles (a 64 KB BK = 64 stage would leave two ring stages, BK = 32 gives four); 64 for 64-wide tiles when
 // Kc % 64 == 0 (else 32: the 80-channel mel input, the 513-wide linear output, the 16-wide speaker embedding).
 int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc, int Nc, int T, int k, int dilation,
                 int causal, int transpose_taps, const float* bias, int relu, float p_drop,
                 const unsigned long long* seed_ptr, unsigned salt, int addmode, const float* e1, const float* e2,
-                float alpha, const Dv3TcFuse* fuse, void* stream) {
+                float alpha, const void* fuse, void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS_TC && (k == 1 || Nc % 128 == 0) && B <= 65535,
                 "tc_conv: unsupported shape B=%d Kc=%d Nc=%d T=%d k=%d", B, Kc, Nc, T, k);
     DV3_REQUIRE(npl == 2, "tc_conv: npl must be 2");
+    DV3_REQUIRE(fuse == nullptr, "tc_conv: fuse must be NULL");
     const int Kp = (Kc + 7) / 8 * 8;
     const int t_tiles = (T + 127) / 128;
     cudaStream_t st = (cudaStream_t)stream;
@@ -797,7 +606,6 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (bk / 16));
     // forward conv: fp16 activation x fp16 weight planes; data gradient: bf16 gradient x bf16 weight planes
     p.operand_bf16 = transpose_taps ? 1 : 0;
-    if (apply_fuse(p, maps, fuse, B, T, Nc, "tc_conv")) return 1;
     const int tiles_y = (Nc + br - 1) / br;
     if (narrow) {
         if (k64) return launch_conv<TC_CONV, 1, 64, 64>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64)");

@@ -108,16 +108,15 @@ def test_product_never_imports_oracle():
 
 
 def test_ctypes_structs_match_the_c_header(tmp_path):
-    """The structs that cross the C ABI by pointer (Dv3WnEntry, Dv3TcFuse, Dv3IncStep, Dv3IncAttn) are mirrored by hand in
+    """The structs that cross the C ABI by pointer (Dv3WnEntry, Dv3IncStep, Dv3IncAttn) are mirrored by hand in
     ctypes; compile the header with gcc and compare sizeof / every field offset."""
     import ctypes
     import os
     import subprocess
     from deepvoice3_pytorch_b200.weight_bank import Dv3WnEntry
     from deepvoice3_pytorch_b200.incremental import Dv3IncStep, Dv3IncAttn
-    from deepvoice3_pytorch_b200.ops import Dv3TcFuse
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    structs = {"Dv3WnEntry": Dv3WnEntry, "Dv3IncStep": Dv3IncStep, "Dv3IncAttn": Dv3IncAttn, "Dv3TcFuse": Dv3TcFuse}
+    structs = {"Dv3WnEntry": Dv3WnEntry, "Dv3IncStep": Dv3IncStep, "Dv3IncAttn": Dv3IncAttn}
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "dv3b200.h"', 'int main(void) {']
     for name, st in structs.items():
         lines.append('printf("%s sizeof %%zu\\n", sizeof(%s));' % (name, name))

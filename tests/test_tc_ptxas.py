@@ -1,5 +1,6 @@
 """Compile-time guard of the tensor-core conv kernel (no GPU needed): every tc_conv_kernel instantiation must keep its
-wgmma chain pipelined (no ptxas C7511 "wgmma.mma_async instructions are serialized") and must not spill."""
+wgmma chain pipelined (no ptxas C7511 "wgmma.mma_async instructions are serialized"), must not spill and must use no
+local memory at all (0-byte stack frame)."""
 import os
 import re
 import shutil
@@ -31,16 +32,17 @@ def ptxas_report(tmp_path_factory):
 
 
 def _conv_kernels(report):
-    """-> {mangled name: (spill store bytes, spill load bytes)} of every tc_conv_kernel instantiation."""
+    """-> {mangled name: (stack frame bytes, spill store bytes, spill load bytes)} of every tc_conv_kernel
+    instantiation."""
     kernels, cur = {}, None
     for line in report.splitlines():
         m = re.search(r"Compiling entry function '(\w+)'", line)
         if m:
             cur = m.group(1) if "tc_conv_kernel" in m.group(1) else None
             continue
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", line)
+        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", line)
         if m and cur is not None:
-            kernels[cur] = (int(m.group(1)), int(m.group(2)))
+            kernels[cur] = (int(m.group(1)), int(m.group(2)), int(m.group(3)))
             cur = None
     return kernels
 
@@ -54,5 +56,12 @@ def test_tc_conv_kernel_wgmma_not_serialized(ptxas_report):
 def test_tc_conv_kernel_no_spills(ptxas_report):
     kernels = _conv_kernels(ptxas_report)
     assert kernels, "no tc_conv_kernel instantiation in the ptxas report"
-    spilling = {k: v for k, v in kernels.items() if v != (0, 0)}
+    spilling = {k: v[1:] for k, v in kernels.items() if v[1:] != (0, 0)}
     assert not spilling, "tc_conv_kernel spills (store, load bytes): %s" % spilling
+
+
+def test_tc_conv_kernel_no_stack_frame(ptxas_report):
+    kernels = _conv_kernels(ptxas_report)
+    assert kernels, "no tc_conv_kernel instantiation in the ptxas report"
+    framed = {k: v[0] for k, v in kernels.items() if v[0] != 0}
+    assert not framed, "tc_conv_kernel uses local memory (stack frame bytes): %s" % framed
