@@ -198,25 +198,44 @@ def inv_num_samples(n_frames):
 
 def griffin_lim(mag, n_iter=None):
     """mag: (T, 513) fp32 CUDA tensor of linear magnitudes -> waveform (n,) whose STFT magnitude approximates it.
-    x <- istft(mag * exp(i*angle(stft(x)))), started from the zero-phase inverse; every arrow is one kernel launch."""
+    x <- istft(mag * exp(i*angle(stft(x)))), started from the zero-phase inverse; every arrow is one kernel launch
+    (the batched kernels with one clip: ``griffin_lim_batch``)."""
     if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 2):
         raise Dv3Error("griffin_lim needs a (T, 513) fp32 CUDA tensor; there is no CPU path")
-    if hparams.fft_size != 1024 or hparams.hop_size != 256 or mag.shape[1] != 513:
+    return griffin_lim_batch(mag[None], [mag.shape[0]], n_iter)[0]
+
+
+def griffin_lim_batch(mag, n_frames, n_iter=None):
+    """mag: (nclips, T_max, 513) fp32 CUDA tensor, clip c valid for its first n_frames[c] frames -> waveforms
+    (nclips, n_max), clip c valid for its first inv_num_samples(n_frames[c]) samples and zero after them.  Each clip
+    comes out bit-identical to ``griffin_lim`` on that clip alone: the kernels read and write only a clip's own frames
+    and samples, and the overlap-add is deterministic (csrc/istft.cu)."""
+    if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 3):
+        raise Dv3Error("griffin_lim_batch needs a (nclips, T, 513) fp32 CUDA tensor; there is no CPU path")
+    if hparams.fft_size != 1024 or hparams.hop_size != 256 or mag.shape[2] != 513:
         raise Dv3Error("the inverse kernels are built for fft_size=1024, hop_size=256")
     mag = mag.contiguous()
-    T = mag.shape[0]
-    n = inv_num_samples(T)
-    if n < 1:
-        raise Dv3Error("too few frames (%d) to reconstruct a waveform" % T)
+    nclips, T_max = mag.shape[:2]
+    n_frames = [int(t) for t in n_frames]
+    if len(n_frames) != nclips or not all(1 <= t <= T_max for t in n_frames):
+        raise Dv3Error("n_frames must give 1..%d frames for each of the %d clips" % (T_max, nclips))
+    n_samples = [inv_num_samples(t) for t in n_frames]
+    if min(n_samples) < 1:
+        raise Dv3Error("too few frames (%d) to reconstruct a waveform" % min(n_frames))
+    dev = mag.device
+    n_max = max(n_samples)
+    frames_d = torch.tensor(n_frames, dtype=torch.int32).to(dev)
+    samples_d = torch.tensor(n_samples, dtype=torch.int32).to(dev)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    spec = torch.zeros(T, 513, 2, device=mag.device)
+    spec = torch.zeros(nclips, T_max, 513, 2, device=dev)
     spec[..., 0] = mag                                   # zero phase
-    x = torch.zeros(n, device=mag.device)
-    lib.call("dv3_istft", _cp(spec), _cp(x), n, T, st)
+    x = torch.zeros(nclips, n_max, device=dev)
+    lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
     for _ in range(hparams.griffin_lim_iters if n_iter is None else n_iter):
-        lib.call("dv3_stft_complex", _cp(x), n, _cp(mag), _cp(spec), T, st)
+        lib.call("dv3_stft_complex_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
+                 T_max, nclips, st)
         x.zero_()
-        lib.call("dv3_istft", _cp(spec), _cp(x), n, T, st)
+        lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
     return x
 
 
@@ -236,9 +255,29 @@ def inv_preemphasis(x):
 def inv_spectrogram(spectrogram, n_iter=None):
     """(513, T) normalised dB spectrogram (what ``spectrogram`` returns / the model predicts, transposed) -> waveform
     float32 numpy array -- reference audio.py:37-43: denormalise, dB -> amplitude, ** power, phase recovery, inverse
-    STFT, de-emphasis."""
-    S = torch.as_tensor(np.ascontiguousarray(np.asarray(spectrogram, dtype=np.float32).T)).cuda()   # (T, 513)
+    STFT, de-emphasis.  The one-clip case of ``inv_spectrogram_batch``."""
+    return inv_spectrogram_batch([spectrogram], n_iter)[0]
+
+
+def inv_spectrogram_batch(spectrograms, n_iter=None):
+    """[(513, T_c) normalised dB spectrograms] -> [waveform c (float32 numpy array)], all clips in one set of launches
+    per Griffin-Lim iteration.  Clip c is bit-identical to ``inv_spectrogram(spectrograms[c])``: the magnitude and
+    de-emphasis kernels work element by element / causally along each clip, and the phase recovery is
+    ``griffin_lim_batch``."""
+    specs = [np.asarray(s, dtype=np.float32) for s in spectrograms]
+    if not specs:
+        raise ValueError("inv_spectrogram_batch needs at least one spectrogram")
+    for s in specs:
+        if s.ndim != 2 or s.shape[0] != 513:
+            raise Dv3Error("spectrograms must be (513, T) arrays, got %s" % (s.shape,))
+    n_frames = [s.shape[1] for s in specs]
+    S = np.zeros((len(specs), max(n_frames), 513), dtype=np.float32)
+    for c, s in enumerate(specs):
+        S[c, :s.shape[1]] = s.T
+    S = torch.from_numpy(S).cuda()
     amp = torch.empty_like(S)
+    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     lib.call("dv3_spec_to_amp", _cp(S), _cp(amp), S.numel(), float(hparams.min_level_db), float(hparams.ref_level_db),
-             float(hparams.power), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
-    return inv_preemphasis(griffin_lim(amp, n_iter)).cpu().numpy()
+             float(hparams.power), st)
+    wav = inv_preemphasis(griffin_lim_batch(amp, n_frames, n_iter)).cpu().numpy()
+    return [wav[c, :inv_num_samples(t)].copy() for c, t in enumerate(n_frames)]

@@ -139,8 +139,11 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
     }
 }
 
-// one CTA per batch row: scores = q . keys, monotonic window, softmax, context = probs . values * Ts*sqrt(1/Ts)
-__global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constant__ Dv3IncAttn p) {
+// one CTA per batch row: scores = q . keys, monotonic window, softmax, context = probs . values * Ts*sqrt(1/Ts).
+// ROWS (ragged batch): row b sees only its own Ts = text_len[b] keys (the key pitch stays p.Ts) and keeps its own
+// cursor; with Ts substituted, the arithmetic is that of the single-row launch, so each row matches it bit for bit.
+template <bool ROWS>
+__global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constant__ Dv3IncAttn p, const int* text_len) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     extern __shared__ float sm[];
     float* q = sm;                 // [E]
@@ -149,19 +152,23 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
     __shared__ float bcast;
     const int b = blockIdx.x, tid = threadIdx.x;
     const long long t = p.t_ptr ? (long long)*p.t_ptr : 0;
+    const int Ts = ROWS ? text_len[b] : p.Ts;
+    // cursor slots: [2] (row 0 leads every row, reference deepvoice3.py:443) or [2][B] (one per row)
+    const int cur_rd = ROWS ? (int)(t & 1) * p.B + b : (int)(t & 1);
+    const int cur_wr = ROWS ? (int)((t + 1) & 1) * p.B + b : (int)((t + 1) & 1);
     for (int e = tid; e < p.E; e += 256) q[e] = p.q[b * p.q_ld + e];
     __syncthreads();
-    int lo = 0, hi = p.Ts;                                  // unmasked key range
+    int lo = 0, hi = Ts;                                    // unmasked key range
     if (p.last_attended) {
-        const int la = p.last_attended[t & 1];
+        const int la = p.last_attended[cur_rd];
         const int backward = la - p.window_backward;
         if (backward > 0) lo = backward;
         const int ahead = la + p.window_ahead;
-        if (ahead < p.Ts) hi = ahead;
+        if (ahead < Ts) hi = ahead;
     }
     const float* __restrict__ K = p.keys + (size_t)b * p.E * p.Ts;
     float mx = -INFINITY;
-    for (int s = tid; s < p.Ts; s += 256) {
+    for (int s = tid; s < Ts; s += 256) {
         float acc = 0.f;
         for (int e = 0; e < p.E; ++e) acc = fmaf(q[e], K[(size_t)e * p.Ts + s], acc);
         if (s < lo || s >= hi) acc = -INFINITY;
@@ -176,7 +183,7 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
     __syncthreads();
     mx = bcast;
     float sum = 0.f;
-    for (int s = tid; s < p.Ts; s += 256) { const float e = expf(sc[s] - mx); sc[s] = e; sum += e; }
+    for (int s = tid; s < Ts; s += 256) { const float e = expf(sc[s] - mx); sc[s] = e; sum += e; }
     sum = warp_sum(sum);
     __syncthreads();                                        // everybody has read bcast
     if ((tid & 31) == 0) red[tid >> 5] = sum;
@@ -184,22 +191,24 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
     if (tid == 0) { float s = 0.f; for (int i = 0; i < 8; ++i) s += red[i]; bcast = s; }
     __syncthreads();
     const float inv = 1.f / bcast;
-    for (int s = tid; s < p.Ts; s += 256) {
+    for (int s = tid; s < Ts; s += 256) {
         const float pr = sc[s] * inv;
         sc[s] = pr;
         if (p.align) p.align[b * p.align_ld + t * p.align_t + s] = pr * p.align_scale;
     }
+    if (ROWS && p.align)
+        for (int s = Ts + tid; s < p.Ts; s += 256) p.align[b * p.align_ld + t * p.align_t + s] = 0.f;
     __syncthreads();
-    if (p.last_attended && b == 0 && tid == 0) {            // reference: alignment.max(-1)[1] of batch row 0
+    if (p.last_attended && (ROWS || b == 0) && tid == 0) {  // reference: alignment.max(-1)[1] of batch row 0
         int best = 0; float bv = sc[0];
-        for (int s = 1; s < p.Ts; ++s) if (sc[s] > bv) { bv = sc[s]; best = s; }
-        p.last_attended[(t + 1) & 1] = best;
+        for (int s = 1; s < Ts; ++s) if (sc[s] > bv) { bv = sc[s]; best = s; }
+        p.last_attended[cur_wr] = best;
     }
     const float* __restrict__ V = p.values + (size_t)b * p.Ts * p.E;
-    const float scale = (float)p.Ts * sqrtf(1.0f / (float)p.Ts);
+    const float scale = (float)Ts * sqrtf(1.0f / (float)Ts);
     for (int e = tid; e < p.E; e += 256) {
         float acc = 0.f;
-        for (int s = 0; s < p.Ts; ++s) acc = fmaf(sc[s], V[(size_t)s * p.E + e], acc);
+        for (int s = 0; s < Ts; ++s) acc = fmaf(sc[s], V[(size_t)s * p.E + e], acc);
         p.ctx[b * p.ctx_ld + e] = acc * scale;
     }
 }
@@ -231,8 +240,17 @@ int dv3_inc_attn_step(const Dv3IncAttn* p, void* stream) {
     DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0, "inc_attn_step: bad shape");
     const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
     DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step: E + Ts = %d floats exceed 48 KB of shared memory", p->E + p->Ts);
-    launch_k(inc_attn_step_kernel, p->B, 256, smem, (cudaStream_t)stream, *p);
+    launch_k(inc_attn_step_kernel<false>, p->B, 256, smem, (cudaStream_t)stream, *p, (const int*)nullptr);
     return check_launch("inc_attn_step");
+}
+
+int dv3_inc_attn_step_rows(const Dv3IncAttn* p, const int* text_len, void* stream) {
+    DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0 && text_len, "inc_attn_step_rows: bad shape");
+    const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
+    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_rows: E + Ts = %d floats exceed 48 KB of shared memory",
+                p->E + p->Ts);
+    launch_k(inc_attn_step_kernel<true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
+    return check_launch("inc_attn_step_rows");
 }
 
 int dv3_inc_advance(int* t_ptr, void* stream) {

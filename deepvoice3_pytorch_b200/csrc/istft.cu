@@ -9,7 +9,12 @@
 // Kernels (one CTA of 256 threads per frame, the shared-memory radix-2 transform of stft.cu):
 //   spec_to_amp_kernel      normalised dB spectrogram -> linear magnitude ** power
 //   stft_complex_kernel     waveform -> complex half spectrum (frames, 513) [optionally projected onto a magnitude]
-//   istft_kernel            complex half spectrum -> windowed frame, overlap-added into the waveform (atomicAdd)
+//   istft_kernel            complex half spectrum -> windowed frame, overlap-added into the waveform: frames f and f+4
+//                           do not overlap (fsize = 4*hop), so one launch per residue class f mod 4 adds with plain
+//                           loads and stores -- deterministic, each sample summed in the same order every run
+// Both take a clip grid dimension (blockIdx.y): clip c has its own sample / frame counts (lens / frames arrays, or the
+// scalar when the array is NULL) and pitches, so a ragged batch of clips runs in one launch and every clip gets exactly
+// what it gets alone.
 //   deemphasis_kernel       y[n] = x[n] + c*y[n-1] (a 1st-order IIR: one thread per clip, chunks staged through smem)
 #include "common.cuh"
 
@@ -53,13 +58,19 @@ __global__ void spec_to_amp_kernel(const float* __restrict__ s, float* __restric
 
 // wav (len) -> spec (nframes, 513, 2).  mag != null: the result is projected onto that magnitude (Griffin-Lim step):
 // spec = mag * X / |X| (X == 0 keeps phase 0).  No preemphasis here (the iteration runs on the pre-emphasised signal).
-__global__ void __launch_bounds__(256) stft_complex_kernel(const float* __restrict__ x, int len,
-                                                           const float* __restrict__ mag, float* __restrict__ spec,
-                                                           int nframes) {
+// Clip c = blockIdx.y: x + c*x_pitch, spec / mag + c*frame_pitch frames; len / nframes from lens / frames when given.
+__global__ void __launch_bounds__(256) stft_complex_kernel(const float* __restrict__ x, int len0, const int* lens,
+                                                           long long x_pitch, const float* __restrict__ mag,
+                                                           float* __restrict__ spec, int nframes0, const int* frames,
+                                                           long long frame_pitch) {
     pdl_trigger(); pdl_wait();
     __shared__ float zr[INH], zi[INH], twr[INH / 2], twi[INH / 2];
-    const int frame = blockIdx.x, tid = threadIdx.x;
+    const int frame = blockIdx.x, clip = blockIdx.y, tid = threadIdx.x;
+    const int nframes = frames ? frames[clip] : nframes0, len = lens ? lens[clip] : len0;
     if (frame >= nframes) return;
+    x += clip * x_pitch;
+    spec += clip * frame_pitch * INBINS * 2;
+    if (mag) mag += clip * frame_pitch * INBINS;
     { float s, c; sincospif(-(float)tid / 256.f, &s, &c); twr[tid] = c; twi[tid] = s; }
     const int base = frame * IHOP - IPAD;
 #pragma unroll
@@ -94,17 +105,21 @@ __global__ void __launch_bounds__(256) stft_complex_kernel(const float* __restri
 }
 
 // spec (nframes, 513, 2) -> y (len) += window * irfft(spec[frame]) placed at frame*hop - pad   (y zeroed by the caller)
+// for the frames frame = 4*blockIdx.x + residue: no two of them overlap, so the add is a plain load and store.
 // Inverse real FFT through the same 512-point complex transform: Z[k] = E[k] + i*O[k] with
 // E = (X[k] + conj(X[512-k]))/2, O = (X[k] - conj(X[512-k]))/2 * conj(W1024^k); z = IFFT512(Z); x[2n] = Re z, x[2n+1] = Im z.
 // IFFT via conjugation: ifft(Z) = conj(fft(conj(Z))) / 512.
-__global__ void __launch_bounds__(256) istft_kernel(const float* __restrict__ spec, float* __restrict__ y, int len,
-                                                    int nframes) {
+__global__ void __launch_bounds__(256) istft_kernel(const float* __restrict__ spec, float* __restrict__ y, int len0,
+                                                    const int* lens, long long y_pitch, int nframes0,
+                                                    const int* frames, long long frame_pitch, int residue) {
     pdl_trigger(); pdl_wait();
     __shared__ float zr[INH], zi[INH], twr[INH / 2], twi[INH / 2];
-    const int frame = blockIdx.x, tid = threadIdx.x;
+    const int frame = 4 * blockIdx.x + residue, clip = blockIdx.y, tid = threadIdx.x;
+    const int nframes = frames ? frames[clip] : nframes0, len = lens ? lens[clip] : len0;
     if (frame >= nframes) return;
+    y += clip * y_pitch;
     { float s, c; sincospif(-(float)tid / 256.f, &s, &c); twr[tid] = c; twi[tid] = s; }
-    const float* X = spec + (size_t)frame * INBINS * 2;
+    const float* X = spec + (clip * frame_pitch + frame) * INBINS * 2;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
         const int k = tid + h * 256;                                   // 0..511
@@ -128,8 +143,8 @@ __global__ void __launch_bounds__(256) istft_kernel(const float* __restrict__ sp
         const int n = tid + h * 256;
         const float v0 = zr[n] * inv, v1 = -zi[n] * inv;                 // conj back
         const int s0 = base + 2 * n, s1 = s0 + 1;
-        if (s0 >= 0 && s0 < len) atomicAdd(&y[s0], v0 * frame_window(2 * n));
-        if (s1 >= 0 && s1 < len) atomicAdd(&y[s1], v1 * frame_window(2 * n + 1));
+        if (s0 >= 0 && s0 < len) y[s0] += v0 * frame_window(2 * n);
+        if (s1 >= 0 && s1 < len) y[s1] += v1 * frame_window(2 * n + 1);
     }
 }
 
@@ -171,16 +186,51 @@ int dv3_spec_to_amp(const float* spec_norm, float* amp, long long n, float min_l
     return check_launch("spec_to_amp");
 }
 
+static int stft_complex_launch(const float* wav, int len0, const int* lens, long long pitch, const float* mag,
+                               float* spec, int nframes0, const int* frames, int max_frames, int nclips,
+                               cudaStream_t st) {
+    launch_k(stft_complex_kernel, dim3(max_frames, nclips), 256, 0, st, wav, len0, lens, pitch, mag, spec, nframes0,
+             frames, (long long)max_frames);
+    return check_launch("stft_complex");
+}
+
+// four ordered launches, one per residue class of the frame index (see istft_kernel)
+static int istft_launch(const float* spec, float* wav, int len0, const int* lens, long long pitch, int nframes0,
+                        const int* frames, int max_frames, int nclips, cudaStream_t st) {
+    for (int r = 0; r < 4; ++r) {
+        const int gx = (max_frames - r + 3) / 4;
+        if (gx < 1) break;
+        launch_k(istft_kernel, dim3(gx, nclips), 256, 0, st, spec, wav, len0, lens, pitch, nframes0, frames,
+                 (long long)max_frames, r);
+        if (int e = check_launch("istft")) return e;
+    }
+    return 0;
+}
+
 int dv3_stft_complex(const float* wav, int n_samples, const float* mag, float* spec, int nframes, void* stream) {
     DV3_REQUIRE(nframes >= 1 && n_samples >= 1, "stft_complex: empty input");
-    launch_k(stft_complex_kernel, nframes, 256, 0, (cudaStream_t)stream, wav, n_samples, mag, spec, nframes);
-    return check_launch("stft_complex");
+    return stft_complex_launch(wav, n_samples, nullptr, 0, mag, spec, nframes, nullptr, nframes, 1,
+                               (cudaStream_t)stream);
 }
 
 int dv3_istft(const float* spec, float* wav, int n_samples, int nframes, void* stream) {
     DV3_REQUIRE(nframes >= 1 && n_samples >= 1, "istft: empty input");
-    launch_k(istft_kernel, nframes, 256, 0, (cudaStream_t)stream, spec, wav, n_samples, nframes);
-    return check_launch("istft");
+    return istft_launch(spec, wav, n_samples, nullptr, 0, nframes, nullptr, nframes, 1, (cudaStream_t)stream);
+}
+
+int dv3_stft_complex_batched(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
+                             float* spec, const int* nframes, int max_frames, int nclips, void* stream) {
+    DV3_REQUIRE(max_frames >= 1 && nclips >= 1 && nclips <= 65535 && n_samples && nframes,
+                "stft_complex_batched: bad shape");
+    return stft_complex_launch(wav, 0, n_samples, wav_pitch, mag, spec, 0, nframes, max_frames, nclips,
+                               (cudaStream_t)stream);
+}
+
+int dv3_istft_batched(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
+                      int max_frames, int nclips, void* stream) {
+    DV3_REQUIRE(max_frames >= 1 && nclips >= 1 && nclips <= 65535 && n_samples && nframes,
+                "istft_batched: bad shape");
+    return istft_launch(spec, wav, 0, n_samples, wav_pitch, 0, nframes, max_frames, nclips, (cudaStream_t)stream);
 }
 
 int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long long stride, float coef, void* stream) {

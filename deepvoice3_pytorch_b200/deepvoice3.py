@@ -13,7 +13,7 @@ from torch.nn import functional as F
 
 from . import ops
 from .modules import (Conv1d, ConvTranspose1d, Embedding, Linear, SinusoidalEncoding, Conv1dGLU,
-                      get_mask_from_lengths, run_conv_stack)
+                      get_mask_from_lengths, mask_conv_input, run_conv_stack)
 
 SQRT_HALF = math.sqrt(0.5)
 
@@ -322,7 +322,7 @@ class Converter(nn.Module):
         i = 0
         while i < len(layers):
             if _is_upsampler(layers[i]):
-                x = layers[i](x)
+                x = layers[i](mask_conv_input(layers[i], x))
                 i += 1
                 continue
             j = i

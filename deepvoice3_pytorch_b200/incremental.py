@@ -12,6 +12,10 @@ and discards the few frames computed past the reference's stopping point.  Weigh
 key / value projections are hoisted out of the loop (the reference recomputes them every step, deepvoice3.py:136-141).
 Quirks kept on purpose: the "average" alignment is first_layer * 2**(n-1) / n (``ave_alignment + ave_alignment``,
 deepvoice3.py:446) and the monotonic cursor follows batch row 0 only (deepvoice3.py:443).
+
+``decode_ragged`` is the batched form for rows of different text lengths (``synthesis.tts_batch``): row b attends to
+its own text_lengths[b] keys with its own monotonic cursor and stops by the reference's rule applied to it alone, so
+every row gets what ``decode`` gives for that row on its own, bit for bit (every step kernel works per row).
 """
 import ctypes
 import os
@@ -76,7 +80,7 @@ class StepProgram:
 
     def __init__(self, B, device):
         self.B, self.dev = B, device
-        self.calls = []                     # (entry point name, ctypes struct)
+        self.calls = []                     # (entry point name, ctypes struct, extra arguments)
         self.keep = []                      # tensors the structs point into
         self.t = torch.zeros(1, dtype=torch.int32, device=device)
         self.graph = None
@@ -120,10 +124,12 @@ class StepProgram:
         s.B, s.Cin, s.Cout, s.k, s.dilation, s.mode, s.act = self.B, Cin, Cout, k, d, mode, act
         s.vec4 = int(Cin % 4 == 0 and x.aligned16() and (add is None or add.aligned16()))
         self.keep += [w, bias]
-        self.calls.append(("dv3_inc_conv_step", s))
+        self.calls.append(("dv3_inc_conv_step", s, ()))
         return y
 
-    def attention(self, q, keys_bet, values_bte, ctx, align, align_scale, last_attended, window_backward, window_ahead):
+    def attention(self, q, keys_bet, values_bte, ctx, align, align_scale, last_attended, window_backward, window_ahead,
+                  text_len=None):
+        """text_len: int32 (B,) device tensor -> the per-row (ragged) step, last_attended then holds [2][B] cursors."""
         a = Dv3IncAttn()
         B, E, Ts = keys_bet.shape
         a.q, a.q_ld = q.ptr, q.ld
@@ -137,13 +143,17 @@ class StepProgram:
         a.align_scale = align_scale
         a.B, a.E, a.Ts, a.window_backward, a.window_ahead = B, E, Ts, window_backward, window_ahead
         self.keep += [keys_bet, values_bte]
-        self.calls.append(("dv3_inc_attn_step", a))
+        if text_len is None:
+            self.calls.append(("dv3_inc_attn_step", a, ()))
+        else:
+            self.keep.append(text_len)
+            self.calls.append(("dv3_inc_attn_step_rows", a, (ctypes.c_void_p(text_len.data_ptr()),)))
 
     # -- execution --------------------------------------------------------------------------------
     def _launch_step(self):
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        for name, s in self.calls:
-            lib.call(name, ctypes.byref(s), st)
+        for name, s, extra in self.calls:
+            lib.call(name, ctypes.byref(s), *extra, st)
         lib.call("dv3_inc_advance", ctypes.c_void_p(self.t.data_ptr()), st)
 
     def run(self, n_steps, use_graph=True):
@@ -236,11 +246,35 @@ def _stop_step(done, min_steps, max_steps):
     return None
 
 
+def _row_stop_steps(done, min_steps, max_steps):
+    """The stop rule of ``_stop_step`` applied to every row alone: [N_b or None] for done flags (B, n)."""
+    return [_stop_step(done[b:b + 1], min_steps, max_steps) for b in range(done.size(0))]
+
+
 @torch.no_grad()
 def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_input=None, test_inputs=None,
            use_graph=None):
     """-> outputs (B, N, in_dim*r), alignments (B, N, T_text), dones [N x (B,1,1)], decoder_states (B, N, C): what
     the reference's Decoder.incremental_forward returns."""
+    return _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph)
+
+
+@torch.no_grad()
+def decode_ragged(decoder, encoder_out, text_positions, text_lengths, speaker_embed=None, initial_input=None,
+                  test_inputs=None, use_graph=None):
+    """Batched decode of rows with text_lengths (B,) valid keys each (encoder outputs padded to T_text).
+    -> outputs (B, N, in_dim*r), alignments (B, N, T_text), dones (B, N), decoder_states (B, N, C), steps [B]:
+    row b is valid for its first steps[b] decoder steps (and its first text_lengths[b] alignment columns; the rest are
+    0) and there equals ``decode`` run on that row alone with its encoder outputs cut to text_lengths[b].  Free-running,
+    row b stops by the reference rule applied to its own done flags; rows that stopped keep computing until the last
+    one does, their extra frames are not part of the result.  Teacher-forced (test_inputs (B, N, in_dim*r)), every row
+    runs N steps."""
+    return _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph,
+                   text_lengths=text_lengths)
+
+
+def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph,
+            text_lengths=None):
     if decoder.training:
         raise RuntimeError("incremental_forward only supports eval mode")     # reference conv.py:19-20
     if use_graph is None:
@@ -251,6 +285,14 @@ def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_inp
         raise RuntimeError("incremental decoding runs on the GPU only (no CPU fallback)")
     B, Ts, E = keys.shape
     dev = keys.device
+    ragged = text_lengths is not None
+    if ragged:
+        text_len = torch.as_tensor(text_lengths).to(device=dev, dtype=torch.int32).reshape(-1).contiguous()
+        lens_host = text_len.tolist()
+        if len(lens_host) != B or min(lens_host) < 1 or max(lens_host) > Ts:
+            raise ValueError("text_lengths must hold B = %d lengths in [1, %d], got %s" % (B, Ts, lens_host))
+    else:
+        text_len = None
     Fr = decoder.in_dim * decoder.r
     old_math = ops.conv_math
     ops.conv_math = "fp32"                       # one-off set-up GEMMs (projections) in exact fp32
@@ -312,7 +354,7 @@ def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_inp
         def cursor(force):
             if not force:
                 return None
-            la = torch.zeros(2, dtype=torch.int32, device=dev)
+            la = torch.zeros(2 * B if ragged else 2, dtype=torch.int32, device=dev)
             prog.keep.append(la)
             return la
 
@@ -326,7 +368,7 @@ def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_inp
             q = prog.conv(q_in, att.query_projection)
             ctx = _Rows(prog.buf(B, E), E)
             prog.attention(q, kv[0][0], kv[0][1], ctx, align_rows, 1.0, cursor(decoder.force_monotonic_attention),
-                           att.window_backward, att.window_ahead)
+                           att.window_backward, att.window_ahead, text_len)
             prog.conv(ctx, att.out_projection, res1=q_in, y=_Rows(cat, D, ld=2 * D))
             cur = _run_stack(prog, decoder.audio_decoder_modules, _Rows(cat, 2 * D), last_y=states_rows)
         else:
@@ -347,7 +389,7 @@ def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_inp
                 first = ai == 0
                 prog.attention(q, kv[ai][0], kv[ai][1], ctx, align_rows if first else None,
                                float(2 ** (n_att - 1)) / n_att, cursor(decoder.force_monotonic_attention[idx]),
-                               att.window_backward, att.window_ahead)
+                               att.window_backward, att.window_ahead, text_len)
                 cur = prog.conv(ctx, att.out_projection, res1=q_in, res2=residual, y=dst)
                 ai += 1
         xraw = _Rows(prog.buf(B, Fr), Fr)
@@ -358,17 +400,29 @@ def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_inp
         ops.conv_math = old_math
 
     # ---- run ---------------------------------------------------------------------------------------
+    def stop_steps(done):
+        """-> steps per row once every row has stopped, else None (decode: all rows stop together)."""
+        if ragged:
+            steps = _row_stop_steps(done, decoder.min_decoder_steps, decoder.max_decoder_steps)
+            return None if None in steps else steps
+        n = _stop_step(done, decoder.min_decoder_steps, decoder.max_decoder_steps)
+        return None if n is None else [n] * B
+
     if test_inputs is not None:
         prog.run(Tmax, use_graph)
-        N = Tmax
+        steps = [Tmax] * B
     else:
-        N, done_steps = None, 0
-        while N is None:
+        steps, done_steps = None, 0
+        while steps is None:
             n = min(CHECK_EVERY, Tmax - done_steps)
             prog.run(n, use_graph)
             done_steps += n
-            N = _stop_step(dones[:, :done_steps], decoder.min_decoder_steps, decoder.max_decoder_steps)
-            assert N is not None or done_steps < Tmax
+            steps = stop_steps(dones[:, :done_steps])
+            assert steps is not None or done_steps < Tmax
+    N = max(steps)
+    if ragged:
+        return (frames[:, 1:N + 1].contiguous(), aligns[:, :N].clone(), dones[:, :N].clone(),
+                states[:, :N].contiguous(), steps)
     outputs = frames[:, 1:N + 1].contiguous()
     done_list = [dones[:, t].reshape(B, 1, 1).clone() for t in range(N)]
     return outputs, aligns[:, :N].clone(), done_list, states[:, :N].contiguous()

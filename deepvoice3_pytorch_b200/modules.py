@@ -199,6 +199,17 @@ def get_mask_from_lengths(memory, memory_lengths):
     return (~mask).to(memory.device)
 
 
+def mask_conv_input(f, x):
+    """Inside an ``ops.length_scope``: zero each row's frames past its length before a layer whose kernel spans more
+    than one frame.  Outside one, x unchanged."""
+    if ops._length_scope is None:
+        return x
+    conv = f.conv if isinstance(f, _GatedConv) else f
+    if isinstance(conv, (_Conv1d, _ConvTranspose1d)) and conv.kernel_size[0] > 1:
+        return ops.mask_time(x)
+    return x
+
+
 def run_conv_stack(layers, x, speaker_embed_btc=None, boundaries=None):
     """Run a ModuleList/Sequential of [Conv1d | ReLU | Sigmoid | ConvTranspose1d | Conv1dGLU | HighwayConv1d]
     on x (B, C, T), fusing every ``Conv1d -> ReLU`` pair into one kernel launch.
@@ -210,6 +221,7 @@ def run_conv_stack(layers, x, speaker_embed_btc=None, boundaries=None):
         f = layers[i]
         if boundaries and i in boundaries:
             x = ops.grad_boundary(x, boundaries[i])
+        x = mask_conv_input(f, x)
         fuse_relu = isinstance(f, _Conv1d) and i + 1 < len(layers) and isinstance(layers[i + 1], nn.ReLU)
         if isinstance(f, _Conv1d):
             x = f(x, relu=fuse_relu)

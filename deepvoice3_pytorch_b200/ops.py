@@ -838,6 +838,56 @@ def linear(x, v, g, bias):
 
 
 # ----------------------------------------------------------------------------------------------
+# length scope of a padded inference batch
+# ----------------------------------------------------------------------------------------------
+_length_scope = None          # (lengths int64 (B,) on the device, T of the scope) while a scope is active
+
+
+class length_scope:
+    """``with ops.length_scope(lengths, T):`` -- the stacks run inside (``modules.run_conv_stack`` and the deepvoice3
+    converter) zero every row's frames past its own length before each conv whose kernel spans more than one frame,
+    so that each row of a padded batch sees the zeros it would see alone.  ``lengths`` counts frames at time length
+    ``T``; a stack running at T' = mult*T (after the converter's 2x upsamplers) masks from mult*lengths[b].
+    Inference only: entering with grad enabled raises.  Scopes do not nest."""
+
+    def __init__(self, lengths, T):
+        self.lengths, self.T = lengths, int(T)
+
+    def __enter__(self):
+        global _length_scope
+        if torch.is_grad_enabled():
+            raise RuntimeError("ops.length_scope is for inference: enter it under torch.no_grad()")
+        if _length_scope is not None:
+            raise RuntimeError("ops.length_scope does not nest")
+        lengths = self.lengths
+        if not (torch.is_tensor(lengths) and lengths.is_cuda and lengths.dtype == torch.int64 and lengths.dim() == 1):
+            raise Dv3Error("length_scope needs an int64 (B,) CUDA tensor of lengths")
+        _length_scope = (lengths.contiguous(), self.T)
+        return self
+
+    def __exit__(self, *exc):
+        global _length_scope
+        _length_scope = None
+        return False
+
+
+def mask_time(x):
+    """x (B,C,T) -> a new tensor with frames t >= mult*lengths[b] zeroed (mult = T // T_scope); x itself when no
+    length scope is active.  Never writes into x."""
+    if _length_scope is None:
+        return x
+    lengths, T0 = _length_scope
+    _chk(x)
+    B, C, T = x.shape
+    if B != lengths.numel() or T % T0 != 0:
+        raise Dv3Error("mask_time: x %s does not fit a length scope of %d rows at T = %d" % (tuple(x.shape),
+                                                                                          lengths.numel(), T0))
+    y = torch.empty_like(x)
+    lib.call("dv3_mask_time", _p(x), _p(y), _p(lengths), T // T0, B, C, T, _stream())
+    return y
+
+
+# ----------------------------------------------------------------------------------------------
 # attention core (channel-major): q (B,E,Td), k (B,E,Ts), v (B,E,Ts) -> out (B,E,Td), probs (B,Td,Ts)
 # ----------------------------------------------------------------------------------------------
 def _bgemm(A, sA, Bm, sB, C, sCb, ldc, batch, M, N, K, alpha=1.0, accumulate=False):

@@ -1,0 +1,118 @@
+"""Batched text-to-speech synthesis: many utterances per set of launches, each exactly as if synthesized alone.
+
+Reference synthesis.py:42-73 (``tts``) runs one sentence per call: text ids -> ``model(...)`` (encoder, autoregressive
+decoder, converter) -> ``audio.inv_spectrogram``.  ``tts_batch`` runs the same four stages on padded batches:
+
+* encoder and converter inside an ``ops.length_scope``: every row's frames past its own length are zeroed before each
+  conv that spans several frames, so each row sees the zero padding it would see alone;
+* ``incremental.decode_ragged``: per-row attention length, context scale, monotonic cursor and stopping step;
+* ``audio.inv_spectrogram_batch``: Griffin-Lim over a ragged batch of clips with a deterministic overlap-add.
+
+Every kernel on this path computes a row from that row's data alone, in an order that does not depend on the batch,
+so with ``ops.conv_math = "fp32"`` each result is bit-identical to the one-utterance path.  In the default tensor-core
+mode the batch's larger GEMMs may take the tensor-core kernels where a short single sentence runs on the exact-fp32 ones
+(``ops._use_tc_conv``), so results then agree to the tensor-core tolerance instead.
+"""
+import contextlib
+
+import numpy as np
+import torch
+
+from . import audio, incremental, ops
+
+
+def _check_inputs(model, sequences, speaker_ids, batch_size):
+    if len(sequences) == 0:
+        raise ValueError("tts_batch needs at least one sequence")
+    seqs = []
+    max_len = model.seq2seq.decoder.embed_keys_positions.num_embeddings - 1      # positions 1..L index the table
+    for i, s in enumerate(sequences):
+        s = np.asarray(s)
+        if s.ndim != 1 or s.size == 0:
+            raise ValueError("sequence %d must be a non-empty 1-D array of token ids, got shape %s" % (i, s.shape))
+        if not np.issubdtype(s.dtype, np.integer):
+            raise ValueError("sequence %d must hold integer token ids, got %s" % (i, s.dtype))
+        if s.size > max_len:
+            raise ValueError("sequence %d has %d tokens; the position tables hold %d" % (i, s.size, max_len))
+        seqs.append(s.astype(np.int64))
+    if speaker_ids is not None:
+        if model.n_speakers <= 1:
+            raise ValueError("speaker_ids given for a single-speaker model")
+        speaker_ids = [int(x) for x in speaker_ids]
+        if len(speaker_ids) != len(seqs):
+            raise ValueError("%d speaker_ids for %d sequences" % (len(speaker_ids), len(seqs)))
+    elif model.n_speakers > 1:
+        raise ValueError("a multi-speaker model needs speaker_ids")
+    if int(batch_size) < 1:
+        raise ValueError("batch_size must be >= 1, got %r" % (batch_size,))
+    if model.training:
+        raise RuntimeError("incremental_forward only supports eval mode")         # as incremental.decode
+    if not next(model.parameters()).is_cuda:
+        raise RuntimeError("incremental decoding runs on the GPU only (no CPU fallback)")
+    return seqs, speaker_ids
+
+
+@torch.no_grad()
+def _synthesize_chunk(model, seqs, speaker_ids, stage):
+    """seqs: list of int64 arrays -> [(waveform, alignment, spectrogram, mel)] for one padded batch."""
+    dev = next(model.parameters()).device
+    B = len(seqs)
+    lens = [s.size for s in seqs]
+    L = max(lens)
+    text = np.zeros((B, L), dtype=np.int64)
+    tpos = np.zeros((B, L), dtype=np.int64)
+    for b, s in enumerate(seqs):
+        text[b, :s.size] = s
+        tpos[b, :s.size] = np.arange(1, s.size + 1)
+    text, tpos = torch.from_numpy(text).to(dev), torch.from_numpy(tpos).to(dev)
+    text_len = torch.tensor(lens, dtype=torch.int64).to(dev)
+    ops.rng.begin_forward(False, dev)
+    try:
+        spk = None if speaker_ids is None else model._speaker_embedding(torch.tensor(speaker_ids).to(dev))
+        dec = model.seq2seq.decoder
+        with stage("encoder"), ops.length_scope(text_len, L):
+            keys, values = model.seq2seq.encoder(text, speaker_embed=spk)
+        with stage("decoder"):
+            outputs, aligns, _, states, steps = incremental.decode_ragged(dec, (keys, values), tpos, text_len, spk)
+        with stage("converter"):
+            mel = outputs.reshape(B, -1, model.mel_dim)
+            r = mel.size(1) // outputs.size(1)
+            post_in = states.reshape(B, mel.size(1), -1) if model.use_decoder_state_for_postnet_input else mel
+            frames = torch.tensor(steps, dtype=torch.int64).to(dev) * r
+            with ops.length_scope(frames, mel.size(1)):
+                linear = model.postnet(post_in, spk)
+            up = linear.size(1) // mel.size(1)
+            mel, linear, aligns = mel.cpu().numpy(), linear.cpu().numpy(), aligns.cpu().numpy()
+    finally:
+        ops.rng.end_forward()
+    lin_rows = [linear[b, :steps[b] * r * up] for b in range(B)]
+    with stage("vocoder"):
+        wavs = audio.inv_spectrogram_batch([x.T for x in lin_rows])
+    return [(wavs[b], aligns[b, :steps[b], :lens[b]], audio._denormalize(lin_rows[b]),
+             audio._denormalize(mel[b, :steps[b] * r])) for b in range(B)]
+
+
+def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None):
+    """Synthesize many utterances at once.
+
+    model: a ``MultiSpeakerTTSModel`` in eval mode on CUDA.  sequences: list of 1-D token-id arrays (what a text
+    frontend's ``text_to_sequence`` returns).  speaker_ids: one id per sequence for a multi-speaker model, else None.
+    Sequences are sorted by length and synthesized in padded batches of ``batch_size`` (similar lengths share a batch,
+    which bounds the decoder steps spent on rows that already stopped).
+
+    -> list, in input order, of (waveform, alignment (N_b, L_b), spectrogram, mel): what reference ``synthesis.tts``
+    returns for that sequence synthesized alone -- the same decoder steps, the denormalised linear and mel spectrograms
+    cut to the row's own frames, and its Griffin-Lim waveform (see the module docstring for when this is bit-exact).
+
+    stage_timer: optional callable ``name -> context manager`` wrapped around each stage ("encoder", "decoder",
+    "converter", "vocoder") of every batch, e.g. to time them."""
+    seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size)
+    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    order = sorted(range(len(seqs)), key=lambda i: -seqs[i].size)
+    out = [None] * len(seqs)
+    for c in range(0, len(order), int(batch_size)):
+        idx = order[c:c + int(batch_size)]
+        ids = None if speaker_ids is None else [speaker_ids[i] for i in idx]
+        for i, res in zip(idx, _synthesize_chunk(model, [seqs[i] for i in idx], ids, stage)):
+            out[i] = res
+    return out

@@ -115,6 +115,11 @@ int dv3_softmax_bwd(const float* probs, const float* dpd, const float* dprobs_ex
  * in (B,2C,T) rows ordered (j,co) -> out (B,C,2T), out[b,co,2t+j] = in[b,j*C+co,t]; inverse=1 undoes it. */
 int dv3_interleave2(const float* in, float* out, int B, int C, int T, int inverse, void* stream);
 
+/* ---- length mask of a padded batch (batched synthesis): y = x, with y[b,:,t] = 0 for t >= mult*lengths[b].
+ * x, y (B,C,T); x == y allowed; lengths int64 [B] on the device.  Zeroing a row's frames past its end before every
+ * conv that mixes time steps makes each row see exactly the zero padding it would see alone. */
+int dv3_mask_time(const float* x, float* y, const long long* lengths, int mult, int B, int C, int T, void* stream);
+
 /* ---- batched strided GEMM C[b] = alpha*A_b*B_b (+C): the attention contractions, reference
  * deepvoice3.py:143 (bmm(q,k)), :167 (bmm(p,v)) and their gradients.  A_b(m,k)=A[b*sAb+m*sAm+k*sAk],
  * B_b(k,n)=B[b*sBb+k*sBk+n*sBn], C_b(m,n)=C[b*sCb+m*ldc+n]; each operand needs one unit stride. */
@@ -167,11 +172,22 @@ int dv3_stft_mel(const float* wav, const int* lengths, const float* mel_basis, c
  * window).  The iteration x <- istft(mag * exp(i angle(stft(x)))) is driven by the host (audio.inv_spectrogram).
  * dv3_spec_to_amp: normalised dB (n) -> (10^((S*(-min)+min+ref)/20))^power.  dv3_stft_complex: wav (n_samples) ->
  * spec (nframes,513,2) [re,im]; mag (nframes,513) != NULL projects the result onto that magnitude.  dv3_istft: spec ->
- * wav (n_samples) += overlap-added frames (zero wav first).  dv3_deemphasis: y[n] = x[n] + coef*y[n-1] per clip. */
+ * wav (n_samples) += overlap-added frames (zero wav first).  dv3_deemphasis: y[n] = x[n] + coef*y[n-1] per clip.
+ * The overlap-add is deterministic: frames whose indices differ by 4 do not overlap (1024 = 4 * hop), so the four
+ * residue classes f mod 4 are added in four ordered launches with plain stores; a sample's value depends only on its
+ * own clip's frames, always summed in the same order.
+ * Batched forms: clip c has n_samples[c] samples at wav + c*wav_pitch and nframes[c] <= max_frames frames at
+ * spec + c*max_frames*513*2 (mag likewise with 513 floats per frame); both count arrays are int32 [nclips] on the
+ * device.  Samples and frames past a clip's counts are neither read nor written.  The one-clip entry points above are
+ * the same kernels with nclips = 1. */
 int dv3_spec_to_amp(const float* spec_norm, float* amp, long long n, float min_level_db, float ref_level_db,
                     float power, void* stream);
 int dv3_stft_complex(const float* wav, int n_samples, const float* mag, float* spec, int nframes, void* stream);
 int dv3_istft(const float* spec, float* wav, int n_samples, int nframes, void* stream);
+int dv3_stft_complex_batched(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
+                             float* spec, const int* nframes, int max_frames, int nclips, void* stream);
+int dv3_istft_batched(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
+                      int max_frames, int nclips, void* stream);
 int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long long stride, float coef, void* stream);
 
 /* ================= tensor-core ConvBlock / conv path: wgmma + TMA, split 16-bit operands =================
@@ -287,6 +303,12 @@ typedef struct Dv3IncAttn {
     int B, E, Ts, window_backward, window_ahead;
 } Dv3IncAttn;
 int dv3_inc_attn_step(const Dv3IncAttn* attn, void* stream);
+/* Ragged batch: row b attends to s < text_len[b] only (text_len: int32 [B] on the device, 1 <= text_len[b] <= Ts),
+ * its context is scaled by text_len[b]*sqrt(1/text_len[b]) and alignment entries s >= text_len[b] are 0.  A non-NULL
+ * last_attended holds B cursors per slot, int[2][B] (slot t&1 read, (t+1)&1 written): every row keeps its own
+ * monotonic window, clamped to its own text length.  Each row gives what dv3_inc_attn_step gives for that row alone
+ * with Ts = text_len[b], bit for bit. */
+int dv3_inc_attn_step_rows(const Dv3IncAttn* attn, const int* text_len, void* stream);
 int dv3_inc_advance(int* t_ptr, void* stream);
 
 #ifdef __cplusplus
