@@ -96,6 +96,7 @@ __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-
 //   FMT_BF16  gradients (magnitudes down to 1e-10: need the fp32 exponent range): 8 + 8 bits, products to ~2^-17.
 constexpr float LO_SCALE = 2048.f, LO_INV = 1.f / 2048.f;
 enum { FMT_BF16 = 2, FMT_F16 = 16 };
+typedef __nv_bfloat16 bf16;
 template <int FMT>
 __device__ __forceinline__ void split_pair(float v, uint16_t& hi, uint16_t& lo) {
     if (FMT == FMT_F16) {

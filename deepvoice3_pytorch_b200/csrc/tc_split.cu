@@ -1,13 +1,13 @@
-// Operand preparation for the tensor-core path (tc_gemm.cu): every fp32 operand x becomes a 16-bit (hi, lo * 2^11) pair
-// (common.cuh: fp16 pairs for forward operands, bf16 pairs for gradients), written in the (B,T,C) layout each implicit
-// GEMM consumes (K-major for the forward / data gradient, MN-major for the weight gradient).  These passes are pure HBM
-// streaming and absorb work the fp32 path
-// does inside its loaders: the conv-input dropout mask, the ReLU mask of the incoming gradient, the bias-gradient
-// reduction and the (B,C,T) <-> (B,T,C) layout change.  Channel pitches are padded to a multiple of 8 (16 bytes,
-// the TMA stride granularity); pad columns are never read (the tensor maps carry the true extent).
+// Activation and gradient operand preparation for the tensor-core path (tc_gemm.cu): every fp32 operand x becomes a
+// 16-bit (hi, lo * 2^11) pair (common.cuh: fp16 pairs for forward operands, bf16 pairs for gradients), written in the
+// (B,T,C) layout each implicit GEMM consumes (K-major for the forward / data gradient, MN-major for the weight
+// gradient).  The weight operands come from the weight norm (weightnorm.cu per layer, wn_batched.cu for all layers at
+// once).  These passes are pure HBM streaming and absorb work the fp32 path does inside its loaders: the conv-input
+// dropout mask, the ReLU mask of the incoming gradient, the bias-gradient reduction and the (B,C,T) <-> (B,T,C)
+// layout change.  Channel pitches are padded to a multiple of 8 (16 bytes, the TMA stride granularity); pad columns
+// are never read (the tensor maps carry the true extent).
 #include <cuda_bf16.h>
 #include "common.cuh"
-#include "wn_device.cuh"
 
 namespace dv3 {
 
@@ -144,26 +144,6 @@ __global__ void __launch_bounds__(256) plane_split_kernel(const __grid_constant_
     }
 }
 
-// weight-norm pack: v [R][X][k] fp32, scale[R] = g/||v|| -> two plane sets with element (r,x,j) at
-// r*s_r + x*s_x + j*s_j: outA is written with lanes along (x,j) (choose the set whose unit stride is s_x),
-// outB with lanes along r (unit stride s_r).
-template <int FMTA, int FMTB>
-__global__ void wn_pack_split_kernel(const float* __restrict__ v, const float* __restrict__ scale,
-                                     bf16* __restrict__ outA, long long a_r, long long a_x, long long a_j,
-                                     long long a_plane, bf16* __restrict__ outB, long long b_r, long long b_x,
-                                     long long b_j, long long b_plane, int R, int X, int k) {
-    pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
-    __shared__ float tile[32][33];
-    wn_pack_split_tile<FMTA, FMTB>(v, scale, outA, a_r, a_x, a_j, a_plane, outB, b_r, b_x, b_j, b_plane, R, X, k,
-                                   blockIdx.x, blockIdx.y, tile);
-}
-
-__global__ void wn_norm_kernel2(const float* __restrict__ v, const float* __restrict__ g,
-                                float* __restrict__ inv_norm, float* __restrict__ scale, int R, int L) {
-    pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
-    wn_norm_row(v, g, inv_norm, scale, R, L, (blockIdx.x * blockDim.x + threadIdx.x) >> 5, threadIdx.x & 31);
-}
-
 }  // namespace dv3
 
 using namespace dv3;
@@ -204,43 +184,6 @@ int dv3_tc_grad_split(const float* dy, const float* y, void* btc, void* bct, flo
     p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8; p.relu = relu;
     launch_k(plane_split_kernel<SPLIT_GRAD>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
     return check_launch("tc_grad_split");
-}
-
-// Weight norm + split for a conv weight v (Cout, Cin, k), g [Cout]:
-//   wfwd: [2][k][Cout][Cinp] fp16 planes (forward operand: rows co, K = ci)
-//   wbwd: [2][k][Cin][Coutp] bf16 planes (data-gradient operand, multiplied with bf16 gradient planes)
-int dv3_tc_weightnorm_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
-                          void* wbwd, int Cout, int Cin, int k, void* stream) {
-    DV3_REQUIRE(npl == 2, "tc_weightnorm_fwd: npl must be 2");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int L = Cin * k;
-    const long long Cinp = (Cin + 7) / 8 * 8, Coutp = (Cout + 7) / 8 * 8;
-    launch_k(wn_norm_kernel2, (Cout * 32 + 255) / 256, 256, 0, st, v, g, inv_norm, scale, Cout, L);
-    if (int e = check_launch("tc_weightnorm_fwd(norm)")) return e;
-    dim3 grid((L + 31) / 32, (Cout + 31) / 32);
-    launch_k(wn_pack_split_kernel<FMT_F16, FMT_BF16>, grid, dim3(32, 8), 0, st, v, scale, (bf16*)wfwd, Cinp, 1,
-             (long long)Cout * Cinp, (long long)k * Cout * Cinp, (bf16*)wbwd, 1, Coutp, (long long)Cin * Coutp,
-             (long long)k * Cin * Coutp, Cout, Cin, k);
-    return check_launch("tc_weightnorm_fwd(pack)");
-}
-
-// ConvTranspose1d(k=2,s=2) weight v (Cin, Cout, 2), g [Cin] (norm over dim 0 = Cin), run as a 1x1 conv with
-// 2*Cout output rows ordered (j, co):
-//   wfwd: [2][2*Cout][Cinp] fp16, rows (j,co), K = ci        wbwd: [2][Cin][K2p] bf16, rows ci, K = (j,co)
-int dv3_tc_weightnorm_convt_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
-                                void* wbwd, int Cin, int Cout, void* stream) {
-    DV3_REQUIRE(npl == 2, "tc_weightnorm_convt_fwd: npl must be 2");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int L = Cout * 2;
-    const long long Cinp = (Cin + 7) / 8 * 8, K2p = (2 * Cout + 7) / 8 * 8;
-    launch_k(wn_norm_kernel2, (Cin * 32 + 255) / 256, 256, 0, st, v, g, inv_norm, scale, Cin, L);
-    if (int e = check_launch("tc_weightnorm_convt_fwd(norm)")) return e;
-    dim3 grid((L + 31) / 32, (Cin + 31) / 32);
-    // r = ci, x = co, j: outA (lanes along (x,j)) = wbwd [ci][j*Cout+co] ; outB (lanes along r) = wfwd [(j*Cout+co)][ci]
-    launch_k(wn_pack_split_kernel<FMT_BF16, FMT_F16>, grid, dim3(32, 8), 0, st, v, scale, (bf16*)wbwd, K2p, 1,
-             (long long)Cout, (long long)Cin * K2p, (bf16*)wfwd, 1, Cinp, (long long)Cout * Cinp,
-             (long long)2 * Cout * Cinp, Cin, Cout, 2);
-    return check_launch("tc_weightnorm_convt_fwd(pack)");
 }
 
 }  // extern "C"

@@ -1,7 +1,7 @@
 // Weight norm for ALL weight-normed convolutions of the model in one launch per phase.
-// The per-layer kernels (wn_norm_kernel2 + wn_pack_split_kernel in the forward, wn_bwd_kernel in the backward) are
-// tiny: 127 launches per training step that together move ~0.5 GB but cost ~1.1 ms of GPU time because each one is
-// latency bound (6-14 us for a few hundred KB).  The weights do not depend on activations, so the training step
+// The per-layer kernels (weightnorm.cu: wn_norm_kernel + wn_pack_split_kernel in the forward, wn_bwd_kernel in the
+// backward) are tiny: 127 launches per training step that together move ~0.5 GB but cost ~1.1 ms of GPU time because
+// each one is latency bound (6-14 us for a few hundred KB).  The weights do not depend on activations, so the training step
 // prepares every layer's packed bf16 operand planes up front (norm, then pack: 2 launches) and folds every layer's
 // split-K reduction + g/v gradient into one launch after the backward pass.  A device-resident table of Dv3WnEntry
 // records (built once on the host) maps a block index to (layer, block-within-layer).
@@ -42,8 +42,8 @@ __global__ void __launch_bounds__(256) wn_pack_batched_kernel(const Dv3WnEntry* 
     const int lb = blockIdx.x - e.blk_pack;
     const int by = lb / e.pack_gx, bx = lb - by * e.pack_gx;
     const long long Cinp = (e.Cin + 7) / 8 * 8, Coutp = (e.Cout + 7) / 8 * 8;
-    wn_pack_split_tile<FMT_F16, FMT_BF16>(e.v, e.scale, (bf16*)e.wfwd, Cinp, 1, (long long)e.Cout * Cinp,
-                             (long long)e.k * e.Cout * Cinp, (bf16*)e.wbwd, 1, Coutp, (long long)e.Cin * Coutp,
+    wn_pack_split_tile<FMT_F16, FMT_BF16>(e.v, e.scale, e.wfwd, Cinp, 1, (long long)e.Cout * Cinp,
+                             (long long)e.k * e.Cout * Cinp, e.wbwd, 1, Coutp, (long long)e.Cin * Coutp,
                              (long long)e.k * e.Cin * Coutp, e.Cout, e.Cin, e.k, bx, by, tile);
 }
 

@@ -1,20 +1,25 @@
-// Device-side bodies of the weight-norm kernels, shared by the per-layer launches (weightnorm.cu, tc_split.cu) and
-// the batched "all layers in one launch" variants (wn_batched.cu).
+// Device-side bodies of the weight-norm kernels, shared by the per-layer launches (weightnorm.cu) and the batched
+// "all layers in one launch" variants (wn_batched.cu).
 #pragma once
 #include <cuda_bf16.h>
 #include "common.cuh"
 
 namespace dv3 {
 
-typedef __nv_bfloat16 bf16;
+// Output formats of the weight-norm pack: the (hi, lo) pairs of common.cuh (FMT_F16 forward operands, FMT_BF16
+// gradients) or FMT_F32, w itself in one fp32 plane (the operands of the exact-fp32 kernels).
+enum { FMT_F32 = 32 };
 
-// x -> (hi, lo) planes in format FMT (common.cuh: FMT_F16 forward operands, FMT_BF16 gradients)
 template <int FMT>
-__device__ __forceinline__ void split_store(float v, bf16* __restrict__ base, size_t idx, size_t plane_stride) {
-    uint16_t h, l;
-    split_pair<FMT>(v, h, l);
-    reinterpret_cast<uint16_t*>(base)[idx] = h;
-    reinterpret_cast<uint16_t*>(base)[plane_stride + idx] = l;
+__device__ __forceinline__ void split_store(float v, void* __restrict__ base, size_t idx, size_t plane_stride) {
+    if constexpr (FMT == FMT_F32) {
+        static_cast<float*>(base)[idx] = v;
+    } else {
+        uint16_t h, l;
+        split_pair<FMT>(v, h, l);
+        static_cast<uint16_t*>(base)[idx] = h;
+        static_cast<uint16_t*>(base)[plane_stride + idx] = l;
+    }
 }
 
 // one warp per row r: inv_norm[r] = 1/||v[r,:]||, scale[r] = g[r]*inv_norm[r]
@@ -29,13 +34,14 @@ __device__ __forceinline__ void wn_norm_row(const float* __restrict__ v, const f
     if (lane == 0) { const float inv = 1.f / sqrtf(s); inv_norm[r] = inv; scale[r] = g[r] * inv; }
 }
 
-// weight-norm pack of one 32(r) x 32(e) tile, block (32, 8): v [R][X][k] fp32, scale[R] = g/||v|| -> two plane sets
-// with element (r,x,j) at r*s_r + x*s_x + j*s_j: outA is written with lanes along (x,j) (choose the set whose unit
-// stride is s_x), outB with lanes along r (unit stride s_r).
-template <int NPLA, int NPLB>
+// weight-norm pack of one 32(r) x 32(e) tile, block (32, 8): v [R][X][k] fp32, scale[R] = g/||v|| -> w = v * scale
+// in two plane sets of format FMTA / FMTB with element (r,x,j) at r*s_r + x*s_x + j*s_j (either set may be null; the
+// plane stride is unused for FMT_F32): outA is written with lanes along (x,j) (choose the set whose unit stride is
+// s_x), outB with lanes along r (unit stride s_r).
+template <int FMTA, int FMTB>
 __device__ __forceinline__ void wn_pack_split_tile(const float* __restrict__ v, const float* __restrict__ scale,
-                                                   bf16* __restrict__ outA, long long a_r, long long a_x,
-                                                   long long a_j, long long a_plane, bf16* __restrict__ outB,
+                                                   void* __restrict__ outA, long long a_r, long long a_x,
+                                                   long long a_j, long long a_plane, void* __restrict__ outB,
                                                    long long b_r, long long b_x, long long b_j, long long b_plane,
                                                    int R, int X, int k, int bx, int by, float (*tile)[33]) {
     const int L = X * k;
@@ -47,7 +53,7 @@ __device__ __forceinline__ void wn_pack_split_tile(const float* __restrict__ v, 
         if (r < R && e < L) {
             w = v[(size_t)r * L + e] * scale[r];
             const int xx = e / k, j = e - xx * k;
-            if (outA) split_store<NPLA>(w, outA, (size_t)(r * a_r + xx * a_x + j * a_j), (size_t)a_plane);
+            if (outA) split_store<FMTA>(w, outA, (size_t)(r * a_r + xx * a_x + j * a_j), (size_t)a_plane);
         }
         tile[threadIdx.y + 8 * i][threadIdx.x] = w;
     }
@@ -58,7 +64,7 @@ __device__ __forceinline__ void wn_pack_split_tile(const float* __restrict__ v, 
             const int e = e0 + threadIdx.y + 8 * i, r = r0 + threadIdx.x;
             if (r < R && e < L) {
                 const int xx = e / k, j = e - xx * k;
-                split_store<NPLB>(tile[threadIdx.x][threadIdx.y + 8 * i], outB,
+                split_store<FMTB>(tile[threadIdx.x][threadIdx.y + 8 * i], outB,
                                   (size_t)(r * b_r + xx * b_x + j * b_j), (size_t)b_plane);
             }
         }

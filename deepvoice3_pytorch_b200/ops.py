@@ -180,13 +180,10 @@ def grad_boundary(x, tag):
 weight_bank = None
 
 
-def _bank_weights(v, g):
-    return weight_bank.weights_for(v, g) if weight_bank is not None else None
-
-
 def _sink(*params):
-    """The .grad buffers to accumulate into, or None when the sink is off / not every buffer exists."""
-    if not grad_sink or any(p.grad is None or not p.grad.is_contiguous() for p in params):
+    """The .grad buffers to accumulate into, or None when the sink is off / a parameter is not a leaf (e.g. the views
+    ``linear`` passes) / not every buffer exists."""
+    if not grad_sink or any(not p.is_leaf or p.grad is None or not p.grad.is_contiguous() for p in params):
         return None
     return [p.grad for p in params]
 
@@ -194,15 +191,9 @@ def _sink(*params):
 def _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=0, out=None, accumulate=False):
     """tap_major_k = 0: partials in v's layout; = k (> 0): partials as [j][R][X] (tensor-core weight gradient)."""
     dv, dg = out if out is not None else (torch.empty_like(v), torch.empty_like(g))
-    R = v.shape[0]
-    if tap_major_k:
-        X = v.numel() // R // tap_major_k
-        lib.call("dv3_weightnorm_bwd", _p(partials), v.numel(), nsplit, 1, _p(v), _p(g), _p(inv), _p(dv), _p(dg), R, X,
-                 tap_major_k, int(accumulate), _stream())
-    else:
-        X = v.numel() // R
-        lib.call("dv3_weightnorm_bwd", _p(partials), v.numel(), nsplit, 0, _p(v), _p(g), _p(inv), _p(dv), _p(dg), R, X,
-                 1, int(accumulate), _stream())
+    R, k = v.shape[0], tap_major_k or 1
+    lib.call("dv3_weightnorm_bwd", _p(partials), v.numel(), nsplit, int(tap_major_k > 0), _p(v), _p(g), _p(inv),
+             _p(dv), _p(dg), R, v.numel() // R // k, k, int(accumulate), _stream())
     return dv, dg
 
 
@@ -221,6 +212,14 @@ def _wgrad_conv(dab, x, v_shape, k, dilation, causal, p, seed_ptr, salt):
 # ----------------------------------------------------------------------------------------------
 # fused ConvBlock (Conv1dGLU / HighwayConv1d)
 # ----------------------------------------------------------------------------------------------
+def _gate_addend(mode, residual, dy, s):
+    """(addmode, e1, e2, alpha) of a gated block's data-gradient GEMM: the gradient that reaches x around the conv --
+    sqrt(0.5) * dy through the GLU residual, dy * (1 - s) through the highway carry gate, nothing for a plain GLU."""
+    if mode == MODE_GLU:
+        return (1, dy, None, 0.7071067811865476) if residual else (0, None, None, 0.0)
+    return 2, dy, s, 0.0
+
+
 class _ConvBlockFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training):
@@ -256,10 +255,7 @@ class _ConvBlockFn(torch.autograd.Function):
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
-            if mode == MODE_GLU:
-                addmode, e1, e2, alpha = (1, dy, None, 0.7071067811865476) if residual else (0, None, None, 0.0)
-            else:
-                addmode, e1, e2, alpha = 2, dy, s, 0.0
+            addmode, e1, e2, alpha = _gate_addend(mode, residual, dy, s)
             lib.call("dv3_conv1d_dgrad", _p(dab), _p(w_b), _p(dx), B, 2 * C, C, T, k, dilation,
                      int(causal), p, seed_ptr, salt, addmode, _p(e1), _p(e2), alpha, _stream())
         dv = dg = None
@@ -309,6 +305,70 @@ def _pad8(n):
     return (n + 7) // 8 * 8
 
 
+def _tc_weights(v, g):
+    """Tensor-core weight operands of a conv v (Cout, Cin, k) -> (inv, wfwd, wbwd, bank record or None, side or None):
+    wfwd [2][k][Cout][pad8(Cin)] fp16 pair (forward GEMM), wbwd [2][k][Cin][pad8(Cout)] bf16 pair (data gradient).
+    Without a weight-bank record the per-layer weight norm is started on the side stream -- it depends only on the
+    parameters, so it overlaps the caller's activation split; the caller joins ``side`` before its GEMM."""
+    bank = weight_bank.weights_for(v, g) if weight_bank is not None else None   # planes prepared for this step?
+    if bank is not None:
+        return bank.inv, bank.wfwd, bank.wbwd, bank, None
+    Cout, Cin, k = v.shape
+    dev = v.device
+    inv = torch.empty(Cout, device=dev)
+    scale = torch.empty_like(inv)
+    wfwd = torch.empty(2, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16)
+    wbwd = torch.empty(2, k, Cin, _pad8(Cout), device=dev, dtype=torch.bfloat16)
+    side = _SideStream(dev)
+    side.keep = scale                 # written and read on the side stream: must outlive the caller's join
+    with side:
+        lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), 2, _p(wbwd), Cout, Cin, k,
+                 _stream())
+    return inv, wfwd, wbwd, bank, side
+
+
+class _TCWeightGrad:
+    """Weight and bias gradients of a weight-normed tensor-core conv v (M, N, k), bias [M]: ``dbias`` is where the
+    gradient split sums the bias gradient; start() runs the weight-gradient GEMM and the weight-norm backward on the
+    side stream, finish() joins it after the data gradient.  With the gradient sink they are accumulated into .grad (a
+    weight-bank layer's reduction deferred to WeightBank.end_backward()) and finish() returns None for them."""
+
+    def __init__(self, ctx, v, g):
+        self.ctx, self.v, self.g = ctx, v, g
+        self.sink = _sink(v, g, ctx.bias_param) if ctx.bias_param is not None else None
+        self.dbias = self.sink[2] if self.sink else torch.zeros(v.shape[0], device=v.device)
+        self.side = self.dv = self.dg = self.partials = None
+
+    def start(self, d_planes, x_wg, inv, B, T, dilation, causal):
+        ctx, v, g, sink = self.ctx, self.v, self.g, self.sink
+        if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
+            return
+        M, N, k = v.shape
+        nsplit = lib.raw("dv3_tc_wgrad_nsplit")(B, M, N, T, k)
+        numel = v.numel()
+        # allocated on the main stream (and held until finish()), computed on the side stream
+        partials = weight_bank.partials_for(ctx.bank, nsplit, numel) if (sink and ctx.bank is not None) else None
+        deferred = partials is not None
+        if not deferred:
+            partials = torch.empty(nsplit, numel, device=v.device)
+        self.partials = partials
+        self.dv, self.dg = (sink[0], sink[1]) if sink else (torch.empty_like(v), torch.empty_like(g))
+        self.side = _SideStream(v.device)
+        with self.side:
+            # partials [split][j][M][N]: contiguous float4 stores from the GEMM epilogue
+            lib.call("dv3_tc_wgrad_mn", _p(d_planes), _p(x_wg), _p(partials), numel, B, M, N, T, k, dilation,
+                     int(causal), M, N, 0, 1, M * N, _stream())
+            if not deferred:
+                _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=k, out=(self.dv, self.dg), accumulate=bool(sink))
+
+    def finish(self):
+        if self.side is not None:
+            self.side.join()
+        if self.sink:                 # already accumulated into the .grad arena views
+            return None, None, None
+        return self.dv, self.dg, self.dbias
+
+
 class _ConvBlockTCFn(torch.autograd.Function):
     """Same contract as _ConvBlockFn on the tensor-core path: operands are 16-bit hi/lo planes (fp16 pairs in the
     forward GEMM, bf16 pairs in the gradient GEMMs)."""
@@ -320,27 +380,14 @@ class _ConvBlockTCFn(torch.autograd.Function):
         dev = x.device
         bf = torch.bfloat16
         need_bwd = any(ctx.needs_input_grad)
-        bank = _bank_weights(v, g)        # operand planes already prepared for the whole model this step?
-        if bank is not None:
-            inv, wfwd, wbwd = bank.inv, bank.wfwd, bank.wbwd
-        else:
-            inv = torch.empty(2 * C, device=dev)
-            scale = torch.empty_like(inv)
-            wfwd = torch.empty(2, k, 2 * C, C, device=dev, dtype=torch.float16)
-            wbwd = torch.empty(2, k, C, 2 * C, device=dev, dtype=bf)
         p, seed_t, salt = _drop_args(p_drop, training, dev)
+        inv, wfwd, wbwd, bank, side = _tc_weights(v, g)
         x_btc = torch.empty(2, B, T, C, device=dev, dtype=torch.float16)        # forward operand (fp16 pair)
         x_wg = torch.empty(2, B, T, C, device=dev, dtype=bf) if need_bwd else None  # weight-gradient operand
         seed_ptr = _p(seed_t)
         y = torch.empty_like(x)
         a = torch.empty_like(x) if need_bwd else None
         s = torch.empty_like(x) if need_bwd else None
-        side = None
-        if bank is None:
-            side = _SideStream(dev)
-            with side:                    # weight norm + split depends only on the parameters: overlap it with
-                lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), 2, _p(wbwd), 2 * C, C,
-                         k, _stream())    # the activation split below
         lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, C, T, k, dilation, int(causal), p,
                  seed_ptr, salt, _stream())
         if side is not None:
@@ -362,45 +409,18 @@ class _ConvBlockTCFn(torch.autograd.Function):
         seed_ptr = _p(ctx.seed_t)          # the forward's own seed snapshot
         dy = _c(dy)
         B, C, T = x.shape
-        bf = torch.bfloat16
-        sink = _sink(v, g, ctx.bias_param) if ctx.bias_param is not None else None
-        d_btc = torch.empty(2, B, T, 2 * C, device=dev, dtype=bf)
-        dbias = sink[2] if sink else torch.zeros(2 * C, device=dev)
-        lib.call("dv3_tc_gate_bwd_split", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(dbias), B, C, T,
+        d_btc = torch.empty(2, B, T, 2 * C, device=dev, dtype=torch.bfloat16)
+        wg = _TCWeightGrad(ctx, v, g)
+        lib.call("dv3_tc_gate_bwd_split", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(wg.dbias), B, C, T,
                  mode, int(residual), _stream())
-        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
-        dv = dg = partials = None
-        if need_w:                                   # allocate on the main stream, compute on the side stream
-            nsplit = lib.raw("dv3_tc_wgrad_nsplit")(B, 2 * C, C, T, k)
-            numel = v.numel()
-            # with the weight bank the split-K partials go to the layer's persistent buffer and the weight-norm
-            # backward of ALL layers runs as one launch after loss.backward() (WeightBank.end_backward)
-            partials = weight_bank.partials_for(ctx.bank, nsplit, numel) if (sink and ctx.bank is not None) else None
-            deferred = partials is not None
-            if not deferred:
-                partials = torch.empty(nsplit, numel, device=dev)
-            dv, dg = (sink[0], sink[1]) if sink else (torch.empty_like(v), torch.empty_like(g))
-        side = _SideStream(dev)
-        if need_w:
-            with side:
-                # partials [split][j][2C][C]: contiguous float4 stores from the GEMM epilogue
-                lib.call("dv3_tc_wgrad_mn", _p(d_btc), _p(x_wg), _p(partials), numel, B, 2 * C, C, T, k, dilation,
-                         int(causal), 2 * C, C, 0, 1, 2 * C * C, _stream())
-                if not deferred:
-                    _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=k, out=(dv, dg), accumulate=bool(sink))
+        wg.start(d_btc, x_wg, inv, B, T, dilation, causal)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
-            if mode == MODE_GLU:
-                addmode, e1, e2, alpha = (1, dy, None, 0.7071067811865476) if residual else (0, None, None, 0.0)
-            else:
-                addmode, e1, e2, alpha = 2, dy, s, 0.0
+            addmode, e1, e2, alpha = _gate_addend(mode, residual, dy, s)
             lib.call("dv3_tc_conv", _p(d_btc), _p(wbwd), 2, _p(dx), B, 2 * C, C, T, k, dilation, int(causal), 1,
                      None, 0, p, seed_ptr, salt, addmode, _p(e1), _p(e2), alpha, None, _stream())
-        if need_w:
-            side.join()
-        if sink:                                     # already accumulated into the .grad arena views
-            dv = dg = dbias = None
+        dv, dg, dbias = wg.finish()
         dspk = None
         if has_spk and ctx.needs_input_grad[4]:     # d_a = hi + lo * 2^-11 of the (B,T,2C) planes, back to (B,C,T)
             dspk = transpose12((d_btc[0, :, :, :C].float() + d_btc[1, :, :, :C].float() * (1.0 / 2048.0)).contiguous())
@@ -417,25 +437,12 @@ class _Conv1dTCFn(torch.autograd.Function):
         Cout = v.shape[0]
         dev, bf = x.device, torch.bfloat16
         need_bwd = any(ctx.needs_input_grad)
-        Cinp, Coutp = _pad8(Cin), _pad8(Cout)
-        bank = _bank_weights(v, g)
-        if bank is not None:
-            inv, wfwd, wbwd = bank.inv, bank.wfwd, bank.wbwd
-        else:
-            inv = torch.empty(Cout, device=dev)
-            scale = torch.empty_like(inv)
-            wfwd = torch.empty(2, k, Cout, Cinp, device=dev, dtype=torch.float16)
-            wbwd = torch.empty(2, k, Cin, Coutp, device=dev, dtype=bf)
+        Cinp = _pad8(Cin)
+        inv, wfwd, wbwd, bank, side = _tc_weights(v, g)
         need_w = need_bwd and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
         x_btc = torch.empty(2, B, T, Cinp, device=dev, dtype=torch.float16)
         x_wg = torch.empty(2, B, T, Cinp, device=dev, dtype=bf) if need_w else None
         y = torch.empty(B, Cout, T, device=dev)
-        side = None
-        if bank is None:
-            side = _SideStream(dev)
-            with side:
-                lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), 2, _p(wbwd), Cout, Cin,
-                         k, _stream())
         lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, k, dilation, int(causal), 0.0,
                  None, 0, _stream())
         if side is not None:
@@ -454,38 +461,17 @@ class _Conv1dTCFn(torch.autograd.Function):
         v, g, x_wg, wbwd, inv, y = ctx.saved_tensors
         B, Cin, Cout, T, k, dilation, causal, relu = ctx.cfg
         dy = _c(dy)
-        dev, bf = dy.device, torch.bfloat16
-        Coutp = _pad8(Cout)
-        need_x = ctx.needs_input_grad[0]
-        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
-        sink = _sink(v, g, ctx.bias_param) if (ctx.bias_param is not None and v.is_leaf and g.is_leaf) else None
-        g_btc = torch.empty(2, B, T, Coutp, device=dev, dtype=bf)
-        dbias = sink[2] if sink else torch.zeros(Cout, device=dev)
-        lib.call("dv3_tc_grad_split", _p(dy), _p(y), _p(g_btc), None, _p(dbias), B, Cout, T, int(relu), _stream())
-        dv = dg = None
-        side = _SideStream(dev)
-        if need_w:
-            nsplit = lib.raw("dv3_tc_wgrad_nsplit")(B, Cout, Cin, T, k)
-            numel = v.numel()
-            partials = weight_bank.partials_for(ctx.bank, nsplit, numel) if (sink and ctx.bank is not None) else None
-            deferred = partials is not None
-            if not deferred:
-                partials = torch.empty(nsplit, numel, device=dev)
-            dv, dg = (sink[0], sink[1]) if sink else (torch.empty_like(v), torch.empty_like(g))
-            with side:
-                lib.call("dv3_tc_wgrad_mn", _p(g_btc), _p(x_wg), _p(partials), numel, B, Cout, Cin, T, k, dilation,
-                         int(causal), Cout, Cin, 0, 1, Cout * Cin, _stream())
-                if not deferred:
-                    _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=k, out=(dv, dg), accumulate=bool(sink))
+        dev = dy.device
+        g_btc = torch.empty(2, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
+        wg = _TCWeightGrad(ctx, v, g)
+        lib.call("dv3_tc_grad_split", _p(dy), _p(y), _p(g_btc), None, _p(wg.dbias), B, Cout, T, int(relu), _stream())
+        wg.start(g_btc, x_wg, inv, B, T, dilation, causal)
         dx = None
-        if need_x:
+        if ctx.needs_input_grad[0]:
             dx = torch.empty(B, Cin, T, device=dev)
             lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), 2, _p(dx), B, Cout, Cin, T, k, dilation, int(causal), 1, None,
                      0, 0.0, None, 0, 0, None, None, 0.0, None, _stream())
-        if need_w:
-            side.join()
-        if sink:
-            dv = dg = dbias = None
+        dv, dg, dbias = wg.finish()
         return (dx, dv, dg, dbias) + (None,) * 4
 
 
@@ -549,6 +535,15 @@ class _ConvT2TCFn(torch.autograd.Function):
         return dx, dv, dg, dbias
 
 
+def _tc_selected():
+    """Whether conv_math selects the tensor-core kernels; an unknown value raises."""
+    if conv_math in ("tc", "bf16x3"):
+        return True
+    if conv_math != "fp32":
+        raise Dv3Error("unknown conv_math %r" % (conv_math,))
+    return False
+
+
 # 16 keeps the 16-wide speaker projections of the multi-speaker model on tensor cores (measured: vctk step 11.8 -> 10.6 ms)
 TC_MIN_CHANNELS = int(os.environ.get("DV3_TC_MIN_CHANNELS", "16"))
 
@@ -556,7 +551,7 @@ TC_MIN_CHANNELS = int(os.environ.get("DV3_TC_MIN_CHANNELS", "16"))
 def _use_tc_conv(x, Cin, Cout, k):
     """Tensor cores for plain convs when the mode asks for it, the shape is supported and the GEMM is big enough to
     amortise the operand-split passes."""
-    if conv_math not in ("tc", "bf16x3") or not x.is_cuda:
+    if not _tc_selected() or not x.is_cuda:
         return False
     B, _, T = x.shape
     if not lib.raw("dv3_tc_conv_supported")(B, Cin, Cout, T, int(k)):
@@ -574,11 +569,9 @@ def convblock(x, v, g, bias, spk=None, k=3, dilation=1, causal=False, mode=MODE_
               p_drop=0.0, training=False):
     """Fused weight-normed dilated conv + gate.  x (B,C,T); v (2C,C,k); g (2C,1,1); bias (2C);
     spk (B,C,T) already softsign'ed (or None)."""
-    if conv_math in ("tc", "bf16x3") and x.is_cuda and tc_supported(x.shape[0], x.shape[1], x.shape[2], int(k)):
+    if _tc_selected() and x.is_cuda and tc_supported(x.shape[0], x.shape[1], x.shape[2], int(k)):
         return _ConvBlockTCFn.apply(_c(x), v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
                                     bool(causal), int(mode), bool(residual), float(p_drop), bool(training))
-    if conv_math not in ("fp32", "bf16x3", "tc"):
-        raise Dv3Error("unknown conv_math %r" % (conv_math,))
     return _ConvBlockFn.apply(_c(x), v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
                               bool(causal), int(mode), bool(residual), float(p_drop), bool(training))
 
@@ -993,7 +986,7 @@ def attention_core(q, k, v, mask=None, p_drop=0.0, training=False):
     if mask is not None:
         mask = mask.to(torch.uint8).contiguous()
     B, E, Td = q.shape
-    tc = (conv_math in ("tc", "bf16x3") and tc_attention and q.is_cuda and
+    tc = (_tc_selected() and tc_attention and q.is_cuda and
           lib.raw("dv3_tc_attn_supported")(B, E, Td, k.shape[2]))
     fn = _AttentionTCFn if tc else _AttentionCoreFn
     return fn.apply(_c(q), _c(k), _c(v), mask, float(p_drop), bool(training))
