@@ -3,8 +3,13 @@
 Everything is a pure function of a reference-keyed ``state_dict`` (old-style weight-norm keys
 ``*.weight_g`` / ``*.weight_v``), a spec from ``oracle/specs.py`` and the inputs; gradients come from
 torch autograd on CPU.  Works in fp32 (the parity target) or fp64 (error yardstick).
-Dropout is NOT restated: parity runs use dropout=0 exactly as the reference's own incremental
-tests do with ``.eval()`` (reference tests/test_deepvoice3.py:184-235).
+Dropout is not drawn here: parity runs use dropout=0 exactly as the reference's own incremental
+tests do with ``.eval()`` (reference tests/test_deepvoice3.py:184-235).  ``conv1d_glu``,
+``highway_conv1d`` and ``attention_core`` take an optional explicit multiplicative mask ``drop``
+(0 or 1/(1-p) per element, e.g. ``oracle/dropout_mask.py``'s restatement of the device mask) at the
+reference's dropout site: the conv input only (the residual / highway carry stay unmasked), and
+the attention probabilities after they are returned, before P.V.  ``drop=None`` is the
+dropout-free forward, unchanged.
 
 PARITY: pinned.  ``tests/golden/make_golden.py`` runs the live reference modules
 (/root/reference/deepvoice3_pytorch, importable in the build container) and stores their outputs;
@@ -53,9 +58,9 @@ def conv_transpose1d(sd, prefix, x):
     return F.conv_transpose1d(x, _w(sd, prefix), sd[prefix + ".bias"], stride=2)
 
 
-def conv1d_glu(sd, prefix, x, k, dilation, causal, residual, speaker_embed_btc=None):
-    """reference modules.py:145-164 (dropout omitted)."""
-    y = conv1d(sd, prefix + ".conv", x, k, dilation, causal)
+def conv1d_glu(sd, prefix, x, k, dilation, causal, residual, speaker_embed_btc=None, drop=None):
+    """reference modules.py:145-164; ``drop`` (B,C,T) multiplies the conv input only (modules.py:147)."""
+    y = conv1d(sd, prefix + ".conv", x if drop is None else x * drop, k, dilation, causal)
     a, b = y.split(y.size(1) // 2, dim=1)
     if (prefix + ".speaker_proj.weight_v") in sd:
         a = a + F.softsign(linear(sd, prefix + ".speaker_proj", speaker_embed_btc)).transpose(1, 2)
@@ -63,9 +68,10 @@ def conv1d_glu(sd, prefix, x, k, dilation, causal, residual, speaker_embed_btc=N
     return (y + x) * SQRT_HALF if residual else y
 
 
-def highway_conv1d(sd, prefix, x, k, dilation, causal):
-    """reference modules.py:200-226, glu=False branch (the only one the builders use)."""
-    y = conv1d(sd, prefix + ".conv", x, k, dilation, causal)
+def highway_conv1d(sd, prefix, x, k, dilation, causal, drop=None):
+    """reference modules.py:200-226, glu=False branch (the only one the builders use); ``drop`` (B,C,T)
+    multiplies the conv input only (modules.py:214), the carry (1 - t) * x takes x unmasked."""
+    y = conv1d(sd, prefix + ".conv", x if drop is None else x * drop, k, dilation, causal)
     a, b = y.split(y.size(1) // 2, dim=1)
     t = torch.sigmoid(b)
     return t * a + (1 - t) * x
@@ -107,6 +113,19 @@ def memory_mask(lengths, max_len=None):
     return ~(torch.arange(max_len)[None, :] < lengths[:, None])
 
 
+def attention_core(query, keys_bct, values, mask=None, drop=None):
+    """reference deepvoice3.py:142-171 between the projections: query (B,Td,E); keys_bct (B,E,Ts);
+    values (B,Ts,E); mask (B,Ts) bool, True = padding; drop (B,Td,Ts) multiplies the probabilities
+    after they are returned and before P.V (deepvoice3.py:161-165).  -> (context (B,Td,E), probs)."""
+    x = torch.bmm(query, keys_bct)  # no 1/sqrt(d)
+    if mask is not None:
+        x = x.masked_fill(mask[:, None, :], -float("inf"))
+    probs = F.softmax(x, dim=-1)
+    x = torch.bmm(probs if drop is None else probs * drop, values)
+    s = values.size(1)
+    return x * (s * math.sqrt(1.0 / s)), probs
+
+
 def attention_layer(sd, prefix, query, keys_bct, values, mask=None):
     """reference deepvoice3.py:132-176 (training path; no window, dropout omitted).
     query (B,Td,C); keys_bct (B,E,Ts) pre-transposed; values (B,Ts,E); mask (B,Ts) bool."""
@@ -115,13 +134,7 @@ def attention_layer(sd, prefix, query, keys_bct, values, mask=None):
         values = linear(sd, prefix + ".value_projection", values)
     if (prefix + ".key_projection.weight_v") in sd:
         keys_bct = linear(sd, prefix + ".key_projection", keys_bct.transpose(1, 2)).transpose(1, 2)
-    x = torch.bmm(linear(sd, prefix + ".query_projection", query), keys_bct)  # no 1/sqrt(d)
-    if mask is not None:
-        x = x.masked_fill(mask[:, None, :], -float("inf"))
-    probs = F.softmax(x, dim=-1)
-    x = torch.bmm(probs, values)
-    s = values.size(1)
-    x = x * (s * math.sqrt(1.0 / s))
+    x, probs = attention_core(linear(sd, prefix + ".query_projection", query), keys_bct, values, mask)
     x = linear(sd, prefix + ".out_projection", x)
     return (x + residual) * SQRT_HALF, probs
 
