@@ -47,12 +47,13 @@ class Conv1d(_WeightNormed):
         b = init_bias if init_bias is not None else torch.zeros(out_channels)
         self._set_params(w, b)
 
-    def forward(self, x, relu=False, causal=None):
+    def forward(self, x, relu=False, causal=None, extent=None):
         """causal=None: treat causal padding like the reference does (output length T + (k-1)d is not
-        produced; callers of the causal form always trim to T, which is what the kernel computes)."""
+        produced; callers of the causal form always trim to T, which is what the kernel computes).
+        extent: ``ops.extent_frames(x)`` inside a bucketed training batch."""
         causal = self.causal_padding if causal is None else causal
         return ops.conv1d(x, self.weight_v, self.weight_g, self.bias, self.kernel_size[0], self.dilation[0],
-                          causal=causal, relu=relu)
+                          causal=causal, relu=relu, extent=extent)
 
     def incremental_forward(self, input):
         """input (B, T, Cin): the newest frame input[:, -1] enters the ring buffer of the last (k-1)*dilation+1
@@ -89,8 +90,8 @@ class ConvTranspose1d(_WeightNormed):
         b = init_bias if init_bias is not None else torch.zeros(out_channels)
         self._set_params(w, b)
 
-    def forward(self, x):
-        return ops.conv_transpose1d_k2s2(x, self.weight_v, self.weight_g, self.bias)
+    def forward(self, x, extent=None):
+        return ops.conv_transpose1d_k2s2(x, self.weight_v, self.weight_g, self.bias, extent=extent)
 
 
 class WNLinear(_WeightNormed):

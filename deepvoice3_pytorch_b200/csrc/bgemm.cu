@@ -16,6 +16,7 @@ struct BgemmParams {
     int M, N, K, ldc;
     float alpha;
     int accumulate;
+    const long long* alpha_ts;   // non-null: alpha = context_scale(*alpha_ts), read from device memory
 };
 
 template <bool A_KMAJOR, bool B_KMAJOR>
@@ -59,6 +60,7 @@ struct BgemmPolicy {
     __device__ static void epilogue(const Params& p, const Acc<BN>& acc, int m_tile, int n_tile, int z, int tx,
                                     int ty) {
         float* C = p.C + (size_t)z * p.sCb;
+        const float alpha = p.alpha_ts ? context_scale(*p.alpha_ts) : p.alpha;
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
             const int m = m_tile * GEMM_BM + (i < 4 ? ty * 4 + i : 64 + ty * 4 + (i - 4));
@@ -68,7 +70,7 @@ struct BgemmPolicy {
                 const int n = n_tile * BN + (q >> 2) * 64 + tx * 4 + (q & 3);
                 if (n >= p.N) continue;
                 float* dst = &C[(size_t)m * p.ldc + n];
-                const float v = p.alpha * acc.v[i][q];
+                const float v = alpha * acc.v[i][q];
                 *dst = p.accumulate ? (*dst + v) : v;
             }
         }
@@ -93,17 +95,32 @@ static int launch_bgemm(const BgemmParams& p, int batch, cudaStream_t st) {
 
 using namespace dv3;
 
-extern "C" int dv3_bgemm(const float* A, long long sAb, long long sAm, long long sAk, const float* B,
-                         long long sBb, long long sBk, long long sBn, float* C, long long sCb, int ldc,
-                         int batch, int M, int N, int K, float alpha, int accumulate, void* stream) {
+static int bgemm(const float* A, long long sAb, long long sAm, long long sAk, const float* B, long long sBb,
+                 long long sBk, long long sBn, float* C, long long sCb, int ldc, int batch, int M, int N, int K,
+                 float alpha, const long long* alpha_ts, int accumulate, void* stream) {
     DV3_REQUIRE(batch >= 1 && batch <= 65535, "bgemm: batch %d out of range", batch);
     DV3_REQUIRE(sAm == 1 || sAk == 1, "bgemm: A needs unit stride along M or K");
     DV3_REQUIRE(sBn == 1 || sBk == 1, "bgemm: B needs unit stride along N or K");
-    BgemmParams p = {A, B, C, sAb, sAm, sAk, sBb, sBk, sBn, sCb, M, N, K, ldc, alpha, accumulate};
+    BgemmParams p = {A, B, C, sAb, sAm, sAk, sBb, sBk, sBn, sCb, M, N, K, ldc, alpha, accumulate, alpha_ts};
     cudaStream_t st = (cudaStream_t)stream;
     const bool ak = (sAm != 1), bk = (sBn != 1);
     if (ak && bk) return launch_bgemm<true, true>(p, batch, st);
     if (ak) return launch_bgemm<true, false>(p, batch, st);
     if (bk) return launch_bgemm<false, true>(p, batch, st);
     return launch_bgemm<false, false>(p, batch, st);
+}
+
+extern "C" int dv3_bgemm(const float* A, long long sAb, long long sAm, long long sAk, const float* B,
+                         long long sBb, long long sBk, long long sBn, float* C, long long sCb, int ldc,
+                         int batch, int M, int N, int K, float alpha, int accumulate, void* stream) {
+    return bgemm(A, sAb, sAm, sAk, B, sBb, sBk, sBn, C, sCb, ldc, batch, M, N, K, alpha, nullptr, accumulate, stream);
+}
+
+// alpha = Ts*sqrt(1/Ts) (the attention context scale) of a key count read from device memory
+extern "C" int dv3_bgemm_ctx_scale(const float* A, long long sAb, long long sAm, long long sAk, const float* B,
+                                   long long sBb, long long sBk, long long sBn, float* C, long long sCb, int ldc,
+                                   int batch, int M, int N, int K, const long long* ts_log, int accumulate,
+                                   void* stream) {
+    DV3_REQUIRE(ts_log != nullptr, "bgemm_ctx_scale: ts_log is NULL");
+    return bgemm(A, sAb, sAm, sAk, B, sBb, sBk, sBn, C, sCb, ldc, batch, M, N, K, 0.f, ts_log, accumulate, stream);
 }

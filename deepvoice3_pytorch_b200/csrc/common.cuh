@@ -50,6 +50,13 @@ static inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 
+// ---- attention context scale Ts * sqrt(1/Ts) (reference deepvoice3.py:170-171) of a key count read from device memory:
+// a batch padded to a larger bucket scales by its logical text length, not by the padded one -------------------------
+__device__ __forceinline__ float context_scale(long long ts) {
+    const double t = (double)(ts < 1 ? 1 : ts);
+    return (float)(t * sqrt(1.0 / t));
+}
+
 // ---- counter-based dropout mask ----------------------------------------------------------------
 // keep(idx) is a pure function of (step seed in device memory, call-site salt, element index), so the
 // backward pass and the weight-gradient pass regenerate exactly the mask the forward used, and a

@@ -211,15 +211,16 @@ __global__ void interleave2_kernel(const float* __restrict__ in, float* __restri
     }
 }
 
-// y = x with y[b,:,t] = 0 for t >= mult*lengths[b]   (B,C,T); x == y allowed
-__global__ void mask_time_kernel(const float* x, float* y, const long long* __restrict__ lengths, int mult, int C,
-                                 int T, long long total) {
+// y = x with y[b,:,t] = 0 for t >= mult*lengths[b * len_stride]   (B,C,T); x == y allowed.  len_stride 0: one length
+// for every row (the logical extent of a batch padded to a bucket).
+__global__ void mask_time_kernel(const float* x, float* y, const long long* __restrict__ lengths, int len_stride,
+                                 int mult, int C, int T, long long total) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         const int t = (int)(i % T);
         const int b = (int)(i / ((long long)C * T));
-        y[i] = (long long)t < (long long)mult * lengths[b] ? x[i] : 0.f;
+        y[i] = (long long)t < (long long)mult * lengths[(long long)b * len_stride] ? x[i] : 0.f;
     }
 }
 
@@ -304,8 +305,15 @@ int dv3_interleave2(const float* in, float* out, int B, int C, int T, int invers
 int dv3_mask_time(const float* x, float* y, const long long* lengths, int mult, int B, int C, int T, void* stream) {
     DV3_REQUIRE(B >= 1 && C >= 1 && T >= 1 && mult >= 1, "mask_time: bad shape");
     const long long total = (long long)B * C * T;
-    launch_k(mask_time_kernel, ew_blocks(total, 256), 256, 0, (cudaStream_t)stream, x, y, lengths, mult, C, T, total);
+    launch_k(mask_time_kernel, ew_blocks(total, 256), 256, 0, (cudaStream_t)stream, x, y, lengths, 1, mult, C, T, total);
     return check_launch("mask_time");
+}
+
+int dv3_mask_frames(const float* x, float* y, const long long* extent, int mult, int B, int C, int T, void* stream) {
+    DV3_REQUIRE(B >= 1 && C >= 1 && T >= 1 && mult >= 1 && extent != nullptr, "mask_frames: bad arguments");
+    const long long total = (long long)B * C * T;
+    launch_k(mask_time_kernel, ew_blocks(total, 256), 256, 0, (cudaStream_t)stream, x, y, extent, 0, mult, C, T, total);
+    return check_launch("mask_frames");
 }
 
 }  // extern "C"

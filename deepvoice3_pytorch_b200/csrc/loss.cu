@@ -26,26 +26,29 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 //   loss += sum (1-bw)*coef1*|d| + bw*coef*z,  coef = w*m/Sm + (1-w)/N,  m = (t+r < len_b)
 // priority bins (train.py:559-567): the L1 term becomes (1-pw)*L1(all bins) + pw*L1(bins < pbin), i.e.
 //   coef1 = (1-pw)*coef + [d < pbin]*pw*coef*(D/pbin)     (the same masked/plain means over the pbin-wide slice)
+// t_log (int64 in device memory, or null = T): the logical time extent of a batch padded to a larger bucket.  Pairs
+// t >= t_log - r are left out of the loss and its means, and their gradient is written as 0.
 __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* __restrict__ y,
-                                 const long long* __restrict__ lengths, float* __restrict__ grad,
-                                 float* __restrict__ loss, int B, int T, int D, int r, float w, float bw,
-                                 float eps, int pbin, float pw) {
+                                 const long long* __restrict__ lengths, const long long* __restrict__ t_log,
+                                 float* __restrict__ grad, float* __restrict__ loss, int B, int T, int D, int r,
+                                 float w, float bw, float eps, int pbin, float pw) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float red[8];
     __shared__ float s_inv_sm;
+    const int TL = t_log ? (int)min((long long)T, max((long long)r + 1, *t_log)) : T;
     if (threadIdx.x == 0) {
         double sm = 0.0;
         for (int b = 0; b < B; ++b) {
             long long v = lengths[b] - r;
             if (v < 0) v = 0;
-            if (v > T - r) v = T - r;
+            if (v > TL - r) v = TL - r;
             sm += (double)v;
         }
         s_inv_sm = sm > 0 ? (float)(1.0 / (sm * D)) : 0.f;
     }
     __syncthreads();
     const float inv_sm = s_inv_sm;
-    const float inv_n = 1.f / ((float)B * (float)(T - r) * (float)D);
+    const float inv_n = 1.f / ((float)B * (float)(TL - r) * (float)D);
     const long long total = (long long)B * T * D;
     const long long shift = (long long)r * D;
     const bool prio = pbin > 0 && pw > 0.f;
@@ -56,7 +59,7 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
         const long long bt = i / D;
         const int t = (int)(bt % T), b = (int)(bt / T);
         float g = 0.f;
-        if (t < T - r) {
+        if (t < TL - r) {
             const float p = y_hat[i], tg = y[i + shift];
             const float m = (t + r < lengths[b]) ? 1.f : 0.f;
             const float coef = w * m * inv_sm + (1.f - w) * inv_n;
@@ -82,24 +85,30 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
 
 // done BCE (mean) + guided attention (mean of attn*W):
 //   done_hat, done (n_done);  attn (A, B, Td, Ts), in_len / dec_len int64 [B];  grads written in full.
+// ext (int64 [2] in device memory, or null): logical (decoder steps, text positions) of a batch padded to a larger
+// bucket -- done_hat is then (B, Td); steps >= ext[0] and text positions >= ext[1] are left out of both means and
+// their gradient is written as 0.
 __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float* __restrict__ done,
                                 float* __restrict__ d_done, long long n_done, const float* __restrict__ attn,
                                 float* __restrict__ d_attn, const long long* __restrict__ in_len,
-                                const long long* __restrict__ dec_len, int A, int B, int Td, int Ts, float sigma,
-                                int use_attn, float* __restrict__ loss) {
+                                const long long* __restrict__ dec_len, const long long* __restrict__ ext, int A,
+                                int B, int Td, int Ts, float sigma, int use_attn, float* __restrict__ loss) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float red[8];
     float acc = 0.f;
     const long long stride = (long long)gridDim.x * blockDim.x, start = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    const float inv_nd = 1.f / (float)n_done;
+    const int TdL = ext ? (int)min((long long)Td, max(1LL, ext[0])) : Td;
+    const int TsL = ext ? (int)min((long long)Ts, max(1LL, ext[1])) : Ts;
+    const float inv_nd = 1.f / (float)(ext ? (long long)B * TdL : n_done);
     for (long long i = start; i < n_done; i += stride) {
+        if (ext && (int)(i % Td) >= TdL) { d_done[i] = 0.f; continue; }
         const float p = done_hat[i], t = done[i];
         acc -= inv_nd * (t * fmaxf(logf(p), -100.f) + (1.f - t) * fmaxf(logf(1.f - p), -100.f));
         d_done[i] = inv_nd * (p - t) / fmaxf((1.f - p) * p, 1e-12f);
     }
     if (use_attn) {
         const long long n_attn = (long long)A * B * Td * Ts;
-        const float inv_na = 1.f / (float)n_attn;
+        const float inv_na = 1.f / (float)((long long)A * B * TdL * TsL);
         const double inv2g2 = 1.0 / (2.0 * (double)sigma * (double)sigma);
         for (long long i = start; i < n_attn; i += stride) {
             const int n = (int)(i % Ts);
@@ -107,7 +116,7 @@ __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float*
             const int b = (int)((i / ((long long)Ts * Td)) % B);
             const long long N = in_len[b], Tl = dec_len[b];
             float wv = 0.f;
-            if (n < N && t < Tl) {
+            if (n < N && t < Tl && n < TsL && t < TdL) {
                 const double q = (double)n / (double)N - (double)t / (double)Tl;
                 wv = (float)(1.0 - exp(-q * q * inv2g2));
             }
@@ -136,18 +145,42 @@ int dv3_spec_loss(const float* y_hat, const float* y, const long long* lengths, 
                 "spec_loss: priority_bin=%d (D=%d) priority_weight=%g out of range", priority_bin, D, priority_weight);
     long long blocks = ((long long)B * T * D + 255) / 256;
     if (blocks > 132 * 8) blocks = 132 * 8;
-    launch_k(spec_loss_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, grad, loss, B, T, D, r,
-                                                                   masked_loss_weight, binary_divergence_weight, 1e-8f,
-                                                                   priority_bin, priority_weight);
+    launch_k(spec_loss_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths,
+             (const long long*)nullptr, grad, loss, B, T, D, r, masked_loss_weight, binary_divergence_weight, 1e-8f,
+             priority_bin, priority_weight);
     return check_launch("spec_loss");
+}
+
+int dv3_spec_loss_ext(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
+                      float* grad, float* loss, int B, int T, int D, int r, float masked_loss_weight,
+                      float binary_divergence_weight, int priority_bin, float priority_weight, void* stream) {
+    DV3_REQUIRE(t_log != nullptr, "spec_loss_ext: t_log is NULL");
+    DV3_REQUIRE(T > r && r >= 0, "spec_loss_ext: need T > r");
+    DV3_REQUIRE(priority_bin >= 0 && priority_bin <= D && priority_weight >= 0.f && priority_weight <= 1.f,
+                "spec_loss_ext: priority_bin=%d (D=%d) priority_weight=%g out of range", priority_bin, D,
+                priority_weight);
+    long long blocks = ((long long)B * T * D + 255) / 256;
+    if (blocks > 132 * 8) blocks = 132 * 8;
+    launch_k(spec_loss_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, t_log, grad, loss, B, T,
+             D, r, masked_loss_weight, binary_divergence_weight, 1e-8f, priority_bin, priority_weight);
+    return check_launch("spec_loss_ext");
 }
 
 int dv3_aux_loss(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
                  float* d_attn, const long long* in_len, const long long* dec_len, int A, int B, int Td, int Ts,
                  float sigma, int use_attn, float* loss, void* stream) {
     launch_k(aux_loss_kernel, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done, attn, d_attn, in_len,
-                                                              dec_len, A, B, Td, Ts, sigma, use_attn, loss);
+             dec_len, (const long long*)nullptr, A, B, Td, Ts, sigma, use_attn, loss);
     return check_launch("aux_loss");
+}
+
+int dv3_aux_loss_ext(const float* done_hat, const float* done, float* d_done, const float* attn, float* d_attn,
+                     const long long* in_len, const long long* dec_len, const long long* ext, int A, int B, int Td,
+                     int Ts, float sigma, int use_attn, float* loss, void* stream) {
+    DV3_REQUIRE(ext != nullptr, "aux_loss_ext: ext is NULL");
+    launch_k(aux_loss_kernel, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, (long long)B * Td, attn,
+             d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma, use_attn, loss);
+    return check_launch("aux_loss_ext");
 }
 
 }  // extern "C"

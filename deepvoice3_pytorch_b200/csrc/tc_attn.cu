@@ -47,6 +47,7 @@ struct AttnParams {
     float scale, p_drop;
     const unsigned long long* seed_ptr;
     uint32_t salt;
+    const long long* ts_log;   // logical key count in device memory, or null: scale = ts_log * sqrt(1/ts_log) then
 };
 
 // 8 fp32 -> 8 bf16 hi (16 bytes) + 8 bf16 lo
@@ -203,6 +204,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
     const bool vec_td = (Td & 3) == 0, vec_ts = (Ts & 3) == 0;
     float* sc = reinterpret_cast<float*>(smem + 65536);
     pdl_wait();                 // global memory from here on
+    const float scale = p.ts_log ? context_scale(*p.ts_log) : p.scale;
 
     // ---------------- GEMM 1: D1[t][s] = sum_e A1[e][t0+t] * B1[e][s] -----------------------------------
     float acc[128];
@@ -284,7 +286,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
                 for (int i = 0; i < 32; ++i) {
                     const int s = c32 + i;
                     if (tv && s < Ts) {
-                        float g = p.scale * srow[s] * drop_scale(drop, (uint32_t)(rbase + s));
+                        float g = scale * srow[s] * drop_scale(drop, (uint32_t)(rbase + s));
                         if (p.dprobs) g += tile[lane * TILE_PITCH + i];
                         dot = fmaf(g, pv[i], dot);
                     }
@@ -317,7 +319,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
                         wr = pr;
                         a2 = pr * drop_scale(drop, (uint32_t)(rbase + s));
                     } else {
-                        float g = p.scale * v * drop_scale(drop, (uint32_t)(rbase + s));
+                        float g = scale * v * drop_scale(drop, (uint32_t)(rbase + s));
                         if (p.dprobs) g += tile[lane * TILE_PITCH + i];
                         a2 = pv[i] * (g - r0v);
                         wr = a2;
@@ -352,7 +354,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_rows_kernel(const __grid_c
     __syncthreads();
 
     // ---------------- GEMM 2: D2[t][e] = sum_s A2[t][s] * B2[e][s], 128 channels at a time -------------------------
-    const float scl = BWD == 0 ? p.scale : 1.f;
+    const float scl = BWD == 0 ? scale : 1.f;
     float* __restrict__ out = p.out + (size_t)b * E * Td;
     const uint32_t sa = smem_u32(smem) + wg * 8192, sb = smem_u32(smem + 65536);
     for (int e0 = 0; e0 < E; e0 += AT_NS) {               // rows of B2 past E are never stored
@@ -388,6 +390,7 @@ struct AttnColsParams {
     float scale, p_drop;
     const unsigned long long* seed_ptr;
     uint32_t salt;
+    const long long* ts_log;   // as AttnParams::ts_log
 };
 
 __global__ void __launch_bounds__(AT_THREADS, 1) attn_cols_kernel(const __grid_constant__ AttnColsParams p) {
@@ -400,6 +403,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_cols_kernel(const __grid_c
     const bool vec_td = (Td & 3) == 0, vec_ts = (Ts & 3) == 0;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
     pdl_wait();                 // global memory from here on
+    const float scale = p.ts_log ? context_scale(*p.ts_log) : p.scale;
 
     const int kchunks = (Td + 63) / 64;
     const uint32_t sa = smem_u32(smem);
@@ -452,7 +456,7 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attn_cols_kernel(const __grid_c
         }
         // rows e of dV / dK are contiguous along the keys
         float* __restrict__ dst = (pass == 0 ? p.dv : p.dk) + (size_t)b * E * Ts;
-        const float scl = pass == 0 ? p.scale : 1.f;
+        const float scl = pass == 0 ? scale : 1.f;
 #pragma unroll
         for (int i = 0; i < 64; ++i) {
             const int e = e0 + 64 * wg + frag_row(i, wq, lane), s = frag_col(i, lane);
@@ -479,23 +483,39 @@ int dv3_tc_attn_supported(int B, int E, int Td, int Ts) {
     return B >= 1 && B <= 65535 && E >= 16 && E <= 256 && (E % 16) == 0 && Ts >= 1 && Ts <= AT_NS && Td >= 1;
 }
 
-int dv3_tc_attn_fwd(const float* q, const float* k, const float* v, const unsigned char* mask, float* probs,
-                    float* out, int B, int E, int Td, int Ts, float scale, float p_drop,
-                    const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+static int tc_attn_fwd(const float* q, const float* k, const float* v, const unsigned char* mask, float* probs,
+                       float* out, int B, int E, int Td, int Ts, float scale, const long long* ts_log, float p_drop,
+                       const unsigned long long* seed_ptr, unsigned salt, void* stream) {
     DV3_REQUIRE(dv3_tc_attn_supported(B, E, Td, Ts), "tc_attn_fwd: unsupported shape B=%d E=%d Td=%d Ts=%d", B, E, Td, Ts);
     static bool configured = false;
     if (!configured) { if (set_smem(attn_rows_kernel<0>, ROWS_SMEM, "tc_attn_fwd")) return 1; configured = true; }
     AttnParams p = {};
     p.a1 = q; p.b1 = k; p.b2 = v; p.mask = mask; p.probs = probs; p.out = out;
     p.B = B; p.E = E; p.Td = Td; p.Ts = Ts; p.scale = scale; p.p_drop = p_drop; p.seed_ptr = seed_ptr; p.salt = salt;
+    p.ts_log = ts_log;
     launch_k(attn_rows_kernel<0>, dim3((Td + 127) / 128, B), AT_THREADS, ROWS_SMEM, (cudaStream_t)stream, p);
     return check_launch("tc_attn_fwd");
 }
 
+int dv3_tc_attn_fwd(const float* q, const float* k, const float* v, const unsigned char* mask, float* probs,
+                    float* out, int B, int E, int Td, int Ts, float scale, float p_drop,
+                    const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+    return tc_attn_fwd(q, k, v, mask, probs, out, B, E, Td, Ts, scale, nullptr, p_drop, seed_ptr, salt, stream);
+}
+
+// the context scale Ts*sqrt(1/Ts) taken from a logical key count in device memory (a batch padded to a bucket)
+int dv3_tc_attn_fwd_ext(const float* q, const float* k, const float* v, const unsigned char* mask, float* probs,
+                        float* out, int B, int E, int Td, int Ts, const long long* ts_log, float p_drop,
+                        const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+    DV3_REQUIRE(ts_log != nullptr, "tc_attn_fwd_ext: ts_log is NULL");
+    return tc_attn_fwd(q, k, v, mask, probs, out, B, E, Td, Ts, 0.f, ts_log, p_drop, seed_ptr, salt, stream);
+}
+
 // ds: scratch (B,Td,Ts) fp32 written by the first launch and read by the second; dprobs may be null
-int dv3_tc_attn_bwd(const float* dout, const float* q, const float* k, const float* v, const float* probs,
-                    const float* dprobs, float* ds, float* dq, float* dk, float* dv, int B, int E, int Td, int Ts,
-                    float scale, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+static int tc_attn_bwd(const float* dout, const float* q, const float* k, const float* v, const float* probs,
+                       const float* dprobs, float* ds, float* dq, float* dk, float* dv, int B, int E, int Td, int Ts,
+                       float scale, const long long* ts_log, float p_drop, const unsigned long long* seed_ptr,
+                       unsigned salt, void* stream) {
     DV3_REQUIRE(dv3_tc_attn_supported(B, E, Td, Ts), "tc_attn_bwd: unsupported shape B=%d E=%d Td=%d Ts=%d", B, E, Td, Ts);
     static bool configured = false;
     if (!configured) {
@@ -506,13 +526,31 @@ int dv3_tc_attn_bwd(const float* dout, const float* q, const float* k, const flo
     AttnParams p = {};
     p.a1 = dout; p.b1 = v; p.b2 = k; p.probs = const_cast<float*>(probs); p.dprobs = dprobs; p.ds = ds; p.out = dq;
     p.B = B; p.E = E; p.Td = Td; p.Ts = Ts; p.scale = scale; p.p_drop = p_drop; p.seed_ptr = seed_ptr; p.salt = salt;
+    p.ts_log = ts_log;
     launch_k(attn_rows_kernel<1>, dim3((Td + 127) / 128, B), AT_THREADS, ROWS_SMEM, (cudaStream_t)stream, p);
     if (check_launch("tc_attn_bwd(rows)")) return 1;
     AttnColsParams c = {};
     c.dout = dout; c.q = q; c.probs = probs; c.ds = ds; c.dv = dv; c.dk = dk;
     c.B = B; c.E = E; c.Td = Td; c.Ts = Ts; c.scale = scale; c.p_drop = p_drop; c.seed_ptr = seed_ptr; c.salt = salt;
+    c.ts_log = ts_log;
     launch_k(attn_cols_kernel, dim3((E + 127) / 128, B), AT_THREADS, COLS_SMEM, (cudaStream_t)stream, c);
     return check_launch("tc_attn_bwd(cols)");
+}
+
+int dv3_tc_attn_bwd(const float* dout, const float* q, const float* k, const float* v, const float* probs,
+                    const float* dprobs, float* ds, float* dq, float* dk, float* dv, int B, int E, int Td, int Ts,
+                    float scale, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+    return tc_attn_bwd(dout, q, k, v, probs, dprobs, ds, dq, dk, dv, B, E, Td, Ts, scale, nullptr, p_drop, seed_ptr,
+                       salt, stream);
+}
+
+int dv3_tc_attn_bwd_ext(const float* dout, const float* q, const float* k, const float* v, const float* probs,
+                        const float* dprobs, float* ds, float* dq, float* dk, float* dv, int B, int E, int Td, int Ts,
+                        const long long* ts_log, float p_drop, const unsigned long long* seed_ptr, unsigned salt,
+                        void* stream) {
+    DV3_REQUIRE(ts_log != nullptr, "tc_attn_bwd_ext: ts_log is NULL");
+    return tc_attn_bwd(dout, q, k, v, probs, dprobs, ds, dq, dk, dv, B, E, Td, Ts, 0.f, ts_log, p_drop, seed_ptr, salt,
+                       stream);
 }
 
 }  // extern "C"

@@ -36,16 +36,20 @@ struct SplitParams {
     int B, C, T, pitch;
     int mode, residual, relu;  // gate mode (0 GLU, 1 highway), GLU residual flag; ReLU flag
     float p; const unsigned long long* seed_ptr; unsigned salt;     // SPLIT_INPUT dropout
+    const long long* tlen; int tmult;   // or null: frames t >= tmult * tlen[0] are written as 0 (and leave dbias)
 };
 
+// 6 CTAs per SM: holds the gate split (33 KB of shared memory: 6 fit) at 40 registers with the extent mask, no spills.
 template <int KIND>
-__global__ void __launch_bounds__(256) plane_split_kernel(const __grid_constant__ SplitParams p) {
+__global__ void __launch_bounds__(256, 6) plane_split_kernel(const __grid_constant__ SplitParams p) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float sa[64][65];
     __shared__ float sb[KIND == SPLIT_GATE ? 64 : 1][65];
     const int tid = threadIdx.x;
     const int b = blockIdx.z, c0 = blockIdx.y * 64, t0 = blockIdx.x * 64;
     const int C = p.C, T = p.T;
+    // the logical extent of a batch padded to a bucket (device memory): the frames past it read as zeros
+    const int TL = p.tlen ? (int)min((long long)T, (long long)p.tmult * *p.tlen) : T;
     const bool vec = (T & 3) == 0;
     const DropCfg drop = make_drop(KIND == SPLIT_INPUT ? p.p : 0.f, p.seed_ptr, p.salt);
     const float gs = (KIND == SPLIT_GATE && p.mode == 0 && p.residual) ? 0.70710678118654752f : 1.f;
@@ -81,7 +85,7 @@ __global__ void __launch_bounds__(256) plane_split_kernel(const __grid_constant_
                 } else {
                     v0[e] = (p.relu && !(x1[e] > 0.f)) ? 0.f : x0[e];
                 }
-                if (t + e >= T) { v0[e] = 0.f; v1[e] = 0.f; }
+                if (t + e >= TL) { v0[e] = 0.f; v1[e] = 0.f; }
             }
         }
 #pragma unroll
@@ -152,38 +156,78 @@ extern "C" {
 
 static dim3 split_grid(int B, int C, int T) { return dim3((T + 63) / 64, (C + 63) / 64, B); }
 
-int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, int k, int dilation,
-                       int causal, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+static int split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, float p_drop,
+                       const unsigned long long* seed_ptr, unsigned salt, const long long* tlen, int tmult,
+                       void* stream) {
     DV3_REQUIRE(B <= 65535 && (C + 63) / 64 <= 65535, "tc_split_input: grid too large");
     DV3_REQUIRE(npl == 2, "tc_split_input: npl must be 2");
-    (void)k; (void)dilation; (void)causal;
+    DV3_REQUIRE(!tlen || tmult >= 1, "tc_split_input: tmult must be >= 1");
     SplitParams p = {};
     p.in0 = x; p.planes = (bf16*)btc; p.wg = (bf16*)bct; p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8;
-    p.p = p_drop; p.seed_ptr = seed_ptr; p.salt = salt;
+    p.p = p_drop; p.seed_ptr = seed_ptr; p.salt = salt; p.tlen = tlen; p.tmult = tmult;
     launch_k(plane_split_kernel<SPLIT_INPUT>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
     return check_launch("tc_split_input");
 }
 
-int dv3_tc_gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
-                          float* dbias, int B, int C, int T, int mode, int residual, void* stream) {
+static int gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
+                          float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
+                          int tmult, void* stream) {
     DV3_REQUIRE(bct == nullptr, "tc_gate_bwd_split: bct must be NULL");
     DV3_REQUIRE(C % 8 == 0 && (mode == 0 || x != nullptr), "tc_gate_bwd_split: C %% 8 != 0 or highway without x");
+    DV3_REQUIRE(!tlen || tmult >= 1, "tc_gate_bwd_split: tmult must be >= 1");
     SplitParams p = {};
     p.in0 = dy; p.in1 = a; p.in2 = s; p.in3 = x; p.planes = (bf16*)btc; p.dbias = dbias;
-    p.B = B; p.C = C; p.T = T; p.pitch = 2 * C; p.mode = mode; p.residual = residual;
+    p.B = B; p.C = C; p.T = T; p.pitch = 2 * C; p.mode = mode; p.residual = residual; p.tlen = tlen; p.tmult = tmult;
     launch_k(plane_split_kernel<SPLIT_GATE>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
     return check_launch("tc_gate_bwd_split");
 }
 
-int dv3_tc_grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
-                      int relu, void* stream) {
+static int grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
+                      int relu, const long long* tlen, int tmult, void* stream) {
     DV3_REQUIRE(bct == nullptr, "tc_grad_split: bct must be NULL");
     DV3_REQUIRE(!relu || y != nullptr, "tc_grad_split: ReLU backward needs the forward output");
+    DV3_REQUIRE(!tlen || tmult >= 1, "tc_grad_split: tmult must be >= 1");
     SplitParams p = {};
     p.in0 = dy; p.in1 = y; p.planes = (bf16*)btc; p.dbias = dbias;
-    p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8; p.relu = relu;
+    p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8; p.relu = relu; p.tlen = tlen; p.tmult = tmult;
     launch_k(plane_split_kernel<SPLIT_GRAD>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
     return check_launch("tc_grad_split");
+}
+
+int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, int k, int dilation,
+                       int causal, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+    (void)k; (void)dilation; (void)causal;
+    return split_input(x, btc, npl, bct, B, C, T, p_drop, seed_ptr, salt, nullptr, 1, stream);
+}
+
+int dv3_tc_gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
+                          float* dbias, int B, int C, int T, int mode, int residual, void* stream) {
+    return gate_bwd_split(dy, a, s, x, btc, bct, dbias, B, C, T, mode, residual, nullptr, 1, stream);
+}
+
+int dv3_tc_grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
+                      int relu, void* stream) {
+    return grad_split(dy, y, btc, bct, dbias, B, C, T, relu, nullptr, 1, stream);
+}
+
+// The same with an optional logical time extent in device memory (a batch padded to a bucket): tlen null behaves as
+// above; otherwise frames t >= tmult * tlen[0] of the input (forward operand) or of the incoming gradient are taken
+// as 0 -- the time mask of the padded frames and its gradient, folded into the passes that read those tensors anyway.
+int dv3_tc_split_input_ext(const float* x, void* btc, int npl, void* bct, int B, int C, int T, float p_drop,
+                           const unsigned long long* seed_ptr, unsigned salt, const long long* tlen, int tmult,
+                           void* stream) {
+    return split_input(x, btc, npl, bct, B, C, T, p_drop, seed_ptr, salt, tlen, tmult, stream);
+}
+
+int dv3_tc_gate_bwd_split_ext(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
+                              float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
+                              int tmult, void* stream) {
+    return gate_bwd_split(dy, a, s, x, btc, bct, dbias, B, C, T, mode, residual, tlen, tmult, stream);
+}
+
+int dv3_tc_grad_split_ext(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
+                          int relu, const long long* tlen, int tmult, void* stream) {
+    return grad_split(dy, y, btc, bct, dbias, B, C, T, relu, tlen, tmult, stream);
 }
 
 }  // extern "C"

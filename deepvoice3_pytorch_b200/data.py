@@ -68,6 +68,75 @@ def collate(batch, r=1, downsample_step=4, pin=False):
     return out
 
 
+# Bucket grid of the CUDA-graph training step (train_step.TrainStep): a batch whose shape differs from the first one is
+# padded up to the next multiple of BUCKET_TEXT text positions and BUCKET_DEC decoder steps, and one graph is captured
+# per bucket.  Multiples of 4 keep the float4 paths of the operand-split and attention kernels on (T % 4 == 0); the
+# tensor-core convs themselves take any T.  On the LJSpeech-like length model of bench_train_ragged.py (64 batches of
+# 16, 53 distinct shapes) this grid adds 2 % padded frames to collate's own padding and needs 9 buckets.
+BUCKET_TEXT, BUCKET_DEC = 16, 8
+
+
+def bucket_shape(T_text, T_dec):
+    """(text positions, decoder steps) of a batch -> the bucket it is padded to (rounded up to the grid)."""
+    return -(-int(T_text) // BUCKET_TEXT) * BUCKET_TEXT, -(-int(T_dec) // BUCKET_DEC) * BUCKET_DEC
+
+
+def batch_extents(batch):
+    """Logical extents of a batch as ``collate`` returns it: (decoder steps, text positions, mel frames, linear
+    frames), the slots ops.EXT_DEC, EXT_TEXT, EXT_MEL, EXT_LIN."""
+    return (int(batch["done"].shape[1]), int(batch["x"].shape[1]), int(batch["mel"].shape[1]), int(batch["y"].shape[1]))
+
+
+def pad_to_bucket(batch, T_text, T_dec, r=1, downsample_step=4, out=None):
+    """Pad a batch as ``collate`` returns it (host or device tensors) to T_text text positions and T_dec decoder steps
+    (T_dec*r mel frames, T_dec*r*downsample_step linear frames) and attach its logical extents.
+
+    Text, text positions, mel, y and done are zero past the logical extent; frame positions are 1..T_dec_logical, then 0
+    (so a bucket never indexes past the model's max_positions); per-row lengths and speaker ids are unchanged.
+    ``extents`` is int64[4] (``batch_extents``) on the batch's device.  ``TrainStep`` runs such a batch with the loss,
+    gradients and update of the unpadded one.  out: a dict of the same keys in the bucket shape to fill in place
+    (``out["extents"]`` included) -- then nothing is allocated but the 32-byte staging of the extents."""
+    ext = batch_extents(batch)
+    T_dec_log, T_text_log = ext[0], ext[1]
+    if ext[2] != T_dec_log * r or ext[3] != T_dec_log * r * downsample_step:
+        raise ValueError("batch shapes %s do not fit r=%d downsample_step=%d" % (ext, r, downsample_step))
+    if T_text < T_text_log or T_dec < T_dec_log:
+        raise ValueError("bucket (T_text=%d, T_dec=%d) is smaller than the batch (%d, %d)" % (T_text, T_dec,
+                                                                                            T_text_log, T_dec_log))
+    if batch.get("extents") is not None:
+        raise ValueError("batch is already padded to a bucket")
+    sizes = {"x": T_text, "text_positions": T_text, "frame_positions": T_dec, "mel": T_dec * r,
+             "y": T_dec * r * downsample_step, "done": T_dec}
+    fill = out is not None
+    out = {} if out is None else out
+    for k, v in batch.items():
+        if k == "extents":
+            continue
+        if k not in sizes or not torch.is_tensor(v):
+            if not fill:
+                out[k] = v.clone() if torch.is_tensor(v) else v
+            elif torch.is_tensor(v):
+                out[k].copy_(v, non_blocking=True)
+            else:
+                out[k] = v
+            continue
+        T = v.shape[1]
+        if not fill:
+            shape = (v.shape[0], sizes[k]) + tuple(v.shape[2:])
+            out[k] = torch.empty(shape, dtype=v.dtype, device=v.device, pin_memory=v.is_pinned())
+        out[k][:, :T].copy_(v, non_blocking=True)
+        out[k][:, T:].zero_()
+    dev = batch["x"].device
+    host = torch.tensor(ext, dtype=torch.int64)
+    if dev.type == "cuda" or batch["x"].is_pinned():
+        host = host.pin_memory()
+    if fill:
+        out["extents"].copy_(host, non_blocking=True)
+    else:
+        out["extents"] = host.to(dev, non_blocking=True) if dev.type == "cuda" else host
+    return out
+
+
 class TrainTxtDataset(torch.utils.data.Dataset):
     """Items are what ``collate`` consumes: (token ids int32, mel (T, num_mels) float32, linear (T, n_freq) float32
     [, speaker_id]).  ``frame_lengths`` (column 3 of train.txt) feeds the length-bucketed sampler without touching

@@ -322,7 +322,7 @@ class Converter(nn.Module):
         i = 0
         while i < len(layers):
             if _is_upsampler(layers[i]):
-                x = layers[i](mask_conv_input(layers[i], x))
+                x = layers[i](mask_conv_input(layers[i], x), extent=ops.extent_frames(x))
                 i += 1
                 continue
             j = i

@@ -139,18 +139,18 @@ class Conv1dGLU(_GatedConv):
         self._make_conv(in_channels, out_channels, kernel_size, padding, dilation, causal, dropout, std_mul)
         self.speaker_proj = Linear(speaker_embed_dim, out_channels) if n_speakers > 1 else None
 
-    def forward(self, x, speaker_embed=None, fuse_residual=None):
+    def forward(self, x, speaker_embed=None, fuse_residual=None, extent=None):
         """x (B, C, T); speaker_embed (B, T, S) time-expanded (and, in training, dropped-out) embedding.
         fuse_residual=True computes (block(x) + x)*sqrt(.5) in the kernel even when the module was built with
         residual=False -- the decoder applies exactly that outside the block when no attention layer sits in between
-        (reference deepvoice3.py:333-349)."""
+        (reference deepvoice3.py:333-349).  extent: ``ops.extent_frames(x)`` inside a bucketed training batch."""
         spk = None
         if self.speaker_proj is not None:
             spk = F.softsign(self.speaker_proj.forward_bct(ops.transpose12(speaker_embed)))
         c = self.conv
         residual = self.residual if fuse_residual is None else bool(fuse_residual)
         return ops.convblock(x, c.weight_v, c.weight_g, c.bias, spk, c.kernel_size[0], c.dilation[0],
-                             self.causal, ops.MODE_GLU, residual, self.dropout, self.training)
+                             self.causal, ops.MODE_GLU, residual, self.dropout, self.training, extent=extent)
 
 
     def incremental_forward(self, x, speaker_embed=None):
@@ -175,10 +175,10 @@ class HighwayConv1d(_GatedConv):
         self._make_conv(in_channels, out_channels, kernel_size, padding, dilation, causal, dropout,
                         1.0 if std_mul is None else std_mul)
 
-    def forward(self, x):
+    def forward(self, x, extent=None):
         c = self.conv
         return ops.convblock(x, c.weight_v, c.weight_g, c.bias, None, c.kernel_size[0], c.dilation[0],
-                             self.causal, ops.MODE_HIGHWAY, True, self.dropout, self.training)
+                             self.causal, ops.MODE_HIGHWAY, True, self.dropout, self.training, extent=extent)
 
     def incremental_forward(self, x):
         """reference modules.py:197-198."""
@@ -201,7 +201,8 @@ def get_mask_from_lengths(memory, memory_lengths):
 
 def mask_conv_input(f, x):
     """Inside an ``ops.length_scope``: zero each row's frames past its length before a layer whose kernel spans more
-    than one frame.  Outside one, x unchanged."""
+    than one frame.  Outside one, x unchanged.  (Inside an ``ops.extent_scope`` the layers mask themselves: see
+    ``run_conv_stack``.)"""
     if ops._length_scope is None:
         return x
     conv = f.conv if isinstance(f, _GatedConv) else f
@@ -214,21 +215,31 @@ def run_conv_stack(layers, x, speaker_embed_btc=None, boundaries=None):
     """Run a ModuleList/Sequential of [Conv1d | ReLU | Sigmoid | ConvTranspose1d | Conv1dGLU | HighwayConv1d]
     on x (B, C, T), fusing every ``Conv1d -> ReLU`` pair into one kernel launch.
     boundaries: {layer index: tag} -- the input of that layer is an ops.grad_boundary (its gradient being ready means
-    the parameter gradients of layers[index:] are final)."""
+    the parameter gradients of layers[index:] are final).
+
+    Inside an ``ops.extent_scope`` (a training batch padded to a bucket) every conv layer gets the logical extent of
+    its input: a conv spanning more than one frame reads the frames past it as zeros, and every layer takes the
+    gradient arriving there as 0 -- in the operand-split passes on the tensor-core path.  The data gradient of such a
+    conv still spreads into the padded frames of its input, so the gradient leaving the stack is masked once."""
     layers = list(layers)
+    x = ops.extent_grad_mask(x, ops.extent_frames(x))
     i = 0
     while i < len(layers):
         f = layers[i]
         if boundaries and i in boundaries:
             x = ops.grad_boundary(x, boundaries[i])
         x = mask_conv_input(f, x)
+        ext = ops.extent_frames(x)
+        kw = {} if ext is None else {"extent": ext}
         fuse_relu = isinstance(f, _Conv1d) and i + 1 < len(layers) and isinstance(layers[i + 1], nn.ReLU)
         if isinstance(f, _Conv1d):
-            x = f(x, relu=fuse_relu)
+            x = f(x, relu=fuse_relu, **kw)
         elif isinstance(f, Conv1dGLU):
-            x = f(x, speaker_embed_btc)
+            x = f(x, speaker_embed_btc, **kw)
         elif isinstance(f, nn.ReLU):
             x = torch.relu(x)
+        elif isinstance(f, (_GatedConv, _ConvTranspose1d)):
+            x = f(x, **kw)
         else:
             x = f(x)
         i += 2 if fuse_relu else 1

@@ -374,7 +374,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
     forward GEMM, bf16 pairs in the gradient GEMMs)."""
 
     @staticmethod
-    def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training):
+    def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training, extent):
         _chk(x, v, g, bias, spk)
         B, C, T = x.shape
         dev = x.device
@@ -388,8 +388,12 @@ class _ConvBlockTCFn(torch.autograd.Function):
         y = torch.empty_like(x)
         a = torch.empty_like(x) if need_bwd else None
         s = torch.empty_like(x) if need_bwd else None
-        lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, C, T, k, dilation, int(causal), p,
-                 seed_ptr, salt, _stream())
+        if extent is not None and k > 1:    # frames past the logical extent enter the conv as zeros
+            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), 2, _p(x_wg), B, C, T, p, seed_ptr, salt, extent[0],
+                     extent[1], _stream())
+        else:
+            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, C, T, k, dilation, int(causal), p,
+                     seed_ptr, salt, _stream())
         if side is not None:
             side.join()
         lib.call("dv3_tc_convblock_fwd", _p(x_btc), _p(wfwd), 2, _p(bias), _p(spk), _p(x), _p(y), _p(a), _p(s),
@@ -400,6 +404,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
             ctx.seed_t = seed_t
             ctx.bias_param = bias if bias.is_leaf else None
             ctx.bank = bank
+            ctx.extent = extent
         return y
 
     @staticmethod
@@ -411,8 +416,12 @@ class _ConvBlockTCFn(torch.autograd.Function):
         B, C, T = x.shape
         d_btc = torch.empty(2, B, T, 2 * C, device=dev, dtype=torch.bfloat16)
         wg = _TCWeightGrad(ctx, v, g)
-        lib.call("dv3_tc_gate_bwd_split", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(wg.dbias), B, C, T,
-                 mode, int(residual), _stream())
+        if ctx.extent is not None:          # the gradient past the extent is taken as 0 (see ops.extent_frames)
+            lib.call("dv3_tc_gate_bwd_split_ext", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(wg.dbias), B, C,
+                     T, mode, int(residual), ctx.extent[0], ctx.extent[1], _stream())
+        else:
+            lib.call("dv3_tc_gate_bwd_split", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(wg.dbias), B, C, T,
+                     mode, int(residual), _stream())
         wg.start(d_btc, x_wg, inv, B, T, dilation, causal)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -424,14 +433,14 @@ class _ConvBlockTCFn(torch.autograd.Function):
         dspk = None
         if has_spk and ctx.needs_input_grad[4]:     # d_a = hi + lo * 2^-11 of the (B,T,2C) planes, back to (B,C,T)
             dspk = transpose12((d_btc[0, :, :, :C].float() + d_btc[1, :, :, :C].float() * (1.0 / 2048.0)).contiguous())
-        return (dx, dv, dg, dbias, dspk) + (None,) * 7
+        return (dx, dv, dg, dbias, dspk) + (None,) * 8
 
 
 class _Conv1dTCFn(torch.autograd.Function):
     """Plain weight-normed conv (+ReLU) on the tensor-core path (1x1 convs, projections)."""
 
     @staticmethod
-    def forward(ctx, x, v, g, bias, k, dilation, causal, relu):
+    def forward(ctx, x, v, g, bias, k, dilation, causal, relu, extent):
         _chk(x, v, g, bias)
         B, Cin, T = x.shape
         Cout = v.shape[0]
@@ -443,8 +452,12 @@ class _Conv1dTCFn(torch.autograd.Function):
         x_btc = torch.empty(2, B, T, Cinp, device=dev, dtype=torch.float16)
         x_wg = torch.empty(2, B, T, Cinp, device=dev, dtype=bf) if need_w else None
         y = torch.empty(B, Cout, T, device=dev)
-        lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, k, dilation, int(causal), 0.0,
-                 None, 0, _stream())
+        if extent is not None and k > 1:
+            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, 0.0, None, 0, extent[0],
+                     extent[1], _stream())
+        else:
+            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, k, dilation, int(causal), 0.0,
+                     None, 0, _stream())
         if side is not None:
             side.join()
         lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), 2, _p(y), B, Cin, Cout, T, k, dilation, int(causal), 0,
@@ -454,6 +467,7 @@ class _Conv1dTCFn(torch.autograd.Function):
             ctx.cfg = (B, Cin, Cout, T, k, dilation, causal, relu)
             ctx.bias_param = bias if bias.is_leaf else None
             ctx.bank = bank
+            ctx.extent = extent
         return y
 
     @staticmethod
@@ -464,7 +478,12 @@ class _Conv1dTCFn(torch.autograd.Function):
         dev = dy.device
         g_btc = torch.empty(2, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
         wg = _TCWeightGrad(ctx, v, g)
-        lib.call("dv3_tc_grad_split", _p(dy), _p(y), _p(g_btc), None, _p(wg.dbias), B, Cout, T, int(relu), _stream())
+        if ctx.extent is not None:
+            lib.call("dv3_tc_grad_split_ext", _p(dy), _p(y), _p(g_btc), None, _p(wg.dbias), B, Cout, T, int(relu),
+                     ctx.extent[0], ctx.extent[1], _stream())
+        else:
+            lib.call("dv3_tc_grad_split", _p(dy), _p(y), _p(g_btc), None, _p(wg.dbias), B, Cout, T, int(relu),
+                     _stream())
         wg.start(g_btc, x_wg, inv, B, T, dilation, causal)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -472,14 +491,14 @@ class _Conv1dTCFn(torch.autograd.Function):
             lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), 2, _p(dx), B, Cout, Cin, T, k, dilation, int(causal), 1, None,
                      0, 0.0, None, 0, 0, None, None, 0.0, None, _stream())
         dv, dg, dbias = wg.finish()
-        return (dx, dv, dg, dbias) + (None,) * 4
+        return (dx, dv, dg, dbias) + (None,) * 5
 
 
 class _ConvT2TCFn(torch.autograd.Function):
     """ConvTranspose1d(k=2,s=2) on the tensor-core path: a 1x1 conv with 2*Cout rows (j,co) + the time interleave."""
 
     @staticmethod
-    def forward(ctx, x, v, g, bias):
+    def forward(ctx, x, v, g, bias, extent):
         _chk(x, v, g, bias)
         B, Cin, T = x.shape
         Cout = v.shape[1]
@@ -502,6 +521,7 @@ class _ConvT2TCFn(torch.autograd.Function):
         lib.call("dv3_interleave2", _p(yp), _p(y), B, Cout, T, 0, _stream())
         ctx.save_for_backward(v, g, x_wg, wbwd, inv)
         ctx.cfg = (B, Cin, Cout, T)
+        ctx.extent = extent                 # a 2x upsampler mixes no frames: only its incoming gradient is masked
         return y
 
     @staticmethod
@@ -515,7 +535,11 @@ class _ConvT2TCFn(torch.autograd.Function):
         lib.call("dv3_interleave2", _p(dy), _p(dyp), B, Cout, T, 1, _stream())
         g_btc = torch.empty(2, B, T, K2p, device=dev, dtype=bf)
         db2 = torch.zeros(2 * Cout, device=dev)
-        lib.call("dv3_tc_grad_split", _p(dyp), None, _p(g_btc), None, _p(db2), B, 2 * Cout, T, 0, _stream())
+        if ctx.extent is not None:          # dyp is in the input's time units
+            lib.call("dv3_tc_grad_split_ext", _p(dyp), None, _p(g_btc), None, _p(db2), B, 2 * Cout, T, 0,
+                     ctx.extent[0], ctx.extent[1], _stream())
+        else:
+            lib.call("dv3_tc_grad_split", _p(dyp), None, _p(g_btc), None, _p(db2), B, 2 * Cout, T, 0, _stream())
         dbias = db2[:Cout] + db2[Cout:]
         dx = None
         if ctx.needs_input_grad[0]:
@@ -532,7 +556,7 @@ class _ConvT2TCFn(torch.autograd.Function):
             lib.call("dv3_tc_wgrad_mn", _p(g_btc), _p(x_wg), _p(partials), numel, B, M, Cin, T, 1, 1, 0, Cout, 2, 1,
                      2 * Cout, 0, _stream())
             dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
-        return dx, dv, dg, dbias
+        return dx, dv, dg, dbias, None
 
 
 def _tc_selected():
@@ -566,14 +590,19 @@ def tc_supported(B, C, T, k):
 
 
 def convblock(x, v, g, bias, spk=None, k=3, dilation=1, causal=False, mode=MODE_GLU, residual=True,
-              p_drop=0.0, training=False):
+              p_drop=0.0, training=False, extent=None):
     """Fused weight-normed dilated conv + gate.  x (B,C,T); v (2C,C,k); g (2C,1,1); bias (2C);
-    spk (B,C,T) already softsign'ed (or None)."""
+    spk (B,C,T) already softsign'ed (or None).  extent (``extent_frames``): frames past it are taken as 0 in the conv
+    input (k > 1) and in the incoming gradient."""
+    if causal:
+        extent = None
     if _tc_selected() and x.is_cuda and tc_supported(x.shape[0], x.shape[1], x.shape[2], int(k)):
         return _ConvBlockTCFn.apply(_c(x), v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
-                                    bool(causal), int(mode), bool(residual), float(p_drop), bool(training))
-    return _ConvBlockFn.apply(_c(x), v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
-                              bool(causal), int(mode), bool(residual), float(p_drop), bool(training))
+                                    bool(causal), int(mode), bool(residual), float(p_drop), bool(training), extent)
+    x = _fp32_extent_in(_c(x), k, extent)
+    y = _ConvBlockFn.apply(x, v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
+                           bool(causal), int(mode), bool(residual), float(p_drop), bool(training))
+    return extent_grad_mask(y, extent)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -617,11 +646,16 @@ class _Conv1dFn(torch.autograd.Function):
         return dx, dv, dg, dbias, None, None, None, None
 
 
-def conv1d(x, v, g, bias, k=1, dilation=1, causal=False, relu=False):
-    """Weight-normed Conv1d with 'same' (or causal) padding, optional fused ReLU.  x (B,Cin,T)."""
+def conv1d(x, v, g, bias, k=1, dilation=1, causal=False, relu=False, extent=None):
+    """Weight-normed Conv1d with 'same' (or causal) padding, optional fused ReLU.  x (B,Cin,T).  extent: as
+    ``convblock``."""
+    if causal:
+        extent = None
     if _use_tc_conv(x, v.shape[1], v.shape[0], k):
-        return _Conv1dTCFn.apply(_c(x), v, g, bias, int(k), int(dilation), bool(causal), bool(relu))
-    return _Conv1dFn.apply(_c(x), v, g, bias, int(k), int(dilation), bool(causal), bool(relu))
+        return _Conv1dTCFn.apply(_c(x), v, g, bias, int(k), int(dilation), bool(causal), bool(relu), extent)
+    y = _Conv1dFn.apply(_fp32_extent_in(_c(x), k, extent), v, g, bias, int(k), int(dilation), bool(causal),
+                        bool(relu))
+    return extent_grad_mask(y, extent)
 
 
 # ----------------------------------------------------------------------------------------------
@@ -814,10 +848,12 @@ class _ConvT2Fn(torch.autograd.Function):
         return dx, dv, dg, dbias
 
 
-def conv_transpose1d_k2s2(x, v, g, bias):
+def conv_transpose1d_k2s2(x, v, g, bias, extent=None):
+    """extent: of x's time axis; the incoming gradient past it (2x in output frames) is taken as 0."""
     if _use_tc_conv(x, v.shape[0], 2 * v.shape[1], 1):
-        return _ConvT2TCFn.apply(_c(x), v, g, bias)
-    return _ConvT2Fn.apply(_c(x), v, g, bias)
+        return _ConvT2TCFn.apply(_c(x), v, g, bias, extent)
+    y = _ConvT2Fn.apply(_c(x), v, g, bias)
+    return extent_grad_mask(y, None if extent is None else (extent[0], 2 * extent[1]))
 
 
 def linear(x, v, g, bias):
@@ -864,6 +900,128 @@ class length_scope:
         return False
 
 
+# ----------------------------------------------------------------------------------------------
+# logical extents of a training batch padded to a bucket shape
+# ----------------------------------------------------------------------------------------------
+EXT_DEC, EXT_TEXT, EXT_MEL, EXT_LIN = 0, 1, 2, 3    # slots of the int64[4] extents: decoder steps, text positions,
+                                                    # mel frames (= decoder steps * r), linear frames
+_extent = None          # {"ext", "padded", "axis", "keymask"} while an extent scope is active
+
+
+class extent_scope:
+    """``with ops.extent_scope(extents, padded):`` -- the forward of a training batch that was padded past its own
+    longest utterance to a bucket shape (``data.pad_to_bucket``).  ``extents`` is an int64[4] CUDA tensor of the
+    batch's logical sizes (slots EXT_*), ``padded`` the host tuple of the padded sizes in the same slots.  The kernels
+    read the extents from device memory, so one captured CUDA graph serves every batch of its bucket.  Inside:
+
+    * the encoder's and the converter's stacks (whichever container selects the axis with ``extent_axis``) zero the
+      frames t >= mult*extent before each conv whose kernel spans more than one frame, forward and backward
+      (``mask_time``);
+    * attention masks the keys s >= the logical text length and scales its context by the logical Ts*sqrt(1/Ts);
+    * ``train_step.fused_training_loss`` divides its means by the logical sizes and leaves the padding out.
+
+    Works with autograd and under graph capture.  Per-row masking of an inference batch is ``length_scope``."""
+
+    def __init__(self, extents, padded):
+        self.ext, self.padded = extents, tuple(int(v) for v in padded)
+
+    def __enter__(self):
+        global _extent
+        ext = self.ext
+        if _extent is not None or _length_scope is not None:
+            raise RuntimeError("ops.extent_scope does not nest, nor run inside a length_scope")
+        if not (torch.is_tensor(ext) and ext.is_cuda and ext.dtype == torch.int64 and ext.shape == (4,) and
+                ext.is_contiguous()):
+            raise Dv3Error("extent_scope needs a contiguous int64 (4,) CUDA tensor of logical extents")
+        if len(self.padded) != 4:
+            raise Dv3Error("extent_scope needs the 4 padded sizes")
+        _extent = {"ext": ext, "padded": self.padded, "axis": None, "keymask": {}}
+        return self
+
+    def __exit__(self, *exc):
+        global _extent
+        _extent = None
+        return False
+
+
+class extent_axis:
+    """``with ops.extent_axis(EXT_TEXT):`` -- the time axis of the stacks run inside (the encoder on text positions,
+    the converter on mel frames) for the masking of an active ``extent_scope``; a no-op without one.  Stacks run
+    outside an axis (the causal decoder: padded frames come after the valid ones) are not masked."""
+
+    def __init__(self, slot):
+        self.slot = slot
+
+    def __enter__(self):
+        if _extent is not None:
+            self.prev = _extent["axis"]
+            _extent["axis"] = self.slot
+        return self
+
+    def __exit__(self, *exc):
+        if _extent is not None:
+            _extent["axis"] = self.prev
+        return False
+
+
+def _ext_ptr(slot):
+    """Device address of one extent."""
+    ext = _extent["ext"]
+    return ctypes.c_void_p(ext.data_ptr() + slot * ext.element_size())
+
+
+def extent_frames(x):
+    """(device address of the logical extent, mult) of the time axis of a stack activation x (B,C,T) inside an
+    ``extent_scope`` and an ``extent_axis`` (mult = T // padded T: 2 and 4 after the converter's upsamplers), else
+    None.  The conv stacks (``modules.run_conv_stack``) hand it to every layer they run: the tensor-core kernels read
+    it in their operand-split passes, the exact-fp32 path masks with ``dv3_mask_frames``."""
+    if _extent is None or _extent["axis"] is None:
+        return None
+    _chk(x)
+    T, T0 = x.shape[2], _extent["padded"][_extent["axis"]]
+    if T % T0 != 0:
+        raise Dv3Error("x %s does not fit a padded extent of %d frames" % (tuple(x.shape), T0))
+    return _ext_ptr(_extent["axis"]), T // T0
+
+
+class _MaskFramesFn(torch.autograd.Function):
+    """y = x with frames t >= mult*extent zeroed in every row; the mask is its own adjoint.  grad_only: the forward
+    is the identity and only the gradient is masked (what leaves a stack, or enters an exact-fp32 layer's backward,
+    must be 0 past the extent)."""
+
+    @staticmethod
+    def forward(ctx, x, ext_ptr, mult, grad_only):
+        ctx.cfg = (ext_ptr, mult)
+        if grad_only:
+            return x.view_as(x)
+        B, C, T = x.shape
+        y = torch.empty_like(x)
+        lib.call("dv3_mask_frames", _p(x), _p(y), ext_ptr, mult, B, C, T, _stream())
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        ext_ptr, mult = ctx.cfg
+        dy = _c(dy)
+        B, C, T = dy.shape
+        dx = torch.empty_like(dy)
+        lib.call("dv3_mask_frames", _p(dy), _p(dx), ext_ptr, mult, B, C, T, _stream())
+        return dx, None, None, None
+
+
+def extent_grad_mask(x, extent):
+    """x unchanged; its gradient zeroed past the extent (``extent_frames``; None: x itself)."""
+    return x if extent is None else _MaskFramesFn.apply(x, extent[0], extent[1], True)
+
+
+def _fp32_extent_in(x, k, extent):
+    """Exact-fp32 layer inside an extent scope: the input of a conv spanning more than one frame is masked (forward and
+    backward); the tensor-core Functions do the same inside their operand splits."""
+    if extent is None or k <= 1:
+        return x
+    return _MaskFramesFn.apply(x, extent[0], extent[1], False)
+
+
 def mask_time(x):
     """x (B,C,T) -> a new tensor with frames t >= mult*lengths[b] zeroed (mult = T // T_scope); x itself when no
     length scope is active.  Never writes into x."""
@@ -883,14 +1041,19 @@ def mask_time(x):
 # ----------------------------------------------------------------------------------------------
 # attention core (channel-major): q (B,E,Td), k (B,E,Ts), v (B,E,Ts) -> out (B,E,Td), probs (B,Td,Ts)
 # ----------------------------------------------------------------------------------------------
-def _bgemm(A, sA, Bm, sB, C, sCb, ldc, batch, M, N, K, alpha=1.0, accumulate=False):
+def _bgemm(A, sA, Bm, sB, C, sCb, ldc, batch, M, N, K, alpha=1.0, accumulate=False, ts_ptr=None):
+    """ts_ptr (device address of a key count): alpha = Ts*sqrt(1/Ts) of that count instead of ``alpha``."""
+    if ts_ptr is not None:
+        lib.call("dv3_bgemm_ctx_scale", _p(A), sA[0], sA[1], sA[2], _p(Bm), sB[0], sB[1], sB[2], _p(C), sCb, ldc,
+                 batch, M, N, K, ts_ptr, int(accumulate), _stream())
+        return
     lib.call("dv3_bgemm", _p(A), sA[0], sA[1], sA[2], _p(Bm), sB[0], sB[1], sB[2], _p(C), sCb, ldc, batch, M, N,
              K, float(alpha), int(accumulate), _stream())
 
 
 class _AttentionCoreFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, mask, p_drop, training):
+    def forward(ctx, q, k, v, mask, p_drop, training, ts_ptr):
         _chk(q, k, v)
         B, E, Td = q.shape
         Ts = k.shape[2]
@@ -908,9 +1071,9 @@ class _AttentionCoreFn(torch.autograd.Function):
         scale = Ts * (1.0 / Ts) ** 0.5                         # deepvoice3.py:170-171
         out = torch.empty(B, E, Td, device=dev, dtype=torch.float32)
         # O[e,t] = scale * sum_s v[e,s] pd[t,s]
-        _bgemm(v, (E * Ts, Ts, 1), pv, (Td * Ts, 1, Ts), out, E * Td, Td, B, E, Td, Ts, alpha=scale)
+        _bgemm(v, (E * Ts, Ts, 1), pv, (Td * Ts, 1, Ts), out, E * Td, Td, B, E, Td, Ts, alpha=scale, ts_ptr=ts_ptr)
         ctx.save_for_backward(q, k, v, probs, pd)
-        ctx.cfg = (p, salt, scale)
+        ctx.cfg = (p, salt, scale, ts_ptr)
         ctx.seed_t = seed_t
         ctx.mark_non_differentiable()
         return out, probs
@@ -918,7 +1081,7 @@ class _AttentionCoreFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout, dprobs_ext):
         q, k, v, probs, pd = ctx.saved_tensors
-        p, salt, scale = ctx.cfg
+        p, salt, scale, ts_ptr = ctx.cfg
         B, E, Td = q.shape
         Ts = k.shape[2]
         dev = q.device
@@ -927,10 +1090,10 @@ class _AttentionCoreFn(torch.autograd.Function):
         pv = pd if pd is not None else probs
         # dPd[t,s] = scale * sum_e dO[e,t] v[e,s]
         dpd = torch.empty(B, Td, Ts, device=dev, dtype=torch.float32)
-        _bgemm(dout, (E * Td, 1, Td), v, (E * Ts, Ts, 1), dpd, Td * Ts, Ts, B, Td, Ts, E, alpha=scale)
+        _bgemm(dout, (E * Td, 1, Td), v, (E * Ts, Ts, 1), dpd, Td * Ts, Ts, B, Td, Ts, E, alpha=scale, ts_ptr=ts_ptr)
         # dV[e,s] = scale * sum_t dO[e,t] pd[t,s]
         dv = torch.empty_like(v)
-        _bgemm(dout, (E * Td, Td, 1), pv, (Td * Ts, Ts, 1), dv, E * Ts, Ts, B, E, Ts, Td, alpha=scale)
+        _bgemm(dout, (E * Td, Td, 1), pv, (Td * Ts, Ts, 1), dv, E * Ts, Ts, B, E, Ts, Td, alpha=scale, ts_ptr=ts_ptr)
         ds = torch.empty_like(dpd)
         dpe = _c(dprobs_ext) if dprobs_ext is not None else None
         lib.call("dv3_softmax_bwd", _p(probs), _p(dpd), _p(dpe), _p(ds), B * Td, Ts, p, seed_ptr, salt, _stream())
@@ -939,7 +1102,7 @@ class _AttentionCoreFn(torch.autograd.Function):
         _bgemm(k, (E * Ts, Ts, 1), ds, (Td * Ts, 1, Ts), dq, E * Td, Td, B, E, Td, Ts)
         dk = torch.empty_like(k)
         _bgemm(q, (E * Td, Td, 1), ds, (Td * Ts, Ts, 1), dk, E * Ts, Ts, B, E, Ts, Td)
-        return dq, dk, dv, None, None, None
+        return dq, dk, dv, None, None, None, None
 
 
 tc_attention = os.environ.get("DV3_TC_ATTN", "1") == "1"      # 0: attention on the exact-fp32 bgemm + softmax kernels
@@ -949,7 +1112,7 @@ class _AttentionTCFn(torch.autograd.Function):
     """The same contract on the fused tensor-core kernels (csrc/tc_attn.cu): one launch forward, two backward."""
 
     @staticmethod
-    def forward(ctx, q, k, v, mask, p_drop, training):
+    def forward(ctx, q, k, v, mask, p_drop, training, ts_ptr):
         _chk(q, k, v)
         B, E, Td = q.shape
         Ts = k.shape[2]
@@ -958,17 +1121,21 @@ class _AttentionTCFn(torch.autograd.Function):
         scale = Ts * (1.0 / Ts) ** 0.5                         # deepvoice3.py:170-171
         probs = torch.empty(B, Td, Ts, device=dev, dtype=torch.float32)
         out = torch.empty(B, E, Td, device=dev, dtype=torch.float32)
-        lib.call("dv3_tc_attn_fwd", _p(q), _p(k), _p(v), _p(mask), _p(probs), _p(out), B, E, Td, Ts, scale, p,
-                 _p(seed_t), salt, _stream())
+        if ts_ptr is not None:
+            lib.call("dv3_tc_attn_fwd_ext", _p(q), _p(k), _p(v), _p(mask), _p(probs), _p(out), B, E, Td, Ts, ts_ptr,
+                     p, _p(seed_t), salt, _stream())
+        else:
+            lib.call("dv3_tc_attn_fwd", _p(q), _p(k), _p(v), _p(mask), _p(probs), _p(out), B, E, Td, Ts, scale, p,
+                     _p(seed_t), salt, _stream())
         ctx.save_for_backward(q, k, v, probs)
-        ctx.cfg = (p, salt, scale)
+        ctx.cfg = (p, salt, scale, ts_ptr)
         ctx.seed_t = seed_t
         return out, probs
 
     @staticmethod
     def backward(ctx, dout, dprobs_ext):
         q, k, v, probs = ctx.saved_tensors
-        p, salt, scale = ctx.cfg
+        p, salt, scale, ts_ptr = ctx.cfg
         B, E, Td = q.shape
         Ts = k.shape[2]
         dev = q.device
@@ -976,17 +1143,38 @@ class _AttentionTCFn(torch.autograd.Function):
         dpe = _c(dprobs_ext) if dprobs_ext is not None else None
         ds = torch.empty(B, Td, Ts, device=dev, dtype=torch.float32)
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        lib.call("dv3_tc_attn_bwd", _p(dout), _p(q), _p(k), _p(v), _p(probs), _p(dpe), _p(ds), _p(dq), _p(dk), _p(dv),
-                 B, E, Td, Ts, scale, p, _p(ctx.seed_t), salt, _stream())
-        return dq, dk, dv, None, None, None
+        if ts_ptr is not None:
+            lib.call("dv3_tc_attn_bwd_ext", _p(dout), _p(q), _p(k), _p(v), _p(probs), _p(dpe), _p(ds), _p(dq), _p(dk),
+                     _p(dv), B, E, Td, Ts, ts_ptr, p, _p(ctx.seed_t), salt, _stream())
+        else:
+            lib.call("dv3_tc_attn_bwd", _p(dout), _p(q), _p(k), _p(v), _p(probs), _p(dpe), _p(ds), _p(dq), _p(dk),
+                     _p(dv), B, E, Td, Ts, scale, p, _p(ctx.seed_t), salt, _stream())
+        return dq, dk, dv, None, None, None, None
+
+
+def _extent_key_mask(B, Ts, device):
+    """(B, Ts) uint8, 1 at keys s >= the logical text length of the active extent scope (built once per scope)."""
+    km = _extent["keymask"].get((B, Ts))
+    if km is None:
+        ext = _extent["ext"]
+        s = torch.arange(Ts, device=device)
+        km = (s[None, :] >= ext[EXT_TEXT:EXT_TEXT + 1]).to(torch.uint8).expand(B, Ts).contiguous()
+        _extent["keymask"][(B, Ts)] = km
+    return km
 
 
 def attention_core(q, k, v, mask=None, p_drop=0.0, training=False):
-    """mask: (B, Ts) uint8/bool, 1 = padding.  Returns (out (B,E,Td), probs (B,Td,Ts))."""
+    """mask: (B, Ts) uint8/bool, 1 = padding.  Returns (out (B,E,Td), probs (B,Td,Ts)).  Inside an
+    ``extent_scope`` the keys past the logical text length are masked too and the context scale is the logical one."""
     if mask is not None:
         mask = mask.to(torch.uint8).contiguous()
     B, E, Td = q.shape
+    ts_ptr = None
+    if _extent is not None:
+        km = _extent_key_mask(B, k.shape[2], k.device)
+        mask = km if mask is None else (mask | km)
+        ts_ptr = _ext_ptr(EXT_TEXT)
     tc = (_tc_selected() and tc_attention and q.is_cuda and
           lib.raw("dv3_tc_attn_supported")(B, E, Td, k.shape[2]))
     fn = _AttentionTCFn if tc else _AttentionCoreFn
-    return fn.apply(_c(q), _c(k), _c(v), mask, float(p_drop), bool(training))
+    return fn.apply(_c(q), _c(k), _c(v), mask, float(p_drop), bool(training), ts_ptr)

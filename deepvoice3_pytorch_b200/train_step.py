@@ -13,16 +13,18 @@ backward, ``clip_grad_norm_``, ``Adam.step`` -- restated around three ideas:
   once in a CUDA graph and replayed, which removes the ~1.5 k kernel-launch / autograd dispatch overhead that
   dominates once the convolutions run on tensor cores.
 """
+import contextlib
 import ctypes
 import math
 import os
+import time
 
 import numpy as np
 import torch
 import torch.distributed as dist
 import torch.nn.functional as F
 
-from . import ops
+from . import data, ops
 from ._lib import lib
 from .weight_bank import WeightBank
 
@@ -89,6 +91,8 @@ def training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, b
                   guided_attention_sigma=0.2, use_guided_attention=True, priority_freq=3000, priority_freq_weight=0.0,
                   sample_rate=22050):
     """Total loss of one step with seq2seq and postnet trained jointly (reference train.py:665-740)."""
+    if batch.get("extents") is not None:
+        raise ValueError("training_loss does not take a batch padded to a bucket (extents): use fused_training_loss")
     mel_out, lin_out, attn, done_hat = outs
     mel, y, done = batch["mel"], batch["y"], batch["done"]
     tl = batch["target_lengths"]
@@ -117,7 +121,7 @@ class _FusedLossFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, mel_out, lin_out, attn, done_hat, mel, y, done, target_lengths, input_lengths, r,
-                downsample_step, w, bw, sigma, use_attn, pbin, pw):
+                downsample_step, w, bw, sigma, use_attn, pbin, pw, ext):
         dev = mel_out.device
         vp = lambda t: ctypes.c_void_p(t.data_ptr())
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -127,36 +131,53 @@ class _FusedLossFn(torch.autograd.Function):
         g_attn, g_done = torch.empty_like(attn), torch.empty_like(done_hat)
         dec_len = (target_lengths // (r * downsample_step)).contiguous()
         B, Td, Dm = mel_out.shape
-        lib.call("dv3_spec_loss", vp(mel_out), vp(mel.contiguous()), vp(dec_len), vp(g_mel), vp(loss), B, Td, Dm, r,
-                 float(w), float(bw), 0, 0.0, st)
         _, Tl, Dl = lin_out.shape
         lin_len = target_lengths.contiguous() if downsample_step > 1 else dec_len
-        lib.call("dv3_spec_loss", vp(lin_out), vp(y.contiguous()), vp(lin_len), vp(g_lin), vp(loss), B, Tl, Dl, r,
-                 float(w), float(bw), int(pbin), float(pw), st)
         A, _, _, Ts = attn.shape
         dec_len_attn = (target_lengths // r // downsample_step).contiguous()
-        lib.call("dv3_aux_loss", vp(done_hat), vp(done.contiguous()), vp(g_done), done_hat.numel(), vp(attn),
-                 vp(g_attn), vp(input_lengths.contiguous()), vp(dec_len_attn), A, B, attn.shape[2], Ts, float(sigma),
-                 int(use_attn), vp(loss), st)
+        if ext is None:
+            lib.call("dv3_spec_loss", vp(mel_out), vp(mel.contiguous()), vp(dec_len), vp(g_mel), vp(loss), B, Td, Dm,
+                     r, float(w), float(bw), 0, 0.0, st)
+            lib.call("dv3_spec_loss", vp(lin_out), vp(y.contiguous()), vp(lin_len), vp(g_lin), vp(loss), B, Tl, Dl,
+                     r, float(w), float(bw), int(pbin), float(pw), st)
+            lib.call("dv3_aux_loss", vp(done_hat), vp(done.contiguous()), vp(g_done), done_hat.numel(), vp(attn),
+                     vp(g_attn), vp(input_lengths.contiguous()), vp(dec_len_attn), A, B, attn.shape[2], Ts,
+                     float(sigma), int(use_attn), vp(loss), st)
+        else:                   # a batch padded to a bucket: the kernels read the logical extents (ops.EXT_* slots)
+            at = lambda slot: ctypes.c_void_p(ext.data_ptr() + 8 * slot)
+            lib.call("dv3_spec_loss_ext", vp(mel_out), vp(mel.contiguous()), vp(dec_len), at(ops.EXT_MEL), vp(g_mel),
+                     vp(loss), B, Td, Dm, r, float(w), float(bw), 0, 0.0, st)
+            lib.call("dv3_spec_loss_ext", vp(lin_out), vp(y.contiguous()), vp(lin_len),
+                     at(ops.EXT_LIN if downsample_step > 1 else ops.EXT_MEL), vp(g_lin), vp(loss), B, Tl, Dl, r,
+                     float(w), float(bw), int(pbin), float(pw), st)
+            assert done_hat.numel() == B * attn.shape[2] and ops.EXT_TEXT == ops.EXT_DEC + 1
+            lib.call("dv3_aux_loss_ext", vp(done_hat), vp(done.contiguous()), vp(g_done), vp(attn), vp(g_attn),
+                     vp(input_lengths.contiguous()), vp(dec_len_attn), at(ops.EXT_DEC), A, B, attn.shape[2], Ts,
+                     float(sigma), int(use_attn), vp(loss), st)
         ctx.save_for_backward(g_mel, g_lin, g_attn, g_done)
         return loss[0]
 
     @staticmethod
     def backward(ctx, gout):
         g_mel, g_lin, g_attn, g_done = ctx.saved_tensors
-        return (g_mel * gout, g_lin * gout, g_attn * gout, g_done * gout) + (None,) * 13
+        return (g_mel * gout, g_lin * gout, g_attn * gout, g_done * gout) + (None,) * 14
 
 
 def fused_training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, binary_divergence_weight=0.1,
                         guided_attention_sigma=0.2, use_guided_attention=True, priority_freq=3000,
                         priority_freq_weight=0.0, sample_rate=22050):
-    """Same value and gradients as ``training_loss`` (reference train.py:665-740), computed by csrc/loss.cu."""
+    """Same value and gradients as ``training_loss`` (reference train.py:665-740), computed by csrc/loss.cu.  A batch
+    padded to a bucket (``data.pad_to_bucket``: it carries ``extents``) gives the loss and gradients of the unpadded
+    batch: the padding leaves every mean and its gradient is 0."""
     mel_out, lin_out, attn, done_hat = outs
+    ext = batch.get("extents")
+    if ext is not None and not (ext.is_cuda and ext.dtype == torch.int64 and ext.shape == (4,) and ext.is_contiguous()):
+        raise ValueError("batch['extents'] must be a contiguous int64 (4,) CUDA tensor")
     return _FusedLossFn.apply(mel_out, lin_out, attn, done_hat, batch["mel"], batch["y"], batch["done"],
                               batch["target_lengths"], batch["input_lengths_dev"], r, downsample_step,
                               masked_loss_weight, binary_divergence_weight, guided_attention_sigma,
                               use_guided_attention, priority_bin_of(priority_freq, sample_rate, lin_out.size(-1)),
-                              priority_freq_weight)
+                              priority_freq_weight, ext)
 
 
 class ParameterArena:
@@ -367,6 +388,12 @@ class TrainStep:
         self._static = None
         self._loss = None
         self.launches_per_step = None       # dv3 kernel launches inside one captured step (graph mode)
+        # graph mode with batches of other shapes than the first: one graph per bucket (data.bucket_shape), all in
+        # one memory pool; the first shape keeps its own exact graph
+        self._pool = None
+        self._graph_key = None
+        self._buckets = {}                  # bucket key -> (graph, static inputs, loss buffer, launches)
+        self.capture_seconds = 0.0          # wall time spent warming up and capturing graphs
         if weight_bank is None:
             weight_bank = os.environ.get("DV3_WEIGHT_BANK", "1") == "1"
         self.bank = WeightBank() if weight_bank else None
@@ -428,10 +455,13 @@ class TrainStep:
             self.arena.all_reduce_grads([rng])
 
     def _forward_backward_inner(self, batch):
-        outs = self.model(batch["x"], batch["mel"], speaker_ids=batch.get("speaker_ids"),
-                          text_positions=batch["text_positions"], frame_positions=batch["frame_positions"],
-                          input_lengths=batch["input_lengths_dev"])
-        loss = self.loss_fn(outs, batch, **self.loss_kw)
+        ext = batch.get("extents")          # a batch padded to a bucket (data.pad_to_bucket)
+        scope = ops.extent_scope(ext, data.batch_extents(batch)) if ext is not None else contextlib.nullcontext()
+        with scope:
+            outs = self.model(batch["x"], batch["mel"], speaker_ids=batch.get("speaker_ids"),
+                              text_positions=batch["text_positions"], frame_positions=batch["frame_positions"],
+                              input_lengths=batch["input_lengths_dev"])
+            loss = self.loss_fn(outs, batch, **self.loss_kw)
         loss.backward()
         if self.bank is not None:
             self.bank.end_backward()
@@ -451,9 +481,18 @@ class TrainStep:
         self.opt.apply()          # (fresh dropout masks per step: the model's forward draws a new seed itself)
 
     # -- public -------------------------------------------------------------------------------
+    @property
+    def graphs_captured(self):
+        return (self._graph is not None) + len(self._buckets)
+
     def step(self, batch):
         """batch: dict of DEVICE tensors (x, text_positions, frame_positions int64; mel, y, done fp32;
-        target_lengths, input_lengths_dev int64) + host numpy ``input_lengths``.  Returns the loss (device)."""
+        target_lengths, input_lengths_dev int64) + host numpy ``input_lengths``.  Returns the loss (device).
+
+        Batches may differ in shape from step to step (``data.collate`` pads each to its own longest utterance).  In
+        graph mode the first shape runs its own exact graph; any other is padded to its bucket (``data.bucket_shape``,
+        ``data.pad_to_bucket``) and replays that bucket's graph, with the loss, gradients and update of the unpadded
+        batch.  A batch that already carries ``extents`` is its own bucket."""
         self.model.train()
         lr = self.lr_schedule(self.init_lr, self.global_step) if self.lr_schedule else self.init_lr
         self.opt.set_hyper(lr, 1.0 / self.world)
@@ -465,35 +504,94 @@ class TrainStep:
         self.global_step += 1
         return loss
 
+    def _shape_key(self, batch):
+        return tuple((k, tuple(v.shape)) for k, v in sorted(batch.items()) if torch.is_tensor(v))
+
+    def _warm_up(self, static):
+        """Two eager passes on a side stream before a capture (allocator, NCCL, weight-bank tables); they do not
+        consume dropout seeds."""
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            dev = self.arena.flat.device
+            ops.rng.seed_tensor(dev)
+            seed0 = ops.rng.base.clone()
+            for _ in range(2):
+                self._forward_backward(static)
+                if self.world > 1 and self.overlap_comm:    # NCCL communicators / bucket tables exist before capture
+                    pend = [r for t, r in self.buckets.items() if t not in self._reduced]
+                    with torch.cuda.stream(self._comm):
+                        self._comm.wait_stream(s)
+                        self.arena.all_reduce_grads(pend + self.rest_ranges)
+                    s.wait_stream(self._comm)
+            ops.rng.base.copy_(seed0)           # the warm-up passes do not consume dropout seeds
+        torch.cuda.current_stream().wait_stream(s)
+
+    def _bucket_step(self, batch):
+        """A batch of another shape than the first graph's: pad it to its bucket and replay (capturing on first use)
+        that bucket's graph."""
+        if self.loss_fn is not fused_training_loss:
+            raise ValueError("TrainStep(use_graph=True, fused_loss=False) needs every batch in the shape of the first "
+                             "one: padding to a bucket is supported by the fused loss kernels only")
+        if self.world > 1:
+            raise ValueError("TrainStep(use_graph=True) with world_size > 1 needs every batch in the shape of the "
+                             "first one (pad the batches to one shape, or train in eager mode)")
+        r, ds = self.loss_kw["r"], self.loss_kw["downsample_step"]
+        if batch.get("extents") is not None:                      # already padded by the caller: its own bucket
+            key = ("padded", self._shape_key(batch))
+            shape = None
+        else:
+            ext = data.batch_extents(batch)
+            shape = data.bucket_shape(ext[1], ext[0])
+            key = ("bucket", shape, int(batch["x"].shape[0]), "speaker_ids" in batch)
+        rec = self._buckets.get(key)
+        if rec is None:
+            t0 = time.perf_counter()
+            if shape is None:
+                static = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in batch.items()}
+            else:
+                static = data.pad_to_bucket(batch, shape[0], shape[1], r, ds)
+            out = torch.zeros((), device=self.arena.flat.device)   # outside the graph pool: read after the replay
+            self._warm_up(static)
+            graph = torch.cuda.CUDAGraph()
+            n0 = lib.raw("dv3_launch_count")()
+            with torch.cuda.graph(graph, pool=self._pool):
+                out.copy_(self._forward_backward(static))
+                self._exchange_and_update()
+            rec = self._buckets[key] = (graph, static, out, int(lib.raw("dv3_launch_count")() - n0))
+            torch.cuda.synchronize()
+            self.capture_seconds += time.perf_counter() - t0
+        graph, static, out, _ = rec
+        if shape is None:
+            for k, v in batch.items():
+                if torch.is_tensor(v):
+                    static[k].copy_(v, non_blocking=True)
+        else:
+            data.pad_to_bucket(batch, shape[0], shape[1], r, ds, out=static)
+        graph.replay()
+        return out
+
     def _graph_step(self, batch):
+        if self._graph is not None and self._shape_key(batch) != self._graph_key:
+            return self._bucket_step(batch)
         if self._graph is None:
+            t0 = time.perf_counter()
+            self._pool = torch.cuda.graph_pool_handle()
+            self._graph_key = self._shape_key(batch)
             # static input buffers; warm up on a side stream, then capture forward+loss+backward (+update when
             # there is no collective to run in between)
             self._static = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in batch.items()}
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                dev = self.arena.flat.device
-                ops.rng.seed_tensor(dev)
-                seed0 = ops.rng.base.clone()
-                for _ in range(2):
-                    self._forward_backward(self._static)
-                    if self.world > 1 and self.overlap_comm:    # NCCL communicators / bucket tables exist before capture
-                        pend = [r for t, r in self.buckets.items() if t not in self._reduced]
-                        with torch.cuda.stream(self._comm):
-                            self._comm.wait_stream(s)
-                            self.arena.all_reduce_grads(pend + self.rest_ranges)
-                        s.wait_stream(self._comm)
-                ops.rng.base.copy_(seed0)           # the warm-up passes do not consume dropout seeds
-            torch.cuda.current_stream().wait_stream(s)
+            self._warm_up(self._static)
             self._graph = torch.cuda.CUDAGraph()
             n0 = lib.raw("dv3_launch_count")()
             capture_all = self.world == 1 or self.graph_comm
-            with torch.cuda.graph(self._graph):
+            with torch.cuda.graph(self._graph, pool=self._pool):
                 self._loss = self._forward_backward(self._static)
                 if capture_all:                     # NCCL all-reduces are captured as graph nodes on the comm stream
                     self._exchange_and_update()
             self.launches_per_step = int(lib.raw("dv3_launch_count")() - n0) + (0 if capture_all else 2)
+            torch.cuda.synchronize()
+            self.capture_seconds += time.perf_counter() - t0
         for k, v in batch.items():
             if torch.is_tensor(v):
                 self._static[k].copy_(v, non_blocking=True)

@@ -24,7 +24,8 @@ class AttentionSeq2Seq(nn.Module):
         # forward is drawn by whichever container is outermost (ops.DropoutState.begin_forward)
         ops.rng.begin_forward(self.training, text_sequences.device)
         try:
-            memory = self.encoder(text_sequences, lengths=input_lengths, speaker_embed=speaker_embed)
+            with ops.extent_axis(ops.EXT_TEXT):             # masks the padding of a bucketed batch (ops.extent_scope)
+                memory = self.encoder(text_sequences, lengths=input_lengths, speaker_embed=speaker_embed)
             # -> mel (B, T//r, mel_dim*r), alignments (N, B, T_dec, T_text), done (B, T//r, 1), decoder states
             return self.decoder(memory, mel_targets, text_positions=text_positions,
                                 frame_positions=frame_positions, speaker_embed=speaker_embed, lengths=input_lengths)
@@ -93,7 +94,8 @@ class MultiSpeakerTTSModel(nn.Module):
             mel = mel.reshape(batch, -1, self.mel_dim)    # un-group the r frames per decoder step
             post_in = states.reshape(batch, mel.size(1), -1) if self.use_decoder_state_for_postnet_input else mel
             post_in = ops.grad_boundary(post_in, "postnet")     # its gradient ready <=> the postnet's backward is done
-            linear = self.postnet(post_in, spk)
+            with ops.extent_axis(ops.EXT_MEL):
+                linear = self.postnet(post_in, spk)
             assert linear.size(-1) == self.linear_dim
             return mel, linear, alignments, done
         finally:

@@ -46,6 +46,7 @@ class _Layer:
         self.wbwd = torch.empty(2, k, Cin, _pad8(Cout), device=dev, dtype=bf)
         self.partials = None
         self.nsplit = 0
+        self.partials_by_shape = {}      # (nsplit, numel) -> buffer: graphs captured at other shapes keep theirs
         self.prepared = False
         self.pending = False
 
@@ -120,9 +121,12 @@ class WeightBank:
         if not self.active or L.pending or L.v.grad is None or L.g.grad is None:
             return None
         if L.partials is None or L.nsplit != nsplit or L.partials.shape[1] != numel:
-            if torch.cuda.is_current_stream_capturing():
-                return None
-            L.partials = torch.empty(nsplit, numel, device=L.v.device)
+            buf = L.partials_by_shape.get((nsplit, numel))
+            if buf is None:
+                if torch.cuda.is_current_stream_capturing():
+                    return None
+                buf = L.partials_by_shape[(nsplit, numel)] = torch.empty(nsplit, numel, device=L.v.device)
+            L.partials = buf
             L.nsplit = nsplit
         L.pending = True
         return L.partials

@@ -119,6 +119,9 @@ int dv3_interleave2(const float* in, float* out, int B, int C, int T, int invers
  * x, y (B,C,T); x == y allowed; lengths int64 [B] on the device.  Zeroing a row's frames past its end before every
  * conv that mixes time steps makes each row see exactly the zero padding it would see alone. */
 int dv3_mask_time(const float* x, float* y, const long long* lengths, int mult, int B, int C, int T, void* stream);
+/* y = x with y[b,:,t] = 0 for t >= mult * extent[0] in every row: the logical time extent (int64 in device memory) of a
+ * training batch padded to a bucket shape.  The mask is its own adjoint: the same call is its backward. */
+int dv3_mask_frames(const float* x, float* y, const long long* extent, int mult, int B, int C, int T, void* stream);
 
 /* ---- batched strided GEMM C[b] = alpha*A_b*B_b (+C): the attention contractions, reference
  * deepvoice3.py:143 (bmm(q,k)), :167 (bmm(p,v)) and their gradients.  A_b(m,k)=A[b*sAb+m*sAm+k*sAk],
@@ -126,6 +129,10 @@ int dv3_mask_time(const float* x, float* y, const long long* lengths, int mult, 
 int dv3_bgemm(const float* A, long long sAb, long long sAm, long long sAk, const float* B, long long sBb,
               long long sBk, long long sBn, float* C, long long sCb, int ldc, int batch, int M, int N, int K,
               float alpha, int accumulate, void* stream);
+/* the same with alpha = Ts*sqrt(1/Ts), the attention context scale, of the key count ts_log[0] in device memory */
+int dv3_bgemm_ctx_scale(const float* A, long long sAb, long long sAm, long long sAk, const float* B, long long sBb,
+                        long long sBk, long long sBn, float* C, long long sCb, int ldc, int batch, int M, int N, int K,
+                        const long long* ts_log, int accumulate, void* stream);
 
 /* ---- fused tensor-core attention (wgmma, split-bf16 operands staged and split in-kernel): reference
  * deepvoice3.py:132-176 between the projections.  q (B,E,Td), k / v (B,E,Ts), mask (B,Ts) bytes (1 = padding) or
@@ -140,6 +147,14 @@ int dv3_tc_attn_fwd(const float* q, const float* k, const float* v, const unsign
 int dv3_tc_attn_bwd(const float* dout, const float* q, const float* k, const float* v, const float* probs,
                     const float* dprobs, float* ds, float* dq, float* dk, float* dv, int B, int E, int Td, int Ts,
                     float scale, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream);
+/* the same with scale = Ts*sqrt(1/Ts) of the logical key count ts_log[0] in device memory (a padded bucket batch) */
+int dv3_tc_attn_fwd_ext(const float* q, const float* k, const float* v, const unsigned char* mask, float* probs,
+                        float* out, int B, int E, int Td, int Ts, const long long* ts_log, float p_drop,
+                        const unsigned long long* seed_ptr, unsigned salt, void* stream);
+int dv3_tc_attn_bwd_ext(const float* dout, const float* q, const float* k, const float* v, const float* probs,
+                        const float* dprobs, float* ds, float* dq, float* dk, float* dv, int B, int E, int Td, int Ts,
+                        const long long* ts_log, float p_drop, const unsigned long long* seed_ptr, unsigned salt,
+                        void* stream);
 
 /* ---- optimizer step over a flat fp32 arena: reference train.py:756-759 (clip_grad_norm_ + Adam.step).
  * dv3_sumsq: out[0] = sum(x^2), deterministic (per-block partials in `scratch`, summed in index order by the block
@@ -212,6 +227,17 @@ int dv3_tc_gate_bwd_split(const float* dy, const float* a, const float* s, const
 /* plain-conv backward prologue: g = dy*(relu ? y>0 : 1) -> btc: [2][B][T][Cp], bct: [2][B][C][T]; dbias[C] += sums. */
 int dv3_tc_grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
                       int relu, void* stream);
+/* The three splits with an optional logical time extent in device memory (a training batch padded to a bucket):
+ * tlen NULL = the calls above; else frames t >= tmult * tlen[0] of x (forward operand) / of dy (gradient) are taken as
+ * 0: the extent time mask and its gradient, folded into passes that read those tensors anyway. */
+int dv3_tc_split_input_ext(const float* x, void* btc, int npl, void* bct, int B, int C, int T, float p_drop,
+                           const unsigned long long* seed_ptr, unsigned salt, const long long* tlen, int tmult,
+                           void* stream);
+int dv3_tc_gate_bwd_split_ext(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
+                              float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
+                              int tmult, void* stream);
+int dv3_tc_grad_split_ext(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
+                          int relu, const long long* tlen, int tmult, void* stream);
 /* weight norm + split: v (Cout,Cin,k), g [Cout] -> wfwd: [npl][k][Cout][Cinp] (forward), wbwd: [2][k][Cin][Coutp] (dgrad). */
 int dv3_tc_weightnorm_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
                           void* wbwd, int Cout, int Cin, int k, void* stream);
@@ -268,6 +294,16 @@ int dv3_spec_loss(const float* y_hat, const float* y, const long long* lengths, 
 int dv3_aux_loss(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
                  float* d_attn, const long long* in_len, const long long* dec_len, int A, int B, int Td, int Ts,
                  float sigma, int use_attn, float* loss, void* stream);
+/* Extent variants for a batch padded to a bucket shape (logical extents in device memory, read by the kernels):
+ * dv3_spec_loss_ext: pairs t >= t_log[0] - r leave the loss and the means (which divide by B*(t_log-r)*D);
+ * dv3_aux_loss_ext: done_hat / done are (B, Td); ext = {decoder steps, text positions}: steps >= ext[0] and text
+ * positions >= ext[1] leave both means (B*ext[0] and A*B*ext[0]*ext[1]).  Gradients there are written as 0. */
+int dv3_spec_loss_ext(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
+                      float* grad, float* loss, int B, int T, int D, int r, float masked_loss_weight,
+                      float binary_divergence_weight, int priority_bin, float priority_weight, void* stream);
+int dv3_aux_loss_ext(const float* done_hat, const float* done, float* d_done, const float* attn, float* d_attn,
+                     const long long* in_len, const long long* dec_len, const long long* ext, int A, int B, int Td,
+                     int Ts, float sigma, int use_attn, float* loss, void* stream);
 
 /* ---- incremental (autoregressive) decoding: reference conv.py:17-46, deepvoice3.py:367-485, nyanko.py:250-338 ----
  * All loop state lives in device memory so that one decoder step is the same launch sequence every time (CUDA-graph
