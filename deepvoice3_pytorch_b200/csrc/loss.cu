@@ -28,10 +28,13 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 //   coef1 = (1-pw)*coef + [d < pbin]*pw*coef*(D/pbin)     (the same masked/plain means over the pbin-wide slice)
 // t_log (int64 in device memory, or null = T): the logical time extent of a batch padded to a larger bucket.  Pairs
 // t >= t_log - r are left out of the loss and its means, and their gradient is written as 0.
+// TERMS: also add the two parts of the loss to terms[0] (the L1 part, priority bins combined) and terms[1] (the
+// binary-divergence part) -- the l1_loss / binary_div pair reference spec_loss returns.  loss and grad are unchanged.
+template <bool TERMS>
 __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* __restrict__ y,
                                  const long long* __restrict__ lengths, const long long* __restrict__ t_log,
                                  float* __restrict__ grad, float* __restrict__ loss, int B, int T, int D, int r,
-                                 float w, float bw, float eps, int pbin, float pw) {
+                                 float w, float bw, float eps, int pbin, float pw, float* __restrict__ terms) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float red[8];
     __shared__ float s_inv_sm;
@@ -53,7 +56,7 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
     const long long shift = (long long)r * D;
     const bool prio = pbin > 0 && pw > 0.f;
     const float prio_gain = prio ? pw * ((float)D / (float)pbin) : 0.f;
-    float acc = 0.f;
+    float acc = 0.f, acc_l1 = 0.f, acc_bd = 0.f;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         const long long bt = i / D;
@@ -68,11 +71,14 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
             if (prio) c1 = (1.f - pw) + ((int)(i - bt * D) < pbin ? prio_gain : 0.f);
             float e = c1 * (1.f - bw) * fabsf(d);
             float de = c1 * (1.f - bw) * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
+            if (TERMS) acc_l1 += coef * (c1 * fabsf(d));
             if (bw > 0.f) {
                 const float L = logf(p + eps) - logf(1.f - p + eps);
                 const float u = expf(L);
-                e += bw * (-tg * L + log1pf(u));
+                const float z = -tg * L + log1pf(u);
+                e += bw * z;
                 de += bw * (u / (1.f + u) - tg) * (1.f / (p + eps) + 1.f / (1.f - p + eps));
+                if (TERMS) acc_bd += coef * z;
             }
             acc += coef * e;
             g = coef * de;
@@ -81,6 +87,12 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
     }
     const float s = block_sum_256(acc, red);
     if (threadIdx.x == 0) atomicAdd(loss, s);
+    if (TERMS) {
+        const float s1 = block_sum_256(acc_l1, red);
+        if (threadIdx.x == 0) atomicAdd(&terms[0], s1);
+        const float s2 = block_sum_256(acc_bd, red);
+        if (threadIdx.x == 0) atomicAdd(&terms[1], s2);
+    }
 }
 
 // done BCE (mean) + guided attention (mean of attn*W):
@@ -88,14 +100,17 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
 // ext (int64 [2] in device memory, or null): logical (decoder steps, text positions) of a batch padded to a larger
 // bucket -- done_hat is then (B, Td); steps >= ext[0] and text positions >= ext[1] are left out of both means and
 // their gradient is written as 0.
+// TERMS: also add the done BCE to terms[0] and the guided-attention term to terms[1].
+template <bool TERMS>
 __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float* __restrict__ done,
                                 float* __restrict__ d_done, long long n_done, const float* __restrict__ attn,
                                 float* __restrict__ d_attn, const long long* __restrict__ in_len,
                                 const long long* __restrict__ dec_len, const long long* __restrict__ ext, int A,
-                                int B, int Td, int Ts, float sigma, int use_attn, float* __restrict__ loss) {
+                                int B, int Td, int Ts, float sigma, int use_attn, float* __restrict__ loss,
+                                float* __restrict__ terms) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float red[8];
-    float acc = 0.f;
+    float acc = 0.f, acc_done = 0.f, acc_attn = 0.f;
     const long long stride = (long long)gridDim.x * blockDim.x, start = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     const int TdL = ext ? (int)min((long long)Td, max(1LL, ext[0])) : Td;
     const int TsL = ext ? (int)min((long long)Ts, max(1LL, ext[1])) : Ts;
@@ -106,6 +121,7 @@ __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float*
         acc -= inv_nd * (t * fmaxf(logf(p), -100.f) + (1.f - t) * fmaxf(logf(1.f - p), -100.f));
         d_done[i] = inv_nd * (p - t) / fmaxf((1.f - p) * p, 1e-12f);
     }
+    if (TERMS) acc_done = acc;
     if (use_attn) {
         const long long n_attn = (long long)A * B * Td * Ts;
         const float inv_na = 1.f / (float)((long long)A * B * TdL * TsL);
@@ -121,6 +137,7 @@ __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float*
                 wv = (float)(1.0 - exp(-q * q * inv2g2));
             }
             acc += inv_na * attn[i] * wv;
+            if (TERMS) acc_attn += inv_na * attn[i] * wv;
             d_attn[i] = inv_na * wv;
         }
     } else if (d_attn) {
@@ -129,6 +146,12 @@ __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float*
     }
     const float s = block_sum_256(acc, red);
     if (threadIdx.x == 0) atomicAdd(loss, s);
+    if (TERMS) {
+        const float s1 = block_sum_256(acc_done, red);
+        if (threadIdx.x == 0) atomicAdd(&terms[0], s1);
+        const float s2 = block_sum_256(acc_attn, red);
+        if (threadIdx.x == 0) atomicAdd(&terms[1], s2);
+    }
 }
 
 }  // namespace dv3
@@ -137,50 +160,66 @@ using namespace dv3;
 
 extern "C" {
 
-int dv3_spec_loss(const float* y_hat, const float* y, const long long* lengths, float* grad, float* loss, int B,
-                  int T, int D, int r, float masked_loss_weight, float binary_divergence_weight, int priority_bin,
-                  float priority_weight, void* stream) {
+int dv3_spec_loss_terms(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
+                        float* grad, float* loss, float* terms, int B, int T, int D, int r, float masked_loss_weight,
+                        float binary_divergence_weight, int priority_bin, float priority_weight, void* stream) {
     DV3_REQUIRE(T > r && r >= 0, "spec_loss: need T > r");
     DV3_REQUIRE(priority_bin >= 0 && priority_bin <= D && priority_weight >= 0.f && priority_weight <= 1.f,
                 "spec_loss: priority_bin=%d (D=%d) priority_weight=%g out of range", priority_bin, D, priority_weight);
     long long blocks = ((long long)B * T * D + 255) / 256;
     if (blocks > 132 * 8) blocks = 132 * 8;
-    launch_k(spec_loss_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths,
-             (const long long*)nullptr, grad, loss, B, T, D, r, masked_loss_weight, binary_divergence_weight, 1e-8f,
-             priority_bin, priority_weight);
+    if (terms)
+        launch_k(spec_loss_kernel<true>, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, t_log, grad,
+                 loss, B, T, D, r, masked_loss_weight, binary_divergence_weight, 1e-8f, priority_bin, priority_weight,
+                 terms);
+    else
+        launch_k(spec_loss_kernel<false>, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, t_log, grad,
+                 loss, B, T, D, r, masked_loss_weight, binary_divergence_weight, 1e-8f, priority_bin, priority_weight,
+                 terms);
     return check_launch("spec_loss");
+}
+
+int dv3_spec_loss(const float* y_hat, const float* y, const long long* lengths, float* grad, float* loss, int B,
+                  int T, int D, int r, float masked_loss_weight, float binary_divergence_weight, int priority_bin,
+                  float priority_weight, void* stream) {
+    return dv3_spec_loss_terms(y_hat, y, lengths, nullptr, grad, loss, nullptr, B, T, D, r, masked_loss_weight,
+                               binary_divergence_weight, priority_bin, priority_weight, stream);
 }
 
 int dv3_spec_loss_ext(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
                       float* grad, float* loss, int B, int T, int D, int r, float masked_loss_weight,
                       float binary_divergence_weight, int priority_bin, float priority_weight, void* stream) {
     DV3_REQUIRE(t_log != nullptr, "spec_loss_ext: t_log is NULL");
-    DV3_REQUIRE(T > r && r >= 0, "spec_loss_ext: need T > r");
-    DV3_REQUIRE(priority_bin >= 0 && priority_bin <= D && priority_weight >= 0.f && priority_weight <= 1.f,
-                "spec_loss_ext: priority_bin=%d (D=%d) priority_weight=%g out of range", priority_bin, D,
-                priority_weight);
-    long long blocks = ((long long)B * T * D + 255) / 256;
-    if (blocks > 132 * 8) blocks = 132 * 8;
-    launch_k(spec_loss_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, t_log, grad, loss, B, T,
-             D, r, masked_loss_weight, binary_divergence_weight, 1e-8f, priority_bin, priority_weight);
-    return check_launch("spec_loss_ext");
+    return dv3_spec_loss_terms(y_hat, y, lengths, t_log, grad, loss, nullptr, B, T, D, r, masked_loss_weight,
+                               binary_divergence_weight, priority_bin, priority_weight, stream);
+}
+
+int dv3_aux_loss_terms(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
+                       float* d_attn, const long long* in_len, const long long* dec_len, const long long* ext, int A,
+                       int B, int Td, int Ts, float sigma, int use_attn, float* loss, float* terms, void* stream) {
+    DV3_REQUIRE(ext == nullptr || n_done == (long long)B * Td, "aux_loss: with extents done_hat must be (B, Td)");
+    if (terms)
+        launch_k(aux_loss_kernel<true>, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done, attn,
+                 d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma, use_attn, loss, terms);
+    else
+        launch_k(aux_loss_kernel<false>, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done, attn,
+                 d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma, use_attn, loss, terms);
+    return check_launch("aux_loss");
 }
 
 int dv3_aux_loss(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
                  float* d_attn, const long long* in_len, const long long* dec_len, int A, int B, int Td, int Ts,
                  float sigma, int use_attn, float* loss, void* stream) {
-    launch_k(aux_loss_kernel, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done, attn, d_attn, in_len,
-             dec_len, (const long long*)nullptr, A, B, Td, Ts, sigma, use_attn, loss);
-    return check_launch("aux_loss");
+    return dv3_aux_loss_terms(done_hat, done, d_done, n_done, attn, d_attn, in_len, dec_len, nullptr, A, B, Td, Ts,
+                              sigma, use_attn, loss, nullptr, stream);
 }
 
 int dv3_aux_loss_ext(const float* done_hat, const float* done, float* d_done, const float* attn, float* d_attn,
                      const long long* in_len, const long long* dec_len, const long long* ext, int A, int B, int Td,
                      int Ts, float sigma, int use_attn, float* loss, void* stream) {
     DV3_REQUIRE(ext != nullptr, "aux_loss_ext: ext is NULL");
-    launch_k(aux_loss_kernel, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, (long long)B * Td, attn,
-             d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma, use_attn, loss);
-    return check_launch("aux_loss_ext");
+    return dv3_aux_loss_terms(done_hat, done, d_done, (long long)B * Td, attn, d_attn, in_len, dec_len, ext, A, B, Td,
+                              Ts, sigma, use_attn, loss, nullptr, stream);
 }
 
 }  // extern "C"

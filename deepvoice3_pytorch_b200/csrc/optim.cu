@@ -63,10 +63,13 @@ __global__ void sumsq_kernel(const float* __restrict__ x, long long n, float* __
 }
 
 // hyper = {lr, bias_correction1, bias_correction2, grad_scale}; sumsq[0] = ||g*grad_scale||^2 before clipping.
+// WD: torch.optim.Adam's L2 weight decay, g' = clipped g + wd*p before the moments.  AMS: AMSGrad, the denominator
+// takes vmax = max(vmax, v).  <false, false> is the plain clip + Adam step.
+template <bool WD, bool AMS>
 __global__ void adam_clip_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                 float* __restrict__ v, long long n, const float* __restrict__ hyper,
-                                 const float* __restrict__ sumsq, float beta1, float beta2, float eps,
-                                 float max_norm) {
+                                 float* __restrict__ v, float* __restrict__ vmax, long long n,
+                                 const float* __restrict__ hyper, const float* __restrict__ sumsq, float beta1,
+                                 float beta2, float eps, float max_norm, float wd) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     const float lr = hyper[0], bc1 = hyper[1], bc2 = hyper[2], gscale = hyper[3];
     float coef = gscale;
@@ -78,11 +81,14 @@ __global__ void adam_clip_kernel(float* __restrict__ p, const float* __restrict_
     const float step = lr / bc1, rs2 = rsqrtf(bc2);
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
          i += (long long)gridDim.x * blockDim.x) {
-        const float gi = g[i] * coef;
+        float gi = g[i] * coef;
+        if (WD) gi += wd * p[i];
         const float mi = beta1 * m[i] + (1.f - beta1) * gi;
         const float vi = beta2 * v[i] + (1.f - beta2) * gi * gi;
         m[i] = mi; v[i] = vi;
-        p[i] -= step * mi / (sqrtf(vi) * rs2 + eps);
+        float vd = vi;
+        if (AMS) { vd = fmaxf(vmax[i], vi); vmax[i] = vd; }
+        p[i] -= step * mi / (sqrtf(vd) * rs2 + eps);
     }
 }
 
@@ -104,14 +110,40 @@ int dv3_sumsq(const float* x, long long n, float* out, float* scratch, void* str
     return check_launch("sumsq");
 }
 
-int dv3_adam_clip(float* p, const float* g, float* m, float* v, long long n, const float* hyper,
-                  const float* sumsq, float beta1, float beta2, float eps, float max_norm, void* stream) {
+static long long adam_blocks(long long n) {
     long long blocks = (n + 255) / 256;
     if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks < 1) blocks = 1;
-    launch_k(adam_clip_kernel, (int)blocks, 256, 0, (cudaStream_t)stream, p, g, m, v, n, hyper, sumsq, beta1, beta2,
-                                                                   eps, max_norm);
+    return blocks;
+}
+
+int dv3_adam_clip(float* p, const float* g, float* m, float* v, long long n, const float* hyper,
+                  const float* sumsq, float beta1, float beta2, float eps, float max_norm, void* stream) {
+    launch_k(adam_clip_kernel<false, false>, (int)adam_blocks(n), 256, 0, (cudaStream_t)stream, p, g, m, v,
+             (float*)nullptr, n, hyper, sumsq, beta1, beta2, eps, max_norm, 0.f);
     return check_launch("adam_clip");
+}
+
+int dv3_adam_clip_opts(float* p, const float* g, float* m, float* v, float* vmax, long long n, const float* hyper,
+                       const float* sumsq, float beta1, float beta2, float eps, float max_norm, float weight_decay,
+                       void* stream) {
+    DV3_REQUIRE(weight_decay >= 0.f, "adam_clip_opts: weight_decay=%g < 0", weight_decay);
+    const int blocks = (int)adam_blocks(n);
+    const bool wd = weight_decay != 0.f, ams = vmax != nullptr;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (wd && ams)
+        launch_k(adam_clip_kernel<true, true>, blocks, 256, 0, st, p, g, m, v, vmax, n, hyper, sumsq, beta1, beta2,
+                 eps, max_norm, weight_decay);
+    else if (wd)
+        launch_k(adam_clip_kernel<true, false>, blocks, 256, 0, st, p, g, m, v, vmax, n, hyper, sumsq, beta1, beta2,
+                 eps, max_norm, weight_decay);
+    else if (ams)
+        launch_k(adam_clip_kernel<false, true>, blocks, 256, 0, st, p, g, m, v, vmax, n, hyper, sumsq, beta1, beta2,
+                 eps, max_norm, weight_decay);
+    else
+        launch_k(adam_clip_kernel<false, false>, blocks, 256, 0, st, p, g, m, v, vmax, n, hyper, sumsq, beta1, beta2,
+                 eps, max_norm, weight_decay);
+    return check_launch("adam_clip_opts");
 }
 
 }  // extern "C"

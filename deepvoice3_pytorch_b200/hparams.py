@@ -7,7 +7,7 @@ anybody who switches packages, so they are restated here:
   reference does NOT forward: ``query_position_rate`` / ``key_position_rate`` / ``embedding_weight_std`` of the preset
   are ignored and the builder defaults (1.0 / 1.29 / 0.1) apply -- kept, because checkpoints were trained that way.
 * ``train_step_kwargs(hp)``: the optimiser / loss settings ``train.py`` reads in its loop (train.py:704-759, 939-946)
-  as keyword arguments of ``train_step.TrainStep``.
+  and passes to torch.optim.Adam (train.py:975-979) as keyword arguments of ``train_step.TrainStep``.
 """
 import json
 
@@ -50,12 +50,8 @@ def build_model(hp, n_vocab):
 
 
 def train_step_kwargs(hp):
-    """Keyword arguments of ``TrainStep`` for this hyper-parameter set."""
-    # settings train.py reads that this step does not implement must not be dropped silently
-    if hp.get("weight_decay", 0.0) != 0.0 or hp.get("amsgrad", False):
-        raise ValueError("TrainStep's flat Adam implements torch.optim.Adam without weight_decay / amsgrad "
-                         "(reference train.py:975-979); got weight_decay=%r amsgrad=%r"
-                         % (hp.get("weight_decay"), hp.get("amsgrad")))
+    """Keyword arguments of ``TrainStep`` for this hyper-parameter set.  The training mode (train_seq2seq /
+    train_postnet) is a command-line choice of train.py, not an hparam: pass it alongside."""
     schedule = hp.get("lr_schedule")
     if schedule is not None and not callable(schedule):
         base = getattr(_ts, schedule)          # reference: getattr(lrschedule, hparams.lr_schedule)
@@ -66,4 +62,5 @@ def train_step_kwargs(hp):
                 masked_loss_weight=hp["masked_loss_weight"], binary_divergence_weight=hp["binary_divergence_weight"],
                 guided_attention_sigma=hp["guided_attention_sigma"], use_guided_attention=hp["use_guided_attention"],
                 priority_freq=hp.get("priority_freq", 3000), priority_freq_weight=hp.get("priority_freq_weight", 0.0),
-                sample_rate=hp.get("sample_rate", 22050), lr_schedule=schedule)
+                sample_rate=hp.get("sample_rate", 22050), lr_schedule=schedule,
+                weight_decay=hp.get("weight_decay", 0.0), amsgrad=hp.get("amsgrad", False))

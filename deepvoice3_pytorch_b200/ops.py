@@ -907,6 +907,9 @@ EXT_DEC, EXT_TEXT, EXT_MEL, EXT_LIN = 0, 1, 2, 3    # slots of the int64[4] exte
                                                     # mel frames (= decoder steps * r), linear frames
 _extent = None          # {"ext", "padded", "axis", "keymask"} while an extent scope is active
 
+# slots of the per-term loss block of dv3_spec_loss_terms / dv3_aux_loss_terms (DV3_TERM_* in include/dv3b200.h)
+TERM_MEL_L1, TERM_MEL_BD, TERM_LIN_L1, TERM_LIN_BD, TERM_DONE, TERM_ATTN, TERM_COUNT = 0, 1, 2, 3, 4, 5, 6
+
 
 class extent_scope:
     """``with ops.extent_scope(extents, padded):`` -- the forward of a training batch that was padded past its own

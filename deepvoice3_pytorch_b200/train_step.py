@@ -36,6 +36,17 @@ def noam_learning_rate_decay(init_lr, global_step, warmup_steps=4000):
     return init_lr * warmup_steps ** 0.5 * min(step * warmup_steps ** -1.5, step ** -0.5)
 
 
+def step_learning_rate_decay(init_lr, global_step, anneal_rate=0.98, anneal_interval=30000):
+    """reference lrschedule.py:14-17: x anneal_rate every anneal_interval steps."""
+    return init_lr * anneal_rate ** (global_step // anneal_interval)
+
+
+def cyclic_cosine_annealing(init_lr, global_step, T, M):
+    """reference lrschedule.py:20-35: M cosine cycles of T // M steps each over T steps (arXiv:1704.00109)."""
+    TdivM = T // M
+    return float(init_lr / 2.0 * (np.cos(np.pi * ((global_step - 1) % TdivM) / TdivM) + 1.0))
+
+
 def sequence_mask(lengths, max_len):
     """(B,) int64 device tensor -> (B, max_len) float mask (reference train.py:261-271)."""
     return (torch.arange(max_len, device=lengths.device)[None, :] < lengths[:, None]).float()
@@ -90,7 +101,9 @@ def priority_bin_of(priority_freq, sample_rate, linear_dim):
 def training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, binary_divergence_weight=0.1,
                   guided_attention_sigma=0.2, use_guided_attention=True, priority_freq=3000, priority_freq_weight=0.0,
                   sample_rate=22050):
-    """Total loss of one step with seq2seq and postnet trained jointly (reference train.py:665-740)."""
+    """Total loss of one step (reference train.py:665-740).  outs = (mel, linear, attention, done) predictions; a
+    seq2seq-only step passes linear = None (mel + done + attention losses), a postnet-only step everything but linear
+    as None (linear loss only)."""
     if batch.get("extents") is not None:
         raise ValueError("training_loss does not take a batch padded to a bucket (extents): use fused_training_loss")
     mel_out, lin_out, attn, done_hat = outs
@@ -102,14 +115,17 @@ def training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, b
         tgt_mask = sequence_mask(tl, y.size(1)).unsqueeze(-1) if downsample_step > 1 else dec_mask
         dec_mask, tgt_mask = dec_mask[:, r:, :], tgt_mask[:, r:, :]
     w = binary_divergence_weight
-    l1, bd = spec_loss(mel_out[:, :-r, :], mel[:, r:, :], dec_mask, masked_loss_weight, w)
-    loss = (1 - w) * l1 + w * bd
-    loss = loss + F.binary_cross_entropy(done_hat, done)
-    l1, bd = spec_loss(lin_out[:, :-r, :], y[:, r:, :], tgt_mask, masked_loss_weight, w,
-                       priority_bin=priority_bin_of(priority_freq, sample_rate, lin_out.size(-1)),
-                       priority_w=priority_freq_weight)
-    loss = loss + (1 - w) * l1 + w * bd
-    if use_guided_attention:
+    loss = 0.0
+    if mel_out is not None:
+        l1, bd = spec_loss(mel_out[:, :-r, :], mel[:, r:, :], dec_mask, masked_loss_weight, w)
+        loss = (1 - w) * l1 + w * bd
+        loss = loss + F.binary_cross_entropy(done_hat, done)
+    if lin_out is not None:
+        l1, bd = spec_loss(lin_out[:, :-r, :], y[:, r:, :], tgt_mask, masked_loss_weight, w,
+                           priority_bin=priority_bin_of(priority_freq, sample_rate, lin_out.size(-1)),
+                           priority_w=priority_freq_weight)
+        loss = loss + (1 - w) * l1 + w * bd
+    if use_guided_attention and attn is not None:
         soft = guided_attention_mask(batch["input_lengths_dev"], tl // r // downsample_step, attn.size(-2),
                                      attn.size(-1), guided_attention_sigma)
         loss = loss + (attn * soft).mean()
@@ -117,67 +133,72 @@ def training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, b
 
 
 class _FusedLossFn(torch.autograd.Function):
-    """All four training losses and their gradients in 3 kernel launches (csrc/loss.cu)."""
+    """All four training losses and their gradients in 3 kernel launches (csrc/loss.cu).  Predictions passed as None
+    (a seq2seq-only or postnet-only step) leave their loss out and get no launch.  terms: optional float
+    (ops.TERM_COUNT,) device block the kernels add the per-term losses to."""
 
     @staticmethod
     def forward(ctx, mel_out, lin_out, attn, done_hat, mel, y, done, target_lengths, input_lengths, r,
-                downsample_step, w, bw, sigma, use_attn, pbin, pw, ext):
-        dev = mel_out.device
+                downsample_step, w, bw, sigma, use_attn, pbin, pw, ext, terms):
+        dev = target_lengths.device
         vp = lambda t: ctypes.c_void_p(t.data_ptr())
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        mel_out, lin_out, attn, done_hat = [t.contiguous() for t in (mel_out, lin_out, attn, done_hat)]
+        # a batch padded to a bucket: the kernels read the logical extents (ops.EXT_* slots)
+        at = (lambda slot: ctypes.c_void_p(ext.data_ptr() + 8 * slot)) if ext is not None else (lambda slot: None)
+        tp = (lambda slot: ctypes.c_void_p(terms.data_ptr() + 4 * slot)) if terms is not None else (lambda slot: None)
         loss = torch.zeros(1, device=dev)
-        g_mel, g_lin = torch.empty_like(mel_out), torch.empty_like(lin_out)
-        g_attn, g_done = torch.empty_like(attn), torch.empty_like(done_hat)
         dec_len = (target_lengths // (r * downsample_step)).contiguous()
-        B, Td, Dm = mel_out.shape
-        _, Tl, Dl = lin_out.shape
-        lin_len = target_lengths.contiguous() if downsample_step > 1 else dec_len
-        A, _, _, Ts = attn.shape
-        dec_len_attn = (target_lengths // r // downsample_step).contiguous()
-        if ext is None:
-            lib.call("dv3_spec_loss", vp(mel_out), vp(mel.contiguous()), vp(dec_len), vp(g_mel), vp(loss), B, Td, Dm,
-                     r, float(w), float(bw), 0, 0.0, st)
-            lib.call("dv3_spec_loss", vp(lin_out), vp(y.contiguous()), vp(lin_len), vp(g_lin), vp(loss), B, Tl, Dl,
-                     r, float(w), float(bw), int(pbin), float(pw), st)
-            lib.call("dv3_aux_loss", vp(done_hat), vp(done.contiguous()), vp(g_done), done_hat.numel(), vp(attn),
-                     vp(g_attn), vp(input_lengths.contiguous()), vp(dec_len_attn), A, B, attn.shape[2], Ts,
-                     float(sigma), int(use_attn), vp(loss), st)
-        else:                   # a batch padded to a bucket: the kernels read the logical extents (ops.EXT_* slots)
-            at = lambda slot: ctypes.c_void_p(ext.data_ptr() + 8 * slot)
-            lib.call("dv3_spec_loss_ext", vp(mel_out), vp(mel.contiguous()), vp(dec_len), at(ops.EXT_MEL), vp(g_mel),
-                     vp(loss), B, Td, Dm, r, float(w), float(bw), 0, 0.0, st)
-            lib.call("dv3_spec_loss_ext", vp(lin_out), vp(y.contiguous()), vp(lin_len),
-                     at(ops.EXT_LIN if downsample_step > 1 else ops.EXT_MEL), vp(g_lin), vp(loss), B, Tl, Dl, r,
-                     float(w), float(bw), int(pbin), float(pw), st)
-            assert done_hat.numel() == B * attn.shape[2] and ops.EXT_TEXT == ops.EXT_DEC + 1
-            lib.call("dv3_aux_loss_ext", vp(done_hat), vp(done.contiguous()), vp(g_done), vp(attn), vp(g_attn),
-                     vp(input_lengths.contiguous()), vp(dec_len_attn), at(ops.EXT_DEC), A, B, attn.shape[2], Ts,
-                     float(sigma), int(use_attn), vp(loss), st)
+        g_mel = g_lin = g_attn = g_done = None
+        if mel_out is not None:
+            mel_out = mel_out.contiguous()
+            g_mel = torch.empty_like(mel_out)
+            B, Td, Dm = mel_out.shape
+            lib.call("dv3_spec_loss_terms", vp(mel_out), vp(mel.contiguous()), vp(dec_len), at(ops.EXT_MEL), vp(g_mel),
+                     vp(loss), tp(ops.TERM_MEL_L1), B, Td, Dm, r, float(w), float(bw), 0, 0.0, st)
+        if lin_out is not None:
+            lin_out = lin_out.contiguous()
+            g_lin = torch.empty_like(lin_out)
+            B, Tl, Dl = lin_out.shape
+            lin_len = target_lengths.contiguous() if downsample_step > 1 else dec_len
+            lib.call("dv3_spec_loss_terms", vp(lin_out), vp(y.contiguous()), vp(lin_len),
+                     at(ops.EXT_LIN if downsample_step > 1 else ops.EXT_MEL), vp(g_lin), vp(loss), tp(ops.TERM_LIN_L1),
+                     B, Tl, Dl, r, float(w), float(bw), int(pbin), float(pw), st)
+        if done_hat is not None:
+            attn, done_hat = attn.contiguous(), done_hat.contiguous()
+            g_attn, g_done = torch.empty_like(attn), torch.empty_like(done_hat)
+            A, B, Td, Ts = attn.shape
+            dec_len_attn = (target_lengths // r // downsample_step).contiguous()
+            assert ext is None or (done_hat.numel() == B * Td and ops.EXT_TEXT == ops.EXT_DEC + 1)
+            lib.call("dv3_aux_loss_terms", vp(done_hat), vp(done.contiguous()), vp(g_done), done_hat.numel(), vp(attn),
+                     vp(g_attn), vp(input_lengths.contiguous()), vp(dec_len_attn), at(ops.EXT_DEC), A, B, Td, Ts,
+                     float(sigma), int(use_attn), vp(loss), tp(ops.TERM_DONE), st)
         ctx.save_for_backward(g_mel, g_lin, g_attn, g_done)
         return loss[0]
 
     @staticmethod
     def backward(ctx, gout):
-        g_mel, g_lin, g_attn, g_done = ctx.saved_tensors
-        return (g_mel * gout, g_lin * gout, g_attn * gout, g_done * gout) + (None,) * 14
+        return tuple(None if g is None else g * gout for g in ctx.saved_tensors) + (None,) * 15
 
 
 def fused_training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, binary_divergence_weight=0.1,
                         guided_attention_sigma=0.2, use_guided_attention=True, priority_freq=3000,
-                        priority_freq_weight=0.0, sample_rate=22050):
+                        priority_freq_weight=0.0, sample_rate=22050, terms=None):
     """Same value and gradients as ``training_loss`` (reference train.py:665-740), computed by csrc/loss.cu.  A batch
     padded to a bucket (``data.pad_to_bucket``: it carries ``extents``) gives the loss and gradients of the unpadded
-    batch: the padding leaves every mean and its gradient is 0."""
+    batch: the padding leaves every mean and its gradient is 0.  terms: a zeroed float (ops.TERM_COUNT,) CUDA tensor
+    that receives the per-term losses (L1 and binary-divergence parts of the mel and linear losses, done BCE, guided
+    attention) without a launch of their own."""
     mel_out, lin_out, attn, done_hat = outs
     ext = batch.get("extents")
     if ext is not None and not (ext.is_cuda and ext.dtype == torch.int64 and ext.shape == (4,) and ext.is_contiguous()):
         raise ValueError("batch['extents'] must be a contiguous int64 (4,) CUDA tensor")
-    return _FusedLossFn.apply(mel_out, lin_out, attn, done_hat, batch["mel"], batch["y"], batch["done"],
-                              batch["target_lengths"], batch["input_lengths_dev"], r, downsample_step,
+    if terms is not None and not (terms.is_cuda and terms.dtype == torch.float32 and terms.shape == (ops.TERM_COUNT,)):
+        raise ValueError("terms must be a float32 (%d,) CUDA tensor" % ops.TERM_COUNT)
+    pbin = priority_bin_of(priority_freq, sample_rate, lin_out.size(-1)) if lin_out is not None else 0
+    return _FusedLossFn.apply(mel_out, lin_out, attn, done_hat, batch["mel"], batch.get("y"), batch.get("done"),
+                              batch["target_lengths"], batch.get("input_lengths_dev"), r, downsample_step,
                               masked_loss_weight, binary_divergence_weight, guided_attention_sigma,
-                              use_guided_attention, priority_bin_of(priority_freq, sample_rate, lin_out.size(-1)),
-                              priority_freq_weight, ext)
+                              use_guided_attention, pbin, priority_freq_weight, ext, terms)
 
 
 class ParameterArena:
@@ -273,33 +294,84 @@ def gradient_buckets(model, arena):
     return tagged, rest
 
 
-class FlatAdam:
-    """torch.optim.Adam(betas, eps) + clip_grad_norm_(clip) over a ParameterArena in two launches."""
+def arena_parts(model, arena):
+    """[lo, hi) arena ranges of ``model.seq2seq``'s and ``model.postnet``'s parameters, plus whatever lies between or
+    after them (the speaker embedding) as parts of their own: the units that keep their own Adam step count."""
+    cuts = sorted(r for r in (arena.range_of(list(getattr(model, name).parameters()))
+                              for name in ("seq2seq", "postnet") if hasattr(model, name)) if r)
+    parts, pos = [], 0
+    for lo, hi in cuts:
+        if lo > pos:
+            parts.append((pos, lo))
+        parts.append((lo, hi))
+        pos = hi
+    if pos < arena.numel:
+        parts.append((pos, arena.numel))
+    return parts
 
-    def __init__(self, arena, lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1):
+
+class FlatAdam:
+    """torch.optim.Adam(betas, eps, weight_decay, amsgrad) + clip_grad_norm_(clip) over a ParameterArena in two
+    launches.
+
+    parts: [lo, hi) arena ranges that keep their own step count (bias-correction clock); default one part.  State
+    loaded for only some parts (a checkpoint of a seq2seq-only or postnet-only run) resumes those at their step and
+    starts the others at 0, as torch.optim.Adam does for parameters it has no state for.  While all clocks agree the
+    update is one launch over the arena; otherwise one per part (``split_update()``; a captured CUDA graph keeps the
+    plan it was captured with, and TrainStep.load_state_dict drops its graphs when the plan changes).
+    State loaded for parameters outside the arena (the other part, in a seq2seq-only or postnet-only run) is kept
+    as it is and written back by ``state_dict()``, as torch.optim.Adam keeps state for parameters without gradients.
+    index / n_index: position of each arena parameter in the optimizer's parameter list (the indices of the checkpoint
+    format) and that list's length; default the arena's own parameters."""
+
+    def __init__(self, arena, lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1, weight_decay=0.0, amsgrad=False,
+                 parts=None, index=None, n_index=None):
+        if weight_decay < 0:
+            raise ValueError("weight_decay=%r < 0" % weight_decay)
         self.arena = arena
         self.lr, self.betas, self.eps, self.clip = lr, betas, eps, clip_thresh
+        self.weight_decay, self.amsgrad = float(weight_decay), bool(amsgrad)
         dev = arena.flat.device
         self.m = torch.zeros_like(arena.flat)
         self.v = torch.zeros_like(arena.flat)
-        self.hyper = torch.zeros(4, device=dev)
+        self.vmax = torch.zeros_like(arena.flat) if self.amsgrad else None
+        self.parts = list(parts) if parts else [(0, arena.numel)]
+        self.part_t = [0] * len(self.parts)
+        self._part_of = [next(k for k, (lo, hi) in enumerate(self.parts) if lo <= o < hi) for o in arena.offsets]
+        self.index = list(range(len(arena.params))) if index is None else list(index)
+        self.n_index = len(self.index) if n_index is None else int(n_index)
+        nh = 4 * len(self.parts)
+        self.hyper = torch.zeros(nh, device=dev)
         # ring of pinned staging slots: the host may run several steps ahead of the stream, so a slot is only
         # rewritten after the copy that last read it has completed (event wait, normally already signalled)
-        self._slots = [torch.zeros(4).pin_memory() if dev.type == "cuda" else torch.zeros(4) for _ in range(4)]
+        self._slots = [torch.zeros(nh).pin_memory() if dev.type == "cuda" else torch.zeros(nh) for _ in range(4)]
         self._events = [None] * 4
+        self._n = 0
+        self._foreign = {}          # loaded state of parameters outside the arena: list index -> torch Adam state
         self.sumsq = torch.zeros(1, device=dev)
         self._scratch = torch.zeros(lib.raw("dv3_sumsq_scratch_floats")(), device=dev) if dev.type == "cuda" else None
-        self.t = 0
+
+    def split_update(self):
+        """True when the parts' step counts differ: one update launch per part instead of one over the arena."""
+        return len(set(self.part_t)) > 1
+
+    @property
+    def t(self):
+        """Step count (of the part that has taken the most steps)."""
+        return max(self.part_t)
 
     def set_hyper(self, lr, grad_scale=1.0):
-        """Host-side scalar prep; the async H2D copy of 16 bytes is the only thing the stream sees."""
-        self.t += 1
+        """Host-side scalar prep; the async H2D copy of 16 bytes per part is the only thing the stream sees.
+        hyper[4k:4k+4] = {lr, bias correction 1, bias correction 2, grad_scale} of part k."""
+        self.part_t = [t + 1 for t in self.part_t]
+        self._n += 1
         b1, b2 = self.betas
-        i = self.t % 4
+        i = self._n % 4
         if self._events[i] is not None:
             self._events[i].synchronize()
         h = self._slots[i]
-        h[0], h[1], h[2], h[3] = lr, 1.0 - b1 ** self.t, 1.0 - b2 ** self.t, grad_scale
+        for k, t in enumerate(self.part_t):
+            h[4 * k], h[4 * k + 1], h[4 * k + 2], h[4 * k + 3] = lr, 1.0 - b1 ** t, 1.0 - b2 ** t, grad_scale
         self.hyper.copy_(h, non_blocking=True)
         self._events[i] = torch.cuda.Event()
         self._events[i].record()
@@ -310,70 +382,123 @@ class FlatAdam:
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         lib.call("dv3_sumsq", ctypes.c_void_p(a.grad.data_ptr()), a.numel, ctypes.c_void_p(self.sumsq.data_ptr()),
                  ctypes.c_void_p(self._scratch.data_ptr()), st)
-        lib.call("dv3_adam_clip", ctypes.c_void_p(a.flat.data_ptr()), ctypes.c_void_p(a.grad.data_ptr()),
-                 ctypes.c_void_p(self.m.data_ptr()), ctypes.c_void_p(self.v.data_ptr()), a.numel,
-                 ctypes.c_void_p(self.hyper.data_ptr()), ctypes.c_void_p(self.sumsq.data_ptr()),
-                 self.betas[0], self.betas[1], self.eps, float(self.clip), st)
+        if not self.split_update():
+            plan = [(0, a.numel, 0)]
+        else:
+            plan = [(lo, hi, k) for k, (lo, hi) in enumerate(self.parts)]
+        for lo, hi, k in plan:
+            at = lambda t: ctypes.c_void_p(t.data_ptr() + 4 * lo) if t is not None else None
+            lib.call("dv3_adam_clip_opts", at(a.flat), at(a.grad), at(self.m), at(self.v), at(self.vmax), hi - lo,
+                     ctypes.c_void_p(self.hyper.data_ptr() + 16 * k), ctypes.c_void_p(self.sumsq.data_ptr()),
+                     self.betas[0], self.betas[1], self.eps, float(self.clip), self.weight_decay, st)
 
     def grad_norm(self):
         return self.sumsq.sqrt() * self.hyper[3]
 
     # -- checkpoint format of torch.optim.Adam (what reference train.py:save_checkpoint stores under "optimizer",
-    #    train.py:787-810, and load_checkpoint restores, :843-860): parameter i of get_trainable_parameters() <->
-    #    state[i] = {step, exp_avg, exp_avg_sq}
+    #    train.py:787-810, and load_checkpoint restores, :843-860): parameter index[j] of the optimizer's list <->
+    #    state = {step, exp_avg, exp_avg_sq[, max_exp_avg_sq]}; parameters that have not stepped have no state
     def state_dict(self):
         a = self.arena
         state = {}
-        for i, (p, o) in enumerate(zip(a.params, a.offsets)):
+        for p, o, i, k in zip(a.params, a.offsets, self.index, self._part_of):
+            if self.part_t[k] == 0:
+                continue
             n = p.numel()
-            state[i] = {"step": torch.tensor(float(self.t)),
+            state[i] = {"step": torch.tensor(float(self.part_t[k])),
                         "exp_avg": self.m[o:o + n].view_as(p).clone(),
                         "exp_avg_sq": self.v[o:o + n].view_as(p).clone()}
-        group = {"lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": 0, "amsgrad": False,
-                 "maximize": False, "foreach": None, "capturable": False, "differentiable": False, "fused": None,
-                 "decoupled_weight_decay": False, "params": list(range(len(a.params)))}
+            if self.amsgrad:
+                state[i]["max_exp_avg_sq"] = self.vmax[o:o + n].view_as(p).clone()
+        for i, st in self._foreign.items():
+            state[i] = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in st.items()}
+        group = {"lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
+                 "amsgrad": self.amsgrad, "maximize": False, "foreach": None, "capturable": False,
+                 "differentiable": False, "fused": None, "decoupled_weight_decay": False,
+                 "params": list(range(self.n_index))}
         return {"state": state, "param_groups": [group]}
 
     def load_state_dict(self, sd):
-        """Accepts a torch.optim.Adam state_dict over the same parameter list (e.g. from a reference checkpoint)."""
+        """Accepts a torch.optim.Adam state_dict over the same parameter list (e.g. from a reference checkpoint, whole
+        or partial).  Every part resumes at the step count of its parameters' state, or at 0 if it has none."""
         a = self.arena
         groups = sd["param_groups"]
         ids = [i for g in groups for i in g["params"]]
-        if len(ids) != len(a.params):
-            raise ValueError("optimizer state has %d parameters, the model %d" % (len(ids), len(a.params)))
+        if len(ids) != self.n_index:
+            raise ValueError("optimizer state has %d parameters, the model %d" % (len(ids), self.n_index))
         g0 = groups[0]
-        if g0.get("weight_decay", 0) != 0 or g0.get("amsgrad", False):
-            raise ValueError("FlatAdam implements plain Adam: weight_decay / amsgrad states cannot be loaded")
+        if float(g0.get("weight_decay", 0)) != self.weight_decay or bool(g0.get("amsgrad", False)) != self.amsgrad:
+            raise ValueError("optimizer state has weight_decay=%r amsgrad=%r, this optimizer weight_decay=%r amsgrad=%r"
+                             % (g0.get("weight_decay", 0), g0.get("amsgrad", False), self.weight_decay, self.amsgrad))
         self.lr, self.betas, self.eps = g0["lr"], tuple(g0["betas"]), g0["eps"]
-        steps = set()
+        mine = set(self.index)
+        self._foreign = {j: {k: (v.clone() if torch.is_tensor(v) else v) for k, v in sd["state"][ids[j]].items()}
+                         for j in range(self.n_index) if j not in mine and ids[j] in sd["state"]}
+        steps = [set() for _ in self.parts]
         self.m.zero_()
         self.v.zero_()
-        for i, p, o in zip(ids, a.params, a.offsets):
-            st = sd["state"].get(i)
+        if self.vmax is not None:
+            self.vmax.zero_()
+        for j, p, o, k in zip(self.index, a.params, a.offsets, self._part_of):
+            st = sd["state"].get(ids[j])
             if st is None:                      # parameter that never received a gradient
                 continue
             n = p.numel()
             if tuple(st["exp_avg"].shape) != tuple(p.shape):
-                raise ValueError("optimizer state %d has shape %s, parameter %s" % (i, tuple(st["exp_avg"].shape),
+                raise ValueError("optimizer state %d has shape %s, parameter %s" % (ids[j], tuple(st["exp_avg"].shape),
                                                                                    tuple(p.shape)))
             self.m[o:o + n].view_as(p).copy_(st["exp_avg"])
             self.v[o:o + n].view_as(p).copy_(st["exp_avg_sq"])
-            steps.add(int(st["step"]))
-        if len(steps) > 1:
-            raise ValueError("per-parameter step counts differ (%s): not representable in a flat Adam" % sorted(steps))
-        self.t = steps.pop() if steps else 0
+            if self.vmax is not None:
+                self.vmax[o:o + n].view_as(p).copy_(st["max_exp_avg_sq"])
+            steps[k].add(int(st["step"]))
+        for k, s in enumerate(steps):
+            if len(s) > 1:
+                raise ValueError("step counts differ within arena part %d (%s): not representable in a flat Adam"
+                                 % (k, sorted(s)))
+        self.part_t = [s.pop() if s else 0 for s in steps]
+
+
+def check_train_mode(model, train_seq2seq, train_postnet):
+    """ValueError for a training mode the reference would assert on or crash in later (train.py:615, 690, 699)."""
+    if not (train_seq2seq or train_postnet):
+        raise ValueError("train_seq2seq and train_postnet are both False: nothing to train")
+    if train_seq2seq and train_postnet:
+        return
+    if getattr(model, "n_speakers", 1) > 1:
+        raise ValueError("seq2seq-only / postnet-only training needs a single-speaker model (n_speakers=%d)"
+                         % model.n_speakers)
+    if train_postnet and getattr(model, "use_decoder_state_for_postnet_input", False):
+        raise ValueError("postnet-only training feeds the converter ground-truth mels, but this model was built with "
+                         "use_decoder_state_for_postnet_input=True (its converter reads decoder states)")
 
 
 class TrainStep:
-    """model + losses + flat optimizer (+ NCCL gradient all-reduce when torch.distributed is initialised)."""
+    """model + losses + flat optimizer (+ NCCL gradient all-reduce when torch.distributed is initialised): reference
+    train.py's ``train()``.
+
+    train_seq2seq / train_postnet: the reference's two-stage training (train.py:655-740).  Seq2seq-only runs
+    ``model.seq2seq`` and the mel + done + guided-attention losses; postnet-only runs ``model.postnet`` on the
+    ground-truth mel and the linear loss.  The arena, the optimizer state and the gradient norm then cover only the
+    trained part; the other part's parameters keep their bits.  weight_decay / amsgrad: torch.optim.Adam's."""
 
     def __init__(self, model, init_lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1, r=1, downsample_step=4,
                  masked_loss_weight=0.5, binary_divergence_weight=0.1, guided_attention_sigma=0.2,
                  use_guided_attention=True, priority_freq=3000, priority_freq_weight=0.0, sample_rate=22050,
-                 lr_schedule=noam_learning_rate_decay, use_graph=False, fused_loss=True, weight_bank=None):
+                 lr_schedule=noam_learning_rate_decay, use_graph=False, fused_loss=True, weight_bank=None,
+                 train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False):
+        check_train_mode(model, train_seq2seq, train_postnet)
         self.model = model
-        self.arena = ParameterArena(model)
-        self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh)
+        self.train_seq2seq, self.train_postnet = bool(train_seq2seq), bool(train_postnet)
+        # the module whose parameters are trained and checkpointed (reference save_checkpoint, train.py:787-808)
+        self.trained = model if self.train_seq2seq and self.train_postnet else \
+            (model.seq2seq if self.train_seq2seq else model.postnet)
+        trainable = list(model.get_trainable_parameters())
+        own = {id(p) for p in self.trained.parameters()}
+        index = [i for i, p in enumerate(trainable) if id(p) in own]
+        self.arena = ParameterArena(model, [trainable[i] for i in index])
+        self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad,
+                            arena_parts(model, self.arena), index, len(trainable))
         self.init_lr, self.lr_schedule = init_lr, lr_schedule
         self.loss_kw = dict(r=r, downsample_step=downsample_step, masked_loss_weight=masked_loss_weight,
                             binary_divergence_weight=binary_divergence_weight,
@@ -381,6 +506,8 @@ class TrainStep:
                             use_guided_attention=use_guided_attention, priority_freq=priority_freq,
                             priority_freq_weight=priority_freq_weight, sample_rate=sample_rate)
         self.loss_fn = fused_training_loss if fused_loss else training_loss
+        # per-term losses of the last step (ops.TERM_* slots); outside every graph pool, like the bucket loss scalars
+        self._terms = torch.zeros(ops.TERM_COUNT, device=self.arena.flat.device)
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.global_step = 0
         self.use_graph = use_graph
@@ -410,15 +537,28 @@ class TrainStep:
 
     # -- checkpointing: the reference's checkpoint keys (train.py:787-810) ---------------------------------
     def state_dict(self, global_epoch=0):
-        return {"state_dict": self.model.state_dict(), "optimizer": self.opt.state_dict(),
+        """The reference's checkpoint: in a partial mode the trained part's state_dict (model.seq2seq or
+        model.postnet), with optimizer state for its parameters only."""
+        return {"state_dict": self.trained.state_dict(), "optimizer": self.opt.state_dict(),
                 "global_step": self.global_step, "global_epoch": global_epoch}
 
     def load_state_dict(self, ckpt, load_optimizer=True):
-        """Resume from ``state_dict()`` or from a reference checkpoint (same keys).  Restores the Adam moments, the
-        bias-correction step and the position in the learning-rate schedule."""
-        self.model.load_state_dict(ckpt["state_dict"])      # copies into the arena views in place
+        """Resume from ``state_dict()`` or from a reference checkpoint (same keys), of the whole model or of
+        model.seq2seq / model.postnet alone, in any mode.  Restores the Adam moments, the bias-correction steps (parts
+        without optimizer state start at step 0) and the position in the learning-rate schedule."""
+        sd = ckpt["state_dict"]
+        target = self.model
+        for part in (self.model.seq2seq, self.model.postnet):
+            if set(sd) == set(part.state_dict()):
+                target = part
+        target.load_state_dict(sd)      # copies into the arena views in place
         if load_optimizer and ckpt.get("optimizer") is not None:
+            split = self.opt.split_update()
             self.opt.load_state_dict(ckpt["optimizer"])
+            if self.opt.split_update() != split:       # captured graphs hold the other update plan: capture anew
+                self._graph = self._static = self._loss = self._graph_key = self._pool = None
+                self._buckets = {}
+                self.launches_per_step = None
         self.global_step = int(ckpt.get("global_step", 0))
         return int(ckpt.get("global_epoch", 0))
 
@@ -458,14 +598,60 @@ class TrainStep:
         ext = batch.get("extents")          # a batch padded to a bucket (data.pad_to_bucket)
         scope = ops.extent_scope(ext, data.batch_extents(batch)) if ext is not None else contextlib.nullcontext()
         with scope:
-            outs = self.model(batch["x"], batch["mel"], speaker_ids=batch.get("speaker_ids"),
-                              text_positions=batch["text_positions"], frame_positions=batch["frame_positions"],
-                              input_lengths=batch["input_lengths_dev"])
-            loss = self.loss_fn(outs, batch, **self.loss_kw)
+            outs = self._forward(batch)
+            if self.loss_fn is fused_training_loss:
+                self._terms.zero_()
+                loss = self.loss_fn(outs, batch, terms=self._terms, **self.loss_kw)
+            else:
+                loss = self.loss_fn(outs, batch, **self.loss_kw)
         loss.backward()
         if self.bank is not None:
             self.bank.end_backward()
         return loss.detach()
+
+    def _forward(self, batch):
+        """-> (mel, linear, attention, done) predictions; the parts this mode does not run are None."""
+        m = self.model
+        if self.train_seq2seq and self.train_postnet:
+            return m(batch["x"], batch["mel"], speaker_ids=batch.get("speaker_ids"),
+                     text_positions=batch["text_positions"], frame_positions=batch["frame_positions"],
+                     input_lengths=batch["input_lengths_dev"])
+        mel = batch["mel"]
+        if self.train_seq2seq:                  # reference train.py:690-697
+            mel_out, attn, done_hat, _ = m.seq2seq(batch["x"], mel, text_positions=batch["text_positions"],
+                                                   frame_positions=batch["frame_positions"],
+                                                   input_lengths=batch["input_lengths_dev"])
+            return mel_out.reshape(mel.size(0), -1, mel.size(-1)), None, attn, done_hat
+        with ops.extent_axis(ops.EXT_MEL):      # reference train.py:698-700
+            return None, m.postnet(mel), None, None
+
+    def _mode_batch(self, batch):
+        """A postnet-only step reads no text: its batch keeps zero text positions, so that graphs and buckets follow
+        the mel / linear axes alone."""
+        if self.train_seq2seq:
+            return batch
+        return {k: (v[:, :0] if k in ("x", "text_positions") and torch.is_tensor(v) else v) for k, v in batch.items()}
+
+    def loss_terms(self):
+        """The per-term losses of the last step under the tags reference train.py logs (:761-776), for the terms this
+        mode has, plus "gradient norm" when clipping is on.  Device scalars (no host sync), valid until the next
+        ``step()``; on a data-parallel run, this rank's losses and the norm of the averaged gradient."""
+        if self.loss_fn is not fused_training_loss:
+            raise ValueError("loss_terms() needs the fused loss kernels (TrainStep(fused_loss=True))")
+        t, w = self._terms, self.loss_kw["binary_divergence_weight"]
+        out = {}
+        if self.train_seq2seq:
+            out["mel loss"] = (1 - w) * t[ops.TERM_MEL_L1] + w * t[ops.TERM_MEL_BD]
+            out["mel_l1_loss"], out["mel_binary_div_loss"] = t[ops.TERM_MEL_L1], t[ops.TERM_MEL_BD]
+            out["done_loss"] = t[ops.TERM_DONE]
+        if self.train_postnet:
+            out["linear_loss"] = (1 - w) * t[ops.TERM_LIN_L1] + w * t[ops.TERM_LIN_BD]
+            out["linear_l1_loss"], out["linear_binary_div_loss"] = t[ops.TERM_LIN_L1], t[ops.TERM_LIN_BD]
+        if self.train_seq2seq and self.loss_kw["use_guided_attention"]:
+            out["attn_loss"] = t[ops.TERM_ATTN]
+        if self.opt.clip > 0:
+            out["gradient norm"] = self.opt.grad_norm()[0]
+        return out
 
     def _exchange_and_update(self):
         """Gradient exchange (sum; the 1/world average is folded into hyper[3]) + clip + Adam."""
@@ -494,6 +680,7 @@ class TrainStep:
         ``data.pad_to_bucket``) and replays that bucket's graph, with the loss, gradients and update of the unpadded
         batch.  A batch that already carries ``extents`` is its own bucket."""
         self.model.train()
+        batch = self._mode_batch(batch)
         lr = self.lr_schedule(self.init_lr, self.global_step) if self.lr_schedule else self.init_lr
         self.opt.set_hyper(lr, 1.0 / self.world)
         if not self.use_graph:

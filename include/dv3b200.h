@@ -166,6 +166,14 @@ int dv3_sumsq_scratch_floats(void);
 int dv3_sumsq(const float* x, long long n, float* out, float* scratch, void* stream);
 int dv3_adam_clip(float* p, const float* g, float* m, float* v, long long n, const float* hyper,
                   const float* sumsq, float beta1, float beta2, float eps, float max_norm, void* stream);
+/* dv3_adam_clip_opts: dv3_adam_clip with torch.optim.Adam's other two settings.  weight_decay > 0: L2 decay, the
+ * clipped gradient becomes g' + weight_decay*p before the moments.  vmax != NULL: AMSGrad, vmax = max(vmax, v) and
+ * the denominator is sqrt(vmax)/sqrt(hyper[2]) + eps.  weight_decay = 0 and vmax = NULL is dv3_adam_clip.  sumsq may
+ * cover a larger arena than [p, p+n): a caller whose arena parts have different step counts runs one update per
+ * part, each with its own hyper block, after one dv3_sumsq over the whole arena. */
+int dv3_adam_clip_opts(float* p, const float* g, float* m, float* v, float* vmax, long long n, const float* hyper,
+                       const float* sumsq, float beta1, float beta2, float eps, float max_norm, float weight_decay,
+                       void* stream);
 
 /* ---- fused STFT -> linear + mel front-end: reference audio.py:31-34 (spectrogram) and :46-51 (melspectrogram)
  * incl. preemphasis (:21-23), lws sqrt-Hann STFT 1024/256 with 768-sample zero padding (:54-55), mel basis product
@@ -304,6 +312,22 @@ int dv3_spec_loss_ext(const float* y_hat, const float* y, const long long* lengt
 int dv3_aux_loss_ext(const float* done_hat, const float* done, float* d_done, const float* attn, float* d_attn,
                      const long long* in_len, const long long* dec_len, const long long* ext, int A, int B, int Td,
                      int Ts, float sigma, int use_attn, float* loss, void* stream);
+/* The same kernels with the extents nullable (NULL: the full tensors) and the loss split into the terms reference
+ * train.py logs (:761-776).  terms (nullable) is a float block with the DV3_TERM_* slots below, zeroed by the caller;
+ * each call adds its two parts to two consecutive slots:
+ *   dv3_spec_loss_terms: terms[0] += L1 part (priority bins combined), terms[1] += binary-divergence part (0 when
+ *     binary_divergence_weight <= 0) -- pass terms + DV3_TERM_MEL_L1 or terms + DV3_TERM_LIN_L1;
+ *   dv3_aux_loss_terms: terms[0] += done BCE, terms[1] += guided-attention term -- pass terms + DV3_TERM_DONE.
+ * loss and every gradient are exactly those of the calls without terms.  The other four entry points are these with
+ * terms = NULL. */
+enum { DV3_TERM_MEL_L1 = 0, DV3_TERM_MEL_BD = 1, DV3_TERM_LIN_L1 = 2, DV3_TERM_LIN_BD = 3, DV3_TERM_DONE = 4,
+       DV3_TERM_ATTN = 5, DV3_TERM_COUNT = 6 };
+int dv3_spec_loss_terms(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
+                        float* grad, float* loss, float* terms, int B, int T, int D, int r, float masked_loss_weight,
+                        float binary_divergence_weight, int priority_bin, float priority_weight, void* stream);
+int dv3_aux_loss_terms(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
+                       float* d_attn, const long long* in_len, const long long* dec_len, const long long* ext, int A,
+                       int B, int Td, int Ts, float sigma, int use_attn, float* loss, float* terms, void* stream);
 
 /* ---- incremental (autoregressive) decoding: reference conv.py:17-46, deepvoice3.py:367-485, nyanko.py:250-338 ----
  * All loop state lives in device memory so that one decoder step is the same launch sequence every time (CUDA-graph
