@@ -18,30 +18,50 @@ namespace dv3 {
 
 constexpr float kSqrtHalf = 0.70710678118654752f;
 
-// one warp per output channel c (GLU / highway: rows c and C + c); BT batch rows per pass
-template <int BT>
+// step index of row b: one shared counter t_ptr[0], or (SLOTS) one counter per row t_ptr[b]
+template <bool SLOTS>
+__device__ __forceinline__ long long step_of(const int* t_ptr, int b) {
+    return t_ptr ? (long long)t_ptr[SLOTS ? b : 0] : 0;
+}
+
+// ring slot of the input of time t - back (the ring is zero-initialised, so times before the start read zeros)
+__device__ __forceinline__ int ring_slot(long long t, long long back, int L) {
+    const long long tj = t - back;
+    return (int)(((tj % L) + L) % L);
+}
+
+// one warp per output channel c (GLU / highway: rows c and C + c); BT batch rows per pass.
+// SLOTS: every row has its own step counter t_ptr[b] (continuous batching), so the ring slot of each tap, the filing
+// slot and every per-step stride are per row; the fmaf chain of each output is the same as with the shared counter.
+template <int BT, bool SLOTS>
 __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constant__ Dv3IncStep p) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     const int gated = p.mode != 0;
     const int C = gated ? p.Cout / 2 : p.Cout;
-    const long long t = p.t_ptr ? (long long)*p.t_ptr : 0;
+    const long long t0 = step_of<false>(p.t_ptr, 0);      // the shared counter (unused with SLOTS)
     const int k = p.k, Cin = p.Cin, L = (k - 1) * p.dilation + 1;
-    const int slot_now = (int)(t % L);
     if (warp < C) {
         const int c = warp;
         const float* __restrict__ wa = p.w + (size_t)c * k * Cin;
         const float* __restrict__ wb = p.w + (size_t)(C + c) * k * Cin;
         for (int b0 = 0; b0 < p.B; b0 += BT) {
             float acc_a[BT], acc_b[BT];
+            long long tr[BT];                                // step of each row of this pass
 #pragma unroll
-            for (int i = 0; i < BT; ++i) { acc_a[i] = 0.f; acc_b[i] = 0.f; }
+            for (int i = 0; i < BT; ++i) {
+                acc_a[i] = 0.f; acc_b[i] = 0.f;
+                tr[i] = SLOTS ? (b0 + i < p.B ? step_of<true>(p.t_ptr, b0 + i) : 0) : t0;
+            }
             for (int j = 0; j < k; ++j) {
                 const bool cur = (j == k - 1);
                 // tap j sees the input of time t - (k-1-j)*dilation; older than the sequence start = zero (ring is
                 // zero-initialised), the current input comes straight from x (+ add)
-                int slot = 0;
-                if (!cur) { const long long tj = t - (long long)(k - 1 - j) * p.dilation; slot = (int)(((tj % L) + L) % L); }
+                const long long back = (long long)(k - 1 - j) * p.dilation;
+                const int slot0 = cur || SLOTS ? 0 : ring_slot(t0, back, L);
+                int slots[BT];
+#pragma unroll
+                for (int i = 0; i < BT; ++i) slots[i] = cur || !SLOTS ? slot0 : ring_slot(tr[i], back, L);
                 const float* wja = wa + (size_t)j * Cin;
                 const float* wjb = wb + (size_t)j * Cin;
                 if (p.vec4) {
@@ -53,6 +73,7 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
                         for (int i = 0; i < BT; ++i) {
                             const int b = b0 + i;
                             if (b >= p.B) break;
+                            const long long t = tr[i];
                             float4 x4;
                             if (cur) {
                                 x4 = *reinterpret_cast<const float4*>(p.x + b * p.x_ld + t * p.x_t + ci);
@@ -61,7 +82,7 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
                                     x4.x += e4.x; x4.y += e4.y; x4.z += e4.z; x4.w += e4.w;
                                 }
                             } else {
-                                x4 = *reinterpret_cast<const float4*>(p.ring + ((size_t)b * L + slot) * Cin + ci);
+                                x4 = *reinterpret_cast<const float4*>(p.ring + ((size_t)b * L + slots[i]) * Cin + ci);
                             }
                             acc_a[i] = fmaf(a4.x, x4.x, acc_a[i]); acc_a[i] = fmaf(a4.y, x4.y, acc_a[i]);
                             acc_a[i] = fmaf(a4.z, x4.z, acc_a[i]); acc_a[i] = fmaf(a4.w, x4.w, acc_a[i]);
@@ -79,12 +100,13 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
                         for (int i = 0; i < BT; ++i) {
                             const int b = b0 + i;
                             if (b >= p.B) break;
+                            const long long t = tr[i];
                             float xv;
                             if (cur) {
                                 xv = p.x[b * p.x_ld + t * p.x_t + ci];
                                 if (p.add) xv += p.add[b * p.add_ld + t * p.add_t + ci];
                             } else {
-                                xv = p.ring[((size_t)b * L + slot) * Cin + ci];
+                                xv = p.ring[((size_t)b * L + slots[i]) * Cin + ci];
                             }
                             acc_a[i] = fmaf(a1, xv, acc_a[i]);
                             if (gated) acc_b[i] = fmaf(b1, xv, acc_b[i]);
@@ -96,6 +118,7 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
             for (int i = 0; i < BT; ++i) {
                 const int b = b0 + i;
                 if (b >= p.B) break;                       // uniform across the warp
+                const long long t = tr[i];
                 float a = warp_sum(acc_a[i]);
                 float g = gated ? warp_sum(acc_b[i]) : 0.f;
                 if (lane != 0) continue;
@@ -132,6 +155,8 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
     if (p.ring && blockIdx.x == gridDim.x - 1) {
         for (int i = threadIdx.x; i < p.B * Cin; i += blockDim.x) {
             const int b = i / Cin, ci = i - b * Cin;
+            const long long t = SLOTS ? step_of<true>(p.t_ptr, b) : t0;
+            const int slot_now = (int)(t % L);
             float xv = p.x[b * p.x_ld + t * p.x_t + ci];
             if (p.add) xv += p.add[b * p.add_ld + t * p.add_t + ci];
             p.ring[((size_t)b * L + slot_now) * Cin + ci] = xv;
@@ -142,7 +167,8 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
 // one CTA per batch row: scores = q . keys, monotonic window, softmax, context = probs . values * Ts*sqrt(1/Ts).
 // ROWS (ragged batch): row b sees only its own Ts = text_len[b] keys (the key pitch stays p.Ts) and keeps its own
 // cursor; with Ts substituted, the arithmetic is that of the single-row launch, so each row matches it bit for bit.
-template <bool ROWS>
+// SLOTS (with ROWS): row b runs at its own step t_ptr[b] -- alignment row and cursor parity follow it.
+template <bool ROWS, bool SLOTS>
 __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constant__ Dv3IncAttn p, const int* text_len) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     extern __shared__ float sm[];
@@ -151,7 +177,7 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
     __shared__ float red[8];
     __shared__ float bcast;
     const int b = blockIdx.x, tid = threadIdx.x;
-    const long long t = p.t_ptr ? (long long)*p.t_ptr : 0;
+    const long long t = step_of<SLOTS>(p.t_ptr, b);
     const int Ts = ROWS ? text_len[b] : p.Ts;
     // cursor slots: [2] (row 0 leads every row, reference deepvoice3.py:443) or [2][B] (one per row)
     const int cur_rd = ROWS ? (int)(t & 1) * p.B + b : (int)(t & 1);
@@ -216,6 +242,39 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
 __global__ void inc_advance_kernel(int* t) {
     pdl_trigger(); pdl_wait(); *t += 1; }
 
+// per-row counters: a row that has stopped (stop[b] != 0) keeps its step, so it recomputes that same step -- the
+// same inputs give the same bits, and no row ever writes past frame max_decoder_steps + 1
+__global__ void inc_advance_rows_kernel(int* t, const int* stop, int B) {
+    pdl_trigger(); pdl_wait();
+    for (int b = threadIdx.x; b < B; b += blockDim.x)
+        if (!stop || stop[b] == 0) t[b] += 1;
+}
+
+// the reference stop rule (incremental._stop_step) on each row alone, after step t[b] wrote done[b*done_ld + t[b]]:
+// n = t[b] + 1 steps ran; stop after them if done > 0.5 and n > min_steps, or if n > max_steps.  Written once.
+__global__ void inc_stop_rows_kernel(const float* done, long long done_ld, const int* t, int* stop, int B,
+                                     int min_steps, int max_steps) {
+    pdl_trigger(); pdl_wait();
+    for (int b = threadIdx.x; b < B; b += blockDim.x) {
+        if (stop[b] != 0) continue;
+        const int n = t[b] + 1;
+        if ((done[b * done_ld + t[b]] > 0.5f && n > min_steps) || n > max_steps) stop[b] = n;
+    }
+}
+
+// entry e, slot list index i: row slots[i] of e.dst <- row i of e.src (zeros when e.src is NULL), in 4-byte words
+__global__ void __launch_bounds__(256) inc_refill_kernel(const Dv3IncRefill* table, const int* slots) {
+    pdl_trigger(); pdl_wait();
+    const Dv3IncRefill e = table[blockIdx.y];
+    const int i = blockIdx.z, b = slots[i];
+    int* dst = reinterpret_cast<int*>(reinterpret_cast<char*>(e.dst) + (size_t)b * e.dst_row_stride);
+    const int* src = e.src ? reinterpret_cast<const int*>(reinterpret_cast<const char*>(e.src) +
+                                                          (size_t)i * e.src_row_stride) : nullptr;
+    const long long n = e.row_bytes / 4;
+    for (long long w = (long long)blockIdx.x * blockDim.x + threadIdx.x; w < n; w += (long long)gridDim.x * blockDim.x)
+        dst[w] = src ? src[w] : 0;
+}
+
 }  // namespace dv3
 
 using namespace dv3;
@@ -230,17 +289,32 @@ int dv3_inc_conv_step(const Dv3IncStep* p, void* stream) {
     const int C = p->mode != 0 ? p->Cout / 2 : p->Cout;
     const int blocks = (C * 32 + 255) / 256;
     cudaStream_t st = (cudaStream_t)stream;
-    if (p->B == 1) launch_k(inc_conv_step_kernel<1>, blocks, 256, 0, st, *p);
-    else if (p->B == 2) launch_k(inc_conv_step_kernel<2>, blocks, 256, 0, st, *p);
-    else launch_k(inc_conv_step_kernel<4>, blocks, 256, 0, st, *p);
+    if (p->B == 1) launch_k(inc_conv_step_kernel<1, false>, blocks, 256, 0, st, *p);
+    else if (p->B == 2) launch_k(inc_conv_step_kernel<2, false>, blocks, 256, 0, st, *p);
+    else launch_k(inc_conv_step_kernel<4, false>, blocks, 256, 0, st, *p);
     return check_launch("inc_conv_step");
+}
+
+int dv3_inc_conv_step_slots(const Dv3IncStep* p, void* stream) {
+    DV3_REQUIRE(p && p->B > 0 && p->Cin > 0 && p->Cout > 0 && p->k >= 1 && p->dilation >= 1,
+                "inc_conv_step_slots: bad shape");
+    DV3_REQUIRE(p->mode == 0 || (p->Cout == 2 * p->Cin), "inc_conv_step_slots: gated blocks need Cout == 2*Cin");
+    DV3_REQUIRE(p->k == 1 || p->ring != nullptr, "inc_conv_step_slots: k > 1 needs a ring buffer");
+    DV3_REQUIRE(p->t_ptr != nullptr, "inc_conv_step_slots: needs the per-row step counters t_ptr[B]");
+    const int C = p->mode != 0 ? p->Cout / 2 : p->Cout;
+    const int blocks = (C * 32 + 255) / 256;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (p->B == 1) launch_k(inc_conv_step_kernel<1, true>, blocks, 256, 0, st, *p);
+    else if (p->B == 2) launch_k(inc_conv_step_kernel<2, true>, blocks, 256, 0, st, *p);
+    else launch_k(inc_conv_step_kernel<4, true>, blocks, 256, 0, st, *p);
+    return check_launch("inc_conv_step_slots");
 }
 
 int dv3_inc_attn_step(const Dv3IncAttn* p, void* stream) {
     DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0, "inc_attn_step: bad shape");
     const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
     DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step: E + Ts = %d floats exceed 48 KB of shared memory", p->E + p->Ts);
-    launch_k(inc_attn_step_kernel<false>, p->B, 256, smem, (cudaStream_t)stream, *p, (const int*)nullptr);
+    launch_k(inc_attn_step_kernel<false, false>, p->B, 256, smem, (cudaStream_t)stream, *p, (const int*)nullptr);
     return check_launch("inc_attn_step");
 }
 
@@ -249,13 +323,43 @@ int dv3_inc_attn_step_rows(const Dv3IncAttn* p, const int* text_len, void* strea
     const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
     DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_rows: E + Ts = %d floats exceed 48 KB of shared memory",
                 p->E + p->Ts);
-    launch_k(inc_attn_step_kernel<true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
+    launch_k(inc_attn_step_kernel<true, false>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
     return check_launch("inc_attn_step_rows");
+}
+
+int dv3_inc_attn_step_slots(const Dv3IncAttn* p, const int* text_len, void* stream) {
+    DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0 && text_len && p->t_ptr, "inc_attn_step_slots: bad shape");
+    const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
+    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_slots: E + Ts = %d floats exceed 48 KB of shared memory",
+                p->E + p->Ts);
+    launch_k(inc_attn_step_kernel<true, true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
+    return check_launch("inc_attn_step_slots");
 }
 
 int dv3_inc_advance(int* t_ptr, void* stream) {
     launch_k(inc_advance_kernel, 1, 1, 0, (cudaStream_t)stream, t_ptr);
     return check_launch("inc_advance");
+}
+
+int dv3_inc_advance_rows(int* t, const int* stop, int B, void* stream) {
+    DV3_REQUIRE(t && B > 0 && B <= 1024, "inc_advance_rows: bad shape (B = %d)", B);
+    launch_k(inc_advance_rows_kernel, 1, B, 0, (cudaStream_t)stream, t, stop, B);
+    return check_launch("inc_advance_rows");
+}
+
+int dv3_inc_stop_rows(const float* done, long long done_ld, const int* t, int* stop, int B, int min_steps,
+                      int max_steps, void* stream) {
+    DV3_REQUIRE(done && t && stop && B > 0 && B <= 1024 && done_ld > max_steps, "inc_stop_rows: bad shape");
+    launch_k(inc_stop_rows_kernel, 1, B, 0, (cudaStream_t)stream, done, done_ld, t, stop, B, min_steps, max_steps);
+    return check_launch("inc_stop_rows");
+}
+
+int dv3_inc_refill(const Dv3IncRefill* table, int n_entries, const int* slots, int n_slots, void* stream) {
+    DV3_REQUIRE(table && slots && n_entries > 0 && n_entries <= 65535 && n_slots >= 0 && n_slots <= 65535,
+                "inc_refill: bad table (%d entries, %d slots)", n_entries, n_slots);
+    if (n_slots == 0) return 0;
+    launch_k(inc_refill_kernel, dim3(16, n_entries, n_slots), 256, 0, (cudaStream_t)stream, table, slots);
+    return check_launch("inc_refill");
 }
 
 }  // extern "C"

@@ -16,7 +16,12 @@ deepvoice3.py:446) and the monotonic cursor follows batch row 0 only (deepvoice3
 ``decode_ragged`` is the batched form for rows of different text lengths (``synthesis.tts_batch``): row b attends to
 its own text_lengths[b] keys with its own monotonic cursor and stops by the reference's rule applied to it alone, so
 every row gets what ``decode`` gives for that row on its own, bit for bit (every step kernel works per row).
+
+``decode_stream`` is continuous batching (``synthesis.tts_stream``): a fixed set of decoder slots, each with its own
+step counter; when a slot's utterance stops (the stop rule runs on the device, per row), the host gathers it at the next
+check and one ``dv3_inc_refill`` launch resets the slot and loads the next waiting utterance into it.
 """
+import contextlib
 import ctypes
 import os
 
@@ -49,6 +54,10 @@ class Dv3IncAttn(ctypes.Structure):
                 ("window_ahead", _I)]
 
 
+class Dv3IncRefill(ctypes.Structure):
+    _fields_ = [("dst", _P), ("src", _P), ("row_bytes", _LL), ("dst_row_stride", _LL), ("src_row_stride", _LL)]
+
+
 class _Rows:
     """(B, C) rows of a float32 buffer that may advance with the step: row b of step t = ptr + b*ld + t*t (floats)."""
 
@@ -76,13 +85,18 @@ def _folded_weight(m):
 
 
 class StepProgram:
-    """The launch sequence of one decoder step + its device-resident state."""
+    """The launch sequence of one decoder step + its device-resident state.
 
-    def __init__(self, B, device):
-        self.B, self.dev = B, device
+    slots=True: every row has its own step counter (``t`` is int32 (B,)) and runs the ``_slots`` step kernels; the step
+    ends with the device-side stop rule (``stop_rule``) and a per-row advance that holds rows which stopped."""
+
+    def __init__(self, B, device, slots=False):
+        self.B, self.dev, self.slots = B, device, slots
         self.calls = []                     # (entry point name, ctypes struct, extra arguments)
         self.keep = []                      # tensors the structs point into
-        self.t = torch.zeros(1, dtype=torch.int32, device=device)
+        self.t = torch.zeros(B if slots else 1, dtype=torch.int32, device=device)
+        self.rings, self.cursors = [], []   # the per-row history a new utterance starts from zero
+        self.stop = None                    # slots: int32 (B,) stop steps, 0 while the row runs
         self.graph = None
 
     def buf(self, *shape):
@@ -107,6 +121,7 @@ class StepProgram:
             s.add, s.add_ld, s.add_t = add.ptr, add.ld, add.t
         if k > 1:
             ring = self.buf(self.B, (k - 1) * d + 1, Cin)
+            self.rings.append(ring)
             s.ring = ring.data_ptr()
         s.w, s.bias = w.data_ptr(), bias.data_ptr()
         if spk is not None:
@@ -124,8 +139,14 @@ class StepProgram:
         s.B, s.Cin, s.Cout, s.k, s.dilation, s.mode, s.act = self.B, Cin, Cout, k, d, mode, act
         s.vec4 = int(Cin % 4 == 0 and x.aligned16() and (add is None or add.aligned16()))
         self.keep += [w, bias]
-        self.calls.append(("dv3_inc_conv_step", s, ()))
+        self.calls.append(("dv3_inc_conv_step_slots" if self.slots else "dv3_inc_conv_step", s, ()))
         return y
+
+    def cursor(self, per_row):
+        """Monotonic-attention cursors: int[2] (row 0 leads, ``decode``) or int[2][B] (one per row)."""
+        la = torch.zeros(2 * self.B if per_row else 2, dtype=torch.int32, device=self.dev)
+        self.cursors.append(la)
+        return la
 
     def attention(self, q, keys_bet, values_bte, ctx, align, align_scale, last_attended, window_backward, window_ahead,
                   text_len=None):
@@ -144,17 +165,32 @@ class StepProgram:
         a.B, a.E, a.Ts, a.window_backward, a.window_ahead = B, E, Ts, window_backward, window_ahead
         self.keep += [keys_bet, values_bte]
         if text_len is None:
+            assert not self.slots, "the slot program attends per row: it needs text_len"
             self.calls.append(("dv3_inc_attn_step", a, ()))
         else:
             self.keep.append(text_len)
-            self.calls.append(("dv3_inc_attn_step_rows", a, (ctypes.c_void_p(text_len.data_ptr()),)))
+            name = "dv3_inc_attn_step_slots" if self.slots else "dv3_inc_attn_step_rows"
+            self.calls.append((name, a, (ctypes.c_void_p(text_len.data_ptr()),)))
+
+    def stop_rule(self, dones, min_steps, max_steps):
+        """slots: apply the reference stop rule to row b's done flag dones[b, t[b]] at the end of every step.  Rows
+        start idle (stop = -1: held at step 0) until ``dv3_inc_refill`` loads them."""
+        assert self.slots and dones.size(1) > max_steps
+        self.stop = torch.full((self.B,), -1, dtype=torch.int32, device=self.dev)
+        self._stop_args = (ctypes.c_void_p(dones.data_ptr()), dones.size(1), ctypes.c_void_p(self.t.data_ptr()),
+                           ctypes.c_void_p(self.stop.data_ptr()), self.B, min_steps, max_steps)
 
     # -- execution --------------------------------------------------------------------------------
     def _launch_step(self):
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         for name, s, extra in self.calls:
             lib.call(name, ctypes.byref(s), *extra, st)
-        lib.call("dv3_inc_advance", ctypes.c_void_p(self.t.data_ptr()), st)
+        if self.slots:
+            lib.call("dv3_inc_stop_rows", *self._stop_args, st)
+            lib.call("dv3_inc_advance_rows", ctypes.c_void_p(self.t.data_ptr()),
+                     ctypes.c_void_p(self.stop.data_ptr()), self.B, st)
+        else:
+            lib.call("dv3_inc_advance", ctypes.c_void_p(self.t.data_ptr()), st)
 
     def run(self, n_steps, use_graph=True):
         if use_graph and self.graph is None:
@@ -273,13 +309,112 @@ def decode_ragged(decoder, encoder_out, text_positions, text_lengths, speaker_em
                    text_lengths=text_lengths)
 
 
+def _constants(decoder, keys, values, text_positions, speaker_embed, Tmax):
+    """The per-utterance constants of the step program, for B rows (call in exact-fp32 mode):
+    [(keys (B, E, Ts), values (B, Ts, E))] per attention layer (key-position embedding added, projected once), the
+    query-position table (B, Tmax, C) and ``addend(f)``: the softsign speaker addend (B, C) of GLU block f, or None."""
+    nyanko = hasattr(decoder, "audio_encoder_modules")
+    B = keys.size(0)
+    if nyanko:
+        if text_positions is not None:
+            keys = keys + decoder.embed_keys_positions(text_positions)
+    else:
+        w = decoder._position_rate(decoder.key_position_rate, decoder.speaker_proj1, speaker_embed)
+        keys = keys + decoder.embed_keys_positions(text_positions, w)
+    frame_pos = torch.arange(1, Tmax + 1, device=keys.device).view(1, -1).repeat(B, 1)
+    if nyanko:
+        pos_table = decoder.embed_query_positions(frame_pos)
+    else:
+        w2 = decoder._position_rate(decoder.query_position_rate, decoder.speaker_proj2, speaker_embed)
+        pos_table = decoder.embed_query_positions(frame_pos, w2)
+    pos_table = pos_table.contiguous()                     # (B, Tmax, C)
+    att_layers = [decoder.attention] if nyanko else [a for a in decoder.attention if a is not None]
+    kv = []
+    for att in att_layers:
+        k_ = keys if att.key_projection is None else att.key_projection(keys)
+        v_ = values if att.value_projection is None else att.value_projection(values)
+        kv.append((k_.transpose(1, 2).contiguous(), v_.contiguous()))
+
+    def addend(f):
+        if f.speaker_proj is None or speaker_embed is None:
+            return None
+        return torch.nn.functional.softsign(f.speaker_proj(speaker_embed)).contiguous()     # (B, C)
+    return kv, pos_table, addend
+
+
+def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, frames, test_inputs=None):
+    """Record one decoder step into prog (B rows): input frame t of ``frames`` (B, Tmax + 1, Fr) -- or of test_inputs
+    (B, Tmax, Fr) -- to output frame t + 1.  spk_of(f) -> _Rows of GLU block f's speaker addend, or None; text_len:
+    int32 (B,) per-row attention lengths, or None (``decode``).  -> states (B, Tmax, Cs), aligns (B, Tmax, Ts),
+    dones (B, Tmax)."""
+    nyanko = hasattr(decoder, "audio_encoder_modules")
+    B, Ts = prog.B, kv[0][0].size(2)
+    Fr = decoder.in_dim * decoder.r
+    C = pos_table.size(-1)
+    prog.keep += [pos_table]
+    states = prog.buf(B, Tmax, C if not nyanko else decoder.last_conv.in_channels)
+    Cs = states.size(-1)
+    aligns = prog.buf(B, Tmax, Ts)
+    dones = prog.buf(B, Tmax)
+    if test_inputs is not None:
+        prog.keep.append(test_inputs)
+        cur = _Rows(test_inputs, Fr, ld=Tmax * Fr, t=Fr)
+    else:
+        cur = _Rows(frames, Fr, ld=(Tmax + 1) * Fr, t=Fr)
+    pos_rows = _Rows(pos_table, C, ld=Tmax * C, t=C)
+    states_rows = _Rows(states, Cs, ld=Tmax * Cs, t=Cs)
+    align_rows = _Rows(aligns, Ts, ld=Tmax * Ts, t=Ts)
+
+    def cursor(force):
+        return prog.cursor(text_len is not None) if force else None
+
+    if nyanko:
+        D = C
+        cat = prog.buf(B, 2 * D)
+        q_in = _Rows(prog.buf(B, D), D)
+        _run_stack(prog, decoder.audio_encoder_modules, cur, last_y=_Rows(cat, D, ld=2 * D, offset=D),
+                   last_y2=q_in, last_yadd=pos_rows)
+        att = decoder.attention
+        q = prog.conv(q_in, att.query_projection)
+        ctx = _Rows(prog.buf(B, E), E)
+        prog.attention(q, kv[0][0], kv[0][1], ctx, align_rows, 1.0, cursor(decoder.force_monotonic_attention),
+                       att.window_backward, att.window_ahead, text_len)
+        prog.conv(ctx, att.out_projection, res1=q_in, y=_Rows(cat, D, ld=2 * D))
+        cur = _run_stack(prog, decoder.audio_decoder_modules, _Rows(cat, 2 * D), last_y=states_rows)
+    else:
+        cur = _run_stack(prog, decoder.preattention, cur, spk_of)
+        n_att = len(kv)
+        n_conv = len(decoder.convolutions)
+        ai = 0
+        for idx, (f, att) in enumerate(zip(decoder.convolutions, decoder.attention)):
+            dst = states_rows if idx == n_conv - 1 else None
+            residual = cur
+            if att is None:
+                cur = prog.conv(cur, f.conv, mode=1, spk=spk_of(f), res1=residual, y=dst)
+                continue
+            q_in = _Rows(prog.buf(B, C), C)                # x + frame position encoding
+            prog.conv(cur, f.conv, mode=1, spk=spk_of(f), y2=q_in, y2_mode=2, yadd=pos_rows)
+            q = prog.conv(q_in, att.query_projection)
+            ctx = _Rows(prog.buf(B, E), E)
+            first = ai == 0
+            prog.attention(q, kv[ai][0], kv[ai][1], ctx, align_rows if first else None,
+                           float(2 ** (n_att - 1)) / n_att, cursor(decoder.force_monotonic_attention[idx]),
+                           att.window_backward, att.window_ahead, text_len)
+            cur = prog.conv(ctx, att.out_projection, res1=q_in, res2=residual, y=dst)
+            ai += 1
+    xraw = _Rows(prog.buf(B, Fr), Fr)
+    prog.conv(states_rows, decoder.last_conv, y=xraw,
+              y2=_Rows(frames, Fr, ld=(Tmax + 1) * Fr, t=Fr, offset=Fr), y2_mode=1)
+    prog.conv(xraw, decoder.fc, act=2, y=_Rows(dones, 1, ld=Tmax, t=1))
+    return states, aligns, dones
+
+
 def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph,
             text_lengths=None):
     if decoder.training:
         raise RuntimeError("incremental_forward only supports eval mode")     # reference conv.py:19-20
     if use_graph is None:
         use_graph = os.environ.get("DV3_INC_GRAPH", "1") == "1"
-    nyanko = hasattr(decoder, "audio_encoder_modules")
     keys, values = encoder_out
     if not keys.is_cuda:
         raise RuntimeError("incremental decoding runs on the GPU only (no CPU fallback)")
@@ -297,105 +432,27 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
     old_math = ops.conv_math
     ops.conv_math = "fp32"                       # one-off set-up GEMMs (projections) in exact fp32
     try:
-        # ---- per-utterance constants --------------------------------------------------------------
-        if nyanko:
-            if text_positions is not None:
-                keys = keys + decoder.embed_keys_positions(text_positions)
-        else:
-            w = decoder._position_rate(decoder.key_position_rate, decoder.speaker_proj1, speaker_embed)
-            keys = keys + decoder.embed_keys_positions(text_positions, w)
         if test_inputs is not None:
             test_inputs = test_inputs.to(torch.float32).contiguous()
             assert test_inputs.size(-1) == Fr
             Tmax = test_inputs.size(1)
         else:
             Tmax = decoder.max_decoder_steps + 1
-        frame_pos = torch.arange(1, Tmax + 1, device=dev).view(1, -1).repeat(B, 1)
-        if nyanko:
-            pos_table = decoder.embed_query_positions(frame_pos)
-        else:
-            w2 = decoder._position_rate(decoder.query_position_rate, decoder.speaker_proj2, speaker_embed)
-            pos_table = decoder.embed_query_positions(frame_pos, w2)
-        pos_table = pos_table.contiguous()                     # (B, Tmax, C)
-        C = pos_table.size(-1)
-        att_layers = [decoder.attention] if nyanko else [a for a in decoder.attention if a is not None]
-        kv = []
-        for att in att_layers:
-            k_ = keys if att.key_projection is None else att.key_projection(keys)
-            v_ = values if att.value_projection is None else att.value_projection(values)
-            kv.append((k_.transpose(1, 2).contiguous(), v_.contiguous()))
+        kv, pos_table, addend = _constants(decoder, keys, values, text_positions, speaker_embed, Tmax)
 
         def spk_of(f):
-            if f.speaker_proj is None or speaker_embed is None:
+            s = addend(f)
+            if s is None:
                 return None
-            s = torch.nn.functional.softsign(f.speaker_proj(speaker_embed)).contiguous()     # (B, C)
             prog.keep.append(s)
             return _Rows(s, s.size(-1))
 
-        # ---- the step program ---------------------------------------------------------------------
         prog = StepProgram(B, dev)
-        prog.keep += [pos_table]
         frames = prog.buf(B, Tmax + 1, Fr)                     # frame 0 = initial input, frame t+1 = output of step t
         if initial_input is not None:
             frames[:, 0] = initial_input.reshape(B, Fr)
-        states = prog.buf(B, Tmax, C if not nyanko else decoder.last_conv.in_channels)
-        Cs = states.size(-1)
-        aligns = prog.buf(B, Tmax, Ts)
-        dones = prog.buf(B, Tmax)
-        if test_inputs is not None:
-            prog.keep.append(test_inputs)
-            cur = _Rows(test_inputs, Fr, ld=Tmax * Fr, t=Fr)
-        else:
-            cur = _Rows(frames, Fr, ld=(Tmax + 1) * Fr, t=Fr)
-        pos_rows = _Rows(pos_table, C, ld=Tmax * C, t=C)
-        states_rows = _Rows(states, Cs, ld=Tmax * Cs, t=Cs)
-        align_rows = _Rows(aligns, Ts, ld=Tmax * Ts, t=Ts)
-
-        def cursor(force):
-            if not force:
-                return None
-            la = torch.zeros(2 * B if ragged else 2, dtype=torch.int32, device=dev)
-            prog.keep.append(la)
-            return la
-
-        if nyanko:
-            D = C
-            cat = prog.buf(B, 2 * D)
-            q_in = _Rows(prog.buf(B, D), D)
-            _run_stack(prog, decoder.audio_encoder_modules, cur, last_y=_Rows(cat, D, ld=2 * D, offset=D),
-                       last_y2=q_in, last_yadd=pos_rows)
-            att = decoder.attention
-            q = prog.conv(q_in, att.query_projection)
-            ctx = _Rows(prog.buf(B, E), E)
-            prog.attention(q, kv[0][0], kv[0][1], ctx, align_rows, 1.0, cursor(decoder.force_monotonic_attention),
-                           att.window_backward, att.window_ahead, text_len)
-            prog.conv(ctx, att.out_projection, res1=q_in, y=_Rows(cat, D, ld=2 * D))
-            cur = _run_stack(prog, decoder.audio_decoder_modules, _Rows(cat, 2 * D), last_y=states_rows)
-        else:
-            cur = _run_stack(prog, decoder.preattention, cur, spk_of)
-            n_att = len(att_layers)
-            n_conv = len(decoder.convolutions)
-            ai = 0
-            for idx, (f, att) in enumerate(zip(decoder.convolutions, decoder.attention)):
-                dst = states_rows if idx == n_conv - 1 else None
-                residual = cur
-                if att is None:
-                    cur = prog.conv(cur, f.conv, mode=1, spk=spk_of(f), res1=residual, y=dst)
-                    continue
-                q_in = _Rows(prog.buf(B, C), C)                # x + frame position encoding
-                prog.conv(cur, f.conv, mode=1, spk=spk_of(f), y2=q_in, y2_mode=2, yadd=pos_rows)
-                q = prog.conv(q_in, att.query_projection)
-                ctx = _Rows(prog.buf(B, E), E)
-                first = ai == 0
-                prog.attention(q, kv[ai][0], kv[ai][1], ctx, align_rows if first else None,
-                               float(2 ** (n_att - 1)) / n_att, cursor(decoder.force_monotonic_attention[idx]),
-                               att.window_backward, att.window_ahead, text_len)
-                cur = prog.conv(ctx, att.out_projection, res1=q_in, res2=residual, y=dst)
-                ai += 1
-        xraw = _Rows(prog.buf(B, Fr), Fr)
-        prog.conv(states_rows, decoder.last_conv, y=xraw,
-                  y2=_Rows(frames, Fr, ld=(Tmax + 1) * Fr, t=Fr, offset=Fr), y2_mode=1)
-        prog.conv(xraw, decoder.fc, act=2, y=_Rows(dones, 1, ld=Tmax, t=1))
+        states, aligns, dones = _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, frames,
+                                               test_inputs)
     finally:
         ops.conv_math = old_math
 
@@ -426,3 +483,196 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
     outputs = frames[:, 1:N + 1].contiguous()
     done_list = [dones[:, t].reshape(B, 1, 1).clone() for t in range(N)]
     return outputs, aligns[:, :N].clone(), done_list, states[:, :N].contiguous()
+
+
+def _refill_table(entries, device):
+    """[(dst tensor, src tensor or None, row_bytes, byte offset)] -> the Dv3IncRefill table on the device: row b is
+    row_bytes from the offset of dst's b-th slice along dim 0; src (dst's shape) holds one row per refilled slot."""
+    table = (Dv3IncRefill * len(entries))()
+    for e, (dst, src, row_bytes, offset) in zip(table, entries):
+        stride = dst.stride(0) * dst.element_size()
+        assert dst.is_contiguous() and row_bytes % 4 == 0 and stride % 4 == 0 and offset % 4 == 0
+        e.dst, e.row_bytes, e.dst_row_stride = dst.data_ptr() + offset, row_bytes, stride
+        if src is not None:
+            assert src.is_contiguous() and src.shape[1:] == dst.shape[1:] and src.dtype == dst.dtype
+            e.src, e.src_row_stride = src.data_ptr(), stride
+    return torch.frombuffer(bytearray(table), dtype=torch.uint8).to(device)
+
+
+def _reset_entries(prog, frames):
+    """Refill-table entries that return a slot of a slot program to the state of a fresh one: zero ring rows, cursors
+    (int[2][B]), step counter and stop step, and a zero go frame frames[b, 0]."""
+    B = prog.B
+    entries = [(r, None, r[0].numel() * 4, 0) for r in prog.rings]
+    entries += [(c, None, 4, half * B * 4) for c in prog.cursors for half in (0, 1)]
+    return entries + [(prog.t, None, 4, 0), (prog.stop, None, 4, 0), (frames, None, frames.size(2) * 4, 0)]
+
+
+@torch.no_grad()
+def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_timer=None):
+    """Continuous batching: decode many utterances on a fixed set of ``slots`` decoder rows, refilling a row with the
+    next waiting utterance as soon as its own one stops.
+
+    requests: iterable of (request_id, keys (T, E), values (T, E), text_positions (T,), speaker_embed (D,) or None) --
+    one utterance's encoder outputs -- consumed lazily, as slots free up.  Yields, in completion order,
+    (request_id, outputs (N, in_dim*r), alignment (N, T), dones (N,), decoder_states (N, C), N): what ``decode`` gives
+    for that utterance alone (free-running, from a zero go frame), bit for bit -- every step kernel computes row b from
+    row b's own data at its own step t[b], and a refilled slot starts from the zeros of a fresh program.
+
+    The step program is built and captured once, for ``slots`` rows with the longest text the key-position table holds
+    and max_decoder_steps + 1 frames.  Every ``CHECK_EVERY`` steps the host reads the slots' stop steps (set on the
+    device by the reference stop rule), gathers the finished utterances and reloads their slots in one launch.
+    stats: optional dict, filled with "replays" (steps of the program), "useful_steps" (sum of N), "slots" and
+    "refills" [(replays so far, slots reloaded, slots mid-decode)].  stage_timer: optional ``name -> context
+    manager`` around the decoder work ("decoder"); pulling requests happens outside it."""
+    if decoder.training:
+        raise RuntimeError("incremental_forward only supports eval mode")     # reference conv.py:19-20
+    S = int(slots)
+    if S < 1:
+        raise ValueError("slots must be >= 1, got %r" % (slots,))
+    if use_graph is None:
+        use_graph = os.environ.get("DV3_INC_GRAPH", "1") == "1"
+    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    it = iter(requests)
+    waiting = []
+
+    def take(n):
+        got, waiting[:] = waiting[:n], waiting[n:]
+        while len(got) < n:
+            r = next(it, None)
+            if r is None:
+                break
+            got.append(r)
+        return got
+
+    first = take(1)
+    if not first:
+        return
+    waiting[:] = first
+    keys0 = first[0][1]
+    if not keys0.is_cuda:
+        raise RuntimeError("incremental decoding runs on the GPU only (no CPU fallback)")
+    dev, E = keys0.device, keys0.size(-1)
+    multi = first[0][4] is not None
+    Tp = decoder.embed_keys_positions.num_embeddings - 1      # the longest text: positions 1..Tp index the table
+    Tmax = decoder.max_decoder_steps + 1
+    Fr = decoder.in_dim * decoder.r
+    if stats is not None:
+        stats.update(replays=0, useful_steps=0, slots=S, refills=[])
+
+    def constants(reqs):
+        """per-request constants of a group, padded to its longest text, in exact fp32 as ``_decode`` computes them"""
+        G, L = len(reqs), max(r[1].size(0) for r in reqs)
+        keys = torch.zeros(G, L, E, device=dev)
+        values = torch.zeros(G, L, E, device=dev)
+        tpos = torch.zeros(G, L, dtype=torch.long, device=dev)
+        for g, (_, k, v, p, _) in enumerate(reqs):
+            if (k.size(0) > Tp or (reqs[g][4] is not None) != multi or k.shape != v.shape
+                    or p.shape != k.shape[:1]):
+                raise ValueError("request %r: keys / values (T, %d), T <= %d, text_positions (T,) and a speaker "
+                                 "embedding for every request or for none" % (reqs[g][0], E, Tp))
+            keys[g, :k.size(0)], values[g, :k.size(0)], tpos[g, :k.size(0)] = k, v, p
+        spk = torch.stack([r[4] for r in reqs]) if multi else None
+        old_math = ops.conv_math
+        ops.conv_math = "fp32"
+        try:
+            kv, pos_table, addend = _constants(decoder, keys, values, tpos, spk, Tmax)
+            return kv, pos_table, [addend(f) for f in spk_layers] if spk_layers else []
+        finally:
+            ops.conv_math = old_math
+
+    # ---- the slot program: per-request constants live in slot buffers, loaded from staging by dv3_inc_refill ----
+    spk_layers, spk_slot = [], []
+    prog = StepProgram(S, dev, slots=True)
+    text_len = torch.ones(S, dtype=torch.int32, device=dev)     # idle slots attend one (zero) key
+    with stage("decoder"):
+        kv0, pos0, _ = constants(first)                         # the shapes of the slot buffers
+        kv_slot = [(torch.zeros(S, k.size(1), Tp, device=dev), torch.zeros(S, Tp, v.size(2), device=dev))
+                   for k, v in kv0]
+        pos_slot = torch.zeros(S, Tmax, pos0.size(-1), device=dev)
+
+        def spk_of(f):
+            if f.speaker_proj is None or not multi:
+                return None
+            buf = torch.zeros(S, f.speaker_proj.out_features, device=dev)
+            spk_layers.append(f)
+            spk_slot.append(buf)
+            return _Rows(buf, buf.size(-1))
+
+        old_math = ops.conv_math
+        ops.conv_math = "fp32"
+        try:
+            frames = prog.buf(S, Tmax + 1, Fr)
+            states, aligns, dones = _build_program(decoder, prog, Tmax, E, kv_slot, pos_slot, spk_of, text_len,
+                                                   frames)
+        finally:
+            ops.conv_math = old_math
+        prog.keep += spk_slot
+        prog.stop_rule(dones, decoder.min_decoder_steps, decoder.max_decoder_steps)
+
+        # staging: row i holds the constants of the i-th slot of the next refill
+        kv_stage = [(torch.zeros_like(k), torch.zeros_like(v)) for k, v in kv_slot]
+        pos_stage, len_stage = torch.zeros_like(pos_slot), torch.ones_like(text_len)
+        spk_stage = [torch.zeros_like(b) for b in spk_slot]
+        slot_list = torch.zeros(S, dtype=torch.int32, device=dev)
+        entries = _reset_entries(prog, frames)
+        entries += [(text_len, len_stage, 4, 0), (pos_slot, pos_stage, pos_slot[0].numel() * 4, 0)]
+        for (k, v), (ks, vs) in zip(kv_slot, kv_stage):
+            entries += [(k, ks, k[0].numel() * 4, 0), (v, vs, v[0].numel() * 4, 0)]
+        entries += [(b, bs, b[0].numel() * 4, 0) for b, bs in zip(spk_slot, spk_stage)]
+        table = _refill_table(entries, dev)
+        prog.keep += [table, slot_list, kv_stage, pos_stage, len_stage, spk_stage]
+
+    occupant = [None] * S                                       # (request_id, text length) per slot
+    replays = 0
+
+    def load(free):
+        """load the next waiting requests into the free slots (one refill launch); -> slots loaded"""
+        reqs = take(len(free))
+        if not reqs:
+            return []
+        with stage("decoder"):
+            kv, pos, spk = constants(reqs)
+            G = len(reqs)
+            for (k, v), (ks, vs) in zip(kv, kv_stage):
+                ks[:G, :, :k.size(2)] = k
+                vs[:G, :v.size(1)] = v
+            pos_stage[:G] = pos
+            for s, ss in zip(spk, spk_stage):
+                ss[:G] = s
+            lens = [r[1].size(0) for r in reqs]
+            len_stage[:G] = torch.tensor(lens, dtype=torch.int32)
+            slot_list[:G] = torch.tensor(free[:G], dtype=torch.int32)
+            st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            lib.call("dv3_inc_refill", ctypes.c_void_p(table.data_ptr()), len(entries),
+                     ctypes.c_void_p(slot_list.data_ptr()), G, st)
+        for b, r, n in zip(free, reqs, lens):
+            occupant[b] = (r[0], n)
+        return free[:G]
+
+    load(list(range(S)))
+    while any(o is not None for o in occupant):
+        with stage("decoder"):
+            prog.run(CHECK_EVERY, use_graph)
+            replays += CHECK_EVERY
+            stop = prog.stop.tolist()
+        free = []
+        for b in range(S):
+            if occupant[b] is None or stop[b] <= 0:
+                continue
+            rid, L = occupant[b]
+            n = stop[b]
+            out = (rid, frames[b, 1:n + 1].clone(), aligns[b, :n, :L].clone(), dones[b, :n].clone(),
+                   states[b, :n].clone(), n)
+            occupant[b] = None
+            free.append(b)
+            if stats is not None:
+                stats["useful_steps"] += n
+            yield out
+        if free:
+            busy = sum(o is not None for o in occupant)
+            loaded = load(free)
+            if stats is not None and loaded:
+                stats["refills"].append((replays, loaded, busy))
+        if stats is not None:
+            stats["replays"] = replays

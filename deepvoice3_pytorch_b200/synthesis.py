@@ -8,6 +8,11 @@ decoder, converter) -> ``audio.inv_spectrogram``.  ``tts_batch`` runs the same f
 * ``incremental.decode_ragged``: per-row attention length, context scale, monotonic cursor and stopping step;
 * ``audio.inv_spectrogram_batch``: Griffin-Lim over a ragged batch of clips with a deterministic overlap-add.
 
+``tts_stream`` runs the decoder with continuous batching instead (``incremental.decode_stream``): a fixed set of decoder
+slots, each refilled with the next waiting utterance as soon as its own one stops, so no slot idles until the longest
+utterance of a chunk is done.  Finished utterances go through the post-net and vocoder in groups and are yielded as
+they complete.
+
 Every kernel on this path computes a row from that row's data alone, in an order that does not depend on the batch,
 so with ``ops.conv_math = "fp32"`` each result is bit-identical to the one-utterance path.  In the default tensor-core
 mode the batch's larger GEMMs may take the tensor-core kernels where a short single sentence runs on the exact-fp32 ones
@@ -21,9 +26,10 @@ import torch
 from . import audio, incremental, ops
 
 
-def _check_inputs(model, sequences, speaker_ids, batch_size):
+def _check_inputs(model, sequences, speaker_ids, **counts):
+    """-> int64 token arrays, int speaker ids; counts: name=value arguments that must be >= 1 (batch_size, slots)."""
     if len(sequences) == 0:
-        raise ValueError("tts_batch needs at least one sequence")
+        raise ValueError("synthesis needs at least one sequence")
     seqs = []
     max_len = model.seq2seq.decoder.embed_keys_positions.num_embeddings - 1      # positions 1..L index the table
     for i, s in enumerate(sequences):
@@ -43,8 +49,9 @@ def _check_inputs(model, sequences, speaker_ids, batch_size):
             raise ValueError("%d speaker_ids for %d sequences" % (len(speaker_ids), len(seqs)))
     elif model.n_speakers > 1:
         raise ValueError("a multi-speaker model needs speaker_ids")
-    if int(batch_size) < 1:
-        raise ValueError("batch_size must be >= 1, got %r" % (batch_size,))
+    for name, value in counts.items():
+        if int(value) < 1:
+            raise ValueError("%s must be >= 1, got %r" % (name, value))
     if model.training:
         raise RuntimeError("incremental_forward only supports eval mode")         # as incremental.decode
     if not next(model.parameters()).is_cuda:
@@ -74,22 +81,35 @@ def _synthesize_chunk(model, seqs, speaker_ids, stage):
             keys, values = model.seq2seq.encoder(text, speaker_embed=spk)
         with stage("decoder"):
             outputs, aligns, _, states, steps = incremental.decode_ragged(dec, (keys, values), tpos, text_len, spk)
+        aligns = aligns.cpu().numpy()
+    finally:
+        ops.rng.end_forward()
+    post = _postnet_vocode(model, outputs, states, steps, spk, stage)
+    return [(w, aligns[b, :steps[b], :lens[b]], lin, mel) for b, (w, lin, mel) in enumerate(post)]
+
+
+@torch.no_grad()
+def _postnet_vocode(model, outputs, states, steps, spk, stage):
+    """Decoder outputs (B, N, in_dim*r) and states (B, N, C), row b valid for its first steps[b] decoder steps ->
+    [(waveform, spectrogram, mel)] of each row, denormalised and cut to its own frames."""
+    B = outputs.size(0)
+    ops.rng.begin_forward(False, outputs.device)
+    try:
         with stage("converter"):
             mel = outputs.reshape(B, -1, model.mel_dim)
             r = mel.size(1) // outputs.size(1)
             post_in = states.reshape(B, mel.size(1), -1) if model.use_decoder_state_for_postnet_input else mel
-            frames = torch.tensor(steps, dtype=torch.int64).to(dev) * r
+            frames = torch.tensor(steps, dtype=torch.int64).to(outputs.device) * r
             with ops.length_scope(frames, mel.size(1)):
                 linear = model.postnet(post_in, spk)
             up = linear.size(1) // mel.size(1)
-            mel, linear, aligns = mel.cpu().numpy(), linear.cpu().numpy(), aligns.cpu().numpy()
+            mel, linear = mel.cpu().numpy(), linear.cpu().numpy()
     finally:
         ops.rng.end_forward()
     lin_rows = [linear[b, :steps[b] * r * up] for b in range(B)]
     with stage("vocoder"):
         wavs = audio.inv_spectrogram_batch([x.T for x in lin_rows])
-    return [(wavs[b], aligns[b, :steps[b], :lens[b]], audio._denormalize(lin_rows[b]),
-             audio._denormalize(mel[b, :steps[b] * r])) for b in range(B)]
+    return [(wavs[b], audio._denormalize(lin_rows[b]), audio._denormalize(mel[b, :steps[b] * r])) for b in range(B)]
 
 
 def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None):
@@ -106,7 +126,7 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
 
     stage_timer: optional callable ``name -> context manager`` wrapped around each stage ("encoder", "decoder",
     "converter", "vocoder") of every batch, e.g. to time them."""
-    seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size)
+    seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
     order = sorted(range(len(seqs)), key=lambda i: -seqs[i].size)
     out = [None] * len(seqs)
@@ -116,3 +136,69 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
         for i, res in zip(idx, _synthesize_chunk(model, [seqs[i] for i in idx], ids, stage)):
             out[i] = res
     return out
+
+
+def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stage_timer=None, stats=None):
+    """Synthesize many utterances with continuous batching; a generator of (index, (waveform, alignment, spectrogram,
+    mel)) in completion order, each item what ``tts_batch`` gives for that sequence (bit for bit in exact-fp32 mode).
+
+    The encoder runs on groups of ``slots`` waiting sequences (inside a length scope) as the decoder needs them; the
+    decoder is ``incremental.decode_stream`` on ``slots`` rows; finished utterances go through the post-net (inside a
+    length scope on their frames) and Griffin-Lim in groups of ``post_batch``, the last partial group when the decoder
+    is done.  Inputs are checked as ``tts_batch`` checks them, before the first item.  stage_timer: as for
+    ``tts_batch``; stats: a dict ``decode_stream`` fills (decoder occupancy)."""
+    seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, slots=slots, post_batch=post_batch)
+    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    return _stream(model, seqs, speaker_ids, int(slots), int(post_batch), stage, stats)
+
+
+@torch.no_grad()
+def _encode(model, idx, seqs, speaker_ids, stage):
+    """Encode one padded group -> [(index, keys (T, E), values (T, E), text_positions (T,), speaker_embed or None)]."""
+    dev = next(model.parameters()).device
+    lens = [s.size for s in seqs]
+    L = max(lens)
+    text = np.zeros((len(seqs), L), dtype=np.int64)
+    for b, s in enumerate(seqs):
+        text[b, :s.size] = s
+    text = torch.from_numpy(text).to(dev)
+    text_len = torch.tensor(lens, dtype=torch.int64).to(dev)
+    ops.rng.begin_forward(False, dev)
+    try:
+        spk = None if speaker_ids is None else model._speaker_embedding(torch.tensor(speaker_ids).to(dev))
+        with stage("encoder"), ops.length_scope(text_len, L):
+            keys, values = model.seq2seq.encoder(text, speaker_embed=spk)
+    finally:
+        ops.rng.end_forward()
+    return [(i, keys[b, :n], values[b, :n], torch.arange(1, n + 1, device=dev), None if spk is None else spk[b])
+            for b, (i, n) in enumerate(zip(idx, lens))]
+
+
+def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats):
+    def requests():
+        for g in range(0, len(seqs), slots):
+            idx = list(range(g, min(g + slots, len(seqs))))
+            yield from _encode(model, idx, [seqs[i] for i in idx],
+                               None if speaker_ids is None else [speaker_ids[i] for i in idx], stage)
+
+    def flush(group):
+        N = max(r[5] for r in group)
+        Fr, Cs = group[0][1].size(1), group[0][4].size(1)
+        outputs = group[0][1].new_zeros(len(group), N, Fr)
+        states = group[0][4].new_zeros(len(group), N, Cs)
+        for b, r in enumerate(group):
+            outputs[b, :r[5]], states[b, :r[5]] = r[1], r[4]
+        spk = None if speaker_ids is None else \
+            model._speaker_embedding(torch.tensor([speaker_ids[r[0]] for r in group]).to(outputs.device))
+        post = _postnet_vocode(model, outputs, states, [r[5] for r in group], spk, stage)
+        for r, (w, lin, mel) in zip(group, post):
+            yield r[0], (w, r[2].cpu().numpy(), lin, mel)
+
+    group = []
+    for r in incremental.decode_stream(model.seq2seq.decoder, slots, requests(), stats=stats, stage_timer=stage):
+        group.append(r)
+        if len(group) == post_batch:
+            yield from flush(group)
+            group = []
+    if group:
+        yield from flush(group)

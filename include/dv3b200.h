@@ -371,6 +371,29 @@ int dv3_inc_attn_step(const Dv3IncAttn* attn, void* stream);
 int dv3_inc_attn_step_rows(const Dv3IncAttn* attn, const int* text_len, void* stream);
 int dv3_inc_advance(int* t_ptr, void* stream);
 
+/* ---- continuous batching: a fixed set of B decoder slots, each running its own utterance at its own step ----
+ * The _slots step variants read t_ptr as int[B]: row b runs step t_ptr[b] (every per-step stride, the ring slot of
+ * each tap, the filing slot, the alignment row and the cursor parity follow it) with the same per-output arithmetic
+ * as dv3_inc_conv_step / dv3_inc_attn_step_rows, so a row at step t gets the bits those give at step t. */
+int dv3_inc_conv_step_slots(const Dv3IncStep* step, void* stream);
+int dv3_inc_attn_step_slots(const Dv3IncAttn* attn, const int* text_len, void* stream);
+/* The reference stop rule on each row: after step t[b] wrote done[b*done_ld + t[b]], n = t[b]+1 steps ran; if
+ * stop[b] == 0 and (done > 0.5 and n > min_steps, or n > max_steps), stop[b] = n.  done_ld > max_steps. */
+int dv3_inc_stop_rows(const float* done, long long done_ld, const int* t, int* stop, int B, int min_steps,
+                      int max_steps, void* stream);
+/* t[b] += 1 for every row with stop[b] == 0 (every row when stop is NULL).  A stopped row keeps its step and so
+ * recomputes it bit for bit; the host gathers it and refills the slot. */
+int dv3_inc_advance_rows(int* t, const int* stop, int B, void* stream);
+/* One row copy of a slot refill: row b of dst (at dst + b*dst_row_stride bytes) <- row i of src (src + i*src_row_stride)
+ * for the i-th refilled slot b, or zeros when src is NULL.  Pointers, row_bytes and strides are multiples of 4. */
+typedef struct Dv3IncRefill {
+    void* dst; const void* src;
+    long long row_bytes, dst_row_stride, src_row_stride;
+} Dv3IncRefill;
+/* table: n_entries Dv3IncRefill in device memory; slots: n_slots slot indices (int32, device).  One launch resets the
+ * listed slots (ring rows, cursors, counters, go frame) and loads their next utterances' constants from staging. */
+int dv3_inc_refill(const Dv3IncRefill* table, int n_entries, const int* slots, int n_slots, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
