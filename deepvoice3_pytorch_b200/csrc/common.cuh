@@ -118,6 +118,13 @@ __device__ __forceinline__ void split_pair(float v, uint16_t& hi, uint16_t& lo) 
     }
 }
 
+// The single-pass operand (ops.conv_math = "tc1"): plane hi of split_pair alone, the same bits.
+template <int FMT>
+__device__ __forceinline__ uint16_t split_hi(float v) {
+    if (FMT == FMT_F16) return __half_as_ushort(__float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f)));
+    return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

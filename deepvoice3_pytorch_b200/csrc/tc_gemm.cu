@@ -19,6 +19,11 @@
 // accumulator.  Main and cross are two disjoint register tuples: when an in-flight MMA's accumulator partially overlaps
 // the next one's, ptxas serialises the whole wgmma chain (C7511), whatever the register budget.
 //
+// Single-pass mode (NPL = 1, ops.conv_math = "tc1", DESIGN.md section 2.7): each operand travels as its plane p0 alone
+// (fp16 forward, bf16 gradients) and each K = 16 step issues the one MMA p0(A) x p0(W) into the main accumulator: the
+// producer loads one plane per operand, there is no cross accumulator, and the hand-off writes main * gmain.  One
+// kernel body serves both plane counts.
+//
 // tc_conv_kernel is PERSISTENT: one CTA per SM walks a static round-robin list of output tiles and the TMA ring
 // streams across tile boundaries.  Warp roles (512 threads, one setmaxnreg budget per warpgroup):
 //   * warpgroups 0 and 1 = consumers (176 registers): each accumulates 64 of the 128 tile rows in registers (wgmma),
@@ -90,12 +95,13 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     return make_wgmma_desc(saddr, 16, SwizzleOf<BK>::sbo, SwizzleOf<BK>::layout);
 }
 
-// BR = rows of one B-operand box (128, or 64 for problems too small to fill the machine with 128-wide tiles)
-template <int NBOX, int BK, int BR>
+// BR = rows of one B-operand box (128, or 64 for problems too small to fill the machine with 128-wide tiles); NPL =
+// operand planes per stage (2: hi / lo pairs, 1: single pass)
+template <int NBOX, int BK, int BR, int NPL = 2>
 struct TcCfg {
     static constexpr int TILE = 128 * BK * 2;            // A tile (128 rows)
     static constexpr int TILE_B = BR * BK * 2;           // one B box
-    static constexpr int STAGE = 2 * (TILE + NBOX * TILE_B);
+    static constexpr int STAGE = NPL * (TILE + NBOX * TILE_B);
     static constexpr int NCOLS = BR * NBOX;              // columns per accumulator (main, cross)
     // consumer -> epilogue hand-off: the whole fp32 output tile, [128 rows][NCOLS + 1].  The odd pitch keeps the
     // epilogue's column reads (a warp reads one column of 32 consecutive rows) conflict-free; every access is a row
@@ -111,6 +117,14 @@ static_assert(TcCfg<2, 32, 64>::STAGES == 4, "gated forward: 4-stage ring");
 static_assert(TcCfg<1, 32, 128>::STAGES == 4, "128-column conv: 4-stage ring");
 static_assert(TcCfg<1, 64, 64>::STAGES == 3, "64-column conv at BK = 64: 3-stage ring");
 static_assert(TcCfg<1, 32, 64>::STAGES == 6, "64-column conv at BK = 32: 6-stage ring");
+// Single pass: BK = 64 wherever the contraction is a multiple of 64 channels, so a one-plane stage carries 32 KB
+// (4 stages) or 24 KB (6 stages) and feeds the MMA 4 K-steps per barrier round trip (a one-plane BK = 32 stage would
+// carry 12-16 KB for 2).  Chosen from the bytes per stage, not from an A/B of the two BK values (DESIGN.md §2.7).
+static_assert(TcCfg<2, 64, 64, 1>::STAGES == 4, "single-pass gated forward: 4-stage ring");
+static_assert(TcCfg<1, 64, 128, 1>::STAGES == 4, "single-pass 128-column conv at BK = 64: 4-stage ring");
+static_assert(TcCfg<1, 32, 128, 1>::STAGES == 6, "single-pass 128-column conv at BK = 32: 6-stage ring");
+static_assert(TcCfg<1, 64, 64, 1>::STAGES == 6, "single-pass 64-column conv at BK = 64: 6-stage ring");
+static_assert(TcCfg<1, 32, 64, 1>::STAGES == 6, "single-pass 64-column conv at BK = 32: 6-stage ring");
 
 // ---- epilogues -----------------------------------------------------------------------------------------------
 // NOTE on the epilogue loads: residual / addend / bias reads go through __ldg (ld.global.nc) and are issued as a
@@ -212,14 +226,15 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
 // GATED / CONV kernel (persistent, see file header).  N per tile is limited to 128 columns: the main and cross
 // accumulators of a consumer warpgroup take 2 x 64 registers per thread.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int NBOX, int BR, int BK, bool BF16>
+template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
 __global__ void __launch_bounds__(TC_CONV_THREADS, 1)
 tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int tiles_x, int tiles_y,
                int num_tiles) {
     pdl_trigger();
-    using Cfg = TcCfg<NBOX, BK, BR>;
+    static_assert(NPL == 1 || NPL == 2, "one or two operand planes");
+    using Cfg = TcCfg<NBOX, BK, BR, NPL>;
     constexpr int TILE = Cfg::TILE, TILE_B = Cfg::TILE_B, STAGE = Cfg::STAGE, STAGES = Cfg::STAGES, NCOLS = Cfg::NCOLS;
-    constexpr int B_OFF = 2 * TILE;
+    constexpr int B_OFF = NPL * TILE;
     constexpr int NR = NCOLS / 2;                            // registers per accumulator per thread
     constexpr int A_HALF = 64 * BK * 2;                      // rows [64 wg, 64 wg + 64) of the A tile
     static_assert(NCOLS <= 128, "main + cross accumulators must fit in the registers of a consumer thread");
@@ -235,7 +250,10 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     const int n_iters = p.k * p.kb_n;
 
     if (threadIdx.x == 0) {
-        prefetch_tmap(&maps.a[0]); prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.b[0]); prefetch_tmap(&maps.b[1]);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.a[pl]);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.b[pl]);
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         mbar_init(acc_full, 256);
         mbar_init(acc_empty, 128);
@@ -282,7 +300,7 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
                     const int by0 = j * p.rows_per_tap + b_row0, by1 = j * p.rows_per_tap + b_row1;
                     mbar_arrive_expect_tx(&full[s], STAGE);
 #pragma unroll
-                    for (int pl = 0; pl < 2; ++pl) {
+                    for (int pl = 0; pl < NPL; ++pl) {
                         tma_load_3d(st + pl * TILE, &maps.a[pl], &full[s], ax, ay, a_z);
                         uint8_t* bdst = st + B_OFF + pl * NBOX * TILE_B;
                         tma_load_3d(bdst, &maps.b[pl], &full[s], ax, by0, 0);
@@ -296,13 +314,16 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         const int wg = warp >> 2, wq = warp & 3;
         // Two disjoint register tuples: an MMA in flight may not share accumulator registers with the next one, or
         // ptxas serialises every wgmma of the chain.
-        float acc[NR], xacc[NR];                             // main (p0 x p0), cross (p0 x p1 + p1 x p0)
+        float acc[NR], xacc[NPL == 2 ? NR : 1];              // main (p0 x p0), cross (p0 x p1 + p1 x p0)
         int it = 0, n = 0;
         for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
             int a_row0, a_z, b_row0, b_row1;
             decode(tile, a_row0, a_z, b_row0, b_row1);
 #pragma unroll
-            for (int i = 0; i < NR; ++i) { acc[i] = 0.f; xacc[i] = 0.f; }
+            for (int i = 0; i < NR; ++i) {
+                acc[i] = 0.f;
+                if constexpr (NPL == 2) xacc[i] = 0.f;
+            }
             for (int kit = 0; kit < n_iters; ++kit, ++it) {
                 const int s = it % STAGES, ph = (it / STAGES) & 1;
                 mbar_wait(&full[s], ph);
@@ -312,11 +333,13 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
 #pragma unroll
                 for (int kk = 0; kk < BK / 16; ++kk) {
                     const uint32_t ko = kk * 32;
-                    const uint64_t a0 = make_desc<BK>(sa + ko), a1 = make_desc<BK>(sa + TILE + ko);
-                    const uint64_t b0 = make_desc<BK>(sb + ko), b1 = make_desc<BK>(sb + NBOX * TILE_B + ko);
+                    const uint64_t a0 = make_desc<BK>(sa + ko), b0 = make_desc<BK>(sb + ko);
                     wgmma_mma<NCOLS, 0, 0>(BF16, acc, a0, b0, 1);
-                    wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a0, b1, 1);
-                    wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a1, b0, 1);
+                    if constexpr (NPL == 2) {
+                        const uint64_t a1 = make_desc<BK>(sa + TILE + ko), b1 = make_desc<BK>(sb + NBOX * TILE_B + ko);
+                        wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a0, b1, 1);
+                        wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a1, b0, 1);
+                    }
                 }
                 wgmma_commit();
                 wgmma_wait<1>();                                  // the previous stage's MMAs have retired
@@ -326,9 +349,11 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
             if (n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
             mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous tile
 #pragma unroll
-            for (int i = 0; i < NR; ++i)                              // lo planes carry 2^11
-                acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)] =
-                    fmaf(xacc[i], LO_INV, acc[i] * p.gmain);
+            for (int i = 0; i < NR; ++i) {                            // lo planes carry 2^11
+                float* dst = &acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)];
+                if constexpr (NPL == 2) *dst = fmaf(xacc[i], LO_INV, acc[i] * p.gmain);
+                else *dst = acc[i] * p.gmain;
+            }
             mbar_arrive(acc_full);
         }
     }
@@ -354,13 +379,21 @@ struct TcMnParams {
 };
 
 constexpr int WG_BOX = 64 * 32 * 2;                      // 64 channels x 32 time steps of bf16 = 4 KB
-constexpr int WG_STAGE = 2 * (2 * WG_BOX + 2 * WG_BOX);  // per plane: 128 channels of m, 128 channels of n
-constexpr int WG_STAGES = ((SMEM_LIMIT - 2048) / WG_STAGE) > 6 ? 6 : ((SMEM_LIMIT - 2048) / WG_STAGE);
-constexpr int WG_SMEM = WG_STAGES * WG_STAGE + 1024 + 512;
+// per plane: 128 channels of m, 128 channels of n; NPL planes per stage, at most 6 stages
+template <int NPL>
+struct WgCfg {
+    static constexpr int STAGE = NPL * (2 * WG_BOX + 2 * WG_BOX);
+    static constexpr int STAGES = ((SMEM_LIMIT - 2048) / STAGE) > 6 ? 6 : ((SMEM_LIMIT - 2048) / STAGE);
+    static constexpr int SMEM = STAGES * STAGE + 1024 + 512;
+};
+static_assert(WgCfg<2>::STAGES == 6 && WgCfg<1>::STAGES == 6, "weight gradient: 6-stage ring");
 
+template <int NPL>
 __global__ void __launch_bounds__(TC_WGRAD_THREADS, 1)
 tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcMnParams p) {
     pdl_trigger();
+    static_assert(NPL == 1 || NPL == 2, "one or two operand planes");
+    constexpr int WG_STAGE = WgCfg<NPL>::STAGE, WG_STAGES = WgCfg<NPL>::STAGES;
     constexpr int A_PL = 2 * WG_BOX, B_PL = 2 * WG_BOX;
     constexpr uint32_t LBO = 4096, SBO = 1024;           // 64-channel chunks one TMA box apart; 8-row groups 1 KB apart
     extern __shared__ uint8_t smem_raw[];
@@ -376,7 +409,10 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
     const int n_iters = (b_end > b_beg ? b_end - b_beg : 0) * p.kb_n;
 
     if (threadIdx.x == 0) {
-        prefetch_tmap(&maps.a[0]); prefetch_tmap(&maps.a[1]); prefetch_tmap(&maps.b[0]); prefetch_tmap(&maps.b[1]);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.a[pl]);
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.b[pl]);
         for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         fence_barrier_init();
     }
@@ -393,13 +429,13 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
                 const int b = b_beg + bi, t0 = tc_ * 32;
                 mbar_arrive_expect_tx(&full[s], WG_STAGE);
 #pragma unroll
-                for (int pl = 0; pl < 2; ++pl) {
+                for (int pl = 0; pl < NPL; ++pl) {
 #pragma unroll
                     for (int h = 0; h < 2; ++h)
                         tma_load_3d(st + pl * A_PL + h * WG_BOX, &maps.a[pl], &full[s], m0 + h * 64, t0, b);
 #pragma unroll
                     for (int q = 0; q < 2; ++q)
-                        tma_load_3d(st + 2 * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], &full[s], n0 + q * 64,
+                        tma_load_3d(st + NPL * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], &full[s], n0 + q * 64,
                                     t0 + p.tap_off[wg_j], b);
                 }
             }
@@ -407,9 +443,9 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
     } else {
         // A = gradient planes, B = the bf16 copy of the forward operand planes; both MN-major
         const int wg = warp >> 2, wq = warp & 3;
-        float acc[128];                                      // [0, 64): main, [64, 128): cross
+        float acc[NPL * 64];                                 // [0, 64): main, [64, 128): cross
 #pragma unroll
-        for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+        for (int i = 0; i < NPL * 64; ++i) acc[i] = 0.f;
         for (int it = 0; it < n_iters; ++it) {
             const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
             mbar_wait(&full[s], ph);
@@ -419,12 +455,14 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
             for (int kk = 0; kk < 2; ++kk) {                        // 2 x K = 16 rows of 128 B
                 const uint32_t ko = kk * 16 * 128;
                 const uint64_t a0 = make_wgmma_desc(sa + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
-                const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
-                const uint64_t b0 = make_wgmma_desc(sa + 2 * A_PL + ko, LBO, SBO, WG_SW128);
-                const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
+                const uint64_t b0 = make_wgmma_desc(sa + NPL * A_PL + ko, LBO, SBO, WG_SW128);
                 wgmma_mma<128, 1, 1>(true, acc, a0, b0, 1);
-                wgmma_mma<128, 1, 1>(true, acc + 64, a0, b1, 1);
-                wgmma_mma<128, 1, 1>(true, acc + 64, a1, b0, 1);
+                if constexpr (NPL == 2) {
+                    const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+                    const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
+                    wgmma_mma<128, 1, 1>(true, acc + 64, a0, b1, 1);
+                    wgmma_mma<128, 1, 1>(true, acc + 64, a1, b0, 1);
+                }
             }
             wgmma_commit();
             wgmma_wait<1>();
@@ -438,7 +476,8 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
             const int m = m0 + 64 * wg + frag_row(i, wq, lane), n = n0 + frag_col(i, lane);
             if (m < p.Mw && n < p.Nw) {
                 const size_t ma = (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh;
-                out[ma + (size_t)n * p.s_n] = fmaf(acc[64 + i], LO_INV, acc[i] * gmain);
+                if constexpr (NPL == 2) out[ma + (size_t)n * p.s_n] = fmaf(acc[64 + i], LO_INV, acc[i] * gmain);
+                else out[ma + (size_t)n * p.s_n] = acc[i] * gmain;
             }
         }
     }
@@ -490,11 +529,11 @@ static int ensure_smem(K kern, int bytes, const char* what) {
     return 0;
 }
 
-template <int MODE, int NBOX, int BR, int BK, bool BF16>
+template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
 static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
                        const char* what) {
-    using Cfg = TcCfg<NBOX, BK, BR>;
-    auto kern = tc_conv_kernel<MODE, NBOX, BR, BK, BF16>;
+    using Cfg = TcCfg<NBOX, BK, BR, NPL>;
+    auto kern = tc_conv_kernel<MODE, NBOX, BR, BK, BF16, NPL>;
     static const int configured = ensure_smem(kern, Cfg::SMEM, what);       // once per instantiation, thread-safe
     if (configured) return 1;
     const int sms = config().sms;
@@ -506,11 +545,12 @@ static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, i
     return check_launch(what);
 }
 
-template <int MODE, int NBOX, int BR, int BK>
+template <int MODE, int NBOX, int BR, int BK, int NPL = 2>
 static int launch_conv(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
                        const char* what) {
-    if (p.operand_bf16) return launch_conv_fmt<MODE, NBOX, BR, BK, true>(maps, p, tiles_x, tiles_y, batch, st, what);
-    return launch_conv_fmt<MODE, NBOX, BR, BK, false>(maps, p, tiles_x, tiles_y, batch, st, what);
+    if (p.operand_bf16)
+        return launch_conv_fmt<MODE, NBOX, BR, BK, true, NPL>(maps, p, tiles_x, tiles_y, batch, st, what);
+    return launch_conv_fmt<MODE, NBOX, BR, BK, false, NPL>(maps, p, tiles_x, tiles_y, batch, st, what);
 }
 
 static void fill_taps_tc(int* tap_off, int k, int dilation, int causal, bool transpose) {
@@ -541,20 +581,20 @@ int dv3_tc_conv_supported(int B, int Cin, int Cout, int T, int k) {
            Cout >= 1;
 }
 
-// Gated forward.  xd: [2][B][T][C] fp16 planes of the (dropped-out) input; w: [2][k][2C][C] fp16 planes of the
-// normalised weight; the rest as dv3_convblock_fwd.  64-channel tiles (64 a | 64 b columns), BK = 32: a BK = 64
-// stage (64 KB) leaves room for only two ring stages, BK = 32 for four (with five, H100: 1.45x faster at C=512,
-// T=800).
+// Gated forward.  xd: [npl][B][T][C] fp16 planes of the (dropped-out) input; w: [npl][k][2C][C] fp16 planes of the
+// normalised weight; the rest as dv3_convblock_fwd.  64-channel tiles (64 a | 64 b columns).  Two planes: BK = 32,
+// a BK = 64 stage (64 KB) leaves room for only two ring stages, BK = 32 for four (with five, H100: 1.45x faster at
+// C=512, T=800).  One plane: BK = 64 (C % 128 == 0), four 32 KB stages.
 int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bias, const float* spk,
                          const float* res, float* y, float* save_a, float* save_s, int B, int C, int T, int k,
                          int dilation, int causal, int mode, int residual, const void* fuse, void* stream) {
     DV3_REQUIRE(dv3_tc_supported(B, C, T, k), "tc_convblock_fwd: unsupported shape B=%d C=%d T=%d k=%d", B, C, T, k);
-    DV3_REQUIRE(npl == 2, "tc_convblock_fwd: npl must be 2");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_convblock_fwd: npl must be 1 or 2");
     DV3_REQUIRE(fuse == nullptr, "tc_convblock_fwd: fuse must be NULL");
     TcMaps maps;
     const int t_tiles = (T + 127) / 128;
-    constexpr int BK = 32;
-    for (int pl = 0; pl < 2; ++pl) {
+    const int BK = npl == 2 ? 32 : 64;
+    for (int pl = 0; pl < npl; ++pl) {
         if (encode_tmap_bf16_3d(&maps.a[pl], plane(xd, pl, (long long)B * T * C), C, T, B, (uint64_t)C * 2,
                                 (uint64_t)T * C * 2, BK, 128)) return 1;
         if (encode_tmap_bf16_3d(&maps.b[pl], plane(w, pl, (long long)k * 2 * C * C), C, (uint64_t)k * 2 * C, 1,
@@ -566,23 +606,26 @@ int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bi
     p.bias = bias; p.spk = spk; p.res = res; p.y = y; p.save_a = save_a; p.save_s = save_s;
     p.gate_mode = mode; p.residual = residual;
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (BK / 16));
-    p.operand_bf16 = 0;                                          // forward operands: fp16 hi/lo planes
-    return launch_conv<TC_GATED, 2, 64, BK>(maps, p, t_tiles, C / 64, B, (cudaStream_t)stream, "tc_convblock_fwd");
+    p.operand_bf16 = 0;                                          // forward operands: fp16 planes
+    cudaStream_t st = (cudaStream_t)stream;
+    if (npl == 1) return launch_conv<TC_GATED, 2, 64, 64, 1>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
+    return launch_conv<TC_GATED, 2, 64, 32>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
 }
 
 // Generic conv / data-gradient:  out (B, Nc, T) fp32 = sum_j A[b, t+off_j, :] . W[j, n, :]  (+ epilogue)
-//   a: [2][B][T][Kp] planes, Kp = Kc rounded up to 8;  w: [2][k][Nc][Kp] planes (fp16 pairs for a forward conv, bf16
-//   pairs for a data gradient).  transpose_taps = 1 for a data gradient (offsets padl - j*d), 0 for a forward conv.
-// Tile width: 128 output channels, or 64 when 128-wide tiles would leave most of the SMs idle.  BK: 32 for 128-wide
-// tiles (a 64 KB BK = 64 stage would leave two ring stages, BK = 32 gives four); 64 for 64-wide tiles when
-// Kc % 64 == 0 (else 32: the 80-channel mel input, the 513-wide linear output, the 16-wide speaker embedding).
+//   a: [npl][B][T][Kp] planes, Kp = Kc rounded up to 8;  w: [npl][k][Nc][Kp] planes (fp16 for a forward conv, bf16
+//   for a data gradient).  transpose_taps = 1 for a data gradient (offsets padl - j*d), 0 for a forward conv.
+// Tile width: 128 output channels, or 64 when 128-wide tiles would leave most of the SMs idle.  BK with two planes:
+// 32 for 128-wide tiles (a 64 KB BK = 64 stage would leave two ring stages, BK = 32 gives four); 64 for 64-wide tiles
+// when Kc % 64 == 0 (else 32: the 80-channel mel input, the 513-wide linear output, the 16-wide speaker embedding).
+// One plane: 64 whenever Kc % 64 == 0, at both tile widths (stages of half the bytes), else 32.
 int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc, int Nc, int T, int k, int dilation,
                 int causal, int transpose_taps, const float* bias, int relu, float p_drop,
                 const unsigned long long* seed_ptr, unsigned salt, int addmode, const float* e1, const float* e2,
                 float alpha, const void* fuse, void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS_TC && (k == 1 || Nc % 128 == 0) && B <= 65535,
                 "tc_conv: unsupported shape B=%d Kc=%d Nc=%d T=%d k=%d", B, Kc, Nc, T, k);
-    DV3_REQUIRE(npl == 2, "tc_conv: npl must be 2");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_conv: npl must be 1 or 2");
     DV3_REQUIRE(fuse == nullptr, "tc_conv: fuse must be NULL");
     const int Kp = (Kc + 7) / 8 * 8;
     const int t_tiles = (T + 127) / 128;
@@ -590,9 +633,9 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     const long long tiles128 = (long long)t_tiles * ((Nc + 127) / 128) * B;
     const bool narrow = Nc > 64 && (k == 1 || Nc % 64 == 0) && tiles128 < 100;
     const bool k64 = Kc % 64 == 0;
-    const int bk = (narrow && k64) ? 64 : 32, br = narrow ? 64 : 128;
+    const int bk = ((narrow || npl == 1) && k64) ? 64 : 32, br = narrow ? 64 : 128;
     TcMaps maps;
-    for (int pl = 0; pl < 2; ++pl) {
+    for (int pl = 0; pl < npl; ++pl) {
         if (encode_tmap_bf16_3d(&maps.a[pl], plane(a, pl, (long long)B * T * Kp), Kc, T, B, (uint64_t)Kp * 2,
                                 (uint64_t)T * Kp * 2, bk, 128)) return 1;
         if (encode_tmap_bf16_3d(&maps.b[pl], plane(w, pl, (long long)k * Nc * Kp), Kc, (uint64_t)k * Nc, 1,
@@ -607,6 +650,14 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     // forward conv: fp16 activation x fp16 weight planes; data gradient: bf16 gradient x bf16 weight planes
     p.operand_bf16 = transpose_taps ? 1 : 0;
     const int tiles_y = (Nc + br - 1) / br;
+    if (npl == 1) {
+        if (narrow) {
+            if (k64) return launch_conv<TC_CONV, 1, 64, 64, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
+            return launch_conv<TC_CONV, 1, 64, 32, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
+        }
+        if (k64) return launch_conv<TC_CONV, 1, 128, 64, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128,bk64)");
+        return launch_conv<TC_CONV, 1, 128, 32, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
+    }
     if (narrow) {
         if (k64) return launch_conv<TC_CONV, 1, 64, 64>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
         return launch_conv<TC_CONV, 1, 64, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
@@ -631,15 +682,16 @@ int dv3_tc_wgrad_nsplit(int B, int Mw, int Nw, int T, int k) {
     return best;
 }
 
-// Weight gradient from (B,T,C) planes.  dy: [2][B][T][pad8(Mw)], xd: [2][B][T][pad8(Nw)]; partial element (m, n, j) at
-// (m%msplit)*s_m + (m/msplit)*s_mh + n*s_n + j*s_j of split `s` at dw_partials + s*split_stride.
-int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long long split_stride, int B, int Mw,
-                    int Nw, int T, int k, int dilation, int causal, int msplit, long long s_m, long long s_mh,
-                    long long s_n, long long s_j, void* stream) {
+// Weight gradient from (B,T,C) planes.  dy: [npl][B][T][pad8(Mw)], xd: [npl][B][T][pad8(Nw)]; partial element
+// (m, n, j) at (m%msplit)*s_m + (m/msplit)*s_mh + n*s_n + j*s_j of split `s` at dw_partials + s*split_stride.
+int dv3_tc_wgrad_mn_npl(const void* dy, const void* xd, int npl, float* dw_partials, long long split_stride, int B,
+                        int Mw, int Nw, int T, int k, int dilation, int causal, int msplit, long long s_m,
+                        long long s_mh, long long s_n, long long s_j, void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS_TC && B <= 65535, "tc_wgrad_mn: unsupported shape k=%d", k);
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_wgrad_mn: npl must be 1 or 2");
     const int Mp = (Mw + 7) / 8 * 8, Np = (Nw + 7) / 8 * 8;
     TcMaps maps;
-    for (int pl = 0; pl < 2; ++pl) {
+    for (int pl = 0; pl < npl; ++pl) {
         if (encode_tmap_bf16_3d(&maps.a[pl], plane(dy, pl, (long long)B * T * Mp), Mw, T, B, (uint64_t)Mp * 2,
                                 (uint64_t)T * Mp * 2, 64, 32)) return 1;
         if (encode_tmap_bf16_3d(&maps.b[pl], plane(xd, pl, (long long)B * T * Np), Nw, T, B, (uint64_t)Np * 2,
@@ -653,14 +705,27 @@ int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long lon
     p.dw = dw_partials; p.split_stride = split_stride;
     p.msplit = msplit; p.s_m = s_m; p.s_mh = s_mh; p.s_n = s_n; p.s_j = s_j;
     p.gcoef = config().tc_gamma;
+    const dim3 grid((Nw + 127) / 128, (Mw + 127) / 128, p.nsplit * k);
     cudaStream_t st = (cudaStream_t)stream;
-    const int m_tiles = (Mw + 127) / 128;
-    static const int configured = ensure_smem(tc_wgrad_mn_kernel, WG_SMEM, "tc_wgrad_mn");
-    if (configured) return 1;
-    const cudaError_t e = launch_k(tc_wgrad_mn_kernel, dim3((Nw + 127) / 128, m_tiles, p.nsplit * k), dim3(TC_WGRAD_THREADS),
-                                   (size_t)WG_SMEM, st, maps, p);
+    cudaError_t e;
+    if (npl == 1) {
+        static const int configured = ensure_smem(tc_wgrad_mn_kernel<1>, WgCfg<1>::SMEM, "tc_wgrad_mn");
+        if (configured) return 1;
+        e = launch_k(tc_wgrad_mn_kernel<1>, grid, dim3(TC_WGRAD_THREADS), (size_t)WgCfg<1>::SMEM, st, maps, p);
+    } else {
+        static const int configured = ensure_smem(tc_wgrad_mn_kernel<2>, WgCfg<2>::SMEM, "tc_wgrad_mn");
+        if (configured) return 1;
+        e = launch_k(tc_wgrad_mn_kernel<2>, grid, dim3(TC_WGRAD_THREADS), (size_t)WgCfg<2>::SMEM, st, maps, p);
+    }
     if (e != cudaSuccess) { set_error("tc_wgrad_mn: launch failed: %s", cudaGetErrorString(e)); return 1; }
     return check_launch("tc_wgrad_mn");
+}
+
+int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long long split_stride, int B, int Mw,
+                    int Nw, int T, int k, int dilation, int causal, int msplit, long long s_m, long long s_mh,
+                    long long s_n, long long s_j, void* stream) {
+    return dv3_tc_wgrad_mn_npl(dy, xd, 2, dw_partials, split_stride, B, Mw, Nw, T, k, dilation, causal, msplit, s_m,
+                               s_mh, s_n, s_j, stream);
 }
 
 }  // extern "C"

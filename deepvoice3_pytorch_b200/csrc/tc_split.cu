@@ -5,7 +5,8 @@
 // once).  These passes are pure HBM streaming and absorb work the fp32 path does inside its loaders: the conv-input
 // dropout mask, the ReLU mask of the incoming gradient, the bias-gradient reduction and the (B,C,T) <-> (B,T,C)
 // layout change.  Channel pitches are padded to a multiple of 8 (16 bytes, the TMA stride granularity); pad columns
-// are never read (the tensor maps carry the true extent).
+// are never read (the tensor maps carry the true extent).  With one plane (single-pass mode, npl = 1) only the hi
+// plane is computed and written: the same bits as plane 0 of the pair.
 #include <cuda_bf16.h>
 #include "common.cuh"
 
@@ -30,8 +31,8 @@ struct SplitParams {
     const float* in1;          // - | a  | y (relu) or null
     const float* in2;          // - | s  | -
     const float* in3;          // - | x (highway) | -
-    bf16* planes;              // [2][B][T][pitch]
-    bf16* wg;                  // SPLIT_INPUT: bf16 copy [2][B][T][pitch] or null
+    bf16* planes;              // [npl][B][T][pitch]
+    bf16* wg;                  // SPLIT_INPUT: bf16 copy [npl][B][T][pitch] or null
     float* dbias;              // null | [2C] | [C]
     int B, C, T, pitch;
     int mode, residual, relu;  // gate mode (0 GLU, 1 highway), GLU residual flag; ReLU flag
@@ -39,8 +40,22 @@ struct SplitParams {
     const long long* tlen; int tmult;   // or null: frames t >= tmult * tlen[0] are written as 0 (and leave dbias)
 };
 
+// two consecutive channels -> their 16-bit hi words (and, with two planes, lo words) packed as one 32-bit word each
+template <int FMT, int NPL>
+__device__ __forceinline__ void pack_planes(float x0, float x1, uint32_t& h, uint32_t& l) {
+    if constexpr (NPL == 1) {
+        h = (uint32_t)split_hi<FMT>(x0) | ((uint32_t)split_hi<FMT>(x1) << 16);
+    } else {
+        uint16_t h0, l0, h1, l1;
+        split_pair<FMT>(x0, h0, l0);
+        split_pair<FMT>(x1, h1, l1);
+        h = (uint32_t)h0 | ((uint32_t)h1 << 16);
+        l = (uint32_t)l0 | ((uint32_t)l1 << 16);
+    }
+}
+
 // 6 CTAs per SM: holds the gate split (33 KB of shared memory: 6 fit) at 40 registers with the extent mask, no spills.
-template <int KIND>
+template <int KIND, int NPL>
 __global__ void __launch_bounds__(256, 6) plane_split_kernel(const __grid_constant__ SplitParams p) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float sa[64][65];
@@ -121,31 +136,28 @@ __global__ void __launch_bounds__(256, 6) plane_split_kernel(const __grid_consta
             for (int i = 0; i < 8; ++i) e[i] = half ? sb[(cg * 8 + i) % 64][tt] : sa[cg * 8 + i][tt];
             uint32_t h[4], l[4];
 #pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                uint16_t h0, l0, h1, l1;
-                split_pair<FMT>(e[2 * i], h0, l0);
-                split_pair<FMT>(e[2 * i + 1], h1, l1);
-                h[i] = (uint32_t)h0 | ((uint32_t)h1 << 16);
-                l[i] = (uint32_t)l0 | ((uint32_t)l1 << 16);
-            }
+            for (int i = 0; i < 4; ++i) pack_planes<FMT, NPL>(e[2 * i], e[2 * i + 1], h[i], l[i]);
             uint16_t* d = reinterpret_cast<uint16_t*>(p.planes) + off + (half ? C : 0);
             *reinterpret_cast<uint4*>(d) = make_uint4(h[0], h[1], h[2], h[3]);
-            *reinterpret_cast<uint4*>(d + plane) = make_uint4(l[0], l[1], l[2], l[3]);
+            if constexpr (NPL == 2) *reinterpret_cast<uint4*>(d + plane) = make_uint4(l[0], l[1], l[2], l[3]);
             if (KIND == SPLIT_INPUT && p.wg) {
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    uint16_t h0, l0, h1, l1;
-                    split_pair<FMT_BF16>(e[2 * i], h0, l0);
-                    split_pair<FMT_BF16>(e[2 * i + 1], h1, l1);
-                    h[i] = (uint32_t)h0 | ((uint32_t)h1 << 16);
-                    l[i] = (uint32_t)l0 | ((uint32_t)l1 << 16);
-                }
+                for (int i = 0; i < 4; ++i) pack_planes<FMT_BF16, NPL>(e[2 * i], e[2 * i + 1], h[i], l[i]);
                 uint16_t* w = reinterpret_cast<uint16_t*>(p.wg) + off;
                 *reinterpret_cast<uint4*>(w) = make_uint4(h[0], h[1], h[2], h[3]);
-                *reinterpret_cast<uint4*>(w + plane) = make_uint4(l[0], l[1], l[2], l[3]);
+                if constexpr (NPL == 2) *reinterpret_cast<uint4*>(w + plane) = make_uint4(l[0], l[1], l[2], l[3]);
             }
         }
     }
+}
+
+static dim3 split_grid(int B, int C, int T) { return dim3((T + 63) / 64, (C + 63) / 64, B); }
+
+template <int KIND>
+static int launch_split(const SplitParams& p, int npl, void* stream, const char* what) {
+    if (npl == 1) launch_k(plane_split_kernel<KIND, 1>, split_grid(p.B, p.C, p.T), dim3(256), 0, (cudaStream_t)stream, p);
+    else launch_k(plane_split_kernel<KIND, 2>, split_grid(p.B, p.C, p.T), dim3(256), 0, (cudaStream_t)stream, p);
+    return check_launch(what);
 }
 
 }  // namespace dv3
@@ -154,44 +166,41 @@ using namespace dv3;
 
 extern "C" {
 
-static dim3 split_grid(int B, int C, int T) { return dim3((T + 63) / 64, (C + 63) / 64, B); }
-
 static int split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, float p_drop,
                        const unsigned long long* seed_ptr, unsigned salt, const long long* tlen, int tmult,
                        void* stream) {
     DV3_REQUIRE(B <= 65535 && (C + 63) / 64 <= 65535, "tc_split_input: grid too large");
-    DV3_REQUIRE(npl == 2, "tc_split_input: npl must be 2");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_split_input: npl must be 1 or 2");
     DV3_REQUIRE(!tlen || tmult >= 1, "tc_split_input: tmult must be >= 1");
     SplitParams p = {};
     p.in0 = x; p.planes = (bf16*)btc; p.wg = (bf16*)bct; p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8;
     p.p = p_drop; p.seed_ptr = seed_ptr; p.salt = salt; p.tlen = tlen; p.tmult = tmult;
-    launch_k(plane_split_kernel<SPLIT_INPUT>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
-    return check_launch("tc_split_input");
+    return launch_split<SPLIT_INPUT>(p, npl, stream, "tc_split_input");
 }
 
-static int gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
-                          float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
+static int gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, int npl,
+                          void* bct, float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
                           int tmult, void* stream) {
     DV3_REQUIRE(bct == nullptr, "tc_gate_bwd_split: bct must be NULL");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_gate_bwd_split: npl must be 1 or 2");
     DV3_REQUIRE(C % 8 == 0 && (mode == 0 || x != nullptr), "tc_gate_bwd_split: C %% 8 != 0 or highway without x");
     DV3_REQUIRE(!tlen || tmult >= 1, "tc_gate_bwd_split: tmult must be >= 1");
     SplitParams p = {};
     p.in0 = dy; p.in1 = a; p.in2 = s; p.in3 = x; p.planes = (bf16*)btc; p.dbias = dbias;
     p.B = B; p.C = C; p.T = T; p.pitch = 2 * C; p.mode = mode; p.residual = residual; p.tlen = tlen; p.tmult = tmult;
-    launch_k(plane_split_kernel<SPLIT_GATE>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
-    return check_launch("tc_gate_bwd_split");
+    return launch_split<SPLIT_GATE>(p, npl, stream, "tc_gate_bwd_split");
 }
 
-static int grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
-                      int relu, const long long* tlen, int tmult, void* stream) {
+static int grad_split(const float* dy, const float* y, void* btc, int npl, void* bct, float* dbias, int B, int C,
+                      int T, int relu, const long long* tlen, int tmult, void* stream) {
     DV3_REQUIRE(bct == nullptr, "tc_grad_split: bct must be NULL");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_grad_split: npl must be 1 or 2");
     DV3_REQUIRE(!relu || y != nullptr, "tc_grad_split: ReLU backward needs the forward output");
     DV3_REQUIRE(!tlen || tmult >= 1, "tc_grad_split: tmult must be >= 1");
     SplitParams p = {};
     p.in0 = dy; p.in1 = y; p.planes = (bf16*)btc; p.dbias = dbias;
     p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8; p.relu = relu; p.tlen = tlen; p.tmult = tmult;
-    launch_k(plane_split_kernel<SPLIT_GRAD>, split_grid(B, C, T), dim3(256), 0, (cudaStream_t)stream, p);
-    return check_launch("tc_grad_split");
+    return launch_split<SPLIT_GRAD>(p, npl, stream, "tc_grad_split");
 }
 
 int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, int k, int dilation,
@@ -202,12 +211,12 @@ int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int
 
 int dv3_tc_gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
                           float* dbias, int B, int C, int T, int mode, int residual, void* stream) {
-    return gate_bwd_split(dy, a, s, x, btc, bct, dbias, B, C, T, mode, residual, nullptr, 1, stream);
+    return gate_bwd_split(dy, a, s, x, btc, 2, bct, dbias, B, C, T, mode, residual, nullptr, 1, stream);
 }
 
 int dv3_tc_grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
                       int relu, void* stream) {
-    return grad_split(dy, y, btc, bct, dbias, B, C, T, relu, nullptr, 1, stream);
+    return grad_split(dy, y, btc, 2, bct, dbias, B, C, T, relu, nullptr, 1, stream);
 }
 
 // The same with an optional logical time extent in device memory (a batch padded to a bucket): tlen null behaves as
@@ -222,12 +231,24 @@ int dv3_tc_split_input_ext(const float* x, void* btc, int npl, void* bct, int B,
 int dv3_tc_gate_bwd_split_ext(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
                               float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
                               int tmult, void* stream) {
-    return gate_bwd_split(dy, a, s, x, btc, bct, dbias, B, C, T, mode, residual, tlen, tmult, stream);
+    return gate_bwd_split(dy, a, s, x, btc, 2, bct, dbias, B, C, T, mode, residual, tlen, tmult, stream);
 }
 
 int dv3_tc_grad_split_ext(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
                           int relu, const long long* tlen, int tmult, void* stream) {
-    return grad_split(dy, y, btc, bct, dbias, B, C, T, relu, tlen, tmult, stream);
+    return grad_split(dy, y, btc, 2, bct, dbias, B, C, T, relu, tlen, tmult, stream);
+}
+
+// Both gradient splits with the plane count (1 or 2) and the nullable extent: one entry point each for every form.
+int dv3_tc_gate_bwd_split_npl(const float* dy, const float* a, const float* s, const float* x, void* btc, int npl,
+                              void* bct, float* dbias, int B, int C, int T, int mode, int residual,
+                              const long long* tlen, int tmult, void* stream) {
+    return gate_bwd_split(dy, a, s, x, btc, npl, bct, dbias, B, C, T, mode, residual, tlen, tmult, stream);
+}
+
+int dv3_tc_grad_split_npl(const float* dy, const float* y, void* btc, int npl, void* bct, float* dbias, int B, int C,
+                          int T, int relu, const long long* tlen, int tmult, void* stream) {
+    return grad_split(dy, y, btc, npl, bct, dbias, B, C, T, relu, tlen, tmult, stream);
 }
 
 }  // extern "C"

@@ -18,14 +18,14 @@ __global__ void wn_norm_kernel(const float* __restrict__ v, const float* __restr
 }
 
 // pack of one 32 x 32 tile per CTA (block 32x8), see wn_pack_split_tile
-template <int FMTA, int FMTB>
+template <int FMTA, int FMTB, int NPL>
 __global__ void wn_pack_split_kernel(const float* __restrict__ v, const float* __restrict__ scale,
                                      void* __restrict__ outA, long long a_r, long long a_x, long long a_j,
                                      long long a_plane, void* __restrict__ outB, long long b_r, long long b_x,
                                      long long b_j, long long b_plane, int R, int X, int k) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float tile[32][33];
-    wn_pack_split_tile<FMTA, FMTB>(v, scale, outA, a_r, a_x, a_j, a_plane, outB, b_r, b_x, b_j, b_plane, R, X, k,
+    wn_pack_split_tile<FMTA, FMTB, NPL>(v, scale, outA, a_r, a_x, a_j, a_plane, outB, b_r, b_x, b_j, b_plane, R, X, k,
                                    blockIdx.x, blockIdx.y, tile);
 }
 
@@ -40,14 +40,14 @@ __global__ void __launch_bounds__(256) wn_bwd_kernel(float* __restrict__ dw_part
 }
 
 // norm of R rows of length X*k, then the pack of both layouts: outA with lanes along (x,j), outB with lanes along r
-template <int FMTA, int FMTB>
+template <int FMTA, int FMTB, int NPL = 2>
 static int weightnorm_launch(const float* v, const float* g, float* inv_norm, float* scale, void* outA, long long a_r,
                              long long a_x, long long a_j, long long a_plane, void* outB, long long b_r, long long b_x,
                              long long b_j, long long b_plane, int R, int X, int k, cudaStream_t st, const char* what) {
     const int L = X * k;
     launch_k(wn_norm_kernel, ceil_div(R * 32, 256), 256, 0, st, v, g, inv_norm, scale, R, L);
     if (int e = check_launch(what)) return e;
-    launch_k(wn_pack_split_kernel<FMTA, FMTB>, dim3(ceil_div(L, 32), ceil_div(R, 32)), dim3(32, 8), 0, st, v, scale,
+    launch_k(wn_pack_split_kernel<FMTA, FMTB, NPL>, dim3(ceil_div(L, 32), ceil_div(R, 32)), dim3(32, 8), 0, st, v, scale,
              outA, a_r, a_x, a_j, a_plane, outB, b_r, b_x, b_j, b_plane, R, X, k);
     return check_launch(what);
 }
@@ -79,30 +79,30 @@ int dv3_weightnorm_bwd(float* dw_partials, long long split_stride, int nsplit, i
 }
 
 // Weight norm + split for a conv weight v (Cout, Cin, k), g [Cout]:
-//   wfwd: [2][k][Cout][Cinp] fp16 planes (forward operand: rows co, K = ci)
-//   wbwd: [2][k][Cin][Coutp] bf16 planes (data-gradient operand, multiplied with bf16 gradient planes)
+//   wfwd: [npl][k][Cout][Cinp] fp16 planes (forward operand: rows co, K = ci)
+//   wbwd: [npl][k][Cin][Coutp] bf16 planes (data-gradient operand, multiplied with bf16 gradient planes)
 int dv3_tc_weightnorm_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
                           void* wbwd, int Cout, int Cin, int k, void* stream) {
-    DV3_REQUIRE(npl == 2, "tc_weightnorm_fwd: npl must be 2");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_weightnorm_fwd: npl must be 1 or 2");
     const long long Cinp = (Cin + 7) / 8 * 8, Coutp = (Cout + 7) / 8 * 8;
-    return weightnorm_launch<FMT_F16, FMT_BF16>(v, g, inv_norm, scale, wfwd, Cinp, 1, (long long)Cout * Cinp,
-                                                (long long)k * Cout * Cinp, wbwd, 1, Coutp, (long long)Cin * Coutp,
-                                                (long long)k * Cin * Coutp, Cout, Cin, k, (cudaStream_t)stream,
-                                                "tc_weightnorm_fwd");
+    auto launch = npl == 1 ? weightnorm_launch<FMT_F16, FMT_BF16, 1> : weightnorm_launch<FMT_F16, FMT_BF16, 2>;
+    return launch(v, g, inv_norm, scale, wfwd, Cinp, 1, (long long)Cout * Cinp, (long long)k * Cout * Cinp, wbwd, 1,
+                  Coutp, (long long)Cin * Coutp, (long long)k * Cin * Coutp, Cout, Cin, k, (cudaStream_t)stream,
+                  "tc_weightnorm_fwd");
 }
 
 // ConvTranspose1d(k=2,s=2) weight v (Cin, Cout, 2), g [Cin] (norm over dim 0 = Cin), run as a 1x1 conv with
 // 2*Cout output rows ordered (j, co):
-//   wfwd: [2][2*Cout][Cinp] fp16, rows (j,co), K = ci        wbwd: [2][Cin][K2p] bf16, rows ci, K = (j,co)
+//   wfwd: [npl][2*Cout][Cinp] fp16, rows (j,co), K = ci        wbwd: [npl][Cin][K2p] bf16, rows ci, K = (j,co)
 int dv3_tc_weightnorm_convt_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
                                 void* wbwd, int Cin, int Cout, void* stream) {
-    DV3_REQUIRE(npl == 2, "tc_weightnorm_convt_fwd: npl must be 2");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_weightnorm_convt_fwd: npl must be 1 or 2");
     const long long Cinp = (Cin + 7) / 8 * 8, K2p = (2 * Cout + 7) / 8 * 8;
     // r = ci, x = co, j: outA (lanes along (x,j)) = wbwd [ci][j*Cout+co] ; outB (lanes along r) = wfwd [(j*Cout+co)][ci]
-    return weightnorm_launch<FMT_BF16, FMT_F16>(v, g, inv_norm, scale, wbwd, K2p, 1, (long long)Cout,
-                                                (long long)Cin * K2p, wfwd, 1, Cinp, (long long)Cout * Cinp,
-                                                (long long)2 * Cout * Cinp, Cin, Cout, 2, (cudaStream_t)stream,
-                                                "tc_weightnorm_convt_fwd");
+    auto launch = npl == 1 ? weightnorm_launch<FMT_BF16, FMT_F16, 1> : weightnorm_launch<FMT_BF16, FMT_F16, 2>;
+    return launch(v, g, inv_norm, scale, wbwd, K2p, 1, (long long)Cout, (long long)Cin * K2p, wfwd, 1, Cinp,
+                  (long long)Cout * Cinp, (long long)2 * Cout * Cinp, Cin, Cout, 2, (cudaStream_t)stream,
+                  "tc_weightnorm_convt_fwd");
 }
 
 }  // extern "C"

@@ -33,7 +33,8 @@ __global__ void __launch_bounds__(256) wn_norm_batched_kernel(const Dv3WnEntry* 
     wn_norm_row(e.v, e.g, e.inv_norm, e.scale, e.Cout, e.Cin * e.k, (lb * 256 + threadIdx.x) >> 5, threadIdx.x & 31);
 }
 
-// same layouts as dv3_tc_weightnorm_fwd (npl = 2): wfwd [2][k][Cout][Cinp], wbwd [2][k][Cin][Coutp]
+// same layouts as dv3_tc_weightnorm_fwd: wfwd [NPL][k][Cout][Cinp], wbwd [NPL][k][Cin][Coutp]
+template <int NPL>
 __global__ void __launch_bounds__(256) wn_pack_batched_kernel(const Dv3WnEntry* __restrict__ tab, int n) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float tile[32][33];
@@ -42,7 +43,7 @@ __global__ void __launch_bounds__(256) wn_pack_batched_kernel(const Dv3WnEntry* 
     const int lb = blockIdx.x - e.blk_pack;
     const int by = lb / e.pack_gx, bx = lb - by * e.pack_gx;
     const long long Cinp = (e.Cin + 7) / 8 * 8, Coutp = (e.Cout + 7) / 8 * 8;
-    wn_pack_split_tile<FMT_F16, FMT_BF16>(e.v, e.scale, e.wfwd, Cinp, 1, (long long)e.Cout * Cinp,
+    wn_pack_split_tile<FMT_F16, FMT_BF16, NPL>(e.v, e.scale, e.wfwd, Cinp, 1, (long long)e.Cout * Cinp,
                              (long long)e.k * e.Cout * Cinp, e.wbwd, 1, Coutp, (long long)e.Cin * Coutp,
                              (long long)e.k * e.Cin * Coutp, e.Cout, e.Cin, e.k, bx, by, tile);
 }
@@ -65,14 +66,21 @@ using namespace dv3;
 
 extern "C" {
 
-int dv3_tc_weightnorm_fwd_batched(const Dv3WnEntry* table_dev, int n, int norm_blocks, int pack_blocks,
-                                  void* stream) {
+int dv3_tc_weightnorm_fwd_batched_npl(const Dv3WnEntry* table_dev, int n, int norm_blocks, int pack_blocks, int npl,
+                                      void* stream) {
     DV3_REQUIRE(n > 0 && norm_blocks > 0 && pack_blocks > 0, "tc_weightnorm_fwd_batched: empty table");
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_weightnorm_fwd_batched: npl must be 1 or 2");
     cudaStream_t st = (cudaStream_t)stream;
     launch_k(wn_norm_batched_kernel, norm_blocks, 256, 0, st, table_dev, n);
     if (int e = check_launch("tc_weightnorm_fwd_batched(norm)")) return e;
-    launch_k(wn_pack_batched_kernel, pack_blocks, dim3(32, 8), 0, st, table_dev, n);
+    if (npl == 1) launch_k(wn_pack_batched_kernel<1>, pack_blocks, dim3(32, 8), 0, st, table_dev, n);
+    else launch_k(wn_pack_batched_kernel<2>, pack_blocks, dim3(32, 8), 0, st, table_dev, n);
     return check_launch("tc_weightnorm_fwd_batched(pack)");
+}
+
+int dv3_tc_weightnorm_fwd_batched(const Dv3WnEntry* table_dev, int n, int norm_blocks, int pack_blocks,
+                                  void* stream) {
+    return dv3_tc_weightnorm_fwd_batched_npl(table_dev, n, norm_blocks, pack_blocks, 2, stream);
 }
 
 int dv3_weightnorm_bwd_batched(const Dv3WnEntry* table_dev, int n, int bwd_blocks, int accumulate, void* stream) {

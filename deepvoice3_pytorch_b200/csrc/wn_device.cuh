@@ -10,10 +10,13 @@ namespace dv3 {
 // gradients) or FMT_F32, w itself in one fp32 plane (the operands of the exact-fp32 kernels).
 enum { FMT_F32 = 32 };
 
-template <int FMT>
+// NPL = 1: plane hi alone (single-pass mode), the same bits as plane 0 of the pair.
+template <int FMT, int NPL = 2>
 __device__ __forceinline__ void split_store(float v, void* __restrict__ base, size_t idx, size_t plane_stride) {
     if constexpr (FMT == FMT_F32) {
         static_cast<float*>(base)[idx] = v;
+    } else if constexpr (NPL == 1) {
+        static_cast<uint16_t*>(base)[idx] = split_hi<FMT>(v);
     } else {
         uint16_t h, l;
         split_pair<FMT>(v, h, l);
@@ -36,9 +39,9 @@ __device__ __forceinline__ void wn_norm_row(const float* __restrict__ v, const f
 
 // weight-norm pack of one 32(r) x 32(e) tile, block (32, 8): v [R][X][k] fp32, scale[R] = g/||v|| -> w = v * scale
 // in two plane sets of format FMTA / FMTB with element (r,x,j) at r*s_r + x*s_x + j*s_j (either set may be null; the
-// plane stride is unused for FMT_F32): outA is written with lanes along (x,j) (choose the set whose unit stride is
-// s_x), outB with lanes along r (unit stride s_r).
-template <int FMTA, int FMTB>
+// plane stride is unused for FMT_F32 and NPL = 1): outA is written with lanes along (x,j) (choose the set whose unit
+// stride is s_x), outB with lanes along r (unit stride s_r).  NPL: 16-bit planes per set.
+template <int FMTA, int FMTB, int NPL = 2>
 __device__ __forceinline__ void wn_pack_split_tile(const float* __restrict__ v, const float* __restrict__ scale,
                                                    void* __restrict__ outA, long long a_r, long long a_x,
                                                    long long a_j, long long a_plane, void* __restrict__ outB,
@@ -53,7 +56,7 @@ __device__ __forceinline__ void wn_pack_split_tile(const float* __restrict__ v, 
         if (r < R && e < L) {
             w = v[(size_t)r * L + e] * scale[r];
             const int xx = e / k, j = e - xx * k;
-            if (outA) split_store<FMTA>(w, outA, (size_t)(r * a_r + xx * a_x + j * a_j), (size_t)a_plane);
+            if (outA) split_store<FMTA, NPL>(w, outA, (size_t)(r * a_r + xx * a_x + j * a_j), (size_t)a_plane);
         }
         tile[threadIdx.y + 8 * i][threadIdx.x] = w;
     }
@@ -64,7 +67,7 @@ __device__ __forceinline__ void wn_pack_split_tile(const float* __restrict__ v, 
             const int e = e0 + threadIdx.y + 8 * i, r = r0 + threadIdx.x;
             if (r < R && e < L) {
                 const int xx = e / k, j = e - xx * k;
-                split_store<FMTB>(tile[threadIdx.x][threadIdx.y + 8 * i], outB,
+                split_store<FMTB, NPL>(tile[threadIdx.x][threadIdx.y + 8 * i], outB,
                                   (size_t)(r * b_r + xx * b_x + j * b_j), (size_t)b_plane);
             }
         }

@@ -19,7 +19,13 @@ MODE_GLU, MODE_HIGHWAY = 0, 1
 #            GEMMs, bf16 pairs in the gradient GEMMs.  Full-depth preset models match the fp32 oracle at rtol 1e-3 /
 #            atol 1e-4 (tests/test_gpu_models.py).  Shapes the tensor-core kernels do not cover (C % 128 != 0, tiny
 #            GEMMs) run on the exact-fp32 kernels automatically.  ("bf16x3" is accepted as an alias.)
+#   "tc1"    opt-in single pass (DESIGN.md section 2.7): the conv GEMMs take one 16-bit plane per operand and issue one
+#            MMA per K-step with fp32 accumulation -- fp16 operands (TF32-class: 11-bit significands) in the forward GEMMs,
+#            bf16 operands (bf16-autocast class) in the data- and weight-gradient GEMMs.  Everything else keeps the "tc"
+#            arithmetic: the attention kernels, the exact-fp32 fallback shapes, the losses, the optimizer, the
+#            autoregressive step kernels.  Dropout masks are the same bits as in "tc".
 #   "fp32"   exact-fp32 CUDA-core kernels everywhere (csrc/conv.cu, bgemm.cu): much slower, the strict reference mode.
+# A TrainStep records the mode it was built in: its captured graphs hold that mode's kernels and planes.
 conv_math = os.environ.get("DV3_CONV_MATH", "tc")
 
 
@@ -305,24 +311,24 @@ def _pad8(n):
     return (n + 7) // 8 * 8
 
 
-def _tc_weights(v, g):
+def _tc_weights(v, g, npl):
     """Tensor-core weight operands of a conv v (Cout, Cin, k) -> (inv, wfwd, wbwd, bank record or None, side or None):
-    wfwd [2][k][Cout][pad8(Cin)] fp16 pair (forward GEMM), wbwd [2][k][Cin][pad8(Cout)] bf16 pair (data gradient).
-    Without a weight-bank record the per-layer weight norm is started on the side stream -- it depends only on the
-    parameters, so it overlaps the caller's activation split; the caller joins ``side`` before its GEMM."""
-    bank = weight_bank.weights_for(v, g) if weight_bank is not None else None   # planes prepared for this step?
+    wfwd [npl][k][Cout][pad8(Cin)] fp16 planes (forward GEMM), wbwd [npl][k][Cin][pad8(Cout)] bf16 planes (data
+    gradient).  Without a weight-bank record the per-layer weight norm is started on the side stream -- it depends only
+    on the parameters, so it overlaps the caller's activation split; the caller joins ``side`` before its GEMM."""
+    bank = weight_bank.weights_for(v, g, npl) if weight_bank is not None else None   # planes prepared for this step?
     if bank is not None:
         return bank.inv, bank.wfwd, bank.wbwd, bank, None
     Cout, Cin, k = v.shape
     dev = v.device
     inv = torch.empty(Cout, device=dev)
     scale = torch.empty_like(inv)
-    wfwd = torch.empty(2, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16)
-    wbwd = torch.empty(2, k, Cin, _pad8(Cout), device=dev, dtype=torch.bfloat16)
+    wfwd = torch.empty(npl, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16)
+    wbwd = torch.empty(npl, k, Cin, _pad8(Cout), device=dev, dtype=torch.bfloat16)
     side = _SideStream(dev)
     side.keep = scale                 # written and read on the side stream: must outlive the caller's join
     with side:
-        lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), 2, _p(wbwd), Cout, Cin, k,
+        lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cout, Cin, k,
                  _stream())
     return inv, wfwd, wbwd, bank, side
 
@@ -339,7 +345,7 @@ class _TCWeightGrad:
         self.dbias = self.sink[2] if self.sink else torch.zeros(v.shape[0], device=v.device)
         self.side = self.dv = self.dg = self.partials = None
 
-    def start(self, d_planes, x_wg, inv, B, T, dilation, causal):
+    def start(self, d_planes, x_wg, inv, B, T, dilation, causal, npl):
         ctx, v, g, sink = self.ctx, self.v, self.g, self.sink
         if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
             return
@@ -356,8 +362,8 @@ class _TCWeightGrad:
         self.side = _SideStream(v.device)
         with self.side:
             # partials [split][j][M][N]: contiguous float4 stores from the GEMM epilogue
-            lib.call("dv3_tc_wgrad_mn", _p(d_planes), _p(x_wg), _p(partials), numel, B, M, N, T, k, dilation,
-                     int(causal), M, N, 0, 1, M * N, _stream())
+            lib.call("dv3_tc_wgrad_mn_npl", _p(d_planes), _p(x_wg), npl, _p(partials), numel, B, M, N, T, k,
+                     dilation, int(causal), M, N, 0, 1, M * N, _stream())
             if not deferred:
                 _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=k, out=(self.dv, self.dg), accumulate=bool(sink))
 
@@ -370,8 +376,8 @@ class _TCWeightGrad:
 
 
 class _ConvBlockTCFn(torch.autograd.Function):
-    """Same contract as _ConvBlockFn on the tensor-core path: operands are 16-bit hi/lo planes (fp16 pairs in the
-    forward GEMM, bf16 pairs in the gradient GEMMs)."""
+    """Same contract as _ConvBlockFn on the tensor-core path: operands are 16-bit planes, npl per operand (fp16 in the
+    forward GEMM, bf16 in the gradient GEMMs)."""
 
     @staticmethod
     def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training, extent):
@@ -379,24 +385,25 @@ class _ConvBlockTCFn(torch.autograd.Function):
         B, C, T = x.shape
         dev = x.device
         bf = torch.bfloat16
+        npl = _npl()
         need_bwd = any(ctx.needs_input_grad)
         p, seed_t, salt = _drop_args(p_drop, training, dev)
-        inv, wfwd, wbwd, bank, side = _tc_weights(v, g)
-        x_btc = torch.empty(2, B, T, C, device=dev, dtype=torch.float16)        # forward operand (fp16 pair)
-        x_wg = torch.empty(2, B, T, C, device=dev, dtype=bf) if need_bwd else None  # weight-gradient operand
+        inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl)
+        x_btc = torch.empty(npl, B, T, C, device=dev, dtype=torch.float16)        # forward operand (fp16)
+        x_wg = torch.empty(npl, B, T, C, device=dev, dtype=bf) if need_bwd else None  # weight-gradient operand
         seed_ptr = _p(seed_t)
         y = torch.empty_like(x)
         a = torch.empty_like(x) if need_bwd else None
         s = torch.empty_like(x) if need_bwd else None
         if extent is not None and k > 1:    # frames past the logical extent enter the conv as zeros
-            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), 2, _p(x_wg), B, C, T, p, seed_ptr, salt, extent[0],
-                     extent[1], _stream())
+            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), npl, _p(x_wg), B, C, T, p, seed_ptr, salt,
+                     extent[0], extent[1], _stream())
         else:
-            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, C, T, k, dilation, int(causal), p,
+            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, C, T, k, dilation, int(causal), p,
                      seed_ptr, salt, _stream())
         if side is not None:
             side.join()
-        lib.call("dv3_tc_convblock_fwd", _p(x_btc), _p(wfwd), 2, _p(bias), _p(spk), _p(x), _p(y), _p(a), _p(s),
+        lib.call("dv3_tc_convblock_fwd", _p(x_btc), _p(wfwd), npl, _p(bias), _p(spk), _p(x), _p(y), _p(a), _p(s),
                  B, C, T, k, dilation, int(causal), mode, int(residual), None, _stream())
         if need_bwd:
             ctx.save_for_backward(x, v, g, a, s, x_wg, wbwd, inv)
@@ -405,34 +412,37 @@ class _ConvBlockTCFn(torch.autograd.Function):
             ctx.bias_param = bias if bias.is_leaf else None
             ctx.bank = bank
             ctx.extent = extent
+            ctx.npl = npl
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, v, g, a, s, x_wg, wbwd, inv = ctx.saved_tensors
+        npl = ctx.npl                       # the forward's plane count, whatever ops.conv_math says now
         k, dilation, causal, mode, residual, p, salt, has_spk, dev = ctx.cfg
         seed_ptr = _p(ctx.seed_t)          # the forward's own seed snapshot
         dy = _c(dy)
         B, C, T = x.shape
-        d_btc = torch.empty(2, B, T, 2 * C, device=dev, dtype=torch.bfloat16)
+        d_btc = torch.empty(npl, B, T, 2 * C, device=dev, dtype=torch.bfloat16)
         wg = _TCWeightGrad(ctx, v, g)
-        if ctx.extent is not None:          # the gradient past the extent is taken as 0 (see ops.extent_frames)
-            lib.call("dv3_tc_gate_bwd_split_ext", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(wg.dbias), B, C,
-                     T, mode, int(residual), ctx.extent[0], ctx.extent[1], _stream())
-        else:
-            lib.call("dv3_tc_gate_bwd_split", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), None, _p(wg.dbias), B, C, T,
-                     mode, int(residual), _stream())
-        wg.start(d_btc, x_wg, inv, B, T, dilation, causal)
+        # the gradient past the extent is taken as 0 (see ops.extent_frames)
+        ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
+        lib.call("dv3_tc_gate_bwd_split_npl", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), npl, None, _p(wg.dbias), B, C,
+                 T, mode, int(residual), ext_p, ext_m, _stream())
+        wg.start(d_btc, x_wg, inv, B, T, dilation, causal, npl)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
             addmode, e1, e2, alpha = _gate_addend(mode, residual, dy, s)
-            lib.call("dv3_tc_conv", _p(d_btc), _p(wbwd), 2, _p(dx), B, 2 * C, C, T, k, dilation, int(causal), 1,
+            lib.call("dv3_tc_conv", _p(d_btc), _p(wbwd), npl, _p(dx), B, 2 * C, C, T, k, dilation, int(causal), 1,
                      None, 0, p, seed_ptr, salt, addmode, _p(e1), _p(e2), alpha, None, _stream())
         dv, dg, dbias = wg.finish()
         dspk = None
-        if has_spk and ctx.needs_input_grad[4]:     # d_a = hi + lo * 2^-11 of the (B,T,2C) planes, back to (B,C,T)
-            dspk = transpose12((d_btc[0, :, :, :C].float() + d_btc[1, :, :, :C].float() * (1.0 / 2048.0)).contiguous())
+        if has_spk and ctx.needs_input_grad[4]:     # d_a = hi (+ lo * 2^-11) of the (B,T,2C) planes, back to (B,C,T)
+            da = d_btc[0, :, :, :C].float()
+            if npl == 2:
+                da = da + d_btc[1, :, :, :C].float() * (1.0 / 2048.0)
+            dspk = transpose12(da.contiguous())
         return (dx, dv, dg, dbias, dspk) + (None,) * 8
 
 
@@ -447,20 +457,21 @@ class _Conv1dTCFn(torch.autograd.Function):
         dev, bf = x.device, torch.bfloat16
         need_bwd = any(ctx.needs_input_grad)
         Cinp = _pad8(Cin)
-        inv, wfwd, wbwd, bank, side = _tc_weights(v, g)
+        npl = _npl()
+        inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl)
         need_w = need_bwd and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
-        x_btc = torch.empty(2, B, T, Cinp, device=dev, dtype=torch.float16)
-        x_wg = torch.empty(2, B, T, Cinp, device=dev, dtype=bf) if need_w else None
+        x_btc = torch.empty(npl, B, T, Cinp, device=dev, dtype=torch.float16)
+        x_wg = torch.empty(npl, B, T, Cinp, device=dev, dtype=bf) if need_w else None
         y = torch.empty(B, Cout, T, device=dev)
         if extent is not None and k > 1:
-            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, 0.0, None, 0, extent[0],
+            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, 0.0, None, 0, extent[0],
                      extent[1], _stream())
         else:
-            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, k, dilation, int(causal), 0.0,
-                     None, 0, _stream())
+            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, k, dilation, int(causal),
+                     0.0, None, 0, _stream())
         if side is not None:
             side.join()
-        lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), 2, _p(y), B, Cin, Cout, T, k, dilation, int(causal), 0,
+        lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), npl, _p(y), B, Cin, Cout, T, k, dilation, int(causal), 0,
                  _p(bias), int(relu), 0.0, None, 0, 0, None, None, 0.0, None, _stream())
         if need_bwd:
             ctx.save_for_backward(v, g, x_wg, wbwd, inv, y if relu else None)
@@ -468,27 +479,26 @@ class _Conv1dTCFn(torch.autograd.Function):
             ctx.bias_param = bias if bias.is_leaf else None
             ctx.bank = bank
             ctx.extent = extent
+            ctx.npl = npl
         return y
 
     @staticmethod
     def backward(ctx, dy):
         v, g, x_wg, wbwd, inv, y = ctx.saved_tensors
         B, Cin, Cout, T, k, dilation, causal, relu = ctx.cfg
+        npl = ctx.npl
         dy = _c(dy)
         dev = dy.device
-        g_btc = torch.empty(2, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
+        g_btc = torch.empty(npl, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
         wg = _TCWeightGrad(ctx, v, g)
-        if ctx.extent is not None:
-            lib.call("dv3_tc_grad_split_ext", _p(dy), _p(y), _p(g_btc), None, _p(wg.dbias), B, Cout, T, int(relu),
-                     ctx.extent[0], ctx.extent[1], _stream())
-        else:
-            lib.call("dv3_tc_grad_split", _p(dy), _p(y), _p(g_btc), None, _p(wg.dbias), B, Cout, T, int(relu),
-                     _stream())
-        wg.start(g_btc, x_wg, inv, B, T, dilation, causal)
+        ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
+        lib.call("dv3_tc_grad_split_npl", _p(dy), _p(y), _p(g_btc), npl, None, _p(wg.dbias), B, Cout, T, int(relu),
+                 ext_p, ext_m, _stream())
+        wg.start(g_btc, x_wg, inv, B, T, dilation, causal, npl)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(B, Cin, T, device=dev)
-            lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), 2, _p(dx), B, Cout, Cin, T, k, dilation, int(causal), 1, None,
+            lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), npl, _p(dx), B, Cout, Cin, T, k, dilation, int(causal), 1, None,
                      0, 0.0, None, 0, 0, None, None, 0.0, None, _stream())
         dv, dg, dbias = wg.finish()
         return (dx, dv, dg, dbias) + (None,) * 5
@@ -504,47 +514,49 @@ class _ConvT2TCFn(torch.autograd.Function):
         Cout = v.shape[1]
         dev, bf = x.device, torch.bfloat16
         Cinp, K2p = _pad8(Cin), _pad8(2 * Cout)
+        npl = _npl()
         inv = torch.empty(Cin, device=dev)
         scale = torch.empty_like(inv)
-        wfwd = torch.empty(2, 2 * Cout, Cinp, device=dev, dtype=torch.float16)
-        wbwd = torch.empty(2, Cin, K2p, device=dev, dtype=bf)
-        lib.call("dv3_tc_weightnorm_convt_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), 2, _p(wbwd), Cin, Cout,
+        wfwd = torch.empty(npl, 2 * Cout, Cinp, device=dev, dtype=torch.float16)
+        wbwd = torch.empty(npl, Cin, K2p, device=dev, dtype=bf)
+        lib.call("dv3_tc_weightnorm_convt_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cin,
+                 Cout, _stream())
+        x_btc = torch.empty(npl, B, T, Cinp, device=dev, dtype=torch.float16)
+        x_wg = torch.empty(npl, B, T, Cinp, device=dev, dtype=bf)
+        lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, 1, 1, 0, 0.0, None, 0,
                  _stream())
-        x_btc = torch.empty(2, B, T, Cinp, device=dev, dtype=torch.float16)
-        x_wg = torch.empty(2, B, T, Cinp, device=dev, dtype=bf)
-        lib.call("dv3_tc_split_input", _p(x), _p(x_btc), 2, _p(x_wg), B, Cin, T, 1, 1, 0, 0.0, None, 0, _stream())
         bias2 = bias.repeat(2)
         yp = torch.empty(B, 2 * Cout, T, device=dev)
-        lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), 2, _p(yp), B, Cin, 2 * Cout, T, 1, 1, 0, 0, _p(bias2), 0, 0.0,
+        lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), npl, _p(yp), B, Cin, 2 * Cout, T, 1, 1, 0, 0, _p(bias2), 0, 0.0,
                  None, 0, 0, None, None, 0.0, None, _stream())
         y = torch.empty(B, Cout, 2 * T, device=dev)
         lib.call("dv3_interleave2", _p(yp), _p(y), B, Cout, T, 0, _stream())
         ctx.save_for_backward(v, g, x_wg, wbwd, inv)
         ctx.cfg = (B, Cin, Cout, T)
         ctx.extent = extent                 # a 2x upsampler mixes no frames: only its incoming gradient is masked
+        ctx.npl = npl
         return y
 
     @staticmethod
     def backward(ctx, dy):
         v, g, x_wg, wbwd, inv = ctx.saved_tensors
         B, Cin, Cout, T = ctx.cfg
+        npl = ctx.npl
         dy = _c(dy)
         dev, bf = dy.device, torch.bfloat16
         K2p = _pad8(2 * Cout)
         dyp = torch.empty(B, 2 * Cout, T, device=dev)
         lib.call("dv3_interleave2", _p(dy), _p(dyp), B, Cout, T, 1, _stream())
-        g_btc = torch.empty(2, B, T, K2p, device=dev, dtype=bf)
+        g_btc = torch.empty(npl, B, T, K2p, device=dev, dtype=bf)
         db2 = torch.zeros(2 * Cout, device=dev)
-        if ctx.extent is not None:          # dyp is in the input's time units
-            lib.call("dv3_tc_grad_split_ext", _p(dyp), None, _p(g_btc), None, _p(db2), B, 2 * Cout, T, 0,
-                     ctx.extent[0], ctx.extent[1], _stream())
-        else:
-            lib.call("dv3_tc_grad_split", _p(dyp), None, _p(g_btc), None, _p(db2), B, 2 * Cout, T, 0, _stream())
+        ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)     # dyp is in the input's time units
+        lib.call("dv3_tc_grad_split_npl", _p(dyp), None, _p(g_btc), npl, None, _p(db2), B, 2 * Cout, T, 0, ext_p,
+                 ext_m, _stream())
         dbias = db2[:Cout] + db2[Cout:]
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(B, Cin, T, device=dev)
-            lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), 2, _p(dx), B, 2 * Cout, Cin, T, 1, 1, 0, 1, None, 0, 0.0, None,
+            lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), npl, _p(dx), B, 2 * Cout, Cin, T, 1, 1, 0, 1, None, 0, 0.0, None,
                      0, 0, None, None, 0.0, None, _stream())
         dv = dg = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
@@ -553,19 +565,29 @@ class _ConvT2TCFn(torch.autograd.Function):
             numel = v.numel()
             partials = torch.empty(nsplit, numel, device=dev)
             # element (m=(j,co), ci) -> v layout (ci, co, j): ci*2*Cout + co*2 + j
-            lib.call("dv3_tc_wgrad_mn", _p(g_btc), _p(x_wg), _p(partials), numel, B, M, Cin, T, 1, 1, 0, Cout, 2, 1,
-                     2 * Cout, 0, _stream())
+            lib.call("dv3_tc_wgrad_mn_npl", _p(g_btc), _p(x_wg), npl, _p(partials), numel, B, M, Cin, T, 1, 1, 0,
+                     Cout, 2, 1, 2 * Cout, 0, _stream())
             dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
         return dx, dv, dg, dbias, None
 
 
+def math_mode():
+    """conv_math normalised: "tc" (also for its alias "bf16x3"), "tc1" or "fp32"; an unknown value raises."""
+    if conv_math in ("tc", "bf16x3"):
+        return "tc"
+    if conv_math not in ("tc1", "fp32"):
+        raise Dv3Error("unknown conv_math %r" % (conv_math,))
+    return conv_math
+
+
 def _tc_selected():
     """Whether conv_math selects the tensor-core kernels; an unknown value raises."""
-    if conv_math in ("tc", "bf16x3"):
-        return True
-    if conv_math != "fp32":
-        raise Dv3Error("unknown conv_math %r" % (conv_math,))
-    return False
+    return math_mode() != "fp32"
+
+
+def _npl():
+    """16-bit operand planes of the tensor-core conv GEMMs in the current mode: 1 single pass ("tc1"), 2 hi / lo pairs."""
+    return 1 if math_mode() == "tc1" else 2
 
 
 # 16 keeps the 16-wide speaker projections of the multi-speaker model on tensor cores (measured: vctk step 11.8 -> 10.6 ms)

@@ -480,7 +480,10 @@ class TrainStep:
     train_seq2seq / train_postnet: the reference's two-stage training (train.py:655-740).  Seq2seq-only runs
     ``model.seq2seq`` and the mel + done + guided-attention losses; postnet-only runs ``model.postnet`` on the
     ground-truth mel and the linear loss.  The arena, the optimizer state and the gradient norm then cover only the
-    trained part; the other part's parameters keep their bits.  weight_decay / amsgrad: torch.optim.Adam's."""
+    trained part; the other part's parameters keep their bits.  weight_decay / amsgrad: torch.optim.Adam's.
+
+    The step runs in the ``ops.conv_math`` mode current at construction ("tc", "tc1" or "fp32"): its weight bank and
+    captured graphs hold that mode's kernels and operand planes, so ``step()`` under another mode raises ValueError."""
 
     def __init__(self, model, init_lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1, r=1, downsample_step=4,
                  masked_loss_weight=0.5, binary_divergence_weight=0.1, guided_attention_sigma=0.2,
@@ -488,6 +491,7 @@ class TrainStep:
                  lr_schedule=noam_learning_rate_decay, use_graph=False, fused_loss=True, weight_bank=None,
                  train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False):
         check_train_mode(model, train_seq2seq, train_postnet)
+        self.math = ops.math_mode()
         self.model = model
         self.train_seq2seq, self.train_postnet = bool(train_seq2seq), bool(train_postnet)
         # the module whose parameters are trained and checkpointed (reference save_checkpoint, train.py:787-808)
@@ -523,7 +527,7 @@ class TrainStep:
         self.capture_seconds = 0.0          # wall time spent warming up and capturing graphs
         if weight_bank is None:
             weight_bank = os.environ.get("DV3_WEIGHT_BANK", "1") == "1"
-        self.bank = WeightBank() if weight_bank else None
+        self.bank = WeightBank(ops._npl()) if weight_bank else None
         self.arena.broadcast(model)             # replicas start from rank 0's weights (no-op for world == 1)
         # overlapped gradient exchange (world > 1): buckets are all-reduced on a communication stream as soon as the
         # backward pass has finished them; only the last ("rest") bucket is exposed
@@ -679,6 +683,9 @@ class TrainStep:
         graph mode the first shape runs its own exact graph; any other is padded to its bucket (``data.bucket_shape``,
         ``data.pad_to_bucket``) and replays that bucket's graph, with the loss, gradients and update of the unpadded
         batch.  A batch that already carries ``extents`` is its own bucket."""
+        if ops.math_mode() != self.math:
+            raise ValueError("TrainStep was built with ops.conv_math = %r and cannot step under %r: its weight bank and "
+                             "CUDA graphs hold that mode's kernels (build a new TrainStep)" % (self.math, ops.conv_math))
         self.model.train()
         batch = self._mode_batch(batch)
         lr = self.lr_schedule(self.init_lr, self.global_step) if self.lr_schedule else self.init_lr

@@ -10,7 +10,8 @@ launches per step.  Weights do not depend on activations, so ``TrainStep`` lets 
 
 using a device-resident table of ``Dv3WnEntry`` records (include/dv3b200.h).  Layers register themselves the first
 time the tensor-core autograd Functions see them (that step runs the per-layer path); buffers are persistent, so the
-whole thing is CUDA-graph capturable from the second step on.
+whole thing is CUDA-graph capturable from the second step on.  A bank packs the operand planes of the mode it was built
+in (``npl``: 2 planes per operand in ``ops.conv_math = "tc"``, 1 in ``"tc1"``).
 """
 import ctypes
 
@@ -35,15 +36,15 @@ def _pad8(n):
 class _Layer:
     """Persistent per-layer buffers: what dv3_tc_weightnorm_fwd would allocate on every call."""
 
-    def __init__(self, v, g):
+    def __init__(self, v, g, npl=2):
         Cout, Cin, k = v.shape
         dev, bf = v.device, torch.bfloat16
         self.v, self.g = v, g
         self.Cout, self.Cin, self.k = Cout, Cin, k
         self.inv = torch.empty(Cout, device=dev)
         self.scale = torch.empty(Cout, device=dev)
-        self.wfwd = torch.empty(2, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16)
-        self.wbwd = torch.empty(2, k, Cin, _pad8(Cout), device=dev, dtype=bf)
+        self.wfwd = torch.empty(npl, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16)
+        self.wbwd = torch.empty(npl, k, Cin, _pad8(Cout), device=dev, dtype=bf)
         self.partials = None
         self.nsplit = 0
         self.partials_by_shape = {}      # (nsplit, numel) -> buffer: graphs captured at other shapes keep theirs
@@ -67,7 +68,10 @@ def _upload(entries, device):
 
 
 class WeightBank:
-    def __init__(self):
+    def __init__(self, npl=2):
+        if npl not in (1, 2):
+            raise Dv3Error("WeightBank: npl must be 1 or 2")
+        self.npl = npl                   # operand planes packed per layer (the mode the bank was built in)
         self.layers = {}                 # v.data_ptr() -> _Layer, in registration (= forward) order
         self.active = False              # inside TrainStep._forward_backward
         self.fresh = False               # operand planes match the current parameter values
@@ -95,20 +99,21 @@ class WeightBank:
             self._fwd = (_upload(ents, layers[0].v.device), len(ents), nb, pb, layers)
         tab, n, nb, pb, layers = self._fwd
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        lib.call("dv3_tc_weightnorm_fwd_batched", ctypes.c_void_p(tab.data_ptr()), n, nb, pb, st)
+        lib.call("dv3_tc_weightnorm_fwd_batched_npl", ctypes.c_void_p(tab.data_ptr()), n, nb, pb, self.npl, st)
         for L in layers:
             L.prepared = True
         self.fresh = True
 
-    def weights_for(self, v, g):
-        """The prepared (wfwd, wbwd, inv) record of parameter pair (v, g), or None -> caller runs the per-layer
-        kernels (first step, or bank idle).  Unknown layers are registered for the next step."""
-        if not self.active:
+    def weights_for(self, v, g, npl=2):
+        """The prepared (wfwd, wbwd, inv) record of parameter pair (v, g) with ``npl`` planes per operand, or None ->
+        caller runs the per-layer kernels (first step, bank idle, or a bank built for the other plane count).  Unknown
+        layers are registered for the next step."""
+        if not self.active or npl != self.npl:
             return None
         L = self.layers.get(v.data_ptr())
         if L is None:
             if v.dim() == 3 and v.is_leaf and g.is_leaf and not torch.cuda.is_current_stream_capturing():
-                self.layers[v.data_ptr()] = _Layer(v, g)
+                self.layers[v.data_ptr()] = _Layer(v, g, self.npl)
             return None
         if not (self.fresh and L.prepared) or tuple(L.v.shape) != tuple(v.shape):
             return None

@@ -216,9 +216,12 @@ int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long lon
 /* ================= tensor-core ConvBlock / conv path: wgmma + TMA, split 16-bit operands =================
  * Same reference code as dv3_convblock_fwd / dv3_conv1d_fwd / dv3_conv1d_dgrad / dv3_conv1d_wgrad (modules.py:94-100,
  * 145-164, 200-226 and their autograd).  Every fp32 operand is split into a (hi, lo) pair of 16-bit planes (below) and
- * each GEMM issues hi*hi + hi*lo + lo*hi.  Plane buffers are 16-bit device memory laid out [2][...] (the `npl`
- * arguments must be 2); channel pitches are padded to a multiple of 8.  Callers use the exact-fp32 entry points for
- * unsupported shapes. */
+ * each GEMM issues hi*hi + hi*lo + lo*hi.  Plane buffers are 16-bit device memory laid out [npl][...]; channel pitches
+ * are padded to a multiple of 8.  Callers use the exact-fp32 entry points for unsupported shapes.
+ * npl = 2 is the (hi, lo) pair.  npl = 1 is the single-pass mode: every buffer holds plane hi alone ([1][...], the same
+ * bits as plane 0 of the pair: fp16 rn(x) clamped to +-65504 for forward operands, bf16 rn(x) for gradients and the
+ * weight-gradient copy of the input) and each GEMM issues hi*hi only -- TF32-class forward GEMMs, bf16-class gradient
+ * GEMMs, fp32 accumulation.  Entry points without an `npl` argument work on pairs; their _npl forms take both. */
 int dv3_tc_supported(int B, int C, int T, int k);           /* gated block: C % 128 == 0, k <= 8 */
 int dv3_tc_conv_supported(int B, int Cin, int Cout, int T, int k);   /* plain conv: k == 1 or Cout % 128 == 0 */
 /* Operand planes: every fp32 operand x travels as hi = rn16(x), lo = rn16((x - hi) * 2^11) (csrc/common.cuh).
@@ -226,7 +229,8 @@ int dv3_tc_conv_supported(int B, int Cin, int Cout, int T, int k);   /* plain co
  * values are clamped to +-65504); gradient GEMMs multiply bf16 pairs (gradients need the fp32 exponent range for any
  * loss scale) -- a wgmma does not mix operand formats, so a conv input is split into both.
  * x (B,C,T) fp32 -> conv-input dropout -> btc: [2][B][T][Cp] fp16 pair (forward operand, Cp = pad8(C)) and
- * bct (may be NULL): [2][B][T][Cp] bf16 pair of the same values (operand of the weight gradient). npl must be 2. */
+ * bct (may be NULL): [2][B][T][Cp] bf16 pair of the same values (operand of the weight gradient).  npl = 1: btc and bct
+ * hold plane hi alone, [1][B][T][Cp]. */
 int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, int k, int dilation,
                        int causal, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream);
 /* gate backward writing dAB = [da ; db] as planes btc: [2][B][T][2C] (dgrad operand), bct: [2][B][2C][T] (wgrad). */
@@ -246,11 +250,19 @@ int dv3_tc_gate_bwd_split_ext(const float* dy, const float* a, const float* s, c
                               int tmult, void* stream);
 int dv3_tc_grad_split_ext(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
                           int relu, const long long* tlen, int tmult, void* stream);
-/* weight norm + split: v (Cout,Cin,k), g [Cout] -> wfwd: [npl][k][Cout][Cinp] (forward), wbwd: [2][k][Cin][Coutp] (dgrad). */
+/* Both gradient splits with the plane count: btc [npl][B][T][2C] / [npl][B][T][Cp], npl in {1, 2}; tlen / tmult as the
+ * _ext forms (tlen NULL: no extent).  npl = 2 gives what the calls above give. */
+int dv3_tc_gate_bwd_split_npl(const float* dy, const float* a, const float* s, const float* x, void* btc, int npl,
+                              void* bct, float* dbias, int B, int C, int T, int mode, int residual,
+                              const long long* tlen, int tmult, void* stream);
+int dv3_tc_grad_split_npl(const float* dy, const float* y, void* btc, int npl, void* bct, float* dbias, int B, int C,
+                          int T, int relu, const long long* tlen, int tmult, void* stream);
+/* weight norm + split: v (Cout,Cin,k), g [Cout] -> wfwd: [npl][k][Cout][Cinp] (forward), wbwd: [npl][k][Cin][Coutp]
+ * (dgrad); npl in {1, 2}. */
 int dv3_tc_weightnorm_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
                           void* wbwd, int Cout, int Cin, int k, void* stream);
 /* ConvTranspose1d(k=2,s=2) weight v (Cin,Cout,2), g [Cin] as a 1x1 conv with 2*Cout rows ordered (j,co):
- * wfwd: [npl][2*Cout][Cinp], wbwd: [2][Cin][pad8(2*Cout)]. */
+ * wfwd: [npl][2*Cout][Cinp], wbwd: [npl][Cin][pad8(2*Cout)]; npl in {1, 2}. */
 int dv3_tc_weightnorm_convt_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
                                 void* wbwd, int Cin, int Cout, void* stream);
 /* Batched weight norm (csrc/wn_batched.cu): one record per weight-normed conv (v (Cout,Cin,k), g [Cout]); the table
@@ -265,19 +277,22 @@ typedef struct Dv3WnEntry {
     int Cout, Cin, k, nsplit;
     int blk_norm, blk_pack, blk_bwd, pack_gx;
 } Dv3WnEntry;
-/* norm + pack of every record: 2 launches (replaces 2 launches per layer). */
+/* norm + pack of every record: 2 launches (replaces 2 launches per layer).  The _npl form packs npl in {1, 2} planes
+ * per layout (wfwd [npl][k][Cout][Cinp], wbwd [npl][k][Cin][Coutp]); the plain form is npl = 2. */
 int dv3_tc_weightnorm_fwd_batched(const Dv3WnEntry* table_dev, int n, int norm_blocks, int pack_blocks,
                                   void* stream);
+int dv3_tc_weightnorm_fwd_batched_npl(const Dv3WnEntry* table_dev, int n, int norm_blocks, int pack_blocks, int npl,
+                                      void* stream);
 /* split-K reduction + dg / dv of every record: 1 launch; accumulate = 1 adds into dv / dg. */
 int dv3_weightnorm_bwd_batched(const Dv3WnEntry* table_dev, int n, int bwd_blocks, int accumulate, void* stream);
-/* gated forward: xd = btc planes of dv3_tc_split_input, w = wfwd planes [2][k][2C][C]; npl must be 2, fuse is
+/* gated forward: xd = btc planes of dv3_tc_split_input, w = wfwd planes [npl][k][2C][C]; npl in {1, 2}, fuse is
  * reserved and must be NULL. */
 int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bias, const float* spk,
                          const float* res, float* y, float* save_a, float* save_s, int B, int C, int T, int k,
                          int dilation, int causal, int mode, int residual, const void* fuse, void* stream);
 /* generic conv / data gradient: out (B,Nc,T) = sum_j A[b,t+off_j,:].W[j,n,:], then *dropmask, +bias, +addend, relu.
- * a: [2][B][T][pad8(Kc)], w: [2][k][Nc][pad8(Kc)] (fp16 pairs for a forward conv, bf16 pairs for a data gradient);
- * transpose_taps = 1 for a data gradient.  npl must be 2, fuse is reserved and must be NULL. */
+ * a: [npl][B][T][pad8(Kc)], w: [npl][k][Nc][pad8(Kc)] (fp16 planes for a forward conv, bf16 planes for a data
+ * gradient); transpose_taps = 1 for a data gradient.  npl in {1, 2}, fuse is reserved and must be NULL. */
 int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc, int Nc, int T, int k, int dilation,
                 int causal, int transpose_taps, const float* bias, int relu, float p_drop,
                 const unsigned long long* seed_ptr, unsigned salt, int addmode, const float* e1, const float* e2,
@@ -289,6 +304,10 @@ int dv3_tc_wgrad_nsplit(int B, int Mw, int Nw, int T, int k);
 int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long long split_stride, int B, int Mw,
                     int Nw, int T, int k, int dilation, int causal, int msplit, long long s_m, long long s_mh,
                     long long s_n, long long s_j, void* stream);
+/* the same with the plane count: dy [npl][B][T][pad8(Mw)], xd [npl][B][T][pad8(Nw)], npl in {1, 2} */
+int dv3_tc_wgrad_mn_npl(const void* dy, const void* xd, int npl, float* dw_partials, long long split_stride, int B,
+                        int Mw, int Nw, int T, int k, int dilation, int causal, int msplit, long long s_m,
+                        long long s_mh, long long s_n, long long s_j, void* stream);
 
 /* ---- fused training losses + gradients: reference train.py:537-601 (spec_loss, guided_attention) and :704-740.
  * dv3_spec_loss: pairs (y_hat[b,t], y[b,t+r]), t < T-r; lengths int64 [B] valid target frames; adds
