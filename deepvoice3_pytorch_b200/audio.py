@@ -3,8 +3,9 @@
 GPU pass (csrc/stft.cu) instead of two CPU lws STFTs.  ``stft_mel_batch`` is the batched device API the
 preprocessors should use (a whole shard of clips per launch; one H2D, one D2H).
 
-``inv_spectrogram`` (reference audio.py:37-43) is provided with Griffin-Lim phase recovery on the same STFT frame: the
-reference's LWS (``lws`` package) is an un-vendored dependency, so that path's parity is unpinned (csrc/istft.cu).
+``inv_spectrogram`` (reference audio.py:37-43) recovers the phase on the same STFT frame with Griffin-Lim (the default,
+csrc/istft.cu) or with Local Weighted Sums (``method="lws"``, csrc/lws.cu), the algorithm of the reference's
+``lws.run_lws``.  The ``lws`` package is an un-vendored dependency whose source is absent, so parity with it is unpinned.
 """
 import ctypes
 
@@ -27,6 +28,7 @@ class _HP:
     ref_level_db = 20
     power = 1.4                   # spectrogram sharpening before phase recovery (presets/*.json)
     griffin_lim_iters = 60
+    lws_iters = 30                # LWS batch iterations after the no-future initialisation (DESIGN.md section 7)
     rescaling = False             # preprocess.py: y = x / |x|.max() * rescaling_max (hparams.py:46-48)
     rescaling_max = 0.999
     min_text = 20                 # utterances with shorter transcripts are skipped (hparams.py:137)
@@ -205,13 +207,10 @@ def griffin_lim(mag, n_iter=None):
     return griffin_lim_batch(mag[None], [mag.shape[0]], n_iter)[0]
 
 
-def griffin_lim_batch(mag, n_frames, n_iter=None):
-    """mag: (nclips, T_max, 513) fp32 CUDA tensor, clip c valid for its first n_frames[c] frames -> waveforms
-    (nclips, n_max), clip c valid for its first inv_num_samples(n_frames[c]) samples and zero after them.  Each clip
-    comes out bit-identical to ``griffin_lim`` on that clip alone: the kernels read and write only a clip's own frames
-    and samples, and the overlap-add is deterministic (csrc/istft.cu)."""
+def _ragged_clips(mag, n_frames, name):
+    """Checks of a (nclips, T_max, 513) magnitude batch -> (mag, n_max, frames_d, samples_d, stream)."""
     if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 3):
-        raise Dv3Error("griffin_lim_batch needs a (nclips, T, 513) fp32 CUDA tensor; there is no CPU path")
+        raise Dv3Error("%s needs a (nclips, T, 513) fp32 CUDA tensor; there is no CPU path" % name)
     if hparams.fft_size != 1024 or hparams.hop_size != 256 or mag.shape[2] != 513:
         raise Dv3Error("the inverse kernels are built for fft_size=1024, hop_size=256")
     mag = mag.contiguous()
@@ -223,10 +222,19 @@ def griffin_lim_batch(mag, n_frames, n_iter=None):
     if min(n_samples) < 1:
         raise Dv3Error("too few frames (%d) to reconstruct a waveform" % min(n_frames))
     dev = mag.device
-    n_max = max(n_samples)
     frames_d = torch.tensor(n_frames, dtype=torch.int32).to(dev)
     samples_d = torch.tensor(n_samples, dtype=torch.int32).to(dev)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return mag, max(n_samples), frames_d, samples_d, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def griffin_lim_batch(mag, n_frames, n_iter=None):
+    """mag: (nclips, T_max, 513) fp32 CUDA tensor, clip c valid for its first n_frames[c] frames -> waveforms
+    (nclips, n_max), clip c valid for its first inv_num_samples(n_frames[c]) samples and zero after them.  Each clip
+    comes out bit-identical to ``griffin_lim`` on that clip alone: the kernels read and write only a clip's own frames
+    and samples, and the overlap-add is deterministic (csrc/istft.cu)."""
+    mag, n_max, frames_d, samples_d, st = _ragged_clips(mag, n_frames, "griffin_lim_batch")
+    nclips, T_max = mag.shape[:2]
+    dev = mag.device
     spec = torch.zeros(nclips, T_max, 513, 2, device=dev)
     spec[..., 0] = mag                                   # zero phase
     x = torch.zeros(nclips, n_max, device=dev)
@@ -237,6 +245,83 @@ def griffin_lim_batch(mag, n_frames, n_iter=None):
         x.zero_()
         lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
     return x
+
+
+def _lws_weights_fp64():
+    """(7, 11) complex128, [q + 3, d + 5] = beta_q(d) = (1/N) sum_n w(n) w(n - q*hop) exp(-2 pi i d n / N), the sum over
+    the n where both window indices lie in [0, N): the local-weighted-sum weights of csrc/lws.cu."""
+    N, R = 1024, 256
+    n = np.arange(N)
+    w = np.sqrt(0.5 * (1.0 - np.cos(2.0 * np.pi * (n + 0.5) / N)) * 2.0 * R / N)     # istft.cu frame_window
+    beta = np.zeros((7, 11), dtype=np.complex128)
+    for q in range(-3, 4):
+        j = n - q * R
+        ok = (j >= 0) & (j < N)
+        ww = np.where(ok, w * w[np.clip(j, 0, N - 1)], 0.0)
+        for d in range(-5, 6):
+            beta[q + 3, d + 5] = np.sum(ww * np.exp(-2j * np.pi * d * n / N)) / N
+    return beta
+
+
+_lws_weight_cache = {}
+
+
+def _lws_weights(device):
+    """The weights as 77 [re, im] fp32 pairs on ``device`` (computed once per device)."""
+    key = str(device)
+    if key not in _lws_weight_cache:
+        b = _lws_weights_fp64()
+        w = np.stack([b.real, b.imag], axis=-1).astype(np.float32)
+        _lws_weight_cache[key] = torch.from_numpy(np.ascontiguousarray(w)).to(device)
+    return _lws_weight_cache[key]
+
+
+def _check_count(name, value):
+    if int(value) != value or value < 0:
+        raise ValueError("%s must be a non-negative integer, got %r" % (name, value))
+    return int(value)
+
+
+def lws(mag, n_iter=None, init_iters=1):
+    """mag: (T, 513) fp32 CUDA tensor of linear magnitudes -> waveform (n,) by LWS phase recovery: the one-clip case of
+    ``lws_batch``."""
+    n_iter = hparams.lws_iters if n_iter is None else _check_count("n_iter", n_iter)
+    init_iters = _check_count("init_iters", init_iters)
+    if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 2):
+        raise Dv3Error("lws needs a (T, 513) fp32 CUDA tensor; there is no CPU path")
+    return lws_batch(mag[None], [mag.shape[0]], n_iter, init_iters)[0]
+
+
+def lws_batch(mag, n_frames, n_iter=None, init_iters=1):
+    """Local Weighted Sums phase recovery (Le Roux et al., DAFx 2010; the algorithm of the reference's ``lws.run_lws``,
+    parity unpinned: csrc/lws.cu) with the contract of ``griffin_lim_batch``: mag (nclips, T_max, 513), clip c valid
+    for its first n_frames[c] frames -> waveforms (nclips, n_max), zero past each clip's own samples, each clip
+    bit-identical to the clip alone.  The no-future initialisation (``init_iters`` in-frame passes per frame), then
+    ``n_iter`` batch iterations (``hparams.lws_iters`` when None), then the inverse STFT."""
+    n_iter = hparams.lws_iters if n_iter is None else _check_count("n_iter", n_iter)
+    init_iters = _check_count("init_iters", init_iters)
+    mag, n_max, frames_d, samples_d, st = _ragged_clips(mag, n_frames, "lws_batch")
+    nclips, T_max = mag.shape[:2]
+    dev = mag.device
+    w = _lws_weights(dev)
+    spec = torch.empty(nclips, T_max, 513, 2, device=dev)
+    other = torch.empty_like(spec) if n_iter else None
+    lib.call("dv3_lws_nofuture_batched", _cp(mag), _cp(spec), _cp(w), _cp(frames_d), T_max, nclips, init_iters, st)
+    for _ in range(n_iter):
+        lib.call("dv3_lws_iterate_batched", _cp(mag), _cp(spec), _cp(other), _cp(w), _cp(frames_d), T_max, nclips, st)
+        spec, other = other, spec
+    x = torch.zeros(nclips, n_max, device=dev)
+    lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
+    return x
+
+
+PHASE_METHODS = ("griffin_lim", "lws")
+
+
+def check_phase_method(method):
+    if method not in PHASE_METHODS:
+        raise ValueError("method must be one of %s, got %r" % (", ".join(PHASE_METHODS), method))
+    return method
 
 
 def inv_preemphasis(x):
@@ -252,18 +337,23 @@ def inv_preemphasis(x):
     return y.view_as(x)
 
 
-def inv_spectrogram(spectrogram, n_iter=None):
+def inv_spectrogram(spectrogram, n_iter=None, method="griffin_lim"):
     """(513, T) normalised dB spectrogram (what ``spectrogram`` returns / the model predicts, transposed) -> waveform
     float32 numpy array -- reference audio.py:37-43: denormalise, dB -> amplitude, ** power, phase recovery, inverse
     STFT, de-emphasis.  The one-clip case of ``inv_spectrogram_batch``."""
-    return inv_spectrogram_batch([spectrogram], n_iter)[0]
+    return inv_spectrogram_batch([spectrogram], n_iter, method)[0]
 
 
-def inv_spectrogram_batch(spectrograms, n_iter=None):
+def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
     """[(513, T_c) normalised dB spectrograms] -> [waveform c (float32 numpy array)], all clips in one set of launches
-    per Griffin-Lim iteration.  Clip c is bit-identical to ``inv_spectrogram(spectrograms[c])``: the magnitude and
-    de-emphasis kernels work element by element / causally along each clip, and the phase recovery is
-    ``griffin_lim_batch``."""
+    per iteration.  Clip c is bit-identical to ``inv_spectrogram(spectrograms[c])``: the magnitude and de-emphasis
+    kernels work element by element / causally along each clip, and the phase recovery is ``griffin_lim_batch``
+    (``method="griffin_lim"``, ``hparams.griffin_lim_iters`` iterations when n_iter is None) or ``lws_batch``
+    (``method="lws"``, ``hparams.lws_iters``).  An unknown method, or a negative LWS iteration count, raises
+    ValueError before anything runs."""
+    check_phase_method(method)
+    if method == "lws" and n_iter is not None:
+        _check_count("n_iter", n_iter)
     specs = [np.asarray(s, dtype=np.float32) for s in spectrograms]
     if not specs:
         raise ValueError("inv_spectrogram_batch needs at least one spectrogram")
@@ -279,5 +369,6 @@ def inv_spectrogram_batch(spectrograms, n_iter=None):
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     lib.call("dv3_spec_to_amp", _cp(S), _cp(amp), S.numel(), float(hparams.min_level_db), float(hparams.ref_level_db),
              float(hparams.power), st)
-    wav = inv_preemphasis(griffin_lim_batch(amp, n_frames, n_iter)).cpu().numpy()
+    recover = lws_batch if method == "lws" else griffin_lim_batch
+    wav = inv_preemphasis(recover(amp, n_frames, n_iter)).cpu().numpy()
     return [wav[c, :inv_num_samples(t)].copy() for c, t in enumerate(n_frames)]

@@ -16,6 +16,7 @@
 // scalar when the array is NULL) and pitches, so a ragged batch of clips runs in one launch and every clip gets exactly
 // what it gets alone.
 //   deemphasis_kernel       y[n] = x[n] + c*y[n-1] (a 1st-order IIR: one thread per clip, chunks staged through smem)
+// The reference's own algorithm, LWS phase recovery on this frame, is csrc/lws.cu (audio.inv_spectrogram(method="lws")).
 #include "common.cuh"
 
 namespace dv3 {

@@ -6,7 +6,8 @@ decoder, converter) -> ``audio.inv_spectrogram``.  ``tts_batch`` runs the same f
 * encoder and converter inside an ``ops.length_scope``: every row's frames past its own length are zeroed before each
   conv that spans several frames, so each row sees the zero padding it would see alone;
 * ``incremental.decode_ragged``: per-row attention length, context scale, monotonic cursor and stopping step;
-* ``audio.inv_spectrogram_batch``: Griffin-Lim over a ragged batch of clips with a deterministic overlap-add.
+* ``audio.inv_spectrogram_batch``: Griffin-Lim (or LWS, ``vocoder="lws"``) over a ragged batch of clips with a
+  deterministic overlap-add.
 
 ``tts_stream`` runs the decoder with continuous batching instead (``incremental.decode_stream``): a fixed set of decoder
 slots, each refilled with the next waiting utterance as soon as its own one stops, so no slot idles until the longest
@@ -60,7 +61,7 @@ def _check_inputs(model, sequences, speaker_ids, **counts):
 
 
 @torch.no_grad()
-def _synthesize_chunk(model, seqs, speaker_ids, stage):
+def _synthesize_chunk(model, seqs, speaker_ids, stage, vocoder):
     """seqs: list of int64 arrays -> [(waveform, alignment, spectrogram, mel)] for one padded batch."""
     dev = next(model.parameters()).device
     B = len(seqs)
@@ -84,14 +85,15 @@ def _synthesize_chunk(model, seqs, speaker_ids, stage):
         aligns = aligns.cpu().numpy()
     finally:
         ops.rng.end_forward()
-    post = _postnet_vocode(model, outputs, states, steps, spk, stage)
+    post = _postnet_vocode(model, outputs, states, steps, spk, stage, vocoder)
     return [(w, aligns[b, :steps[b], :lens[b]], lin, mel) for b, (w, lin, mel) in enumerate(post)]
 
 
 @torch.no_grad()
-def _postnet_vocode(model, outputs, states, steps, spk, stage):
+def _postnet_vocode(model, outputs, states, steps, spk, stage, vocoder="griffin_lim"):
     """Decoder outputs (B, N, in_dim*r) and states (B, N, C), row b valid for its first steps[b] decoder steps ->
-    [(waveform, spectrogram, mel)] of each row, denormalised and cut to its own frames."""
+    [(waveform, spectrogram, mel)] of each row, denormalised and cut to its own frames; the waveform's phase recovered
+    with ``vocoder`` (an ``audio.inv_spectrogram`` method)."""
     B = outputs.size(0)
     ops.rng.begin_forward(False, outputs.device)
     try:
@@ -108,11 +110,11 @@ def _postnet_vocode(model, outputs, states, steps, spk, stage):
         ops.rng.end_forward()
     lin_rows = [linear[b, :steps[b] * r * up] for b in range(B)]
     with stage("vocoder"):
-        wavs = audio.inv_spectrogram_batch([x.T for x in lin_rows])
+        wavs = audio.inv_spectrogram_batch([x.T for x in lin_rows], method=vocoder)
     return [(wavs[b], audio._denormalize(lin_rows[b]), audio._denormalize(mel[b, :steps[b] * r])) for b in range(B)]
 
 
-def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None):
+def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None, vocoder="griffin_lim"):
     """Synthesize many utterances at once.
 
     model: a ``MultiSpeakerTTSModel`` in eval mode on CUDA.  sequences: list of 1-D token-id arrays (what a text
@@ -122,10 +124,12 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
 
     -> list, in input order, of (waveform, alignment (N_b, L_b), spectrogram, mel): what reference ``synthesis.tts``
     returns for that sequence synthesized alone -- the same decoder steps, the denormalised linear and mel spectrograms
-    cut to the row's own frames, and its Griffin-Lim waveform (see the module docstring for when this is bit-exact).
+    cut to the row's own frames, and its waveform (see the module docstring for when this is bit-exact).
 
     stage_timer: optional callable ``name -> context manager`` wrapped around each stage ("encoder", "decoder",
-    "converter", "vocoder") of every batch, e.g. to time them."""
+    "converter", "vocoder") of every batch, e.g. to time them.  vocoder: the phase recovery of
+    ``audio.inv_spectrogram``, "griffin_lim" (the default) or "lws" (the reference's algorithm); checked first."""
+    audio.check_phase_method(vocoder)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
     order = sorted(range(len(seqs)), key=lambda i: -seqs[i].size)
@@ -133,23 +137,25 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
     for c in range(0, len(order), int(batch_size)):
         idx = order[c:c + int(batch_size)]
         ids = None if speaker_ids is None else [speaker_ids[i] for i in idx]
-        for i, res in zip(idx, _synthesize_chunk(model, [seqs[i] for i in idx], ids, stage)):
+        for i, res in zip(idx, _synthesize_chunk(model, [seqs[i] for i in idx], ids, stage, vocoder)):
             out[i] = res
     return out
 
 
-def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stage_timer=None, stats=None):
+def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stage_timer=None, stats=None,
+               vocoder="griffin_lim"):
     """Synthesize many utterances with continuous batching; a generator of (index, (waveform, alignment, spectrogram,
     mel)) in completion order, each item what ``tts_batch`` gives for that sequence (bit for bit in exact-fp32 mode).
 
     The encoder runs on groups of ``slots`` waiting sequences (inside a length scope) as the decoder needs them; the
     decoder is ``incremental.decode_stream`` on ``slots`` rows; finished utterances go through the post-net (inside a
-    length scope on their frames) and Griffin-Lim in groups of ``post_batch``, the last partial group when the decoder
-    is done.  Inputs are checked as ``tts_batch`` checks them, before the first item.  stage_timer: as for
+    length scope on their frames) and the vocoder in groups of ``post_batch``, the last partial group when the decoder
+    is done.  Inputs are checked as ``tts_batch`` checks them, before the first item.  stage_timer, vocoder: as for
     ``tts_batch``; stats: a dict ``decode_stream`` fills (decoder occupancy)."""
+    audio.check_phase_method(vocoder)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, slots=slots, post_batch=post_batch)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
-    return _stream(model, seqs, speaker_ids, int(slots), int(post_batch), stage, stats)
+    return _stream(model, seqs, speaker_ids, int(slots), int(post_batch), stage, stats, vocoder)
 
 
 @torch.no_grad()
@@ -174,7 +180,7 @@ def _encode(model, idx, seqs, speaker_ids, stage):
             for b, (i, n) in enumerate(zip(idx, lens))]
 
 
-def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats):
+def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats, vocoder="griffin_lim"):
     def requests():
         for g in range(0, len(seqs), slots):
             idx = list(range(g, min(g + slots, len(seqs))))
@@ -190,10 +196,11 @@ def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats):
             outputs[b, :r[5]], states[b, :r[5]] = r[1], r[4]
         spk = None if speaker_ids is None else \
             model._speaker_embedding(torch.tensor([speaker_ids[r[0]] for r in group]).to(outputs.device))
-        post = _postnet_vocode(model, outputs, states, [r[5] for r in group], spk, stage)
+        post = _postnet_vocode(model, outputs, states, [r[5] for r in group], spk, stage, **vocoder_kw)
         for r, (w, lin, mel) in zip(group, post):
             yield r[0], (w, r[2].cpu().numpy(), lin, mel)
 
+    vocoder_kw = {} if vocoder == "griffin_lim" else {"vocoder": vocoder}     # the default: the six-argument call
     group = []
     for r in incremental.decode_stream(model.seq2seq.decoder, slots, requests(), stats=stats, stage_timer=stage):
         group.append(r)

@@ -211,6 +211,20 @@ int dv3_stft_complex_batched(const float* wav, const int* n_samples, long long w
                              float* spec, const int* nframes, int max_frames, int nclips, void* stream);
 int dv3_istft_batched(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
                       int max_frames, int nclips, void* stream);
+/* LWS phase recovery (csrc/lws.cu; Local Weighted Sums, the algorithm of the reference's lws.run_lws -- parity
+ * UNPINNED, the package's source is absent).  mag (nframes,513) target magnitude; spec (nframes,513,2) [re,im];
+ * weights: 7 x 11 complex fp32 [q+3][d+5] = beta_q(d) = (1/1024) sum_n w(n) w(n-256q) e^{-2 pi i d n/1024}
+ * (audio._lws_weights).  dv3_lws_nofuture: the no-future initialisation -> spec (frames in order from their 3 past
+ * frames, then init_iters in-frame Jacobi passes).  dv3_lws_iterate: one batch iteration spec_in -> spec_out (distinct
+ * buffers).  Batched forms: clip c has nframes[c] <= max_frames frames at spec + c*max_frames*513*2 (mag with 513
+ * floats per frame), nframes int32 [nclips] on the device; frames past a clip's count are neither read nor written. */
+int dv3_lws_nofuture(const float* mag, float* spec, const float* weights, int nframes, int init_iters, void* stream);
+int dv3_lws_iterate(const float* mag, const float* spec_in, float* spec_out, const float* weights, int nframes,
+                    void* stream);
+int dv3_lws_nofuture_batched(const float* mag, float* spec, const float* weights, const int* nframes, int max_frames,
+                             int nclips, int init_iters, void* stream);
+int dv3_lws_iterate_batched(const float* mag, const float* spec_in, float* spec_out, const float* weights,
+                            const int* nframes, int max_frames, int nclips, void* stream);
 int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long long stride, float coef, void* stream);
 
 /* ================= tensor-core ConvBlock / conv path: wgmma + TMA, split 16-bit operands =================
