@@ -1,7 +1,9 @@
 """Audio front-end with the reference's function names (reference audio.py): ``spectrogram(y)`` and
 ``melspectrogram(y)`` take a float waveform and return (n_freq, n_frames) arrays in [0, 1] -- computed by ONE fused
 GPU pass (csrc/stft.cu) instead of two CPU lws STFTs.  ``stft_mel_batch`` is the batched device API the
-preprocessors should use (a whole shard of clips per launch; one H2D, one D2H).
+preprocessors should use (a whole shard of clips per launch; one H2D, one D2H).  ``stft_mel_targets`` runs the same
+transform on a training batch's waveforms and writes the padded, decimated target layout of ``data.collate`` directly
+(training from wav files, ``data.WavDataset``).
 
 ``inv_spectrogram`` (reference audio.py:37-43) recovers the phase on the same STFT frame with Griffin-Lim (the default,
 csrc/istft.cu) or with Local Weighted Sums (``method="lws"``, csrc/lws.cu), the algorithm of the reference's
@@ -126,6 +128,61 @@ def _linear_to_mel(spectrogram):
 
 def num_frames(n_samples):
     return lib.raw("dv3_stft_num_frames")(int(n_samples))
+
+
+def num_frames_host(n_samples):
+    """``num_frames`` restated in Python (no CUDA library load), for DataLoader workers: frames of the padded STFT,
+    ceil((n + 2*(fft - hop) - fft) / hop) + 1."""
+    fft, hop = hparams.fft_size, hparams.hop_size
+    return (int(n_samples) + 2 * (fft - hop) - fft + hop - 1) // hop + 1
+
+
+def stft_mel_targets(wav, lengths, T_lin, r, downsample_step, lengths_dev=None):
+    """Training targets of a waveform batch in ``data.collate``'s layout, in one launch (plus the peak pass when
+    ``hparams.rescaling`` is on).
+
+    wav: (B, pitch) int16 PCM (read as x / 32768, like ``load_wav``) or fp32 CUDA tensor; lengths: host sequence of
+    the B clip lengths in samples; T_lin: collate's ``max_target_len``.  -> y (B, T_lin, 513) with clip c's frame f at
+    row r + f, and mel (B, T_lin / downsample_step, num_mels) = the padded mel rows 0, ds, 2*ds, ...; every other row
+    zero.  Bit-identical to ``collate`` of the preprocessed .npy features.  lengths_dev: the same lengths as an int32
+    tensor on wav's device (otherwise they are copied from the host).  No host synchronisation: every check below
+    uses host values only, and all of them run before any launch."""
+    if not (torch.is_tensor(wav) and wav.is_cuda and wav.dim() == 2):
+        raise Dv3Error("stft_mel_targets needs a (B, pitch) CUDA tensor; there is no CPU path")
+    if wav.dtype not in (torch.int16, torch.float32):
+        raise Dv3Error("stft_mel_targets takes int16 PCM or fp32 waveforms, got %s" % wav.dtype)
+    if hparams.fft_size != 1024 or hparams.hop_size != 256:
+        raise Dv3Error("the fused kernel is built for fft_size=1024, hop_size=256 (every reference preset)")
+    lengths = [int(n) for n in (lengths.tolist() if torch.is_tensor(lengths) else lengths)]
+    B, pitch = wav.shape
+    r, ds, T_lin = int(r), int(downsample_step), int(T_lin)
+    if len(lengths) != B or not all(0 <= n <= pitch for n in lengths):
+        raise Dv3Error("lengths must give 0..%d samples for each of the %d clips" % (pitch, B))
+    if r < 1 or ds < 1:
+        raise Dv3Error("r and downsample_step must be >= 1 (got %d, %d)" % (r, ds))
+    need = r + max(num_frames_host(n) for n in lengths)
+    if T_lin < need:
+        raise Dv3Error("T_lin=%d is smaller than the %d rows the longest clip needs (r=%d + its frames)"
+                       % (T_lin, need, r))
+    wav = wav.contiguous()
+    dev = wav.device
+    if lengths_dev is None:
+        lengths_dev = torch.tensor(lengths, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    elif not (lengths_dev.device == dev and lengths_dev.dtype == torch.int32 and lengths_dev.numel() == B):
+        raise Dv3Error("lengths_dev must be an int32 tensor of %d lengths on %s" % (B, dev))
+    basis, start, length = _device_basis(dev)
+    y = torch.empty(B, T_lin, hparams.fft_size // 2 + 1, device=dev)      # the kernel writes every row
+    mel = torch.empty(B, -(-T_lin // ds), hparams.num_mels, device=dev)
+    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    is16 = int(wav.dtype == torch.int16)
+    peak = None
+    if hparams.rescaling:
+        peak = torch.empty(B, device=dev)
+        lib.call("dv3_peak_abs_batched", _cp(wav), is16, _cp(lengths_dev), pitch, B, _cp(peak), st)
+    lib.call("dv3_stft_mel_targets", _cp(wav), is16, _cp(lengths_dev), _cp(peak), float(hparams.rescaling_max),
+             _cp(basis), _cp(start), _cp(length), _cp(y), _cp(mel), B, pitch, T_lin, r, ds, hparams.num_mels,
+             float(hparams.preemphasis), float(hparams.min_level_db), float(hparams.ref_level_db), st)
+    return y, mel
 
 
 def stft_mel_batch(wav, lengths=None, want_linear=True, want_mel=True):

@@ -20,6 +20,17 @@
 //     copied into shared memory per CTA; dB through lg2.approx.
 // Frames beyond a clip's own count (ragged batches) are zero-filled by the kernel, so callers pass uninitialised
 // output buffers.
+//
+// Output descriptor (StftParams::lead / ds / lin_rows / mel_rows): frame f of a clip goes to linear row lead + f, and
+// to mel row (lead + f) / ds when (lead + f) % ds == 0; every other row of both outputs is written as zero.  With
+// lead = 0, ds = 1 this is the preprocessing layout (dv3_stft_mel); with lead = r and ds = downsample_step it is the
+// padded, decimated layout of the training batch (data.collate), so a batch's targets come straight from its
+// waveforms (dv3_stft_mel_targets).  The mel stage then runs only on kept frames: for ds in {2, 4, 8} the 8/ds kept
+// frames of a group take all lanes, ds quads of filters per warp pass instead of one.  The waveform is fp32 or int16
+// PCM (template), the int16 staged as is (half the shared-memory bytes) and converted x / 32768 where pass 1 reads it;
+// the optional per-clip rescale x / peak * gain is applied there too, with correctly rounded division and product.
+#include <type_traits>
+
 #include "tc_common.cuh"
 #include "stft_core.cuh"
 
@@ -35,14 +46,18 @@ constexpr int MEL_NNZ = 2048;           // packed (zero-padded) mel weights kept
 constexpr int MEL_REACH = 568;          // a packed row may read magnitude-plane words below this index (all written)
 
 struct StftParams {
-    const float* wav;          // (nclips, max_len)
+    const void* wav;           // (nclips, max_len) fp32 or int16 (kernel template)
     const int* lengths;        // (nclips) valid samples per clip
     const float* mel_basis;    // (n_mels, 513) dense
     const int* mel_start;      // (n_mels) first non-zero bin
     const int* mel_len;        // (n_mels) number of non-zero bins
-    float* linear;             // (nclips, max_frames, 513) or null
-    float* mel;                // (nclips, max_frames, n_mels) or null
-    int max_len, max_frames, n_mels;
+    float* linear;             // (nclips, lin_rows, 513) or null
+    float* mel;                // (nclips, mel_rows, n_mels) or null
+    int max_len, max_frames, n_mels;     // max_frames: frames computed per clip (lead + max_frames <= lin_rows)
+    int lead, ds, qsh;         // output descriptor (top of file); qsh = log2(ds) for ds in {2, 4, 8}, else 0
+    int lin_rows, mel_rows;
+    const float* peak;         // (nclips) max |x| of each clip: x -> x / peak * gain (kernel template SCALE), or null
+    float gain;
     float preemph;
     // normalised dB: clip((20*log10(max(min_level, v)) - ref - min_db) / -min_db, 0, 1)   (audio.py:79-81, :88-89)
     //   = sat(c2 * log2(max(min_level, v)) + c0);  on p4 = |2X|^2 (log2(v) = log2(p4)/2 - 1): sat(c2h * log2(max(min_p4, p4)) + c0l)
@@ -74,45 +89,96 @@ static_assert((WORK * 4) % 8 == 0, "the im plane must be 8-byte aligned");
 __device__ __forceinline__ float lg2_approx(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sqrt_approx(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-// raw samples x[s0-4 .. s0+STAGE_N) of the clip -> sm.raw[0 ..], zero outside [0, len).  Three ways:
+// raw samples x[s0-VEC .. s0+STAGE_N) of the clip -> raw[0 ..], zero outside [0, len); VEC = samples per 16 bytes
+// (4 fp32 / 8 int16), so that raw[VEC] (sample s0) is 16-byte aligned and raw[VEC-1] holds x[s0-1].  Three ways:
 //   BULK   the whole span lies inside the clip and is 16-byte aligned: ONE cp.async.bulk (TMA) issued by thread 0,
 //          completion on sm.mbar -- no LSU instructions or shared-memory wavefronts spent on staging;
 //   A16    16-byte cp.async pieces with zero fill (a clip's first / last groups);
-//   else   4-byte cp.async pieces (rows that do not start on 16-byte boundaries).
-constexpr int STAGE_BYTES = (STAGE_N + 4) * 4;
-static_assert(STAGE_BYTES % 16 == 0, "bulk copies move multiples of 16 bytes");
-__device__ __forceinline__ bool stage_is_bulk(bool a16, int s0, int len) { return a16 && s0 >= 4 && s0 + STAGE_N <= len; }
-__device__ __forceinline__ void stage_async(float* raw, uint64_t* mbar, const float* x, int s0, int len, int tid,
-                                            bool a16) {
-    if (stage_is_bulk(a16, s0, len)) {                         // uniform over the CTA
+//   else   4-byte cp.async pieces (fp32 rows that do not start on 16-byte boundaries), or plain loads and stores
+//          (int16 rows likewise: cp.async has no 2-byte form).
+template <typename In> struct Stage {
+    static constexpr int VEC = 16 / (int)sizeof(In), BYTES = (STAGE_N + VEC) * (int)sizeof(In);
+    static_assert(BYTES % 16 == 0, "bulk copies move multiples of 16 bytes");
+    static_assert(BYTES <= (int)sizeof(float) * (STAGE_N + 8), "the staged span must fit StftSmem::raw");
+};
+template <typename In>
+__device__ __forceinline__ bool stage_is_bulk(bool a16, int s0, int len) {
+    return a16 && s0 >= Stage<In>::VEC && s0 + STAGE_N <= len;
+}
+template <typename In>
+__device__ __forceinline__ void stage_async(In* raw, uint64_t* mbar, const In* x, int s0, int len, int tid, bool a16) {
+    constexpr int VEC = Stage<In>::VEC;
+    if (stage_is_bulk<In>(a16, s0, len)) {                     // uniform over the CTA
         if (tid == 0) {
             tc::fence_proxy_async();                             // earlier generic-proxy reads of raw[] are ordered by the barrier
-            tc::mbar_arrive_expect_tx(mbar, STAGE_BYTES);
+            tc::mbar_arrive_expect_tx(mbar, Stage<In>::BYTES);
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(tc::smem_u32(raw)), "l"(x + s0 - 4), "r"(STAGE_BYTES), "r"(tc::smem_u32(mbar)) : "memory");
+                         ::"r"(tc::smem_u32(raw)), "l"(x + s0 - VEC), "r"(Stage<In>::BYTES), "r"(tc::smem_u32(mbar))
+                         : "memory");
         }
         return;
     }
     if (a16) {
-        for (int i = tid; i < (STAGE_N + 4) / 4; i += STFT_WARPS * 32) {
-            const int s = s0 - 4 + 4 * i;                        // multiple of 4: a piece never straddles sample 0
-            const int nb = s < 0 ? 0 : min(max(len - s, 0), 4) * 4;
-            const unsigned dst = (unsigned)__cvta_generic_to_shared(raw + 4 * i);
+        for (int i = tid; i < (STAGE_N + VEC) / VEC; i += STFT_WARPS * 32) {
+            const int s = s0 - VEC + VEC * i;                    // multiple of VEC: a piece never straddles sample 0
+            const int nb = s < 0 ? 0 : min(max(len - s, 0), VEC) * (int)sizeof(In);
+            const unsigned dst = (unsigned)__cvta_generic_to_shared(raw + VEC * i);
             asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(x + (nb ? s : 0)), "r"(nb)
+                         : "memory");
+        }
+    } else if constexpr (sizeof(In) == 4) {
+        for (int i = tid; i < STAGE_N + 1; i += STFT_WARPS * 32) {
+            const int s = s0 - 1 + i;
+            const bool ok = s >= 0 && s < len;
+            const unsigned dst = (unsigned)__cvta_generic_to_shared(raw + VEC - 1 + i);
+            asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(x + (ok ? s : 0)), "r"(ok ? 4 : 0)
                          : "memory");
         }
     } else {
         for (int i = tid; i < STAGE_N + 1; i += STFT_WARPS * 32) {
             const int s = s0 - 1 + i;
-            const bool ok = s >= 0 && s < len;
-            const unsigned dst = (unsigned)__cvta_generic_to_shared(raw + 3 + i);
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(x + (ok ? s : 0)), "r"(ok ? 4 : 0)
-                         : "memory");
+            raw[VEC - 1 + i] = (s >= 0 && s < len) ? x[s] : In(0);
         }
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
 }
 
+// pass-1 sample sources over the staged span (stft_core.cuh RawF32 is the plain fp32 one): int16 -> x / 32768 (exact),
+// then, with SCALE, x / peak * gain with a correctly rounded division and product (numpy's float32 arithmetic)
+template <bool SCALE> __device__ __forceinline__ float rescale(float v, float peak, float gain) {
+    return SCALE ? __fmul_rn(__fdiv_rn(v, peak), gain) : v;
+}
+template <bool SCALE> struct StagedF32 {
+    const float* x; float peak, gain;
+    __device__ __forceinline__ f4 load4(int i) const {
+        const f4 s = *reinterpret_cast<const f4*>(x + i);
+        return f4{rescale<SCALE>(s.x, peak, gain), rescale<SCALE>(s.y, peak, gain), rescale<SCALE>(s.z, peak, gain),
+                  rescale<SCALE>(s.w, peak, gain)};
+    }
+    __device__ __forceinline__ float load1(int i) const { return rescale<SCALE>(x[i], peak, gain); }
+};
+template <bool SCALE> struct StagedS16 {
+    const short* x; float peak, gain;
+    __device__ __forceinline__ float cvt(short v) const {
+        return rescale<SCALE>(__fmul_rn((float)v, 3.0517578125e-05f), peak, gain);         // 1 / 32768
+    }
+    __device__ __forceinline__ f4 load4(int i) const {
+        const short4 s = *reinterpret_cast<const short4*>(x + i);
+        return f4{cvt(s.x), cvt(s.y), cvt(s.z), cvt(s.w)};
+    }
+    __device__ __forceinline__ float load1(int i) const { return cvt(x[i]); }
+};
+template <typename In, bool SCALE> struct SourceOf { typedef StagedF32<SCALE> type; };
+template <bool SCALE> struct SourceOf<short, SCALE> { typedef StagedS16<SCALE> type; };
+
+template <bool TAIL, typename In, bool SCALE>
+__device__ __forceinline__ void pass1_staged(int lane, const In* xs, float peak, float gain, float c, int lim,
+                                             const f4* win, const f4* tw1, pr (&vr)[8], pr (&vi)[8]) {
+    if constexpr (std::is_same<In, float>::value && !SCALE) pass1<TAIL>(lane, xs, c, lim, win, tw1, vr, vi);
+    else pass1_src<TAIL>(lane, typename SourceOf<In, SCALE>::type{xs, peak, gain}, c, lim, win, tw1, vr, vi);
+}
+
+template <typename In, bool SCALE>
 __global__ void __launch_bounds__(STFT_WARPS * 32, 3) stft_mel_kernel(const __grid_constant__ StftParams p) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -122,28 +188,36 @@ __global__ void __launch_bounds__(STFT_WARPS * 32, 3) stft_mel_kernel(const __gr
     const int len = p.lengths[clip];
     const int nframes = min((len + 2 * PAD - FFT_N + HOP - 1) / HOP + 1, p.max_frames);   // ceil((len+2*768-1024)/256)+1
     const int f_end = min(f_begin + STFT_FRAMES, p.max_frames);
+    const int lead = p.lead, ds = p.ds;
 
-    // frames of this chunk past the clip's own end: zero-fill (contiguous rows)
+    // zero rows (contiguous runs): the rows of this chunk's frames past the clip's own end, and in the first chunk the
+    // lead rows in front of frame 0; a mel row j belongs to frame j*ds - lead
     {
         const int z0 = max(f_begin, nframes);
-        if (z0 < f_end) {
-            const size_t row0 = (size_t)clip * p.max_frames + z0;
+        const int zr[2][2] = {{lead + z0, lead + f_end}, {0, blockIdx.x == 0 ? lead : 0}};
+#pragma unroll
+        for (int z = 0; z < 2; ++z) {
+            const int r0 = zr[z][0], r1 = zr[z][1];
+            if (r0 >= r1) continue;
             if (p.linear) {
-                float* o = p.linear + row0 * NBINS;
-                for (int i = tid; i < (f_end - z0) * NBINS; i += blockDim.x) o[i] = 0.f;
+                float* o = p.linear + ((size_t)clip * p.lin_rows + r0) * NBINS;
+                for (int i = tid; i < (r1 - r0) * NBINS; i += blockDim.x) o[i] = 0.f;
             }
             if (p.mel) {
-                float* o = p.mel + row0 * p.n_mels;
-                for (int i = tid; i < (f_end - z0) * p.n_mels; i += blockDim.x) o[i] = 0.f;
+                const int m0 = (r0 + ds - 1) / ds, m1 = (r1 + ds - 1) / ds;
+                float* o = p.mel + ((size_t)clip * p.mel_rows + m0) * p.n_mels;
+                for (int i = tid; i < (m1 - m0) * p.n_mels; i += blockDim.x) o[i] = 0.f;
             }
         }
     }
     if (f_begin >= nframes) return;
 
-    const float* x = p.wav + (size_t)clip * p.max_len;
+    const In* x = reinterpret_cast<const In*>(p.wav) + (size_t)clip * p.max_len;
+    In* raw = reinterpret_cast<In*>(sm.raw);
+    const float peak = SCALE ? p.peak[clip] : 1.f, gain = p.gain;
     const bool a16 = p.aligned16 != 0;
     if (tid == 0) { tc::mbar_init(&sm.mbar, 1); tc::fence_barrier_init(); }   // thread 0 is also the only issuer
-    stage_async(sm.raw, &sm.mbar, x, f_begin * HOP - PAD, len, tid, a16);     // in flight while the tables are set up
+    stage_async(raw, &sm.mbar, x, f_begin * HOP - PAD, len, tid, a16);     // in flight while the tables are set up
     uint32_t bulk_parity = 0;
 
     // ---- tables, once per CTA ----
@@ -216,16 +290,17 @@ __global__ void __launch_bounds__(STFT_WARPS * 32, 3) stft_mel_kernel(const __gr
         const int f0 = f_begin + g * STFT_WARPS;
         if (f0 >= nframes) break;                                   // uniform over the CTA
         asm volatile("cp.async.wait_group 0;" ::: "memory");
-        if (stage_is_bulk(a16, f0 * HOP - PAD, len)) { tc::mbar_wait(&sm.mbar, bulk_parity); bulk_parity ^= 1; }
+        if (stage_is_bulk<In>(a16, f0 * HOP - PAD, len)) { tc::mbar_wait(&sm.mbar, bulk_parity); bulk_parity ^= 1; }
         __syncthreads();                                            // raw[] landed; the previous group's mel stage is done
         const int frame = f0 + warp;
-        const size_t fidx = (size_t)clip * p.max_frames + frame;
+        const size_t fidx = (size_t)clip * p.lin_rows + lead + frame;
         if (frame < nframes) {                                      // warp-uniform
             pr vr[8], vi[8];
             const int lim = len - (frame * HOP - PAD);              // samples of the frame before the clip's end
-            const float* xs = sm.raw + 4 + warp * HOP;
-            if (lim < FFT_N) pass1<true>(lane, xs, p.preemph, lim, win, tw1, vr, vi);     // warp-uniform
-            else pass1<false>(lane, xs, p.preemph, lim, win, tw1, vr, vi);
+            const In* xs = raw + Stage<In>::VEC + warp * HOP;
+            if (lim < FFT_N)                                        // warp-uniform
+                pass1_staged<true, In, SCALE>(lane, xs, peak, gain, p.preemph, lim, win, tw1, vr, vi);
+            else pass1_staged<false, In, SCALE>(lane, xs, peak, gain, p.preemph, lim, win, tw1, vr, vi);
             store1(lane, vr, vi, re, im);
             __syncwarp();
             pass2(lane, re, im, tw2, vr, vi);
@@ -264,17 +339,23 @@ __global__ void __launch_bounds__(STFT_WARPS * 32, 3) stft_mel_kernel(const __gr
         }
         __syncthreads();                                            // all 8 frames' magnitudes are in place; raw[] is free
         if (g + 1 < STFT_GROUPS && f0 + STFT_WARPS < nframes)
-            stage_async(sm.raw, &sm.mbar, x, (f0 + STFT_WARPS) * HOP - PAD, len, tid, a16);
+            stage_async(raw, &sm.mbar, x, (f0 + STFT_WARPS) * HOP - PAD, len, tid, a16);
 
         if (p.mel) {
             // lane = (frame fl, filter q of the quad): all 8 frames of the group in one go.  Quads are dealt to the
             // warps longest first in snake order (rows grow with the filter index), so the warps finish together.
-            const int fl = lane & 7, q = lane >> 3;
+            // Decimated output (ds = 2^qsh): lane = (quad sub of the pass, kept frame kf, q) -- the 8/ds kept frames
+            // times ds quads per pass; any other ds keeps lane = (fl, q) and drops the rows that are not kept.
+            const int qsh = p.qsh, slot = lane & 7, q = lane >> 3;
+            const int sub = slot >> (3 - qsh), kf = slot & ((8 >> qsh) - 1);
+            const int fl = (qsh ? (-(lead + f0)) & (ds - 1) : 0) + (kf << qsh);     // < 8
+            const int t = lead + f0 + fl;                                            // padded frame index
+            const bool keep = qsh != 0 || ds == 1 || t % ds == 0;
             const float* magf = sm.work[fl][0];
-            const bool fvalid = f0 + fl < nframes;
-            float* out = p.mel + ((size_t)clip * p.max_frames + f0 + fl) * p.n_mels;
-            for (int k = 0; 8 * k < nquads; ++k) {
-                const int i = 8 * k + ((k & 1) ? STFT_WARPS - 1 - warp : warp);
+            const bool fvalid = f0 + fl < nframes && keep;
+            float* out = p.mel + ((size_t)clip * p.mel_rows + (qsh ? t >> qsh : (ds == 1 ? t : t / ds))) * p.n_mels;
+            for (int k = 0; (8 * k << qsh) < nquads; ++k) {
+                const int i = ((8 * k + ((k & 1) ? STFT_WARPS - 1 - warp : warp)) << qsh) + sub;
                 if (i >= nquads) continue;
                 const int Q = nquads - 1 - i, m = 4 * Q + q;
                 float acc = 0.f;
@@ -311,6 +392,44 @@ __global__ void __launch_bounds__(STFT_WARPS * 32, 3) stft_mel_kernel(const __gr
     asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// peak[c] = max |x| over clip c's own samples (int16 as x / 32768): the rescaling divisor of preprocess._load.  One CTA
+// per clip; a max is exact in any order.
+constexpr int PEAK_THREADS = 1024;
+template <typename In>
+__global__ void __launch_bounds__(PEAK_THREADS) peak_abs_kernel(const In* wav, const int* lengths, int max_len,
+                                                                float* peak) {
+    pdl_trigger(); pdl_wait();
+    __shared__ float part[PEAK_THREADS / 32];
+    const int clip = blockIdx.x, len = lengths[clip];
+    const In* x = wav + (size_t)clip * max_len;
+    float m = 0.f;
+    for (int i = threadIdx.x; i < len; i += PEAK_THREADS) {
+        const float v = std::is_same<In, float>::value ? (float)x[i] : __fmul_rn((float)x[i], 3.0517578125e-05f);
+        m = fmaxf(m, fabsf(v));
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        m = part[threadIdx.x];
+#pragma unroll
+        for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if (threadIdx.x == 0) peak[clip] = m;
+    }
+}
+
+template <typename In, bool SCALE>
+static int launch_stft(const StftParams& p, int nclips, cudaStream_t st, const char* what) {
+    static const cudaError_t attr = cudaFuncSetAttribute(stft_mel_kernel<In, SCALE>,
+                                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                         (int)sizeof(StftSmem));
+    DV3_REQUIRE(attr == cudaSuccess, "%s: cannot reserve %zu bytes of shared memory", what, sizeof(StftSmem));
+    launch_k(stft_mel_kernel<In, SCALE>, dim3((p.max_frames + STFT_FRAMES - 1) / STFT_FRAMES, nclips),
+             STFT_WARPS * 32, sizeof(StftSmem), st, p);
+    return check_launch(what);
+}
+
 }  // namespace dv3
 
 using namespace dv3;
@@ -338,26 +457,69 @@ static int stft_tables(cudaStream_t st) {
     return 0;
 }
 
+// the parameters shared by both entry points, in the identity layout (lead 0, ds 1, one row per frame)
+static int stft_params(StftParams& p, const char* what, const void* wav, const int* lengths, const float* mel_basis,
+                       const int* mel_start, const int* mel_len, float* linear, float* mel, int nclips, int max_len,
+                       int max_frames, int n_mels, float preemph, float min_level_db, float ref_level_db,
+                       int aligned16, void* stream) {
+    DV3_REQUIRE(nclips >= 1 && nclips <= 65535, "%s: nclips %d out of range", what, nclips);
+    DV3_REQUIRE(max_frames >= 1, "%s: bad max_frames %d", what, max_frames);
+    DV3_REQUIRE(n_mels >= 0 && n_mels <= MAX_MELS, "%s: n_mels %d > %d", what, n_mels, MAX_MELS);
+    DV3_REQUIRE(stft_tables((cudaStream_t)stream) == 0, "%s: cannot build the transform tables", what);
+    DV3_REQUIRE(min_level_db < 0.f, "%s: min_level_db must be negative (got %g)", what, (double)min_level_db);
+    const double inv = 1.0 / -(double)min_level_db, c2 = 20.0 * 0.30102999566398120 * inv;      // 20*log10(2) / -min_db
+    const double c0 = 1.0 - (double)ref_level_db * inv, min_level = pow(10.0, (double)min_level_db / 20.0);
+    p = StftParams{wav, lengths, mel_basis, mel_start, mel_len, linear, mel, max_len, max_frames, n_mels,
+                   /*lead*/ 0, /*ds*/ 1, /*qsh*/ 0, /*lin_rows*/ max_frames, /*mel_rows*/ max_frames,
+                   /*peak*/ nullptr, /*gain*/ 1.f, preemph, (float)c2, (float)c0, (float)min_level, (float)(0.5 * c2),
+                   (float)(c0 - c2), (float)(4.0 * min_level * min_level), aligned16};
+    return 0;
+}
+
 int dv3_stft_mel(const float* wav, const int* lengths, const float* mel_basis, const int* mel_start,
                  const int* mel_len, float* linear, float* mel, int nclips, int max_len, int max_frames,
                  int n_mels, float preemph, float min_level_db, float ref_level_db, void* stream) {
-    DV3_REQUIRE(nclips >= 1 && nclips <= 65535, "stft_mel: nclips %d out of range", nclips);
-    DV3_REQUIRE(max_frames >= 1, "stft_mel: bad max_frames %d", max_frames);
-    DV3_REQUIRE(n_mels >= 0 && n_mels <= MAX_MELS, "stft_mel: n_mels %d > %d", n_mels, MAX_MELS);
-    DV3_REQUIRE(stft_tables((cudaStream_t)stream) == 0, "stft_mel: cannot build the transform tables");
+    StftParams p;
     const int aligned16 = (reinterpret_cast<uintptr_t>(wav) % 16 == 0) && (max_len % 4 == 0);
-    DV3_REQUIRE(min_level_db < 0.f, "stft_mel: min_level_db must be negative (got %g)", (double)min_level_db);
-    const double inv = 1.0 / -(double)min_level_db, c2 = 20.0 * 0.30102999566398120 * inv;      // 20*log10(2) / -min_db
-    const double c0 = 1.0 - (double)ref_level_db * inv, min_level = pow(10.0, (double)min_level_db / 20.0);
-    StftParams p = {wav, lengths, mel_basis, mel_start, mel_len, linear, mel, max_len, max_frames, n_mels, preemph,
-                    (float)c2, (float)c0, (float)min_level, (float)(0.5 * c2), (float)(c0 - c2),
-                    (float)(4.0 * min_level * min_level), aligned16};
-    static const cudaError_t attr = cudaFuncSetAttribute(stft_mel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                         (int)sizeof(StftSmem));
-    DV3_REQUIRE(attr == cudaSuccess, "stft_mel: cannot reserve %zu bytes of shared memory", sizeof(StftSmem));
-    launch_k(stft_mel_kernel, dim3((max_frames + STFT_FRAMES - 1) / STFT_FRAMES, nclips), STFT_WARPS * 32,
-             sizeof(StftSmem), (cudaStream_t)stream, p);
-    return check_launch("stft_mel");
+    if (stft_params(p, "stft_mel", wav, lengths, mel_basis, mel_start, mel_len, linear, mel, nclips, max_len,
+                    max_frames, n_mels, preemph, min_level_db, ref_level_db, aligned16, stream))
+        return 1;
+    return launch_stft<float, false>(p, nclips, (cudaStream_t)stream, "stft_mel");
+}
+
+int dv3_stft_mel_targets(const void* wav, int wav_int16, const int* lengths, const float* peak, float rescaling_max,
+                         const float* mel_basis, const int* mel_start, const int* mel_len, float* linear, float* mel,
+                         int nclips, int max_len, int T_lin, int lead, int downsample_step, int n_mels, float preemph,
+                         float min_level_db, float ref_level_db, void* stream) {
+    const char* what = "stft_mel_targets";
+    DV3_REQUIRE(lead >= 0 && lead < T_lin, "%s: lead %d must lie in [0, T_lin = %d)", what, lead, T_lin);
+    DV3_REQUIRE(downsample_step >= 1, "%s: bad downsample_step %d", what, downsample_step);
+    StftParams p;
+    const int vec = wav_int16 ? 8 : 4;                            // samples per 16 bytes
+    const int aligned16 = (reinterpret_cast<uintptr_t>(wav) % 16 == 0) && (max_len % vec == 0);
+    if (stft_params(p, what, wav, lengths, mel_basis, mel_start, mel_len, linear, mel, nclips, max_len, T_lin - lead,
+                    n_mels, preemph, min_level_db, ref_level_db, aligned16, stream))
+        return 1;
+    const int ds = downsample_step;
+    p.lead = lead; p.ds = ds;
+    p.qsh = ds == 2 ? 1 : ds == 4 ? 2 : ds == 8 ? 3 : 0;
+    p.lin_rows = T_lin; p.mel_rows = (T_lin + ds - 1) / ds;
+    p.peak = peak; p.gain = rescaling_max;
+    const cudaStream_t st = (cudaStream_t)stream;
+    if (wav_int16) return peak ? launch_stft<short, true>(p, nclips, st, what) : launch_stft<short, false>(p, nclips, st, what);
+    return peak ? launch_stft<float, true>(p, nclips, st, what) : launch_stft<float, false>(p, nclips, st, what);
+}
+
+int dv3_peak_abs_batched(const void* wav, int wav_int16, const int* lengths, int max_len, int nclips, float* peak,
+                         void* stream) {
+    DV3_REQUIRE(nclips >= 1, "peak_abs: nclips %d out of range", nclips);
+    if (wav_int16)
+        launch_k(peak_abs_kernel<short>, dim3(nclips), PEAK_THREADS, 0, (cudaStream_t)stream,
+                 reinterpret_cast<const short*>(wav), lengths, max_len, peak);
+    else
+        launch_k(peak_abs_kernel<float>, dim3(nclips), PEAK_THREADS, 0, (cudaStream_t)stream,
+                 reinterpret_cast<const float*>(wav), lengths, max_len, peak);
+    return check_launch("peak_abs");
 }
 
 }  // extern "C"

@@ -156,11 +156,20 @@ STFT_HD f4 rot16(f4 w, int j) {
     return f4{r.x.x, r.x.y, r.y.x, r.y.y};
 }
 
+// Sample source of pass 1: the staged fp32 waveform itself.  stft.cu adds sources that convert staged int16 PCM and
+// rescale as the samples are read; a source has load4(i) = samples i..i+3 (i a multiple of 4) and load1(i) = sample i.
+struct RawF32 {
+    const float* x;
+    STFT_HD f4 load4(int i) const { return *reinterpret_cast<const f4*>(x + i); }
+    STFT_HD float load1(int i) const { return x[i]; }
+};
+
 // pass 1: x -> sample 0 of the frame window in the RAW waveform (16-byte aligned, x[-1] readable; samples outside the
 // clip are 0); pre-emphasis e[i] = x[i] - c*x[i-1] (audio.py:21-23) is applied on the fly.  TAIL: e[i] = 0 for
 // i >= lim (the zero padding after the clip's last sample starts inside this frame).
-template <bool TAIL>
-STFT_HD void pass1(int lane, const float* x, float c, int lim, const f4* win, const f4* tw1, pr (&vr)[8], pr (&vi)[8]) {
+template <bool TAIL, typename Src>
+STFT_HD void pass1_src(int lane, const Src& x, float c, int lim, const f4* win, const f4* tw1, pr (&vr)[8],
+                       pr (&vi)[8]) {
     const f4 ws = win[lane], wc = win[32 + lane];
     const pr sA = {ws.x, ws.y}, sB = {ws.z, ws.w}, cA = {wc.x, wc.y}, cB = {wc.z, wc.w};
     const float C1 = 0.92387953251128674f, S1 = 0.38268343236508977f, H = 0.70710678118654752f;
@@ -168,13 +177,13 @@ STFT_HD void pass1(int lane, const float* x, float c, int lim, const f4* win, co
 #pragma unroll
     for (int n2 = 0; n2 < 8; ++n2) {
         const int i0 = 128 * n2 + 4 * lane;                  // first of the 4 samples of points a, b
-        const f4 s = *reinterpret_cast<const f4*>(x + i0);
+        const f4 s = x.load4(i0);
 #if defined(__CUDA_ARCH__)
         // x[i0 - 1] is the previous lane's last sample: a shuffle instead of a 4-way conflicting load
         float xm = __shfl_up_sync(0xffffffffu, s.w, 1);
-        if (lane == 0) xm = x[i0 - 1];
+        if (lane == 0) xm = x.load1(i0 - 1);
 #else
-        const float xm = x[i0 - 1];
+        const float xm = x.load1(i0 - 1);
 #endif
         float e0 = fmaf(-c, xm, s.x), e1 = fmaf(-c, s.x, s.y), e2 = fmaf(-c, s.y, s.z), e3 = fmaf(-c, s.z, s.w);
         if (TAIL) {
@@ -196,6 +205,10 @@ STFT_HD void pass1(int lane, const float* x, float c, int lim, const f4* win, co
     }
     radix8p(vr, vi);
     twiddle7(vr, vi, tw1[lane], tw1[32 + lane]);
+}
+template <bool TAIL>
+STFT_HD void pass1(int lane, const float* x, float c, int lim, const f4* win, const f4* tw1, pr (&vr)[8], pr (&vi)[8]) {
+    pass1_src<TAIL>(lane, RawF32{x}, c, lim, win, tw1, vr, vi);
 }
 STFT_HD void store1(int lane, const pr (&vr)[8], const pr (&vi)[8], float* re, float* im) {
     f2* re2 = reinterpret_cast<f2*>(re);

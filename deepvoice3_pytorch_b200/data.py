@@ -8,6 +8,9 @@ padding rules, and a distributed variant of its length-bucketed sampler.
   ``spec.npy|mel.npy|n_frames|text[|speaker_id]`` line per utterance, preprocess.py:27-30; the three reference data
   sources TextDataSource / MelSpecDataSource / LinearSpecDataSource + PyTorchDataset, train.py:96-257, in one class).
   The text frontend (string -> token ids) stays the caller's: pass the reference's ``frontend.text_to_sequence``.
+* ``WavDataset`` + ``collate_wav`` + ``wav_batch_to_device`` train from the wav files instead: the loader moves
+  waveforms (int16 where the files are), and the GPU computes each batch's targets in ``collate``'s layout, bit-identical
+  to ``TrainTxtDataset`` + ``collate`` over what ``preprocess.build_from_path`` writes for the same corpus.
 * ``DistributedSimilarLengthSampler`` restates ``PartialyRandomizedSimilarTimeLengthSampler`` (train.py:195-239):
   sort by length, shuffle inside groups of ``batch_group_size``, permute whole mini-batches -- then deals the
   mini-batches round-robin to the ranks, so every rank sees disjoint batches of similar length (what the
@@ -31,41 +34,96 @@ def collate(batch, r=1, downsample_step=4, pin=False):
     Padding rules of the reference: target length rounded up to a multiple of r and of downsample_step, plus r *
     downsample_step leading zero frames ("initial decoder state"); text / text positions zero-padded; frame positions
     1..T_dec; done = 0 for the first len//r//ds - 1 decoder steps, then 1."""
-    multi_speaker = len(batch[0]) == 4
-    input_lengths = [len(x[0]) for x in batch]
-    max_input_len = max(input_lengths)
-    target_lengths = [len(x[1]) for x in batch]
+    max_target_len = max_target_length([len(b[1]) for b in batch], r, downsample_step)
+    b_pad = r
+    mel = torch.from_numpy(np.array([_pad_2d(b[1], max_target_len, b_pad=b_pad) for b in batch], dtype=np.float32))
+    y = torch.from_numpy(np.array([_pad_2d(b[2], max_target_len, b_pad=b_pad) for b in batch], dtype=np.float32))
+    if downsample_step > 1:
+        mel = mel[:, 0::downsample_step, :].contiguous()          # train.py:639-640
+    return _collate_common(batch, [len(b[1]) for b in batch], r, downsample_step, pin, {"mel": mel, "y": y})
+
+
+def max_target_length(target_lengths, r=1, downsample_step=4):
+    """collate's padded frame count of a batch: the longest target rounded up to a multiple of r and of
+    downsample_step, plus the r * downsample_step leading zero frames."""
     max_target_len = max(target_lengths)
     if max_target_len % r != 0:
         max_target_len += r - max_target_len % r
     if max_target_len % downsample_step != 0:
         max_target_len += downsample_step - max_target_len % downsample_step
-    b_pad = r
-    max_target_len += b_pad * downsample_step
+    return max_target_len + r * downsample_step
+
+
+def _collate_common(batch, target_lengths, r, downsample_step, pin, spectrograms):
+    """Every key of a collated batch but the spectrograms, with ``spectrograms`` ({"mel", "y"} for collate; the
+    waveforms for collate_wav) placed after frame_positions.  batch items: (text ids, target, ...[, speaker_id])."""
+    multi_speaker = len(batch[0]) == 4
+    input_lengths = [len(x[0]) for x in batch]
+    max_input_len = max(input_lengths)
+    max_target_len = max_target_length(target_lengths, r, downsample_step)
 
     x = torch.from_numpy(np.array([_pad(np.asarray(b[0]), max_input_len) for b in batch], dtype=np.int64))
-    mel = torch.from_numpy(np.array([_pad_2d(b[1], max_target_len, b_pad=b_pad) for b in batch], dtype=np.float32))
-    y = torch.from_numpy(np.array([_pad_2d(b[2], max_target_len, b_pad=b_pad) for b in batch], dtype=np.float32))
     text_positions = torch.from_numpy(np.array(
         [_pad(np.arange(1, len(b[0]) + 1), max_input_len) for b in batch], dtype=np.int64))
     T_dec = max_target_len // r // downsample_step
     frame_positions = torch.arange(1, T_dec + 1).long().unsqueeze(0).expand(len(batch), T_dec).clone()
     done = torch.from_numpy(np.array(
-        [_pad(np.zeros(len(b[1]) // r // downsample_step - 1), T_dec, constant_values=1) for b in batch],
+        [_pad(np.zeros(n // r // downsample_step - 1), T_dec, constant_values=1) for n in target_lengths],
         dtype=np.float32)).unsqueeze(-1)
-    if downsample_step > 1:
-        mel = mel[:, 0::downsample_step, :].contiguous()          # train.py:639-640
-    out = {
-        "x": x, "text_positions": text_positions, "frame_positions": frame_positions, "mel": mel, "y": y,
-        "done": done, "target_lengths": torch.tensor(target_lengths, dtype=torch.int64),
-        "input_lengths_dev": torch.tensor(input_lengths, dtype=torch.int64),
-    }
+    out = {"x": x, "text_positions": text_positions, "frame_positions": frame_positions, **spectrograms,
+           "done": done, "target_lengths": torch.tensor(target_lengths, dtype=torch.int64),
+           "input_lengths_dev": torch.tensor(input_lengths, dtype=torch.int64)}
     if multi_speaker:
         out["speaker_ids"] = torch.tensor([b[3] for b in batch], dtype=torch.int64)
     if pin:
         out = {k: v.pin_memory() for k, v in out.items()}
     out["input_lengths"] = np.asarray(input_lengths, dtype=np.int64)
     return out
+
+
+def collate_wav(batch, r=1, downsample_step=4, pin=False):
+    """batch: list of ``WavDataset`` items (text_ids, pcm (n,) int16 or float32, n_frames[, speaker_id]).
+
+    Host-only (safe in DataLoader workers): every key of ``collate`` except "mel" and "y", computed by the same code,
+    plus "wav" (B, pitch) -- the waveforms zero-padded to a pitch of a multiple of 8 samples, int16 when every clip is
+    int16, else float32 (int16 / 32768 is exact) -- and "wav_lengths" (B) int32.  ``wav_batch_to_device`` computes the
+    two spectrogram targets on the GPU."""
+    lens = [len(b[1]) for b in batch]
+    for b, n in zip(batch, lens):
+        if b[2] != _num_frames(n):
+            raise ValueError("item has %d samples but n_frames=%d (expected %d)" % (n, b[2], _num_frames(n)))
+    pitch = max(8, -(-max(lens) // 8) * 8)                  # 16-byte rows for int16 and fp32 alike
+    int16 = all(b[1].dtype == np.int16 for b in batch)
+    wav = np.zeros((len(batch), pitch), dtype=np.int16 if int16 else np.float32)
+    for i, b in enumerate(batch):
+        w = b[1]
+        wav[i, :len(w)] = w if int16 or w.dtype != np.int16 else w.astype(np.float32) / np.float32(32768.0)
+    spectrograms = {"wav": torch.from_numpy(wav), "wav_lengths": torch.tensor(lens, dtype=torch.int32)}
+    return _collate_common(batch, [b[2] for b in batch], r, downsample_step, pin, spectrograms)
+
+
+def wav_batch_to_device(batch, device, r=1, downsample_step=4):
+    """A ``collate_wav`` batch -> the dict ``collate`` + ``train_step.to_device`` give for the same utterances after
+    ``preprocess.build_from_path``, bit for bit: asynchronous H2D copies (pin the batch for them to overlap), then
+    the targets in one launch on the current stream (``audio.stft_mel_targets``; the peak pass first when
+    ``hparams.rescaling`` is on).  No host synchronisation."""
+    from . import audio
+    out = {}
+    for k, v in batch.items():
+        if k in ("wav", "wav_lengths"):
+            continue
+        out[k] = v.to(device, non_blocking=True) if torch.is_tensor(v) else v
+    wav = batch["wav"].to(device, non_blocking=True)
+    lens_dev = batch["wav_lengths"].to(device, non_blocking=True)
+    T_lin = max_target_length(batch["target_lengths"].tolist(), r, downsample_step)
+    y, mel = audio.stft_mel_targets(wav, batch["wav_lengths"], T_lin, r, downsample_step, lengths_dev=lens_dev)
+    order = ("x", "text_positions", "frame_positions")
+    return {**{k: out[k] for k in order}, "mel": mel, "y": y, **{k: v for k, v in out.items() if k not in order}}
+
+
+def _num_frames(n_samples):
+    from .audio import num_frames_host
+    return num_frames_host(n_samples)
 
 
 # Bucket grid of the CUDA-graph training step (train_step.TrainStep): a batch whose shape differs from the first one is
@@ -172,6 +230,87 @@ class TrainTxtDataset(torch.utils.data.Dataset):
         seq = np.asarray(self.text_to_sequence(r[3]), dtype=np.int32)
         item = (seq, np.asarray(self._load(r[1]), dtype=np.float32), np.asarray(self._load(r[0]), dtype=np.float32))
         return item + (int(r[4]),) if self.multi_speaker else item
+
+
+def _wav_header(path):
+    """-> (sample rate, samples, channels, dtype) of a wav file, reading only its header (memory map)."""
+    from scipy.io import wavfile
+    sr, x = wavfile.read(path, mmap=True)
+    return int(sr), int(x.shape[0]), (1 if x.ndim == 1 else int(x.shape[1])), x.dtype
+
+
+def _resampled_length(n, sr_from, sr_to):
+    """Output length of ``audio.load_wav``'s resampling (scipy resample_poly): ceil(n * up / down)."""
+    from math import gcd
+    g = gcd(int(sr_from), int(sr_to))
+    up, down = sr_to // g, sr_from // g
+    return -(-n * up // down)
+
+
+class WavDataset(torch.utils.data.Dataset):
+    """Training straight from wav files: items are what ``collate_wav`` consumes, (token ids int32, pcm, n_frames
+    [, speaker_id]); the spectrogram targets are computed per batch on the GPU (``wav_batch_to_device``), bit-identical
+    to training on what ``preprocess.build_from_path`` writes for the same files.
+
+    items: [(wav_path, text[, speaker_id])].  pcm is the file's int16 samples when it is 16-bit mono PCM at
+    ``hparams.sample_rate`` (half the bytes of fp32 through the loader and over PCIe), otherwise ``audio.load_wav``'s
+    float32 waveform.  ``frame_lengths`` comes from the wav headers alone (the resampled length where the rate
+    differs), so ``DistributedSimilarLengthSampler`` runs without decoding any audio.  ``speaker_id`` keeps only that
+    speaker's items (and then yields 3-tuples), like ``TrainTxtDataset``."""
+
+    def __init__(self, items, text_to_sequence, speaker_id=None):
+        from .audio import hparams
+        items = [tuple(it) for it in items]
+        if not items:
+            raise ValueError("WavDataset needs at least one item")
+        n = len(items[0])
+        if n not in (2, 3) or any(len(it) != n for it in items):
+            raise ValueError("items must all be (wav_path, text) or all (wav_path, text, speaker_id)")
+        self.multi_speaker = n == 3
+        if self.multi_speaker and speaker_id is not None:
+            items = [it[:2] for it in items if int(it[2]) == speaker_id]
+            self.multi_speaker = False
+        self.items, self.text_to_sequence = items, text_to_sequence
+        self.sample_rate = hparams.sample_rate
+        self.frame_lengths = []
+        self._native = []                    # 16-bit mono at the training rate: returned as int16 without conversion
+        for it in items:
+            sr, n_samples, channels, dtype = _wav_header(it[0])
+            if sr != self.sample_rate:
+                n_samples = _resampled_length(n_samples, sr, self.sample_rate)
+            self._native.append(sr == self.sample_rate and channels == 1 and dtype == np.int16)
+            self.frame_lengths.append(_num_frames(n_samples))
+
+    @classmethod
+    def from_ljspeech(cls, in_dir, text_to_sequence):
+        """The utterances ``preprocess.build_from_path(in_dir, ...)`` processes, in its order (metadata.csv, the
+        ``hparams.min_text`` filter): item i is row i of the train.txt it writes."""
+        import os
+        from .audio import hparams
+        items = []
+        with open(os.path.join(in_dir, "metadata.csv"), encoding="utf-8") as f:
+            for line in f:
+                parts = line.strip().split("|")
+                text = parts[2]
+                if len(text) < hparams.min_text:
+                    continue
+                items.append((os.path.join(in_dir, "wavs", "%s.wav" % parts[0]), text))
+        return cls(items, text_to_sequence)
+
+    def __len__(self):
+        return len(self.items)
+
+    def __getitem__(self, idx):
+        it = self.items[idx]
+        if self._native[idx]:
+            from scipy.io import wavfile
+            pcm = np.array(wavfile.read(it[0], mmap=True)[1], dtype=np.int16)
+        else:
+            from .audio import load_wav
+            pcm = load_wav(it[0])
+        seq = np.asarray(self.text_to_sequence(it[1]), dtype=np.int32)
+        item = (seq, pcm, self.frame_lengths[idx])
+        return item + (int(it[2]),) if self.multi_speaker else item
 
 
 class DistributedSimilarLengthSampler(torch.utils.data.Sampler):

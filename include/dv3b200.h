@@ -188,6 +188,20 @@ int dv3_stft_num_frames(int n_samples);
 int dv3_stft_mel(const float* wav, const int* lengths, const float* mel_basis, const int* mel_start,
                  const int* mel_len, float* linear, float* mel, int nclips, int max_len, int max_frames,
                  int n_mels, float preemph, float min_level_db, float ref_level_db, void* stream);
+/* The same transform written straight into a training batch's target layout (data.collate after the preprocessing
+ * pass): linear (nclips, T_lin, 513) holds clip c's frame f at row lead + f; mel (nclips, ceil(T_lin / downsample_step),
+ * n_mels) holds it at row (lead + f) / downsample_step when (lead + f) % downsample_step == 0; every other row of both
+ * is written as zero.  Frames computed per clip: at most T_lin - lead.  wav (nclips, max_len) is fp32 or, with
+ * wav_int16 != 0, int16 PCM read as x / 32768 (fast staging when 16-byte aligned and max_len % 8 == 0).  peak != NULL
+ * (nclips floats on the device, dv3_peak_abs_batched) rescales each clip to x / peak * rescaling_max in fp32.  With
+ * lead = 0, downsample_step = 1, T_lin = max_frames and fp32 input this is dv3_stft_mel.  No host synchronisation. */
+int dv3_stft_mel_targets(const void* wav, int wav_int16, const int* lengths, const float* peak, float rescaling_max,
+                         const float* mel_basis, const int* mel_start, const int* mel_len, float* linear, float* mel,
+                         int nclips, int max_len, int T_lin, int lead, int downsample_step, int n_mels, float preemph,
+                         float min_level_db, float ref_level_db, void* stream);
+/* peak[c] = max |x| over the first lengths[c] samples of clip c (int16 as x / 32768); wav as above. */
+int dv3_peak_abs_batched(const void* wav, int wav_int16, const int* lengths, int max_len, int nclips, float* peak,
+                         void* stream);
 
 /* ---- inverse audio path: reference audio.py:37-43 (inv_spectrogram) and :26-28 (inv_preemphasis).  The reference
  * recovers the phase with the un-vendored `lws` package (parity UNPINNED); restated here as Griffin-Lim on the same
