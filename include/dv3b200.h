@@ -261,10 +261,12 @@ int dv3_tc_conv_supported(int B, int Cin, int Cout, int T, int k);   /* plain co
  * hold plane hi alone, [1][B][T][Cp]. */
 int dv3_tc_split_input(const float* x, void* btc, int npl, void* bct, int B, int C, int T, int k, int dilation,
                        int causal, float p_drop, const unsigned long long* seed_ptr, unsigned salt, void* stream);
-/* gate backward writing dAB = [da ; db] as planes btc: [2][B][T][2C] (dgrad operand), bct: [2][B][2C][T] (wgrad). */
+/* gate backward writing dAB = [da ; db] as planes btc: [2][B][T][2C], the operand of both the data and the weight
+ * gradient; bct is reserved and must be NULL. */
 int dv3_tc_gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, void* bct,
                           float* dbias, int B, int C, int T, int mode, int residual, void* stream);
-/* plain-conv backward prologue: g = dy*(relu ? y>0 : 1) -> btc: [2][B][T][Cp], bct: [2][B][C][T]; dbias[C] += sums. */
+/* plain-conv backward prologue: g = dy*(relu ? y>0 : 1) -> btc: [2][B][T][Cp] (the operand of both gradient GEMMs);
+ * bct is reserved and must be NULL; dbias[C] += sums. */
 int dv3_tc_grad_split(const float* dy, const float* y, void* btc, void* bct, float* dbias, int B, int C, int T,
                       int relu, void* stream);
 /* The three splits with an optional logical time extent in device memory (a training batch padded to a bucket):
