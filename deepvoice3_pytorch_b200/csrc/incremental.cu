@@ -17,6 +17,7 @@
 namespace dv3 {
 
 constexpr float kSqrtHalf = 0.70710678118654752f;
+constexpr int kAttnScratch = 9;    // floats of reduction scratch ahead of q and the scores in the attention step
 
 // step index of row b: one shared counter t_ptr[0], or (SLOTS) one counter per row t_ptr[b]
 template <bool SLOTS>
@@ -164,18 +165,18 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
     }
 }
 
-// one CTA per batch row: scores = q . keys, monotonic window, softmax, context = probs . values * Ts*sqrt(1/Ts).
+// one CTA per batch row: scores = q . keys, monotonic window, softmax, context = probs . values * float(Ts*sqrt(1/Ts)).
 // ROWS (ragged batch): row b sees only its own Ts = text_len[b] keys (the key pitch stays p.Ts) and keeps its own
 // cursor; with Ts substituted, the arithmetic is that of the single-row launch, so each row matches it bit for bit.
 // SLOTS (with ROWS): row b runs at its own step t_ptr[b] -- alignment row and cursor parity follow it.
 template <bool ROWS, bool SLOTS>
 __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constant__ Dv3IncAttn p, const int* text_len) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
-    extern __shared__ float sm[];
-    float* q = sm;                 // [E]
-    float* sc = sm + p.E;          // [Ts]
-    __shared__ float red[8];
-    __shared__ float bcast;
+    extern __shared__ float sm[];  // all of it dynamic, so the host's size check is the whole budget
+    float* red = sm;               // [kAttnScratch]: 8 per-warp partials + the broadcast slot red[8]
+    float* q = sm + kAttnScratch;  // [E]
+    float* sc = q + p.E;           // [Ts]
+    float& bcast = red[8];
     const int b = blockIdx.x, tid = threadIdx.x;
     const long long t = step_of<SLOTS>(p.t_ptr, b);
     const int Ts = ROWS ? text_len[b] : p.Ts;
@@ -231,7 +232,7 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
         p.last_attended[cur_wr] = best;
     }
     const float* __restrict__ V = p.values + (size_t)b * p.Ts * p.E;
-    const float scale = (float)Ts * sqrtf(1.0f / (float)Ts);
+    const float scale = context_scale(Ts);                  // float(Ts*sqrt(1/Ts)) rounded once, as the reference
     for (int e = tid; e < p.E; e += 256) {
         float acc = 0.f;
         for (int s = 0; s < Ts; ++s) acc = fmaf(sc[s], V[(size_t)s * p.E + e], acc);
@@ -279,6 +280,10 @@ __global__ void __launch_bounds__(256) inc_refill_kernel(const Dv3IncRefill* tab
 
 using namespace dv3;
 
+// dynamic shared memory of the attention step: the reduction scratch, q and the scores (the kernel has no static part)
+static size_t attn_smem(const Dv3IncAttn* p) { return (size_t)(kAttnScratch + p->E + p->Ts) * sizeof(float); }
+static constexpr int kAttnMaxKeys = 48 * 1024 / (int)sizeof(float) - kAttnScratch;    // largest E + Ts
+
 extern "C" {
 
 int dv3_inc_conv_step(const Dv3IncStep* p, void* stream) {
@@ -312,26 +317,27 @@ int dv3_inc_conv_step_slots(const Dv3IncStep* p, void* stream) {
 
 int dv3_inc_attn_step(const Dv3IncAttn* p, void* stream) {
     DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0, "inc_attn_step: bad shape");
-    const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
-    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step: E + Ts = %d floats exceed 48 KB of shared memory", p->E + p->Ts);
+    const size_t smem = attn_smem(p);
+    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
+                p->E + p->Ts, kAttnMaxKeys);
     launch_k(inc_attn_step_kernel<false, false>, p->B, 256, smem, (cudaStream_t)stream, *p, (const int*)nullptr);
     return check_launch("inc_attn_step");
 }
 
 int dv3_inc_attn_step_rows(const Dv3IncAttn* p, const int* text_len, void* stream) {
     DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0 && text_len, "inc_attn_step_rows: bad shape");
-    const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
-    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_rows: E + Ts = %d floats exceed 48 KB of shared memory",
-                p->E + p->Ts);
+    const size_t smem = attn_smem(p);
+    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_rows: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
+                p->E + p->Ts, kAttnMaxKeys);
     launch_k(inc_attn_step_kernel<true, false>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
     return check_launch("inc_attn_step_rows");
 }
 
 int dv3_inc_attn_step_slots(const Dv3IncAttn* p, const int* text_len, void* stream) {
     DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0 && text_len && p->t_ptr, "inc_attn_step_slots: bad shape");
-    const size_t smem = (size_t)(p->E + p->Ts) * sizeof(float);
-    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_slots: E + Ts = %d floats exceed 48 KB of shared memory",
-                p->E + p->Ts);
+    const size_t smem = attn_smem(p);
+    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_slots: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
+                p->E + p->Ts, kAttnMaxKeys);
     launch_k(inc_attn_step_kernel<true, true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
     return check_launch("inc_attn_step_slots");
 }

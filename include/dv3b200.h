@@ -404,12 +404,12 @@ int dv3_inc_conv_step(const Dv3IncStep* step, void* stream);
 typedef struct Dv3IncAttn {
     const float* q; long long q_ld;                /* projected query (B, E) */
     const float* keys; const float* values;        /* (B, E, Ts) pre-transposed, (B, Ts, E): projected once */
-    float* ctx; long long ctx_ld;                  /* context * Ts*sqrt(1/Ts) (B, E) */
+    float* ctx; long long ctx_ld;                  /* context * float(Ts*sqrt(1/Ts)) (B, E) */
     float* align; long long align_ld, align_t;     /* probabilities * align_scale, or NULL */
     int* last_attended;                            /* int[2] (slot t&1 read, (t+1)&1 written) or NULL: no window */
     const int* t_ptr;
     float align_scale;
-    int B, E, Ts, window_backward, window_ahead;
+    int B, E, Ts, window_backward, window_ahead;   /* E + Ts <= 12279: with 9 floats of scratch, 48 KB of smem */
 } Dv3IncAttn;
 int dv3_inc_attn_step(const Dv3IncAttn* attn, void* stream);
 /* Ragged batch: row b attends to s < text_len[b] only (text_len: int32 [B] on the device, 1 <= text_len[b] <= Ts),
