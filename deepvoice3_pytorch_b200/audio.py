@@ -84,11 +84,8 @@ def _device_basis(device):
     return _basis_cache[key]
 
 
-def load_wav(path):
-    """float32 mono waveform in [-1, 1] at ``hparams.sample_rate`` -- reference audio.py:12-13
-    (``librosa.core.load(path, sr=hparams.sample_rate)[0]``).  Host-side file plumbing (scipy): integer PCM is scaled by
-    its full range, channels are averaged, and a file at another rate is resampled with a polyphase filter (librosa
-    uses resampy's kaiser_best; identical output only when the rates already agree, as for the reference's datasets)."""
+def decode_wav(path):
+    """-> (sample rate, float32 mono waveform): ``load_wav`` before its resampling step."""
     from scipy.io import wavfile
     sr, x = wavfile.read(path)
     if np.issubdtype(x.dtype, np.integer):
@@ -98,6 +95,15 @@ def load_wav(path):
         x = x.astype(np.float32)
     if x.ndim > 1:
         x = x.mean(axis=1)
+    return int(sr), x
+
+
+def load_wav(path):
+    """float32 mono waveform in [-1, 1] at ``hparams.sample_rate`` -- reference audio.py:12-13
+    (``librosa.core.load(path, sr=hparams.sample_rate)[0]``).  Host-side file plumbing (scipy): integer PCM is scaled by
+    its full range, channels are averaged, and a file at another rate is resampled with a polyphase filter (librosa
+    uses resampy's kaiser_best; identical output only when the rates already agree, as for the reference's datasets)."""
+    sr, x = decode_wav(path)
     if sr != hparams.sample_rate:
         from math import gcd
         from scipy.signal import resample_poly
@@ -209,6 +215,147 @@ def stft_mel_batch(wav, lengths=None, want_linear=True, want_mel=True):
              max_frames, hparams.num_mels, float(hparams.preemphasis), float(hparams.min_level_db),
              float(hparams.ref_level_db), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     return lin, mel
+
+
+def resample_ratio(sr_from, sr_to=None):
+    """(up, down) = sr_to / sr_from reduced by its gcd (``sr_to`` defaults to ``hparams.sample_rate``)."""
+    from math import gcd
+    sr_from, sr_to = int(sr_from), int(hparams.sample_rate if sr_to is None else sr_to)
+    if sr_from < 1 or sr_to < 1:
+        raise ValueError("sample rates must be positive, got %d -> %d" % (sr_from, sr_to))
+    g = gcd(sr_from, sr_to)
+    return sr_to // g, sr_from // g
+
+
+def resample_filter_bank(up, down):
+    """The filter of ``scipy.signal.resample_poly(x, up, down)`` for fp64 x, in polyphase form: -> (bank (ntaps, up)
+    float64 with bank[j, p] = h[p + j * up], pre_remove).  h is ``firwin(2 * half_len + 1, 1 / max(up, down),
+    window=('kaiser', 5.0)) * up`` with half_len = 10 * max(up, down), preceded by resample_poly's down - half_len % down
+    zeros; pre_remove is the number of leading outputs resample_poly drops.  up == down == 1 is the identity."""
+    from scipy.signal import firwin
+    if up == 1 and down == 1:
+        return np.ones((1, 1)), 0
+    max_rate = max(up, down)
+    half_len = 10 * max_rate
+    h = firwin(2 * half_len + 1, 1.0 / max_rate, window=("kaiser", 5.0)) * up
+    n_pre_pad = down - half_len % down
+    h = np.concatenate([np.zeros(n_pre_pad), h])
+    ntaps = -(-len(h) // up)
+    h = np.concatenate([h, np.zeros(ntaps * up - len(h))])
+    return np.ascontiguousarray(h.reshape(ntaps, up)), (half_len + n_pre_pad) // down
+
+
+_bank_cache = {}
+
+
+def _device_bank(device, up, down):
+    key = (str(device), up, down)
+    if key not in _bank_cache:
+        bank, pre_remove = resample_filter_bank(up, down)
+        _bank_cache[key] = (torch.from_numpy(bank).to(device), bank.shape[0], pre_remove)
+    return _bank_cache[key]
+
+
+def resampled_length(n, up, down):
+    """Samples of resample_poly's output for n input samples: ceil(n * up / down)."""
+    return -(-int(n) * up // down)
+
+
+def _pcm_batch(wav, name):
+    if not (torch.is_tensor(wav) and wav.is_cuda and wav.dim() == 2):
+        raise Dv3Error("%s needs a (nclips, pitch) CUDA tensor; there is no CPU path" % name)
+    if wav.dtype not in (torch.int16, torch.float32):
+        raise Dv3Error("%s takes int16 PCM or fp32 waveforms, got %s" % (name, wav.dtype))
+    if wav.shape[0] < 1:
+        raise Dv3Error("%s needs at least one clip" % name)
+    return wav.contiguous()
+
+
+def _host_ints(values, n, name, what):
+    values = [int(v) for v in (values.tolist() if torch.is_tensor(values) else values)]
+    if len(values) != n:
+        raise Dv3Error("%s: %s must give one value per clip (%d), got %d" % (name, what, n, len(values)))
+    return values
+
+
+def resample_batch(wav, lengths, sr_from):
+    """Resample a ragged batch from ``sr_from`` to ``hparams.sample_rate`` in one launch: wav (nclips, pitch) int16 PCM
+    (read as x / 32768, like ``load_wav``) or fp32 CUDA tensor, clip c valid for its first lengths[c] samples (host
+    sequence).  -> (out (nclips, pitch_out) fp32 with clip c's ``resampled_length`` samples and zeros after them, the
+    output lengths as a list).  Each output sample is scipy's ``resample_poly`` of the fp64 clip rounded to fp32
+    (csrc/resample.cu), bit-identical whatever else is in the batch."""
+    wav = _pcm_batch(wav, "resample_batch")
+    nclips, pitch = wav.shape
+    lengths = _host_ints(lengths, nclips, "resample_batch", "lengths")
+    if not all(0 <= n <= pitch for n in lengths):
+        raise Dv3Error("resample_batch: lengths must lie in 0..%d" % pitch)
+    up, down = resample_ratio(sr_from)
+    out_lens = [resampled_length(n, up, down) for n in lengths]
+    pitch_out = max(4, (max(out_lens) + 3) // 4 * 4)
+    if pitch_out >= 2 ** 31:
+        raise Dv3Error("resample_batch: %d output samples per clip is too many" % pitch_out)
+    dev = wav.device
+    bank, ntaps, pre_remove = _device_bank(dev, up, down)
+    lengths_dev = torch.tensor(lengths, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    out = torch.empty(nclips, pitch_out, device=dev)                   # the kernel writes every sample
+    lib.call("dv3_resample_poly_batched", _cp(wav), int(wav.dtype == torch.int16), _cp(lengths_dev), pitch, _cp(out),
+             pitch_out, nclips, _cp(bank), up, down, ntaps, pre_remove,
+             ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+    return out, out_lens
+
+
+def trim_bounds_batch(wav, lengths, top_db, offsets=None):
+    """Silence-trim bounds of a ragged batch in one launch: ``librosa.effects.trim(y, top_db)`` with the librosa
+    0.6-0.9 defaults (frame 2048, hop 512, ref = max, centred frames with reflect padding) computed in fp64, where
+    y = wav[c, offsets[c] : offsets[c] + lengths[c]].  wav as in ``resample_batch``; lengths, offsets (default 0) and
+    top_db (a number, or one per clip) are host values.  -> (nclips, 2) int32 CUDA tensor of (start, end) relative to
+    y, (0, 0) for a clip with no frame above the threshold (csrc/resample.cu)."""
+    wav = _pcm_batch(wav, "trim_bounds_batch")
+    nclips, pitch = wav.shape
+    lengths = _host_ints(lengths, nclips, "trim_bounds_batch", "lengths")
+    offs = [0] * nclips if offsets is None else _host_ints(offsets, nclips, "trim_bounds_batch", "offsets")
+    if not all(n >= 0 and o >= 0 and o + n <= pitch for n, o in zip(lengths, offs)):
+        raise Dv3Error("trim_bounds_batch: every segment must lie inside its row of %d samples" % pitch)
+    dbs = [float(top_db)] * nclips if np.ndim(top_db) == 0 else [float(t) for t in top_db]
+    if len(dbs) != nclips:
+        raise Dv3Error("trim_bounds_batch: top_db must be a number or one value per clip")
+    dev = wav.device
+    ints = torch.tensor(lengths + offs, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
+    dbs = torch.tensor(dbs, dtype=torch.float64).pin_memory().to(dev, non_blocking=True)
+    bounds = torch.empty(nclips, 2, dtype=torch.int32, device=dev)
+    lib.call("dv3_trim_bounds_batched", _cp(wav), int(wav.dtype == torch.int16), _cp(ints),
+             None if offsets is None else _cp(ints[nclips:]), pitch, nclips, _cp(dbs), _cp(bounds),
+             ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+    return bounds
+
+
+def trim_bounds_reference(y, top_db):
+    """``trim_bounds_batch``'s definition restated in numpy fp64 for one segment y -> (start, end): the test oracle of
+    the kernel and the host arm of bench_preprocess_vctk.py.  librosa >= 0.10 pads with zeros instead of reflecting,
+    which changes the edge frames only."""
+    y = np.asarray(y, dtype=np.float64)
+    L = len(y)
+    if L == 0:
+        return 0, 0
+    frame, hop = 2048, 512
+    padded = y[reflect_index(np.arange(-frame // 2, L + frame // 2), L)]
+    mse = np.array([np.mean(padded[hop * f: hop * f + frame] ** 2) for f in range(L // hop + 1)])
+    db = 10.0 * np.log10(np.maximum(1e-10, mse))
+    keep = np.flatnonzero(db - 10.0 * np.log10(np.maximum(1e-10, mse.max())) > -top_db)
+    if keep.size == 0:
+        return 0, 0
+    return int(hop * keep[0]), int(min(L, hop * (keep[-1] + 1)))
+
+
+def reflect_index(q, L):
+    """Index into a length-L signal of positions q of its ``np.pad(mode='reflect')`` extension (numpy reflects again
+    and again when the pad is longer than the signal): period 2 (L - 1), mirrored about 0 and L - 1."""
+    q = np.asarray(q)
+    if L == 1:
+        return np.zeros_like(q)
+    period = 2 * (L - 1)
+    r = np.mod(q, period)
+    return np.where(r >= L, period - r, r)
 
 
 def _single(y, want_linear, want_mel):

@@ -203,6 +203,27 @@ int dv3_stft_mel_targets(const void* wav, int wav_int16, const int* lengths, con
 int dv3_peak_abs_batched(const void* wav, int wav_int16, const int* lengths, int max_len, int nclips, float* peak,
                          void* stream);
 
+/* ---- corpus front-end ahead of the STFT (csrc/resample.cu): the resampling inside reference audio.py:12-13
+ * (load_wav) and the silence trimming of vctk.py:52-68 (librosa.effects.trim), for a ragged batch of clips.
+ * dv3_resample_poly_batched: scipy.signal.resample_poly(x.astype(float64), up, down) rounded to fp32 (window
+ * ('kaiser', 5.0), zero padding), up / down reduced.  wav (nclips, pitch_in) fp32 or, with wav_int16 != 0, int16 PCM
+ * read as x / 32768; lengths int32 [nclips]; out (nclips, pitch_out) fp32 holds clip c's
+ * dv3_resample_out_len(lengths[c], up, down) = ceil(n * up / down) samples, zero after them.  bank (ntaps, up) fp64 is
+ * the polyphase filter bank, bank[j][p] = h[p + j * up] of the zero-padded filter h, and pre_remove the outputs
+ * resample_poly drops in front (audio.resample_filter_bank).  Products and sums in fp64, in a fixed order per output:
+ * a clip is bit-identical alone and in any batch.  The bank and a window of input stay in shared memory
+ * (8 * up * ntaps + 4 * (4095 * down / up + ntaps + 2) bytes, at most the device's opt-in limit).
+ * dv3_trim_bounds_batched: librosa.effects.trim(y, top_db[c]) (frame 2048, hop 512, ref = max, centred frames,
+ * reflect padding; the librosa 0.6-0.9 defaults) of y = clip c's samples [offsets[c], offsets[c] + lengths[c]), in
+ * fp64 -> bounds (nclips, 2) int32 (start, end) relative to y, (0, 0) when no frame is above the threshold.  wav as
+ * above with row pitch `pitch`; offsets may be NULL (all 0); top_db fp64 [nclips].  No host synchronisation. */
+int dv3_resample_out_len(int n_samples, int up, int down);
+int dv3_resample_poly_batched(const void* wav, int wav_int16, const int* lengths, int pitch_in, float* out,
+                              int pitch_out, int nclips, const double* bank, int up, int down, int ntaps,
+                              int pre_remove, void* stream);
+int dv3_trim_bounds_batched(const void* wav, int wav_int16, const int* lengths, const int* offsets, int pitch,
+                            int nclips, const double* top_db, int* bounds, void* stream);
+
 /* ---- inverse audio path: reference audio.py:37-43 (inv_spectrogram) and :26-28 (inv_preemphasis).  The reference
  * recovers the phase with the un-vendored `lws` package (parity UNPINNED); restated here as Griffin-Lim on the same
  * sqrt-Hann 1024 / hop 256 / 768-pad frame as dv3_stft_mel (sum of squared windows == 1: synthesis window = analysis
