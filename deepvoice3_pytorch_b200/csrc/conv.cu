@@ -410,7 +410,8 @@ int dv3_convblock_fwd(const float* x, const float* w_f, const float* bias, const
                       int mode, int residual, float p_drop, const unsigned long long* seed_ptr,
                       unsigned salt, void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS, "convblock_fwd: kernel size %d not in [1,%d]", k, MAX_TAPS);
-    DV3_REQUIRE((long long)B * C * T < (1LL << 31), "convblock_fwd: tensor too large for 32-bit indexing");
+    DV3_REQUIRE((long long)B * C * T < (1LL << 31),
+                "convblock_fwd: tensor of %lld elements too large for 32-bit indexing", (long long)B * C * T);
     DV3_REQUIRE(mode == 0 || mode == 1, "convblock_fwd: mode must be 0 (GLU) or 1 (highway)");
     ConvParams p = {};
     p.x = x; p.w = w_f; p.bias = bias; p.spk = spk; p.res = x; p.y = y; p.save_a = save_a; p.save_s = save_s;
@@ -425,7 +426,9 @@ int dv3_convblock_fwd(const float* x, const float* w_f, const float* bias, const
 int dv3_conv1d_fwd(const float* x, const float* w_f, const float* bias, float* y, int B, int Cin, int Cout,
                    int T, int k, int dilation, int causal, int relu, void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS, "conv1d_fwd: kernel size %d not in [1,%d]", k, MAX_TAPS);
-    DV3_REQUIRE((long long)B * (Cin > Cout ? Cin : Cout) * T < (1LL << 31), "conv1d_fwd: tensor too large");
+    DV3_REQUIRE((long long)B * (Cin > Cout ? Cin : Cout) * T < (1LL << 31),
+                "conv1d_fwd: tensor of %lld elements too large for 32-bit indexing",
+                (long long)B * (Cin > Cout ? Cin : Cout) * T);
     ConvParams p = {};
     p.x = x; p.w = w_f; p.bias = bias; p.y = y;
     p.B = B; p.Cin = Cin; p.T = T; p.N = B * T; p.Mtot = Cout; p.k = k; p.cpt = ceil_div(Cin, GEMM_BK);
@@ -441,6 +444,9 @@ int dv3_conv1d_dgrad(const float* dab, const float* w_b, float* dx, int B, int M
                      void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS, "conv1d_dgrad: kernel size %d not in [1,%d]", k, MAX_TAPS);
     DV3_REQUIRE(addmode >= 0 && addmode <= 2, "conv1d_dgrad: bad addmode");
+    DV3_REQUIRE((long long)B * (M > Cin ? M : Cin) * T < (1LL << 31),
+                "conv1d_dgrad: tensor of %lld elements too large for 32-bit indexing",
+                (long long)B * (M > Cin ? M : Cin) * T);
     ConvParams p = {};
     p.x = dab; p.w = w_b; p.y = dx;
     p.B = B; p.Cin = M; p.T = T; p.N = B * T; p.Mtot = Cin; p.k = k; p.cpt = ceil_div(M, GEMM_BK);
@@ -468,6 +474,9 @@ int dv3_conv1d_wgrad(const float* dab, const float* x, float* dw_partials, long 
                      const unsigned long long* seed_ptr, unsigned salt, int msplit, int s_m, int s_mh,
                      int s_n, int s_j, void* stream) {
     DV3_REQUIRE(k >= 1 && k <= MAX_TAPS, "conv1d_wgrad: kernel size %d not in [1,%d]", k, MAX_TAPS);
+    DV3_REQUIRE((long long)B * (M > Cin ? M : Cin) * T < (1LL << 31),
+                "conv1d_wgrad: tensor of %lld elements too large for 32-bit indexing",
+                (long long)B * (M > Cin ? M : Cin) * T);
     WgradParams p = {};
     p.dab = dab; p.x = x; p.dw = dw_partials; p.split_stride = (size_t)split_stride;
     p.B = B; p.M = M; p.Cin = Cin; p.T = T; p.N = B * T; p.k = k;
