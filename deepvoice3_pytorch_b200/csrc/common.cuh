@@ -131,4 +131,7 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
+// ---- deterministic mode: dbias[c] += sum_i scratch[i][c], i < nparts, in a fixed order (conv.cu bias_reduce_kernel) ----
+int bias_reduce(const float* scratch, int nparts, int nch, float* dbias, cudaStream_t st);
+
 }  // namespace dv3

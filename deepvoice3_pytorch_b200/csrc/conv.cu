@@ -316,7 +316,10 @@ struct WgradPolicy {
 //   GLU     : y = a*s [ (.+x)*sqrt.5 ]      da = g*s ; db = g*a*s*(1-s)            g = dy*(res?sqrt.5:1)
 //   highway : y = s*a + (1-s)*x             da = dy*s ; db = dy*(a-x)*s*(1-s)
 // writes dAB (B, 2C, T) = [da ; db], dbias[2C] += row sums.  One warp per (b, c) row.
+// DET (deterministic mode): dbias is a scratch [B][2C] instead; the warp stores its row sums at [b][c], [b][C + c] and
+// bias_reduce_kernel adds them to the bias gradient in a fixed order.
 // ------------------------------------------------------------------------------------------------
+template <bool DET>
 __global__ void gate_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ a,
                                 const float* __restrict__ s, const float* __restrict__ x,
                                 float* __restrict__ dab, float* __restrict__ dbias, int B, int C, int T,
@@ -338,10 +341,16 @@ __global__ void gate_bwd_kernel(const float* __restrict__ dy, const float* __res
         sa += da; sb += db;
     }
     sa = warp_sum(sa); sb = warp_sum(sb);
+    if (DET) {
+        if (lane == 0) { dbias[(size_t)b * 2 * C + c] = sa; dbias[(size_t)b * 2 * C + C + c] = sb; }
+        return;
+    }
     if (lane == 0 && dbias) { atomicAdd(&dbias[c], sa); atomicAdd(&dbias[C + c], sb); }
 }
 
 // plain conv: dyr = dy * (relu ? y>0 : 1) ; dbias[c] += sum_{b,t} dyr.  One warp per (b,c) row.
+// DET: dbias is a scratch [B][C] that receives the row sums, as in gate_bwd_kernel.
+template <bool DET>
 __global__ void bias_act_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y,
                                     float* __restrict__ dyr, float* __restrict__ dbias, int B, int C,
                                     int T, int relu) {
@@ -357,7 +366,39 @@ __global__ void bias_act_bwd_kernel(const float* __restrict__ dy, const float* _
         sum += g;
     }
     sum = warp_sum(sum);
+    if (DET) {
+        if (lane == 0) dbias[warp] = sum;            // [b][c]
+        return;
+    }
     if (lane == 0 && dbias) atomicAdd(&dbias[c], sum);
+}
+
+// Deterministic mode: dbias[c] += sum over the partials scratch[i][c], i < nparts, in a fixed order.  A block owns 32
+// channels x 8 slices; slice s adds the partials [s * per, (s + 1) * per) in ascending order (coalesced across the
+// channels), then thread (c, 0) adds the eight slice sums in slice order.  per = ceil(nparts / 8): the order depends
+// on the shapes alone.
+__global__ void __launch_bounds__(256) bias_reduce_kernel(const float* __restrict__ scratch, int nparts, int nch,
+                                                          float* __restrict__ dbias) {
+    pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
+    __shared__ float part[8][33];
+    const int c = blockIdx.x * 32 + threadIdx.x, s = threadIdx.y;
+    const int per = (nparts + 7) / 8, i0 = s * per, i1 = min(nparts, i0 + per);
+    float acc = 0.f;
+    if (c < nch)
+        for (int i = i0; i < i1; ++i) acc += scratch[(size_t)i * nch + c];
+    part[s][threadIdx.x] = acc;
+    __syncthreads();
+    if (s == 0 && c < nch) {
+        float t = part[0][threadIdx.x];
+#pragma unroll
+        for (int j = 1; j < 8; ++j) t += part[j][threadIdx.x];
+        dbias[c] += t;
+    }
+}
+
+int bias_reduce(const float* scratch, int nparts, int nch, float* dbias, cudaStream_t st) {
+    launch_k(bias_reduce_kernel, ceil_div(nch, 32), dim3(32, 8), 0, st, scratch, nparts, nch, dbias);
+    return check_launch("bias_reduce");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -492,17 +533,48 @@ int dv3_conv1d_wgrad(const float* dab, const float* x, float* dw_partials, long 
 int dv3_convblock_gate_bwd(const float* dy, const float* a, const float* s, const float* x, float* dab,
                            float* dbias, int B, int C, int T, int mode, int residual, void* stream) {
     const int warps = B * C, threads = 256;
-    launch_k(gate_bwd_kernel, ceil_div(warps * 32, threads), threads, 0, (cudaStream_t)stream, 
+    launch_k(gate_bwd_kernel<false>, ceil_div(warps * 32, threads), threads, 0, (cudaStream_t)stream, 
         dy, a, s, x, dab, dbias, B, C, T, mode, residual);
     return check_launch("convblock_gate_bwd");
+}
+
+// Deterministic form: the same dAB; the row sums go to scratch [B][2C] (>= dv3_bias_det_scratch_floats(B, 2C, T, 0)
+// floats) and are added to dbias in batch order by a second launch.
+int dv3_convblock_gate_bwd_det(const float* dy, const float* a, const float* s, const float* x, float* dab,
+                               float* dbias, float* scratch, long long scratch_floats, int B, int C, int T, int mode,
+                               int residual, void* stream) {
+    DV3_REQUIRE(dbias != nullptr && scratch != nullptr && scratch_floats >= (long long)B * 2 * C,
+                "convblock_gate_bwd_det: dbias and a scratch of >= %lld floats required", (long long)B * 2 * C);
+    const int warps = B * C, threads = 256;
+    launch_k(gate_bwd_kernel<true>, ceil_div(warps * 32, threads), threads, 0, (cudaStream_t)stream,
+        dy, a, s, x, dab, scratch, B, C, T, mode, residual);
+    if (int e = check_launch("convblock_gate_bwd_det")) return e;
+    return bias_reduce(scratch, B, 2 * C, dbias, (cudaStream_t)stream);
 }
 
 int dv3_bias_act_bwd(const float* dy, const float* y, float* dyr, float* dbias, int B, int C, int T,
                      int relu, void* stream) {
     const int warps = B * C, threads = 256;
-    launch_k(bias_act_bwd_kernel, ceil_div(warps * 32, threads), threads, 0, (cudaStream_t)stream, 
+    launch_k(bias_act_bwd_kernel<false>, ceil_div(warps * 32, threads), threads, 0, (cudaStream_t)stream, 
         dy, y, dyr, dbias, B, C, T, relu);
     return check_launch("bias_act_bwd");
+}
+
+int dv3_bias_act_bwd_det(const float* dy, const float* y, float* dyr, float* dbias, float* scratch,
+                         long long scratch_floats, int B, int C, int T, int relu, void* stream) {
+    DV3_REQUIRE(dbias != nullptr && scratch != nullptr && scratch_floats >= (long long)B * C,
+                "bias_act_bwd_det: dbias and a scratch of >= %lld floats required", (long long)B * C);
+    const int warps = B * C, threads = 256;
+    launch_k(bias_act_bwd_kernel<true>, ceil_div(warps * 32, threads), threads, 0, (cudaStream_t)stream,
+        dy, y, dyr, scratch, B, C, T, relu);
+    if (int e = check_launch("bias_act_bwd_det")) return e;
+    return bias_reduce(scratch, B, C, dbias, (cudaStream_t)stream);
+}
+
+// Floats of scratch the deterministic bias-gradient entry points need for nch channels: one partial row per utterance
+// (the exact-fp32 kernels, tiled = 0) or per (utterance, 64-frame tile) (the tensor-core operand splits, tiled = 1).
+long long dv3_bias_det_scratch_floats(int B, int nch, int T, int tiled) {
+    return (long long)B * (tiled ? ceil_div(T, 64) : 1) * nch;
 }
 
 }  // extern "C"

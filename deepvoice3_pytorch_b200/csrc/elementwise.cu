@@ -88,6 +88,70 @@ __global__ void sinusoid_bwd_kernel(const long long* __restrict__ pos, const flo
     }
 }
 
+// ---- deterministic mode: the two table gradients without atomics -----------------------------------------------------
+// One CTA (256 threads) per table row.  The CTA scans the id list 256 entries at a time and compacts the entries that
+// name its row into shared memory IN INDEX ORDER (warp ballots + a prefix over the 8 warp counts); every thread then
+// walks that list and accumulates its columns (d = tid, tid + 256, ...: D <= TABLE_DET_MAX_D) in registers, and the row
+// is stored once, coalesced: dtable[row] += sum.  Each element is therefore the sum of its tokens in ascending token
+// index, whatever order blocks run in.  SINUSOID = false: dtable[ids[n]] += dy[n] (row padding_idx gets nothing);
+// SINUSOID = true: the position-table gradient of sinusoid_bwd_kernel, term for term (row 0 gets nothing).
+constexpr int TABLE_DET_MAX_D = 1024;
+template <bool SINUSOID>
+__global__ void __launch_bounds__(256) table_bwd_det_kernel(const long long* __restrict__ ids,
+                                                            const float* __restrict__ table,
+                                                            const float* __restrict__ w, int nw, int T,
+                                                            const float* __restrict__ dy, float* __restrict__ dtable,
+                                                            int N, int D, long long padding_idx) {
+    pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
+    __shared__ int s_list[256];
+    __shared__ int s_cnt[8];
+    const int row = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (row == padding_idx) return;
+    float acc[4] = {0.f, 0.f, 0.f, 0.f}, tv[4] = {0.f, 0.f, 0.f, 0.f};
+    if (SINUSOID) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+            if (tid + 256 * q < D) tv[q] = table[(size_t)row * D + tid + 256 * q];
+    }
+    bool any = false;
+    for (int base = 0; base < N; base += 256) {
+        const int n = base + tid;
+        const bool match = n < N && ids[n] == row;
+        const unsigned bal = __ballot_sync(0xffffffffu, match);
+        if (lane == 0) s_cnt[warp] = __popc(bal);
+        __syncthreads();
+        int off = 0, total = 0;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) { if (i < warp) off += s_cnt[i]; total += s_cnt[i]; }
+        if (match) s_list[off + __popc(bal & ((1u << lane) - 1u))] = n;
+        __syncthreads();
+        for (int j = 0; j < total; ++j) {
+            const int m = s_list[j];
+            const float wb = SINUSOID ? w[nw == 1 ? 0 : m / T] : 0.f;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int d = tid + 256 * q;
+                if (d < D) {
+                    const float g = dy[(size_t)m * D + d];
+                    if (SINUSOID) {
+                        const float a = wb * tv[q];
+                        const float da = g * ((d & 1) ? -sinf(a) : cosf(a));
+                        acc[q] += __fmul_rn(da, wb);      // the rounded product the atomic kernel adds: no fma
+                    } else {
+                        acc[q] += g;
+                    }
+                }
+            }
+        }
+        any |= total > 0;
+        __syncthreads();
+    }
+    if (!any) return;
+#pragma unroll
+    for (int q = 0; q < 4; ++q)
+        if (tid + 256 * q < D) dtable[(size_t)row * D + tid + 256 * q] += acc[q];
+}
+
 // d(loss)/d(position rate): dw[wi] = sum over the rows of utterance wi (all rows if nw == 1) of <dy * d(enc)/d(a), table>.
 // The sum cancels heavily (its terms are O(1), the result often 1e-4 of that), so it is accumulated in double by ONE
 // CTA per rate, in a fixed order: deterministic, and as accurate as the fp32 CPU reference (float atomics over the
@@ -272,6 +336,30 @@ int dv3_sinusoid_bwd(const long long* pos, const float* table, const float* w, i
     if (dw) {
         launch_k(sinusoid_dw_kernel, nw, 256, 0, (cudaStream_t)stream, pos, table, w, nw, dy, dw, B, T, D, P);
         if (int e = check_launch("sinusoid_bwd(rate)")) return e;
+    }
+    return 0;
+}
+
+// Deterministic forms of the two table gradients (table_bwd_det_kernel): same values term for term, summed in token order.
+int dv3_embedding_bwd_det(const long long* ids, const float* dy, float* dtable, int N, int D, int V,
+                          long long padding_idx, void* stream) {
+    DV3_REQUIRE(D >= 1 && D <= TABLE_DET_MAX_D && V >= 1, "embedding_bwd_det: D=%d not in [1,%d]", D, TABLE_DET_MAX_D);
+    launch_k(table_bwd_det_kernel<false>, V, 256, 0, (cudaStream_t)stream, ids, (const float*)nullptr,
+             (const float*)nullptr, 1, 1, dy, dtable, N, D, padding_idx);
+    return check_launch("embedding_bwd_det");
+}
+int dv3_sinusoid_bwd_det(const long long* pos, const float* table, const float* w, int nw, const float* dy,
+                         float* dtable, float* dw, int B, int T, int D, int P, void* stream) {
+    DV3_REQUIRE(nw == 1 || nw == B, "sinusoid_bwd_det: need 1 or B position rates, got %d", nw);
+    if (dtable) {
+        DV3_REQUIRE(D >= 1 && D <= TABLE_DET_MAX_D && P >= 1, "sinusoid_bwd_det: D=%d not in [1,%d]", D, TABLE_DET_MAX_D);
+        launch_k(table_bwd_det_kernel<true>, P, 256, 0, (cudaStream_t)stream, pos, table, w, nw, T, dy, dtable, B * T,
+                 D, 0LL);
+        if (int e = check_launch("sinusoid_bwd_det(table)")) return e;
+    }
+    if (dw) {       // already a fixed-order, one-CTA reduction
+        launch_k(sinusoid_dw_kernel, nw, 256, 0, (cudaStream_t)stream, pos, table, w, nw, dy, dw, B, T, D, P);
+        if (int e = check_launch("sinusoid_bwd_det(rate)")) return e;
     }
     return 0;
 }

@@ -21,6 +21,41 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
     return t;            // valid in thread 0 (and lanes of warp 0)
 }
 
+// ---- deterministic mode (ops.deterministic): fixed-order sums instead of one float atomic per block ----------------
+// Every block stores its (up to) three partial sums at scratch[3 * blockIdx.x ..]; the block that draws the last
+// ticket adds them in a fixed order -- warp j owns sum j, lane l adds the partials of blocks l, l + 32, ... in ascending
+// order, then the xor-shuffle tree of warp_sum -- and adds the totals to loss / terms.  The order depends on the grid
+// alone, and the grid on the tensor shapes alone.  No block waits for another: the last one to arrive does the tail.
+// scratch: LOSS_DET_SCRATCH floats, zero-filled once by the caller; its last word is the ticket, left at zero.
+constexpr int LOSS_MAX_BLOCKS = 132 * 8;
+constexpr int LOSS_DET_SCRATCH = 3 * LOSS_MAX_BLOCKS + 1;
+
+template <bool TERMS>
+__device__ __forceinline__ void det_loss_tail(float s, float s1, float s2, float* __restrict__ loss,
+                                              float* __restrict__ terms, float* __restrict__ scratch) {
+    __shared__ bool last;
+    if (threadIdx.x == 0) {
+        scratch[3 * blockIdx.x] = s;
+        if (TERMS) { scratch[3 * blockIdx.x + 1] = s1; scratch[3 * blockIdx.x + 2] = s2; }
+        __threadfence();
+        unsigned* ticket = reinterpret_cast<unsigned*>(scratch + LOSS_DET_SCRATCH - 1);
+        last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return;
+    __threadfence();
+    const int j = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (j < (TERMS ? 3 : 1)) {
+        float t = 0.f;
+        for (int i = lane; i < (int)gridDim.x; i += 32) t += __ldcg(&scratch[3 * i + j]);
+        t = warp_sum(t);
+        if (lane == 0) {
+            if (j == 0) loss[0] += t; else terms[j - 1] += t;
+        }
+    }
+    if (threadIdx.x == 0) *reinterpret_cast<unsigned*>(scratch + LOSS_DET_SCRATCH - 1) = 0u;
+}
+
 // y_hat (B, T, D) predictions, y (B, T, D) targets; pairs (y_hat[b,t], y[b,t+r]) for t < T-r; lengths int64 [B]
 // (valid target frames per utterance, in this tensor's time units); grad (B, T, D) fully written.
 //   loss += sum (1-bw)*coef1*|d| + bw*coef*z,  coef = w*m/Sm + (1-w)/N,  m = (t+r < len_b)
@@ -30,11 +65,14 @@ __device__ __forceinline__ float block_sum_256(float v, float* red) {
 // t >= t_log - r are left out of the loss and its means, and their gradient is written as 0.
 // TERMS: also add the two parts of the loss to terms[0] (the L1 part, priority bins combined) and terms[1] (the
 // binary-divergence part) -- the l1_loss / binary_div pair reference spec_loss returns.  loss and grad are unchanged.
-template <bool TERMS>
-__global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* __restrict__ y,
-                                 const long long* __restrict__ lengths, const long long* __restrict__ t_log,
-                                 float* __restrict__ grad, float* __restrict__ loss, int B, int T, int D, int r,
-                                 float w, float bw, float eps, int pbin, float pw, float* __restrict__ terms) {
+// DET: the block sums go through det_loss_tail (scratch) instead of the atomics; everything else is the same code.
+template <bool TERMS, bool DET>
+__device__ __forceinline__ void spec_loss_body(const float* __restrict__ y_hat, const float* __restrict__ y,
+                                               const long long* __restrict__ lengths,
+                                               const long long* __restrict__ t_log, float* __restrict__ grad,
+                                               float* __restrict__ loss, int B, int T, int D, int r, float w, float bw,
+                                               float eps, int pbin, float pw, float* __restrict__ terms,
+                                               float* __restrict__ scratch) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float red[8];
     __shared__ float s_inv_sm;
@@ -86,6 +124,11 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
         grad[i] = g;
     }
     const float s = block_sum_256(acc, red);
+    if (DET) {
+        const float s1 = TERMS ? block_sum_256(acc_l1, red) : 0.f, s2 = TERMS ? block_sum_256(acc_bd, red) : 0.f;
+        det_loss_tail<TERMS>(s, s1, s2, loss, terms, scratch);
+        return;
+    }
     if (threadIdx.x == 0) atomicAdd(loss, s);
     if (TERMS) {
         const float s1 = block_sum_256(acc_l1, red);
@@ -95,19 +138,38 @@ __global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* _
     }
 }
 
+template <bool TERMS>
+__global__ void spec_loss_kernel(const float* __restrict__ y_hat, const float* __restrict__ y,
+                                 const long long* __restrict__ lengths, const long long* __restrict__ t_log,
+                                 float* __restrict__ grad, float* __restrict__ loss, int B, int T, int D, int r,
+                                 float w, float bw, float eps, int pbin, float pw, float* __restrict__ terms) {
+    spec_loss_body<TERMS, false>(y_hat, y, lengths, t_log, grad, loss, B, T, D, r, w, bw, eps, pbin, pw, terms, nullptr);
+}
+
+template <bool TERMS>
+__global__ void spec_loss_det_kernel(const float* __restrict__ y_hat, const float* __restrict__ y,
+                                     const long long* __restrict__ lengths, const long long* __restrict__ t_log,
+                                     float* __restrict__ grad, float* __restrict__ loss, int B, int T, int D, int r,
+                                     float w, float bw, float eps, int pbin, float pw, float* __restrict__ terms,
+                                     float* __restrict__ scratch) {
+    spec_loss_body<TERMS, true>(y_hat, y, lengths, t_log, grad, loss, B, T, D, r, w, bw, eps, pbin, pw, terms, scratch);
+}
+
 // done BCE (mean) + guided attention (mean of attn*W):
 //   done_hat, done (n_done);  attn (A, B, Td, Ts), in_len / dec_len int64 [B];  grads written in full.
 // ext (int64 [2] in device memory, or null): logical (decoder steps, text positions) of a batch padded to a larger
 // bucket -- done_hat is then (B, Td); steps >= ext[0] and text positions >= ext[1] are left out of both means and
 // their gradient is written as 0.
 // TERMS: also add the done BCE to terms[0] and the guided-attention term to terms[1].
-template <bool TERMS>
-__global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float* __restrict__ done,
-                                float* __restrict__ d_done, long long n_done, const float* __restrict__ attn,
-                                float* __restrict__ d_attn, const long long* __restrict__ in_len,
-                                const long long* __restrict__ dec_len, const long long* __restrict__ ext, int A,
-                                int B, int Td, int Ts, float sigma, int use_attn, float* __restrict__ loss,
-                                float* __restrict__ terms) {
+template <bool TERMS, bool DET>
+__device__ __forceinline__ void aux_loss_body(const float* __restrict__ done_hat, const float* __restrict__ done,
+                                              float* __restrict__ d_done, long long n_done,
+                                              const float* __restrict__ attn, float* __restrict__ d_attn,
+                                              const long long* __restrict__ in_len,
+                                              const long long* __restrict__ dec_len, const long long* __restrict__ ext,
+                                              int A, int B, int Td, int Ts, float sigma, int use_attn,
+                                              float* __restrict__ loss, float* __restrict__ terms,
+                                              float* __restrict__ scratch) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float red[8];
     float acc = 0.f, acc_done = 0.f, acc_attn = 0.f;
@@ -145,6 +207,11 @@ __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float*
         for (long long i = start; i < n_attn; i += stride) d_attn[i] = 0.f;
     }
     const float s = block_sum_256(acc, red);
+    if (DET) {
+        const float s1 = TERMS ? block_sum_256(acc_done, red) : 0.f, s2 = TERMS ? block_sum_256(acc_attn, red) : 0.f;
+        det_loss_tail<TERMS>(s, s1, s2, loss, terms, scratch);
+        return;
+    }
     if (threadIdx.x == 0) atomicAdd(loss, s);
     if (TERMS) {
         const float s1 = block_sum_256(acc_done, red);
@@ -152,6 +219,28 @@ __global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float*
         const float s2 = block_sum_256(acc_attn, red);
         if (threadIdx.x == 0) atomicAdd(&terms[1], s2);
     }
+}
+
+template <bool TERMS>
+__global__ void aux_loss_kernel(const float* __restrict__ done_hat, const float* __restrict__ done,
+                                float* __restrict__ d_done, long long n_done, const float* __restrict__ attn,
+                                float* __restrict__ d_attn, const long long* __restrict__ in_len,
+                                const long long* __restrict__ dec_len, const long long* __restrict__ ext, int A,
+                                int B, int Td, int Ts, float sigma, int use_attn, float* __restrict__ loss,
+                                float* __restrict__ terms) {
+    aux_loss_body<TERMS, false>(done_hat, done, d_done, n_done, attn, d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma,
+                                use_attn, loss, terms, nullptr);
+}
+
+template <bool TERMS>
+__global__ void aux_loss_det_kernel(const float* __restrict__ done_hat, const float* __restrict__ done,
+                                    float* __restrict__ d_done, long long n_done, const float* __restrict__ attn,
+                                    float* __restrict__ d_attn, const long long* __restrict__ in_len,
+                                    const long long* __restrict__ dec_len, const long long* __restrict__ ext, int A,
+                                    int B, int Td, int Ts, float sigma, int use_attn, float* __restrict__ loss,
+                                    float* __restrict__ terms, float* __restrict__ scratch) {
+    aux_loss_body<TERMS, true>(done_hat, done, d_done, n_done, attn, d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma,
+                               use_attn, loss, terms, scratch);
 }
 
 }  // namespace dv3
@@ -220,6 +309,47 @@ int dv3_aux_loss_ext(const float* done_hat, const float* done, float* d_done, co
     DV3_REQUIRE(ext != nullptr, "aux_loss_ext: ext is NULL");
     return dv3_aux_loss_terms(done_hat, done, d_done, (long long)B * Td, attn, d_attn, in_len, dec_len, ext, A, B, Td,
                               Ts, sigma, use_attn, loss, nullptr, stream);
+}
+
+// ---- deterministic forms (see det_loss_tail): the same grids, arithmetic and gradients; t_log / ext / terms nullable, so
+// each covers the plain, _ext and _terms forms of its atomic twin.  scratch: dv3_loss_det_scratch_floats() floats.
+int dv3_loss_det_scratch_floats(void) { return LOSS_DET_SCRATCH; }
+
+int dv3_spec_loss_det(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
+                      float* grad, float* loss, float* terms, float* scratch, int B, int T, int D, int r,
+                      float masked_loss_weight, float binary_divergence_weight, int priority_bin,
+                      float priority_weight, void* stream) {
+    DV3_REQUIRE(T > r && r >= 0, "spec_loss_det: need T > r");
+    DV3_REQUIRE(priority_bin >= 0 && priority_bin <= D && priority_weight >= 0.f && priority_weight <= 1.f,
+                "spec_loss_det: priority_bin=%d (D=%d) priority_weight=%g out of range", priority_bin, D,
+                priority_weight);
+    DV3_REQUIRE(scratch != nullptr, "spec_loss_det: scratch buffer required");
+    long long blocks = ((long long)B * T * D + 255) / 256;
+    if (blocks > LOSS_MAX_BLOCKS) blocks = LOSS_MAX_BLOCKS;
+    if (terms)
+        launch_k(spec_loss_det_kernel<true>, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, t_log,
+                 grad, loss, B, T, D, r, masked_loss_weight, binary_divergence_weight, 1e-8f, priority_bin,
+                 priority_weight, terms, scratch);
+    else
+        launch_k(spec_loss_det_kernel<false>, (int)blocks, 256, 0, (cudaStream_t)stream, y_hat, y, lengths, t_log,
+                 grad, loss, B, T, D, r, masked_loss_weight, binary_divergence_weight, 1e-8f, priority_bin,
+                 priority_weight, terms, scratch);
+    return check_launch("spec_loss_det");
+}
+
+int dv3_aux_loss_det(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
+                     float* d_attn, const long long* in_len, const long long* dec_len, const long long* ext, int A,
+                     int B, int Td, int Ts, float sigma, int use_attn, float* loss, float* terms, float* scratch,
+                     void* stream) {
+    DV3_REQUIRE(ext == nullptr || n_done == (long long)B * Td, "aux_loss_det: with extents done_hat must be (B, Td)");
+    DV3_REQUIRE(scratch != nullptr, "aux_loss_det: scratch buffer required");
+    if (terms)
+        launch_k(aux_loss_det_kernel<true>, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done,
+                 attn, d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma, use_attn, loss, terms, scratch);
+    else
+        launch_k(aux_loss_det_kernel<false>, 132 * 2, 256, 0, (cudaStream_t)stream, done_hat, done, d_done, n_done,
+                 attn, d_attn, in_len, dec_len, ext, A, B, Td, Ts, sigma, use_attn, loss, terms, scratch);
+    return check_launch("aux_loss_det");
 }
 
 }  // extern "C"

@@ -55,7 +55,10 @@ __device__ __forceinline__ void pack_planes(float x0, float x1, uint32_t& h, uin
 }
 
 // 6 CTAs per SM: holds the gate split (33 KB of shared memory: 6 fit) at 40 registers with the extent mask, no spills.
-template <int KIND, int NPL>
+// DET (deterministic mode, its own instantiations): p.dbias is a scratch [B * gridDim.x][2C | C] instead; every
+// (utterance, 64-frame tile) stores its per-channel sums in its own row -- frames past the extent are already zero in
+// them -- and bias_reduce_kernel (conv.cu) adds the rows to the bias gradient in a fixed order.
+template <int KIND, int NPL, bool DET = false>
 __global__ void __launch_bounds__(256, 6) plane_split_kernel(const __grid_constant__ SplitParams p) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     __shared__ float sa[64][65];
@@ -115,7 +118,13 @@ __global__ void __launch_bounds__(256, 6) plane_split_kernel(const __grid_consta
                 s0 += __shfl_xor_sync(0xffffffffu, s0, o);
                 if (KIND == SPLIT_GATE) s1 += __shfl_xor_sync(0xffffffffu, s1, o);
             }
-            if (q == 0 && c < C) {
+            if (DET) {
+                if (q == 0 && c < C) {
+                    float* row = p.dbias + ((size_t)b * gridDim.x + blockIdx.x) * (KIND == SPLIT_GATE ? 2 * C : C);
+                    row[c] = s0;
+                    if (KIND == SPLIT_GATE) row[C + c] = s1;
+                }
+            } else if (q == 0 && c < C) {
                 atomicAdd(&p.dbias[c], s0);
                 if (KIND == SPLIT_GATE) atomicAdd(&p.dbias[C + c], s1);
             }
@@ -160,6 +169,24 @@ static int launch_split(const SplitParams& p, int npl, void* stream, const char*
     return check_launch(what);
 }
 
+// deterministic bias gradient: partial rows from the split itself (p.dbias = scratch), then the fixed-order reduction
+template <int KIND>
+static int launch_split_det(SplitParams p, int npl, float* dbias, float* scratch, long long scratch_floats,
+                            void* stream, const char* what) {
+    const int nch = KIND == SPLIT_GATE ? 2 * p.C : p.C;
+    const dim3 grid = split_grid(p.B, p.C, p.T);
+    const long long nparts = (long long)p.B * grid.x;
+    if (!dbias || !scratch || scratch_floats < nparts * nch) {
+        set_error("%s: dbias and a scratch of >= %lld floats required", what, nparts * nch);
+        return 1;
+    }
+    p.dbias = scratch;
+    if (npl == 1) launch_k(plane_split_kernel<KIND, 1, true>, grid, dim3(256), 0, (cudaStream_t)stream, p);
+    else launch_k(plane_split_kernel<KIND, 2, true>, grid, dim3(256), 0, (cudaStream_t)stream, p);
+    if (int e = check_launch(what)) return e;
+    return bias_reduce(scratch, (int)nparts, nch, dbias, (cudaStream_t)stream);
+}
+
 }  // namespace dv3
 
 using namespace dv3;
@@ -180,7 +207,8 @@ static int split_input(const float* x, void* btc, int npl, void* bct, int B, int
 
 static int gate_bwd_split(const float* dy, const float* a, const float* s, const float* x, void* btc, int npl,
                           void* bct, float* dbias, int B, int C, int T, int mode, int residual, const long long* tlen,
-                          int tmult, void* stream) {
+                          int tmult, void* stream, bool det = false, float* scratch = nullptr,
+                          long long scratch_floats = 0) {
     DV3_REQUIRE(bct == nullptr, "tc_gate_bwd_split: bct must be NULL");
     DV3_REQUIRE(npl == 1 || npl == 2, "tc_gate_bwd_split: npl must be 1 or 2");
     DV3_REQUIRE(C % 8 == 0 && (mode == 0 || x != nullptr), "tc_gate_bwd_split: C %% 8 != 0 or highway without x");
@@ -188,11 +216,13 @@ static int gate_bwd_split(const float* dy, const float* a, const float* s, const
     SplitParams p = {};
     p.in0 = dy; p.in1 = a; p.in2 = s; p.in3 = x; p.planes = (bf16*)btc; p.dbias = dbias;
     p.B = B; p.C = C; p.T = T; p.pitch = 2 * C; p.mode = mode; p.residual = residual; p.tlen = tlen; p.tmult = tmult;
+    if (det) return launch_split_det<SPLIT_GATE>(p, npl, dbias, scratch, scratch_floats, stream, "tc_gate_bwd_split_det");
     return launch_split<SPLIT_GATE>(p, npl, stream, "tc_gate_bwd_split");
 }
 
 static int grad_split(const float* dy, const float* y, void* btc, int npl, void* bct, float* dbias, int B, int C,
-                      int T, int relu, const long long* tlen, int tmult, void* stream) {
+                      int T, int relu, const long long* tlen, int tmult, void* stream, bool det = false,
+                      float* scratch = nullptr, long long scratch_floats = 0) {
     DV3_REQUIRE(bct == nullptr, "tc_grad_split: bct must be NULL");
     DV3_REQUIRE(npl == 1 || npl == 2, "tc_grad_split: npl must be 1 or 2");
     DV3_REQUIRE(!relu || y != nullptr, "tc_grad_split: ReLU backward needs the forward output");
@@ -200,6 +230,7 @@ static int grad_split(const float* dy, const float* y, void* btc, int npl, void*
     SplitParams p = {};
     p.in0 = dy; p.in1 = y; p.planes = (bf16*)btc; p.dbias = dbias;
     p.B = B; p.C = C; p.T = T; p.pitch = (C + 7) / 8 * 8; p.relu = relu; p.tlen = tlen; p.tmult = tmult;
+    if (det) return launch_split_det<SPLIT_GRAD>(p, npl, dbias, scratch, scratch_floats, stream, "tc_grad_split_det");
     return launch_split<SPLIT_GRAD>(p, npl, stream, "tc_grad_split");
 }
 
@@ -249,6 +280,23 @@ int dv3_tc_gate_bwd_split_npl(const float* dy, const float* a, const float* s, c
 int dv3_tc_grad_split_npl(const float* dy, const float* y, void* btc, int npl, void* bct, float* dbias, int B, int C,
                           int T, int relu, const long long* tlen, int tmult, void* stream) {
     return grad_split(dy, y, btc, npl, bct, dbias, B, C, T, relu, tlen, tmult, stream);
+}
+
+// Deterministic forms of the two calls above (same planes, bit for bit): the per-(utterance, 64-frame tile) channel
+// sums go to scratch (>= dv3_bias_det_scratch_floats(B, 2C | C, T, 1) floats) and are added to dbias in a fixed order by
+// a second launch.  dbias is required.
+int dv3_tc_gate_bwd_split_det(const float* dy, const float* a, const float* s, const float* x, void* btc, int npl,
+                              float* dbias, float* scratch, long long scratch_floats, int B, int C, int T, int mode,
+                              int residual, const long long* tlen, int tmult, void* stream) {
+    return gate_bwd_split(dy, a, s, x, btc, npl, nullptr, dbias, B, C, T, mode, residual, tlen, tmult, stream, true,
+                          scratch, scratch_floats);
+}
+
+int dv3_tc_grad_split_det(const float* dy, const float* y, void* btc, int npl, float* dbias, float* scratch,
+                          long long scratch_floats, int B, int C, int T, int relu, const long long* tlen, int tmult,
+                          void* stream) {
+    return grad_split(dy, y, btc, npl, nullptr, dbias, B, C, T, relu, tlen, tmult, stream, true, scratch,
+                      scratch_floats);
 }
 
 }  // extern "C"

@@ -28,6 +28,22 @@ MODE_GLU, MODE_HIGHWAY = 0, 1
 # A TrainStep records the mode it was built in: its captured graphs hold that mode's kernels and planes.
 conv_math = os.environ.get("DV3_CONV_MATH", "tc")
 
+# Bit-reproducible training (DESIGN.md section 2.10): "0" (default) the training step sums its losses, bias gradients
+# and embedding / position-table gradients with float atomics, whose order differs from run to run; "1" every one of
+# those sums is formed in an order fixed by the tensor shapes (the dv3_*_det entry points), so the same build, GPU model,
+# world size, conv_math, graph / eager setting, seed and batches give the same bits.  The autograd Functions read the
+# switch in their forward and keep it for their backward.
+deterministic = os.environ.get("DV3_DETERMINISTIC", "0")
+
+
+def is_deterministic():
+    """ops.deterministic as a bool ("0" / "1", or a bool); an unknown value raises."""
+    if deterministic in ("0", 0, False):
+        return False
+    if deterministic in ("1", 1, True):
+        return True
+    raise Dv3Error("unknown ops.deterministic %r (DV3_DETERMINISTIC is \"0\" or \"1\")" % (deterministic,))
+
 
 # ----------------------------------------------------------------------------------------------
 # plumbing
@@ -117,6 +133,49 @@ class DropoutState:
 
 
 rng = DropoutState()
+
+
+class DetScratch:
+    """Device scratch of the deterministic kernels: the partial-sum rows of the bias gradients (reused by every layer --
+    a layer's reduction is ordered before the next layer's partials on the stream) and the block partials + ticket of
+    the loss kernels.  Buffers grow on demand but never during a CUDA-graph capture: a captured launch keeps the address
+    it was given, so a TrainStep sizes its scratch in the eager warm-up passes that precede every capture, and outgrown
+    buffers stay alive for the graphs that hold them."""
+
+    def __init__(self):
+        self._bias = {}       # device -> list of buffers, the last one current
+        self._loss = {}
+
+    @staticmethod
+    def _growable(what):
+        if torch.cuda.is_current_stream_capturing():
+            raise Dv3Error("deterministic mode: %s scratch must exist before a CUDA-graph capture (run the step "
+                           "eagerly once, as TrainStep's warm-up does)" % what)
+
+    def bias(self, floats, device):
+        bufs = self._bias.setdefault(device, [])
+        if not bufs or bufs[-1].numel() < floats:
+            self._growable("bias-gradient")
+            bufs.append(torch.empty(max(int(floats), 1 << 18), device=device, dtype=torch.float32))
+        return bufs[-1]
+
+    def loss(self, device):
+        if device not in self._loss:
+            self._growable("loss")
+            self._loss[device] = torch.zeros(lib.raw("dv3_loss_det_scratch_floats")(), device=device)
+        return self._loss[device]
+
+
+# the scratch of Functions called outside a TrainStep; a TrainStep installs its own around its passes
+det_scratch = DetScratch()
+
+
+def _bias_scratch(B, nch, T, tiled, device):
+    """-> (pointer, floats) of the partial rows a deterministic bias-gradient call needs."""
+    lib.load()
+    fn = lib.raw("dv3_bias_det_scratch_floats")
+    buf = det_scratch.bias(fn(B, nch, T, int(tiled)), device)
+    return _p(buf), buf.numel()
 
 
 def forward_scope(fn):
@@ -245,6 +304,7 @@ class _ConvBlockFn(torch.autograd.Function):
             ctx.save_for_backward(x, v, g, a, s, w_b, inv)
             ctx.cfg = (k, dilation, causal, mode, residual, p, salt, spk is not None, x.device)
             ctx.seed_t = seed_t
+            ctx.det = is_deterministic()
         return y
 
     @staticmethod
@@ -256,8 +316,12 @@ class _ConvBlockFn(torch.autograd.Function):
         B, C, T = x.shape
         dab = torch.empty(B, 2 * C, T, device=dev, dtype=torch.float32)
         dbias = torch.zeros(2 * C, device=dev, dtype=torch.float32)
-        lib.call("dv3_convblock_gate_bwd", _p(dy), _p(a), _p(s), _p(x), _p(dab), _p(dbias), B, C, T, mode,
-                 int(residual), _stream())
+        if ctx.det:
+            lib.call("dv3_convblock_gate_bwd_det", _p(dy), _p(a), _p(s), _p(x), _p(dab), _p(dbias),
+                     *_bias_scratch(B, 2 * C, T, False, dev), B, C, T, mode, int(residual), _stream())
+        else:
+            lib.call("dv3_convblock_gate_bwd", _p(dy), _p(a), _p(s), _p(x), _p(dab), _p(dbias), B, C, T, mode,
+                     int(residual), _stream())
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
@@ -413,6 +477,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
             ctx.bank = bank
             ctx.extent = extent
             ctx.npl = npl
+            ctx.det = is_deterministic()
         return y
 
     @staticmethod
@@ -427,8 +492,12 @@ class _ConvBlockTCFn(torch.autograd.Function):
         wg = _TCWeightGrad(ctx, v, g)
         # the gradient past the extent is taken as 0 (see ops.extent_frames)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
-        lib.call("dv3_tc_gate_bwd_split_npl", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), npl, None, _p(wg.dbias), B, C,
-                 T, mode, int(residual), ext_p, ext_m, _stream())
+        if ctx.det:
+            lib.call("dv3_tc_gate_bwd_split_det", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), npl, _p(wg.dbias),
+                     *_bias_scratch(B, 2 * C, T, True, dev), B, C, T, mode, int(residual), ext_p, ext_m, _stream())
+        else:
+            lib.call("dv3_tc_gate_bwd_split_npl", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), npl, None, _p(wg.dbias), B,
+                     C, T, mode, int(residual), ext_p, ext_m, _stream())
         wg.start(d_btc, x_wg, inv, B, T, dilation, causal, npl)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -480,6 +549,7 @@ class _Conv1dTCFn(torch.autograd.Function):
             ctx.bank = bank
             ctx.extent = extent
             ctx.npl = npl
+            ctx.det = is_deterministic()
         return y
 
     @staticmethod
@@ -492,8 +562,12 @@ class _Conv1dTCFn(torch.autograd.Function):
         g_btc = torch.empty(npl, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
         wg = _TCWeightGrad(ctx, v, g)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
-        lib.call("dv3_tc_grad_split_npl", _p(dy), _p(y), _p(g_btc), npl, None, _p(wg.dbias), B, Cout, T, int(relu),
-                 ext_p, ext_m, _stream())
+        if ctx.det:
+            lib.call("dv3_tc_grad_split_det", _p(dy), _p(y), _p(g_btc), npl, _p(wg.dbias),
+                     *_bias_scratch(B, Cout, T, True, dev), B, Cout, T, int(relu), ext_p, ext_m, _stream())
+        else:
+            lib.call("dv3_tc_grad_split_npl", _p(dy), _p(y), _p(g_btc), npl, None, _p(wg.dbias), B, Cout, T,
+                     int(relu), ext_p, ext_m, _stream())
         wg.start(g_btc, x_wg, inv, B, T, dilation, causal, npl)
         dx = None
         if ctx.needs_input_grad[0]:
@@ -535,6 +609,7 @@ class _ConvT2TCFn(torch.autograd.Function):
         ctx.cfg = (B, Cin, Cout, T)
         ctx.extent = extent                 # a 2x upsampler mixes no frames: only its incoming gradient is masked
         ctx.npl = npl
+        ctx.det = is_deterministic()
         return y
 
     @staticmethod
@@ -550,8 +625,12 @@ class _ConvT2TCFn(torch.autograd.Function):
         g_btc = torch.empty(npl, B, T, K2p, device=dev, dtype=bf)
         db2 = torch.zeros(2 * Cout, device=dev)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)     # dyp is in the input's time units
-        lib.call("dv3_tc_grad_split_npl", _p(dyp), None, _p(g_btc), npl, None, _p(db2), B, 2 * Cout, T, 0, ext_p,
-                 ext_m, _stream())
+        if ctx.det:
+            lib.call("dv3_tc_grad_split_det", _p(dyp), None, _p(g_btc), npl, _p(db2),
+                     *_bias_scratch(B, 2 * Cout, T, True, dev), B, 2 * Cout, T, 0, ext_p, ext_m, _stream())
+        else:
+            lib.call("dv3_tc_grad_split_npl", _p(dyp), None, _p(g_btc), npl, None, _p(db2), B, 2 * Cout, T, 0, ext_p,
+                     ext_m, _stream())
         dbias = db2[:Cout] + db2[Cout:]
         dx = None
         if ctx.needs_input_grad[0]:
@@ -644,6 +723,7 @@ class _Conv1dFn(torch.autograd.Function):
         if any(ctx.needs_input_grad):
             ctx.save_for_backward(x, v, g, w_b, inv, y if relu else None)
             ctx.cfg = (k, dilation, causal, relu)
+            ctx.det = is_deterministic()
         return y
 
     @staticmethod
@@ -655,7 +735,11 @@ class _Conv1dFn(torch.autograd.Function):
         Cout = v.shape[0]
         dbias = torch.zeros(Cout, device=x.device, dtype=torch.float32)
         dyr = torch.empty_like(dy) if relu else dy
-        lib.call("dv3_bias_act_bwd", _p(dy), _p(y), _p(dyr), _p(dbias), B, Cout, T, int(relu), _stream())
+        if ctx.det:
+            lib.call("dv3_bias_act_bwd_det", _p(dy), _p(y), _p(dyr), _p(dbias),
+                     *_bias_scratch(B, Cout, T, False, x.device), B, Cout, T, int(relu), _stream())
+        else:
+            lib.call("dv3_bias_act_bwd", _p(dy), _p(y), _p(dyr), _p(dbias), B, Cout, T, int(relu), _stream())
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
@@ -739,6 +823,7 @@ class _EmbeddingFn(torch.autograd.Function):
                  _stream())
         ctx.save_for_backward(ids)
         ctx.cfg = (V, D, -1 if padding_idx is None else int(padding_idx))
+        ctx.det = is_deterministic()
         return out
 
     @staticmethod
@@ -747,7 +832,8 @@ class _EmbeddingFn(torch.autograd.Function):
         V, D, pad = ctx.cfg
         dy = _c(dy)
         dtable = torch.zeros(V, D, device=dy.device, dtype=torch.float32)
-        lib.call("dv3_embedding_bwd", _p(ids), _p(dy), _p(dtable), ids.numel(), D, V, pad, _stream())
+        lib.call("dv3_embedding_bwd_det" if ctx.det else "dv3_embedding_bwd", _p(ids), _p(dy), _p(dtable), ids.numel(),
+                 D, V, pad, _stream())
         return None, dtable, None
 
 
@@ -767,6 +853,7 @@ class _SinusoidFn(torch.autograd.Function):
         lib.call("dv3_sinusoid_fwd", _p(pos), _p(table), _p(w), w.numel(), _p(out), B, T, D, P,
                  _p(_err_flag(table.device)), _stream())
         ctx.save_for_backward(pos, table, w)
+        ctx.det = is_deterministic()
         return out
 
     @staticmethod
@@ -778,8 +865,8 @@ class _SinusoidFn(torch.autograd.Function):
         dtable = torch.zeros_like(table) if ctx.needs_input_grad[1] else None
         dw = torch.zeros_like(w) if ctx.needs_input_grad[2] else None
         if dtable is not None or dw is not None:
-            lib.call("dv3_sinusoid_bwd", _p(pos), _p(table), _p(w), w.numel(), _p(dy), _p(dtable), _p(dw), B, T,
-                     D, P, _stream())
+            lib.call("dv3_sinusoid_bwd_det" if ctx.det else "dv3_sinusoid_bwd", _p(pos), _p(table), _p(w), w.numel(),
+                     _p(dy), _p(dtable), _p(dw), B, T, D, P, _stream())
         return None, dtable, dw
 
 
@@ -838,6 +925,7 @@ class _ConvT2Fn(torch.autograd.Function):
         y = torch.empty(B, Cout, 2 * T, device=dev, dtype=torch.float32)
         lib.call("dv3_interleave2", _p(yp), _p(y), B, Cout, T, 0, _stream())
         ctx.save_for_backward(x, v, g, w_b, inv)
+        ctx.det = is_deterministic()
         return y
 
     @staticmethod
@@ -850,7 +938,11 @@ class _ConvT2Fn(torch.autograd.Function):
         dyp = torch.empty(B, 2 * Cout, T, device=dev, dtype=torch.float32)
         lib.call("dv3_interleave2", _p(dy), _p(dyp), B, Cout, T, 1, _stream())
         db2 = torch.zeros(2 * Cout, device=dev, dtype=torch.float32)
-        lib.call("dv3_bias_act_bwd", _p(dyp), None, None, _p(db2), B, 2 * Cout, T, 0, _stream())
+        if ctx.det:
+            lib.call("dv3_bias_act_bwd_det", _p(dyp), None, None, _p(db2), *_bias_scratch(B, 2 * Cout, T, False, dev),
+                     B, 2 * Cout, T, 0, _stream())
+        else:
+            lib.call("dv3_bias_act_bwd", _p(dyp), None, None, _p(db2), B, 2 * Cout, T, 0, _stream())
         dbias = db2[:Cout] + db2[Cout:]
         dx = None
         if ctx.needs_input_grad[0]:

@@ -135,11 +135,12 @@ def training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, b
 class _FusedLossFn(torch.autograd.Function):
     """All four training losses and their gradients in 3 kernel launches (csrc/loss.cu).  Predictions passed as None
     (a seq2seq-only or postnet-only step) leave their loss out and get no launch.  terms: optional float
-    (ops.TERM_COUNT,) device block the kernels add the per-term losses to."""
+    (ops.TERM_COUNT,) device block the kernels add the per-term losses to.  det: the fixed-order kernels
+    (dv3_spec_loss_det / dv3_aux_loss_det) with the loss scratch of ops.det_scratch."""
 
     @staticmethod
     def forward(ctx, mel_out, lin_out, attn, done_hat, mel, y, done, target_lengths, input_lengths, r,
-                downsample_step, w, bw, sigma, use_attn, pbin, pw, ext, terms):
+                downsample_step, w, bw, sigma, use_attn, pbin, pw, ext, terms, det):
         dev = target_lengths.device
         vp = lambda t: ctypes.c_void_p(t.data_ptr())
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
@@ -149,46 +150,51 @@ class _FusedLossFn(torch.autograd.Function):
         loss = torch.zeros(1, device=dev)
         dec_len = (target_lengths // (r * downsample_step)).contiguous()
         g_mel = g_lin = g_attn = g_done = None
+        spec, aux, scratch = "dv3_spec_loss_terms", "dv3_aux_loss_terms", ()
+        if det:
+            spec, aux, scratch = "dv3_spec_loss_det", "dv3_aux_loss_det", (vp(ops.det_scratch.loss(dev)),)
         if mel_out is not None:
             mel_out = mel_out.contiguous()
             g_mel = torch.empty_like(mel_out)
             B, Td, Dm = mel_out.shape
-            lib.call("dv3_spec_loss_terms", vp(mel_out), vp(mel.contiguous()), vp(dec_len), at(ops.EXT_MEL), vp(g_mel),
-                     vp(loss), tp(ops.TERM_MEL_L1), B, Td, Dm, r, float(w), float(bw), 0, 0.0, st)
+            lib.call(spec, vp(mel_out), vp(mel.contiguous()), vp(dec_len), at(ops.EXT_MEL), vp(g_mel),
+                     vp(loss), tp(ops.TERM_MEL_L1), *scratch, B, Td, Dm, r, float(w), float(bw), 0, 0.0, st)
         if lin_out is not None:
             lin_out = lin_out.contiguous()
             g_lin = torch.empty_like(lin_out)
             B, Tl, Dl = lin_out.shape
             lin_len = target_lengths.contiguous() if downsample_step > 1 else dec_len
-            lib.call("dv3_spec_loss_terms", vp(lin_out), vp(y.contiguous()), vp(lin_len),
+            lib.call(spec, vp(lin_out), vp(y.contiguous()), vp(lin_len),
                      at(ops.EXT_LIN if downsample_step > 1 else ops.EXT_MEL), vp(g_lin), vp(loss), tp(ops.TERM_LIN_L1),
-                     B, Tl, Dl, r, float(w), float(bw), int(pbin), float(pw), st)
+                     *scratch, B, Tl, Dl, r, float(w), float(bw), int(pbin), float(pw), st)
         if done_hat is not None:
             attn, done_hat = attn.contiguous(), done_hat.contiguous()
             g_attn, g_done = torch.empty_like(attn), torch.empty_like(done_hat)
             A, B, Td, Ts = attn.shape
             dec_len_attn = (target_lengths // r // downsample_step).contiguous()
             assert ext is None or (done_hat.numel() == B * Td and ops.EXT_TEXT == ops.EXT_DEC + 1)
-            lib.call("dv3_aux_loss_terms", vp(done_hat), vp(done.contiguous()), vp(g_done), done_hat.numel(), vp(attn),
+            lib.call(aux, vp(done_hat), vp(done.contiguous()), vp(g_done), done_hat.numel(), vp(attn),
                      vp(g_attn), vp(input_lengths.contiguous()), vp(dec_len_attn), at(ops.EXT_DEC), A, B, Td, Ts,
-                     float(sigma), int(use_attn), vp(loss), tp(ops.TERM_DONE), st)
+                     float(sigma), int(use_attn), vp(loss), tp(ops.TERM_DONE), *scratch, st)
         ctx.save_for_backward(g_mel, g_lin, g_attn, g_done)
         return loss[0]
 
     @staticmethod
     def backward(ctx, gout):
-        return tuple(None if g is None else g * gout for g in ctx.saved_tensors) + (None,) * 15
+        return tuple(None if g is None else g * gout for g in ctx.saved_tensors) + (None,) * 16
 
 
 def fused_training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=0.5, binary_divergence_weight=0.1,
                         guided_attention_sigma=0.2, use_guided_attention=True, priority_freq=3000,
-                        priority_freq_weight=0.0, sample_rate=22050, terms=None):
+                        priority_freq_weight=0.0, sample_rate=22050, terms=None, deterministic=None):
     """Same value and gradients as ``training_loss`` (reference train.py:665-740), computed by csrc/loss.cu.  A batch
     padded to a bucket (``data.pad_to_bucket``: it carries ``extents``) gives the loss and gradients of the unpadded
     batch: the padding leaves every mean and its gradient is 0.  terms: a zeroed float (ops.TERM_COUNT,) CUDA tensor
     that receives the per-term losses (L1 and binary-divergence parts of the mel and linear losses, done BCE, guided
-    attention) without a launch of their own."""
+    attention) without a launch of their own.  deterministic (None: ``ops.deterministic``): sum the losses in a fixed
+    order (DESIGN.md section 2.10); the gradients are the same bits either way."""
     mel_out, lin_out, attn, done_hat = outs
+    det = ops.is_deterministic() if deterministic is None else bool(deterministic)
     ext = batch.get("extents")
     if ext is not None and not (ext.is_cuda and ext.dtype == torch.int64 and ext.shape == (4,) and ext.is_contiguous()):
         raise ValueError("batch['extents'] must be a contiguous int64 (4,) CUDA tensor")
@@ -198,7 +204,7 @@ def fused_training_loss(outs, batch, r=1, downsample_step=4, masked_loss_weight=
     return _FusedLossFn.apply(mel_out, lin_out, attn, done_hat, batch["mel"], batch.get("y"), batch.get("done"),
                               batch["target_lengths"], batch.get("input_lengths_dev"), r, downsample_step,
                               masked_loss_weight, binary_divergence_weight, guided_attention_sigma,
-                              use_guided_attention, pbin, priority_freq_weight, ext, terms)
+                              use_guided_attention, pbin, priority_freq_weight, ext, terms, det)
 
 
 class ParameterArena:
@@ -483,15 +489,21 @@ class TrainStep:
     trained part; the other part's parameters keep their bits.  weight_decay / amsgrad: torch.optim.Adam's.
 
     The step runs in the ``ops.conv_math`` mode current at construction ("tc", "tc1" or "fp32"): its weight bank and
-    captured graphs hold that mode's kernels and operand planes, so ``step()`` under another mode raises ValueError."""
+    captured graphs hold that mode's kernels and operand planes, so ``step()`` under another mode raises ValueError.
+
+    deterministic (None: ``ops.deterministic`` at construction): every step runs the fixed-order kernels of DESIGN.md
+    section 2.10 whatever ``ops.deterministic`` says later, eager or captured; the step owns their scratch, which is
+    allocated by the eager passes before a capture and so lies outside every graph pool."""
 
     def __init__(self, model, init_lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1, r=1, downsample_step=4,
                  masked_loss_weight=0.5, binary_divergence_weight=0.1, guided_attention_sigma=0.2,
                  use_guided_attention=True, priority_freq=3000, priority_freq_weight=0.0, sample_rate=22050,
                  lr_schedule=noam_learning_rate_decay, use_graph=False, fused_loss=True, weight_bank=None,
-                 train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False):
+                 train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False, deterministic=None):
         check_train_mode(model, train_seq2seq, train_postnet)
         self.math = ops.math_mode()
+        self.deterministic = ops.is_deterministic() if deterministic is None else bool(deterministic)
+        self._det_scratch = ops.DetScratch() if self.deterministic else None
         self.model = model
         self.train_seq2seq, self.train_postnet = bool(train_seq2seq), bool(train_postnet)
         # the module whose parameters are trained and checkpointed (reference save_checkpoint, train.py:787-808)
@@ -573,11 +585,16 @@ class TrainStep:
         ops.weight_bank = self.bank   # weight norm of all layers: 2 launches up front, 1 per bucket in the backward
         ops.grad_boundary_cb = self._bucket_ready if self.overlap_comm else None
         self._reduced = set()
+        det_outer = (ops.deterministic, ops.det_scratch)
+        ops.deterministic = self.deterministic
+        if self.deterministic:
+            ops.det_scratch = self._det_scratch
         try:
             if self.bank is not None:
                 self.bank.begin_step()
             return self._forward_backward_inner(batch)
         finally:
+            ops.deterministic, ops.det_scratch = det_outer
             ops.grad_sink = False
             ops.weight_bank = None
             ops.grad_boundary_cb = None

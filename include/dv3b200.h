@@ -399,6 +399,45 @@ int dv3_aux_loss_terms(const float* done_hat, const float* done, float* d_done, 
                        float* d_attn, const long long* in_len, const long long* dec_len, const long long* ext, int A,
                        int B, int Td, int Ts, float sigma, int use_attn, float* loss, float* terms, void* stream);
 
+/* ---- deterministic mode (ops.deterministic, DESIGN.md section 2.10): twins of the five entry-point families whose
+ * kernels accumulate floats with cross-block atomics.  Each gives the same values with every sum formed in an order
+ * fixed by the tensor shapes, so two runs give identical bits.  Like their twins they ADD to loss / terms / dbias /
+ * dtable.  The caller owns the scratch; no kernel waits for another block (the last block to finish does the tail, or
+ * a second small launch does).
+ *   losses: every block stores its partial sums in `scratch` (dv3_loss_det_scratch_floats() floats, zero-filled once
+ *     by the caller; the last word is a ticket the kernel leaves at zero); the block that draws the last ticket adds
+ *     them in block order.  t_log / ext / terms are nullable: one call for the plain, _ext and _terms forms.
+ *   bias gradients: partial sums per utterance (exact-fp32 kernels) or per (utterance, 64-frame tile) (tensor-core
+ *     operand splits; frames past tmult * tlen[0] stay out) go to scratch[partial][channel], needing
+ *     dv3_bias_det_scratch_floats(B, channels, T, tiled) floats (channels = 2C for the gated forms; tiled = 1 for the
+ *     tensor-core splits); a second launch adds them to dbias in partial order.  dbias is required.
+ *   table gradients: one CTA per table row gathers its tokens in index order; D <= 1024. */
+int dv3_loss_det_scratch_floats(void);
+int dv3_spec_loss_det(const float* y_hat, const float* y, const long long* lengths, const long long* t_log,
+                      float* grad, float* loss, float* terms, float* scratch, int B, int T, int D, int r,
+                      float masked_loss_weight, float binary_divergence_weight, int priority_bin,
+                      float priority_weight, void* stream);
+int dv3_aux_loss_det(const float* done_hat, const float* done, float* d_done, long long n_done, const float* attn,
+                     float* d_attn, const long long* in_len, const long long* dec_len, const long long* ext, int A,
+                     int B, int Td, int Ts, float sigma, int use_attn, float* loss, float* terms, float* scratch,
+                     void* stream);
+long long dv3_bias_det_scratch_floats(int B, int nch, int T, int tiled);
+int dv3_convblock_gate_bwd_det(const float* dy, const float* a, const float* s, const float* x, float* dab,
+                               float* dbias, float* scratch, long long scratch_floats, int B, int C, int T, int mode,
+                               int residual, void* stream);
+int dv3_bias_act_bwd_det(const float* dy, const float* y, float* dyr, float* dbias, float* scratch,
+                         long long scratch_floats, int B, int C, int T, int relu, void* stream);
+int dv3_tc_gate_bwd_split_det(const float* dy, const float* a, const float* s, const float* x, void* btc, int npl,
+                              float* dbias, float* scratch, long long scratch_floats, int B, int C, int T, int mode,
+                              int residual, const long long* tlen, int tmult, void* stream);
+int dv3_tc_grad_split_det(const float* dy, const float* y, void* btc, int npl, float* dbias, float* scratch,
+                          long long scratch_floats, int B, int C, int T, int relu, const long long* tlen, int tmult,
+                          void* stream);
+int dv3_embedding_bwd_det(const long long* ids, const float* dy, float* dtable, int N, int D, int V,
+                          long long padding_idx, void* stream);
+int dv3_sinusoid_bwd_det(const long long* pos, const float* table, const float* w, int nw, const float* dy,
+                         float* dtable, float* dw, int B, int T, int D, int P, void* stream);
+
 /* ---- incremental (autoregressive) decoding: reference conv.py:17-46, deepvoice3.py:367-485, nyanko.py:250-338 ----
  * All loop state lives in device memory so that one decoder step is the same launch sequence every time (CUDA-graph
  * replay): *t_ptr is the step counter; every row pointer advances by a per-step stride: row b of step t of operand
