@@ -8,8 +8,13 @@ transform on a training batch's waveforms and writes the padded, decimated targe
 ``inv_spectrogram`` (reference audio.py:37-43) recovers the phase on the same STFT frame with Griffin-Lim (the default,
 csrc/istft.cu) or with Local Weighted Sums (``method="lws"``, csrc/lws.cu), the algorithm of the reference's
 ``lws.run_lws``.  The ``lws`` package is an un-vendored dependency whose source is absent, so parity with it is unpinned.
+
+The STFT frame is ``hparams.fft_size`` / ``hparams.hop_size``, as in the reference.  ``check_geometry`` decides which
+frames are supported: at 1024 / 256 (every reference preset) the specialised kernels run; any other supported frame
+runs the general kernels of csrc/stft_any.cu and csrc/lws_any.cu (DESIGN.md, "Other STFT geometries").
 """
 import ctypes
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -38,6 +43,64 @@ class _HP:
 
 hparams = _HP()
 _basis_cache = {}
+
+Geometry = namedtuple("Geometry", "n_fft hop bins overlap default")
+
+
+def check_geometry(mel=True):
+    """The STFT frame of ``hparams`` -> Geometry(n_fft, hop, bins = n_fft // 2 + 1, overlap = n_fft // hop, default),
+    or Dv3Error naming the rule it breaks.  Supported: n_fft even, 256 <= n_fft <= 4096, n_fft / 2 with no prime factor
+    above 5 (the length of the complex transform after real packing: radix-2/3/4/5 passes); hop divides n_fft with
+    n_fft / hop in [2, 8] -- an integer overlap, the only case where the squared windows sqrt(hann * 2 hop / n_fft) sum
+    to exactly 1, so that the inverse STFT can use the analysis window as its synthesis window.  ``mel``: also the
+    filterbank rules of the forward path (num_mels <= 128, fmax <= sample_rate / 2).  Host values only; every audio entry
+    point calls it before anything is allocated or launched.  ``default`` (1024 / 256) selects the specialised kernels."""
+    hp = hparams
+    N, R = hp.fft_size, hp.hop_size
+    if int(N) != N or int(R) != R:
+        raise Dv3Error("fft_size and hop_size must be integers, got %r / %r" % (N, R))
+    N, R = int(N), int(R)
+    if N % 2 or not 256 <= N <= 4096:
+        raise Dv3Error("fft_size must be even and lie in [256, 4096], got %d" % N)
+    m = N // 2
+    for p in (2, 3, 5):
+        while m % p == 0:
+            m //= p
+    if m != 1:
+        raise Dv3Error("fft_size / 2 = %d has a prime factor above 5 (the FFT has radix-2/3/4/5 passes only)" % (N // 2))
+    if R < 1 or N % R or not 2 <= N // R <= 8:
+        raise Dv3Error("hop_size must divide fft_size with fft_size / hop_size in [2, 8] (an integer overlap: only then "
+                       "do the squared windows sum to 1), got %d / %d" % (N, R))
+    if mel:
+        if not 0 <= hp.num_mels <= 128:
+            raise Dv3Error("num_mels must lie in [0, 128], got %r" % (hp.num_mels,))
+        if hp.fmax is not None and hp.fmax > hp.sample_rate / 2:
+            raise Dv3Error("fmax %r lies above the Nyquist frequency %r" % (hp.fmax, hp.sample_rate / 2))
+    return Geometry(N, R, N // 2 + 1, N // R, (N, R) == (1024, 256))
+
+
+_table_cache = {}
+
+
+def _geometry_table_fp64(N, R):
+    """(window w (N,), twiddles W_M^j (M,), split factors W_N^k (M + 1,)) in fp64, M = N / 2: the tables of
+    csrc/fft_any.cuh.  w(i) = sqrt(hann(i + 1/2) * 2R / N), the lws window."""
+    n = np.arange(N)
+    win = np.sqrt(0.5 * (1.0 - np.cos(2.0 * np.pi * (n + 0.5) / N)) * 2.0 * R / N)
+    M = N // 2
+    tw = np.exp(-2j * np.pi * np.arange(M) / M)
+    sp = np.exp(-2j * np.pi * np.arange(M + 1) / N)
+    return win, tw, sp
+
+
+def _geometry_table(device, N, R):
+    """fft_any.cuh's table for (N, R) on ``device``: 3N + 2 fp32 values, each rounded once from fp64 (cached)."""
+    key = (str(device), N, R)
+    if key not in _table_cache:
+        win, tw, sp = _geometry_table_fp64(N, R)
+        flat = np.concatenate([win, np.stack([tw.real, tw.imag], -1).ravel(), np.stack([sp.real, sp.imag], -1).ravel()])
+        _table_cache[key] = torch.from_numpy(flat.astype(np.float32)).to(device)
+    return _table_cache[key]
 
 
 def _hz_to_mel(f):
@@ -133,7 +196,10 @@ def _linear_to_mel(spectrogram):
 
 
 def num_frames(n_samples):
-    return lib.raw("dv3_stft_num_frames")(int(n_samples))
+    g = check_geometry(mel=False)
+    if g.default:
+        return lib.raw("dv3_stft_num_frames")(int(n_samples))
+    return lib.raw("dv3_stft_num_frames_geom")(int(n_samples), g.n_fft, g.hop)
 
 
 def num_frames_host(n_samples):
@@ -148,7 +214,7 @@ def stft_mel_targets(wav, lengths, T_lin, r, downsample_step, lengths_dev=None):
     ``hparams.rescaling`` is on).
 
     wav: (B, pitch) int16 PCM (read as x / 32768, like ``load_wav``) or fp32 CUDA tensor; lengths: host sequence of
-    the B clip lengths in samples; T_lin: collate's ``max_target_len``.  -> y (B, T_lin, 513) with clip c's frame f at
+    the B clip lengths in samples; T_lin: collate's ``max_target_len``.  -> y (B, T_lin, fft_size // 2 + 1) with clip c's frame f at
     row r + f, and mel (B, T_lin / downsample_step, num_mels) = the padded mel rows 0, ds, 2*ds, ...; every other row
     zero.  Bit-identical to ``collate`` of the preprocessed .npy features.  lengths_dev: the same lengths as an int32
     tensor on wav's device (otherwise they are copied from the host).  No host synchronisation: every check below
@@ -157,8 +223,7 @@ def stft_mel_targets(wav, lengths, T_lin, r, downsample_step, lengths_dev=None):
         raise Dv3Error("stft_mel_targets needs a (B, pitch) CUDA tensor; there is no CPU path")
     if wav.dtype not in (torch.int16, torch.float32):
         raise Dv3Error("stft_mel_targets takes int16 PCM or fp32 waveforms, got %s" % wav.dtype)
-    if hparams.fft_size != 1024 or hparams.hop_size != 256:
-        raise Dv3Error("the fused kernel is built for fft_size=1024, hop_size=256 (every reference preset)")
+    g = check_geometry()
     lengths = [int(n) for n in (lengths.tolist() if torch.is_tensor(lengths) else lengths)]
     B, pitch = wav.shape
     r, ds, T_lin = int(r), int(downsample_step), int(T_lin)
@@ -185,19 +250,24 @@ def stft_mel_targets(wav, lengths, T_lin, r, downsample_step, lengths_dev=None):
     if hparams.rescaling:
         peak = torch.empty(B, device=dev)
         lib.call("dv3_peak_abs_batched", _cp(wav), is16, _cp(lengths_dev), pitch, B, _cp(peak), st)
-    lib.call("dv3_stft_mel_targets", _cp(wav), is16, _cp(lengths_dev), _cp(peak), float(hparams.rescaling_max),
-             _cp(basis), _cp(start), _cp(length), _cp(y), _cp(mel), B, pitch, T_lin, r, ds, hparams.num_mels,
-             float(hparams.preemphasis), float(hparams.min_level_db), float(hparams.ref_level_db), st)
+    if g.default:
+        lib.call("dv3_stft_mel_targets", _cp(wav), is16, _cp(lengths_dev), _cp(peak), float(hparams.rescaling_max),
+                 _cp(basis), _cp(start), _cp(length), _cp(y), _cp(mel), B, pitch, T_lin, r, ds, hparams.num_mels,
+                 float(hparams.preemphasis), float(hparams.min_level_db), float(hparams.ref_level_db), st)
+    else:
+        lib.call("dv3_stft_mel_geom", _cp(wav), is16, _cp(lengths_dev), _cp(peak), float(hparams.rescaling_max),
+                 _cp(_geometry_table(dev, g.n_fft, g.hop)), _cp(basis), _cp(start), _cp(length), _cp(y), _cp(mel), B,
+                 pitch, T_lin, r, ds, hparams.num_mels, g.n_fft, g.hop, float(hparams.preemphasis),
+                 float(hparams.min_level_db), float(hparams.ref_level_db), st)
     return y, mel
 
 
 def stft_mel_batch(wav, lengths=None, want_linear=True, want_mel=True):
     """wav: (nclips, max_len) fp32 CUDA tensor; lengths: int32 CUDA tensor (nclips) or None (= all max_len).
-    -> linear (nclips, max_frames, 513), mel (nclips, max_frames, num_mels) in the stored (T, F) layout."""
+    -> linear (nclips, max_frames, fft_size // 2 + 1), mel (nclips, max_frames, num_mels) in the stored (T, F) layout."""
     if not (torch.is_tensor(wav) and wav.is_cuda and wav.dtype == torch.float32 and wav.dim() == 2):
         raise Dv3Error("stft_mel_batch needs a (nclips, max_len) fp32 CUDA tensor; there is no CPU path")
-    if hparams.fft_size != 1024 or hparams.hop_size != 256:
-        raise Dv3Error("the fused kernel is built for fft_size=1024, hop_size=256 (every reference preset)")
+    g = check_geometry()
     wav = wav.contiguous()
     nclips, max_len = wav.shape
     dev = wav.device
@@ -211,9 +281,16 @@ def stft_mel_batch(wav, lengths=None, want_linear=True, want_mel=True):
 
     def p(t):
         return None if t is None else ctypes.c_void_p(t.data_ptr())
-    lib.call("dv3_stft_mel", p(wav), p(lengths), p(basis), p(start), p(length), p(lin), p(mel), nclips, max_len,
-             max_frames, hparams.num_mels, float(hparams.preemphasis), float(hparams.min_level_db),
-             float(hparams.ref_level_db), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    if g.default:
+        lib.call("dv3_stft_mel", p(wav), p(lengths), p(basis), p(start), p(length), p(lin), p(mel), nclips, max_len,
+                 max_frames, hparams.num_mels, float(hparams.preemphasis), float(hparams.min_level_db),
+                 float(hparams.ref_level_db), st)
+    else:
+        lib.call("dv3_stft_mel_geom", p(wav), 0, p(lengths), None, 1.0, p(_geometry_table(dev, g.n_fft, g.hop)),
+                 p(basis), p(start), p(length), p(lin), p(mel), nclips, max_len, max_frames, 0, 1, hparams.num_mels,
+                 g.n_fft, g.hop, float(hparams.preemphasis), float(hparams.min_level_db), float(hparams.ref_level_db),
+                 st)
     return lin, mel
 
 
@@ -403,20 +480,23 @@ def inv_num_samples(n_frames):
 
 
 def griffin_lim(mag, n_iter=None):
-    """mag: (T, 513) fp32 CUDA tensor of linear magnitudes -> waveform (n,) whose STFT magnitude approximates it.
+    """mag: (T, fft_size // 2 + 1) fp32 CUDA tensor of linear magnitudes -> waveform (n,) whose STFT magnitude
+    approximates it.
     x <- istft(mag * exp(i*angle(stft(x)))), started from the zero-phase inverse; every arrow is one kernel launch
     (the batched kernels with one clip: ``griffin_lim_batch``)."""
     if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 2):
-        raise Dv3Error("griffin_lim needs a (T, 513) fp32 CUDA tensor; there is no CPU path")
+        raise Dv3Error("griffin_lim needs a (T, fft_size // 2 + 1) fp32 CUDA tensor; there is no CPU path")
     return griffin_lim_batch(mag[None], [mag.shape[0]], n_iter)[0]
 
 
 def _ragged_clips(mag, n_frames, name):
-    """Checks of a (nclips, T_max, 513) magnitude batch -> (mag, n_max, frames_d, samples_d, stream)."""
+    """Checks of a (nclips, T_max, K) magnitude batch, K = fft_size // 2 + 1 -> (mag, n_max, frames_d, samples_d,
+    stream, geometry)."""
     if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 3):
-        raise Dv3Error("%s needs a (nclips, T, 513) fp32 CUDA tensor; there is no CPU path" % name)
-    if hparams.fft_size != 1024 or hparams.hop_size != 256 or mag.shape[2] != 513:
-        raise Dv3Error("the inverse kernels are built for fft_size=1024, hop_size=256")
+        raise Dv3Error("%s needs a (nclips, T, fft_size // 2 + 1) fp32 CUDA tensor; there is no CPU path" % name)
+    g = check_geometry(mel=False)
+    if mag.shape[2] != g.bins:
+        raise Dv3Error("%s: magnitudes have %d bins, fft_size %d has %d" % (name, mag.shape[2], g.n_fft, g.bins))
     mag = mag.contiguous()
     nclips, T_max = mag.shape[:2]
     n_frames = [int(t) for t in n_frames]
@@ -428,53 +508,82 @@ def _ragged_clips(mag, n_frames, name):
     dev = mag.device
     frames_d = torch.tensor(n_frames, dtype=torch.int32).to(dev)
     samples_d = torch.tensor(n_samples, dtype=torch.int32).to(dev)
-    return mag, max(n_samples), frames_d, samples_d, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+    return mag, max(n_samples), frames_d, samples_d, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream), g
 
 
 def griffin_lim_batch(mag, n_frames, n_iter=None):
-    """mag: (nclips, T_max, 513) fp32 CUDA tensor, clip c valid for its first n_frames[c] frames -> waveforms
+    """mag: (nclips, T_max, K) fp32 CUDA tensor (K = fft_size // 2 + 1), clip c valid for its first n_frames[c] frames -> waveforms
     (nclips, n_max), clip c valid for its first inv_num_samples(n_frames[c]) samples and zero after them.  Each clip
     comes out bit-identical to ``griffin_lim`` on that clip alone: the kernels read and write only a clip's own frames
     and samples, and the overlap-add is deterministic (csrc/istft.cu)."""
-    mag, n_max, frames_d, samples_d, st = _ragged_clips(mag, n_frames, "griffin_lim_batch")
+    mag, n_max, frames_d, samples_d, st, g = _ragged_clips(mag, n_frames, "griffin_lim_batch")
     nclips, T_max = mag.shape[:2]
     dev = mag.device
-    spec = torch.zeros(nclips, T_max, 513, 2, device=dev)
+    spec = torch.zeros(nclips, T_max, g.bins, 2, device=dev)
     spec[..., 0] = mag                                   # zero phase
     x = torch.zeros(nclips, n_max, device=dev)
-    lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
+    if g.default:
+        def stft(x, spec):
+            lib.call("dv3_stft_complex_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
+                     T_max, nclips, st)
+    else:
+        tab = _geometry_table(dev, g.n_fft, g.hop)
+
+        def stft(x, spec):
+            lib.call("dv3_stft_complex_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
+                     T_max, nclips, _cp(tab), g.n_fft, g.hop, st)
+    _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g)
     for _ in range(hparams.griffin_lim_iters if n_iter is None else n_iter):
-        lib.call("dv3_stft_complex_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
-                 T_max, nclips, st)
+        stft(x, spec)
         x.zero_()
-        lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
+        _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g)
     return x
 
 
-def _lws_weights_fp64():
-    """(7, 11) complex128, [q + 3, d + 5] = beta_q(d) = (1/N) sum_n w(n) w(n - q*hop) exp(-2 pi i d n / N), the sum over
-    the n where both window indices lie in [0, N): the local-weighted-sum weights of csrc/lws.cu."""
-    N, R = 1024, 256
+def _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g):
+    if g.default:
+        lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
+    else:
+        lib.call("dv3_istft_geom", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips,
+                 _cp(_geometry_table(x.device, g.n_fft, g.hop)), g.n_fft, g.hop, st)
+
+
+def _lws_weights_fp64(N=1024, R=256):
+    """(2Q - 1, 11) complex128 with Q = N / R, [q + Q - 1, d + 5] = beta_q(d) = (1/N) sum_n w(n) w(n - q*R)
+    exp(-2 pi i d n / N), the sum over the n where both window indices lie in [0, N): the local-weighted-sum weights of
+    csrc/lws.cu (N = 1024, R = 256: (7, 11)) and csrc/lws_any.cu."""
+    Q = N // R
     n = np.arange(N)
     w = np.sqrt(0.5 * (1.0 - np.cos(2.0 * np.pi * (n + 0.5) / N)) * 2.0 * R / N)     # istft.cu frame_window
-    beta = np.zeros((7, 11), dtype=np.complex128)
-    for q in range(-3, 4):
+    beta = np.zeros((2 * Q - 1, 11), dtype=np.complex128)
+    for q in range(-(Q - 1), Q):
         j = n - q * R
         ok = (j >= 0) & (j < N)
         ww = np.where(ok, w * w[np.clip(j, 0, N - 1)], 0.0)
         for d in range(-5, 6):
-            beta[q + 3, d + 5] = np.sum(ww * np.exp(-2j * np.pi * d * n / N)) / N
+            beta[q + Q - 1, d + 5] = np.sum(ww * np.exp(-2j * np.pi * d * n / N)) / N
     return beta
+
+
+def _lws_tables_fp64(N, R):
+    """csrc/lws_any.cu's weight table in fp64: beta_q(d) e^{2 pi i d q / Q} ((2Q - 1) * 11 values, [q + Q - 1][d + 5]),
+    then the Q roots e^{-2 pi i r / Q}."""
+    Q = N // R
+    q = np.arange(-(Q - 1), Q)[:, None]
+    d = np.arange(-5, 6)[None, :]
+    folded = _lws_weights_fp64(N, R) * np.exp(2j * np.pi * d * q / Q)
+    return np.concatenate([folded.ravel(), np.exp(-2j * np.pi * np.arange(Q) / Q)])
 
 
 _lws_weight_cache = {}
 
 
-def _lws_weights(device):
-    """The weights as 77 [re, im] fp32 pairs on ``device`` (computed once per device)."""
-    key = str(device)
+def _lws_weights(device, g=None):
+    """The weights as [re, im] fp32 pairs on ``device`` (computed once per device and geometry): the 77 of csrc/lws.cu
+    at the default frame, csrc/lws_any.cu's table (_lws_tables_fp64) at any other."""
+    key = str(device) if g is None or g.default else (str(device), g.n_fft, g.hop)
     if key not in _lws_weight_cache:
-        b = _lws_weights_fp64()
+        b = _lws_weights_fp64() if g is None or g.default else _lws_tables_fp64(g.n_fft, g.hop)
         w = np.stack([b.real, b.imag], axis=-1).astype(np.float32)
         _lws_weight_cache[key] = torch.from_numpy(np.ascontiguousarray(w)).to(device)
     return _lws_weight_cache[key]
@@ -487,35 +596,44 @@ def _check_count(name, value):
 
 
 def lws(mag, n_iter=None, init_iters=1):
-    """mag: (T, 513) fp32 CUDA tensor of linear magnitudes -> waveform (n,) by LWS phase recovery: the one-clip case of
+    """mag: (T, K) fp32 CUDA tensor of linear magnitudes -> waveform (n,) by LWS phase recovery: the one-clip case of
     ``lws_batch``."""
     n_iter = hparams.lws_iters if n_iter is None else _check_count("n_iter", n_iter)
     init_iters = _check_count("init_iters", init_iters)
     if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 2):
-        raise Dv3Error("lws needs a (T, 513) fp32 CUDA tensor; there is no CPU path")
+        raise Dv3Error("lws needs a (T, fft_size // 2 + 1) fp32 CUDA tensor; there is no CPU path")
     return lws_batch(mag[None], [mag.shape[0]], n_iter, init_iters)[0]
 
 
 def lws_batch(mag, n_frames, n_iter=None, init_iters=1):
     """Local Weighted Sums phase recovery (Le Roux et al., DAFx 2010; the algorithm of the reference's ``lws.run_lws``,
-    parity unpinned: csrc/lws.cu) with the contract of ``griffin_lim_batch``: mag (nclips, T_max, 513), clip c valid
+    parity unpinned: csrc/lws.cu) with the contract of ``griffin_lim_batch``: mag (nclips, T_max, K), clip c valid
     for its first n_frames[c] frames -> waveforms (nclips, n_max), zero past each clip's own samples, each clip
     bit-identical to the clip alone.  The no-future initialisation (``init_iters`` in-frame passes per frame), then
     ``n_iter`` batch iterations (``hparams.lws_iters`` when None), then the inverse STFT."""
     n_iter = hparams.lws_iters if n_iter is None else _check_count("n_iter", n_iter)
     init_iters = _check_count("init_iters", init_iters)
-    mag, n_max, frames_d, samples_d, st = _ragged_clips(mag, n_frames, "lws_batch")
+    mag, n_max, frames_d, samples_d, st, g = _ragged_clips(mag, n_frames, "lws_batch")
     nclips, T_max = mag.shape[:2]
     dev = mag.device
-    w = _lws_weights(dev)
-    spec = torch.empty(nclips, T_max, 513, 2, device=dev)
+    w = _lws_weights(dev, g)
+    spec = torch.empty(nclips, T_max, g.bins, 2, device=dev)
     other = torch.empty_like(spec) if n_iter else None
-    lib.call("dv3_lws_nofuture_batched", _cp(mag), _cp(spec), _cp(w), _cp(frames_d), T_max, nclips, init_iters, st)
+    if g.default:
+        lib.call("dv3_lws_nofuture_batched", _cp(mag), _cp(spec), _cp(w), _cp(frames_d), T_max, nclips, init_iters, st)
+    else:
+        lib.call("dv3_lws_nofuture_geom", _cp(mag), _cp(spec), _cp(w), _cp(frames_d), T_max, nclips, init_iters,
+                 g.n_fft, g.hop, st)
     for _ in range(n_iter):
-        lib.call("dv3_lws_iterate_batched", _cp(mag), _cp(spec), _cp(other), _cp(w), _cp(frames_d), T_max, nclips, st)
+        if g.default:
+            lib.call("dv3_lws_iterate_batched", _cp(mag), _cp(spec), _cp(other), _cp(w), _cp(frames_d), T_max, nclips,
+                     st)
+        else:
+            lib.call("dv3_lws_iterate_geom", _cp(mag), _cp(spec), _cp(other), _cp(w), _cp(frames_d), T_max, nclips,
+                     g.n_fft, g.hop, st)
         spec, other = other, spec
     x = torch.zeros(nclips, n_max, device=dev)
-    lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
+    _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g)
     return x
 
 
@@ -542,14 +660,15 @@ def inv_preemphasis(x):
 
 
 def inv_spectrogram(spectrogram, n_iter=None, method="griffin_lim"):
-    """(513, T) normalised dB spectrogram (what ``spectrogram`` returns / the model predicts, transposed) -> waveform
+    """(K, T) normalised dB spectrogram, K = fft_size // 2 + 1 (what ``spectrogram`` returns / the model predicts,
+    transposed) -> waveform
     float32 numpy array -- reference audio.py:37-43: denormalise, dB -> amplitude, ** power, phase recovery, inverse
     STFT, de-emphasis.  The one-clip case of ``inv_spectrogram_batch``."""
     return inv_spectrogram_batch([spectrogram], n_iter, method)[0]
 
 
 def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
-    """[(513, T_c) normalised dB spectrograms] -> [waveform c (float32 numpy array)], all clips in one set of launches
+    """[(K, T_c) normalised dB spectrograms] -> [waveform c (float32 numpy array)], all clips in one set of launches
     per iteration.  Clip c is bit-identical to ``inv_spectrogram(spectrograms[c])``: the magnitude and de-emphasis
     kernels work element by element / causally along each clip, and the phase recovery is ``griffin_lim_batch``
     (``method="griffin_lim"``, ``hparams.griffin_lim_iters`` iterations when n_iter is None) or ``lws_batch``
@@ -561,11 +680,12 @@ def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
     specs = [np.asarray(s, dtype=np.float32) for s in spectrograms]
     if not specs:
         raise ValueError("inv_spectrogram_batch needs at least one spectrogram")
+    K = check_geometry(mel=False).bins
     for s in specs:
-        if s.ndim != 2 or s.shape[0] != 513:
-            raise Dv3Error("spectrograms must be (513, T) arrays, got %s" % (s.shape,))
+        if s.ndim != 2 or s.shape[0] != K:
+            raise Dv3Error("spectrograms must be (%d, T) arrays, got %s" % (K, s.shape))
     n_frames = [s.shape[1] for s in specs]
-    S = np.zeros((len(specs), max(n_frames), 513), dtype=np.float32)
+    S = np.zeros((len(specs), max(n_frames), K), dtype=np.float32)
     for c, s in enumerate(specs):
         S[c, :s.shape[1]] = s.T
     S = torch.from_numpy(S).cuda()

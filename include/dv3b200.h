@@ -262,6 +262,35 @@ int dv3_lws_iterate_batched(const float* mag, const float* spec_in, float* spec_
                             const int* nframes, int max_frames, int nclips, void* stream);
 int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long long stride, float coef, void* stream);
 
+/* ---- the same audio path for any supported STFT frame (csrc/stft_any.cu, csrc/lws_any.cu; audio.check_geometry):
+ * n_fft even in [256, 4096] with n_fft / 2 free of prime factors above 5, hop = n_fft / Q with Q in [2, 8]; K =
+ * n_fft / 2 + 1 bins; padding n_fft - hop samples on both sides.  An unsupported geometry returns an error before any
+ * launch.  table: 3 * n_fft + 2 floats on the device -- window (n_fft), twiddles exp(-2 pi i j / (n_fft/2)) and split
+ * factors exp(-2 pi i k / n_fft) as [re, im] pairs, computed in fp64 and rounded once (audio._geometry_table).
+ * dv3_stft_num_frames_geom: frames of an n-sample clip, ceil((n + n_fft - 2 hop) / hop) + 1.
+ * dv3_stft_mel_geom: dv3_stft_mel_targets for the geometry (linear rows of K floats, mel_basis (n_mels, K) with the
+ * same sparse span description; lead = 0, downsample_step = 1, T_lin = max_frames is the dv3_stft_mel layout).
+ * dv3_stft_complex_geom / dv3_istft_geom: the batched forms of dv3_stft_complex_batched / dv3_istft_batched with K
+ * bins per frame; the overlap-add runs as Q ordered launches (frames f and f + Q do not overlap), deterministic.
+ * dv3_lws_nofuture_geom / dv3_lws_iterate_geom: the batched LWS forms with K bins; weights ((2Q - 1) * 11 + Q) [re, im]
+ * fp32 pairs = beta_q(d) e^{2 pi i d q / Q} at [q + Q - 1][d + 5], |q| <= Q - 1, |d| <= 5, then the Q roots
+ * e^{-2 pi i r / Q} (audio._lws_tables_fp64).  Every form: each clip of a ragged batch is bit-identical alone. */
+int dv3_stft_num_frames_geom(int n_samples, int n_fft, int hop);
+int dv3_stft_mel_geom(const void* wav, int wav_int16, const int* lengths, const float* peak, float rescaling_max,
+                      const float* table, const float* mel_basis, const int* mel_start, const int* mel_len,
+                      float* linear, float* mel, int nclips, int max_len, int T_lin, int lead, int downsample_step,
+                      int n_mels, int n_fft, int hop, float preemph, float min_level_db, float ref_level_db,
+                      void* stream);
+int dv3_stft_complex_geom(const float* wav, const int* n_samples, long long wav_pitch, const float* mag, float* spec,
+                          const int* nframes, int max_frames, int nclips, const float* table, int n_fft, int hop,
+                          void* stream);
+int dv3_istft_geom(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
+                   int max_frames, int nclips, const float* table, int n_fft, int hop, void* stream);
+int dv3_lws_nofuture_geom(const float* mag, float* spec, const float* weights, const int* nframes, int max_frames,
+                          int nclips, int init_iters, int n_fft, int hop, void* stream);
+int dv3_lws_iterate_geom(const float* mag, const float* spec_in, float* spec_out, const float* weights,
+                         const int* nframes, int max_frames, int nclips, int n_fft, int hop, void* stream);
+
 /* ================= tensor-core ConvBlock / conv path: wgmma + TMA, split 16-bit operands =================
  * Same reference code as dv3_convblock_fwd / dv3_conv1d_fwd / dv3_conv1d_dgrad / dv3_conv1d_wgrad (modules.py:94-100,
  * 145-164, 200-226 and their autograd).  Every fp32 operand is split into a (hi, lo) pair of 16-bit planes (below) and
