@@ -104,25 +104,44 @@ def harness(tmp_path_factory):
 
 
 def test_fft_core_matches_numpy_for_every_supported_length(harness):
-    """Forward rfft and the inverse (merge + passes) of the g++ build against numpy, 1e-5 of the spectrum's /
-    signal's largest value, for every N the geometry rule accepts (radix-2/3/4/5 passes in every combination)."""
+    """Forward rfft and the inverse (merge + passes) of the g++ build against numpy, for every N the geometry rule
+    accepts (radix-2/3/4/5 passes in every combination), within the bounds of tests/audio_bounds.py (kernel "any"):
+    |X_hat - X| <= c_fft u sum|x|, and the inverse against the fp64 packed inverse of the harness' own spectrum,
+    c_fft u sum|X| / M plus the rounding of the division by M.  Noise, a tone with DC and Nyquist, and an impulse."""
+    import audio_bounds as AB
     from deepvoice3_pytorch_b200 import audio
     rng = np.random.default_rng(0)
+    worst = {}
     for N in SUPPORTED_N:
-        x = rng.standard_normal(N).astype(np.float32)
+        n = np.arange(N)
+        signals = {"noise": rng.standard_normal(N),
+                   "tone": 0.5 * np.cos(2 * np.pi * (N // 7) * n / N) + 0.25 + 0.125 * (-1.0) ** n,
+                   "impulse": (n == 3).astype(np.float64)}
         tab = audio._geometry_table_fp64(N, N // 4 if N % 4 == 0 else N // 2)
         flat = np.concatenate([tab[0], np.stack([tab[1].real, tab[1].imag], -1).ravel(),
                                np.stack([tab[2].real, tab[2].imag], -1).ravel()]).astype(np.float32)
-        out = subprocess.run([harness], input=np.int32(N).tobytes() + flat.tobytes() + x.tobytes(),
-                             stdout=subprocess.PIPE, check=True).stdout
-        got = np.frombuffer(out, dtype=np.float32)
-        K = N // 2 + 1
-        X = got[:2 * K].astype(np.float64).view(np.complex128)
-        y = got[2 * K:]
-        ref = np.fft.rfft(x.astype(np.float64))
-        assert np.isfinite(got).all(), N
-        assert np.abs(X - ref).max() <= 1e-5 * np.abs(ref).max(), (N, np.abs(X - ref).max() / np.abs(ref).max())
-        assert np.abs(y - x).max() <= 1e-5 * np.abs(x).max(), N
+        for name, sig in signals.items():
+            x = sig.astype(np.float32)
+            out = subprocess.run([harness], input=np.int32(N).tobytes() + flat.tobytes() + x.tobytes(),
+                                 stdout=subprocess.PIPE, check=True).stdout
+            got = np.frombuffer(out, dtype=np.float32)
+            K, M = N // 2 + 1, N // 2
+            X = got[:2 * K].astype(np.float64).view(np.complex128)
+            y = got[2 * K:].astype(np.float64)
+            assert np.isfinite(got).all(), N
+            ref = np.fft.rfft(x.astype(np.float64))
+            c = AB.c_fft("any", N)
+            r_fwd = np.abs(X - ref).max() / (c * AB.U * np.abs(x).sum())
+            yref = AB.packed_irfft(X, N)
+            r_inv = (np.abs(y - yref) / (c * AB.U * np.abs(X).sum() / M + AB.U * np.abs(yref))).max()
+            assert r_fwd <= 1.0 and r_inv <= 1.0, (N, name, r_fwd, r_inv)
+            # normwise, and the round trip back to x: tighter than the elementwise bound on noise
+            assert np.abs(X - ref).max() <= 1e-5 * np.abs(ref).max(), (N, name)
+            assert np.abs(y - x).max() <= 1e-5 * np.abs(x).max(), (N, name)
+            worst[name] = max(worst.get(name, (0, 0)), (r_fwd, r_inv))
+            worst[name + " u*sum|x|"] = max(worst.get(name + " u*sum|x|", 0),
+                                            np.abs(X - ref).max() / (AB.U * np.abs(x).sum()))
+    print("fft_any harness, largest (forward, inverse) error / bound and forward error in u sum|x|:", worst)
 
 
 def test_plan_covers_every_supported_length():
