@@ -61,6 +61,15 @@ __device__ __forceinline__ void det_loss_tail(float s, float s1, float s2, float
 //   loss += sum (1-bw)*coef1*|d| + bw*coef*z,  coef = w*m/Sm + (1-w)/N,  m = (t+r < len_b)
 // priority bins (train.py:559-567): the L1 term becomes (1-pw)*L1(all bins) + pw*L1(bins < pbin), i.e.
 //   coef1 = (1-pw)*coef + [d < pbin]*pw*coef*(D/pbin)     (the same masked/plain means over the pbin-wide slice)
+// Sm = sum_b clamp(len_b - r, 0, TL - r) * D.  When every row is masked (Sm = 0) the masked mean, 0/0 in the
+// reference, is taken as 0: coef = (1-w)/N.
+// Binary divergence (train.py:537-553) with L = log(p+eps) - log(1-p+eps):  z = -y L + log1p(exp(L)), dz/dp =
+// (sigmoid(L) - y) (1/(p+eps) + 1/(1-p+eps)).  Evaluated as written, both cancel: at saturation z subtracts two values
+// near 18.4, and sigmoid(L) = (p+eps)/(1+2eps) - y cancels before being multiplied by up to 1/eps.  The kernel uses the
+// identical forms
+//   z     = -(y log(p+eps) + (1-y) log(1-p+eps)) + log1p(2 eps)            (a sum of non-negative terms)
+//   dz/dp = (d + eps (1 - 2y)) / ((p+eps) (1-p+eps)),   d = p - y          (d already formed for the L1 term)
+// which are a few ulp from exact for every p, y in [0, 1] and need neither expf nor log1pf of a variable.
 // t_log (int64 in device memory, or null = T): the logical time extent of a batch padded to a larger bucket.  Pairs
 // t >= t_log - r are left out of the loss and its means, and their gradient is written as 0.
 // TERMS: also add the two parts of the loss to terms[0] (the L1 part, priority bins combined) and terms[1] (the
@@ -110,12 +119,11 @@ __device__ __forceinline__ void spec_loss_body(const float* __restrict__ y_hat, 
             float e = c1 * (1.f - bw) * fabsf(d);
             float de = c1 * (1.f - bw) * (d > 0.f ? 1.f : (d < 0.f ? -1.f : 0.f));
             if (TERMS) acc_l1 += coef * (c1 * fabsf(d));
-            if (bw > 0.f) {
-                const float L = logf(p + eps) - logf(1.f - p + eps);
-                const float u = expf(L);
-                const float z = -tg * L + log1pf(u);
+            if (bw > 0.f) {                                   // the cancellation-free forms: see the header
+                const float a = p + eps, c = 1.f - p + eps;
+                const float z = -(tg * logf(a) + (1.f - tg) * logf(c)) + log1pf(2.f * eps);
                 e += bw * z;
-                de += bw * (u / (1.f + u) - tg) * (1.f / (p + eps) + 1.f / (1.f - p + eps));
+                de += bw * ((d + eps * (1.f - 2.f * tg)) / (a * c));
                 if (TERMS) acc_bd += coef * z;
             }
             acc += coef * e;
