@@ -6,8 +6,9 @@ transform on a training batch's waveforms and writes the padded, decimated targe
 (training from wav files, ``data.WavDataset``).
 
 ``inv_spectrogram`` (reference audio.py:37-43) recovers the phase on the same STFT frame with Griffin-Lim (the default,
-csrc/istft.cu) or with Local Weighted Sums (``method="lws"``, csrc/lws.cu), the algorithm of the reference's
-``lws.run_lws``.  The ``lws`` package is an un-vendored dependency whose source is absent, so parity with it is unpinned.
+csrc/istft.cu), with fast Griffin-Lim (``method="fast_griffin_lim"``: Griffin-Lim with momentum, as librosa and
+torchaudio run it by default) or with Local Weighted Sums (``method="lws"``, csrc/lws.cu), the algorithm of the
+reference's ``lws.run_lws``.  The ``lws`` package is an un-vendored dependency whose source is absent, so parity with it is unpinned.
 
 The STFT frame is ``hparams.fft_size`` / ``hparams.hop_size``, as in the reference.  ``check_geometry`` decides which
 frames are supported: at 1024 / 256 (every reference preset) the specialised kernels run; any other supported frame
@@ -36,6 +37,8 @@ class _HP:
     power = 1.4                   # spectrogram sharpening before phase recovery (presets/*.json)
     griffin_lim_iters = 60
     lws_iters = 30                # LWS batch iterations after the no-future initialisation (DESIGN.md section 7)
+    griffin_lim_momentum = 0.99   # fast Griffin-Lim (method="fast_griffin_lim"): librosa's / torchaudio's default
+    fast_griffin_lim_iters = 20   # FGLA iterations that reach Griffin-Lim-60's convergence (DESIGN.md section 7.3)
     rescaling = False             # preprocess.py: y = x / |x|.max() * rescaling_max (hparams.py:46-48)
     rescaling_max = 0.999
     min_text = 20                 # utterances with shorter transcripts are skipped (hparams.py:137)
@@ -479,14 +482,24 @@ def inv_num_samples(n_frames):
     return (int(n_frames) - 1) * hparams.hop_size - (hparams.fft_size - 2 * hparams.hop_size)
 
 
-def griffin_lim(mag, n_iter=None):
+def griffin_lim(mag, n_iter=None, momentum=0.0):
     """mag: (T, fft_size // 2 + 1) fp32 CUDA tensor of linear magnitudes -> waveform (n,) whose STFT magnitude
     approximates it.
     x <- istft(mag * exp(i*angle(stft(x)))), started from the zero-phase inverse; every arrow is one kernel launch
-    (the batched kernels with one clip: ``griffin_lim_batch``)."""
+    (the batched kernels with one clip: ``griffin_lim_batch``, which also describes ``momentum``)."""
+    momentum = _check_momentum(momentum)
     if not (torch.is_tensor(mag) and mag.is_cuda and mag.dtype == torch.float32 and mag.dim() == 2):
         raise Dv3Error("griffin_lim needs a (T, fft_size // 2 + 1) fp32 CUDA tensor; there is no CPU path")
-    return griffin_lim_batch(mag[None], [mag.shape[0]], n_iter)[0]
+    return griffin_lim_batch(mag[None], [mag.shape[0]], n_iter, momentum)[0]
+
+
+def _check_momentum(momentum):
+    """-> momentum as a float in [0, 1), else ValueError (the range torchaudio's GriffinLim accepts)."""
+    if isinstance(momentum, (bool, np.bool_)) or not isinstance(momentum, (int, float, np.integer, np.floating)):
+        raise ValueError("momentum must be a real number in [0, 1), got %r" % (momentum,))
+    if not 0.0 <= float(momentum) < 1.0:                  # also refuses NaN
+        raise ValueError("momentum must lie in [0, 1), got %r" % (momentum,))
+    return float(momentum)
 
 
 def _ragged_clips(mag, n_frames, name):
@@ -511,18 +524,38 @@ def _ragged_clips(mag, n_frames, name):
     return mag, max(n_samples), frames_d, samples_d, ctypes.c_void_p(torch.cuda.current_stream().cuda_stream), g
 
 
-def griffin_lim_batch(mag, n_frames, n_iter=None):
+def griffin_lim_batch(mag, n_frames, n_iter=None, momentum=0.0):
     """mag: (nclips, T_max, K) fp32 CUDA tensor (K = fft_size // 2 + 1), clip c valid for its first n_frames[c] frames -> waveforms
     (nclips, n_max), clip c valid for its first inv_num_samples(n_frames[c]) samples and zero after them.  Each clip
     comes out bit-identical to ``griffin_lim`` on that clip alone: the kernels read and write only a clip's own frames
-    and samples, and the overlap-add is deterministic (csrc/istft.cu)."""
+    and samples, and the overlap-add is deterministic (csrc/istft.cu).
+
+    momentum: 0 (the default) runs plain Griffin-Lim.  0 < momentum < 1 runs fast Griffin-Lim (Perraudin, Balazs &
+    Sondergaard, WASPAA 2013; librosa's and torchaudio's ``momentum``): each iteration projects
+    C = X - beta * X_prev, beta = momentum / (1 + momentum), instead of the new spectrum X, where X_prev is the previous
+    iteration's X (0 before the first); csrc/istft.cu stft_complex_momentum_kernel, csrc/stft_any.cu at other frames.
+    Any other value raises ValueError before anything is allocated or launched."""
+    momentum = _check_momentum(momentum)
     mag, n_max, frames_d, samples_d, st, g = _ragged_clips(mag, n_frames, "griffin_lim_batch")
     nclips, T_max = mag.shape[:2]
     dev = mag.device
     spec = torch.zeros(nclips, T_max, g.bins, 2, device=dev)
     spec[..., 0] = mag                                   # zero phase
     x = torch.zeros(nclips, n_max, device=dev)
-    if g.default:
+    if momentum:
+        prev = torch.zeros_like(spec)
+        beta = momentum / (1.0 + momentum)               # fp64 here, rounded to fp32 once by the call
+        if g.default:
+            def stft(x, spec):
+                lib.call("dv3_stft_complex_momentum_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(prev),
+                         _cp(spec), _cp(frames_d), T_max, nclips, beta, st)
+        else:
+            tab = _geometry_table(dev, g.n_fft, g.hop)
+
+            def stft(x, spec):
+                lib.call("dv3_stft_complex_momentum_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(prev),
+                         _cp(spec), _cp(frames_d), T_max, nclips, beta, _cp(tab), g.n_fft, g.hop, st)
+    elif g.default:
         def stft(x, spec):
             lib.call("dv3_stft_complex_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
                      T_max, nclips, st)
@@ -637,7 +670,7 @@ def lws_batch(mag, n_frames, n_iter=None, init_iters=1):
     return x
 
 
-PHASE_METHODS = ("griffin_lim", "lws")
+PHASE_METHODS = ("griffin_lim", "lws", "fast_griffin_lim")
 
 
 def check_phase_method(method):
@@ -671,12 +704,16 @@ def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
     """[(K, T_c) normalised dB spectrograms] -> [waveform c (float32 numpy array)], all clips in one set of launches
     per iteration.  Clip c is bit-identical to ``inv_spectrogram(spectrograms[c])``: the magnitude and de-emphasis
     kernels work element by element / causally along each clip, and the phase recovery is ``griffin_lim_batch``
-    (``method="griffin_lim"``, ``hparams.griffin_lim_iters`` iterations when n_iter is None) or ``lws_batch``
-    (``method="lws"``, ``hparams.lws_iters``).  An unknown method, or a negative LWS iteration count, raises
-    ValueError before anything runs."""
+    (``method="griffin_lim"``, ``hparams.griffin_lim_iters`` iterations when n_iter is None), ``lws_batch``
+    (``method="lws"``, ``hparams.lws_iters``) or ``griffin_lim_batch`` with ``momentum=hparams.griffin_lim_momentum``
+    (``method="fast_griffin_lim"``, ``hparams.fast_griffin_lim_iters``).  An unknown method, a negative LWS or fast
+    Griffin-Lim iteration count, or a momentum outside [0, 1) raises ValueError before anything runs."""
     check_phase_method(method)
-    if method == "lws" and n_iter is not None:
+    if method in ("lws", "fast_griffin_lim") and n_iter is not None:
         _check_count("n_iter", n_iter)
+    if method == "fast_griffin_lim":
+        momentum = _check_momentum(hparams.griffin_lim_momentum)
+        n_iter = hparams.fast_griffin_lim_iters if n_iter is None else n_iter
     specs = [np.asarray(s, dtype=np.float32) for s in spectrograms]
     if not specs:
         raise ValueError("inv_spectrogram_batch needs at least one spectrogram")
@@ -693,6 +730,9 @@ def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     lib.call("dv3_spec_to_amp", _cp(S), _cp(amp), S.numel(), float(hparams.min_level_db), float(hparams.ref_level_db),
              float(hparams.power), st)
-    recover = lws_batch if method == "lws" else griffin_lim_batch
-    wav = inv_preemphasis(recover(amp, n_frames, n_iter)).cpu().numpy()
+    if method == "fast_griffin_lim":
+        wav = griffin_lim_batch(amp, n_frames, n_iter, momentum)
+    else:
+        wav = (lws_batch if method == "lws" else griffin_lim_batch)(amp, n_frames, n_iter)
+    wav = inv_preemphasis(wav).cpu().numpy()
     return [wav[c, :inv_num_samples(t)].copy() for c, t in enumerate(n_frames)]

@@ -9,6 +9,8 @@
 // Kernels (one CTA of 256 threads per frame, the shared-memory radix-2 transform of stft.cu):
 //   spec_to_amp_kernel      normalised dB spectrogram -> linear magnitude ** power
 //   stft_complex_kernel     waveform -> complex half spectrum (frames, 513) [optionally projected onto a magnitude]
+//   stft_complex_momentum_kernel  the same transform with the fast Griffin-Lim epilogue
+//                           (audio.griffin_lim_batch with momentum > 0, DESIGN.md section 7.3)
 //   istft_kernel            complex half spectrum -> windowed frame, overlap-added into the waveform: frames f and f+4
 //                           do not overlap (fsize = 4*hop), so one launch per residue class f mod 4 adds with plain
 //                           loads and stores -- deterministic, each sample summed in the same order every run
@@ -57,21 +59,13 @@ __global__ void spec_to_amp_kernel(const float* __restrict__ s, float* __restric
     }
 }
 
-// wav (len) -> spec (nframes, 513, 2).  mag != null: the result is projected onto that magnitude (Griffin-Lim step):
-// spec = mag * X / |X| (X == 0 keeps phase 0).  No preemphasis here (the iteration runs on the pre-emphasised signal).
-// Clip c = blockIdx.y: x + c*x_pitch, spec / mag + c*frame_pitch frames; len / nframes from lens / frames when given.
-__global__ void __launch_bounds__(256) stft_complex_kernel(const float* __restrict__ x, int len0, const int* lens,
-                                                           long long x_pitch, const float* __restrict__ mag,
-                                                           float* __restrict__ spec, int nframes0, const int* frames,
-                                                           long long frame_pitch) {
-    pdl_trigger(); pdl_wait();
+// The forward transform of one frame: frame `frame` of the clip x (len samples), windowed, 512-point packed FFT, split
+// into the half spectrum; epi(k, Re X_k, Im X_k) for k = 0..512 (k = tid, tid + 256, and 512 on thread 0).  No
+// preemphasis here (the iteration runs on the pre-emphasised signal).
+template <class Epi>
+__device__ __forceinline__ void stft_frame_1024(const float* __restrict__ x, int len, int frame, Epi epi) {
     __shared__ float zr[INH], zi[INH], twr[INH / 2], twi[INH / 2];
-    const int frame = blockIdx.x, clip = blockIdx.y, tid = threadIdx.x;
-    const int nframes = frames ? frames[clip] : nframes0, len = lens ? lens[clip] : len0;
-    if (frame >= nframes) return;
-    x += clip * x_pitch;
-    spec += clip * frame_pitch * INBINS * 2;
-    if (mag) mag += clip * frame_pitch * INBINS;
+    const int tid = threadIdx.x;
     { float s, c; sincospif(-(float)tid / 256.f, &s, &c); twr[tid] = c; twi[tid] = s; }
     const int base = frame * IHOP - IPAD;
 #pragma unroll
@@ -95,14 +89,58 @@ __global__ void __launch_bounds__(256) stft_complex_kernel(const float* __restri
         const float orr = di, oi = -dr;
         float s, c;
         sincospif(-(float)k / 512.f, &s, &c);
-        float xr = er + c * orr - s * oi, xi = ei + c * oi + s * orr;
-        const size_t o = ((size_t)frame * INBINS + k) * 2;
-        if (mag) {
-            const float m = mag[(size_t)frame * INBINS + k], a = sqrtf(xr * xr + xi * xi);
-            if (a > 0.f) { xr *= m / a; xi *= m / a; } else { xr = m; xi = 0.f; }
-        }
-        spec[o] = xr; spec[o + 1] = xi;
+        epi(k, er + c * orr - s * oi, ei + c * oi + s * orr);
     }
+}
+
+// mag X / |X| (X == 0 gives phase 0): the Griffin-Lim magnitude projection of both complex-STFT kernels
+__device__ __forceinline__ void project_1024(float m, float& xr, float& xi) {
+    const float a = sqrtf(fmaf(xr, xr, xi * xi));      // explicit: both kernels round |X|^2 the same way
+    if (a > 0.f) { xr *= m / a; xi *= m / a; } else { xr = m; xi = 0.f; }
+}
+
+// wav (len) -> spec (nframes, 513, 2).  mag != null: the result is projected onto that magnitude (Griffin-Lim step):
+// spec = mag * X / |X| (X == 0 keeps phase 0).
+// Clip c = blockIdx.y: x + c*x_pitch, spec / mag + c*frame_pitch frames; len / nframes from lens / frames when given.
+__global__ void __launch_bounds__(256) stft_complex_kernel(const float* __restrict__ x, int len0, const int* lens,
+                                                           long long x_pitch, const float* __restrict__ mag,
+                                                           float* __restrict__ spec, int nframes0, const int* frames,
+                                                           long long frame_pitch) {
+    pdl_trigger(); pdl_wait();
+    const int frame = blockIdx.x, clip = blockIdx.y;
+    const int nframes = frames ? frames[clip] : nframes0, len = lens ? lens[clip] : len0;
+    if (frame >= nframes) return;
+    x += clip * x_pitch;
+    spec += clip * frame_pitch * INBINS * 2;
+    if (mag) mag += clip * frame_pitch * INBINS;
+    stft_frame_1024(x, len, frame, [&](int k, float xr, float xi) {
+        const size_t o = ((size_t)frame * INBINS + k) * 2;
+        if (mag) project_1024(mag[(size_t)frame * INBINS + k], xr, xi);
+        spec[o] = xr; spec[o + 1] = xi;
+    });
+}
+
+// The fast Griffin-Lim step (Perraudin, Balazs & Sondergaard, WASPAA 2013) on the same transform: per bin,
+// C = X - beta * prev, prev <- X (read and written in place by the same thread), spec = mag * C / |C| (C == 0 gives
+// (mag, 0)).  beta == 0 takes C = X itself, so the step is then stft_complex_kernel's projection bit for bit whatever
+// prev holds.  Layout and ragged-clip rules as stft_complex_kernel (prev like spec); every clip is batched (lens and
+// frames given).
+__global__ void __launch_bounds__(256) stft_complex_momentum_kernel(const float* __restrict__ x, const int* lens,
+                                                                    long long x_pitch, const float* __restrict__ mag,
+                                                                    float2* __restrict__ prev,
+                                                                    float2* __restrict__ spec, const int* frames,
+                                                                    long long frame_pitch, float beta) {
+    pdl_trigger(); pdl_wait();
+    const int frame = blockIdx.x, clip = blockIdx.y;
+    if (frame >= frames[clip]) return;
+    const size_t row = ((size_t)clip * frame_pitch + frame) * INBINS;
+    stft_frame_1024(x + clip * x_pitch, lens[clip], frame, [&](int k, float xr, float xi) {
+        const float2 p = prev[row + k];
+        prev[row + k] = make_float2(xr, xi);
+        if (beta != 0.f) { xr = fmaf(-beta, p.x, xr); xi = fmaf(-beta, p.y, xi); }
+        project_1024(mag[row + k], xr, xi);
+        spec[row + k] = make_float2(xr, xi);
+    });
 }
 
 // spec (nframes, 513, 2) -> y (len) += window * irfft(spec[frame]) placed at frame*hop - pad   (y zeroed by the caller)
@@ -225,6 +263,17 @@ int dv3_stft_complex_batched(const float* wav, const int* n_samples, long long w
                 "stft_complex_batched: bad shape");
     return stft_complex_launch(wav, 0, n_samples, wav_pitch, mag, spec, 0, nframes, max_frames, nclips,
                                (cudaStream_t)stream);
+}
+
+int dv3_stft_complex_momentum_batched(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
+                                      float* prev, float* spec, const int* nframes, int max_frames, int nclips,
+                                      float beta, void* stream) {
+    DV3_REQUIRE(max_frames >= 1 && nclips >= 1 && nclips <= 65535 && n_samples && nframes && mag && prev,
+                "stft_complex_momentum_batched: bad shape");
+    DV3_REQUIRE(beta >= 0.f && beta < 1.f, "stft_complex_momentum_batched: beta %g outside [0, 1)", (double)beta);
+    launch_k(stft_complex_momentum_kernel, dim3(max_frames, nclips), 256, 0, (cudaStream_t)stream, wav, n_samples,
+             wav_pitch, mag, (float2*)prev, (float2*)spec, nframes, (long long)max_frames, beta);
+    return check_launch("stft_complex_momentum");
 }
 
 int dv3_istft_batched(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,

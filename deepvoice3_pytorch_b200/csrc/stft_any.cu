@@ -13,6 +13,7 @@
 //                       shuffle tree: deterministic).  Output descriptor and zero rows as stft.cu's StftParams.
 //   stft_complex_any    waveform -> complex half spectrum, optionally projected onto a magnitude (Griffin-Lim step);
 //                       one CTA per frame.
+//   stft_complex_momentum_any  the same transform with the fast Griffin-Lim epilogue (DESIGN.md section 7.3).
 //   istft_any           complex half spectrum -> windowed frame, overlap-added in Q ordered launches, one per residue
 //                       class f mod Q: frames f and f+Q do not overlap (N = Q*R), so the adds are plain loads and
 //                       stores and every sample is summed in the same order every run.
@@ -183,6 +184,28 @@ struct WaveLoad {              // first-pass points of a frame read straight fro
     __device__ __forceinline__ c2 operator()(int i) const { return {s(2 * i), s(2 * i + 1)}; }
 };
 
+// The forward transform of frame `frame` of clip `clip` into shared memory: -> the packed transform Z, whose bin k is
+// split_bin(Z, M, k, sp[k]) with the split factors sp it sets.  Shared by both complex-STFT kernels.
+__device__ __forceinline__ const c2* complex_any_frame(const float* x, const int* lens, long long x_pitch, int clip,
+                                                       int frame, const float* tab, int N, int R, Plan plan,
+                                                       const c2*& sp) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int M = N / 2, tid = threadIdx.x;
+    c2* bufa = reinterpret_cast<c2*>(smem_raw);
+    c2* bufb = bufa + M;
+    const c2* tw = reinterpret_cast<const c2*>(tab + tab_tw(N));
+    sp = reinterpret_cast<const c2*>(tab + tab_sp(N));
+    const WaveLoad load{x + clip * x_pitch, tab, frame * R - (N - R), lens[clip]};
+    fft_pass(load, bufa, tw, M, plan.radix(0), 1, tid, ANY_THREADS);
+    return any_passes(plan, bufa, bufb, tw, tid);
+}
+
+// mag X / |X| (X == 0 gives phase 0): the Griffin-Lim magnitude projection of both complex-STFT kernels
+__device__ __forceinline__ void project_any(float m, c2& X) {
+    const float a = sqrtf(fmaf(X.x, X.x, X.y * X.y));  // explicit: both kernels round |X|^2 the same way
+    if (a > 0.f) { X.x *= m / a; X.y *= m / a; } else { X.x = m; X.y = 0.f; }
+}
+
 // wav -> spec (clip, frame, K) float2 [projected onto mag when given]; grid (max_frames, nclips)
 __global__ void __launch_bounds__(ANY_THREADS) stft_complex_any_kernel(const float* __restrict__ x, const int* lens,
                                                                        long long x_pitch, const float* __restrict__ magp,
@@ -190,24 +213,40 @@ __global__ void __launch_bounds__(ANY_THREADS) stft_complex_any_kernel(const flo
                                                                        long long frame_pitch, const float* tab, int N,
                                                                        int R, Plan plan) {
     pdl_trigger(); pdl_wait();
-    extern __shared__ __align__(16) unsigned char smem_raw[];
     const int M = N / 2, K = M + 1;
     const int frame = blockIdx.x, clip = blockIdx.y, tid = threadIdx.x;
     if (frame >= frames[clip]) return;
-    c2* bufa = reinterpret_cast<c2*>(smem_raw);
-    c2* bufb = bufa + M;
-    const c2* tw = reinterpret_cast<const c2*>(tab + tab_tw(N));
-    const c2* sp = reinterpret_cast<const c2*>(tab + tab_sp(N));
-    const WaveLoad load{x + clip * x_pitch, tab, frame * R - (N - R), lens[clip]};
-    fft_pass(load, bufa, tw, M, plan.radix(0), 1, tid, ANY_THREADS);
-    const c2* Z = any_passes(plan, bufa, bufb, tw, tid);
+    const c2* sp;
+    const c2* Z = complex_any_frame(x, lens, x_pitch, clip, frame, tab, N, R, plan, sp);
     const size_t row = ((size_t)clip * frame_pitch + frame) * K;
     for (int k = tid; k < K; k += ANY_THREADS) {
         c2 X = split_bin(Z, M, k, sp[k]);
-        if (magp) {
-            const float m = magp[row + k], a = sqrtf(X.x * X.x + X.y * X.y);
-            if (a > 0.f) { X.x *= m / a; X.y *= m / a; } else { X.x = m; X.y = 0.f; }
-        }
+        if (magp) project_any(magp[row + k], X);
+        spec[row + k] = make_float2(X.x, X.y);
+    }
+}
+
+// The fast Griffin-Lim step on the same transform (istft.cu's stft_complex_momentum_kernel for K bins): per bin
+// C = X - beta * prev, prev <- X in place (same thread, same element), spec = mag * C / |C|; beta == 0 takes C = X,
+// the projection of stft_complex_any_kernel bit for bit.  grid (max_frames, nclips); frames past a clip's count are
+// neither read nor written.
+__global__ void __launch_bounds__(ANY_THREADS) stft_complex_momentum_any_kernel(
+        const float* __restrict__ x, const int* lens, long long x_pitch, const float* __restrict__ magp,
+        float2* __restrict__ prev, float2* __restrict__ spec, const int* frames, long long frame_pitch, float beta,
+        const float* tab, int N, int R, Plan plan) {
+    pdl_trigger(); pdl_wait();
+    const int M = N / 2, K = M + 1;
+    const int frame = blockIdx.x, clip = blockIdx.y, tid = threadIdx.x;
+    if (frame >= frames[clip]) return;
+    const c2* sp;
+    const c2* Z = complex_any_frame(x, lens, x_pitch, clip, frame, tab, N, R, plan, sp);
+    const size_t row = ((size_t)clip * frame_pitch + frame) * K;
+    for (int k = tid; k < K; k += ANY_THREADS) {
+        c2 X = split_bin(Z, M, k, sp[k]);
+        const float2 p = prev[row + k];
+        prev[row + k] = make_float2(X.x, X.y);
+        if (beta != 0.f) { X.x = fmaf(-beta, p.x, X.x); X.y = fmaf(-beta, p.y, X.y); }
+        project_any(magp[row + k], X);
         spec[row + k] = make_float2(X.x, X.y);
     }
 }
@@ -320,6 +359,23 @@ int dv3_stft_complex_geom(const float* wav, const int* n_samples, long long wav_
     if (any_reserve(stft_complex_any_kernel, smem, what)) return 1;
     launch_k(stft_complex_any_kernel, dim3(max_frames, nclips), ANY_THREADS, smem, (cudaStream_t)stream, wav,
              n_samples, wav_pitch, mag, (float2*)spec, nframes, (long long)max_frames, table, n_fft, hop, plan);
+    return check_launch(what);
+}
+
+int dv3_stft_complex_momentum_geom(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
+                                   float* prev, float* spec, const int* nframes, int max_frames, int nclips,
+                                   float beta, const float* table, int n_fft, int hop, void* stream) {
+    const char* what = "stft_complex_momentum_geom";
+    Plan plan;
+    if (any_geometry(n_fft, hop, plan, what)) return 1;
+    DV3_REQUIRE(max_frames >= 1 && max_frames <= 2147483647 && nclips >= 1 && nclips <= 65535 && n_samples && nframes
+                && table && mag && prev, "%s: bad shape", what);
+    DV3_REQUIRE(beta >= 0.f && beta < 1.f, "%s: beta %g outside [0, 1)", what, (double)beta);
+    const size_t smem = 2 * sizeof(c2) * (n_fft / 2);
+    if (any_reserve(stft_complex_momentum_any_kernel, smem, what)) return 1;
+    launch_k(stft_complex_momentum_any_kernel, dim3(max_frames, nclips), ANY_THREADS, smem, (cudaStream_t)stream, wav,
+             n_samples, wav_pitch, mag, (float2*)prev, (float2*)spec, nframes, (long long)max_frames, beta, table,
+             n_fft, hop, plan);
     return check_launch(what);
 }
 

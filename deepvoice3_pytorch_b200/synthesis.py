@@ -6,8 +6,8 @@ decoder, converter) -> ``audio.inv_spectrogram``.  ``tts_batch`` runs the same f
 * encoder and converter inside an ``ops.length_scope``: every row's frames past its own length are zeroed before each
   conv that spans several frames, so each row sees the zero padding it would see alone;
 * ``incremental.decode_ragged``: per-row attention length, context scale, monotonic cursor and stopping step;
-* ``audio.inv_spectrogram_batch``: Griffin-Lim (or LWS, ``vocoder="lws"``) over a ragged batch of clips with a
-  deterministic overlap-add.
+* ``audio.inv_spectrogram_batch``: Griffin-Lim (or LWS, ``vocoder="lws"``, or fast Griffin-Lim,
+  ``vocoder="fast_griffin_lim"``) over a ragged batch of clips with a deterministic overlap-add.
 
 ``tts_stream`` runs the decoder with continuous batching instead (``incremental.decode_stream``): a fixed set of decoder
 slots, each refilled with the next waiting utterance as soon as its own one stops, so no slot idles until the longest
@@ -128,7 +128,8 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
 
     stage_timer: optional callable ``name -> context manager`` wrapped around each stage ("encoder", "decoder",
     "converter", "vocoder") of every batch, e.g. to time them.  vocoder: the phase recovery of
-    ``audio.inv_spectrogram``, "griffin_lim" (the default) or "lws" (the reference's algorithm); checked first."""
+    ``audio.inv_spectrogram``, "griffin_lim" (the default), "lws" (the reference's algorithm) or "fast_griffin_lim"
+    (Griffin-Lim with momentum); checked first."""
     audio.check_phase_method(vocoder)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     stage = stage_timer or (lambda name: contextlib.nullcontext())

@@ -246,6 +246,13 @@ int dv3_stft_complex_batched(const float* wav, const int* n_samples, long long w
                              float* spec, const int* nframes, int max_frames, int nclips, void* stream);
 int dv3_istft_batched(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
                       int max_frames, int nclips, void* stream);
+/* Fast Griffin-Lim step (Perraudin, Balazs & Sondergaard, WASPAA 2013; audio.griffin_lim_batch with momentum > 0,
+ * DESIGN.md section 7.3): the transform of dv3_stft_complex_batched, then per bin C = X - beta * prev, prev <- X (in
+ * place), spec = mag * C / |C| ((mag, 0) where C == 0).  prev has spec's layout; mag and prev are required; beta in
+ * [0, 1) (= momentum / (1 + momentum)); beta == 0 gives dv3_stft_complex_batched's projected spec bit for bit. */
+int dv3_stft_complex_momentum_batched(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
+                                      float* prev, float* spec, const int* nframes, int max_frames, int nclips,
+                                      float beta, void* stream);
 /* LWS phase recovery (csrc/lws.cu; Local Weighted Sums, the algorithm of the reference's lws.run_lws -- parity
  * UNPINNED, the package's source is absent).  mag (nframes,513) target magnitude; spec (nframes,513,2) [re,im];
  * weights: 7 x 11 complex fp32 [q+3][d+5] = beta_q(d) = (1/1024) sum_n w(n) w(n-256q) e^{-2 pi i d n/1024}
@@ -286,6 +293,10 @@ int dv3_stft_complex_geom(const float* wav, const int* n_samples, long long wav_
                           void* stream);
 int dv3_istft_geom(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
                    int max_frames, int nclips, const float* table, int n_fft, int hop, void* stream);
+/* dv3_stft_complex_momentum_batched for the geometry (K bins per frame). */
+int dv3_stft_complex_momentum_geom(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
+                                   float* prev, float* spec, const int* nframes, int max_frames, int nclips,
+                                   float beta, const float* table, int n_fft, int hop, void* stream);
 int dv3_lws_nofuture_geom(const float* mag, float* spec, const float* weights, const int* nframes, int max_frames,
                           int nclips, int init_iters, int n_fft, int hop, void* stream);
 int dv3_lws_iterate_geom(const float* mag, const float* spec_in, float* spec_out, const float* weights,
