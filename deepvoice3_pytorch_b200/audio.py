@@ -384,6 +384,69 @@ def resample_batch(wav, lengths, sr_from):
     return out, out_lens
 
 
+def input_span(n_in, seg_start, seg_len, up, down, ntaps, pre_remove):
+    """-> (start, length): the input samples that resampled outputs [seg_start, seg_start + seg_len) of an n_in-sample
+    clip read (csrc/resample.cu: output m reads x[b - j], j < ntaps, b = (m + pre_remove) * down // up), clipped to
+    [0, n_in).  (0, 0) when they read none, as an empty segment does."""
+    if seg_len <= 0:
+        return 0, 0
+    first = (seg_start + pre_remove) * down // up - (ntaps - 1)
+    end = (seg_start + seg_len - 1 + pre_remove) * down // up + 1
+    first, end = max(0, first), min(int(n_in), end)
+    return (first, end - first) if end > first else (0, 0)
+
+
+SEG_FIELDS = ("row", "n_in", "in_start", "in_len", "seg_start", "seg_len")    # dv3_resample_segments_batched's desc
+
+
+def resample_segments(wav, seg, sr_from, out, seg_dev=None):
+    """Part of each clip's ``resample_batch`` output, bit for bit, in one launch.  seg: host (nclips, 6) ints, one
+    ``SEG_FIELDS`` row per clip: row ``row`` of wav ((rows, pitch_in) int16 PCM or fp32 CUDA tensor) holds samples
+    [in_start, in_start + in_len) of a source clip of n_in samples at ``sr_from``; row ``row`` of out ((rows, pitch_out)
+    fp32 CUDA tensor) gets its resampled samples [seg_start, seg_start + seg_len) in columns [0, seg_len) and zeros after
+    them.  The row must hold ``input_span`` of the segment.  A clip at ``hparams.sample_rate`` runs the same launch with
+    the one-tap identity bank (an exact copy).  seg_dev: seg as an int32 tensor on out's device (else it is copied from
+    the host).  Every check uses host values and runs before the launch; after the first call per (rate, device) there is
+    no host synchronisation."""
+    wav = _pcm_batch(wav, "resample_segments")
+    if not (torch.is_tensor(out) and out.is_cuda and out.dtype == torch.float32 and out.dim() == 2
+            and out.is_contiguous() and out.device == wav.device):
+        raise Dv3Error("resample_segments: out must be a contiguous 2-D fp32 tensor on %s" % wav.device)
+    seg = [[int(v) for v in r] for r in (seg.tolist() if torch.is_tensor(seg) else seg)]
+    if not 1 <= len(seg) <= 65535 or any(len(r) != len(SEG_FIELDS) for r in seg):
+        raise Dv3Error("resample_segments: seg must give 1..65535 rows of %s" % (SEG_FIELDS,))
+    rows_in, pitch_in = wav.shape
+    rows_out, pitch_out = out.shape
+    up, down = resample_ratio(sr_from)
+    bank, ntaps, pre_remove = _device_bank(wav.device, up, down)
+    if len({r[0] for r in seg}) != len(seg):
+        raise Dv3Error("resample_segments: two clips share a row")
+    for row, n_in, in_start, in_len, s0, n in seg:
+        if not (0 <= row < min(rows_in, rows_out)):
+            raise Dv3Error("resample_segments: row %d is not a row of both wav and out" % row)
+        if not (n_in >= 0 and 0 <= s0 and 0 <= n <= pitch_out and s0 + n <= resampled_length(n_in, up, down)):
+            raise Dv3Error("resample_segments: segment [%d, %d) is not inside the %d outputs of an %d-sample clip (or "
+                           "longer than the %d-sample rows)" % (s0, s0 + n, resampled_length(max(n_in, 0), up, down),
+                                                                n_in, pitch_out))
+        if not (0 <= in_start and 0 <= in_len <= pitch_in and in_start + in_len <= n_in):
+            raise Dv3Error("resample_segments: input span [%d, %d) is not inside the clip (%d samples) and its row "
+                           "(%d)" % (in_start, in_start + in_len, n_in, pitch_in))
+        a, m = input_span(n_in, s0, n, up, down, ntaps, pre_remove)
+        if m and not (in_start <= a and a + m <= in_start + in_len):
+            raise Dv3Error("resample_segments: segment [%d, %d) reads input [%d, %d), the row holds [%d, %d)"
+                           % (s0, s0 + n, a, a + m, in_start, in_start + in_len))
+    if seg_dev is None:
+        seg_dev = torch.tensor(seg, dtype=torch.int32).pin_memory().to(out.device, non_blocking=True)
+    elif not (seg_dev.device == out.device and seg_dev.dtype == torch.int32 and seg_dev.is_contiguous()
+              and tuple(seg_dev.shape) == (len(seg), len(SEG_FIELDS))):
+        raise Dv3Error("resample_segments: seg_dev must be a contiguous int32 (%d, %d) tensor on %s"
+                       % (len(seg), len(SEG_FIELDS), out.device))
+    lib.call("dv3_resample_segments_batched", _cp(wav), int(wav.dtype == torch.int16), pitch_in, _cp(seg_dev),
+             len(seg), _cp(out), pitch_out, _cp(bank), up, down, ntaps, pre_remove,
+             ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
+    return out
+
+
 def trim_bounds_batch(wav, lengths, top_db, offsets=None):
     """Silence-trim bounds of a ragged batch in one launch: ``librosa.effects.trim(y, top_db)`` with the librosa
     0.6-0.9 defaults (frame 2048, hop 512, ref = max, centred frames with reflect padding) computed in fp64, where

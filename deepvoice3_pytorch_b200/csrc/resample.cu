@@ -9,6 +9,9 @@
 // bank (52.5 KB at 48 kHz -> 22.05 kHz) and the input window those outputs read are staged in shared memory once, the
 // window as fp32 (int16 read as x / 32768 and fp32 input are both exact in fp32, and exact again in fp64).  Every
 // output reads only its own clip in a fixed order, so a clip is bit-identical alone and inside any batch.
+// dv3_resample_segments_batched runs the same kernel on part of each clip's output: columns [0, seg_len) of a row get
+// outputs [seg_start, seg_start + seg_len) of the whole clip, from a row that holds only the input span those outputs
+// read (audio.input_span).  It is the training-time resampler of data.WavDataset.from_vctk.
 // Per output: ntaps fp64 FMAs against about 4.4 bytes of int16 input and 4 bytes of output at 48 -> 22.05 kHz, so the
 // kernel sits near the ridge of the H100's fp64 (34 TFLOP/s) and HBM (3.35 TB/s) roofs.
 //
@@ -26,6 +29,7 @@
 namespace dv3 {
 
 constexpr int RS_THREADS = 256, RS_TILE = 4096;             // outputs per CTA
+constexpr int RS_DESC = 6;                                  // ints per clip of a segment descriptor
 constexpr int TRIM_WARPS = 8, TRIM_FRAME = 2048, TRIM_HOP = 512, TRIM_PAD = TRIM_FRAME / 2;
 
 template <typename In> __device__ __forceinline__ float pcm(In v) {
@@ -39,42 +43,58 @@ __host__ __device__ inline int rs_window(int up, int down, int ntaps) {
     return (int)(((long long)(RS_TILE - 1) * down) / up) + 2 + ntaps;
 }
 
+// seg == NULL: clip c is row c, its whole output (lengths[c] input samples from row position 0).  Otherwise seg holds
+// RS_DESC ints per clip, {row, n_in, in_start, in_len, seg_start, seg_len}: the row (input and output) holds source
+// samples [in_start, in_start + in_len) of a clip of n_in samples, and output column k is the clip's output
+// seg_start + k for k < seg_len.  Either way an output column reads the same bank entries and input values in the same
+// order as the same absolute output of the whole clip, so its bits are those of the whole-clip output.
 template <typename In>
-__global__ void __launch_bounds__(RS_THREADS) resample_poly_kernel(const In* wav, const int* lengths, int pitch_in,
-                                                                   float* out, int pitch_out, const double* bank,
-                                                                   int up, int down, int ntaps, int pre_remove) {
+__global__ void __launch_bounds__(RS_THREADS) resample_poly_kernel(const In* wav, const int* lengths, const int* seg,
+                                                                   int pitch_in, float* out, int pitch_out,
+                                                                   const double* bank, int up, int down, int ntaps,
+                                                                   int pre_remove) {
     pdl_trigger(); pdl_wait();
     extern __shared__ __align__(16) unsigned char smem_raw[];
     double* sb = reinterpret_cast<double*>(smem_raw);
     float* win = reinterpret_cast<float*>(sb + (size_t)up * ntaps);
     const int clip = blockIdx.y, tid = threadIdx.x;
-    const long long m0 = (long long)blockIdx.x * RS_TILE;
-    const int n = lengths[clip];
-    const long long n_out = min(rs_out_len(n, up, down), (long long)pitch_out);
-    float* o = out + (size_t)clip * pitch_out;
-    const long long m_end = min(m0 + RS_TILE, (long long)pitch_out);
-    if (m0 >= n_out) {                                      // uniform: the tile lies past the clip's output
-        for (long long m = m0 + tid; m < m_end; m += RS_THREADS) o[m] = 0.f;
+    int row = clip, n, in_start = 0, in_len;
+    long long seg_start = 0, n_out;
+    if (seg) {
+        const int* d = seg + RS_DESC * clip;
+        row = d[0]; n = d[1]; in_start = d[2]; in_len = d[3]; seg_start = d[4]; n_out = d[5];
+    } else {
+        n = lengths[clip];
+        in_len = n;
+        n_out = min(rs_out_len(n, up, down), (long long)pitch_out);
+    }
+    const long long k0 = (long long)blockIdx.x * RS_TILE;   // first output column of the tile
+    float* o = out + (size_t)row * pitch_out;
+    const long long k_end = min(k0 + RS_TILE, (long long)pitch_out);
+    if (k0 >= n_out) {                                      // uniform: the tile lies past the clip's output
+        for (long long k = k0 + tid; k < k_end; k += RS_THREADS) o[k] = 0.f;
         return;
     }
-    const In* x = wav + (size_t)clip * pitch_in;
+    const In* x = wav + (size_t)row * pitch_in;             // x[s - in_start] = source sample s
+    const long long s_lo = max(in_start, 0), s_hi = min((long long)n, (long long)in_start + in_len);
+    const long long m0 = seg_start + k0;
     const long long lo = ((m0 + pre_remove) * down) / up - (ntaps - 1);
     const int nwin = rs_window(up, down, ntaps);
     for (int i = tid; i < up * ntaps; i += RS_THREADS) sb[i] = bank[i];
     for (int i = tid; i < nwin; i += RS_THREADS) {
         const long long s = lo + i;
-        win[i] = (s >= 0 && s < n) ? pcm(x[s]) : 0.f;
+        win[i] = (s >= s_lo && s < s_hi) ? pcm(x[s - in_start]) : 0.f;
     }
     __syncthreads();
-    for (long long m = m0 + tid; m < m_end; m += RS_THREADS) {
-        if (m >= n_out) { o[m] = 0.f; continue; }
-        const long long t = (m + pre_remove) * down;
+    for (long long k = k0 + tid; k < k_end; k += RS_THREADS) {
+        if (k >= n_out) { o[k] = 0.f; continue; }
+        const long long t = (seg_start + k + pre_remove) * down;
         const int p = (int)(t % up);
         const float* xw = win + (t / up - lo);               // xw[-j] = x[b - j]
         double acc = 0.0;
 #pragma unroll 4
         for (int j = 0; j < ntaps; ++j) acc = fma(sb[j * up + p], (double)xw[-j], acc);
-        o[m] = (float)acc;
+        o[k] = (float)acc;
     }
 }
 
@@ -149,10 +169,9 @@ int dv3_resample_out_len(int n_samples, int up, int down) {
     return (int)rs_out_len(n_samples, up, down);
 }
 
-int dv3_resample_poly_batched(const void* wav, int wav_int16, const int* lengths, int pitch_in, float* out,
-                              int pitch_out, int nclips, const double* bank, int up, int down, int ntaps,
-                              int pre_remove, void* stream) {
-    const char* what = "resample_poly";
+static int resample_launch(const char* what, const void* wav, int wav_int16, const int* lengths, const int* seg,
+                           int pitch_in, float* out, int pitch_out, int nclips, const double* bank, int up, int down,
+                           int ntaps, int pre_remove, void* stream) {
     DV3_REQUIRE(nclips >= 1 && nclips <= 65535, "%s: nclips %d out of range", what, nclips);
     DV3_REQUIRE(up >= 1 && down >= 1 && ntaps >= 1 && pre_remove >= 0, "%s: bad filter (up %d, down %d, ntaps %d)",
                 what, up, down, ntaps);
@@ -168,13 +187,28 @@ int dv3_resample_poly_batched(const void* wav, int wav_int16, const int* lengths
     if (wav_int16) {
         cudaFuncSetAttribute(resample_poly_kernel<short>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         launch_k(resample_poly_kernel<short>, grid, RS_THREADS, smem, st, reinterpret_cast<const short*>(wav),
-                 lengths, pitch_in, out, pitch_out, bank, up, down, ntaps, pre_remove);
+                 lengths, seg, pitch_in, out, pitch_out, bank, up, down, ntaps, pre_remove);
     } else {
         cudaFuncSetAttribute(resample_poly_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         launch_k(resample_poly_kernel<float>, grid, RS_THREADS, smem, st, reinterpret_cast<const float*>(wav),
-                 lengths, pitch_in, out, pitch_out, bank, up, down, ntaps, pre_remove);
+                 lengths, seg, pitch_in, out, pitch_out, bank, up, down, ntaps, pre_remove);
     }
     return check_launch(what);
+}
+
+int dv3_resample_poly_batched(const void* wav, int wav_int16, const int* lengths, int pitch_in, float* out,
+                              int pitch_out, int nclips, const double* bank, int up, int down, int ntaps,
+                              int pre_remove, void* stream) {
+    return resample_launch("resample_poly", wav, wav_int16, lengths, nullptr, pitch_in, out, pitch_out, nclips, bank,
+                           up, down, ntaps, pre_remove, stream);
+}
+
+int dv3_resample_segments_batched(const void* wav, int wav_int16, int pitch_in, const int* seg, int nclips, float* out,
+                                  int pitch_out, const double* bank, int up, int down, int ntaps, int pre_remove,
+                                  void* stream) {
+    DV3_REQUIRE(seg != nullptr, "resample_segments: no segment descriptors");
+    return resample_launch("resample_segments", wav, wav_int16, nullptr, seg, pitch_in, out, pitch_out, nclips, bank,
+                           up, down, ntaps, pre_remove, stream);
 }
 
 int dv3_trim_bounds_batched(const void* wav, int wav_int16, const int* lengths, const int* offsets, int pitch,

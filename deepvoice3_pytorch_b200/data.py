@@ -11,11 +11,16 @@ padding rules, and a distributed variant of its length-bucketed sampler.
 * ``WavDataset`` + ``collate_wav`` + ``wav_batch_to_device`` train from the wav files instead: the loader moves
   waveforms (int16 where the files are), and the GPU computes each batch's targets in ``collate``'s layout, bit-identical
   to ``TrainTxtDataset`` + ``collate`` over what ``preprocess.build_from_path`` writes for the same corpus.
+  ``WavDataset.from_vctk`` does the same for a VCTK tree at its recording rate: its items carry the part of each file
+  that the label cut and the silence trim keep, and the GPU resamples just that part per batch
+  (``audio.resample_segments``), bit-identical to what ``preprocess.build_vctk_from_path`` writes.
 * ``DistributedSimilarLengthSampler`` restates ``PartialyRandomizedSimilarTimeLengthSampler`` (train.py:195-239):
   sort by length, shuffle inside groups of ``batch_group_size``, permute whole mini-batches -- then deals the
   mini-batches round-robin to the ranks, so every rank sees disjoint batches of similar length (what the
   data-parallel step needs: one utterance batch per GPU, no collective on the data path).
 """
+from collections import namedtuple
+
 import numpy as np
 import torch
 
@@ -81,44 +86,104 @@ def _collate_common(batch, target_lengths, r, downsample_step, pin, spectrograms
     return out
 
 
+SegmentItem = namedtuple("SegmentItem", "text_ids pcm n_frames speaker_id sample_rate n_in in_start seg_start seg_len")
+SegmentItem.__doc__ = """A ``WavDataset.from_vctk`` item: pcm holds samples [in_start, in_start + len(pcm)) of a source clip of n_in
+samples at sample_rate (int16, or float32 for other formats), the input span of resampled samples
+[seg_start, seg_start + seg_len) at ``hparams.sample_rate`` -- the utterance's training segment, n_frames STFT frames."""
+
+
+def _pcm_rows(clips):
+    """[pcm (n,) int16 / float32] -> (B, pitch) zero-padded rows, pitch a multiple of 8 samples (16-byte rows for int16
+    and fp32 alike); int16 when every clip is int16, else float32 (int16 / 32768 is exact)."""
+    pitch = max(8, -(-max(len(w) for w in clips) // 8) * 8)
+    int16 = all(w.dtype == np.int16 for w in clips)
+    wav = np.zeros((len(clips), pitch), dtype=np.int16 if int16 else np.float32)
+    for i, w in enumerate(clips):
+        wav[i, :len(w)] = w if int16 or w.dtype != np.int16 else w.astype(np.float32) / np.float32(32768.0)
+    return torch.from_numpy(wav)
+
+
 def collate_wav(batch, r=1, downsample_step=4, pin=False):
-    """batch: list of ``WavDataset`` items (text_ids, pcm (n,) int16 or float32, n_frames[, speaker_id]).
+    """batch: list of ``WavDataset`` items (text_ids, pcm (n,) int16 or float32, n_frames[, speaker_id]), or of
+    ``SegmentItem`` (``WavDataset.from_vctk``); one batch never mixes the two (ValueError).
 
     Host-only (safe in DataLoader workers): every key of ``collate`` except "mel" and "y", computed by the same code,
     plus "wav" (B, pitch) -- the waveforms zero-padded to a pitch of a multiple of 8 samples, int16 when every clip is
     int16, else float32 (int16 / 32768 is exact) -- and "wav_lengths" (B) int32.  ``wav_batch_to_device`` computes the
-    two spectrogram targets on the GPU."""
+    two spectrogram targets on the GPU.
+
+    For ``SegmentItem`` batches "wav" holds each item's source span and "wav_lengths" its segment length; two more keys
+    describe the sources: "src_desc" (B, 6) int32, one ``audio.SEG_FIELDS`` row per item with the item's batch index
+    as its row, ordered by source rate, and "src_rates" (B) int32, the rate of each "src_desc" row."""
+    kinds = {isinstance(b, SegmentItem) for b in batch}
+    if len(kinds) > 1:
+        raise ValueError("a batch mixes WavDataset.from_vctk segment items with whole-clip items")
+    if kinds == {True}:
+        return _collate_segments(batch, r, downsample_step, pin)
     lens = [len(b[1]) for b in batch]
     for b, n in zip(batch, lens):
         if b[2] != _num_frames(n):
             raise ValueError("item has %d samples but n_frames=%d (expected %d)" % (n, b[2], _num_frames(n)))
-    pitch = max(8, -(-max(lens) // 8) * 8)                  # 16-byte rows for int16 and fp32 alike
-    int16 = all(b[1].dtype == np.int16 for b in batch)
-    wav = np.zeros((len(batch), pitch), dtype=np.int16 if int16 else np.float32)
-    for i, b in enumerate(batch):
-        w = b[1]
-        wav[i, :len(w)] = w if int16 or w.dtype != np.int16 else w.astype(np.float32) / np.float32(32768.0)
-    spectrograms = {"wav": torch.from_numpy(wav), "wav_lengths": torch.tensor(lens, dtype=torch.int32)}
+    spectrograms = {"wav": _pcm_rows([b[1] for b in batch]), "wav_lengths": torch.tensor(lens, dtype=torch.int32)}
     return _collate_common(batch, [b[2] for b in batch], r, downsample_step, pin, spectrograms)
+
+
+def _collate_segments(batch, r, downsample_step, pin):
+    for b in batch:
+        if b.n_frames != _num_frames(b.seg_len):
+            raise ValueError("segment has %d samples but n_frames=%d (expected %d)"
+                             % (b.seg_len, b.n_frames, _num_frames(b.seg_len)))
+    order = sorted(range(len(batch)), key=lambda i: (batch[i].sample_rate, i))     # one launch per source rate
+    desc = [[i, batch[i].n_in, batch[i].in_start, len(batch[i].pcm), batch[i].seg_start, batch[i].seg_len]
+            for i in order]
+    spectrograms = {"wav": _pcm_rows([b.pcm for b in batch]),
+                    "wav_lengths": torch.tensor([b.seg_len for b in batch], dtype=torch.int32),
+                    "src_desc": torch.tensor(desc, dtype=torch.int32),
+                    "src_rates": torch.tensor([batch[i].sample_rate for i in order], dtype=torch.int32)}
+    return _collate_common([(b.text_ids, None, None, b.speaker_id) for b in batch], [b.n_frames for b in batch], r,
+                           downsample_step, pin, spectrograms)
 
 
 def wav_batch_to_device(batch, device, r=1, downsample_step=4):
     """A ``collate_wav`` batch -> the dict ``collate`` + ``train_step.to_device`` give for the same utterances after
-    ``preprocess.build_from_path``, bit for bit: asynchronous H2D copies (pin the batch for them to overlap), then
-    the targets in one launch on the current stream (``audio.stft_mel_targets``; the peak pass first when
-    ``hparams.rescaling`` is on).  No host synchronisation."""
+    ``preprocess.build_from_path`` (``preprocess.build_vctk_from_path`` for ``WavDataset.from_vctk`` items), bit for
+    bit: asynchronous H2D copies (pin the batch for them to overlap), for segment items one
+    ``audio.resample_segments`` launch per source rate, then the targets in one launch on the current stream
+    (``audio.stft_mel_targets``; the peak pass first when ``hparams.rescaling`` is on).  No host synchronisation."""
     from . import audio
     out = {}
     for k, v in batch.items():
-        if k in ("wav", "wav_lengths"):
+        if k in ("wav", "wav_lengths", "src_desc", "src_rates"):
             continue
         out[k] = v.to(device, non_blocking=True) if torch.is_tensor(v) else v
     wav = batch["wav"].to(device, non_blocking=True)
+    if "src_desc" in batch:
+        wav = _resample_rows(wav, batch)
     lens_dev = batch["wav_lengths"].to(device, non_blocking=True)
     T_lin = max_target_length(batch["target_lengths"].tolist(), r, downsample_step)
     y, mel = audio.stft_mel_targets(wav, batch["wav_lengths"], T_lin, r, downsample_step, lengths_dev=lens_dev)
     order = ("x", "text_positions", "frame_positions")
     return {**{k: out[k] for k in order}, "mel": mel, "y": y, **{k: v for k, v in out.items() if k not in order}}
+
+
+def _resample_rows(src, batch):
+    """The segments of a ``SegmentItem`` batch at ``hparams.sample_rate`` from its source spans ``src`` (on the
+    device): (B, pitch) fp32, pitch as ``collate_wav`` pads, one launch per rate."""
+    from . import audio
+    lens = batch["wav_lengths"].tolist()
+    desc, rates = batch["src_desc"].tolist(), batch["src_rates"].tolist()
+    if sorted(d[0] for d in desc) != list(range(len(lens))) or len(rates) != len(desc):
+        raise ValueError("src_desc must give one row per item of the batch")
+    out = torch.empty(len(lens), max(8, -(-max(lens) // 8) * 8), device=src.device)     # every row is written
+    desc_dev = batch["src_desc"].to(src.device, non_blocking=True)
+    g0 = 0
+    while g0 < len(desc):
+        g1 = g0 + 1
+        while g1 < len(desc) and rates[g1] == rates[g0]:
+            g1 += 1
+        audio.resample_segments(src, desc[g0:g1], rates[g0], out, seg_dev=desc_dev[g0:g1])
+        g0 = g1
+    return out
 
 
 def _num_frames(n_samples):
@@ -272,7 +337,7 @@ class WavDataset(torch.utils.data.Dataset):
             self.multi_speaker = False
         self.items, self.text_to_sequence = items, text_to_sequence
         self.sample_rate = hparams.sample_rate
-        self.frame_lengths = []
+        self.frame_lengths, self._segments = [], None
         self._native = []                    # 16-bit mono at the training rate: returned as int16 without conversion
         for it in items:
             sr, n_samples, channels, dtype = _wav_header(it[0])
@@ -297,11 +362,47 @@ class WavDataset(torch.utils.data.Dataset):
                 items.append((os.path.join(in_dir, "wavs", "%s.wav" % parts[0]), text))
         return cls(items, text_to_sequence)
 
+    @classmethod
+    def from_vctk(cls, in_dir, text_to_sequence, speakers=None, index_path=None, batch_clips=64):
+        """The rows ``preprocess.build_vctk_from_path(in_dir, ..., speakers=speakers)`` writes, straight from the wav48
+        files: item i is a ``SegmentItem`` of row i (same order, texts and speaker ids; an utterance whose trimmed
+        segment is empty has no row).  Its segment comes from one indexing pass at construction that resamples
+        whole clips, cuts them to the labels and trims them on the GPU (``preprocess.segment_bounds``, ``batch_clips``
+        clips per set of launches); ``frame_lengths`` is train.txt's n_frames column.  Under an initialised
+        ``torch.distributed`` the pass is dealt round-robin over the ranks and merged with one ``all_gather_object``.
+
+        index_path: a ``.npz`` file that caches the index, keyed by every wav's and label's path, size and mtime, by
+        ``hparams.sample_rate`` and by a format version.  It is used only when its key matches (otherwise the pass runs
+        again) and written by rank 0 after a pass."""
+        from .audio import hparams
+        from . import preprocess
+        utts = preprocess.vctk_utterances(in_dir, speakers)
+        if not utts:
+            raise ValueError("no VCTK utterances under %s" % in_dir)
+        key = _vctk_index_key(utts, hparams.sample_rate)
+        index = _read_vctk_index(index_path, key, [u[0] for u in utts]) if index_path else None
+        if index is None:
+            index, rank = _vctk_index(utts, batch_clips)
+            if index_path and rank == 0:
+                _write_vctk_index(index_path, key, index)
+        ds = cls.__new__(cls)
+        ds.text_to_sequence, ds.sample_rate, ds.multi_speaker = text_to_sequence, hparams.sample_rate, True
+        ds.items, ds._segments, ds.frame_lengths = [], [], []
+        for (_, (wav, _), (text, spk)), (sr, n_in, is16, s0, n) in zip(utts, index[:, 1:].tolist()):
+            if n == 0:
+                continue
+            ds.items.append((wav, text, spk))
+            ds._segments.append((sr, n_in, bool(is16), s0, n) + segment_span(n_in, s0, n, sr))
+            ds.frame_lengths.append(_num_frames(n))
+        return ds
+
     def __len__(self):
         return len(self.items)
 
     def __getitem__(self, idx):
         it = self.items[idx]
+        if self._segments is not None:
+            return self._segment_item(idx)
         if self._native[idx]:
             from scipy.io import wavfile
             pcm = np.array(wavfile.read(it[0], mmap=True)[1], dtype=np.int16)
@@ -311,6 +412,106 @@ class WavDataset(torch.utils.data.Dataset):
         seq = np.asarray(self.text_to_sequence(it[1]), dtype=np.int32)
         item = (seq, pcm, self.frame_lengths[idx])
         return item + (int(it[2]),) if self.multi_speaker else item
+
+
+    def _segment_item(self, idx):
+        wav_path, text, spk = self.items[idx]
+        sr, n_in, is16, s0, n, a, m = self._segments[idx]
+        if is16:                                  # memory-mapped: only the pages of the span are read
+            from scipy.io import wavfile
+            pcm = np.array(wavfile.read(wav_path, mmap=True)[1][a:a + m], dtype=np.int16)
+        else:
+            from .audio import decode_wav
+            pcm = np.ascontiguousarray(decode_wav(wav_path)[1][a:a + m], dtype=np.float32)
+        seq = np.asarray(self.text_to_sequence(text), dtype=np.int32)
+        return SegmentItem(seq, pcm, self.frame_lengths[idx], int(spk), sr, n_in, a, s0, n)
+
+
+def segment_span(n_in, seg_start, seg_len, sr_from):
+    """-> (start, length) of the input samples that resampling an n_in-sample clip from sr_from to
+    ``hparams.sample_rate`` reads for output samples [seg_start, seg_start + seg_len) (``audio.input_span`` with the
+    filter of that rate pair): what a ``SegmentItem`` carries."""
+    from . import audio
+    up, down = audio.resample_ratio(sr_from)
+    ntaps, pre_remove = _host_bank(up, down)
+    return audio.input_span(n_in, seg_start, seg_len, up, down, ntaps, pre_remove)
+
+
+_host_banks = {}
+
+
+def _host_bank(up, down):
+    """(ntaps, pre_remove) of ``audio.resample_filter_bank(up, down)``, cached (the design runs firwin)."""
+    if (up, down) not in _host_banks:
+        from .audio import resample_filter_bank
+        bank, pre_remove = resample_filter_bank(up, down)
+        _host_banks[(up, down)] = (bank.shape[0], pre_remove)
+    return _host_banks[(up, down)]
+
+
+VCTK_INDEX_VERSION = 1
+
+
+def _vctk_index_key(utts, sample_rate):
+    """sha256 over the index format version, the target rate, and every wav's and label's absolute path, size and
+    mtime, in walk order."""
+    import hashlib
+    import os
+    h = hashlib.sha256(("dv3-vctk-index|%d|%d\n" % (VCTK_INDEX_VERSION, int(sample_rate))).encode())
+    for idx, paths, _ in utts:
+        for p in paths:
+            if p is None:
+                h.update(b"-\n")
+                continue
+            st = os.stat(p)
+            h.update(("%d|%s|%d|%d\n" % (idx, os.path.abspath(p), st.st_size, st.st_mtime_ns)).encode("utf-8"))
+    return h.hexdigest()
+
+
+def _vctk_index(utts, batch_clips):
+    """The indexing pass -> ((n, 6) int64 rows [file index, source rate, n_in, int16, seg_start, seg_len] in walk
+    order, this process's rank)."""
+    import torch.distributed as dist
+    from . import preprocess
+    world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
+    rank = dist.get_rank() if world > 1 else 0
+    mine = utts[rank::world]
+    rows = []
+    for i in range(0, len(mine), batch_clips):
+        batch = mine[i:i + batch_clips]
+        clips = [preprocess._load_vctk(src) for _, src, _ in batch]
+        for (idx, _, _), (pcm, sr, _), (s0, n) in zip(batch, clips, preprocess.segment_bounds(clips)):
+            rows.append((idx, sr, len(pcm), int(pcm.dtype == np.int16), s0, n))
+    if world > 1:
+        parts = [None] * world
+        dist.all_gather_object(parts, rows)
+        rows = [r for part in parts for r in part]
+    return np.array(sorted(rows), dtype=np.int64).reshape(-1, 6), rank
+
+
+def _read_vctk_index(path, key, file_indices):
+    """The cached index at path when it exists, is readable and its key and file indices match; else None."""
+    import os
+    if not os.path.exists(path):
+        return None
+    try:
+        with np.load(path, allow_pickle=False) as z:
+            if str(z["key"]) != key:
+                return None
+            index = np.asarray(z["index"], dtype=np.int64)
+    except (OSError, ValueError, KeyError):
+        return None
+    if index.shape != (len(file_indices), 6) or index[:, 0].tolist() != list(file_indices):
+        return None
+    return index
+
+
+def _write_vctk_index(path, key, index):
+    import os
+    tmp = "%s.%d.tmp" % (path, os.getpid())
+    with open(tmp, "wb") as f:
+        np.savez(f, key=np.array(key), index=index)
+    os.replace(tmp, path)
 
 
 class DistributedSimilarLengthSampler(torch.utils.data.Sampler):

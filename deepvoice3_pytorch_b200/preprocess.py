@@ -213,14 +213,12 @@ def _host_buffer(clips):
     return host
 
 
-def resample_trim_batch(clips):
-    """The GPU stages of VCTK preprocessing for one batch.  clips: [(pcm int16 / float32, sample rate, label cut or
-    None)] -> [trimmed float32 segment] (possibly empty): one H2D copy per input dtype, then per source rate one
-    ``audio.resample_batch`` launch (files already at ``hparams.sample_rate`` skip it), one ``audio.trim_bounds_batch``
-    launch on [cut] with top_db 25 or, without labels, on the whole clip with top_db 15, one readback of the
-    resampled audio and the bounds, and the segments sliced on the host."""
+def _resample_trim_launch(clips):
+    """The launches of ``resample_trim_batch`` and ``segment_bounds``: one H2D copy per input dtype, then per source rate
+    one ``audio.resample_batch`` launch (files already at ``hparams.sample_rate`` skip it) and one
+    ``audio.trim_bounds_batch`` launch on [cut] with top_db 25 or, without labels, on the whole clip with top_db 15.
+    -> [(clip indices, cut offsets, resampled batch or None, bounds on the device)], nothing read back yet."""
     sr_to = audio.hparams.sample_rate
-    out = [None] * len(clips)
     pending = []
     for is16 in (True, False):
         rows = sorted((i for i, c in enumerate(clips) if (c[0].dtype == np.int16) == is16), key=lambda i: clips[i][1])
@@ -249,7 +247,27 @@ def resample_trim_batch(clips):
             bounds = audio.trim_bounds_batch(src, segs, tops, offs)
             pending.append((group, offs, src if resampled else None, bounds))
             r0 = r1
-    for group, offs, src, bounds in pending:
+    return pending
+
+
+def segment_bounds(clips):
+    """clips as in ``resample_trim_batch`` -> [(start, length)] of each trimmed segment in samples of the clip
+    resampled to ``hparams.sample_rate`` (length 0: an empty segment): the same launches, reading back only the
+    bounds.  ``data.WavDataset.from_vctk`` indexes a corpus with it."""
+    out = [None] * len(clips)
+    for group, offs, _, bounds in _resample_trim_launch(clips):
+        bounds = bounds.cpu().numpy()
+        for k, (i, off) in enumerate(zip(group, offs)):
+            out[i] = (off + int(bounds[k, 0]), int(bounds[k, 1]) - int(bounds[k, 0]))
+    return out
+
+
+def resample_trim_batch(clips):
+    """The GPU stages of VCTK preprocessing for one batch.  clips: [(pcm int16 / float32, sample rate, label cut or
+    None)] -> [trimmed float32 segment] (possibly empty): the launches of ``_resample_trim_launch``, one readback of the
+    resampled audio and the bounds, and the segments sliced on the host."""
+    out = [None] * len(clips)
+    for group, offs, src, bounds in _resample_trim_launch(clips):
         bounds = bounds.cpu().numpy()
         src = None if src is None else src.cpu().numpy()
         for k, (i, off) in enumerate(zip(group, offs)):

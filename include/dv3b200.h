@@ -216,11 +216,22 @@ int dv3_peak_abs_batched(const void* wav, int wav_int16, const int* lengths, int
  * dv3_trim_bounds_batched: librosa.effects.trim(y, top_db[c]) (frame 2048, hop 512, ref = max, centred frames,
  * reflect padding; the librosa 0.6-0.9 defaults) of y = clip c's samples [offsets[c], offsets[c] + lengths[c]), in
  * fp64 -> bounds (nclips, 2) int32 (start, end) relative to y, (0, 0) when no frame is above the threshold.  wav as
- * above with row pitch `pitch`; offsets may be NULL (all 0); top_db fp64 [nclips].  No host synchronisation. */
+ * above with row pitch `pitch`; offsets may be NULL (all 0); top_db fp64 [nclips].  No host synchronisation.
+ * dv3_resample_segments_batched: part of dv3_resample_poly_batched's output for each of nclips clips, bit for bit.
+ * seg int32 (nclips, 6) = {row, n_in, in_start, in_len, seg_start, seg_len} per clip: row `row` of wav (pitch_in, fp32
+ * or int16 as above) holds samples [in_start, in_start + in_len) of a source clip of n_in samples (0 <= in_start,
+ * in_start + in_len <= n_in, in_len <= pitch_in); row `row` of out (pitch_out fp32) gets the clip's resampled samples
+ * [seg_start, seg_start + seg_len) in columns [0, seg_len) and zeros after them.  The caller keeps seg_start +
+ * seg_len <= dv3_resample_out_len(n_in), seg_len <= pitch_out, the rows distinct, and [in_start, in_start + in_len)
+ * covering every input sample the segment reads (audio.input_span): the kernel reads nothing else, and a sample
+ * outside the row counts as 0.  up = down = 1 with the one-tap bank {1.0} copies (int16 as x / 32768). */
 int dv3_resample_out_len(int n_samples, int up, int down);
 int dv3_resample_poly_batched(const void* wav, int wav_int16, const int* lengths, int pitch_in, float* out,
                               int pitch_out, int nclips, const double* bank, int up, int down, int ntaps,
                               int pre_remove, void* stream);
+int dv3_resample_segments_batched(const void* wav, int wav_int16, int pitch_in, const int* seg, int nclips, float* out,
+                                  int pitch_out, const double* bank, int up, int down, int ntaps, int pre_remove,
+                                  void* stream);
 int dv3_trim_bounds_batched(const void* wav, int wav_int16, const int* lengths, const int* offsets, int pitch,
                             int nclips, const double* top_db, int* bounds, void* stream);
 
