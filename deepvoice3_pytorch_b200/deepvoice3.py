@@ -9,7 +9,6 @@ import math
 
 import torch
 from torch import nn
-from torch.nn import functional as F
 
 from . import ops
 from .modules import (Conv1d, ConvTranspose1d, Embedding, Linear, SinusoidalEncoding, Conv1dGLU,
@@ -83,14 +82,14 @@ class Encoder(nn.Module):
         x = ops.dropout(x, self.dropout, self.training)
         speaker_embed_btc = expand_speaker_embed(x, speaker_embed)
         if speaker_embed_btc is not None:
-            speaker_embed_btc = ops.dropout(speaker_embed_btc, self.dropout, self.training)
-            x = x + F.softsign(self.speaker_fc1(speaker_embed_btc))
+            speaker_embed_btc = ops.speaker_dropout(speaker_embed_btc, self.dropout, self.training)
+            x = ops.speaker_residual(x, self.speaker_fc1, speaker_embed_btc)
         input_embedding = x
         x = run_conv_stack(self.convolutions, ops.transpose12(x), speaker_embed_btc,
                            boundaries={i: tag for tag, i in self.grad_bucket_splits()})
         keys = ops.transpose12(x)
         if speaker_embed_btc is not None:
-            keys = keys + F.softsign(self.speaker_fc2(speaker_embed_btc))
+            keys = ops.speaker_residual(keys, self.speaker_fc2, speaker_embed_btc)
         values = (keys + input_embedding) * SQRT_HALF
         return keys, values
 
@@ -214,7 +213,7 @@ class Decoder(nn.Module):
 
         speaker_embed_btc = expand_speaker_embed(inputs, speaker_embed)
         if speaker_embed_btc is not None:
-            speaker_embed_btc = ops.dropout(speaker_embed_btc, self.dropout, self.training)
+            speaker_embed_btc = ops.speaker_dropout(speaker_embed_btc, self.dropout, self.training)
 
         keys, values = encoder_out
         mask = get_mask_from_lengths(keys, lengths) if (self.use_memory_mask and lengths is not None) else None
@@ -330,7 +329,7 @@ class Converter(nn.Module):
                 j += 1
             spk = expand_speaker_embed(x, speaker_embed, tdim=-1)
             if spk is not None:
-                spk = ops.dropout(spk, self.dropout, self.training)
+                spk = ops.speaker_dropout(spk, self.dropout, self.training)
             x = run_conv_stack(layers[i:j], x, spk)
             i = j
         return torch.sigmoid(ops.transpose12(x))

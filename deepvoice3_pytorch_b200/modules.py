@@ -144,13 +144,17 @@ class Conv1dGLU(_GatedConv):
         fuse_residual=True computes (block(x) + x)*sqrt(.5) in the kernel even when the module was built with
         residual=False -- the decoder applies exactly that outside the block when no attention layer sits in between
         (reference deepvoice3.py:333-349).  extent: ``ops.extent_frames(x)`` inside a bucketed training batch."""
-        spk = None
+        spk = site = None
         if self.speaker_proj is not None:
-            spk = F.softsign(self.speaker_proj.forward_bct(ops.transpose12(speaker_embed)))
+            if ops.speaker_adapt is not None:       # embedding-only adaptation: the collapsed site backward
+                spk, site = ops.speaker_adapt.block_site(self.speaker_proj, speaker_embed)
+            else:
+                spk = F.softsign(self.speaker_proj.forward_bct(ops.transpose12(speaker_embed)))
         c = self.conv
         residual = self.residual if fuse_residual is None else bool(fuse_residual)
         return ops.convblock(x, c.weight_v, c.weight_g, c.bias, spk, c.kernel_size[0], c.dilation[0],
-                             self.causal, ops.MODE_GLU, residual, self.dropout, self.training, extent=extent)
+                             self.causal, ops.MODE_GLU, residual, self.dropout, self.training, extent=extent,
+                             site=site)
 
 
     def incremental_forward(self, x, speaker_embed=None):

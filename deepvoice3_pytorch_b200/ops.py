@@ -203,16 +203,121 @@ def _drop_args(p, training, device):
 # ----------------------------------------------------------------------------------------------
 # weight-norm packing helpers
 # ----------------------------------------------------------------------------------------------
-def _wn_conv_fwd(v, g):
-    """v (Cout, Cin, k), g (Cout,1,1) -> w_f [k][Cin][Cout], w_b [k][Cout][Cin], inv_norm [Cout]."""
+def _wn_conv_fwd(v, g, out=None):
+    """v (Cout, Cin, k), g (Cout,1,1) -> w_f [k][Cin][Cout], w_b [k][Cout][Cin], inv_norm [Cout] (+ the scale buffer
+    when ``out`` -- a previous result to refold into -- is given)."""
     Cout, Cin, k = v.shape
-    w_f = torch.empty(k, Cin, Cout, device=v.device, dtype=torch.float32)
-    w_b = torch.empty(k, Cout, Cin, device=v.device, dtype=torch.float32)
-    inv = torch.empty(Cout, device=v.device, dtype=torch.float32)
-    scale = torch.empty_like(inv)
+    if out is None:
+        w_f = torch.empty(k, Cin, Cout, device=v.device, dtype=torch.float32)
+        w_b = torch.empty(k, Cout, Cin, device=v.device, dtype=torch.float32)
+        inv = torch.empty(Cout, device=v.device, dtype=torch.float32)
+        scale = torch.empty_like(inv)
+    else:
+        w_f, w_b, inv, scale = out
     lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cout, Cin, k,
              1, Cout, Cin * Cout, Cin, 1, Cout * Cin, _stream())
-    return w_f, w_b, inv
+    return (w_f, w_b, inv) if out is None else out
+
+
+def _fp32_weights(v, g):
+    """-> (w_f, w_b, inv) of _wn_conv_fwd, from the frozen-weight cache when it holds the layer."""
+    fz = _frozen("fp32", v, g)
+    return fz[:3] if fz is not None else _wn_conv_fwd(v, g)
+
+
+def _tc_fold(v, g, npl, out=None):
+    """Per-layer tensor-core weight norm on the current stream -> (inv, wfwd, wbwd, scale) (see _tc_weights)."""
+    Cout, Cin, k = v.shape
+    dev = v.device
+    if out is None:
+        inv = torch.empty(Cout, device=dev)
+        out = (inv, torch.empty(npl, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16),
+               torch.empty(npl, k, Cin, _pad8(Cout), device=dev, dtype=torch.bfloat16), torch.empty_like(inv))
+    inv, wfwd, wbwd, scale = out
+    lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cout, Cin, k,
+             _stream())
+    return out
+
+
+def _convt_tc_fold(v, g, npl, out=None):
+    """Tensor-core weight norm of a ConvTranspose1d(k=2, s=2) v (Cin, Cout, 2) -> (inv, wfwd, wbwd, scale)."""
+    Cin, Cout = v.shape[0], v.shape[1]
+    dev = v.device
+    if out is None:
+        inv = torch.empty(Cin, device=dev)
+        out = (inv, torch.empty(npl, 2 * Cout, _pad8(Cin), device=dev, dtype=torch.float16),
+               torch.empty(npl, Cin, _pad8(2 * Cout), device=dev, dtype=torch.bfloat16), torch.empty_like(inv))
+    inv, wfwd, wbwd, scale = out
+    lib.call("dv3_tc_weightnorm_convt_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cin, Cout,
+             _stream())
+    return out
+
+
+def _convt_fp32_fold(v, g, out=None):
+    """Exact-fp32 weight norm of a ConvTranspose1d(k=2, s=2) -> (w_f [ci][(j,co)], w_b [(j,co)][ci], inv, scale)."""
+    Cin, Cout = v.shape[0], v.shape[1]
+    dev = v.device
+    if out is None:
+        inv = torch.empty(Cin, device=dev, dtype=torch.float32)
+        out = (torch.empty(Cin, 2 * Cout, device=dev, dtype=torch.float32),
+               torch.empty(2 * Cout, Cin, device=dev, dtype=torch.float32), inv, torch.empty_like(inv))
+    w_f, w_b, inv, scale = out
+    lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cin, Cout, 2,
+             2 * Cout, 1, Cout, 1, Cin, Cout * Cin, _stream())
+    return out
+
+
+_FOLDS = {"fp32": lambda v, g, npl, out: _wn_conv_fwd(v, g, out if out is not None else
+                                                      _wn_conv_fwd_buffers(v)),
+          "tc": _tc_fold, "convt_tc": _convt_tc_fold, "convt_fp32": lambda v, g, npl, out: _convt_fp32_fold(v, g, out)}
+
+
+def _wn_conv_fwd_buffers(v):
+    Cout, Cin, k = v.shape
+    inv = torch.empty(Cout, device=v.device, dtype=torch.float32)
+    return (torch.empty(k, Cin, Cout, device=v.device, dtype=torch.float32),
+            torch.empty(k, Cout, Cin, device=v.device, dtype=torch.float32), inv, torch.empty_like(inv))
+
+
+class FrozenWeights:
+    """Weight norm and operand planes of layers whose parameters take no gradient, folded once and reused by every
+    pass (installed as ``ops.frozen_weights`` by an embedding-only ``TrainStep(adapt_speakers=...)``).  A layer is
+    folded the first time a Function sees it -- in an eager pass, never inside a CUDA-graph capture -- into persistent
+    buffers; ``refresh()`` refolds every layer in place (the buffers keep their addresses, so captured graphs stay
+    valid), and ``stale()`` tells from the parameters' version counters whether one was written since its fold."""
+
+    def __init__(self):
+        self.entries = {}           # (kind, v.data_ptr(), v.shape, npl) -> [v, g, npl, buffers, versions]
+
+    def get(self, kind, v, g, npl=0):
+        key = (kind, v.data_ptr(), tuple(v.shape), npl)
+        e = self.entries.get(key)
+        if e is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise Dv3Error("frozen weights: layer %s first seen during a CUDA-graph capture (warm up first)"
+                               % (tuple(v.shape),))
+            bufs = _FOLDS[kind](v, g, npl, None)
+            e = self.entries[key] = [kind, v, g, npl, bufs, (v._version, g._version)]
+        return e[4]
+
+    def stale(self):
+        return any((v._version, g._version) != ver for _, v, g, _, _, ver in self.entries.values())
+
+    def refresh(self):
+        for e in self.entries.values():
+            kind, v, g, npl, bufs, _ = e
+            _FOLDS[kind](v, g, npl, bufs)
+            e[5] = (v._version, g._version)
+
+
+frozen_weights = None
+
+
+def _frozen(kind, v, g, npl=0):
+    """Cached fold of a frozen layer (``frozen_weights`` installed and neither parameter takes a gradient), or None."""
+    if frozen_weights is None or v.requires_grad or g.requires_grad:
+        return None
+    return frozen_weights.get(kind, v, g, npl)
 
 
 # Gradient sink (set by train_step.TrainStep): parameter gradients are accumulated by the kernels straight into the
@@ -287,11 +392,11 @@ def _gate_addend(mode, residual, dy, s):
 
 class _ConvBlockFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training):
+    def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training, site, anchor):
         _chk(x, v, g, bias, spk)
         B, C, T = x.shape
         assert v.shape == (2 * C, C, k), "ConvBlock needs in_channels == out_channels"
-        w_f, w_b, inv = _wn_conv_fwd(v, g)
+        w_f, w_b, inv = _fp32_weights(v, g)
         p, seed_t, salt = _drop_args(p_drop, training, x.device)
         seed_ptr = _p(seed_t)
         need_bwd = any(ctx.needs_input_grad)
@@ -305,6 +410,7 @@ class _ConvBlockFn(torch.autograd.Function):
             ctx.cfg = (k, dilation, causal, mode, residual, p, salt, spk is not None, x.device)
             ctx.seed_t = seed_t
             ctx.det = is_deterministic()
+            ctx.site = site
         return y
 
     @staticmethod
@@ -333,7 +439,9 @@ class _ConvBlockFn(torch.autograd.Function):
             partials, nsplit = _wgrad_conv(dab, x, v.shape, k, dilation, causal, p, seed_ptr, salt)
             dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
         dspk = dab[:, :C, :] if has_spk and ctx.needs_input_grad[4] else None
-        return dx, dv, dg, dbias, dspk, None, None, None, None, None, None, None
+        if ctx.site is not None:            # speaker adaptation: d_e from the "a" half of the gate gradient
+            ctx.site.grad_bct(dab, 2 * C * T)
+        return dx, dv, dg, dbias, dspk, None, None, None, None, None, None, None, None, None
 
 
 # The weight-gradient GEMM (+ the weight-norm backward that consumes it) and the data-gradient GEMM of a block are
@@ -383,6 +491,9 @@ def _tc_weights(v, g, npl):
     bank = weight_bank.weights_for(v, g, npl) if weight_bank is not None else None   # planes prepared for this step?
     if bank is not None:
         return bank.inv, bank.wfwd, bank.wbwd, bank, None
+    fz = _frozen("tc", v, g, npl)
+    if fz is not None:
+        return fz[0], fz[1], fz[2], None, None
     Cout, Cin, k = v.shape
     dev = v.device
     inv = torch.empty(Cout, device=dev)
@@ -406,7 +517,8 @@ class _TCWeightGrad:
     def __init__(self, ctx, v, g):
         self.ctx, self.v, self.g = ctx, v, g
         self.sink = _sink(v, g, ctx.bias_param) if ctx.bias_param is not None else None
-        self.dbias = self.sink[2] if self.sink else torch.zeros(v.shape[0], device=v.device)
+        self.dbias = self.sink[2] if self.sink else torch.zeros(v.shape[0], device=v.device) \
+            if ctx.needs_input_grad[3] else None          # a frozen bias: no bias gradient at all
         self.side = self.dv = self.dg = self.partials = None
 
     def start(self, d_planes, x_wg, inv, B, T, dilation, causal, npl):
@@ -444,17 +556,18 @@ class _ConvBlockTCFn(torch.autograd.Function):
     forward GEMM, bf16 in the gradient GEMMs)."""
 
     @staticmethod
-    def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training, extent):
+    def forward(ctx, x, v, g, bias, spk, k, dilation, causal, mode, residual, p_drop, training, extent, site, anchor):
         _chk(x, v, g, bias, spk)
         B, C, T = x.shape
         dev = x.device
         bf = torch.bfloat16
         npl = _npl()
         need_bwd = any(ctx.needs_input_grad)
+        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
         p, seed_t, salt = _drop_args(p_drop, training, dev)
         inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl)
         x_btc = torch.empty(npl, B, T, C, device=dev, dtype=torch.float16)        # forward operand (fp16)
-        x_wg = torch.empty(npl, B, T, C, device=dev, dtype=bf) if need_bwd else None  # weight-gradient operand
+        x_wg = torch.empty(npl, B, T, C, device=dev, dtype=bf) if need_w else None  # weight-gradient operand
         seed_ptr = _p(seed_t)
         y = torch.empty_like(x)
         a = torch.empty_like(x) if need_bwd else None
@@ -478,6 +591,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
             ctx.extent = extent
             ctx.npl = npl
             ctx.det = is_deterministic()
+            ctx.site = site
         return y
 
     @staticmethod
@@ -492,13 +606,15 @@ class _ConvBlockTCFn(torch.autograd.Function):
         wg = _TCWeightGrad(ctx, v, g)
         # the gradient past the extent is taken as 0 (see ops.extent_frames)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
-        if ctx.det:
+        if ctx.det and wg.dbias is not None:
             lib.call("dv3_tc_gate_bwd_split_det", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), npl, _p(wg.dbias),
                      *_bias_scratch(B, 2 * C, T, True, dev), B, C, T, mode, int(residual), ext_p, ext_m, _stream())
         else:
             lib.call("dv3_tc_gate_bwd_split_npl", _p(dy), _p(a), _p(s), _p(x), _p(d_btc), npl, None, _p(wg.dbias), B,
                      C, T, mode, int(residual), ext_p, ext_m, _stream())
         wg.start(d_btc, x_wg, inv, B, T, dilation, causal, npl)
+        if ctx.site is not None:            # speaker adaptation: d_e straight from the "a" half of the planes
+            ctx.site.grad_planes(d_btc, npl)
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty_like(x)
@@ -512,7 +628,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
             if npl == 2:
                 da = da + d_btc[1, :, :, :C].float() * (1.0 / 2048.0)
             dspk = transpose12(da.contiguous())
-        return (dx, dv, dg, dbias, dspk) + (None,) * 8
+        return (dx, dv, dg, dbias, dspk) + (None,) * 10
 
 
 class _Conv1dTCFn(torch.autograd.Function):
@@ -562,7 +678,7 @@ class _Conv1dTCFn(torch.autograd.Function):
         g_btc = torch.empty(npl, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
         wg = _TCWeightGrad(ctx, v, g)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
-        if ctx.det:
+        if ctx.det and wg.dbias is not None:
             lib.call("dv3_tc_grad_split_det", _p(dy), _p(y), _p(g_btc), npl, _p(wg.dbias),
                      *_bias_scratch(B, Cout, T, True, dev), B, Cout, T, int(relu), ext_p, ext_m, _stream())
         else:
@@ -589,14 +705,10 @@ class _ConvT2TCFn(torch.autograd.Function):
         dev, bf = x.device, torch.bfloat16
         Cinp, K2p = _pad8(Cin), _pad8(2 * Cout)
         npl = _npl()
-        inv = torch.empty(Cin, device=dev)
-        scale = torch.empty_like(inv)
-        wfwd = torch.empty(npl, 2 * Cout, Cinp, device=dev, dtype=torch.float16)
-        wbwd = torch.empty(npl, Cin, K2p, device=dev, dtype=bf)
-        lib.call("dv3_tc_weightnorm_convt_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cin,
-                 Cout, _stream())
+        inv, wfwd, wbwd, _ = _frozen("convt_tc", v, g, npl) or _convt_tc_fold(v, g, npl)
         x_btc = torch.empty(npl, B, T, Cinp, device=dev, dtype=torch.float16)
-        x_wg = torch.empty(npl, B, T, Cinp, device=dev, dtype=bf)
+        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+        x_wg = torch.empty(npl, B, T, Cinp, device=dev, dtype=bf) if need_w else None
         lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, 1, 1, 0, 0.0, None, 0,
                  _stream())
         bias2 = bias.repeat(2)
@@ -623,15 +735,15 @@ class _ConvT2TCFn(torch.autograd.Function):
         dyp = torch.empty(B, 2 * Cout, T, device=dev)
         lib.call("dv3_interleave2", _p(dy), _p(dyp), B, Cout, T, 1, _stream())
         g_btc = torch.empty(npl, B, T, K2p, device=dev, dtype=bf)
-        db2 = torch.zeros(2 * Cout, device=dev)
+        db2 = torch.zeros(2 * Cout, device=dev) if ctx.needs_input_grad[3] else None
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)     # dyp is in the input's time units
-        if ctx.det:
+        if ctx.det and db2 is not None:
             lib.call("dv3_tc_grad_split_det", _p(dyp), None, _p(g_btc), npl, _p(db2),
                      *_bias_scratch(B, 2 * Cout, T, True, dev), B, 2 * Cout, T, 0, ext_p, ext_m, _stream())
         else:
             lib.call("dv3_tc_grad_split_npl", _p(dyp), None, _p(g_btc), npl, None, _p(db2), B, 2 * Cout, T, 0, ext_p,
                      ext_m, _stream())
-        dbias = db2[:Cout] + db2[Cout:]
+        dbias = db2[:Cout] + db2[Cout:] if db2 is not None else None
         dx = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(B, Cin, T, device=dev)
@@ -691,18 +803,21 @@ def tc_supported(B, C, T, k):
 
 
 def convblock(x, v, g, bias, spk=None, k=3, dilation=1, causal=False, mode=MODE_GLU, residual=True,
-              p_drop=0.0, training=False, extent=None):
+              p_drop=0.0, training=False, extent=None, site=None):
     """Fused weight-normed dilated conv + gate.  x (B,C,T); v (2C,C,k); g (2C,1,1); bias (2C);
     spk (B,C,T) already softsign'ed (or None).  extent (``extent_frames``): frames past it are taken as 0 in the conv
-    input (k > 1) and in the incoming gradient."""
+    input (k > 1) and in the incoming gradient.  site: a speaker-adaptation site (speaker_adapt.Site) whose embedding
+    gradient the backward adds from the block's gate gradient; spk then takes no gradient of its own."""
     if causal:
         extent = None
+    anchor = None if site is None else site.anchor
     if _tc_selected() and x.is_cuda and tc_supported(x.shape[0], x.shape[1], x.shape[2], int(k)):
         return _ConvBlockTCFn.apply(_c(x), v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
-                                    bool(causal), int(mode), bool(residual), float(p_drop), bool(training), extent)
+                                    bool(causal), int(mode), bool(residual), float(p_drop), bool(training), extent,
+                                    site, anchor)
     x = _fp32_extent_in(_c(x), k, extent)
     y = _ConvBlockFn.apply(x, v, g, bias, None if spk is None else _c(spk), int(k), int(dilation),
-                           bool(causal), int(mode), bool(residual), float(p_drop), bool(training))
+                           bool(causal), int(mode), bool(residual), float(p_drop), bool(training), site, anchor)
     return extent_grad_mask(y, extent)
 
 
@@ -716,7 +831,7 @@ class _Conv1dFn(torch.autograd.Function):
         B, Cin, T = x.shape
         Cout = v.shape[0]
         assert v.shape == (Cout, Cin, k)
-        w_f, w_b, inv = _wn_conv_fwd(v, g)
+        w_f, w_b, inv = _fp32_weights(v, g)
         y = torch.empty(B, Cout, T, device=x.device, dtype=torch.float32)
         lib.call("dv3_conv1d_fwd", _p(x), _p(w_f), _p(bias), _p(y), B, Cin, Cout, T, k, dilation,
                  int(causal), int(relu), _stream())
@@ -899,6 +1014,25 @@ def dropout(x, p, training):
     return _DropoutFn.apply(_c(x), float(p), rng.seed_tensor(x.device), rng.next_salt())
 
 
+# Embedding-only speaker adaptation (speaker_adapt.SpeakerAdapt, installed by TrainStep(adapt_speakers=...) for the
+# duration of one forward/backward): the speaker-conditioned sites run through it.  None: the plain autograd chain.
+speaker_adapt = None
+
+
+def speaker_dropout(e_btc, p, training):
+    """A stack's dropout of its time-expanded speaker embedding (B, T, S)."""
+    if speaker_adapt is None:
+        return dropout(e_btc, p, training)
+    return speaker_adapt.dropout(e_btc, p, training)
+
+
+def speaker_residual(x, fc, e_btc):
+    """x + softsign(fc(e_btc)): the encoder's speaker_fc1 / speaker_fc2 sites (reference deepvoice3.py:84, 101)."""
+    if speaker_adapt is None:
+        return x + torch.nn.functional.softsign(fc(e_btc))
+    return speaker_adapt.residual_site(x, fc, e_btc)
+
+
 # ----------------------------------------------------------------------------------------------
 # ConvTranspose1d(k=2, stride=2) and Linear on the conv kernels
 # ----------------------------------------------------------------------------------------------
@@ -913,12 +1047,7 @@ class _ConvT2Fn(torch.autograd.Function):
         Cout = v.shape[1]
         assert v.shape == (Cin, Cout, 2)
         dev = x.device
-        w_f = torch.empty(Cin, 2 * Cout, device=dev, dtype=torch.float32)     # [ci][(j,co)]
-        w_b = torch.empty(2 * Cout, Cin, device=dev, dtype=torch.float32)     # [(j,co)][ci]
-        inv = torch.empty(Cin, device=dev, dtype=torch.float32)
-        scale = torch.empty_like(inv)
-        lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cin, Cout, 2,
-                 2 * Cout, 1, Cout, 1, Cin, Cout * Cin, _stream())
+        w_f, w_b, inv, _ = _frozen("convt_fp32", v, g) or _convt_fp32_fold(v, g)     # [ci][(j,co)], [(j,co)][ci]
         bias2 = bias.repeat(2)
         yp = torch.empty(B, 2 * Cout, T, device=dev, dtype=torch.float32)
         lib.call("dv3_conv1d_fwd", _p(x), _p(w_f), _p(bias2), _p(yp), B, Cin, 2 * Cout, T, 1, 1, 0, 0, _stream())

@@ -26,6 +26,7 @@ import torch.nn.functional as F
 
 from . import data, ops
 from ._lib import lib
+from .speaker_adapt import SpeakerAdapt, check_adapt_speakers
 from .weight_bank import WeightBank
 
 
@@ -493,13 +494,33 @@ class TrainStep:
 
     deterministic (None: ``ops.deterministic`` at construction): every step runs the fixed-order kernels of DESIGN.md
     section 2.10 whatever ``ops.deterministic`` says later, eager or captured; the step owns their scratch, which is
-    allocated by the eager passes before a capture and so lies outside every graph pool."""
+    allocated by the eager passes before a capture and so lies outside every graph pool.
+
+    adapt_speakers: embedding-only speaker adaptation (DESIGN.md section 2.12; speaker_adapt.py) of a multi-speaker
+    model -- consecutive ascending speaker ids, e.g. what ``model.add_speakers`` returned.  The step runs the joint
+    forward and the full training loss, and updates only those rows of ``embed_speakers.weight``: torch.optim.Adam +
+    clip_grad_norm_ on a leaf holding just those rows (its own step count from 0, the norm over those rows).  Every
+    other parameter, row and buffer keeps its bits; no weight-gradient GEMM and no weight-norm backward runs, and the
+    weight norm and operand planes of the frozen network are folded once, on the first step, and reused.  Writing the
+    frozen weights afterwards is detected from their version counters at the next ``step()``, which refolds them in
+    place (``load_state_dict`` refolds too).  A batch row of a speaker not being adapted changes no parameter and sets
+    the device error flag that ``ops.check_index_errors()`` raises on (no host sync inside the step).  Single process
+    only; train_seq2seq / train_postnet must both be True.  ValueError otherwise, before any launch."""
 
     def __init__(self, model, init_lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1, r=1, downsample_step=4,
                  masked_loss_weight=0.5, binary_divergence_weight=0.1, guided_attention_sigma=0.2,
                  use_guided_attention=True, priority_freq=3000, priority_freq_weight=0.0, sample_rate=22050,
                  lr_schedule=noam_learning_rate_decay, use_graph=False, fused_loss=True, weight_bank=None,
-                 train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False, deterministic=None):
+                 train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False, deterministic=None,
+                 adapt_speakers=None):
+        self.adapt = None
+        if adapt_speakers is not None:
+            ids = check_adapt_speakers(model, adapt_speakers)
+            if not (train_seq2seq and train_postnet):
+                raise ValueError("speaker adaptation trains through the joint forward: train_seq2seq and train_postnet "
+                                 "must both be True")
+            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+                raise ValueError("speaker adaptation runs in a single process (world size %d)" % dist.get_world_size())
         check_train_mode(model, train_seq2seq, train_postnet)
         self.math = ops.math_mode()
         self.deterministic = ops.is_deterministic() if deterministic is None else bool(deterministic)
@@ -509,12 +530,17 @@ class TrainStep:
         # the module whose parameters are trained and checkpointed (reference save_checkpoint, train.py:787-808)
         self.trained = model if self.train_seq2seq and self.train_postnet else \
             (model.seq2seq if self.train_seq2seq else model.postnet)
-        trainable = list(model.get_trainable_parameters())
-        own = {id(p) for p in self.trained.parameters()}
-        index = [i for i, p in enumerate(trainable) if id(p) in own]
-        self.arena = ParameterArena(model, [trainable[i] for i in index])
-        self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad,
-                            arena_parts(model, self.arena), index, len(trainable))
+        if adapt_speakers is not None:
+            self.adapt = SpeakerAdapt(model, ids)
+            self.arena = self.adapt.arena
+            self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad)
+        else:
+            trainable = list(model.get_trainable_parameters())
+            own = {id(p) for p in self.trained.parameters()}
+            index = [i for i, p in enumerate(trainable) if id(p) in own]
+            self.arena = ParameterArena(model, [trainable[i] for i in index])
+            self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad,
+                                arena_parts(model, self.arena), index, len(trainable))
         self.init_lr, self.lr_schedule = init_lr, lr_schedule
         self.loss_kw = dict(r=r, downsample_step=downsample_step, masked_loss_weight=masked_loss_weight,
                             binary_divergence_weight=binary_divergence_weight,
@@ -539,11 +565,12 @@ class TrainStep:
         self.capture_seconds = 0.0          # wall time spent warming up and capturing graphs
         if weight_bank is None:
             weight_bank = os.environ.get("DV3_WEIGHT_BANK", "1") == "1"
-        self.bank = WeightBank(ops._npl()) if weight_bank else None
-        self.arena.broadcast(model)             # replicas start from rank 0's weights (no-op for world == 1)
+        self.bank = WeightBank(ops._npl()) if weight_bank and self.adapt is None else None
+        if self.adapt is None:
+            self.arena.broadcast(model)             # replicas start from rank 0's weights (no-op for world == 1)
         # overlapped gradient exchange (world > 1): buckets are all-reduced on a communication stream as soon as the
         # backward pass has finished them; only the last ("rest") bucket is exposed
-        self.buckets, self.rest_ranges = gradient_buckets(model, self.arena)
+        self.buckets, self.rest_ranges = gradient_buckets(model, self.arena) if self.adapt is None else ({}, [])
         self.overlap_comm = self.world > 1 and os.environ.get("DV3_OVERLAP_COMM", "1") == "1" and \
             self.arena.flat.is_cuda
         self._comm = torch.cuda.Stream(device=self.arena.flat.device) if self.overlap_comm else None
@@ -554,7 +581,12 @@ class TrainStep:
     # -- checkpointing: the reference's checkpoint keys (train.py:787-810) ---------------------------------
     def state_dict(self, global_epoch=0):
         """The reference's checkpoint: in a partial mode the trained part's state_dict (model.seq2seq or
-        model.postnet), with optimizer state for its parameters only."""
+        model.postnet), with optimizer state for its parameters only.  Speaker adaptation: the whole model's
+        state_dict, the Adam state of the adapted rows' leaf and the ids under "adapted_speakers"."""
+        if self.adapt is not None:
+            return {"state_dict": self.model.state_dict(), "optimizer": self.opt.state_dict(),
+                    "adapted_speakers": list(self.adapt.ids), "global_step": self.global_step,
+                    "global_epoch": global_epoch}
         return {"state_dict": self.trained.state_dict(), "optimizer": self.opt.state_dict(),
                 "global_step": self.global_step, "global_epoch": global_epoch}
 
@@ -562,6 +594,8 @@ class TrainStep:
         """Resume from ``state_dict()`` or from a reference checkpoint (same keys), of the whole model or of
         model.seq2seq / model.postnet alone, in any mode.  Restores the Adam moments, the bias-correction steps (parts
         without optimizer state start at step 0) and the position in the learning-rate schedule."""
+        if self.adapt is not None:
+            return self._load_adapt(ckpt, load_optimizer)
         sd = ckpt["state_dict"]
         target = self.model
         for part in (self.model.seq2seq, self.model.postnet):
@@ -578,10 +612,21 @@ class TrainStep:
         self.global_step = int(ckpt.get("global_step", 0))
         return int(ckpt.get("global_epoch", 0))
 
+    def _load_adapt(self, ckpt, load_optimizer):
+        got = ckpt.get("adapted_speakers")
+        if got is not None and [int(i) for i in got] != self.adapt.ids:
+            raise ValueError("checkpoint adapted speakers %s, this step %s" % (list(got), self.adapt.ids))
+        self.model.load_state_dict(ckpt["state_dict"])      # in place: the adapted rows stay the optimizer's view
+        self.adapt.frozen.refresh()                         # outside every graph: same buffers, new values
+        if load_optimizer and ckpt.get("optimizer") is not None:
+            self.opt.load_state_dict(ckpt["optimizer"])
+        self.global_step = int(ckpt.get("global_step", 0))
+        return int(ckpt.get("global_epoch", 0))
+
     # -- pieces -------------------------------------------------------------------------------
     def _forward_backward(self, batch):
         self.arena.zero_grad()
-        ops.grad_sink = True          # kernels accumulate parameter gradients straight into the arena
+        ops.grad_sink = self.adapt is None  # kernels accumulate parameter gradients straight into the arena
         ops.weight_bank = self.bank   # weight norm of all layers: 2 launches up front, 1 per bucket in the backward
         ops.grad_boundary_cb = self._bucket_ready if self.overlap_comm else None
         self._reduced = set()
@@ -592,6 +637,8 @@ class TrainStep:
         try:
             if self.bank is not None:
                 self.bank.begin_step()
+            if self.adapt is not None:
+                return self.adapt.run(batch, self._forward_backward_inner)
             return self._forward_backward_inner(batch)
         finally:
             ops.deterministic, ops.det_scratch = det_outer
@@ -703,6 +750,14 @@ class TrainStep:
         if ops.math_mode() != self.math:
             raise ValueError("TrainStep was built with ops.conv_math = %r and cannot step under %r: its weight bank and "
                              "CUDA graphs hold that mode's kernels (build a new TrainStep)" % (self.math, ops.conv_math))
+        if self.adapt is not None:
+            if batch.get("speaker_ids") is None:
+                raise ValueError("speaker adaptation needs batch['speaker_ids']")
+            if self.model.embed_speakers.weight is not self.adapt.table:
+                raise ValueError("the speaker table was replaced (add_speakers) after this TrainStep was built: build a "
+                                 "new TrainStep")
+            if self.adapt.frozen.stale():       # frozen weights written since their fold: refold in place
+                self.adapt.frozen.refresh()
         self.model.train()
         batch = self._mode_batch(batch)
         lr = self.lr_schedule(self.init_lr, self.global_step) if self.lr_schedule else self.init_lr

@@ -2,6 +2,7 @@
 speaker table and the post-net.  Public surface (attribute names, call signatures, return tuples) follows what
 reference train.py / synthesis.py touch (SURVEY.md section 8b); see reference deepvoice3_pytorch/__init__.py:11-126.
 """
+import torch
 from torch import nn
 
 from . import ops
@@ -47,9 +48,42 @@ class MultiSpeakerTTSModel(nn.Module):
         self.trainable_positional_encodings = trainable_positional_encodings
         self.use_decoder_state_for_postnet_input = use_decoder_state_for_postnet_input
         self.freeze_embedding = freeze_embedding
+        self.speaker_embedding_weight_std = speaker_embedding_weight_std
         if n_speakers > 1:
             self.embed_speakers = Embedding(n_speakers, speaker_embed_dim, padding_idx=None,
                                             std=speaker_embedding_weight_std)
+
+    def add_speakers(self, n, init="mean"):
+        """Append ``n`` rows to the speaker table and return their ids [n_speakers, n_speakers + n): one contiguous
+        block at the end, the existing rows bit-identical, the state_dict keys unchanged (a model built with
+        n_speakers + n loads the result strictly).  init: "mean" (the mean of the existing rows, in fp64, rounded
+        once), "normal" (the builder's N(0, speaker_embedding_weight_std) init from the torch RNG) or an
+        (n, speaker_embed_dim) tensor of the table's dtype.  Raises ValueError, changing nothing, for a
+        single-speaker model, n < 1 or a malformed init.  Train the new rows with TrainStep(adapt_speakers=ids)."""
+        if self.n_speakers <= 1 or not hasattr(self, "embed_speakers"):
+            raise ValueError("add_speakers needs a multi-speaker model (n_speakers=%d)" % self.n_speakers)
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError("add_speakers: n=%r must be an int >= 1" % (n,))
+        old = self.embed_speakers.weight
+        S = self.speaker_embed_dim
+        if torch.is_tensor(init):
+            if tuple(init.shape) != (n, S) or init.dtype != old.dtype:
+                raise ValueError("add_speakers: init of shape %s dtype %s, expected (%d, %d) %s"
+                                 % (tuple(init.shape), init.dtype, n, S, old.dtype))
+            rows = init.detach().to(old.device)
+        elif init == "mean":
+            rows = old.detach().double().mean(0, keepdim=True).to(old.dtype).expand(n, S)
+        elif init == "normal":
+            rows = torch.empty(n, S, dtype=old.dtype).normal_(0, self.speaker_embedding_weight_std).to(old.device)
+        else:
+            raise ValueError("add_speakers: init must be \"mean\", \"normal\" or a tensor (got %r)" % (init,))
+        ids = list(range(self.n_speakers, self.n_speakers + n))
+        with torch.no_grad():
+            table = torch.cat([old.detach(), rows], 0)
+        self.embed_speakers.weight = nn.Parameter(table, requires_grad=old.requires_grad)
+        self.embed_speakers.num_embeddings = table.shape[0]
+        self.n_speakers += n
+        return ids
 
     # -- optimiser view ---------------------------------------------------------------------------------
     def _frozen_parameters(self):
@@ -77,6 +111,8 @@ class MultiSpeakerTTSModel(nn.Module):
         if speaker_ids is None:
             return None
         assert self.n_speakers > 1
+        if ops.speaker_adapt is not None:            # embedding-only adaptation: e is the one tensor with a gradient
+            return ops.speaker_adapt.embed(self.embed_speakers, speaker_ids)
         return self.embed_speakers(speaker_ids)
 
     def forward(self, text_sequences, mel_targets=None, speaker_ids=None, text_positions=None,

@@ -554,6 +554,36 @@ typedef struct Dv3IncRefill {
  * listed slots (ring rows, cursors, counters, go frame) and loads their next utterances' constants from staging. */
 int dv3_inc_refill(const Dv3IncRefill* table, int n_entries, const int* slots, int n_slots, void* stream);
 
+/* ---- speaker adaptation: embedding gradient of a speaker-conditioned site with its weights frozen (spk_adapt.cu) ----
+ * The site's share of d_e[b*S + s] = sum_{t < T_b} m(b,t,s)/(1-p) * sum_c w[c*S + s] * G(b,c,t) * (1 - |y(b,c,t)|)^2
+ * is written as dv3_spk_grad_splits() partial rows: partials[(k*B + b)*S + s], k < splits (every one written).
+ * y = softsign(z) of the site's forward; w (C, S) its folded weight; m the dropout mask of the stack's (B,T,S)
+ * expanded embedding at element (b*T + t)*S + s (seed_ptr / salt of that dropout call; p = 0 or seed_ptr NULL: none).
+ * T_b = min(T, ext[0] * ext_mult) when ext is given, else T.  Fixed summation order, no atomics.  S <= 64,
+ * B <= 65535.
+ * Layouts of G: _planes  bf16 [npl][B][T][ldg] operand planes of the gate split (channels [0, C) are the "a" half),
+ *                        plane_stride elements apart, value hi + lo * 2^-11; y (B,C,T)
+ *               _bct     fp32 (B,C,T) with batch stride g_bstride (the a half of the exact path's (B,2C,T) gate
+ *                        gradient); y (B,C,T)
+ *               _btc     fp32 (B,T,C) residual-stream gradient; y (B,T,C)
+ * dv3_spk_grad_reduce: d_e[b*S + s] = sum over i < nparts, in order, of partials[(i*B + b)*S + s] -- the partial rows
+ * of every site of a pass, laid out one after the other. */
+int dv3_spk_grad_splits(void);
+int dv3_spk_grad_planes(const void* g_planes, int npl, long long plane_stride, int ldg, const float* y_bct,
+                        const float* w, float* partials, int B, int C, int T, int S, const long long* ext,
+                        int ext_mult, float p, const unsigned long long* seed_ptr, unsigned salt, void* stream);
+int dv3_spk_grad_bct(const float* g_bct, long long g_bstride, const float* y_bct, const float* w, float* partials,
+                     int B, int C, int T, int S, const long long* ext, int ext_mult, float p,
+                     const unsigned long long* seed_ptr, unsigned salt, void* stream);
+int dv3_spk_grad_btc(const float* g_btc, const float* y_btc, const float* w, float* partials, int B, int C,
+                     int T, int S, const long long* ext, int ext_mult, float p, const unsigned long long* seed_ptr,
+                     unsigned salt, void* stream);
+int dv3_spk_grad_reduce(const float* partials, long long nparts, float* d_e, int B, int S, void* stream);
+/* grad[j*S + s] = sum over rows b (ascending) with ids[b] == lo + j of d_e[b*S + s] (+ d_e2[b*S + s] when non-NULL),
+ * j < n; rows whose id lies outside [lo, lo + n) contribute nothing and set *err_flag = 1 (when non-NULL). */
+int dv3_spk_rows_grad(const float* d_e, const float* d_e2, const long long* ids, long long lo, int n, float* grad,
+                      int* err_flag, int B, int S, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
