@@ -45,14 +45,14 @@ namespace dv3 {
 
 using namespace tc;
 
-constexpr int TC_CONV_THREADS = 512;        // tc_conv_kernel: consumers 0-1, producer 2, epilogue 3 (warpgroups)
+constexpr int TC_CONV_THREADS = 512;        // tc_conv_kernel, tc_wgrad_mn_kernel: consumers 0-1, producer 2,
+                                            // epilogue 3 (warpgroups)
 constexpr int TC_PRODUCER_REGS = 24;        // setmaxnreg budgets: 128 x 24 + 256 x 176 + 128 x 136 = 65 536 registers
 constexpr int TC_CONSUMER_REGS = 176;
 constexpr int TC_EPILOGUE_REGS = 136;       // > 65 536 / 512: claimed with setmaxnreg.inc (.dec may not raise it)
 static_assert(TC_PRODUCER_REGS <= 65536 / TC_CONV_THREADS && TC_CONSUMER_REGS >= 65536 / TC_CONV_THREADS &&
               TC_EPILOGUE_REGS >= 65536 / TC_CONV_THREADS, "setmaxnreg direction of each warpgroup");
 static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS + 128 * TC_EPILOGUE_REGS <= 65536, "register file");
-constexpr int TC_WGRAD_THREADS = 288;       // tc_wgrad_mn_kernel: consumer warpgroups 0-1, producer warp 8
 constexpr int MAX_TAPS_TC = 8;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memory per CTA
 // Shared memory tc_conv_kernel leaves unused, so that every configuration keeps the ring depth it was measured with
@@ -366,47 +366,60 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
 // TMA boxes (128-byte rows, SWIZZLE_128B), wgmma descriptors with the MN-major canonical layout
 // ((64 channels contiguous, chunk stride LBO), (8 rows x 128 B, group stride SBO)) and both operands transposed in the
 // instruction.  The tap shift is a ROW coordinate of the TMA box (any alignment, out-of-bounds rows are zero = the
-// conv padding), so no time-shifted copies of the input are needed.  Tile 128 (m) x 128 (n); each consumer warpgroup
-// owns 64 rows of m and writes its partials straight from the accumulator registers.
+// conv padding), so no time-shifted copies of the input are needed.
+//
+// A work unit is one 128 (m) x 128 (n) tile of one tap j and one split s: the sum over the utterances
+// [s * bps, min(B, (s + 1) * bps)) of the split, all their 32-row time chunks, written to slot s.  The kernel is
+// PERSISTENT with the warp roles of tc_conv_kernel: min(units, SMs) CTAs, CTA c walks units c, c + grid, ... of a
+// fixed list in which the split index varies slowest, so every split but the last (the only one that can be short)
+// comes first: units run longest first.  The producer streams the next unit's chunks straight after the current
+// one's; the consumers hand each finished tile to the epilogue warpgroup through a shared-memory fp32 tile and go on
+// to the next unit's MMAs while the epilogue stores it.  The schedule, and with it every value, is a function of the
+// shape and the SM count.
 // ------------------------------------------------------------------------------------------------
 struct TcMnParams {
     int T, B, Mw, Nw, k;
     int tap_off[MAX_TAPS_TC];
     int nsplit, batches_per_split, kb_n;      // kb_n = 32-row time chunks per utterance
+    int tiles_n, tiles_m, num_units;          // units: n-tile fastest, then m-tile, tap, split
     float* dw; long long split_stride;
     int msplit; long long s_m, s_mh, s_n, s_j;
     float gcoef;                              // see TcParams::gmain (n_mma = 2 per 32-row time chunk)
 };
 
 constexpr int WG_BOX = 64 * 32 * 2;                      // 64 channels x 32 time steps of bf16 = 4 KB
-// per plane: 128 channels of m, 128 channels of n; NPL planes per stage, at most 6 stages
+// per plane: 128 channels of m, 128 channels of n; NPL planes per stage.  The hand-off tile [128 m][128 n + 1] fp32
+// (66 KB; the odd pitch keeps both epilogue access patterns conflict-free) leaves room for five 32 KB two-plane stages.
 template <int NPL>
 struct WgCfg {
     static constexpr int STAGE = NPL * (2 * WG_BOX + 2 * WG_BOX);
-    static constexpr int STAGES = ((SMEM_LIMIT - 2048) / STAGE) > 6 ? 6 : ((SMEM_LIMIT - 2048) / STAGE);
-    static constexpr int SMEM = STAGES * STAGE + 1024 + 512;
+    static constexpr int ACC_PITCH = 128 + 1;
+    static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
+    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - ACC_TILE) / STAGE;
+    static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
+    static constexpr int SMEM = STAGES * STAGE + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
 };
-static_assert(WgCfg<2>::STAGES == 6 && WgCfg<1>::STAGES == 6, "weight gradient: 6-stage ring");
+static_assert(WgCfg<2>::STAGES == 5, "two-plane weight gradient: 5-stage ring");
+static_assert(WgCfg<1>::STAGES == 6, "single-pass weight gradient: 6-stage ring");
+static_assert(WgCfg<2>::SMEM <= SMEM_LIMIT && WgCfg<1>::SMEM <= SMEM_LIMIT, "weight gradient shared memory");
 
 template <int NPL>
-__global__ void __launch_bounds__(TC_WGRAD_THREADS, 1)
+__global__ void __launch_bounds__(TC_CONV_THREADS, 1)
 tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcMnParams p) {
     pdl_trigger();
     static_assert(NPL == 1 || NPL == 2, "one or two operand planes");
-    constexpr int WG_STAGE = WgCfg<NPL>::STAGE, WG_STAGES = WgCfg<NPL>::STAGES;
+    using Cfg = WgCfg<NPL>;
+    constexpr int WG_STAGE = Cfg::STAGE, WG_STAGES = Cfg::STAGES;
     constexpr int A_PL = 2 * WG_BOX, B_PL = 2 * WG_BOX;
     constexpr uint32_t LBO = 4096, SBO = 1024;           // 64-channel chunks one TMA box apart; 8-row groups 1 KB apart
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE);
+    float* acc_tile = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE + Cfg::ACC_TILE);
     uint64_t* empty = full + WG_STAGES;
+    uint64_t* acc_full = empty + WG_STAGES;                  // the consumers have written acc_tile (256 arrivals)
+    uint64_t* acc_empty = acc_full + 1;                      // the epilogue has read acc_tile (128 arrivals)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    const int wg_j = blockIdx.z % p.k, wg_split = blockIdx.z / p.k;
-    const int m0 = blockIdx.y * 128, n0 = blockIdx.x * 128;
-    const int b_beg = wg_split * p.batches_per_split;
-    int b_end = b_beg + p.batches_per_split; if (b_end > p.B) b_end = p.B;
-    const int n_iters = (b_end > b_beg ? b_end - b_beg : 0) * p.kb_n;
 
     if (threadIdx.x == 0) {
 #pragma unroll
@@ -414,71 +427,133 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
 #pragma unroll
         for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.b[pl]);
         for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+        mbar_init(acc_full, 256);
+        mbar_init(acc_empty, 128);
         fence_barrier_init();
     }
     __syncthreads();
     pdl_wait();
 
-    if (warp == 8) {
-        if (lane == 0) {
-            for (int it = 0; it < n_iters; ++it) {
-                const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
-                mbar_wait(&empty[s], ph ^ 1);
-                uint8_t* st = smem + s * WG_STAGE;
-                const int bi = it / p.kb_n, tc_ = it - bi * p.kb_n;
-                const int b = b_beg + bi, t0 = tc_ * 32;
-                mbar_arrive_expect_tx(&full[s], WG_STAGE);
+    // unit -> (m0, n0, tap, split, first utterance, K-iterations)
+    struct Unit { int m0, n0, j, s, b_beg, n_iters; };
+    auto decode = [&](int u) {
+        Unit w;
+        w.n0 = (u % p.tiles_n) * 128;
+        int r = u / p.tiles_n;
+        w.m0 = (r % p.tiles_m) * 128;
+        r /= p.tiles_m;
+        w.j = r % p.k;
+        w.s = r / p.k;
+        w.b_beg = w.s * p.batches_per_split;
+        const int b_end = min(p.B, w.b_beg + p.batches_per_split);
+        w.n_iters = (b_end > w.b_beg ? b_end - w.b_beg : 0) * p.kb_n;
+        return w;
+    };
+
+    if (warp >= 12) {
+        setmaxnreg_inc<TC_EPILOGUE_REGS>();
+        // Tap-major layout (s_n == 1): thread r owns column n0 + r and walks the rows, a warp storing 32 consecutive
+        // floats of one row.  Otherwise (ConvTranspose layout, consecutive m two floats apart): thread r owns row
+        // m0 + r and walks the columns.
+        const int r = threadIdx.x & 127;
+        int n = 0;
+        for (int u = blockIdx.x; u < p.num_units; u += gridDim.x, ++n) {
+            const Unit w = decode(u);
+            float* __restrict__ out = p.dw + (size_t)w.s * p.split_stride + (size_t)w.j * p.s_j;
+            const int rows = min(128, p.Mw - w.m0), cols = min(128, p.Nw - w.n0);
+            mbar_wait(acc_full, n & 1);
+            if (p.s_n == 1) {
+                if (r < cols) {
+                    float* __restrict__ o = out + w.n0 + r;
+#pragma unroll 4
+                    for (int i = 0; i < rows; ++i) {
+                        const int m = w.m0 + i;
+                        o[(size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh] = acc_tile[i * Cfg::ACC_PITCH + r];
+                    }
+                }
+            } else if (r < rows) {
+                const int m = w.m0 + r;
+                float* __restrict__ o = out + (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh +
+                                        (size_t)w.n0 * p.s_n;
+                const float* arow = acc_tile + r * Cfg::ACC_PITCH;
+#pragma unroll 4
+                for (int c = 0; c < cols; ++c) o[(size_t)c * p.s_n] = arow[c];
+            }
+            mbar_arrive(acc_empty);
+        }
+    } else if (warp >= 8) {
+        setmaxnreg_dec<TC_PRODUCER_REGS>();
+        if (warp == 8 && lane == 0) {
+            int it = 0;
+            for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
+                const Unit w = decode(u);
+                for (int kit = 0; kit < w.n_iters; ++kit, ++it) {
+                    const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
+                    mbar_wait(&empty[s], ph ^ 1);
+                    uint8_t* st = smem + s * WG_STAGE;
+                    const int bi = kit / p.kb_n, tc_ = kit - bi * p.kb_n;
+                    const int b = w.b_beg + bi, t0 = tc_ * 32;
+                    mbar_arrive_expect_tx(&full[s], WG_STAGE);
 #pragma unroll
-                for (int pl = 0; pl < NPL; ++pl) {
+                    for (int pl = 0; pl < NPL; ++pl) {
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-                        tma_load_3d(st + pl * A_PL + h * WG_BOX, &maps.a[pl], &full[s], m0 + h * 64, t0, b);
+                        for (int h = 0; h < 2; ++h)
+                            tma_load_3d(st + pl * A_PL + h * WG_BOX, &maps.a[pl], &full[s], w.m0 + h * 64, t0, b);
 #pragma unroll
-                    for (int q = 0; q < 2; ++q)
-                        tma_load_3d(st + NPL * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], &full[s], n0 + q * 64,
-                                    t0 + p.tap_off[wg_j], b);
+                        for (int q = 0; q < 2; ++q)
+                            tma_load_3d(st + NPL * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], &full[s], w.n0 + q * 64,
+                                        t0 + p.tap_off[w.j], b);
+                    }
                 }
             }
         }
     } else {
-        // A = gradient planes, B = the bf16 copy of the forward operand planes; both MN-major
+        setmaxnreg_inc<TC_CONSUMER_REGS>();
+        // A = gradient planes, B = the bf16 copy of the forward operand planes; both MN-major.  Two disjoint register
+        // tuples: an MMA in flight may not share accumulator registers with the next one.
         const int wg = warp >> 2, wq = warp & 3;
-        float acc[NPL * 64];                                 // [0, 64): main, [64, 128): cross
+        float acc[64], xacc[NPL == 2 ? 64 : 1];              // main (p0 x p0), cross (p0 x p1 + p1 x p0)
+        int it = 0, n = 0;
+        for (int u = blockIdx.x; u < p.num_units; u += gridDim.x, ++n) {
+            const Unit w = decode(u);
 #pragma unroll
-        for (int i = 0; i < NPL * 64; ++i) acc[i] = 0.f;
-        for (int it = 0; it < n_iters; ++it) {
-            const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
-            mbar_wait(&full[s], ph);
-            const uint32_t sa = smem_u32(smem + s * WG_STAGE);
-            wgmma_fence();
+            for (int i = 0; i < 64; ++i) {
+                acc[i] = 0.f;
+                if constexpr (NPL == 2) xacc[i] = 0.f;
+            }
+            for (int kit = 0; kit < w.n_iters; ++kit, ++it) {
+                const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
+                mbar_wait(&full[s], ph);
+                const uint32_t sa = smem_u32(smem + s * WG_STAGE);
+                wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 2; ++kk) {                        // 2 x K = 16 rows of 128 B
-                const uint32_t ko = kk * 16 * 128;
-                const uint64_t a0 = make_wgmma_desc(sa + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
-                const uint64_t b0 = make_wgmma_desc(sa + NPL * A_PL + ko, LBO, SBO, WG_SW128);
-                wgmma_mma<128, 1, 1>(true, acc, a0, b0, 1);
-                if constexpr (NPL == 2) {
-                    const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
-                    const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
-                    wgmma_mma<128, 1, 1>(true, acc + 64, a0, b1, 1);
-                    wgmma_mma<128, 1, 1>(true, acc + 64, a1, b0, 1);
+                for (int kk = 0; kk < 2; ++kk) {                        // 2 x K = 16 rows of 128 B
+                    const uint32_t ko = kk * 16 * 128;
+                    const uint64_t a0 = make_wgmma_desc(sa + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+                    const uint64_t b0 = make_wgmma_desc(sa + NPL * A_PL + ko, LBO, SBO, WG_SW128);
+                    wgmma_mma<128, 1, 1>(true, acc, a0, b0, 1);
+                    if constexpr (NPL == 2) {
+                        const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+                        const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
+                        wgmma_mma<128, 1, 1>(true, xacc, a0, b1, 1);
+                        wgmma_mma<128, 1, 1>(true, xacc, a1, b0, 1);
+                    }
                 }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (kit > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
             }
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (it > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
-        }
-        wgmma_wait<0>();
-        float* __restrict__ out = p.dw + (size_t)wg_split * p.split_stride + (size_t)wg_j * p.s_j;
-        const float gmain = 1.f + p.gcoef * (float)(2 * n_iters);
+            wgmma_wait<0>();
+            if (w.n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
+            const float gmain = 1.f + p.gcoef * (float)(2 * w.n_iters);
+            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous unit
 #pragma unroll
-        for (int i = 0; i < 64; ++i) {
-            const int m = m0 + 64 * wg + frag_row(i, wq, lane), n = n0 + frag_col(i, lane);
-            if (m < p.Mw && n < p.Nw) {
-                const size_t ma = (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh;
-                if constexpr (NPL == 2) out[ma + (size_t)n * p.s_n] = fmaf(acc[64 + i], LO_INV, acc[i] * gmain);
-                else out[ma + (size_t)n * p.s_n] = acc[i] * gmain;
+            for (int i = 0; i < 64; ++i) {                            // lo planes carry 2^11
+                float* dst = &acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)];
+                if constexpr (NPL == 2) *dst = fmaf(xacc[i], LO_INV, acc[i] * gmain);
+                else *dst = acc[i] * gmain;
             }
+            mbar_arrive(acc_full);
         }
     }
 }
@@ -665,21 +740,42 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     return launch_conv<TC_CONV, 1, 128, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
 }
 
+// Split count of the weight gradient, chosen for the persistent grid.  A candidate is a batch range of
+// bps = ceil(B / nsplit) utterances per split; it is costed in 32-row K-iterations with the schedule the kernel runs:
+//   tk = m-tiles * n-tiles * k units per split, U = tk * nsplit units, G = min(U, sms) CTAs; a unit of a full split
+//   runs L = bps * kb_n iterations, one of the last split L_last <= L.  Dealt round-robin longest first, CTA 0 carries
+//   the most: ceil(U_full / G) long units (U_full = tk * (nsplit - 1)) and ceil(U / G) units in all, so
+//     makespan = ceil(U_full / G) * (L - L_last) + ceil(U / G) * (L_last + WG_UNIT_ITERS)
+//   plus the partial slabs, nsplit * Mw * Nw * k * 8 bytes (written here, read by the weight-norm backward), at
+//   WG_SLAB_BYTES_PER_ITER bytes per iteration for the whole GPU.
+// The smallest nsplit within 3 % of the cheapest wins.  The result depends on the shape and the SM count only.
+// Both constants from tools/wgrad_time.py --fit on an H100 SXM (700 W): t = 6.6 us + 0.47 us per K-iteration of CTA 0
+// + 11.6 us per unit of CTA 0, i.e. about 25 iterations per unit; 0.47 us at 3.35 TB/s (data sheet) is 1.5 MB.
+constexpr double WG_UNIT_ITERS = 25.0;             // per-unit cost in K-iterations
+constexpr double WG_SLAB_BYTES_PER_ITER = 1.5e6;   // HBM bytes per K-iteration of time, whole GPU
 int dv3_tc_wgrad_nsplit(int B, int Mw, int Nw, int T, int k) {
-    const int tiles = ((Mw + 127) / 128) * ((Nw + 127) / 128) * k;
-    // split (b,t) over enough CTAs for two waves, unless that leaves each CTA fewer than ~64 K-iterations (then the
-    // per-CTA prologue/epilogue and the extra partial traffic cost more than the parallelism buys: one wave).
-    const int kb_n = (T + 31) / 32, sms = config().sms;
-    int best = 1;
-    for (int target = 2 * sms; target >= sms; target -= sms) {
-        int want = (target + tiles - 1) / tiles;
-        if (want > B) want = B;
-        if (want < 1) want = 1;
-        const int bps = (B + want - 1) / want;
-        best = (B + bps - 1) / bps;
-        if (bps * kb_n >= 64) break;
+    const long long tk = (long long)((Mw + 127) / 128) * ((Nw + 127) / 128) * k;
+    const long long kb_n = (T + 31) / 32, sms = config().sms;
+    const double slab = (double)Mw * Nw * k * 8.0 / WG_SLAB_BYTES_PER_ITER;
+    auto cost = [&](int ns) {
+        const long long bps = (B + ns - 1) / ns, U = tk * ns, U_full = tk * (ns - 1), G = U < sms ? U : sms;
+        const long long L = bps * kb_n, L_last = (B - (ns - 1) * bps) * kb_n;
+        return (double)((U_full + G - 1) / G) * (double)(L - L_last) +
+               (double)((U + G - 1) / G) * ((double)L_last + WG_UNIT_ITERS) + ns * slab;
+    };
+    // the distinct batch-range splits, ascending: ns = ceil(B / bps) for bps = B, B - 1, ..., 1
+    double best = 0.0;
+    for (int bps = B, prev = 0; bps >= 1; --bps) {
+        const int ns = (B + bps - 1) / bps;
+        if (ns != prev && (prev == 0 || cost(ns) < best)) best = cost(ns);
+        prev = ns;
     }
-    return best;
+    for (int bps = B, prev = 0; bps >= 1; --bps) {
+        const int ns = (B + bps - 1) / bps;
+        if (ns != prev && cost(ns) <= 1.03 * best) return ns;
+        prev = ns;
+    }
+    return 1;
 }
 
 // Weight gradient from (B,T,C) planes.  dy: [npl][B][T][pad8(Mw)], xd: [npl][B][T][pad8(Nw)]; partial element
@@ -702,20 +798,24 @@ int dv3_tc_wgrad_mn_npl(const void* dy, const void* xd, int npl, float* dw_parti
     fill_taps_tc(p.tap_off, k, dilation, causal, false);
     p.nsplit = dv3_tc_wgrad_nsplit(B, Mw, Nw, T, k);
     p.batches_per_split = (B + p.nsplit - 1) / p.nsplit;
+    p.tiles_n = (Nw + 127) / 128; p.tiles_m = (Mw + 127) / 128;
+    const long long units = (long long)p.tiles_n * p.tiles_m * k * p.nsplit;
+    DV3_REQUIRE(units < (1ll << 31), "tc_wgrad_mn: %lld work units", units);
+    p.num_units = (int)units;
     p.dw = dw_partials; p.split_stride = split_stride;
     p.msplit = msplit; p.s_m = s_m; p.s_mh = s_mh; p.s_n = s_n; p.s_j = s_j;
     p.gcoef = config().tc_gamma;
-    const dim3 grid((Nw + 127) / 128, (Mw + 127) / 128, p.nsplit * k);
+    const int sms = config().sms, grid = p.num_units < sms ? p.num_units : sms;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e;
     if (npl == 1) {
         static const int configured = ensure_smem(tc_wgrad_mn_kernel<1>, WgCfg<1>::SMEM, "tc_wgrad_mn");
         if (configured) return 1;
-        e = launch_k(tc_wgrad_mn_kernel<1>, grid, dim3(TC_WGRAD_THREADS), (size_t)WgCfg<1>::SMEM, st, maps, p);
+        e = launch_k(tc_wgrad_mn_kernel<1>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)WgCfg<1>::SMEM, st, maps, p);
     } else {
         static const int configured = ensure_smem(tc_wgrad_mn_kernel<2>, WgCfg<2>::SMEM, "tc_wgrad_mn");
         if (configured) return 1;
-        e = launch_k(tc_wgrad_mn_kernel<2>, grid, dim3(TC_WGRAD_THREADS), (size_t)WgCfg<2>::SMEM, st, maps, p);
+        e = launch_k(tc_wgrad_mn_kernel<2>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)WgCfg<2>::SMEM, st, maps, p);
     }
     if (e != cudaSuccess) { set_error("tc_wgrad_mn: launch failed: %s", cudaGetErrorString(e)); return 1; }
     return check_launch("tc_wgrad_mn");
