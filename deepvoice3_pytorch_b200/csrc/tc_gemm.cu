@@ -12,32 +12,40 @@
 //           (plain conv forward with bias/ReLU, and every data gradient: A = dY or dAB, W = transposed weight)
 //   WGRAD : D[m, n] (j)   = sum_{b,t}  dY[b, t, m] * Xd[b, t+off_j, n]            MN-major operands, M = 128, N <= 256
 //
-// Operands are 16-bit (B,T,C) planes fetched by TMA as K-major tiles of 128 rows x BK (BK = 64: 128-byte rows,
-// SWIZZLE_128B; BK = 32: 64-byte rows, SWIZZLE_64B; the host launchers pick BK per configuration); the conv's zero
-// padding, the causal shift, ragged T / channel tails are TMA out-of-bounds zero fill.  Each K = 16 step issues three
-// N = NCOLS MMAs: p0(A) x p0(W) into the main accumulator, then p0(A) x p1(W) and p1(A) x p0(W) into the cross
-// accumulator.  Main and cross are two disjoint register tuples: when an in-flight MMA's accumulator partially overlaps
-// the next one's, ptxas serialises the whole wgmma chain (C7511), whatever the register budget.
+// Each K = 16 step issues three MMAs: p0(A) x p0(W) into the main accumulator, then p0(A) x p1(W) and p1(A) x p0(W)
+// into the cross accumulator.  Main and cross are two disjoint register tuples: when an in-flight MMA's accumulator
+// partially overlaps the next one's, ptxas serialises the whole wgmma chain (C7511), whatever the register budget.
 //
 // Single-pass mode (NPL = 1, ops.conv_math = "tc1", DESIGN.md section 2.7): each operand travels as its plane p0 alone
 // (fp16 forward, bf16 gradients) and each K = 16 step issues the one MMA p0(A) x p0(W) into the main accumulator: the
 // producer loads one plane per operand, there is no cross accumulator, and the hand-off writes main * gmain.  One
 // kernel body serves both plane counts.
 //
-// tc_conv_kernel is PERSISTENT: one CTA per SM walks a static round-robin list of output tiles and the TMA ring
-// streams across tile boundaries.  Warp roles (512 threads, one setmaxnreg budget per warpgroup):
+// Both kernels run one PERSISTENT, warp-specialised pipeline (tc_pipeline): min(work units, SMs) CTAs, CTA c walks
+// units c, c + grid, ... of a static list, and the TMA ring streams across unit boundaries.  512 threads, one
+// setmaxnreg budget per warpgroup:
+//   * warpgroup 2 = producer (24 registers): one thread issues the TMA loads of each K-iteration into the next stage of
+//     a STAGES-deep ring (full[s]: one arrival plus the stage's transaction bytes; empty[s]: one arrival per consumer
+//     warpgroup);
 //   * warpgroups 0 and 1 = consumers (176 registers): each accumulates 64 of the 128 tile rows in registers (wgmma),
-//     then writes the summed accumulators into a full-tile fp32 shared-memory hand-off tile (acc_tile) and goes
-//     straight on to the next tile's MMAs;
-//   * warpgroup 2 = producer (24 registers): one thread issues the TMA loads;
-//   * warpgroup 3 = epilogue (136 registers): thread r owns row r (time step) of acc_tile and runs the fused math and
-//     the stores (coalesced along T).
+//     keeping one stage of MMAs in flight (wait_group 1, then release the previous stage), then writes
+//     main * gmain + cross * 2^-11 into a full-tile fp32 shared-memory hand-off tile (acc_tile) and goes straight on
+//     to the next unit's MMAs;
+//   * warpgroup 3 = epilogue (136 registers): reads acc_tile and stores the unit's output.
 // Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (all
-// 128 epilogue threads have read it).  So the epilogue of tile n runs while the consumers issue the MMAs of tile n+1.
+// 128 epilogue threads have read it).  So the epilogue of unit n runs while the consumers issue the MMAs of unit n+1.
+// A kernel supplies only its unit list, the TMA loads of one K-iteration, the MMAs of one stage, its gmain and its
+// epilogue.
 //
-// The epilogues fuse the launch's own math only (gate, bias, speaker bias, residual, dropout mask, addend, ReLU) and
-// write fp32 (B,C,T) outputs.  The operand planes of the next GEMM come from the split kernels of tc_split.cu, which
-// run at full occupancy rather than on one warpgroup per SM.
+// tc_conv_kernel (GATED, CONV): a unit is one 128-step x NCOLS output tile of one utterance.  Operands are 16-bit
+// (B,T,C) planes fetched by TMA as K-major tiles of 128 rows x BK (BK = 64: 128-byte rows, SWIZZLE_128B; BK = 32:
+// 64-byte rows, SWIZZLE_64B; the host launchers pick BK per configuration); the conv's zero padding, the causal shift,
+// ragged T / channel tails are TMA out-of-bounds zero fill.  Epilogue thread r owns row r (time step) of acc_tile and
+// fuses the launch's own math only (gate, bias, speaker bias, residual, dropout mask, addend, ReLU), storing fp32
+// (B,C,T) outputs coalesced along T.  The operand planes of the next GEMM come from the split kernels of tc_split.cu,
+// which run at full occupancy rather than on one warpgroup per SM.
+//
+// tc_wgrad_mn_kernel (WGRAD): MN-major operands and batch-range work units, see the comment at the kernel.
 #include "tc_common.cuh"
 #include "../../include/dv3b200.h"
 
@@ -59,13 +67,30 @@ constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memo
 // (static_asserts after TcCfg).  Claiming it for a deeper ring is a performance change of its own.
 constexpr int RING_RESERVE = 32768;
 
+// Shared-memory layout of the pipeline: STAGES ring stages of STAGE bytes, the consumer -> epilogue hand-off tile (the
+// whole fp32 output tile, [128 rows][NCOLS + 1]), then the barriers full[STAGES], empty[STAGES], acc_full, acc_empty.
+// The ring gets what is left of the 227 KB after 2 KB (alignment slack + barriers), RESERVE and the hand-off tile, at
+// most 6 stages.  The odd pitch keeps the epilogue's column reads (a warp reads one column of 32 consecutive rows)
+// conflict-free; every access is a row base plus an immediate offset, which the register budgets of both sides need
+// (an XOR swizzle that also makes the consumers' fragment-order writes 2-way instead of 4-way conflicted spilled in
+// both warpgroups).
+template <int STAGE_BYTES, int TILE_COLS, int RESERVE>
+struct RingCfg {
+    static constexpr int STAGE = STAGE_BYTES;
+    static constexpr int NCOLS = TILE_COLS;              // columns of the output tile and of each accumulator
+    static constexpr int ACC_PITCH = NCOLS + 1;
+    static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
+    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - RESERVE - ACC_TILE) / STAGE;
+    static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
+    static constexpr int SMEM = STAGES * STAGE + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
+};
+
 enum { TC_GATED = 0, TC_CONV = 1 };
 
 struct TcMaps { CUtensorMap a[2]; CUtensorMap b[2]; };
 
 struct TcParams {
-    int T, B;
-    int Kc;                    // contraction channels per tap
+    int T;
     int Nc;                    // output channels (GATED: C per half)
     int rows_per_tap;          // rows of the weight matrix per tap (GATED: 2C, CONV: Nc)
     int k, kb_n;               // taps; K blocks per tap
@@ -95,24 +120,11 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     return make_wgmma_desc(saddr, 16, SwizzleOf<BK>::sbo, SwizzleOf<BK>::layout);
 }
 
+// Conv ring: a stage holds NPL planes of one 128-row A tile and NBOX B boxes of BR rows, each BK 16-bit channels wide.
 // BR = rows of one B-operand box (128, or 64 for problems too small to fill the machine with 128-wide tiles); NPL =
 // operand planes per stage (2: hi / lo pairs, 1: single pass)
 template <int NBOX, int BK, int BR, int NPL = 2>
-struct TcCfg {
-    static constexpr int TILE = 128 * BK * 2;            // A tile (128 rows)
-    static constexpr int TILE_B = BR * BK * 2;           // one B box
-    static constexpr int STAGE = NPL * (TILE + NBOX * TILE_B);
-    static constexpr int NCOLS = BR * NBOX;              // columns per accumulator (main, cross)
-    // consumer -> epilogue hand-off: the whole fp32 output tile, [128 rows][NCOLS + 1].  The odd pitch keeps the
-    // epilogue's column reads (a warp reads one column of 32 consecutive rows) conflict-free; every access is a row
-    // base plus an immediate offset, which the register budgets of both sides need (an XOR swizzle that also makes
-    // the consumers' fragment-order writes 2-way instead of 4-way conflicted spilled in both warpgroups).
-    static constexpr int ACC_PITCH = NCOLS + 1;
-    static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - RING_RESERVE - ACC_TILE) / STAGE;
-    static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-    static constexpr int SMEM = STAGES * STAGE + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
-};
+using TcCfg = RingCfg<NPL * (128 + NBOX * BR) * BK * 2, BR * NBOX, RING_RESERVE>;
 static_assert(TcCfg<2, 32, 64>::STAGES == 4, "gated forward: 4-stage ring");
 static_assert(TcCfg<1, 32, 128>::STAGES == 4, "128-column conv: 4-stage ring");
 static_assert(TcCfg<1, 64, 64>::STAGES == 3, "64-column conv at BK = 64: 3-stage ring");
@@ -132,8 +144,8 @@ static_assert(TcCfg<1, 32, 64, 1>::STAGES == 6, "single-pass 64-column conv at B
 // must order every load after the previous iteration's stores (possible aliasing), which serialised 128
 // global-memory round trips per thread (ncu: 40 % of the stall samples sat on the first use of these loads).
 // The accumulator values are read from the hand-off tile where they are used rather than staged in registers: the
-// epilogue warpgroup runs on TC_EPILOGUE_REGS.  Each epilogue thread arrives on acc_empty right after its last read of
-// the tile, so the consumers can overwrite it while the last stores are still under way.
+// epilogue warpgroup runs on TC_EPILOGUE_REGS.  Both arrive on acc_empty at the end of their last 32-column chunk,
+// while its stores are still under way (the epilogue contract of tc_pipeline).
 template <int BR>
 __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
                                                int a_z, int b_row0) {
@@ -223,22 +235,28 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
 }
 
 // ------------------------------------------------------------------------------------------------
-// GATED / CONV kernel (persistent, see file header).  N per tile is limited to 128 columns: the main and cross
-// accumulators of a consumer warpgroup take 2 x 64 registers per thread.
+// The persistent warp-specialised pipeline of both GEMM kernels (see file header), with the shared-memory layout of
+// Cfg (a RingCfg) and NPL operand planes.  The kernel supplies the parts specific to its GEMM as force-inlined lambdas:
+//   decode(u) -> w                work unit u; w.n_iters is its number of K-iterations (ring stages)
+//   load(w, kit, stage, bar)      the TMA loads of K-iteration kit of w into `stage`, completing on bar (the producer
+//                                 has already armed bar with the stage's Cfg::STAGE bytes)
+//   mma(stage, wg, acc, xacc)     consumer warpgroup wg's MMAs of one stage: p0 x p0 into acc and, with two planes,
+//                                 p0 x p1 + p1 x p0 into xacc (64 rows x NCOLS columns, NCOLS / 2 registers each)
+//   gmain(w)                      the factor of w's main accumulator (TcParams::gmain)
+//   epilogue(w, acc_tile, acc_empty)   stores w's output from the hand-off tile [128][Cfg::ACC_PITCH].  Contract:
+//                                 every epilogue thread arrives on acc_empty exactly once per unit, right after its
+//                                 last read of acc_tile, so the consumers can overwrite the tile while the epilogue's
+//                                 last stores are still under way.
 // ------------------------------------------------------------------------------------------------
-template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
-__global__ void __launch_bounds__(TC_CONV_THREADS, 1)
-tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int tiles_x, int tiles_y,
-               int num_tiles) {
-    pdl_trigger();
+template <class Cfg, int NPL, class Decode, class Load, class Mma, class Gmain, class Epilogue>
+__device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, Decode decode, Load load, Mma mma,
+                                            Gmain gmain, Epilogue epilogue) {
     static_assert(NPL == 1 || NPL == 2, "one or two operand planes");
-    using Cfg = TcCfg<NBOX, BK, BR, NPL>;
-    constexpr int TILE = Cfg::TILE, TILE_B = Cfg::TILE_B, STAGE = Cfg::STAGE, STAGES = Cfg::STAGES, NCOLS = Cfg::NCOLS;
-    constexpr int B_OFF = NPL * TILE;
-    constexpr int NR = NCOLS / 2;                            // registers per accumulator per thread
-    constexpr int A_HALF = 64 * BK * 2;                      // rows [64 wg, 64 wg + 64) of the A tile
-    static_assert(NCOLS <= 128, "main + cross accumulators must fit in the registers of a consumer thread");
-    static_assert(STAGES >= 2, "pipeline needs at least two stages");
+    static_assert(Cfg::NCOLS <= 128, "main + cross accumulators must fit in the registers of a consumer thread");
+    static_assert(Cfg::STAGES >= 2, "pipeline needs at least two stages");
+    constexpr int STAGE = Cfg::STAGE, STAGES = Cfg::STAGES;
+    constexpr int NR = Cfg::NCOLS / 2;                       // registers per accumulator per thread
+    pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     float* acc_tile = reinterpret_cast<float*>(smem + STAGES * STAGE);
@@ -247,7 +265,6 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     uint64_t* acc_full = empty + STAGES;                     // the consumers have written acc_tile (256 arrivals)
     uint64_t* acc_empty = acc_full + 1;                      // the epilogue has read acc_tile (128 arrivals)
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int n_iters = p.k * p.kb_n;
 
     if (threadIdx.x == 0) {
 #pragma unroll
@@ -262,50 +279,25 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
     __syncthreads();
     pdl_wait();                    // everything above overlapped the previous kernel's tail; global memory from here
 
-    // tile id -> (time tile, channel tile, batch); channel tiles vary fastest so that concurrently running CTAs share
-    // the activation tile in L2
-    auto decode = [&](int tile, int& a_row0, int& a_z, int& b_row0, int& b_row1) {
-        const int ty = tile % tiles_y, r = tile / tiles_y;
-        const int tx = r % tiles_x;
-        a_z = r / tiles_x;
-        a_row0 = tx * 128;
-        if (MODE == TC_GATED) { b_row0 = ty * BR; b_row1 = p.Nc + ty * BR; }
-        else { b_row0 = ty * BR * NBOX; b_row1 = b_row0 + BR; }
-    };
-
     if (warp >= 12) {
         setmaxnreg_inc<TC_EPILOGUE_REGS>();                  // up from the launch's 65 536 / 512 = 128 per thread
-        const float* arow = acc_tile + (threadIdx.x & 127) * Cfg::ACC_PITCH;   // this thread's time step
         int n = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
-            int a_row0, a_z, b_row0, b_row1;
-            decode(tile, a_row0, a_z, b_row0, b_row1);
+        for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++n) {
+            const auto w = decode(u);
             mbar_wait(acc_full, n & 1);
-            if (MODE == TC_GATED) epilogue_gated<BR>(p, arow, acc_empty, a_row0, a_z, b_row0);
-            else epilogue_conv<NCOLS>(p, arow, acc_empty, a_row0, a_z, b_row0);
+            epilogue(w, acc_tile, acc_empty);
         }
     } else if (warp >= 8) {
         setmaxnreg_dec<TC_PRODUCER_REGS>();
         if (warp == 8 && lane == 0) {
             int it = 0;
-            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-                int a_row0, a_z, b_row0, b_row1;
-                decode(tile, a_row0, a_z, b_row0, b_row1);
-                for (int kit = 0; kit < n_iters; ++kit, ++it) {
+            for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+                const auto w = decode(u);
+                for (int kit = 0; kit < w.n_iters; ++kit, ++it) {
                     const int s = it % STAGES, ph = (it / STAGES) & 1;
                     mbar_wait(&empty[s], ph ^ 1);
-                    uint8_t* st = smem + s * STAGE;
-                    const int j = kit / p.kb_n, kb = kit - j * p.kb_n;
-                    const int ax = kb * BK, ay = a_row0 + p.tap_off[j];
-                    const int by0 = j * p.rows_per_tap + b_row0, by1 = j * p.rows_per_tap + b_row1;
                     mbar_arrive_expect_tx(&full[s], STAGE);
-#pragma unroll
-                    for (int pl = 0; pl < NPL; ++pl) {
-                        tma_load_3d(st + pl * TILE, &maps.a[pl], &full[s], ax, ay, a_z);
-                        uint8_t* bdst = st + B_OFF + pl * NBOX * TILE_B;
-                        tma_load_3d(bdst, &maps.b[pl], &full[s], ax, by0, 0);
-                        if (NBOX == 2) tma_load_3d(bdst + TILE_B, &maps.b[pl], &full[s], ax, by1, 0);
-                    }
+                    load(w, kit, smem + s * STAGE, &full[s]);
                 }
             }
         }
@@ -316,47 +308,96 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         // ptxas serialises every wgmma of the chain.
         float acc[NR], xacc[NPL == 2 ? NR : 1];              // main (p0 x p0), cross (p0 x p1 + p1 x p0)
         int it = 0, n = 0;
-        for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++n) {
-            int a_row0, a_z, b_row0, b_row1;
-            decode(tile, a_row0, a_z, b_row0, b_row1);
+        for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++n) {
+            const auto w = decode(u);
 #pragma unroll
             for (int i = 0; i < NR; ++i) {
                 acc[i] = 0.f;
                 if constexpr (NPL == 2) xacc[i] = 0.f;
             }
-            for (int kit = 0; kit < n_iters; ++kit, ++it) {
+            for (int kit = 0; kit < w.n_iters; ++kit, ++it) {
                 const int s = it % STAGES, ph = (it / STAGES) & 1;
                 mbar_wait(&full[s], ph);
-                const uint32_t sa = smem_u32(smem + s * STAGE) + wg * A_HALF;
-                const uint32_t sb = smem_u32(smem + s * STAGE + B_OFF);
                 wgmma_fence();
-#pragma unroll
-                for (int kk = 0; kk < BK / 16; ++kk) {
-                    const uint32_t ko = kk * 32;
-                    const uint64_t a0 = make_desc<BK>(sa + ko), b0 = make_desc<BK>(sb + ko);
-                    wgmma_mma<NCOLS, 0, 0>(BF16, acc, a0, b0, 1);
-                    if constexpr (NPL == 2) {
-                        const uint64_t a1 = make_desc<BK>(sa + TILE + ko), b1 = make_desc<BK>(sb + NBOX * TILE_B + ko);
-                        wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a0, b1, 1);
-                        wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a1, b0, 1);
-                    }
-                }
+                mma(smem + s * STAGE, wg, acc, xacc);
                 wgmma_commit();
                 wgmma_wait<1>();                                  // the previous stage's MMAs have retired
                 if (kit > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
             }
             wgmma_wait<0>();
-            if (n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
-            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous tile
+            if (w.n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
+            const float gm = gmain(w);
+            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous unit
 #pragma unroll
             for (int i = 0; i < NR; ++i) {                            // lo planes carry 2^11
                 float* dst = &acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)];
-                if constexpr (NPL == 2) *dst = fmaf(xacc[i], LO_INV, acc[i] * p.gmain);
-                else *dst = acc[i] * p.gmain;
+                if constexpr (NPL == 2) *dst = fmaf(xacc[i], LO_INV, acc[i] * gm);
+                else *dst = acc[i] * gm;
             }
             mbar_arrive(acc_full);
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------
+// GATED / CONV kernel.  A unit is one output tile; tile ids run channel tiles fastest, then time tiles, then the
+// batch, so that concurrently running CTAs share the activation tile in L2.  N per tile is limited to 128 columns.
+// ------------------------------------------------------------------------------------------------
+template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
+__global__ void __launch_bounds__(TC_CONV_THREADS, 1)
+tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int tiles_x, int tiles_y,
+               int num_tiles) {
+    using Cfg = TcCfg<NBOX, BK, BR, NPL>;
+    constexpr int NCOLS = Cfg::NCOLS;
+    constexpr int TILE = 128 * BK * 2, TILE_B = BR * BK * 2;   // one plane of the A tile (128 rows), one B box
+    constexpr int B_OFF = NPL * TILE;
+    constexpr int A_HALF = 64 * BK * 2;                      // rows [64 wg, 64 wg + 64) of the A tile
+    const int n_iters = p.k * p.kb_n;
+
+    struct Tile { int a_row0, a_z, b_row0, b_row1, n_iters; };
+    auto decode = [&](int tile) {
+        Tile w;
+        const int ty = tile % tiles_y, r = tile / tiles_y;
+        w.a_z = r / tiles_x;
+        w.a_row0 = (r % tiles_x) * 128;
+        if (MODE == TC_GATED) { w.b_row0 = ty * BR; w.b_row1 = p.Nc + ty * BR; }
+        else { w.b_row0 = ty * BR * NBOX; w.b_row1 = w.b_row0 + BR; }
+        w.n_iters = n_iters;
+        return w;
+    };
+    auto load = [&](const Tile& w, int kit, uint8_t* st, uint64_t* bar) {
+        const int j = kit / p.kb_n, kb = kit - j * p.kb_n;
+        const int ax = kb * BK, ay = w.a_row0 + p.tap_off[j];
+        const int by0 = j * p.rows_per_tap + w.b_row0, by1 = j * p.rows_per_tap + w.b_row1;
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) {
+            tma_load_3d(st + pl * TILE, &maps.a[pl], bar, ax, ay, w.a_z);
+            uint8_t* bdst = st + B_OFF + pl * NBOX * TILE_B;
+            tma_load_3d(bdst, &maps.b[pl], bar, ax, by0, 0);
+            if (NBOX == 2) tma_load_3d(bdst + TILE_B, &maps.b[pl], bar, ax, by1, 0);
+        }
+    };
+    auto mma = [&](const uint8_t* st, int wg, float* acc, float* xacc) {
+        const uint32_t sa = smem_u32(st) + wg * A_HALF, sb = smem_u32(st + B_OFF);
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk) {
+            const uint32_t ko = kk * 32;
+            const uint64_t a0 = make_desc<BK>(sa + ko), b0 = make_desc<BK>(sb + ko);
+            wgmma_mma<NCOLS, 0, 0>(BF16, acc, a0, b0, 1);
+            if constexpr (NPL == 2) {
+                const uint64_t a1 = make_desc<BK>(sa + TILE + ko), b1 = make_desc<BK>(sb + NBOX * TILE_B + ko);
+                wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a0, b1, 1);
+                wgmma_mma<NCOLS, 0, 0>(BF16, xacc, a1, b0, 1);
+            }
+        }
+    };
+    auto gmain = [&](const Tile&) { return p.gmain; };
+    auto epilogue = [&](const Tile& w, const float* acc_tile, uint64_t* acc_empty) {
+        const float* arow = acc_tile + (threadIdx.x & 127) * Cfg::ACC_PITCH;   // this thread's time step
+        if (MODE == TC_GATED) epilogue_gated<BR>(p, arow, acc_empty, w.a_row0, w.a_z, w.b_row0);
+        else epilogue_conv<NCOLS>(p, arow, acc_empty, w.a_row0, w.a_z, w.b_row0);
+    };
+    tc_pipeline<Cfg, NPL>(maps, num_tiles, decode, load, mma, gmain, epilogue);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -369,13 +410,9 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
 // conv padding), so no time-shifted copies of the input are needed.
 //
 // A work unit is one 128 (m) x 128 (n) tile of one tap j and one split s: the sum over the utterances
-// [s * bps, min(B, (s + 1) * bps)) of the split, all their 32-row time chunks, written to slot s.  The kernel is
-// PERSISTENT with the warp roles of tc_conv_kernel: min(units, SMs) CTAs, CTA c walks units c, c + grid, ... of a
-// fixed list in which the split index varies slowest, so every split but the last (the only one that can be short)
-// comes first: units run longest first.  The producer streams the next unit's chunks straight after the current
-// one's; the consumers hand each finished tile to the epilogue warpgroup through a shared-memory fp32 tile and go on
-// to the next unit's MMAs while the epilogue stores it.  The schedule, and with it every value, is a function of the
-// shape and the SM count.
+// [s * bps, min(B, (s + 1) * bps)) of the split, all their 32-row time chunks, written to slot s.  In the unit list the
+// split index varies slowest, so every split but the last (the only one that can be short) comes first: units run
+// longest first.  The schedule, and with it every value, is a function of the shape and the SM count.
 // ------------------------------------------------------------------------------------------------
 struct TcMnParams {
     int T, B, Mw, Nw, k;
@@ -388,17 +425,10 @@ struct TcMnParams {
 };
 
 constexpr int WG_BOX = 64 * 32 * 2;                      // 64 channels x 32 time steps of bf16 = 4 KB
-// per plane: 128 channels of m, 128 channels of n; NPL planes per stage.  The hand-off tile [128 m][128 n + 1] fp32
-// (66 KB; the odd pitch keeps both epilogue access patterns conflict-free) leaves room for five 32 KB two-plane stages.
+// Per plane: 128 channels of m, 128 channels of n.  The hand-off tile [128 m][128 n + 1] fp32 (66 KB; the odd pitch
+// keeps both epilogue access patterns conflict-free) leaves room for five 32 KB two-plane stages.
 template <int NPL>
-struct WgCfg {
-    static constexpr int STAGE = NPL * (2 * WG_BOX + 2 * WG_BOX);
-    static constexpr int ACC_PITCH = 128 + 1;
-    static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - ACC_TILE) / STAGE;
-    static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-    static constexpr int SMEM = STAGES * STAGE + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
-};
+using WgCfg = RingCfg<NPL * 4 * WG_BOX, 128, 0>;
 static_assert(WgCfg<2>::STAGES == 5, "two-plane weight gradient: 5-stage ring");
 static_assert(WgCfg<1>::STAGES == 6, "single-pass weight gradient: 6-stage ring");
 static_assert(WgCfg<2>::SMEM <= SMEM_LIMIT && WgCfg<1>::SMEM <= SMEM_LIMIT, "weight gradient shared memory");
@@ -406,33 +436,9 @@ static_assert(WgCfg<2>::SMEM <= SMEM_LIMIT && WgCfg<1>::SMEM <= SMEM_LIMIT, "wei
 template <int NPL>
 __global__ void __launch_bounds__(TC_CONV_THREADS, 1)
 tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcMnParams p) {
-    pdl_trigger();
-    static_assert(NPL == 1 || NPL == 2, "one or two operand planes");
     using Cfg = WgCfg<NPL>;
-    constexpr int WG_STAGE = Cfg::STAGE, WG_STAGES = Cfg::STAGES;
     constexpr int A_PL = 2 * WG_BOX, B_PL = 2 * WG_BOX;
     constexpr uint32_t LBO = 4096, SBO = 1024;           // 64-channel chunks one TMA box apart; 8-row groups 1 KB apart
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-    float* acc_tile = reinterpret_cast<float*>(smem + WG_STAGES * WG_STAGE);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE + Cfg::ACC_TILE);
-    uint64_t* empty = full + WG_STAGES;
-    uint64_t* acc_full = empty + WG_STAGES;                  // the consumers have written acc_tile (256 arrivals)
-    uint64_t* acc_empty = acc_full + 1;                      // the epilogue has read acc_tile (128 arrivals)
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-    if (threadIdx.x == 0) {
-#pragma unroll
-        for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.a[pl]);
-#pragma unroll
-        for (int pl = 0; pl < NPL; ++pl) prefetch_tmap(&maps.b[pl]);
-        for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        mbar_init(acc_full, 256);
-        mbar_init(acc_empty, 128);
-        fence_barrier_init();
-    }
-    __syncthreads();
-    pdl_wait();
 
     // unit -> (m0, n0, tap, split, first utterance, K-iterations)
     struct Unit { int m0, n0, j, s, b_beg, n_iters; };
@@ -449,113 +455,65 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
         w.n_iters = (b_end > w.b_beg ? b_end - w.b_beg : 0) * p.kb_n;
         return w;
     };
-
-    if (warp >= 12) {
-        setmaxnreg_inc<TC_EPILOGUE_REGS>();
-        // Tap-major layout (s_n == 1): thread r owns column n0 + r and walks the rows, a warp storing 32 consecutive
-        // floats of one row.  Otherwise (ConvTranspose layout, consecutive m two floats apart): thread r owns row
-        // m0 + r and walks the columns.
+    auto load = [&](const Unit& w, int kit, uint8_t* st, uint64_t* bar) {
+        const int bi = kit / p.kb_n, tc_ = kit - bi * p.kb_n;
+        const int b = w.b_beg + bi, t0 = tc_ * 32;
+#pragma unroll
+        for (int pl = 0; pl < NPL; ++pl) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                tma_load_3d(st + pl * A_PL + h * WG_BOX, &maps.a[pl], bar, w.m0 + h * 64, t0, b);
+#pragma unroll
+            for (int q = 0; q < 2; ++q)
+                tma_load_3d(st + NPL * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], bar, w.n0 + q * 64,
+                            t0 + p.tap_off[w.j], b);
+        }
+    };
+    // A = gradient planes, B = the bf16 copy of the forward operand planes; both MN-major
+    auto mma = [&](const uint8_t* st, int wg, float* acc, float* xacc) {
+        const uint32_t sa = smem_u32(st);
+#pragma unroll
+        for (int kk = 0; kk < 2; ++kk) {                        // 2 x K = 16 rows of 128 B
+            const uint32_t ko = kk * 16 * 128;
+            const uint64_t a0 = make_wgmma_desc(sa + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+            const uint64_t b0 = make_wgmma_desc(sa + NPL * A_PL + ko, LBO, SBO, WG_SW128);
+            wgmma_mma<128, 1, 1>(true, acc, a0, b0, 1);
+            if constexpr (NPL == 2) {
+                const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
+                const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
+                wgmma_mma<128, 1, 1>(true, xacc, a0, b1, 1);
+                wgmma_mma<128, 1, 1>(true, xacc, a1, b0, 1);
+            }
+        }
+    };
+    auto gmain = [&](const Unit& w) { return 1.f + p.gcoef * (float)(2 * w.n_iters); };
+    // Tap-major layout (s_n == 1): thread r owns column n0 + r and walks the rows, a warp storing 32 consecutive floats
+    // of one row.  Otherwise (ConvTranspose layout, consecutive m two floats apart): thread r owns row m0 + r and walks
+    // the columns.
+    auto epilogue = [&](const Unit& w, const float* acc_tile, uint64_t* acc_empty) {
         const int r = threadIdx.x & 127;
-        int n = 0;
-        for (int u = blockIdx.x; u < p.num_units; u += gridDim.x, ++n) {
-            const Unit w = decode(u);
-            float* __restrict__ out = p.dw + (size_t)w.s * p.split_stride + (size_t)w.j * p.s_j;
-            const int rows = min(128, p.Mw - w.m0), cols = min(128, p.Nw - w.n0);
-            mbar_wait(acc_full, n & 1);
-            if (p.s_n == 1) {
-                if (r < cols) {
-                    float* __restrict__ o = out + w.n0 + r;
+        float* __restrict__ out = p.dw + (size_t)w.s * p.split_stride + (size_t)w.j * p.s_j;
+        const int rows = min(128, p.Mw - w.m0), cols = min(128, p.Nw - w.n0);
+        if (p.s_n == 1) {
+            if (r < cols) {
+                float* __restrict__ o = out + w.n0 + r;
 #pragma unroll 4
-                    for (int i = 0; i < rows; ++i) {
-                        const int m = w.m0 + i;
-                        o[(size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh] = acc_tile[i * Cfg::ACC_PITCH + r];
-                    }
+                for (int i = 0; i < rows; ++i) {
+                    const int m = w.m0 + i;
+                    o[(size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh] = acc_tile[i * Cfg::ACC_PITCH + r];
                 }
-            } else if (r < rows) {
-                const int m = w.m0 + r;
-                float* __restrict__ o = out + (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh +
-                                        (size_t)w.n0 * p.s_n;
-                const float* arow = acc_tile + r * Cfg::ACC_PITCH;
+            }
+        } else if (r < rows) {
+            const int m = w.m0 + r;
+            float* __restrict__ o = out + (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh +
+                                    (size_t)w.n0 * p.s_n;
+            const float* arow = acc_tile + r * Cfg::ACC_PITCH;
 #pragma unroll 4
-                for (int c = 0; c < cols; ++c) o[(size_t)c * p.s_n] = arow[c];
-            }
-            mbar_arrive(acc_empty);
+            for (int c = 0; c < cols; ++c) o[(size_t)c * p.s_n] = arow[c];
         }
-    } else if (warp >= 8) {
-        setmaxnreg_dec<TC_PRODUCER_REGS>();
-        if (warp == 8 && lane == 0) {
-            int it = 0;
-            for (int u = blockIdx.x; u < p.num_units; u += gridDim.x) {
-                const Unit w = decode(u);
-                for (int kit = 0; kit < w.n_iters; ++kit, ++it) {
-                    const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
-                    mbar_wait(&empty[s], ph ^ 1);
-                    uint8_t* st = smem + s * WG_STAGE;
-                    const int bi = kit / p.kb_n, tc_ = kit - bi * p.kb_n;
-                    const int b = w.b_beg + bi, t0 = tc_ * 32;
-                    mbar_arrive_expect_tx(&full[s], WG_STAGE);
-#pragma unroll
-                    for (int pl = 0; pl < NPL; ++pl) {
-#pragma unroll
-                        for (int h = 0; h < 2; ++h)
-                            tma_load_3d(st + pl * A_PL + h * WG_BOX, &maps.a[pl], &full[s], w.m0 + h * 64, t0, b);
-#pragma unroll
-                        for (int q = 0; q < 2; ++q)
-                            tma_load_3d(st + NPL * A_PL + pl * B_PL + q * WG_BOX, &maps.b[pl], &full[s], w.n0 + q * 64,
-                                        t0 + p.tap_off[w.j], b);
-                    }
-                }
-            }
-        }
-    } else {
-        setmaxnreg_inc<TC_CONSUMER_REGS>();
-        // A = gradient planes, B = the bf16 copy of the forward operand planes; both MN-major.  Two disjoint register
-        // tuples: an MMA in flight may not share accumulator registers with the next one.
-        const int wg = warp >> 2, wq = warp & 3;
-        float acc[64], xacc[NPL == 2 ? 64 : 1];              // main (p0 x p0), cross (p0 x p1 + p1 x p0)
-        int it = 0, n = 0;
-        for (int u = blockIdx.x; u < p.num_units; u += gridDim.x, ++n) {
-            const Unit w = decode(u);
-#pragma unroll
-            for (int i = 0; i < 64; ++i) {
-                acc[i] = 0.f;
-                if constexpr (NPL == 2) xacc[i] = 0.f;
-            }
-            for (int kit = 0; kit < w.n_iters; ++kit, ++it) {
-                const int s = it % WG_STAGES, ph = (it / WG_STAGES) & 1;
-                mbar_wait(&full[s], ph);
-                const uint32_t sa = smem_u32(smem + s * WG_STAGE);
-                wgmma_fence();
-#pragma unroll
-                for (int kk = 0; kk < 2; ++kk) {                        // 2 x K = 16 rows of 128 B
-                    const uint32_t ko = kk * 16 * 128;
-                    const uint64_t a0 = make_wgmma_desc(sa + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
-                    const uint64_t b0 = make_wgmma_desc(sa + NPL * A_PL + ko, LBO, SBO, WG_SW128);
-                    wgmma_mma<128, 1, 1>(true, acc, a0, b0, 1);
-                    if constexpr (NPL == 2) {
-                        const uint64_t a1 = make_wgmma_desc(sa + A_PL + wg * WG_BOX + ko, LBO, SBO, WG_SW128);
-                        const uint64_t b1 = make_wgmma_desc(sa + 2 * A_PL + B_PL + ko, LBO, SBO, WG_SW128);
-                        wgmma_mma<128, 1, 1>(true, xacc, a0, b1, 1);
-                        wgmma_mma<128, 1, 1>(true, xacc, a1, b0, 1);
-                    }
-                }
-                wgmma_commit();
-                wgmma_wait<1>();
-                if (kit > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
-            }
-            wgmma_wait<0>();
-            if (w.n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % WG_STAGES]);
-            const float gmain = 1.f + p.gcoef * (float)(2 * w.n_iters);
-            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous unit
-#pragma unroll
-            for (int i = 0; i < 64; ++i) {                            // lo planes carry 2^11
-                float* dst = &acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)];
-                if constexpr (NPL == 2) *dst = fmaf(xacc[i], LO_INV, acc[i] * gmain);
-                else *dst = acc[i] * gmain;
-            }
-            mbar_arrive(acc_full);
-        }
-    }
+        mbar_arrive(acc_empty);
+    };
+    tc_pipeline<Cfg, NPL>(maps, p.num_units, decode, load, mma, gmain, epilogue);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -604,20 +562,23 @@ static int ensure_smem(K kern, int bytes, const char* what) {
     return 0;
 }
 
-template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
-static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
-                       const char* what) {
-    using Cfg = TcCfg<NBOX, BK, BR, NPL>;
-    auto kern = tc_conv_kernel<MODE, NBOX, BR, BK, BF16, NPL>;
+// Persistent launch of a tc_pipeline kernel with the shared-memory layout Cfg: min(units, SMs) CTAs.
+template <class Cfg, auto kern, typename... Args>
+static int launch_persistent(int units, cudaStream_t st, const char* what, const Args&... args) {
     static const int configured = ensure_smem(kern, Cfg::SMEM, what);       // once per instantiation, thread-safe
     if (configured) return 1;
-    const int sms = config().sms;
-    const int num_tiles = tiles_x * tiles_y * batch;
-    const int grid = num_tiles < sms ? num_tiles : sms;
-    cudaError_t e = launch_k(kern, dim3(grid), dim3(TC_CONV_THREADS), (size_t)Cfg::SMEM, st, maps, p, tiles_x, tiles_y,
-                             num_tiles);
+    const int sms = config().sms, grid = units < sms ? units : sms;
+    cudaError_t e = launch_k(kern, dim3(grid), dim3(TC_CONV_THREADS), (size_t)Cfg::SMEM, st, args...);
     if (e != cudaSuccess) { set_error("%s: launch failed: %s", what, cudaGetErrorString(e)); return 1; }
     return check_launch(what);
+}
+
+template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
+static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
+                           const char* what) {
+    const int num_tiles = tiles_x * tiles_y * batch;
+    return launch_persistent<TcCfg<NBOX, BK, BR, NPL>, tc_conv_kernel<MODE, NBOX, BR, BK, BF16, NPL>>(
+        num_tiles, st, what, maps, p, tiles_x, tiles_y, num_tiles);
 }
 
 template <int MODE, int NBOX, int BR, int BK, int NPL = 2>
@@ -676,15 +637,16 @@ int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bi
                                 (uint64_t)C * 2, (uint64_t)k * 2 * C * C * 2, BK, 64)) return 1;
     }
     TcParams p = {};
-    p.T = T; p.B = B; p.Kc = C; p.Nc = C; p.rows_per_tap = 2 * C; p.k = k; p.kb_n = C / BK;
+    p.T = T; p.Nc = C; p.rows_per_tap = 2 * C; p.k = k; p.kb_n = C / BK;
     fill_taps_tc(p.tap_off, k, dilation, causal, false);
     p.bias = bias; p.spk = spk; p.res = res; p.y = y; p.save_a = save_a; p.save_s = save_s;
     p.gate_mode = mode; p.residual = residual;
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (BK / 16));
-    p.operand_bf16 = 0;                                          // forward operands: fp16 planes
     cudaStream_t st = (cudaStream_t)stream;
-    if (npl == 1) return launch_conv<TC_GATED, 2, 64, 64, 1>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
-    return launch_conv<TC_GATED, 2, 64, 32>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
+    // forward operands: fp16 planes (BF16 = false)
+    if (npl == 1)
+        return launch_conv_fmt<TC_GATED, 2, 64, 64, false, 1>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
+    return launch_conv_fmt<TC_GATED, 2, 64, 32, false, 2>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
 }
 
 // Generic conv / data-gradient:  out (B, Nc, T) fp32 = sum_j A[b, t+off_j, :] . W[j, n, :]  (+ epilogue)
@@ -717,7 +679,7 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
                                 (uint64_t)Kp * 2, (uint64_t)k * Nc * Kp * 2, bk, br)) return 1;
     }
     TcParams p = {};
-    p.T = T; p.B = B; p.Kc = Kc; p.Nc = Nc; p.rows_per_tap = Nc; p.k = k; p.kb_n = (Kc + bk - 1) / bk;
+    p.T = T; p.Nc = Nc; p.rows_per_tap = Nc; p.k = k; p.kb_n = (Kc + bk - 1) / bk;
     fill_taps_tc(p.tap_off, k, dilation, causal, transpose_taps != 0);
     p.out = out; p.bias = bias; p.relu = relu; p.e1 = e1; p.e2 = e2; p.alpha = alpha; p.addmode = addmode;
     p.p_drop = p_drop; p.seed_ptr = seed_ptr; p.salt = salt;
@@ -805,20 +767,10 @@ int dv3_tc_wgrad_mn_npl(const void* dy, const void* xd, int npl, float* dw_parti
     p.dw = dw_partials; p.split_stride = split_stride;
     p.msplit = msplit; p.s_m = s_m; p.s_mh = s_mh; p.s_n = s_n; p.s_j = s_j;
     p.gcoef = config().tc_gamma;
-    const int sms = config().sms, grid = p.num_units < sms ? p.num_units : sms;
     cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e;
-    if (npl == 1) {
-        static const int configured = ensure_smem(tc_wgrad_mn_kernel<1>, WgCfg<1>::SMEM, "tc_wgrad_mn");
-        if (configured) return 1;
-        e = launch_k(tc_wgrad_mn_kernel<1>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)WgCfg<1>::SMEM, st, maps, p);
-    } else {
-        static const int configured = ensure_smem(tc_wgrad_mn_kernel<2>, WgCfg<2>::SMEM, "tc_wgrad_mn");
-        if (configured) return 1;
-        e = launch_k(tc_wgrad_mn_kernel<2>, dim3(grid), dim3(TC_CONV_THREADS), (size_t)WgCfg<2>::SMEM, st, maps, p);
-    }
-    if (e != cudaSuccess) { set_error("tc_wgrad_mn: launch failed: %s", cudaGetErrorString(e)); return 1; }
-    return check_launch("tc_wgrad_mn");
+    if (npl == 1)
+        return launch_persistent<WgCfg<1>, tc_wgrad_mn_kernel<1>>(p.num_units, st, "tc_wgrad_mn", maps, p);
+    return launch_persistent<WgCfg<2>, tc_wgrad_mn_kernel<2>>(p.num_units, st, "tc_wgrad_mn", maps, p);
 }
 
 int dv3_tc_wgrad_mn(const void* dy, const void* xd, float* dw_partials, long long split_stride, int B, int Mw,

@@ -41,10 +41,13 @@ def _kernels(report):
     return kernels
 
 
-def test_every_single_pass_instantiation_is_compiled(report):
+def test_every_single_pass_instantiation_is_compiled_gated_fp16_only(report):
     names = list(_kernels(report))
-    # gated forward + 4 conv configurations, each for fp16 and bf16 operands; one weight-gradient kernel
-    assert sum("tc_conv_kernel" in n for n in names) == 10, names
+    # gated forward (fp16 operands only: it is always a forward GEMM) + 4 conv configurations, each for fp16 and bf16
+    # operands; one weight-gradient kernel
+    assert sum("tc_conv_kernel" in n for n in names) == 9, names
+    gated = [n for n in names if "tc_conv_kernelILi0E" in n]      # MODE = TC_GATED
+    assert len(gated) == 1 and "ELb0ELi1E" in gated[0], gated     # BF16 = false
     assert sum("tc_wgrad_mn_kernel" in n for n in names) == 1, names
 
 
