@@ -124,21 +124,23 @@ def main():
     x = torch.zeros(args.clips, n_max, device="cuda")
     prev = torch.zeros_like(spec)
     beta = hp.griffin_lim_momentum / (1.0 + hp.griffin_lim_momentum)
+    g = audio.check_geometry(mel=False)
+    tab = audio._geometry_table(batch.device, g.n_fft, g.hop)
 
     def stft_plain():
-        lib.call("dv3_stft_complex_batched", vp(x), vp(samples_d), n_max, vp(batch), vp(spec), vp(frames_d), T_max,
-                 args.clips, ctypes.c_void_p(st))
+        lib.call("dv3_stft_complex_geom", vp(x), vp(samples_d), n_max, vp(batch), vp(spec), vp(frames_d), T_max,
+                 args.clips, vp(tab), g.n_fft, g.hop, ctypes.c_void_p(st))
 
     def stft_momentum():
-        lib.call("dv3_stft_complex_momentum_batched", vp(x), vp(samples_d), n_max, vp(batch), vp(prev), vp(spec),
-                 vp(frames_d), T_max, args.clips, beta, ctypes.c_void_p(st))
+        lib.call("dv3_stft_complex_momentum_geom", vp(x), vp(samples_d), n_max, vp(batch), vp(prev), vp(spec),
+                 vp(frames_d), T_max, args.clips, beta, vp(tab), g.n_fft, g.hop, ctypes.c_void_p(st))
 
     def gl_iterations(stft, n=20):
         for _ in range(n):
             stft()
             x.zero_()
-            lib.call("dv3_istft_batched", vp(spec), vp(x), vp(samples_d), n_max, vp(frames_d), T_max, args.clips,
-                     ctypes.c_void_p(st))
+            lib.call("dv3_istft_geom", vp(spec), vp(x), vp(samples_d), n_max, vp(frames_d), T_max, args.clips,
+                     vp(tab), g.n_fft, g.hop, ctypes.c_void_p(st))
 
     def stft_launches(stft, n=20):
         for _ in range(n):

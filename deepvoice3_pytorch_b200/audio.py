@@ -6,13 +6,15 @@ transform on a training batch's waveforms and writes the padded, decimated targe
 (training from wav files, ``data.WavDataset``).
 
 ``inv_spectrogram`` (reference audio.py:37-43) recovers the phase on the same STFT frame with Griffin-Lim (the default,
-csrc/istft.cu), with fast Griffin-Lim (``method="fast_griffin_lim"``: Griffin-Lim with momentum, as librosa and
+csrc/stft_any.cu), with fast Griffin-Lim (``method="fast_griffin_lim"``: Griffin-Lim with momentum, as librosa and
 torchaudio run it by default) or with Local Weighted Sums (``method="lws"``, csrc/lws.cu), the algorithm of the
 reference's ``lws.run_lws``.  The ``lws`` package is an un-vendored dependency whose source is absent, so parity with it is unpinned.
 
 The STFT frame is ``hparams.fft_size`` / ``hparams.hop_size``, as in the reference.  ``check_geometry`` decides which
-frames are supported: at 1024 / 256 (every reference preset) the specialised kernels run; any other supported frame
-runs the general kernels of csrc/stft_any.cu and csrc/lws_any.cu (DESIGN.md, "Other STFT geometries").
+frames are supported.  The forward transform and LWS have specialised kernels at 1024 / 256 (every reference preset;
+csrc/stft.cu, csrc/lws.cu) and run the general ones of csrc/stft_any.cu and csrc/lws_any.cu at any other supported
+frame; Griffin-Lim's complex STFT and the inverse STFT run the general kernels of csrc/stft_any.cu at every frame
+(DESIGN.md, "Other STFT geometries").
 """
 import ctypes
 from collections import namedtuple
@@ -57,7 +59,8 @@ def check_geometry(mel=True):
     n_fft / hop in [2, 8] -- an integer overlap, the only case where the squared windows sqrt(hann * 2 hop / n_fft) sum
     to exactly 1, so that the inverse STFT can use the analysis window as its synthesis window.  ``mel``: also the
     filterbank rules of the forward path (num_mels <= 128, fmax <= sample_rate / 2).  Host values only; every audio entry
-    point calls it before anything is allocated or launched.  ``default`` (1024 / 256) selects the specialised kernels."""
+    point calls it before anything is allocated or launched.  ``default`` (1024 / 256) selects the specialised forward
+    and LWS kernels (csrc/stft.cu, csrc/lws.cu); Griffin-Lim and the inverse STFT are the same at every frame."""
     hp = hparams
     N, R = hp.fft_size, hp.hop_size
     if int(N) != N or int(R) != R:
@@ -591,12 +594,12 @@ def griffin_lim_batch(mag, n_frames, n_iter=None, momentum=0.0):
     """mag: (nclips, T_max, K) fp32 CUDA tensor (K = fft_size // 2 + 1), clip c valid for its first n_frames[c] frames -> waveforms
     (nclips, n_max), clip c valid for its first inv_num_samples(n_frames[c]) samples and zero after them.  Each clip
     comes out bit-identical to ``griffin_lim`` on that clip alone: the kernels read and write only a clip's own frames
-    and samples, and the overlap-add is deterministic (csrc/istft.cu).
+    and samples, and the overlap-add is deterministic (csrc/stft_any.cu).
 
     momentum: 0 (the default) runs plain Griffin-Lim.  0 < momentum < 1 runs fast Griffin-Lim (Perraudin, Balazs &
     Sondergaard, WASPAA 2013; librosa's and torchaudio's ``momentum``): each iteration projects
     C = X - beta * X_prev, beta = momentum / (1 + momentum), instead of the new spectrum X, where X_prev is the previous
-    iteration's X (0 before the first); csrc/istft.cu stft_complex_momentum_kernel, csrc/stft_any.cu at other frames.
+    iteration's X (0 before the first); csrc/stft_any.cu stft_complex_momentum_any_kernel.
     Any other value raises ValueError before anything is allocated or launched."""
     momentum = _check_momentum(momentum)
     mag, n_max, frames_d, samples_d, st, g = _ragged_clips(mag, n_frames, "griffin_lim_batch")
@@ -605,43 +608,29 @@ def griffin_lim_batch(mag, n_frames, n_iter=None, momentum=0.0):
     spec = torch.zeros(nclips, T_max, g.bins, 2, device=dev)
     spec[..., 0] = mag                                   # zero phase
     x = torch.zeros(nclips, n_max, device=dev)
+    tab = _geometry_table(dev, g.n_fft, g.hop)
     if momentum:
         prev = torch.zeros_like(spec)
         beta = momentum / (1.0 + momentum)               # fp64 here, rounded to fp32 once by the call
-        if g.default:
-            def stft(x, spec):
-                lib.call("dv3_stft_complex_momentum_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(prev),
-                         _cp(spec), _cp(frames_d), T_max, nclips, beta, st)
-        else:
-            tab = _geometry_table(dev, g.n_fft, g.hop)
 
-            def stft(x, spec):
-                lib.call("dv3_stft_complex_momentum_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(prev),
-                         _cp(spec), _cp(frames_d), T_max, nclips, beta, _cp(tab), g.n_fft, g.hop, st)
-    elif g.default:
         def stft(x, spec):
-            lib.call("dv3_stft_complex_batched", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
-                     T_max, nclips, st)
+            lib.call("dv3_stft_complex_momentum_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(prev),
+                     _cp(spec), _cp(frames_d), T_max, nclips, beta, _cp(tab), g.n_fft, g.hop, st)
     else:
-        tab = _geometry_table(dev, g.n_fft, g.hop)
-
         def stft(x, spec):
             lib.call("dv3_stft_complex_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
                      T_max, nclips, _cp(tab), g.n_fft, g.hop, st)
-    _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g)
+    _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g, tab)
     for _ in range(hparams.griffin_lim_iters if n_iter is None else n_iter):
         stft(x, spec)
         x.zero_()
-        _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g)
+        _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g, tab)
     return x
 
 
-def _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g):
-    if g.default:
-        lib.call("dv3_istft_batched", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, st)
-    else:
-        lib.call("dv3_istft_geom", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips,
-                 _cp(_geometry_table(x.device, g.n_fft, g.hop)), g.n_fft, g.hop, st)
+def _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g, tab):
+    lib.call("dv3_istft_geom", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, _cp(tab), g.n_fft,
+             g.hop, st)
 
 
 def _lws_weights_fp64(N=1024, R=256):
@@ -650,7 +639,7 @@ def _lws_weights_fp64(N=1024, R=256):
     csrc/lws.cu (N = 1024, R = 256: (7, 11)) and csrc/lws_any.cu."""
     Q = N // R
     n = np.arange(N)
-    w = np.sqrt(0.5 * (1.0 - np.cos(2.0 * np.pi * (n + 0.5) / N)) * 2.0 * R / N)     # istft.cu frame_window
+    w = np.sqrt(0.5 * (1.0 - np.cos(2.0 * np.pi * (n + 0.5) / N)) * 2.0 * R / N)     # _geometry_table_fp64's window
     beta = np.zeros((2 * Q - 1, 11), dtype=np.complex128)
     for q in range(-(Q - 1), Q):
         j = n - q * R
@@ -729,7 +718,7 @@ def lws_batch(mag, n_frames, n_iter=None, init_iters=1):
                      g.n_fft, g.hop, st)
         spec, other = other, spec
     x = torch.zeros(nclips, n_max, device=dev)
-    _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g)
+    _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g, _geometry_table(dev, g.n_fft, g.hop))
     return x
 
 

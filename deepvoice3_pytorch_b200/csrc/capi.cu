@@ -46,6 +46,6 @@ int check_launch(const char* what) {
 
 extern "C" {
 const char* dv3_last_error(void) { return dv3::g_err; }
-int dv3_abi_version(void) { return 1; }
+int dv3_abi_version(void) { return 2; }
 long long dv3_launch_count(void) { return (long long)dv3::launch_count(); }
 }

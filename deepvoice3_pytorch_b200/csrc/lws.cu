@@ -3,7 +3,7 @@
 // published algorithm and parity with lws.run_lws is UNPINNED (like the forward STFT, DESIGN.md section 3).  The
 // magnitude-threshold schedule of the package (it skips small bins to save CPU time) and online LWS are not done.
 //
-// Frame: istft.cu's (N = 1024, hop R = 256, synthesis window = analysis window w, K = 513 bins).  X is a (T, 513)
+// Frame: the default one (N = 1024, hop R = 256, synthesis window = analysis window w, K = 513 bins).  X is a (T, 513)
 // complex half spectrum, A the target magnitude.  Weights, computed once on the host in fp64 (audio._lws_weights):
 //     beta_q(d) = (1/N) sum_n w(n) w(n - qR) e^{-2 pi i d n / N},   q in [-3, 3], d in [-5, 5]
 // Local weighted sum (the complex-linear part of STFT(iSTFT(X)) minus the bin's own term):
@@ -13,7 +13,8 @@
 // conj X(m, -k'), bins k' > 512 read conj X(m, 1024 - k').  Frames outside [0, T_c) contribute 0: exact away from the
 // clip's ends, an approximation in its first and last 3 frames, where the inverse STFT crops the 768 padding samples.
 // Update: X <- A Y / |Y| (A + 0i where Y == 0).  Bins 0 and 512 are set real, A sign(Re Y) (+A where Re Y == 0): their
-// Y is real in exact arithmetic, and istft_kernel folds an imaginary part there into the waveform instead of dropping it.
+// Y is real in exact arithmetic, and istft_any_kernel folds an imaginary part there into the waveform instead of dropping
+// it.
 //
 //   lws_nofuture_kernel  one CTA per clip walks the frames in order: past = the q in {-3,-2,-1} terms from the last 3
 //                        frames (a shared-memory ring, zero before the clip), X(m) <- A past/|past|, then init_iters

@@ -1,6 +1,7 @@
 // The audio front-end and Griffin-Lim kernels for every STFT frame audio.check_geometry accepts (fft_size N even,
-// 256 <= N <= 4096, N/2 with no prime factor above 5; hop R = N/Q with Q in [2, 8]).  stft.cu / istft.cu keep the
-// specialised 1024 / 256 kernels; audio.py selects these only for other frames.  The transform is fft_any.cuh's
+// 256 <= N <= 4096, N/2 with no prime factor above 5; hop R = N/Q with Q in [2, 8]).  stft.cu keeps the specialised
+// 1024 / 256 forward kernel, so audio.py selects stft_any_kernel only for other frames; the complex STFT and inverse
+// STFT kernels here run at every frame, 1024 / 256 included.  The transform is fft_any.cuh's
 // mixed-radix Stockham FFT of length N/2 with the real-packing split; window, twiddles and split factors come from a
 // per-geometry fp32 table the host builds in fp64 (audio._geometry_table).
 //
@@ -226,7 +227,7 @@ __global__ void __launch_bounds__(ANY_THREADS) stft_complex_any_kernel(const flo
     }
 }
 
-// The fast Griffin-Lim step on the same transform (istft.cu's stft_complex_momentum_kernel for K bins): per bin
+// The fast Griffin-Lim step on the same transform (Perraudin, Balazs & Sondergaard, WASPAA 2013): per bin
 // C = X - beta * prev, prev <- X in place (same thread, same element), spec = mag * C / |C|; beta == 0 takes C = X,
 // the projection of stft_complex_any_kernel bit for bit.  grid (max_frames, nclips); frames past a clip's count are
 // neither read nor written.

@@ -235,37 +235,14 @@ int dv3_resample_segments_batched(const void* wav, int wav_int16, int pitch_in, 
 int dv3_trim_bounds_batched(const void* wav, int wav_int16, const int* lengths, const int* offsets, int pitch,
                             int nclips, const double* top_db, int* bounds, void* stream);
 
-/* ---- inverse audio path: reference audio.py:37-43 (inv_spectrogram) and :26-28 (inv_preemphasis).  The reference
- * recovers the phase with the un-vendored `lws` package (parity UNPINNED); restated here as Griffin-Lim on the same
- * sqrt-Hann 1024 / hop 256 / 768-pad frame as dv3_stft_mel (sum of squared windows == 1: synthesis window = analysis
- * window).  The iteration x <- istft(mag * exp(i angle(stft(x)))) is driven by the host (audio.inv_spectrogram).
- * dv3_spec_to_amp: normalised dB (n) -> (10^((S*(-min)+min+ref)/20))^power.  dv3_stft_complex: wav (n_samples) ->
- * spec (nframes,513,2) [re,im]; mag (nframes,513) != NULL projects the result onto that magnitude.  dv3_istft: spec ->
- * wav (n_samples) += overlap-added frames (zero wav first).  dv3_deemphasis: y[n] = x[n] + coef*y[n-1] per clip.
- * The overlap-add is deterministic: frames whose indices differ by 4 do not overlap (1024 = 4 * hop), so the four
- * residue classes f mod 4 are added in four ordered launches with plain stores; a sample's value depends only on its
- * own clip's frames, always summed in the same order.
- * Batched forms: clip c has n_samples[c] samples at wav + c*wav_pitch and nframes[c] <= max_frames frames at
- * spec + c*max_frames*513*2 (mag likewise with 513 floats per frame); both count arrays are int32 [nclips] on the
- * device.  Samples and frames past a clip's counts are neither read nor written.  The one-clip entry points above are
- * the same kernels with nclips = 1. */
+/* ---- inverse audio path: reference audio.py:37-43 (inv_spectrogram) and :26-28 (inv_preemphasis).
+ * dv3_spec_to_amp: normalised dB (n) -> (10^((S*(-min)+min+ref)/20))^power.  dv3_deemphasis: y[n] = x[n] + coef*y[n-1]
+ * per clip.  Griffin-Lim and the inverse STFT between them are the _geom entry points below, for every frame; LWS has
+ * the specialised 1024 / 256 entry points here and the _geom ones for every other frame. */
 int dv3_spec_to_amp(const float* spec_norm, float* amp, long long n, float min_level_db, float ref_level_db,
                     float power, void* stream);
-int dv3_stft_complex(const float* wav, int n_samples, const float* mag, float* spec, int nframes, void* stream);
-int dv3_istft(const float* spec, float* wav, int n_samples, int nframes, void* stream);
-int dv3_stft_complex_batched(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
-                             float* spec, const int* nframes, int max_frames, int nclips, void* stream);
-int dv3_istft_batched(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
-                      int max_frames, int nclips, void* stream);
-/* Fast Griffin-Lim step (Perraudin, Balazs & Sondergaard, WASPAA 2013; audio.griffin_lim_batch with momentum > 0,
- * DESIGN.md section 7.3): the transform of dv3_stft_complex_batched, then per bin C = X - beta * prev, prev <- X (in
- * place), spec = mag * C / |C| ((mag, 0) where C == 0).  prev has spec's layout; mag and prev are required; beta in
- * [0, 1) (= momentum / (1 + momentum)); beta == 0 gives dv3_stft_complex_batched's projected spec bit for bit. */
-int dv3_stft_complex_momentum_batched(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
-                                      float* prev, float* spec, const int* nframes, int max_frames, int nclips,
-                                      float beta, void* stream);
-/* LWS phase recovery (csrc/lws.cu; Local Weighted Sums, the algorithm of the reference's lws.run_lws -- parity
- * UNPINNED, the package's source is absent).  mag (nframes,513) target magnitude; spec (nframes,513,2) [re,im];
+/* LWS phase recovery at 1024 / 256 (csrc/lws.cu; Local Weighted Sums, the algorithm of the reference's lws.run_lws --
+ * parity UNPINNED, the package's source is absent).  mag (nframes,513) target magnitude; spec (nframes,513,2) [re,im];
  * weights: 7 x 11 complex fp32 [q+3][d+5] = beta_q(d) = (1/1024) sum_n w(n) w(n-256q) e^{-2 pi i d n/1024}
  * (audio._lws_weights).  dv3_lws_nofuture: the no-future initialisation -> spec (frames in order from their 3 past
  * frames, then init_iters in-frame Jacobi passes).  dv3_lws_iterate: one batch iteration spec_in -> spec_out (distinct
@@ -280,19 +257,33 @@ int dv3_lws_iterate_batched(const float* mag, const float* spec_in, float* spec_
                             const int* nframes, int max_frames, int nclips, void* stream);
 int dv3_deemphasis(const float* x, float* y, int nclips, int n_samples, long long stride, float coef, void* stream);
 
-/* ---- the same audio path for any supported STFT frame (csrc/stft_any.cu, csrc/lws_any.cu; audio.check_geometry):
+/* ---- the audio path for any supported STFT frame (csrc/stft_any.cu, csrc/lws_any.cu; audio.check_geometry):
  * n_fft even in [256, 4096] with n_fft / 2 free of prime factors above 5, hop = n_fft / Q with Q in [2, 8]; K =
  * n_fft / 2 + 1 bins; padding n_fft - hop samples on both sides.  An unsupported geometry returns an error before any
  * launch.  table: 3 * n_fft + 2 floats on the device -- window (n_fft), twiddles exp(-2 pi i j / (n_fft/2)) and split
  * factors exp(-2 pi i k / n_fft) as [re, im] pairs, computed in fp64 and rounded once (audio._geometry_table).
+ * The forward mel path and LWS have specialised 1024 / 256 forms (dv3_stft_mel / dv3_stft_mel_targets and the LWS
+ * entry points above); the complex STFT and inverse STFT entry points here are Griffin-Lim's path for every frame,
+ * 1024 / 256 included.
  * dv3_stft_num_frames_geom: frames of an n-sample clip, ceil((n + n_fft - 2 hop) / hop) + 1.
  * dv3_stft_mel_geom: dv3_stft_mel_targets for the geometry (linear rows of K floats, mel_basis (n_mels, K) with the
  * same sparse span description; lead = 0, downsample_step = 1, T_lin = max_frames is the dv3_stft_mel layout).
- * dv3_stft_complex_geom / dv3_istft_geom: the batched forms of dv3_stft_complex_batched / dv3_istft_batched with K
- * bins per frame; the overlap-add runs as Q ordered launches (frames f and f + Q do not overlap), deterministic.
- * dv3_lws_nofuture_geom / dv3_lws_iterate_geom: the batched LWS forms with K bins; weights ((2Q - 1) * 11 + Q) [re, im]
- * fp32 pairs = beta_q(d) e^{2 pi i d q / Q} at [q + Q - 1][d + 5], |q| <= Q - 1, |d| <= 5, then the Q roots
- * e^{-2 pi i r / Q} (audio._lws_tables_fp64).  Every form: each clip of a ragged batch is bit-identical alone. */
+ * Batched forms: clip c has n_samples[c] samples at wav + c*wav_pitch and nframes[c] <= max_frames frames at
+ * spec + c*max_frames*K*2 (mag and prev likewise, mag with K floats per frame); both count arrays are int32 [nclips] on
+ * the device.  Samples and frames past a clip's counts are neither read nor written.
+ * dv3_stft_complex_geom: wav -> spec (frames, K, 2) [re, im]; mag != NULL projects the result onto that magnitude,
+ * spec = mag * X / |X| ((mag, 0) where X == 0): the Griffin-Lim step x <- istft(mag * exp(i angle(stft(x)))), driven
+ * by the host (audio.griffin_lim_batch).  dv3_istft_geom: wav += overlap-added windowed frames (zero wav first); the
+ * overlap-add runs as Q ordered launches (frames f and f + Q do not overlap) with plain stores, deterministic.
+ * dv3_stft_complex_momentum_geom: the fast Griffin-Lim step (Perraudin, Balazs & Sondergaard, WASPAA 2013;
+ * audio.griffin_lim_batch with momentum > 0, DESIGN.md section 7.3): the transform of dv3_stft_complex_geom, then per
+ * bin C = X - beta * prev, prev <- X (in place), spec = mag * C / |C| ((mag, 0) where C == 0); mag and prev are
+ * required; beta in [0, 1) (= momentum / (1 + momentum)); beta == 0 gives dv3_stft_complex_geom's projected spec bit
+ * for bit.
+ * dv3_lws_nofuture_geom / dv3_lws_iterate_geom: the batched LWS forms with K bins; weights ((2Q - 1) * 11 + Q)
+ * [re, im] fp32 pairs = beta_q(d) e^{2 pi i d q / Q} at [q + Q - 1][d + 5], |q| <= Q - 1, |d| <= 5, then the Q roots
+ * e^{-2 pi i r / Q} (audio._lws_tables_fp64).
+ * Every form: each clip of a ragged batch is bit-identical alone. */
 int dv3_stft_num_frames_geom(int n_samples, int n_fft, int hop);
 int dv3_stft_mel_geom(const void* wav, int wav_int16, const int* lengths, const float* peak, float rescaling_max,
                       const float* table, const float* mel_basis, const int* mel_start, const int* mel_len,
@@ -304,7 +295,6 @@ int dv3_stft_complex_geom(const float* wav, const int* n_samples, long long wav_
                           void* stream);
 int dv3_istft_geom(const float* spec, float* wav, const int* n_samples, long long wav_pitch, const int* nframes,
                    int max_frames, int nclips, const float* table, int n_fft, int hop, void* stream);
-/* dv3_stft_complex_momentum_batched for the geometry (K bins per frame). */
 int dv3_stft_complex_momentum_geom(const float* wav, const int* n_samples, long long wav_pitch, const float* mag,
                                    float* prev, float* spec, const int* nframes, int max_frames, int nclips,
                                    float beta, const float* table, int n_fft, int hop, void* stream);

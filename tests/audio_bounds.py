@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.  Elementwise error bounds for the audio kernels (csrc/stft.cu + stft_core.cuh, the
-1024 / 256 front end; csrc/stft_any.cu + fft_any.cuh, every other frame; csrc/istft.cu, the 1024 / 256 complex STFT,
-inverse STFT, dB -> amplitude and de-emphasis) against the fp64 oracles of oracle/audio_oracle.py and
-tests/stft_geometry_oracle.py.  The reference values come from those oracles; this module adds the bounds.
+1024 / 256 front end; csrc/stft_any.cu + fft_any.cuh, the front end at every other frame and the complex STFT and
+inverse STFT at every frame; csrc/istft.cu, dB -> amplitude and de-emphasis) against the fp64 oracles of
+oracle/audio_oracle.py and tests/stft_geometry_oracle.py.  The reference values come from those oracles; this module adds the bounds.
 
 Error model.  u = 2^-24 (unit roundoff of fp32).  Every bound is first order in u; the sums are scaled by
 (1 + 2^-10) for the second-order terms (below (c u)^2 relative for the c of this file).  Errors of complex values are
@@ -10,9 +10,7 @@ measured in modulus.  The rules, each a rounding of the kernel's own code:
   * a complex product with two roundings per component (cmul, cmulp, twmul, split4's p / q, with or without FMA
     contraction): |d| <= 2 sqrt2 u |a| |t|  (CMUL);
   * a twiddle or split factor t with |t_hat - t| <= tau u: fp32 table entries rounded once from fp64 (audio._geometry_table,
-    stft_core.cuh table_entry) have tau = 1; CUDA sincospif has a maximum error of 1 ulp per component (CUDA C++
-    Programming Guide, single-precision mathematical functions), tau = 2; a product of two factors has
-    tau_a + tau_b + CMUL.
+    stft_core.cuh table_entry) have tau = 1; a product of two factors has tau_a + tau_b + CMUL.
   * A pass of the FFT maps values whose moduli sum, over the inputs that reach one output, to S; its outputs carry an
     error <= c_pass u S, with c_pass = D_p + tau + CMUL: D_p for the radix-p DFT (below), tau + CMUL for the twiddle
     multiply on either side of it.  Every intermediate value of a decimation FFT is a unit-modulus combination of a
@@ -29,13 +27,12 @@ measured in modulus.  The rules, each a rounding of the kernel's own code:
     <= 1 on Z_k and Z_{M-k}, so it doubles the transform error, and rounds E, O (u (|a| + |b|) / 2 each), the product
     ((tau + CMUL) u (|a| + |b|) / 2) and the sum (u (|a| + |b|)); with |a| + |b| <= 2 sum|x|:
         c_fft = 2 c_Z + c_split,  c_split = 4 + tau + CMUL.
-    The inverse merges the half spectrum into Z the same way (merge_bin_conj, istft_kernel), then runs the forward
+    The inverse merges the half spectrum into Z the same way (merge_bin_conj, istft_any_kernel), then runs the forward
     passes on conj Z:  |z_hat_n - z_n| <= (2 c_Z + c_split) u sum_k |X_k|   (sum|Z| <= 2 sum|X|).
-  Per kernel (passes from make_plan, or the fixed plans of the 1024-point kernels):
+  Per kernel (passes from make_plan, or the fixed plan of the 1024-point front end):
     stft1024   stft_core.cuh: 3 radix-8 passes, the first two followed by twiddle7 (tau up to 12.5 for w^7 = w^4 w^2 w^1
                as products of the tabulated w^1, w^4), split4 with W1024^k rotated by a rounded W16^j (tau = 2 + CMUL);
-    any        fft_any.cuh: make_plan's radix-4 / 2 / 3 / 5 passes, table twiddles (tau = 1);
-    c1024      istft.cu: 9 radix-2 passes with sincospif twiddles (tau = 2) and a sincospif split factor.
+    any        fft_any.cuh: make_plan's radix-4 / 2 / 3 / 5 passes, table twiddles (tau = 1).
 
 Input stage.  The kernels' input is reproduced exactly: int16 PCM x 2^-15, and with rescaling rn(rn(x / peak) * gain)
 (numpy float32 division and product are correctly rounded like __fdiv_rn / __fmul_rn), peak = max|x[:len]|.
@@ -43,8 +40,7 @@ Pre-emphasis is one fmaf with the fp32 coefficient: |e_hat_n - e_n| <= u (|x_n| 
 against e_n = x_n - c x_{n-1} with c = 0.97 in fp64.  Window: w_hat = w (1 + u) for the fp32 tables of fft_any.cuh;
 stft_core.cuh builds w = S sin(a + b) = rn(rn(sA cb) + cA sb) from the tabulated sA = rn(S sin a), cA = rn(S cos a)
 and the rounded constants cb, sb = cos b, sin b: |dw| <= u (3 |S sin a cos b| + 2 |S cos a sin b| + |w|) (exact table
-entries at n2 = 0, 4); istft.cu's frame_window computes sqrtf(0.5 (0.5 - 0.5 cospif(t))) with cospif within 1 ulp:
-|dw| <= w u (|cos| / (2 hann) + 3/2), large relative to w only where w is tiny.  The product e w is rounded (u).  An
+entries at n2 = 0, 4).  The product e w is rounded (u).  An
 input error reaches every bin with a coefficient of modulus 1, so the frame bound is
     B_f = c_fft u sum_n |w_n e_n| + sum_n (w_n de_n + dw_n |e_n| + u w_n |e_n|).
 
@@ -86,10 +82,10 @@ SECOND_ORDER = 1.0 + 2.0 ** -10
 LG2_APPROX_ABS = 2.0 ** -22          # PTX ISA, lg2.approx.f32: maximum absolute error
 SQRT_APPROX_REL = 2.0 ** -22         # PTX ISA, sqrt.approx.f32: 2^-23 relative; taken at twice that
 ULP = 2.0 * U                        # one ulp of an fp32 value, relative to the value (at most)
-POWF_ULP, LOG2F_ULP, SINCOSPI_ULP = 4, 1, 1
+POWF_ULP, LOG2F_ULP = 4, 1
 D = {2: 1.0, 3: 5.0, 4: 2.0, 5: 10.0, 8: 5.0}
-TAU_TAB, TAU_SINCOSPI = 1.0, SINCOSPI_ULP * 2.0
-KERNELS = ("stft1024", "any", "c1024")
+TAU_TAB = 1.0
+KERNELS = ("stft1024", "any")
 
 
 def plan(M):
@@ -121,9 +117,6 @@ def c_fft(kernel, N=1024):
     elif kernel == "any":
         c_z = sum(D[p] + TAU_TAB + CMUL for p in plan(N // 2))
         tau_split = TAU_TAB
-    elif kernel == "c1024":
-        c_z = 9 * (D[2] + TAU_SINCOSPI + CMUL)
-        tau_split = TAU_SINCOSPI
     else:
         raise ValueError(kernel)
     return 2 * c_z + 4 + tau_split + CMUL
@@ -144,11 +137,6 @@ def window_error(kernel, N, R):
         dw = U * (3 * np.abs(S * np.sin(a) * np.cos(b)) + 2 * np.abs(S * np.cos(a) * np.sin(b)) + w)
         exact = (n2 == 0) | (n2 == 4)
         return w, np.where(exact, U * w, dw)
-    if kernel == "c1024":
-        assert (N, R) == (1024, 256)
-        cth = np.cos(np.pi * (2 * i + 1) / N)
-        hann = 0.5 - 0.5 * cth
-        return w, w * U * (np.abs(cth) / (2 * hann) + 1.5)
     raise ValueError(kernel)
 
 

@@ -1,6 +1,6 @@
-"""CPU: fast Griffin-Lim (audio.griffin_lim_batch with momentum > 0, csrc/istft.cu / csrc/stft_any.cu momentum kernels)
--- the fp64 oracle against plain Griffin-Lim, argument checks that fire before any library call, the C ABI of the new
-entry points, and the ptxas report of the new kernels."""
+"""CPU: fast Griffin-Lim (audio.griffin_lim_batch with momentum > 0, the csrc/stft_any.cu momentum kernel) -- the fp64
+oracle against plain Griffin-Lim, argument checks that fire before any library call, the C ABI of its entry point, and
+the ptxas report of its kernel."""
 import ctypes
 import os
 import re
@@ -117,7 +117,6 @@ def test_momentum_entry_points_match_the_header():
     decls = parse_header()
     P, I, L, Fl = ctypes.c_void_p, ctypes.c_int, ctypes.c_longlong, ctypes.c_float
     want = {
-        "dv3_stft_complex_momentum_batched": [P, P, L, P, P, P, P, I, I, Fl, P],
         "dv3_stft_complex_momentum_geom": [P, P, L, P, P, P, P, I, I, Fl, P, I, I, P],
     }
     dll = ctypes.CDLL(LIB_PATH)
@@ -127,8 +126,7 @@ def test_momentum_entry_points_match_the_header():
         assert [a for _, a in decls[name][1]][3:6] == ["mag", "prev", "spec"], name
         assert decls[name][0] is ctypes.c_int, name
         assert hasattr(dll, name), name
-    # the plain twins are unchanged
-    assert [t for t, _ in decls["dv3_stft_complex_batched"][1]] == [P, P, L, P, P, P, I, I, P]
+    # the plain twin is unchanged
     assert [t for t, _ in decls["dv3_stft_complex_geom"][1]] == [P, P, L, P, P, P, I, I, P, I, I, P]
 
 
@@ -143,14 +141,11 @@ def test_entry_points_refuse_bad_arguments_before_launch():
     for c in cases:
         mag, prev, beta = c.get("mag", fake), c.get("prev", fake), c.get("beta", 0.5)
         with pytest.raises(Dv3Error, match="momentum"):
-            lib.call("dv3_stft_complex_momentum_batched", fake, fake, 100, mag, prev, fake, fake, 3, 1, beta, None)
-        with pytest.raises(Dv3Error, match="momentum"):
             lib.call("dv3_stft_complex_momentum_geom", fake, fake, 100, mag, prev, fake, fake, 3, 1, beta, fake, 800,
                      200, None)
 
 
-@pytest.mark.parametrize("src,kernel", [("istft.cu", "stft_complex_momentum_kernel"),
-                                        ("stft_any.cu", "stft_complex_momentum_any_kernel")])
+@pytest.mark.parametrize("src,kernel", [("stft_any.cu", "stft_complex_momentum_any_kernel")])
 def test_momentum_kernels_do_not_spill(tmp_path, src, kernel):
     nvcc = _nvcc()
     if nvcc is None:

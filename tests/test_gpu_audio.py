@@ -1,6 +1,6 @@
 """GPU: fused STFT->linear/mel kernel against the numpy restatement of audio.py (oracle/audio_oracle.py;
 parity UNPINNED, see its header).  Values are held to the elementwise fp64 bounds of tests/audio_bounds.py (kernel
-"stft1024" for the fused front end, "c1024" for the complex STFT / iSTFT of csrc/istft.cu)."""
+"stft1024" for the fused front end, "any" for the complex STFT / iSTFT of csrc/stft_any.cu)."""
 import numpy as np
 import pytest
 import torch
@@ -66,8 +66,8 @@ def test_linearity_and_silence():
 
 
 def test_complex_stft_and_istft_against_oracle():
-    """dv3_stft_complex == the oracle's lws_stft (complex values), dv3_istft == lws_istft, and istft(stft(x)) == x
-    (the sqrt-Hann frame with 768-sample padding reconstructs perfectly)."""
+    """At 1024 / 256: dv3_stft_complex_geom == the oracle's lws_stft (complex values), dv3_istft_geom == lws_istft, and
+    istft(stft(x)) == x (the sqrt-Hann frame with 768-sample padding reconstructs perfectly)."""
     import ctypes
     from deepvoice3_pytorch_b200 import audio
     from deepvoice3_pytorch_b200._lib import lib
@@ -81,18 +81,25 @@ def test_complex_stft_and_istft_against_oracle():
     spec = torch.zeros(T, 513, 2, device="cuda")
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     vp = lambda t: ctypes.c_void_p(t.data_ptr())
-    lib.call("dv3_stft_complex", vp(xd), n, None, vp(spec), T, st)
-    fw = AB.Forward(x, 1024, 256, "c1024", preemph=None, T=T)
+    tab = audio._geometry_table(xd.device, 1024, 256)
+    nd = torch.tensor([n], dtype=torch.int32, device="cuda")
+    fd = torch.tensor([T], dtype=torch.int32, device="cuda")
+
+    def stft(mag):
+        lib.call("dv3_stft_complex_geom", vp(xd), vp(nd), n, mag, vp(spec), vp(fd), T, 1, vp(tab), 1024, 256, st)
+    stft(None)
+    fw = AB.Forward(x, 1024, 256, "any", preemph=None, T=T)
     got = spec[..., 0].cpu().numpy().astype(np.float64) + 1j * spec[..., 1].cpu().numpy()
     assert AB.complex_ratio(got, fw) <= 1.0
     y = torch.zeros(n, device="cuda")
-    lib.call("dv3_istft", vp(spec), vp(y), n, T, st)
+    lib.call("dv3_istft_geom", vp(spec), vp(y), vp(nd), n, vp(fd), T, 1, vp(tab), 1024, 256, st)
     np.testing.assert_allclose(y.cpu().numpy(), x, rtol=1e-3, atol=2e-5)            # perfect reconstruction
-    ref_y, bound = AB.istft(got, 1024, 256, n, "c1024")
+    ref_y, bound = AB.istft(got, 1024, 256, n, "any")
     assert AB.abs_ratio(y.cpu().numpy(), ref_y, bound) <= 1.0
     # magnitude projection (one Griffin-Lim step)
     mag_np = np.abs(fw.X).astype(np.float32) * 0.5
-    lib.call("dv3_stft_complex", vp(xd), n, vp(torch.from_numpy(mag_np).cuda()), vp(spec), T, st)
+    magd = torch.from_numpy(mag_np).cuda()
+    stft(vp(magd))
     got = spec[..., 0].cpu().numpy().astype(np.float64) + 1j * spec[..., 1].cpu().numpy()
     assert AB.projection_ratio(got, fw, mag_np) <= 1.0
 

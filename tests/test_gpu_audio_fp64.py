@@ -4,8 +4,8 @@ see them.  Output buffers are filled with NaN first, so every element must be wr
 its length with loud garbage, so a kernel that reads a sample at or past ``len`` fails.
 
 Entry points: dv3_stft_mel, dv3_stft_mel_targets with dv3_peak_abs_batched, dv3_stft_mel_geom (the nine frames of
-test_gpu_stft_geometry.py and 1024 / 256 called directly), dv3_stft_complex[_batched|_geom] with and without the
-magnitude projection, dv3_istft[_batched|_geom], dv3_spec_to_amp, dv3_deemphasis."""
+test_gpu_stft_geometry.py and 1024 / 256 called directly), dv3_stft_complex_geom with and without the magnitude
+projection and dv3_istft_geom (the same frames), dv3_spec_to_amp, dv3_deemphasis."""
 import ctypes
 
 import numpy as np
@@ -215,11 +215,12 @@ def _complex(t):
     return a[..., 0] + 1j * a[..., 1]
 
 
-def _griffin_lim_step(worst, lib, N, R, geom):
-    """stft_complex (plain and projected) and istft, single-clip and batched entry points, each against the fp64
-    reference of its own input; the istft also on spectra with non-zero imaginary parts at bins 0 and N/2.  Clip 2
-    has a silent stretch longer than two frames: there X_hat == 0 and the projection must give exactly (mag, 0)."""
-    kernel = "any" if geom else "c1024"
+def _griffin_lim_step(worst, lib, N, R):
+    """stft_complex (plain and projected) and istft on a ragged batch, each against the fp64 reference of its own
+    input; the istft also on spectra with non-zero imaginary parts at bins 0 and N/2.  Clip 2 has a silent stretch
+    longer than two frames: there X_hat == 0 and the projection must give exactly (mag, 0)."""
+    from deepvoice3_pytorch_b200 import audio
+    kernel = "any"
     K = N // 2 + 1
     frames = [3 * (N // R), 9, 40]
     ns = [(T - 1) * R - (N - 2 * R) for T in frames]
@@ -232,10 +233,7 @@ def _griffin_lim_step(worst, lib, N, R, geom):
     wd = torch.from_numpy(wav).cuda()
     nd, fd = torch.tensor(ns, dtype=torch.int32).cuda(), torch.tensor(frames, dtype=torch.int32).cuda()
     Tm = max(frames)
-    tab = None
-    if geom:
-        from deepvoice3_pytorch_b200 import audio
-        tab = audio._geometry_table(wd.device, N, R)
+    tab = audio._geometry_table(wd.device, N, R)
     refs = [AB.Forward(wav[c, :ns[c]], N, R, kernel, preemph=None, T=frames[c]) for c in range(3)]
     mags = np.zeros((3, Tm, K), np.float32)
     for c in range(3):
@@ -249,15 +247,8 @@ def _griffin_lim_step(worst, lib, N, R, geom):
     for mag in (None, md):
         what = "projected" if mag is not None else "plain"
         spec = _nan(3, Tm, K, 2)
-        if geom:
-            lib.call("dv3_stft_complex_geom", _vp(wd), _vp(nd), pitch, _vp(mag), _vp(spec), _vp(fd), Tm, 3, _vp(tab),
-                     N, R, _st())
-        else:
-            lib.call("dv3_stft_complex_batched", _vp(wd), _vp(nd), pitch, _vp(mag), _vp(spec), _vp(fd), Tm, 3, _st())
-            one = _nan(frames[2], K, 2)
-            lib.call("dv3_stft_complex", _vp(wd[2]), ns[2], _vp(None if mag is None else md[2]), _vp(one), frames[2],
-                     _st())
-            assert torch.equal(one, spec[2, :frames[2]])
+        lib.call("dv3_stft_complex_geom", _vp(wd), _vp(nd), pitch, _vp(mag), _vp(spec), _vp(fd), Tm, 3, _vp(tab),
+                 N, R, _st())
         got = _complex(spec)
         for c in range(3):
             g = got[c, :frames[c]]
@@ -274,13 +265,7 @@ def _griffin_lim_step(worst, lib, N, R, geom):
             src = _complex(sd)
             y = torch.zeros(3, pitch, device="cuda")
             y[:, -1] = 7.0                                   # past every clip's samples: must stay untouched
-            if geom:
-                lib.call("dv3_istft_geom", _vp(sd), _vp(y), _vp(nd), pitch, _vp(fd), Tm, 3, _vp(tab), N, R, _st())
-            else:
-                lib.call("dv3_istft_batched", _vp(sd), _vp(y), _vp(nd), pitch, _vp(fd), Tm, 3, _st())
-                one = torch.zeros(ns[2], device="cuda")
-                lib.call("dv3_istft", _vp(sd[2]), _vp(one), ns[2], frames[2], _st())
-                assert torch.equal(one, y[2, :ns[2]])
+            lib.call("dv3_istft_geom", _vp(sd), _vp(y), _vp(nd), pitch, _vp(fd), Tm, 3, _vp(tab), N, R, _st())
             yy = y.cpu().numpy()
             for c in range(3):
                 ref, bound = AB.istft(src[c, :frames[c]], N, R, ns[c], kernel)
@@ -291,8 +276,7 @@ def _griffin_lim_step(worst, lib, N, R, geom):
 def test_griffin_lim_step_1024():
     from deepvoice3_pytorch_b200._lib import lib
     worst = Worst()
-    _griffin_lim_step(worst, lib, 1024, 256, geom=False)
-    _griffin_lim_step(worst, lib, 1024, 256, geom=True)
+    _griffin_lim_step(worst, lib, 1024, 256)
     worst.report("Griffin-Lim step 1024/256")
 
 
@@ -300,7 +284,7 @@ def test_griffin_lim_step_1024():
 def test_griffin_lim_step_geom(sr, N, R):
     from deepvoice3_pytorch_b200._lib import lib
     worst = Worst()
-    _griffin_lim_step(worst, lib, N, R, geom=True)
+    _griffin_lim_step(worst, lib, N, R)
     worst.report("Griffin-Lim step %d/%d" % (N, R))
 
 

@@ -1,5 +1,5 @@
-"""GPU: fast Griffin-Lim (csrc/istft.cu stft_complex_momentum_kernel at 1024 / 256, csrc/stft_any.cu
-stft_complex_momentum_any_kernel at the other frames; audio.griffin_lim_batch(momentum > 0)) against the fp64 oracle of
+"""GPU: fast Griffin-Lim (csrc/stft_any.cu stft_complex_momentum_any_kernel at every frame;
+audio.griffin_lim_batch(momentum > 0)) against the fp64 oracle of
 tests/fgla_oracle.py: one momentum step elementwise within the bounds of tests/audio_bounds.py, bit identity with the
 plain projection at beta = 0, the ragged-batch contract, end-to-end quality, the entry points each path calls, and
 inv_spectrogram / synthesis with method "fast_griffin_lim"."""
@@ -42,13 +42,12 @@ def _pairs(X):
 
 class _Step:
     """Three clips of a ragged batch at the frame (N, R) with their magnitudes and a prev spectrum; runs the plain and
-    the momentum entry points of that frame.  Clip 0 has a silent stretch of 3 N samples: there X == 0, and prev is
+    the momentum entry points at that frame.  Clip 0 has a silent stretch of 3 N samples: there X == 0, and prev is
     set to 0, so C == 0."""
 
     def __init__(self, N, R):
         from deepvoice3_pytorch_b200 import audio
         self.N, self.R, self.K = N, R, N // 2 + 1
-        self.default = (N, R) == (1024, 256)
         self.frames = [41, 9, 3 * (N // R)]
         self.ns = [audio.inv_num_samples(t) for t in self.frames]
         self.pitch = max(self.ns) + 29
@@ -64,7 +63,7 @@ class _Step:
         self.wd = torch.from_numpy(wav).cuda()
         self.nd = torch.tensor(self.ns, dtype=torch.int32).cuda()
         self.fd = torch.tensor(self.frames, dtype=torch.int32).cuda()
-        self.refs = [AB.Forward(wav[c, :self.ns[c]], N, R, "c1024" if self.default else "any", preemph=None,
+        self.refs = [AB.Forward(wav[c, :self.ns[c]], N, R, "any", preemph=None,
                                 T=self.frames[c]) for c in range(3)]
         self.silent = [f for f in range(self.frames[0]) if not self.refs[0].X[f].any()]
         assert len(self.silent) >= 2, self.silent
@@ -80,17 +79,13 @@ class _Step:
         mags[0, self.silent[0], :5] = 0.0                        # mag 0 on C == 0 bins: (0, 0)
         self.mags, self.md = mags, torch.from_numpy(mags).cuda()
         self.prev = _complex(_pairs(prev))                        # the fp32 values the kernel reads
-        self.tab = None if self.default else audio._geometry_table(self.wd.device, N, R)
+        self.tab = audio._geometry_table(self.wd.device, N, R)
 
     def plain(self, mag):
         from deepvoice3_pytorch_b200._lib import lib
         spec = torch.full((3, self.Tm, self.K, 2), float("nan"), device="cuda")
-        if self.default:
-            lib.call("dv3_stft_complex_batched", _vp(self.wd), _vp(self.nd), self.pitch, _vp(mag), _vp(spec),
-                     _vp(self.fd), self.Tm, 3, _st())
-        else:
-            lib.call("dv3_stft_complex_geom", _vp(self.wd), _vp(self.nd), self.pitch, _vp(mag), _vp(spec),
-                     _vp(self.fd), self.Tm, 3, _vp(self.tab), self.N, self.R, _st())
+        lib.call("dv3_stft_complex_geom", _vp(self.wd), _vp(self.nd), self.pitch, _vp(mag), _vp(spec),
+                 _vp(self.fd), self.Tm, 3, _vp(self.tab), self.N, self.R, _st())
         return spec
 
     def momentum(self, beta):
@@ -98,12 +93,8 @@ class _Step:
         from deepvoice3_pytorch_b200._lib import lib
         prev = _pairs(self.prev)
         spec = torch.full((3, self.Tm, self.K, 2), float("nan"), device="cuda")
-        if self.default:
-            lib.call("dv3_stft_complex_momentum_batched", _vp(self.wd), _vp(self.nd), self.pitch, _vp(self.md),
-                     _vp(prev), _vp(spec), _vp(self.fd), self.Tm, 3, beta, _st())
-        else:
-            lib.call("dv3_stft_complex_momentum_geom", _vp(self.wd), _vp(self.nd), self.pitch, _vp(self.md),
-                     _vp(prev), _vp(spec), _vp(self.fd), self.Tm, 3, beta, _vp(self.tab), self.N, self.R, _st())
+        lib.call("dv3_stft_complex_momentum_geom", _vp(self.wd), _vp(self.nd), self.pitch, _vp(self.md),
+                 _vp(prev), _vp(spec), _vp(self.fd), self.Tm, 3, beta, _vp(self.tab), self.N, self.R, _st())
         return prev, spec
 
 
@@ -226,21 +217,21 @@ def test_existing_paths_call_the_same_entry_points():
     momentum > 0."""
     from deepvoice3_pytorch_b200 import audio, synthesis
     from test_gpu_synthesis import _model, _sequences
-    gl = ["dv3_istft_batched"] + ["dv3_stft_complex_batched", "dv3_istft_batched"] * 3
+    gl = ["dv3_istft_geom"] + ["dv3_stft_complex_geom", "dv3_istft_geom"] * 3
     mag = torch.rand(2, 20, 513, device="cuda")
     assert _recorded(lambda: audio.griffin_lim_batch(mag, [20, 11], n_iter=3)) == gl
     assert _recorded(lambda: audio.griffin_lim_batch(mag, [20, 11], n_iter=3, momentum=0)) == gl
     assert _recorded(lambda: audio.griffin_lim_batch(mag, [20, 11], n_iter=3, momentum=0.5)) == \
-        ["dv3_istft_batched"] + ["dv3_stft_complex_momentum_batched", "dv3_istft_batched"] * 3
+        ["dv3_istft_geom"] + ["dv3_stft_complex_momentum_geom", "dv3_istft_geom"] * 3
     assert _recorded(lambda: audio.lws_batch(mag, [20, 11], n_iter=2)) == \
-        ["dv3_lws_nofuture_batched"] + ["dv3_lws_iterate_batched"] * 2 + ["dv3_istft_batched"]
+        ["dv3_lws_nofuture_batched"] + ["dv3_lws_iterate_batched"] * 2 + ["dv3_istft_geom"]
     S = audio.spectrogram(A.synthetic_clip(8, n=40 * 256 - 512))
-    default_inv = ["dv3_spec_to_amp", "dv3_istft_batched"] + ["dv3_stft_complex_batched", "dv3_istft_batched"] * 60 \
+    default_inv = ["dv3_spec_to_amp", "dv3_istft_geom"] + ["dv3_stft_complex_geom", "dv3_istft_geom"] * 60 \
         + ["dv3_deemphasis"]
     assert _recorded(lambda: audio.inv_spectrogram(S)) == default_inv
     fast = _recorded(lambda: audio.inv_spectrogram(S, method="fast_griffin_lim"))
-    assert fast == ["dv3_spec_to_amp", "dv3_istft_batched"] + \
-        ["dv3_stft_complex_momentum_batched", "dv3_istft_batched"] * audio.hparams.fast_griffin_lim_iters + \
+    assert fast == ["dv3_spec_to_amp", "dv3_istft_geom"] + \
+        ["dv3_stft_complex_momentum_geom", "dv3_istft_geom"] * audio.hparams.fast_griffin_lim_iters + \
         ["dv3_deemphasis"]
     model = _model("nyanko_ljspeech", max_steps=16)
     seqs = _sequences([9, 4], seed=2)
@@ -248,7 +239,7 @@ def test_existing_paths_call_the_same_entry_points():
     assert not [n for n in calls if "momentum" in n]
     assert [n for n in calls if any(a in n for a in AUDIO)] == default_inv
     calls = _recorded(lambda: synthesis.tts_batch(model, seqs, vocoder="fast_griffin_lim"))
-    assert "dv3_stft_complex_momentum_batched" in calls and "dv3_stft_complex_batched" not in calls
+    assert "dv3_stft_complex_momentum_geom" in calls and "dv3_stft_complex_geom" not in calls
 
 
 @pytest.mark.parametrize("preset", ["deepvoice3_ljspeech", "nyanko_ljspeech", "deepvoice3_vctk"])

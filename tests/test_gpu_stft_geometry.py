@@ -2,7 +2,7 @@
 audio.check_geometry) against the fp64 oracles of tests/stft_geometry_oracle.py: the STFT kernels within the
 elementwise bounds of tests/audio_bounds.py (kernel "any"), LWS within the bound of tests/test_gpu_lws.py; the
 ragged-batch and bit-identity contracts; the training targets against the preprocessed corpus; synthesis; and that the
-1024 / 256 frame still calls only its own kernels."""
+1024 / 256 frame calls its own forward and LWS kernels and the general complex-STFT and inverse-STFT ones."""
 import contextlib
 import ctypes
 import os
@@ -330,8 +330,10 @@ def test_synthesis_at_other_frames(sr, N, R):
             ops.conv_math = old
 
 
-def test_default_frame_calls_no_new_entry_point(tmp_path):
-    """At 1024 / 256: preprocessing, targets, Griffin-Lim, LWS and tts_batch call only the specialised kernels."""
+def test_default_frame_entry_points(tmp_path):
+    """At 1024 / 256: preprocessing and targets call only the specialised forward kernels (dv3_stft_mel /
+    dv3_stft_mel_targets, never dv3_stft_mel_geom) and LWS only its specialised kernels; Griffin-Lim, LWS and tts_batch
+    run the complex STFT and the inverse STFT through dv3_stft_complex_geom / dv3_istft_geom."""
     from deepvoice3_pytorch_b200 import audio, preprocess, synthesis, builder
     from deepvoice3_pytorch_b200._lib import lib
     from test_gpu_synthesis import _sequences
@@ -361,9 +363,10 @@ def test_default_frame_calls_no_new_entry_point(tmp_path):
         synthesis.tts_batch(model, _sequences([9, 4], seed=2), vocoder="lws")
     finally:
         lib.call = real
-    assert seen and not [n for n in seen if n.endswith("_geom")], sorted(set(seen))
-    for name in ("dv3_stft_mel", "dv3_stft_mel_targets", "dv3_istft_batched", "dv3_stft_complex_batched",
-                 "dv3_lws_nofuture_batched", "dv3_lws_iterate_batched"):
+    want = {"dv3_stft_mel", "dv3_stft_mel_targets", "dv3_stft_complex_geom", "dv3_istft_geom",
+            "dv3_lws_nofuture_batched", "dv3_lws_iterate_batched"}
+    assert not [n for n in seen if ("stft" in n or "lws" in n) and n not in want], sorted(set(seen))
+    for name in sorted(want):
         assert name in seen, name
 
 
