@@ -4,6 +4,7 @@ PyTorch is plumbing here: it owns device memory, the current stream and autograd
 arithmetic happens in csrc/*.cu.  Every function requires CUDA fp32 tensors and raises otherwise --
 there is no CPU fallback.
 """
+import collections
 import ctypes
 import os
 
@@ -203,80 +204,84 @@ def _drop_args(p, training, device):
 # ----------------------------------------------------------------------------------------------
 # weight-norm packing helpers
 # ----------------------------------------------------------------------------------------------
-def _wn_conv_fwd(v, g, out=None):
-    """v (Cout, Cin, k), g (Cout,1,1) -> w_f [k][Cin][Cout], w_b [k][Cout][Cin], inv_norm [Cout] (+ the scale buffer
-    when ``out`` -- a previous result to refold into -- is given)."""
+# How the plain conv Functions run a weight-normed layer.  A ConvTranspose1d(k=2, s=2) is a 1x1 conv with 2*Cout
+# output rows ordered (j, co) followed by a time interleave (conv_transpose1d_k2s2); all it changes is this record:
+#   dims(v) -> (M, N, k)     output rows, input channels and taps of the layer's GEMM
+#   fp32, tc                 the weight-norm fold kinds (_FOLDS) of the exact-fp32 and the tensor-core path
+#   wgrad(M, N, k, tc) -> (msplit, s_m, s_mh, s_n, s_j, tap_major_k): where the weight-gradient GEMM writes element
+#                            (m, n, j) of a partial (include/dv3b200.h), and how _wn_bwd reads the partials back
+#   bias(b), dbias(db)       the GEMM's bias rows from the layer's bias, and the layer's bias gradient from theirs
+#   banked                   the WeightBank and the gradient sink may take the layer: both assume a (Cout, Cin, k) v
+#                            and one bias row per GEMM row
+_Layout = collections.namedtuple("_Layout", "dims fp32 tc wgrad bias dbias banked")
+# v (Cout, Cin, k); the tensor-core partials are tap-major [j][M][N]: contiguous float4 stores from the GEMM epilogue
+_CONV = _Layout(lambda v: tuple(v.shape), "fp32", "tc",
+                lambda M, N, k, tc: (M, N, 0, 1, M * N, k) if tc else (M, N * k, 0, k, 1, 0),
+                lambda b: b, lambda db: db, True)
+# v (Cin, Cout, 2) normalised over Cin; GEMM element (m = (j, co), ci) is v[ci, co, j] on both paths
+_CONVT = _Layout(lambda v: (2 * v.shape[1], v.shape[0], 1), "convt_fp32", "convt_tc",
+                 lambda M, N, k, tc: (M // 2, 2, 1, M, 0, 0),
+                 lambda b: b.repeat(2), lambda db: db if db is None else db[:db.numel() // 2] + db[db.numel() // 2:],
+                 False)
+
+
+def _wn_buffers(lay, v, npl):
+    """Outputs of a layer's weight-norm fold, for its GEMM (M, N, k) = lay.dims(v): (w_f [k][N][M], w_b [k][M][N],
+    inv, scale) fp32 on the exact-fp32 path (npl = 0); (inv, wfwd [npl][k][M][pad8(N)] fp16 planes of the forward
+    GEMM, wbwd [npl][k][N][pad8(M)] bf16 planes of the data gradient, scale) on the tensor-core path.  inv and scale
+    have one entry per normalised row of v."""
+    M, N, k = lay.dims(v)
+    dev = v.device
+    inv = torch.empty(v.shape[0], device=dev)
+    if npl == 0:
+        return torch.empty(k, N, M, device=dev), torch.empty(k, M, N, device=dev), inv, torch.empty_like(inv)
+    return (inv, torch.empty(npl, k, M, _pad8(N), device=dev, dtype=torch.float16),
+            torch.empty(npl, k, N, _pad8(M), device=dev, dtype=torch.bfloat16), torch.empty_like(inv))
+
+
+def _fold_fp32(v, g, npl, out):
+    w_f, w_b, inv, scale = out
     Cout, Cin, k = v.shape
-    if out is None:
-        w_f = torch.empty(k, Cin, Cout, device=v.device, dtype=torch.float32)
-        w_b = torch.empty(k, Cout, Cin, device=v.device, dtype=torch.float32)
-        inv = torch.empty(Cout, device=v.device, dtype=torch.float32)
-        scale = torch.empty_like(inv)
-    else:
-        w_f, w_b, inv, scale = out
     lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cout, Cin, k,
              1, Cout, Cin * Cout, Cin, 1, Cout * Cin, _stream())
-    return (w_f, w_b, inv) if out is None else out
 
 
-def _fp32_weights(v, g):
-    """-> (w_f, w_b, inv) of _wn_conv_fwd, from the frozen-weight cache when it holds the layer."""
-    fz = _frozen("fp32", v, g)
-    return fz[:3] if fz is not None else _wn_conv_fwd(v, g)
-
-
-def _tc_fold(v, g, npl, out=None):
-    """Per-layer tensor-core weight norm on the current stream -> (inv, wfwd, wbwd, scale) (see _tc_weights)."""
-    Cout, Cin, k = v.shape
-    dev = v.device
-    if out is None:
-        inv = torch.empty(Cout, device=dev)
-        out = (inv, torch.empty(npl, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16),
-               torch.empty(npl, k, Cin, _pad8(Cout), device=dev, dtype=torch.bfloat16), torch.empty_like(inv))
-    inv, wfwd, wbwd, scale = out
-    lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cout, Cin, k,
-             _stream())
-    return out
-
-
-def _convt_tc_fold(v, g, npl, out=None):
-    """Tensor-core weight norm of a ConvTranspose1d(k=2, s=2) v (Cin, Cout, 2) -> (inv, wfwd, wbwd, scale)."""
-    Cin, Cout = v.shape[0], v.shape[1]
-    dev = v.device
-    if out is None:
-        inv = torch.empty(Cin, device=dev)
-        out = (inv, torch.empty(npl, 2 * Cout, _pad8(Cin), device=dev, dtype=torch.float16),
-               torch.empty(npl, Cin, _pad8(2 * Cout), device=dev, dtype=torch.bfloat16), torch.empty_like(inv))
-    inv, wfwd, wbwd, scale = out
-    lib.call("dv3_tc_weightnorm_convt_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cin, Cout,
-             _stream())
-    return out
-
-
-def _convt_fp32_fold(v, g, out=None):
-    """Exact-fp32 weight norm of a ConvTranspose1d(k=2, s=2) -> (w_f [ci][(j,co)], w_b [(j,co)][ci], inv, scale)."""
-    Cin, Cout = v.shape[0], v.shape[1]
-    dev = v.device
-    if out is None:
-        inv = torch.empty(Cin, device=dev, dtype=torch.float32)
-        out = (torch.empty(Cin, 2 * Cout, device=dev, dtype=torch.float32),
-               torch.empty(2 * Cout, Cin, device=dev, dtype=torch.float32), inv, torch.empty_like(inv))
+def _fold_convt_fp32(v, g, npl, out):
     w_f, w_b, inv, scale = out
+    Cin, Cout = v.shape[0], v.shape[1]
     lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cin, Cout, 2,
              2 * Cout, 1, Cout, 1, Cin, Cout * Cin, _stream())
+
+
+def _fold_tc(v, g, npl, out):
+    inv, wfwd, wbwd, scale = out
+    Cout, Cin, k = v.shape
+    lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cout, Cin, k,
+             _stream())
+
+
+def _fold_convt_tc(v, g, npl, out):
+    inv, wfwd, wbwd, scale = out
+    lib.call("dv3_tc_weightnorm_convt_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), v.shape[0],
+             v.shape[1], _stream())
+
+
+_FOLDS = {"fp32": (_CONV, _fold_fp32), "tc": (_CONV, _fold_tc),
+          "convt_fp32": (_CONVT, _fold_convt_fp32), "convt_tc": (_CONVT, _fold_convt_tc)}
+
+
+def _fold(kind, v, g, npl=0, out=None):
+    """Weight norm of a layer by fold kind (_FOLDS) on the current stream into ``out`` (new buffers of _wn_buffers when
+    None) -> out."""
+    lay, fold = _FOLDS[kind]
+    out = out or _wn_buffers(lay, v, npl)
+    fold(v, g, npl, out)
     return out
 
 
-_FOLDS = {"fp32": lambda v, g, npl, out: _wn_conv_fwd(v, g, out if out is not None else
-                                                      _wn_conv_fwd_buffers(v)),
-          "tc": _tc_fold, "convt_tc": _convt_tc_fold, "convt_fp32": lambda v, g, npl, out: _convt_fp32_fold(v, g, out)}
-
-
-def _wn_conv_fwd_buffers(v):
-    Cout, Cin, k = v.shape
-    inv = torch.empty(Cout, device=v.device, dtype=torch.float32)
-    return (torch.empty(k, Cin, Cout, device=v.device, dtype=torch.float32),
-            torch.empty(k, Cout, Cin, device=v.device, dtype=torch.float32), inv, torch.empty_like(inv))
+def _fp32_weights(v, g, lay):
+    """-> (w_f, w_b, inv) of the exact-fp32 weight norm, from the frozen-weight cache when it holds the layer."""
+    return (_frozen(lay.fp32, v, g) or _fold(lay.fp32, v, g))[:3]
 
 
 class FrozenWeights:
@@ -296,8 +301,7 @@ class FrozenWeights:
             if torch.cuda.is_current_stream_capturing():
                 raise Dv3Error("frozen weights: layer %s first seen during a CUDA-graph capture (warm up first)"
                                % (tuple(v.shape),))
-            bufs = _FOLDS[kind](v, g, npl, None)
-            e = self.entries[key] = [kind, v, g, npl, bufs, (v._version, g._version)]
+            e = self.entries[key] = [kind, v, g, npl, _fold(kind, v, g, npl), (v._version, g._version)]
         return e[4]
 
     def stale(self):
@@ -306,7 +310,7 @@ class FrozenWeights:
     def refresh(self):
         for e in self.entries.values():
             kind, v, g, npl, bufs, _ = e
-            _FOLDS[kind](v, g, npl, bufs)
+            _fold(kind, v, g, npl, bufs)
             e[5] = (v._version, g._version)
 
 
@@ -367,15 +371,15 @@ def _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=0, out=None, accumulate=Fal
     return dv, dg
 
 
-def _wgrad_conv(dab, x, v_shape, k, dilation, causal, p, seed_ptr, salt):
-    """partials [nsplit][Cout*Cin*k] in v's layout (Cout, Cin, k)."""
+def _wgrad_conv(dab, x, k, dilation, causal, p, seed_ptr, salt, lay):
+    """Exact-fp32 weight gradient -> partials [nsplit][M*Cin*k] in v's layout (lay.wgrad)."""
     B, M, T = dab.shape
     Cin = x.shape[1]
     nsplit = lib.raw("dv3_conv1d_wgrad_nsplit")(B, M, Cin, T, k)
     numel = M * Cin * k
     partials = torch.empty(nsplit, numel, device=x.device, dtype=torch.float32)
     lib.call("dv3_conv1d_wgrad", _p(dab), _p(x), _p(partials), numel, B, M, Cin, T, k, dilation,
-             int(causal), p, seed_ptr, salt, M, Cin * k, 0, k, 1, _stream())
+             int(causal), p, seed_ptr, salt, *lay.wgrad(M, Cin, k, False)[:5], _stream())
     return partials, nsplit
 
 
@@ -396,7 +400,7 @@ class _ConvBlockFn(torch.autograd.Function):
         _chk(x, v, g, bias, spk)
         B, C, T = x.shape
         assert v.shape == (2 * C, C, k), "ConvBlock needs in_channels == out_channels"
-        w_f, w_b, inv = _fp32_weights(v, g)
+        w_f, w_b, inv = _fp32_weights(v, g, _CONV)
         p, seed_t, salt = _drop_args(p_drop, training, x.device)
         seed_ptr = _p(seed_t)
         need_bwd = any(ctx.needs_input_grad)
@@ -436,7 +440,7 @@ class _ConvBlockFn(torch.autograd.Function):
                      int(causal), p, seed_ptr, salt, addmode, _p(e1), _p(e2), alpha, _stream())
         dv = dg = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            partials, nsplit = _wgrad_conv(dab, x, v.shape, k, dilation, causal, p, seed_ptr, salt)
+            partials, nsplit = _wgrad_conv(dab, x, k, dilation, causal, p, seed_ptr, salt, _CONV)
             dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
         dspk = dab[:, :C, :] if has_spk and ctx.needs_input_grad[4] else None
         if ctx.site is not None:            # speaker adaptation: d_e from the "a" half of the gate gradient
@@ -447,7 +451,6 @@ class _ConvBlockFn(torch.autograd.Function):
 # The weight-gradient GEMM (+ the weight-norm backward that consumes it) and the data-gradient GEMM of a block are
 # independent: run the former on a side stream so the two overlap -- most layers launch only 32-128 CTAs on 132 SMs.
 # Fork/join with stream waits, which a CUDA-graph capture records as graph edges.
-overlap_wgrad = os.environ.get("DV3_OVERLAP_WGRAD", "1") == "1"
 _side_streams = {}
 
 
@@ -456,68 +459,58 @@ class _SideStream:
     current stream waits for it at join()."""
 
     def __init__(self, dev):
-        self.enabled = overlap_wgrad
-        if self.enabled:
-            if dev not in _side_streams:
-                _side_streams[dev] = torch.cuda.Stream(device=dev)
-            self.side = _side_streams[dev]
-            self.main = torch.cuda.current_stream(dev)
-            self.ctx = torch.cuda.stream(self.side)
+        if dev not in _side_streams:
+            _side_streams[dev] = torch.cuda.Stream(device=dev)
+        self.side = _side_streams[dev]
+        self.main = torch.cuda.current_stream(dev)
+        self.ctx = torch.cuda.stream(self.side)
 
     def __enter__(self):
-        if self.enabled:
-            self.side.wait_stream(self.main)
-            self.ctx.__enter__()
+        self.side.wait_stream(self.main)
+        self.ctx.__enter__()
         return self
 
     def __exit__(self, *a):
-        if self.enabled:
-            self.ctx.__exit__(*a)
+        self.ctx.__exit__(*a)
 
     def join(self):
-        if self.enabled:
-            self.main.wait_stream(self.side)
+        self.main.wait_stream(self.side)
 
 
 def _pad8(n):
     return (n + 7) // 8 * 8
 
 
-def _tc_weights(v, g, npl):
-    """Tensor-core weight operands of a conv v (Cout, Cin, k) -> (inv, wfwd, wbwd, bank record or None, side or None):
-    wfwd [npl][k][Cout][pad8(Cin)] fp16 planes (forward GEMM), wbwd [npl][k][Cin][pad8(Cout)] bf16 planes (data
-    gradient).  Without a weight-bank record the per-layer weight norm is started on the side stream -- it depends only
-    on the parameters, so it overlaps the caller's activation split; the caller joins ``side`` before its GEMM."""
-    bank = weight_bank.weights_for(v, g, npl) if weight_bank is not None else None   # planes prepared for this step?
-    if bank is not None:
+def _tc_weights(v, g, npl, lay):
+    """Tensor-core weight operands of a layer -> (inv, wfwd, wbwd, bank record or None, side or None), as _wn_buffers
+    lays them out.  Without a weight-bank record the per-layer weight norm is started on the side stream -- it depends
+    only on the parameters, so it overlaps the caller's activation split; the caller joins ``side`` before its GEMM.
+    Only a banked layout asks the bank: it registers every layer it is asked about as a (Cout, Cin, k) conv."""
+    bank = weight_bank.weights_for(v, g, npl) if weight_bank is not None and lay.banked else None
+    if bank is not None:                                                              # planes prepared for this step
         return bank.inv, bank.wfwd, bank.wbwd, bank, None
-    fz = _frozen("tc", v, g, npl)
+    fz = _frozen(lay.tc, v, g, npl)
     if fz is not None:
         return fz[0], fz[1], fz[2], None, None
-    Cout, Cin, k = v.shape
-    dev = v.device
-    inv = torch.empty(Cout, device=dev)
-    scale = torch.empty_like(inv)
-    wfwd = torch.empty(npl, k, Cout, _pad8(Cin), device=dev, dtype=torch.float16)
-    wbwd = torch.empty(npl, k, Cin, _pad8(Cout), device=dev, dtype=torch.bfloat16)
-    side = _SideStream(dev)
-    side.keep = scale                 # written and read on the side stream: must outlive the caller's join
+    out = _wn_buffers(lay, v, npl)    # allocated on the main stream, written on the side stream
+    side = _SideStream(v.device)
+    side.keep = out[3]                # the scale, written and read on the side stream: must outlive the caller's join
     with side:
-        lib.call("dv3_tc_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), Cout, Cin, k,
-                 _stream())
-    return inv, wfwd, wbwd, bank, side
+        _fold(lay.tc, v, g, npl, out)
+    return out[0], out[1], out[2], None, side
 
 
 class _TCWeightGrad:
-    """Weight and bias gradients of a weight-normed tensor-core conv v (M, N, k), bias [M]: ``dbias`` is where the
-    gradient split sums the bias gradient; start() runs the weight-gradient GEMM and the weight-norm backward on the
-    side stream, finish() joins it after the data gradient.  With the gradient sink they are accumulated into .grad (a
-    weight-bank layer's reduction deferred to WeightBank.end_backward()) and finish() returns None for them."""
+    """Weight and bias gradients of a weight-normed tensor-core layer whose GEMM is (M, N, k) = lay.dims(v), bias rows
+    [M]: ``dbias`` is where the gradient split sums the bias gradient; start() runs the weight-gradient GEMM and the
+    weight-norm backward on the side stream, finish() joins it after the data gradient.  With the gradient sink (a
+    banked layout) they are accumulated into .grad (a weight-bank layer's reduction deferred to
+    WeightBank.end_backward()) and finish() returns None for them."""
 
-    def __init__(self, ctx, v, g):
-        self.ctx, self.v, self.g = ctx, v, g
-        self.sink = _sink(v, g, ctx.bias_param) if ctx.bias_param is not None else None
-        self.dbias = self.sink[2] if self.sink else torch.zeros(v.shape[0], device=v.device) \
+    def __init__(self, ctx, v, g, lay):
+        self.ctx, self.v, self.g, self.lay = ctx, v, g, lay
+        self.sink = _sink(v, g, ctx.bias_param) if ctx.bias_param is not None and lay.banked else None
+        self.dbias = self.sink[2] if self.sink else torch.zeros(lay.dims(v)[0], device=v.device) \
             if ctx.needs_input_grad[3] else None          # a frozen bias: no bias gradient at all
         self.side = self.dv = self.dg = self.partials = None
 
@@ -525,8 +518,9 @@ class _TCWeightGrad:
         ctx, v, g, sink = self.ctx, self.v, self.g, self.sink
         if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
             return
-        M, N, k = v.shape
+        M, N, k = self.lay.dims(v)
         nsplit = lib.raw("dv3_tc_wgrad_nsplit")(B, M, N, T, k)
+        msplit, s_m, s_mh, s_n, s_j, tap_major_k = self.lay.wgrad(M, N, k, True)
         numel = v.numel()
         # allocated on the main stream (and held until finish()), computed on the side stream
         partials = weight_bank.partials_for(ctx.bank, nsplit, numel) if (sink and ctx.bank is not None) else None
@@ -537,18 +531,18 @@ class _TCWeightGrad:
         self.dv, self.dg = (sink[0], sink[1]) if sink else (torch.empty_like(v), torch.empty_like(g))
         self.side = _SideStream(v.device)
         with self.side:
-            # partials [split][j][M][N]: contiguous float4 stores from the GEMM epilogue
             lib.call("dv3_tc_wgrad_mn_npl", _p(d_planes), _p(x_wg), npl, _p(partials), numel, B, M, N, T, k,
-                     dilation, int(causal), M, N, 0, 1, M * N, _stream())
+                     dilation, int(causal), msplit, s_m, s_mh, s_n, s_j, _stream())
             if not deferred:
-                _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=k, out=(self.dv, self.dg), accumulate=bool(sink))
+                _wn_bwd(partials, nsplit, v, g, inv, tap_major_k=tap_major_k, out=(self.dv, self.dg),
+                        accumulate=bool(sink))
 
     def finish(self):
         if self.side is not None:
             self.side.join()
         if self.sink:                 # already accumulated into the .grad arena views
             return None, None, None
-        return self.dv, self.dg, self.dbias
+        return self.dv, self.dg, self.lay.dbias(self.dbias)
 
 
 class _ConvBlockTCFn(torch.autograd.Function):
@@ -565,19 +559,16 @@ class _ConvBlockTCFn(torch.autograd.Function):
         need_bwd = any(ctx.needs_input_grad)
         need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
         p, seed_t, salt = _drop_args(p_drop, training, dev)
-        inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl)
+        inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl, _CONV)
         x_btc = torch.empty(npl, B, T, C, device=dev, dtype=torch.float16)        # forward operand (fp16)
         x_wg = torch.empty(npl, B, T, C, device=dev, dtype=bf) if need_w else None  # weight-gradient operand
         seed_ptr = _p(seed_t)
         y = torch.empty_like(x)
         a = torch.empty_like(x) if need_bwd else None
         s = torch.empty_like(x) if need_bwd else None
-        if extent is not None and k > 1:    # frames past the logical extent enter the conv as zeros
-            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), npl, _p(x_wg), B, C, T, p, seed_ptr, salt,
-                     extent[0], extent[1], _stream())
-        else:
-            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, C, T, k, dilation, int(causal), p,
-                     seed_ptr, salt, _stream())
+        ext_p, ext_m = extent if extent is not None and k > 1 else (None, 1)   # frames past it enter the conv as 0
+        lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), npl, _p(x_wg), B, C, T, p, seed_ptr, salt, ext_p, ext_m,
+                 _stream())
         if side is not None:
             side.join()
         lib.call("dv3_tc_convblock_fwd", _p(x_btc), _p(wfwd), npl, _p(bias), _p(spk), _p(x), _p(y), _p(a), _p(s),
@@ -603,7 +594,7 @@ class _ConvBlockTCFn(torch.autograd.Function):
         dy = _c(dy)
         B, C, T = x.shape
         d_btc = torch.empty(npl, B, T, 2 * C, device=dev, dtype=torch.bfloat16)
-        wg = _TCWeightGrad(ctx, v, g)
+        wg = _TCWeightGrad(ctx, v, g, _CONV)
         # the gradient past the extent is taken as 0 (see ops.extent_frames)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
         if ctx.det and wg.dbias is not None:
@@ -632,35 +623,33 @@ class _ConvBlockTCFn(torch.autograd.Function):
 
 
 class _Conv1dTCFn(torch.autograd.Function):
-    """Plain weight-normed conv (+ReLU) on the tensor-core path (1x1 convs, projections)."""
+    """Plain weight-normed conv (+ReLU) on the tensor-core path (1x1 convs, projections, and in the _CONVT layout the
+    ConvTranspose upsamplers)."""
 
     @staticmethod
-    def forward(ctx, x, v, g, bias, k, dilation, causal, relu, extent):
+    def forward(ctx, x, v, g, bias, k, dilation, causal, relu, extent, lay):
         _chk(x, v, g, bias)
         B, Cin, T = x.shape
-        Cout = v.shape[0]
+        Cout = lay.dims(v)[0]
         dev, bf = x.device, torch.bfloat16
         need_bwd = any(ctx.needs_input_grad)
         Cinp = _pad8(Cin)
         npl = _npl()
-        inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl)
+        inv, wfwd, wbwd, bank, side = _tc_weights(v, g, npl, lay)
         need_w = need_bwd and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
         x_btc = torch.empty(npl, B, T, Cinp, device=dev, dtype=torch.float16)
         x_wg = torch.empty(npl, B, T, Cinp, device=dev, dtype=bf) if need_w else None
         y = torch.empty(B, Cout, T, device=dev)
-        if extent is not None and k > 1:
-            lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, 0.0, None, 0, extent[0],
-                     extent[1], _stream())
-        else:
-            lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, k, dilation, int(causal),
-                     0.0, None, 0, _stream())
+        ext_p, ext_m = extent if extent is not None and k > 1 else (None, 1)
+        lib.call("dv3_tc_split_input_ext", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, 0.0, None, 0, ext_p, ext_m,
+                 _stream())
         if side is not None:
             side.join()
         lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), npl, _p(y), B, Cin, Cout, T, k, dilation, int(causal), 0,
-                 _p(bias), int(relu), 0.0, None, 0, 0, None, None, 0.0, None, _stream())
+                 _p(lay.bias(bias)), int(relu), 0.0, None, 0, 0, None, None, 0.0, None, _stream())
         if need_bwd:
             ctx.save_for_backward(v, g, x_wg, wbwd, inv, y if relu else None)
-            ctx.cfg = (B, Cin, Cout, T, k, dilation, causal, relu)
+            ctx.cfg = (B, Cin, Cout, T, k, dilation, causal, relu, lay)
             ctx.bias_param = bias if bias.is_leaf else None
             ctx.bank = bank
             ctx.extent = extent
@@ -671,12 +660,12 @@ class _Conv1dTCFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         v, g, x_wg, wbwd, inv, y = ctx.saved_tensors
-        B, Cin, Cout, T, k, dilation, causal, relu = ctx.cfg
+        B, Cin, Cout, T, k, dilation, causal, relu, lay = ctx.cfg
         npl = ctx.npl
         dy = _c(dy)
         dev = dy.device
         g_btc = torch.empty(npl, B, T, _pad8(Cout), device=dev, dtype=torch.bfloat16)
-        wg = _TCWeightGrad(ctx, v, g)
+        wg = _TCWeightGrad(ctx, v, g, lay)
         ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)
         if ctx.det and wg.dbias is not None:
             lib.call("dv3_tc_grad_split_det", _p(dy), _p(y), _p(g_btc), npl, _p(wg.dbias),
@@ -691,75 +680,7 @@ class _Conv1dTCFn(torch.autograd.Function):
             lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), npl, _p(dx), B, Cout, Cin, T, k, dilation, int(causal), 1, None,
                      0, 0.0, None, 0, 0, None, None, 0.0, None, _stream())
         dv, dg, dbias = wg.finish()
-        return (dx, dv, dg, dbias) + (None,) * 5
-
-
-class _ConvT2TCFn(torch.autograd.Function):
-    """ConvTranspose1d(k=2,s=2) on the tensor-core path: a 1x1 conv with 2*Cout rows (j,co) + the time interleave."""
-
-    @staticmethod
-    def forward(ctx, x, v, g, bias, extent):
-        _chk(x, v, g, bias)
-        B, Cin, T = x.shape
-        Cout = v.shape[1]
-        dev, bf = x.device, torch.bfloat16
-        Cinp, K2p = _pad8(Cin), _pad8(2 * Cout)
-        npl = _npl()
-        inv, wfwd, wbwd, _ = _frozen("convt_tc", v, g, npl) or _convt_tc_fold(v, g, npl)
-        x_btc = torch.empty(npl, B, T, Cinp, device=dev, dtype=torch.float16)
-        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
-        x_wg = torch.empty(npl, B, T, Cinp, device=dev, dtype=bf) if need_w else None
-        lib.call("dv3_tc_split_input", _p(x), _p(x_btc), npl, _p(x_wg), B, Cin, T, 1, 1, 0, 0.0, None, 0,
-                 _stream())
-        bias2 = bias.repeat(2)
-        yp = torch.empty(B, 2 * Cout, T, device=dev)
-        lib.call("dv3_tc_conv", _p(x_btc), _p(wfwd), npl, _p(yp), B, Cin, 2 * Cout, T, 1, 1, 0, 0, _p(bias2), 0, 0.0,
-                 None, 0, 0, None, None, 0.0, None, _stream())
-        y = torch.empty(B, Cout, 2 * T, device=dev)
-        lib.call("dv3_interleave2", _p(yp), _p(y), B, Cout, T, 0, _stream())
-        ctx.save_for_backward(v, g, x_wg, wbwd, inv)
-        ctx.cfg = (B, Cin, Cout, T)
-        ctx.extent = extent                 # a 2x upsampler mixes no frames: only its incoming gradient is masked
-        ctx.npl = npl
-        ctx.det = is_deterministic()
-        return y
-
-    @staticmethod
-    def backward(ctx, dy):
-        v, g, x_wg, wbwd, inv = ctx.saved_tensors
-        B, Cin, Cout, T = ctx.cfg
-        npl = ctx.npl
-        dy = _c(dy)
-        dev, bf = dy.device, torch.bfloat16
-        K2p = _pad8(2 * Cout)
-        dyp = torch.empty(B, 2 * Cout, T, device=dev)
-        lib.call("dv3_interleave2", _p(dy), _p(dyp), B, Cout, T, 1, _stream())
-        g_btc = torch.empty(npl, B, T, K2p, device=dev, dtype=bf)
-        db2 = torch.zeros(2 * Cout, device=dev) if ctx.needs_input_grad[3] else None
-        ext_p, ext_m = ctx.extent if ctx.extent is not None else (None, 1)     # dyp is in the input's time units
-        if ctx.det and db2 is not None:
-            lib.call("dv3_tc_grad_split_det", _p(dyp), None, _p(g_btc), npl, _p(db2),
-                     *_bias_scratch(B, 2 * Cout, T, True, dev), B, 2 * Cout, T, 0, ext_p, ext_m, _stream())
-        else:
-            lib.call("dv3_tc_grad_split_npl", _p(dyp), None, _p(g_btc), npl, None, _p(db2), B, 2 * Cout, T, 0, ext_p,
-                     ext_m, _stream())
-        dbias = db2[:Cout] + db2[Cout:] if db2 is not None else None
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dx = torch.empty(B, Cin, T, device=dev)
-            lib.call("dv3_tc_conv", _p(g_btc), _p(wbwd), npl, _p(dx), B, 2 * Cout, Cin, T, 1, 1, 0, 1, None, 0, 0.0, None,
-                     0, 0, None, None, 0.0, None, _stream())
-        dv = dg = None
-        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            M = 2 * Cout
-            nsplit = lib.raw("dv3_tc_wgrad_nsplit")(B, M, Cin, T, 1)
-            numel = v.numel()
-            partials = torch.empty(nsplit, numel, device=dev)
-            # element (m=(j,co), ci) -> v layout (ci, co, j): ci*2*Cout + co*2 + j
-            lib.call("dv3_tc_wgrad_mn_npl", _p(g_btc), _p(x_wg), npl, _p(partials), numel, B, M, Cin, T, 1, 1, 0,
-                     Cout, 2, 1, 2 * Cout, 0, _stream())
-            dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
-        return dx, dv, dg, dbias, None
+        return (dx, dv, dg, dbias) + (None,) * 6
 
 
 def math_mode():
@@ -826,28 +747,28 @@ def convblock(x, v, g, bias, spk=None, k=3, dilation=1, causal=False, mode=MODE_
 # ----------------------------------------------------------------------------------------------
 class _Conv1dFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, v, g, bias, k, dilation, causal, relu):
+    def forward(ctx, x, v, g, bias, k, dilation, causal, relu, lay):
         _chk(x, v, g, bias)
         B, Cin, T = x.shape
-        Cout = v.shape[0]
-        assert v.shape == (Cout, Cin, k)
-        w_f, w_b, inv = _fp32_weights(v, g)
+        Cout, N, kv = lay.dims(v)
+        assert (N, kv) == (Cin, k)
+        w_f, w_b, inv = _fp32_weights(v, g, lay)
         y = torch.empty(B, Cout, T, device=x.device, dtype=torch.float32)
-        lib.call("dv3_conv1d_fwd", _p(x), _p(w_f), _p(bias), _p(y), B, Cin, Cout, T, k, dilation,
+        lib.call("dv3_conv1d_fwd", _p(x), _p(w_f), _p(lay.bias(bias)), _p(y), B, Cin, Cout, T, k, dilation,
                  int(causal), int(relu), _stream())
         if any(ctx.needs_input_grad):
             ctx.save_for_backward(x, v, g, w_b, inv, y if relu else None)
-            ctx.cfg = (k, dilation, causal, relu)
+            ctx.cfg = (k, dilation, causal, relu, lay)
             ctx.det = is_deterministic()
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x, v, g, w_b, inv, y = ctx.saved_tensors
-        k, dilation, causal, relu = ctx.cfg
+        k, dilation, causal, relu, lay = ctx.cfg
         dy = _c(dy)
-        B, Cin, T = x.shape
-        Cout = v.shape[0]
+        B, Cout, T = dy.shape
+        Cin = x.shape[1]
         dbias = torch.zeros(Cout, device=x.device, dtype=torch.float32)
         dyr = torch.empty_like(dy) if relu else dy
         if ctx.det:
@@ -862,20 +783,26 @@ class _Conv1dFn(torch.autograd.Function):
                      0.0, None, 0, 0, None, None, 0.0, _stream())
         dv = dg = None
         if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            partials, nsplit = _wgrad_conv(dyr, x, v.shape, k, dilation, causal, 0.0, None, 0)
+            partials, nsplit = _wgrad_conv(dyr, x, k, dilation, causal, 0.0, None, 0, lay)
             dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
-        return dx, dv, dg, dbias, None, None, None, None
+        return dx, dv, dg, lay.dbias(dbias), None, None, None, None, None
 
 
 def conv1d(x, v, g, bias, k=1, dilation=1, causal=False, relu=False, extent=None):
     """Weight-normed Conv1d with 'same' (or causal) padding, optional fused ReLU.  x (B,Cin,T).  extent: as
     ``convblock``."""
+    return _conv1d(_CONV, x, v, g, bias, k, dilation, causal, relu, extent)
+
+
+def _conv1d(lay, x, v, g, bias, k, dilation, causal, relu, extent):
+    """conv1d of a layer whose parameters are in layout ``lay`` (_CONV, _CONVT)."""
     if causal:
         extent = None
-    if _use_tc_conv(x, v.shape[1], v.shape[0], k):
-        return _Conv1dTCFn.apply(_c(x), v, g, bias, int(k), int(dilation), bool(causal), bool(relu), extent)
+    M, N, _ = lay.dims(v)
+    if _use_tc_conv(x, N, M, k):
+        return _Conv1dTCFn.apply(_c(x), v, g, bias, int(k), int(dilation), bool(causal), bool(relu), extent, lay)
     y = _Conv1dFn.apply(_fp32_extent_in(_c(x), k, extent), v, g, bias, int(k), int(dilation), bool(causal),
-                        bool(relu))
+                        bool(relu), lay)
     return extent_grad_mask(y, extent)
 
 
@@ -1036,67 +963,33 @@ def speaker_residual(x, fc, e_btc):
 # ----------------------------------------------------------------------------------------------
 # ConvTranspose1d(k=2, stride=2) and Linear on the conv kernels
 # ----------------------------------------------------------------------------------------------
-class _ConvT2Fn(torch.autograd.Function):
-    """y[b,co,2t+j] = bias[co] + sum_ci x[b,ci,t] w[ci,co,j]; w = g*v/||v|| over dim 0 (= Cin).
-    Runs as a 1x1 conv with 2*Cout output rows ordered (j,co) followed by a time interleave."""
+class _Interleave2Fn(torch.autograd.Function):
+    """x (B, 2C, T) with rows ordered (j, c) -> y (B, C, 2T), y[b, c, 2t + j] = x[b, j*C + c, t]: the time interleave
+    after the 1x1 conv of a ConvTranspose1d(k=2, s=2).  A permutation: its adjoint is its inverse."""
 
     @staticmethod
-    def forward(ctx, x, v, g, bias):
-        _chk(x, v, g, bias)
-        B, Cin, T = x.shape
-        Cout = v.shape[1]
-        assert v.shape == (Cin, Cout, 2)
-        dev = x.device
-        w_f, w_b, inv, _ = _frozen("convt_fp32", v, g) or _convt_fp32_fold(v, g)     # [ci][(j,co)], [(j,co)][ci]
-        bias2 = bias.repeat(2)
-        yp = torch.empty(B, 2 * Cout, T, device=dev, dtype=torch.float32)
-        lib.call("dv3_conv1d_fwd", _p(x), _p(w_f), _p(bias2), _p(yp), B, Cin, 2 * Cout, T, 1, 1, 0, 0, _stream())
-        y = torch.empty(B, Cout, 2 * T, device=dev, dtype=torch.float32)
-        lib.call("dv3_interleave2", _p(yp), _p(y), B, Cout, T, 0, _stream())
-        ctx.save_for_backward(x, v, g, w_b, inv)
-        ctx.det = is_deterministic()
-        return y
+    def forward(ctx, x):
+        return _interleave2(x, 0)
 
     @staticmethod
     def backward(ctx, dy):
-        x, v, g, w_b, inv = ctx.saved_tensors
-        dy = _c(dy)
-        B, Cin, T = x.shape
-        Cout = v.shape[1]
-        dev = x.device
-        dyp = torch.empty(B, 2 * Cout, T, device=dev, dtype=torch.float32)
-        lib.call("dv3_interleave2", _p(dy), _p(dyp), B, Cout, T, 1, _stream())
-        db2 = torch.zeros(2 * Cout, device=dev, dtype=torch.float32)
-        if ctx.det:
-            lib.call("dv3_bias_act_bwd_det", _p(dyp), None, None, _p(db2), *_bias_scratch(B, 2 * Cout, T, False, dev),
-                     B, 2 * Cout, T, 0, _stream())
-        else:
-            lib.call("dv3_bias_act_bwd", _p(dyp), None, None, _p(db2), B, 2 * Cout, T, 0, _stream())
-        dbias = db2[:Cout] + db2[Cout:]
-        dx = None
-        if ctx.needs_input_grad[0]:
-            dx = torch.empty_like(x)
-            lib.call("dv3_conv1d_dgrad", _p(dyp), _p(w_b), _p(dx), B, 2 * Cout, Cin, T, 1, 1, 0, 0.0, None, 0, 0,
-                     None, None, 0.0, _stream())
-        dv = dg = None
-        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
-            M = 2 * Cout
-            nsplit = lib.raw("dv3_conv1d_wgrad_nsplit")(B, M, Cin, T, 1)
-            numel = v.numel()
-            partials = torch.empty(nsplit, numel, device=dev, dtype=torch.float32)
-            # element (m=(j,co), ci) -> v layout (ci, co, j): co*2 + j + ci*Cout*2
-            lib.call("dv3_conv1d_wgrad", _p(dyp), _p(x), _p(partials), numel, B, M, Cin, T, 1, 1, 0, 0.0, None, 0,
-                     Cout, 2, 1, Cout * 2, 0, _stream())
-            dv, dg = _wn_bwd(partials, nsplit, v, g, inv)
-        return dx, dv, dg, dbias
+        return _interleave2(_c(dy), 1)
+
+
+def _interleave2(x, inverse):
+    B, R, T = x.shape
+    C, T = (R, T // 2) if inverse else (R // 2, T)
+    y = torch.empty((B, 2 * C, T) if inverse else (B, C, 2 * T), device=x.device)
+    lib.call("dv3_interleave2", _p(x), _p(y), B, C, T, inverse, _stream())
+    return y
 
 
 def conv_transpose1d_k2s2(x, v, g, bias, extent=None):
-    """extent: of x's time axis; the incoming gradient past it (2x in output frames) is taken as 0."""
-    if _use_tc_conv(x, v.shape[0], 2 * v.shape[1], 1):
-        return _ConvT2TCFn.apply(_c(x), v, g, bias, extent)
-    y = _ConvT2Fn.apply(_c(x), v, g, bias)
-    return extent_grad_mask(y, None if extent is None else (extent[0], 2 * extent[1]))
+    """Weight-normed ConvTranspose1d(k=2, s=2), v (Cin, Cout, 2): y[b,co,2t+j] = bias[co] + sum_ci x[b,ci,t] w[ci,co,j],
+    w = g*v/||v|| over dim 0 (= Cin).  Runs as the 1x1 conv with 2*Cout output rows ordered (j,co) (_CONVT) followed
+    by the time interleave.  extent: of x's time axis; the incoming gradient past it (2x in output frames) is taken
+    as 0."""
+    return _Interleave2Fn.apply(_conv1d(_CONVT, x, v, g, bias, 1, 1, False, False, extent))
 
 
 def linear(x, v, g, bias):

@@ -338,7 +338,7 @@ def test_conv1d_dgrad(case):
 # ---- 4. weight gradient ---------------------------------------------------------------------------------------------
 WGRAD_CASES = [
     # (B, M, Cin, T, k, dilation, causal, layout, p_drop): layout "v" = (M, Cin, k) as ops._wgrad_conv,
-    # "convT" = ConvTranspose1d's v (Cin, Cout, 2) with M = 2 * Cout rows ordered (j, co), as ops._ConvT2Fn
+    # "convT" = ConvTranspose1d's v (Cin, Cout, 2) with M = 2 * Cout rows ordered (j, co), as ops._CONVT
     (2, 64, 80, 37, 3, 2, False, "v", 0.0),         # B*T = 74 < 128: nsplit = 1; B*T % 16 != 0
     (4, 128, 96, 131, 5, 1, True, "v", 0.05),       # nsplit > 1, B*T % 16 != 0
     (16, 256, 128, 200, 3, 1, False, "v", 0.5),     # many splits

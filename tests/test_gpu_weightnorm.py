@@ -67,7 +67,7 @@ def test_fp32_weightnorm_layouts_are_v_times_scale(shape):
 
 @pytest.mark.parametrize("shape", CONVT_SHAPES)
 def test_fp32_weightnorm_convt_layouts_are_v_times_scale(shape):
-    """The ConvTranspose1d(k=2,s=2) layouts of ops._ConvT2Fn: w_f [ci][(j,co)], w_b [(j,co)][ci]."""
+    """The ConvTranspose1d(k=2,s=2) layouts of ops._CONVT: w_f [ci][(j,co)], w_b [(j,co)][ci]."""
     ops = _ops()
     Cin, Cout = shape
     v, g = _params((Cin, Cout, 2), 20 + Cin)

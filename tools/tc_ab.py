@@ -9,7 +9,7 @@ with two operand planes and with one (npl1); the weight gradient (dv3_tc_wgrad_m
 and at two more of tests/test_gpu_tc_wgrad.py, with two planes and with one:
   * the ConvBlock shapes in the tap-major layout; at (512, 800) every CTA walks three work units;
   * (B=37, 512 x 256, T=64, k=3, causal, dilation 27) in the tap-major layout: a short last batch split;
-  * (B=77, 1024 x 512, T=40, k=1) in the ConvTranspose layout of ops._ConvT2TCFn: a short last split.
+  * (B=77, 1024 x 512, T=40, k=1) in the ConvTranspose layout of ops._CONVT: a short last split.
 All operand planes are drawn from a fixed seed; the outputs are compared element-wise (max |delta|, expected 0) and the
 per-launch times (CUDA events, L2 flushed, mean of 20) are printed side by side.
 """
@@ -95,7 +95,7 @@ def child(out_path):
         p8 = lambda n: (n + 7) // 8 * 8  # noqa: E731
         dy = torch.stack([(torch.randn(Bw, T, p8(Mw), generator=g) * s).to(bf) for s in (1e-3, 5e-4)]).to(dev)
         xw = torch.stack([(torch.randn(Bw, T, p8(Nw), generator=g) * s).to(bf) for s in (1.0, 0.5)]).to(dev)
-        if convt:       # ops._ConvT2TCFn: m = (tap, co), Cout = Mw / 2, element (m % Cout) * 2 + m // Cout + n * Mw
+        if convt:       # ops._CONVT: m = (tap, co), Cout = Mw / 2, element (m % Cout) * 2 + m // Cout + n * Mw
             ms, s_m, s_mh, s_n, s_j = Mw // 2, 2, 1, Mw, 0
         else:           # tap-major
             ms, s_m, s_mh, s_n, s_j = Mw, Nw, 0, 1, Mw * Nw
