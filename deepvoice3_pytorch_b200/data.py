@@ -559,3 +559,59 @@ class DistributedSimilarLengthSampler(torch.utils.data.Sampler):
 
     def __len__(self):
         return self.batches_per_rank * self.batch_size
+
+
+class SpeakerSampleBatches:
+    """Training batches of the speaker encoder (speaker_encoder.SpeakerEncoderStep) over a multi-speaker
+    ``TrainTxtDataset``: every batch holds B distinct speakers, each drawn from the speakers with at least N utterances
+    of >= T_crop frames, and N such utterances of each, without replacement, each cropped to T_crop frames at a
+    uniform offset.  Iterating yields {"mels": (B, N, T_crop, num_mels) float32, "speaker_ids": (B,) int64, "items":
+    (B, N) dataset indices, "offsets": (B, N) crop offsets}, len(self) batches per epoch (every eligible speaker at
+    most once), read from the .npy files (memory-mapped).  The draws are a function of (seed, epoch) alone;
+    ``set_epoch`` moves to another epoch.  ValueError when fewer than B speakers qualify."""
+
+    def __init__(self, dataset, B, N, T_crop, seed=0):
+        if not getattr(dataset, "multi_speaker", False):
+            raise ValueError("SpeakerSampleBatches needs a multi-speaker train.txt (5 columns)")
+        if B < 1 or N < 1 or T_crop < 1:
+            raise ValueError("B=%d, N=%d, T_crop=%d must be >= 1" % (B, N, T_crop))
+        self.dataset, self.B, self.N, self.T_crop, self.seed = dataset, int(B), int(N), int(T_crop), int(seed)
+        groups = {}
+        for i, (row, n) in enumerate(zip(dataset.rows, dataset.frame_lengths)):
+            if n >= T_crop:
+                groups.setdefault(int(row[4]), []).append(i)
+        self.groups = {s: idx for s, idx in sorted(groups.items()) if len(idx) >= N}
+        self.speakers = sorted(self.groups)
+        if len(self.speakers) < B:
+            raise ValueError("%d speakers have >= %d utterances of >= %d frames; a batch needs %d"
+                             % (len(self.speakers), N, T_crop, B))
+        self.epoch = 0
+
+    def set_epoch(self, epoch):
+        self.epoch = int(epoch)
+
+    def __len__(self):
+        return len(self.speakers) // self.B
+
+    def __iter__(self):
+        rng = np.random.default_rng([self.seed, self.epoch])
+        order = rng.permutation(len(self.speakers))
+        for k in range(len(self)):
+            spk = [self.speakers[j] for j in order[k * self.B:(k + 1) * self.B]]
+            items = np.stack([rng.choice(self.groups[s], self.N, replace=False) for s in spk])
+            offsets = np.zeros_like(items)
+            mels = None
+            for b in range(self.B):
+                for j in range(self.N):
+                    i = int(items[b, j])
+                    mel = self.dataset._load(self.dataset.rows[i][1])
+                    if mel.shape[0] < self.T_crop:
+                        raise ValueError("%s has %d frames, train.txt says %d"
+                                         % (self.dataset.rows[i][1], mel.shape[0], self.dataset.frame_lengths[i]))
+                    o = int(rng.integers(0, mel.shape[0] - self.T_crop + 1))
+                    offsets[b, j] = o
+                    if mels is None:
+                        mels = np.empty((self.B, self.N, self.T_crop, mel.shape[1]), dtype=np.float32)
+                    mels[b, j] = mel[o:o + self.T_crop]
+            yield {"mels": torch.from_numpy(mels), "speaker_ids": torch.tensor(spk, dtype=torch.int64),
+                   "items": torch.from_numpy(items.astype(np.int64)), "offsets": torch.from_numpy(offsets)}

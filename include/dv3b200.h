@@ -574,6 +574,39 @@ int dv3_spk_grad_reduce(const float* partials, long long nparts, float* d_e, int
 int dv3_spk_rows_grad(const float* d_e, const float* d_e2, const long long* ids, long long lo, int n, float* grad,
                       int* err_flag, int B, int S, void* stream);
 
+/* ---- speaker encoder: masked temporal mean and cloning-sample attention (spk_enc.cu) ----
+ * dv3_spkenc_pool_fwd: y[r*C + c] = sum_{t < len[r]} x[(r*C + c)*T + t] / len[r], summed in an order fixed by
+ * (C, len[r]) alone.  dv3_spkenc_pool_bwd: dx[(r*C + c)*T + t] = dy[r*C + c] / len[r] for t < len[r], else 0.  A
+ * length outside [1, T] sets *err_flag = 1 and yields 0 (nothing is read out of bounds).
+ * dv3_spkenc_attn_fwd: one CTA per speaker b over its counts[b] in [1, N] valid rows h (B, N, C):
+ * q, k, v = W h + b (W (C, C), row-major [out][in]); o = multi-head softmax(q k^T / sqrt(C/heads)) v, keys masked
+ * past counts[b]; s = w_s.o + b_s; a = softmax over the valid rows; e = W_e h + b_e (W_e (S, C)); out[b*S + s] =
+ * sum_i a_i e_i[s].  ws: dv3_spkenc_ws_floats(N, C, S, heads) floats per speaker, what the backward reads.  With a
+ * target (B, S), loss_partials[b] = sum_s |out - target|.  A count outside [1, N] sets *err_flag and yields 0.
+ * dv3_spkenc_attn_bwd: d(out) = d_out (B, S) (nullable) + d_loss[0] * loss_scale * sign(out - target) (when both
+ * are non-NULL); writes d_h (B, N, C) (rows >= counts[b]: 0) and one partial gradient row of
+ * dv3_spkenc_param_floats(C, S) floats per speaker: W_q, W_k, W_v, b_q, b_k, b_v, w_s, b_s, W_e, b_e in that order.
+ * dv3_spkenc_reduce: grad[p] = sum_{b < B} partials[b*P + p] in index order (partials nullable); loss[0] = loss_scale
+ * * sum_b loss_partials[b] in index order (loss nullable).  N <= 32, C <= 256, S <= 64, heads <= 8 dividing C.
+ * No atomics. */
+long long dv3_spkenc_ws_floats(int N, int C, int S, int heads);
+long long dv3_spkenc_param_floats(int C, int S);
+int dv3_spkenc_pool_fwd(const float* x, const int* lengths, float* y, int* err_flag, int R, int C, int T,
+                        void* stream);
+int dv3_spkenc_pool_bwd(const float* dy, const int* lengths, float* dx, int* err_flag, int R, int C, int T,
+                        void* stream);
+int dv3_spkenc_attn_fwd(const float* h, const int* counts, const float* w_q, const float* b_q, const float* w_k,
+                        const float* b_k, const float* w_v, const float* b_v, const float* w_s, const float* b_s,
+                        const float* w_e, const float* b_e, const float* target, float* out, float* ws,
+                        float* loss_partials, int* err_flag, int B, int N, int C, int S, int heads, void* stream);
+int dv3_spkenc_attn_bwd(const float* h, const int* counts, const float* w_q, const float* b_q, const float* w_k,
+                        const float* b_k, const float* w_v, const float* b_v, const float* w_s, const float* b_s,
+                        const float* w_e, const float* b_e, const float* target, const float* d_out,
+                        const float* d_loss, float loss_scale, float* ws, float* d_h, float* partials,
+                        int* err_flag, int B, int N, int C, int S, int heads, void* stream);
+int dv3_spkenc_reduce(const float* partials, long long P, const float* loss_partials, float loss_scale, float* grad,
+                      float* loss, int B, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
