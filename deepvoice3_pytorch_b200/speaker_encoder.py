@@ -128,6 +128,80 @@ class _AttentionFn(torch.autograd.Function):
         return (d_h, None, None, None) + tuple(grads[name] for name in _ATTN_PARAMS)
 
 
+def trunk_layers(mel_dim, channels, n_conv, kernel_size, embed_dim):
+    """The per-utterance trunk shared by the speaker encoder and the speaker verifier -> (spectral, temporal):
+    two weight-normed 1x1 convs mel_dim -> C -> C with ReLU, and ``n_conv`` non-causal residual Conv1dGLU blocks."""
+    C = channels
+    spectral = nn.ModuleList([modules.Conv1d(mel_dim, C, 1, std_mul=2.0), nn.ReLU(),
+                              modules.Conv1d(C, C, 1, std_mul=2.0), nn.ReLU()])
+    temporal = nn.ModuleList([modules.Conv1dGLU(1, embed_dim, C, C, kernel_size, dropout=0.0, causal=False,
+                                                residual=True) for _ in range(n_conv)])
+    return spectral, temporal
+
+
+def pooled_features(net, mels, lengths=None):
+    """The trunk of ``net`` (its ``spectral`` and ``temporal`` stacks, ``mel_dim``, ``channels`` and ``_full``) over
+    mels (B, N, T, mel_dim) -> pooled features (B, N, C).  lengths (B*N,) int32: each sample's own frame count.  The
+    stacks then run inside ``ops.length_scope``, so a sample's features are those of the sample alone, whatever its
+    padding; that is inference only (ValueError with autograd enabled)."""
+    if lengths is not None and torch.is_grad_enabled():
+        raise ValueError("per-sample lengths are for inference: call under torch.no_grad() (training batches are "
+                         "fixed-length crops)")
+    ops._chk(mels)
+    B, N, T, M = mels.shape
+    if M != net.mel_dim:
+        raise Dv3Error("mels have %d channels, the network %d" % (M, net.mel_dim))
+    if lengths is None:
+        lengths, scope = net._full(B * N, T, mels.device), contextlib.nullcontext()
+    else:
+        _chk_index(lengths, "sample lengths")
+        scope = ops.length_scope(lengths.long(), T)
+    with scope:
+        x = ops.transpose12(mels.view(B * N, T, M))
+        x = modules.run_conv_stack(net.spectral, x)
+        x = modules.run_conv_stack(net.temporal, x)
+    return masked_mean(x, lengths).view(B, N, net.channels)
+
+
+def check_samples(samples, mel_dim, max_samples):
+    """-> ``samples`` (a list over speakers of lists of (T, mel_dim) arrays or tensors) as float32 tensors, or
+    ValueError: no speakers, a speaker without samples or with more than max_samples, a sample that is not
+    (T >= 1, mel_dim) floats."""
+    if not isinstance(samples, (list, tuple)) or not samples:
+        raise ValueError("samples must be a non-empty list over speakers of lists of (T, %d) mels" % mel_dim)
+    out = []
+    for k, spk in enumerate(samples):
+        if not isinstance(spk, (list, tuple)) or not spk:
+            raise ValueError("speaker %d has no cloning samples" % k)
+        if len(spk) > max_samples:
+            raise ValueError("speaker %d has %d samples, max_samples is %d" % (k, len(spk), max_samples))
+        rows = []
+        for j, m in enumerate(spk):
+            m = torch.as_tensor(m)
+            if m.dim() != 2 or m.shape[1] != mel_dim or m.shape[0] < 1 or not m.is_floating_point():
+                raise ValueError("speaker %d sample %d: shape %s, expected (T >= 1, %d) floats"
+                                 % (k, j, tuple(m.shape), mel_dim))
+            rows.append(m.to(torch.float32))
+        out.append(rows)
+    return out
+
+
+def pad_samples(samples, mel_dim):
+    """Checked ragged samples -> (mels (n_spk, N, T, mel_dim), lengths int32 (n_spk * N,), counts int32 (n_spk,)) on the
+    host, N and T the largest count and length; a padded sample slot is one zero frame, to be masked out by counts."""
+    n_spk = len(samples)
+    N = max(len(s) for s in samples)
+    T = max(m.shape[0] for s in samples for m in s)
+    mels = torch.zeros(n_spk, N, T, mel_dim)
+    lengths = torch.ones(n_spk * N, dtype=torch.int32)
+    for k, spk in enumerate(samples):
+        for j, m in enumerate(spk):
+            mels[k, j, :m.shape[0]] = m.cpu()
+            lengths[k * N + j] = m.shape[0]
+    counts = torch.tensor([len(s) for s in samples], dtype=torch.int32)
+    return mels, lengths, counts
+
+
 def _check_model(model):
     if getattr(model, "n_speakers", 1) <= 1 or not hasattr(model, "embed_speakers"):
         raise ValueError("speaker encoding needs a multi-speaker model (n_speakers=%d)" % getattr(model, "n_speakers", 1))
@@ -159,10 +233,7 @@ class SpeakerEncoder(nn.Module):
         self.mel_dim, self.speaker_embed_dim, self.channels = mel_dim, speaker_embed_dim, channels
         self.heads, self.max_samples = heads, max_samples
         C, S = channels, speaker_embed_dim
-        self.spectral = nn.ModuleList([modules.Conv1d(mel_dim, C, 1, std_mul=2.0), nn.ReLU(),
-                                       modules.Conv1d(C, C, 1, std_mul=2.0), nn.ReLU()])
-        self.temporal = nn.ModuleList([modules.Conv1dGLU(1, S, C, C, kernel_size, dropout=0.0, causal=False,
-                                                         residual=True) for _ in range(n_conv)])
+        self.spectral, self.temporal = trunk_layers(mel_dim, C, n_conv, kernel_size, S)
 
         def weight(rows, cols):
             return nn.Parameter(torch.randn(rows, cols) / math.sqrt(cols))
@@ -180,26 +251,8 @@ class SpeakerEncoder(nn.Module):
         return self._cache[key]
 
     def pooled(self, mels, lengths=None):
-        """mels (B, N, T, mel_dim) -> pooled features (B, N, C).  lengths (B*N,) int32: each sample's own frame count.
-        The stacks then run inside ``ops.length_scope``, so a sample's features are those of the sample alone, whatever
-        its padding; that is inference only (ValueError with autograd enabled)."""
-        if lengths is not None and torch.is_grad_enabled():
-            raise ValueError("per-sample lengths are for inference: call under torch.no_grad() (training batches are "
-                             "fixed-length crops)")
-        ops._chk(mels)
-        B, N, T, M = mels.shape
-        if M != self.mel_dim:
-            raise Dv3Error("mels have %d channels, the encoder %d" % (M, self.mel_dim))
-        if lengths is None:
-            lengths, scope = self._full(B * N, T, mels.device), contextlib.nullcontext()
-        else:
-            _chk_index(lengths, "sample lengths")
-            scope = ops.length_scope(lengths.long(), T)
-        with scope:
-            x = ops.transpose12(mels.view(B * N, T, M))
-            x = modules.run_conv_stack(self.spectral, x)
-            x = modules.run_conv_stack(self.temporal, x)
-        return masked_mean(x, lengths).view(B, N, self.channels)
+        """mels (B, N, T, mel_dim) -> pooled features (B, N, C) (``pooled_features``)."""
+        return pooled_features(self, mels, lengths)
 
     def attend(self, h, counts=None, target=None):
         """Cloning-sample attention of pooled features h (B, N, C) -> (embeddings (B, S), L1 loss against target)."""
@@ -220,25 +273,8 @@ class SpeakerEncoder(nn.Module):
         return self.attend(self.pooled(mels), None, target)[1]
 
     def check_samples(self, samples):
-        """-> the samples as float32 tensors, or ValueError: no speakers, a speaker without samples or with more than
-        max_samples, a sample that is not (T >= 1, mel_dim)."""
-        if not isinstance(samples, (list, tuple)) or not samples:
-            raise ValueError("samples must be a non-empty list over speakers of lists of (T, %d) mels" % self.mel_dim)
-        out = []
-        for k, spk in enumerate(samples):
-            if not isinstance(spk, (list, tuple)) or not spk:
-                raise ValueError("speaker %d has no cloning samples" % k)
-            if len(spk) > self.max_samples:
-                raise ValueError("speaker %d has %d samples, max_samples is %d" % (k, len(spk), self.max_samples))
-            rows = []
-            for j, m in enumerate(spk):
-                m = torch.as_tensor(m)
-                if m.dim() != 2 or m.shape[1] != self.mel_dim or m.shape[0] < 1 or not m.is_floating_point():
-                    raise ValueError("speaker %d sample %d: shape %s, expected (T >= 1, %d) floats"
-                                     % (k, j, tuple(m.shape), self.mel_dim))
-                rows.append(m.to(torch.float32))
-            out.append(rows)
-        return out
+        """-> the samples as float32 tensors, or ValueError (``check_samples``)."""
+        return check_samples(samples, self.mel_dim, self.max_samples)
 
     def embed_batch(self, samples):
         """samples: a list over speakers of lists of (T_i, mel_dim) arrays or tensors, ragged in length and in count ->
@@ -246,18 +282,8 @@ class SpeakerEncoder(nn.Module):
         be alone: the stacks run inside ``ops.length_scope`` (each sample sees the zeros it would see alone), the pool
         averages each sample's own frames, the attention masks the padded sample slots -- bit-identical under
         ``conv_math="fp32"``, within the tensor-core tolerance otherwise."""
-        samples = self.check_samples(samples)
+        mels, lengths, counts = pad_samples(self.check_samples(samples), self.mel_dim)
         dev = self.w_q.device
-        n_spk = len(samples)
-        N = max(len(s) for s in samples)
-        T = max(m.shape[0] for s in samples for m in s)
-        mels = torch.zeros(n_spk, N, T, self.mel_dim)
-        lengths = torch.ones(n_spk * N, dtype=torch.int32)        # padded slots: one zero frame, masked out below
-        for k, spk in enumerate(samples):
-            for j, m in enumerate(spk):
-                mels[k, j, :m.shape[0]] = m.cpu()
-                lengths[k * N + j] = m.shape[0]
-        counts = torch.tensor([len(s) for s in samples], dtype=torch.int32)
         was_training = self.training
         self.eval()
         try:
@@ -282,52 +308,50 @@ def clone_voices(model, encoder, samples):
     return model.add_speakers(len(samples), init=encoder.embed_batch(samples))
 
 
-class SpeakerEncoderStep:
-    """One training step of a SpeakerEncoder: the L1 regression of ``model.embed_speakers.weight[speaker_ids]``
-    (detached: the multi-speaker model runs no forward and keeps every bit), then clip + Adam (``train_step.FlatAdam``
-    over a ``ParameterArena`` of the encoder's parameters; clip_thresh None: no clipping).
+def check_single_process(name):
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError("%s runs in a single process (world size %d)" % (name, dist.get_world_size()))
 
-    ``step(batch)`` takes {"mels": (B, N, T, mel_dim) fp32, "speaker_ids": (B,) int64} (as ``data.SpeakerSampleBatches``
-    yields them), every batch of one shape.  use_graph: one CUDA graph covers forward, backward and update.  The step
-    runs in the ``ops.conv_math`` and ``ops.deterministic`` modes current at construction.  The graph reads the speaker
-    table at the address it had at capture; when the table has moved since (``add_speakers`` / ``clone_voices`` install
-    a new one, a ``TrainStep`` over the model re-homes it), the next ``step()`` captures a new graph.  Single process
-    only.
-    ValueError before any launch for a world size above 1, a single-speaker model or an encoder whose
-    speaker_embed_dim differs from the model's."""
 
-    def __init__(self, encoder, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, clip_thresh=None, use_graph=True):
+class ArenaGraphStep:
+    """What the speaker encoder's and the speaker verifier's training steps share: clip + Adam (``train_step.FlatAdam``
+    over a ``ParameterArena`` of ``net``'s parameters; clip_thresh None: no clipping), the ``ops.conv_math`` and
+    ``ops.deterministic`` modes current at construction, one batch shape, checkpoints of copies that resume bit-exactly,
+    and with use_graph one CUDA graph for forward, backward and update.  A subclass defines ``_objective(batch)`` (the
+    loss to minimise, on device tensors), ``_check_batch(batch)`` (ValueError before any launch) and may define
+    ``_graph_key()`` (when it changes, the next step captures a new graph)."""
+
+    _net_key = "net"
+
+    def __init__(self, net, lr, betas, eps, clip_thresh, use_graph):
         from .train_step import FlatAdam, ParameterArena
-        if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-            raise ValueError("SpeakerEncoderStep runs in a single process (world size %d)" % dist.get_world_size())
-        _check_model(model)
-        if encoder.speaker_embed_dim != model.speaker_embed_dim:
-            raise ValueError("encoder speaker_embed_dim=%d, model %d" % (encoder.speaker_embed_dim,
-                                                                         model.speaker_embed_dim))
         self.math = ops.math_mode()
         self.deterministic = ops.is_deterministic()
         self._det_scratch = ops.DetScratch() if self.deterministic else None
-        self.encoder, self.model, self.lr = encoder, model, lr
-        self.arena = ParameterArena(encoder, list(encoder.parameters()))
+        self.net, self.lr = net, lr
+        self.arena = ParameterArena(net, list(net.parameters()))
         self.opt = FlatAdam(self.arena, lr, betas, eps, 0.0 if clip_thresh is None else float(clip_thresh))
         self.use_graph = use_graph
         self.global_step = 0
-        self._graph = self._static = self._loss = self._shape = self._table_key = None
+        self._graph = self._static = self._loss = self._shape = self._captured_key = None
         self.launches_per_step = None
         self.graphs_captured = 0
         self.capture_seconds = 0.0
 
     def state_dict(self):
-        """A checkpoint of copies (the encoder's own state_dict holds views of the live parameter arena)."""
-        return {"encoder": {k: v.clone() for k, v in self.encoder.state_dict().items()},
+        """A checkpoint of copies (the network's own state_dict holds views of the live parameter arena)."""
+        return {self._net_key: {k: v.clone() for k, v in self.net.state_dict().items()},
                 "optimizer": self.opt.state_dict(), "global_step": self.global_step}
 
     def load_state_dict(self, ckpt):
         """Resume bit-exactly from ``state_dict()``: parameters (in place, so captured graphs stay valid), Adam moments
         and step count."""
-        self.encoder.load_state_dict(ckpt["encoder"])
+        self.net.load_state_dict(ckpt[self._net_key])
         self.opt.load_state_dict(ckpt["optimizer"])
         self.global_step = int(ckpt.get("global_step", 0))
+
+    def _graph_key(self):
+        return None
 
     def _forward_backward(self, batch):
         self.arena.zero_grad()
@@ -336,33 +360,26 @@ class SpeakerEncoderStep:
         if self.deterministic:
             ops.det_scratch = self._det_scratch
         try:
-            with torch.no_grad():
-                target = ops.embedding(batch["speaker_ids"], self.model.embed_speakers.weight.detach())
-            loss = self.encoder.loss(batch["mels"], target)
+            loss = self._objective(batch)
             loss.backward()
             return loss.detach()
         finally:
             ops.deterministic, ops.det_scratch = outer
 
     def step(self, batch):
-        """-> the batch's L1 loss (a device scalar, valid until the next step)."""
+        """-> the batch's loss (a device scalar, valid until the next step)."""
+        name = type(self).__name__
         if ops.math_mode() != self.math:
-            raise ValueError("SpeakerEncoderStep was built with ops.conv_math = %r and cannot step under %r"
-                             % (self.math, ops.conv_math))
+            raise ValueError("%s was built with ops.conv_math = %r and cannot step under %r"
+                             % (name, self.math, ops.conv_math))
         dev = self.arena.flat.device
         batch = {k: batch[k] for k in ("mels", "speaker_ids")}
-        mels, ids = batch["mels"], batch["speaker_ids"]
-        enc = self.encoder
-        if mels.dim() != 4 or mels.shape[1] > enc.max_samples or mels.shape[3] != enc.mel_dim or \
-                mels.dtype != torch.float32 or tuple(ids.shape) != (mels.shape[0],) or ids.dtype != torch.int64:
-            raise ValueError("batch mels %s %s / speaker_ids %s %s: expected (B, N <= %d, T, %d) float32 and (B,) int64"
-                             % (tuple(mels.shape), mels.dtype, tuple(ids.shape), ids.dtype, enc.max_samples,
-                                enc.mel_dim))
+        self._check_batch(batch)
         shape = tuple(tuple(v.shape) for v in batch.values())
         if self._shape is not None and shape != self._shape:
-            raise ValueError("SpeakerEncoderStep batches have one shape: %s, then %s" % (self._shape, shape))
+            raise ValueError("%s batches have one shape: %s, then %s" % (name, self._shape, shape))
         self._shape = shape
-        self.encoder.train()
+        self.net.train()
         self.opt.set_hyper(self.lr)
         if not self.use_graph:
             loss = self._forward_backward({k: v.to(dev, non_blocking=True) for k, v in batch.items()})
@@ -372,14 +389,9 @@ class SpeakerEncoderStep:
         self.global_step += 1
         return loss
 
-    def _table(self):
-        """(address, shape) of the speaker table the targets are read from."""
-        w = self.model.embed_speakers.weight
-        return w.data_ptr(), tuple(w.shape), w.dtype, w.device
-
     def _graph_step(self, batch):
-        if self._graph is not None and self._table() != self._table_key:
-            self._graph = self._static = self._loss = None     # the captured lookup reads the old table: capture anew
+        if self._graph is not None and self._graph_key() != self._captured_key:
+            self._graph = self._static = self._loss = None     # the captured step reads stale addresses: capture anew
         if self._graph is None:
             t0 = time.perf_counter()
             dev = self.arena.flat.device
@@ -391,7 +403,7 @@ class SpeakerEncoderStep:
                     self._forward_backward(self._static)
             torch.cuda.current_stream().wait_stream(s)
             self._graph = torch.cuda.CUDAGraph()
-            self._table_key = self._table()
+            self._captured_key = self._graph_key()
             n0 = lib.raw("dv3_launch_count")()
             with torch.cuda.graph(self._graph):
                 self._loss = self._forward_backward(self._static)
@@ -404,3 +416,47 @@ class SpeakerEncoderStep:
             self._static[k].copy_(v, non_blocking=True)
         self._graph.replay()
         return self._loss
+
+
+class SpeakerEncoderStep(ArenaGraphStep):
+    """One training step of a SpeakerEncoder: the L1 regression of ``model.embed_speakers.weight[speaker_ids]``
+    (detached: the multi-speaker model runs no forward and keeps every bit), then clip + Adam (``ArenaGraphStep``).
+
+    ``step(batch)`` takes {"mels": (B, N, T, mel_dim) fp32, "speaker_ids": (B,) int64} (as ``data.SpeakerSampleBatches``
+    yields them), every batch of one shape.  use_graph: one CUDA graph covers forward, backward and update.  The step
+    runs in the ``ops.conv_math`` and ``ops.deterministic`` modes current at construction.  The graph reads the speaker
+    table at the address it had at capture; when the table has moved since (``add_speakers`` / ``clone_voices`` install
+    a new one, a ``TrainStep`` over the model re-homes it), the next ``step()`` captures a new graph.  Single process
+    only.
+    ValueError before any launch for a world size above 1, a single-speaker model or an encoder whose
+    speaker_embed_dim differs from the model's."""
+
+    _net_key = "encoder"
+
+    def __init__(self, encoder, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, clip_thresh=None, use_graph=True):
+        check_single_process("SpeakerEncoderStep")
+        _check_model(model)
+        if encoder.speaker_embed_dim != model.speaker_embed_dim:
+            raise ValueError("encoder speaker_embed_dim=%d, model %d" % (encoder.speaker_embed_dim,
+                                                                         model.speaker_embed_dim))
+        super().__init__(encoder, lr, betas, eps, clip_thresh, use_graph)
+        self.encoder, self.model = encoder, model
+
+    def _objective(self, batch):
+        with torch.no_grad():
+            target = ops.embedding(batch["speaker_ids"], self.model.embed_speakers.weight.detach())
+        return self.encoder.loss(batch["mels"], target)
+
+    def _check_batch(self, batch):
+        mels, ids = batch["mels"], batch["speaker_ids"]
+        enc = self.encoder
+        if mels.dim() != 4 or mels.shape[1] > enc.max_samples or mels.shape[3] != enc.mel_dim or \
+                mels.dtype != torch.float32 or tuple(ids.shape) != (mels.shape[0],) or ids.dtype != torch.int64:
+            raise ValueError("batch mels %s %s / speaker_ids %s %s: expected (B, N <= %d, T, %d) float32 and (B,) int64"
+                             % (tuple(mels.shape), mels.dtype, tuple(ids.shape), ids.dtype, enc.max_samples,
+                                enc.mel_dim))
+
+    def _graph_key(self):
+        """(address, shape) of the speaker table the targets are read from."""
+        w = self.model.embed_speakers.weight
+        return w.data_ptr(), tuple(w.shape), w.dtype, w.device

@@ -607,6 +607,36 @@ int dv3_spkenc_attn_bwd(const float* h, const int* counts, const float* w_q, con
 int dv3_spkenc_reduce(const float* partials, long long P, const float* loss_partials, float loss_scale, float* grad,
                       float* loss, int B, void* stream);
 
+/* ---- speaker verifier: enrollment / test embeddings, PLDA-like pair scores, balanced BCE (spk_ver.cu) ----
+ * dv3_spkver_embed_fwd: row b reads counts[b] in [1, N] valid rows h[b*ld + i*C + c] (i < counts[b], C channels):
+ * hbar[b*C + c] = their mean (summed in i order); out[b*D + d] = sum_c w[d*C + c] hbar[b*C + c] + c[d] (w (D, C)).
+ * ld >= N*C is the float stride between rows b (a test row of a (B, N+1, C) batch: h offset by N*C, ld (N+1)*C).
+ * dv3_spkver_embed_bwd: d_h[b*ld + i*C + c] = sum_d w[d*C + c] d_out[b*D + d] / counts[b] for i < counts[b], 0 for
+ * counts[b] <= i < N; one partial row of D*C + D floats per row b: d w = d_out hbar^T, then d c = d_out.  A count
+ * outside [1, N] sets *err_flag = 1 and yields 0 (nothing is read out of bounds).
+ * dv3_spkver_score_fwd: scores[e*B_t + t] = x_e.y_t - x_e^T S x_e - y_t^T S y_t + bias[0] for x (B_e, D), y (B_t, D),
+ * S (D, D); qx (B_e) / qy (B_t) receive the quadratic terms, computed once per row.  A pair's bits depend on its two
+ * rows alone.  With int64 speaker ids ids_e (B_e) / ids_t (B_t) (nullable, with loss_partials), pair (e, t) is a
+ * same-speaker pair when the ids are equal; loss_partials (dv3_spkver_loss_floats(B_e, B_t) floats, row-major over
+ * (e, 32-pair column tile)) receive sum over the tile's t of softplus(-L) / (2 n_same) (same) or softplus(L) /
+ * (2 n_diff) (different), n_same / n_diff counted on the device over the whole batch (an empty class weighs 0).
+ * dv3_spkenc_reduce(NULL, 0, loss_partials, 1, NULL, loss, dv3_spkver_loss_floats(B_e, B_t)) sums them in order.
+ * dv3_spkver_score_bwd: G = d_scores (nullable) + d_loss[0] * d(loss)/d(scores) (when ids and d_loss are non-NULL);
+ * dx_e = sum_t G[e,t] y_t - g_e (S + S^T) x_e with g_e = sum_t G[e,t], dy likewise; one partial row of D*D + 1 floats
+ * per row of x (rows 0..B_e-1) then of y: d S = -g z z^T, then d bias (g_e on x rows, 0 on y rows).
+ * N <= 32, C <= 256, D <= 128.  Every sum runs in an order fixed by the shapes; no atomics. */
+long long dv3_spkver_loss_floats(int B_e, int B_t);
+int dv3_spkver_embed_fwd(const float* h, long long ld, const int* counts, const float* w, const float* c, float* hbar,
+                         float* out, int* err_flag, int B, int N, int C, int D, void* stream);
+int dv3_spkver_embed_bwd(const float* d_out, const float* hbar, const int* counts, const float* w, float* d_h,
+                         long long ld, float* partials, int* err_flag, int B, int N, int C, int D, void* stream);
+int dv3_spkver_score_fwd(const float* x, const float* y, const float* S, const float* bias, const long long* ids_e,
+                         const long long* ids_t, float* qx, float* qy, float* scores, float* loss_partials, int B_e,
+                         int B_t, int D, void* stream);
+int dv3_spkver_score_bwd(const float* x, const float* y, const float* S, const float* scores, const long long* ids_e,
+                         const long long* ids_t, const float* d_scores, const float* d_loss, float* dx, float* dy,
+                         float* partials, int B_e, int B_t, int D, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
