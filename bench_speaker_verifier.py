@@ -49,11 +49,11 @@ class EagerVerifierStep:
         v, g = self.p[pre + "weight_v"], self.p[pre + "weight_g"]
         return g * v / v.pow(2).sum((1, 2), keepdim=True).sqrt()
 
-    def step(self, b):
+    def trunk(self, mels):
+        """mels (B, N, T, M) -> pooled features (B, N, C): the speaker encoder's trunk in eager torch."""
         p = self.p
-        self.opt.zero_grad(set_to_none=False)
-        Bb, Nn, T, M = b["mels"].shape
-        x = b["mels"].view(Bb * Nn, T, M).transpose(1, 2)
+        Bb, Nn, T, M = mels.shape
+        x = mels.view(Bb * Nn, T, M).transpose(1, 2)
         for i in (0, 2):
             x = torch.relu(F.conv1d(x, self._wn("spectral.%d." % i), p["spectral.%d.bias" % i]))
         for i in range(self.n_conv):
@@ -61,7 +61,12 @@ class EagerVerifierStep:
             y = F.conv1d(x, self._wn(pre), p[pre + "bias"], padding=(self.k - 1) // 2)
             a, gate = y.chunk(2, dim=1)
             x = (a * torch.sigmoid(gate) + x) * math.sqrt(0.5)
-        h = x.mean(-1).view(Bb, Nn, -1)
+        return x.mean(-1).view(Bb, Nn, -1)
+
+    def step(self, b):
+        p = self.p
+        self.opt.zero_grad(set_to_none=False)
+        h = self.trunk(b["mels"])
         e = F.linear(h[:, :-1].mean(1), p["w"], p["c"])
         t = F.linear(h[:, -1], p["w"], p["c"])
         S = p["S"]

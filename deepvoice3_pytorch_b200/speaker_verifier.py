@@ -264,6 +264,40 @@ def equal_error_rate(scores, labels):
     return float(eer), float(thr[k - 1] + a * (thr[k] - thr[k - 1]))
 
 
+def cloned_voice_mels(model, mel_dim, speaker_ids, sequences, vocoder, batch_size, device, stage_timer=None):
+    """What the cloned-voice evaluations (``verify_cloned_voices``, ``speaker_classifier.classify_cloned_voices``)
+    share.  First the checks, ValueError before any launch: a single-speaker model, an unknown phase method,
+    mismatched list lengths, speaker ids outside [0, n_speakers), an evaluation network of ``mel_dim`` mel channels
+    where the audio path makes another count, malformed sequences.  Then every ``sequences[k]`` synthesized in the voice
+    ``speaker_ids[k]`` with ``synthesis.tts_batch`` (stage "synthesis") and turned into normalised mels on ``device``
+    with ``audio.stft_mel_batch`` (stage "mel") -> (speaker ids as ints, list of (T_k, num_mels) mels)."""
+    from . import synthesis
+    _check_model(model)
+    audio.check_phase_method(vocoder)
+    speaker_ids = [int(s) for s in speaker_ids]
+    if len(speaker_ids) != len(sequences):
+        raise ValueError("%d speaker_ids for %d sequences" % (len(speaker_ids), len(sequences)))
+    bad = [s for s in speaker_ids if not 0 <= s < model.n_speakers]
+    if bad:
+        raise ValueError("speaker ids %s outside [0, %d)" % (bad, model.n_speakers))
+    if mel_dim != audio.hparams.num_mels:
+        raise ValueError("the evaluation network takes %d mel channels, the audio path makes %d"
+                         % (mel_dim, audio.hparams.num_mels))
+    synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
+    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    with stage("synthesis"):
+        wavs = [w for w, _, _, _ in synthesis.tts_batch(model, sequences, speaker_ids, batch_size=batch_size,
+                                                        vocoder=vocoder)]
+    with stage("mel"):
+        lens = [len(w) for w in wavs]
+        pad = np.zeros((len(wavs), max(lens)), np.float32)
+        for k, w in enumerate(wavs):
+            pad[k, :lens[k]] = w
+        _, mel = audio.stft_mel_batch(torch.from_numpy(pad).to(device), torch.tensor(lens, dtype=torch.int32),
+                                      want_linear=False)
+        return speaker_ids, [mel[k, :audio.num_frames(n)] for k, n in enumerate(lens)]
+
+
 def verify_cloned_voices(model, verifier, speaker_ids, enrollment, sequences, vocoder="griffin_lim", batch_size=16,
                          stage_timer=None):
     """The paper's speaker-verification evaluation of cloned voices in one call:
@@ -277,40 +311,18 @@ def verify_cloned_voices(model, verifier, speaker_ids, enrollment, sequences, vo
     enrollment: {speaker id: list of (T, mel_dim) real normalised mels}; every id of speaker_ids must be enrolled, and at
     least two speakers, so that there are same- and different-speaker trials.  stage_timer: optional ``name -> context
     manager`` around "synthesis", "mel" and "scoring".  ValueError before any launch for a single-speaker model, ids out
-    of range or without enrollment, mismatched list lengths or malformed inputs."""
-    from . import synthesis
-    _check_model(model)
-    audio.check_phase_method(vocoder)
+    of range or without enrollment, mismatched list lengths or malformed inputs (``cloned_voice_mels``)."""
     speaker_ids = [int(s) for s in speaker_ids]
-    if len(speaker_ids) != len(sequences):
-        raise ValueError("%d speaker_ids for %d sequences" % (len(speaker_ids), len(sequences)))
-    bad = [s for s in speaker_ids if not 0 <= s < model.n_speakers]
-    if bad:
-        raise ValueError("speaker ids %s outside [0, %d)" % (bad, model.n_speakers))
     if not isinstance(enrollment, dict) or len(enrollment) < 2:
         raise ValueError("enrollment must map at least two speaker ids to lists of real utterances")
     enrolled = sorted(int(k) for k in enrollment)
     missing = sorted(set(speaker_ids) - set(enrolled))
     if missing:
         raise ValueError("speakers %s have no enrollment utterances" % missing)
-    if verifier.mel_dim != audio.hparams.num_mels:
-        raise ValueError("the verifier takes %d mel channels, the audio path makes %d" % (verifier.mel_dim,
-                                                                                      audio.hparams.num_mels))
     samples = check_samples([enrollment[k] for k in enrolled], verifier.mel_dim, verifier.max_enroll)
-    synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
+    speaker_ids, tests = cloned_voice_mels(model, verifier.mel_dim, speaker_ids, sequences, vocoder, batch_size,
+                                           verifier.w.device, stage_timer)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
-    dev = verifier.w.device
-    with stage("synthesis"):
-        wavs = [w for w, _, _, _ in synthesis.tts_batch(model, sequences, speaker_ids, batch_size=batch_size,
-                                                        vocoder=vocoder)]
-    with stage("mel"):
-        lens = [len(w) for w in wavs]
-        pad = np.zeros((len(wavs), max(lens)), np.float32)
-        for k, w in enumerate(wavs):
-            pad[k, :lens[k]] = w
-        _, mel = audio.stft_mel_batch(torch.from_numpy(pad).to(dev), torch.tensor(lens, dtype=torch.int32),
-                                      want_linear=False)
-        tests = [mel[k, :audio.num_frames(n)] for k, n in enumerate(lens)]
     with stage("scoring"):
         scores = verifier.score(verifier.embed_enrollment(samples), verifier.embed_tests(tests))
         scores = scores.double().cpu().numpy()

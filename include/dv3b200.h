@@ -637,6 +637,25 @@ int dv3_spkver_score_bwd(const float* x, const float* y, const float* S, const f
                          const long long* ids_t, const float* d_scores, const float* d_loss, float* dx, float* dy,
                          float* partials, int B_e, int B_t, int D, void* stream);
 
+/* ---- speaker classifier: logits, log-sum-exp, argmax and softmax cross-entropy over K classes (spk_cls.cu) ----
+ * dv3_spkcls_fwd: logits[r*K + k] = sum_c h[r*ld + c] w[k*C + c] + bias[k] (summed in c order) for R rows of C
+ * channels (ld >= C floats apart) and w (K, C); lse[r] = log sum_k exp(logits[r*K + k]) over a thread partition fixed
+ * by K alone; pred[r] = argmax_k logits[r*K + k], ties to the lowest index.  With int64 labels (R) (nullable, with
+ * loss_partials): loss_partials[r] = lse[r] - logits[r*K + labels[r]];
+ * dv3_spkenc_reduce(NULL, 0, loss_partials, 1/R, NULL, loss, R) gives the mean cross-entropy.  A row's logits, lse and
+ * pred depend on that row alone.
+ * dv3_spkcls_bwd: G[r,k] = d_logits[r*K + k] (nullable) + d_loss[0] * loss_scale * (exp(logits[r*K + k] - lse[r]) -
+ * [k == labels[r]]) (the second term when labels and d_loss are non-NULL), never stored; d_h[r*C + c] = sum_k G[r,k]
+ * w[k*C + c] (k in order, d_h dense); d_w[k*C + c] = sum_r G[r,k] h[r*ld + c] and d_bias[k] = sum_r G[r,k] (r in
+ * order), written directly.  A label outside [0, K) sets *err_flag = 1; its row adds 0 to the loss and nothing to the onehot.
+ * C <= 256, 2 <= K <= 8192, R*K < 2^31.  No atomics. */
+int dv3_spkcls_fwd(const float* h, long long ld, const float* w, const float* bias, const long long* labels,
+                   float* logits, float* lse, int* pred, float* loss_partials, int* err_flag, int R, int C, int K,
+                   void* stream);
+int dv3_spkcls_bwd(const float* h, long long ld, const float* w, const float* logits, const float* lse,
+                   const long long* labels, const float* d_logits, const float* d_loss, float loss_scale, float* d_h,
+                   float* d_w, float* d_bias, int* err_flag, int R, int C, int K, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
