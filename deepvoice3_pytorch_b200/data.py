@@ -14,6 +14,8 @@ padding rules, and a distributed variant of its length-bucketed sampler.
   ``WavDataset.from_vctk`` does the same for a VCTK tree at its recording rate: its items carry the part of each file
   that the label cut and the silence trim keep, and the GPU resamples just that part per batch
   (``audio.resample_segments``), bit-identical to what ``preprocess.build_vctk_from_path`` writes.
+* ``CloningSampleDataset`` + ``collate_cloning`` add each row's cloning samples ("speaker_mels") for fine-tuning a
+  speaker encoder through the training loss (``TrainStep(speaker_encoder=...)``).
 * ``DistributedSimilarLengthSampler`` restates ``PartialyRandomizedSimilarTimeLengthSampler`` (train.py:195-239):
   sort by length, shuffle inside groups of ``batch_group_size``, permute whole mini-batches -- then deals the
   mini-batches round-robin to the ranks, so every rank sees disjoint batches of similar length (what the
@@ -559,6 +561,83 @@ class DistributedSimilarLengthSampler(torch.utils.data.Sampler):
 
     def __len__(self):
         return self.batches_per_rank * self.batch_size
+
+
+class CloningSampleDataset(torch.utils.data.Dataset):
+    """A multi-speaker ``TrainTxtDataset`` whose items carry cloning samples, for fine-tuning a speaker encoder through
+    the training loss (``TrainStep(speaker_encoder=...)``).  Item i is the dataset's item i plus, last, N crops
+    (N, T_crop, num_mels) float32 of T_crop frames each, from other utterances of the same speaker that have at least
+    T_crop frames: drawn without replacement when the speaker has at least N of them, with replacement otherwise; each
+    crop at a uniform offset, read from the memory-mapped .npy file.  The draws are a function of (seed, epoch, i)
+    alone, so a row's samples depend neither on the batch it lands in nor on the DataLoader's workers; ``set_epoch``
+    moves to another epoch.  ValueError at construction for a speaker with fewer than two such utterances (one of its
+    utterances would have no other to draw from)."""
+
+    def __init__(self, dataset, N, T_crop, seed=0):
+        if not getattr(dataset, "multi_speaker", False):
+            raise ValueError("CloningSampleDataset needs a multi-speaker train.txt (5 columns)")
+        if N < 1 or T_crop < 1:
+            raise ValueError("N=%d, T_crop=%d must be >= 1" % (N, T_crop))
+        self.dataset, self.N, self.T_crop, self.seed = dataset, int(N), int(T_crop), int(seed)
+        self.frame_lengths = dataset.frame_lengths
+        self._speaker = np.array([int(row[4]) for row in dataset.rows], dtype=np.int64)
+        eligible = {}
+        for i, (s, n) in enumerate(zip(self._speaker.tolist(), dataset.frame_lengths)):
+            if n >= T_crop:
+                eligible.setdefault(s, []).append(i)
+        # one ascending array per speaker; item i's own utterance is skipped at draw time
+        self._eligible = {s: np.array(idx, dtype=np.int64) for s, idx in eligible.items()}
+        for s in sorted(set(self._speaker.tolist())):
+            n = len(self._eligible.get(s, ()))
+            if n < 2:       # none at all, or one that has no other to draw from
+                raise ValueError("speaker %d has %d utterance(s) of >= %d frames: every utterance of the speaker needs "
+                                 "another one to draw its cloning samples from" % (s, n, T_crop))
+        self.epoch = 0
+
+    def set_epoch(self, epoch):
+        self.epoch = int(epoch)
+
+    def __len__(self):
+        return len(self.dataset)
+
+    def draws(self, i):
+        """-> (dataset indices (N,), crop offsets (N,)) of item i's cloning samples in the current epoch."""
+        rng = np.random.default_rng([self.seed, self.epoch, int(i)])
+        pool = self._eligible[int(self._speaker[i])]
+        p = int(np.searchsorted(pool, i))
+        own = bool(p < pool.size and pool[p] == i)
+        m = pool.size - int(own)                # the pool without item i's own utterance
+        k = rng.choice(m, self.N, replace=m < self.N)
+        if own:
+            k = k + (k >= p)                    # positions at or past the own one shift by one
+        items = pool[k]
+        offsets = np.array([rng.integers(0, self.dataset.frame_lengths[j] - self.T_crop + 1) for j in items],
+                           dtype=np.int64)
+        return items, offsets
+
+    def __getitem__(self, i):
+        import os
+        items, offsets = self.draws(i)
+        crops = None
+        for k, (j, o) in enumerate(zip(items, offsets)):
+            name = self.dataset.rows[j][1]
+            mel = np.load(os.path.join(self.dataset.data_root, name), mmap_mode="r")
+            if mel.shape[0] < o + self.T_crop:
+                raise ValueError("%s has %d frames, train.txt says %d" % (name, mel.shape[0],
+                                                                          self.dataset.frame_lengths[j]))
+            if crops is None:
+                crops = np.empty((self.N, self.T_crop, mel.shape[1]), dtype=np.float32)
+            crops[k] = mel[o:o + self.T_crop]
+        return tuple(self.dataset[i]) + (crops,)
+
+
+def collate_cloning(batch, r=1, downsample_step=4, pin=False):
+    """batch: ``CloningSampleDataset`` items -> ``collate`` of the items without their cloning samples, plus
+    "speaker_mels" (B, N, T_crop, num_mels) float32, the samples stacked."""
+    out = collate([b[:-1] for b in batch], r, downsample_step, pin)
+    mels = torch.from_numpy(np.stack([b[-1] for b in batch]))
+    out["speaker_mels"] = mels.pin_memory() if pin else mels
+    return out
 
 
 class SpeakerSampleBatches:

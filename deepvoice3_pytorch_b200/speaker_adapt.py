@@ -130,17 +130,27 @@ class _SpeakerResidualFn(torch.autograd.Function):
 
 
 class SpeakerAdapt:
-    """State of the adaptation passes of one TrainStep (see the module docstring)."""
+    """State of the adaptation passes of one TrainStep (see the module docstring).
 
-    def __init__(self, model, ids):
+    ids: the table rows being adapted; their gradient goes to a ``RowsArena`` over them.  Or, with ids None, the anchor
+    of each pass is a speaker encoder's output, which the model takes as ``speaker_embed`` (the encoder-only step of
+    DESIGN.md section 2.16): ``arena`` is then the encoder's ``ParameterArena``, and ``run`` hands the per-row gradient
+    to the encoder's backward."""
+
+    def __init__(self, model, ids=None, arena=None):
         self.model = model
-        self.ids = list(ids)
-        self.lo, self.n = self.ids[0], len(self.ids)
         self.S = model.speaker_embed_dim
-        self.arena = RowsArena(model.embed_speakers.weight, self.lo, self.n)
+        if ids is not None:
+            self.ids = list(ids)
+            self.lo, self.n = self.ids[0], len(self.ids)
+            self.arena = RowsArena(model.embed_speakers.weight, self.lo, self.n)
+            self.table = model.embed_speakers.weight    # the Parameter whose storage the Adam leaf views
+        else:
+            self.ids = self.table = None
+            self.arena = arena
         self.frozen = ops.FrozenWeights()
         self.splits = int(lib.raw("dv3_spk_grad_splits")())
-        self.table = model.embed_speakers.weight        # the Parameter whose storage the Adam leaf views
+        self._rows = {}                                 # B -> arange(B): every row its own id (encoder anchor)
         self._reset()
 
     def _reset(self):
@@ -155,10 +165,11 @@ class SpeakerAdapt:
         return self._partials
 
     # -- per pass --------------------------------------------------------------------------------------
-    def run(self, batch, inner):
+    def run(self, batch, inner, spk=None):
         """Forward + loss + backward (``inner(batch)``) with every parameter frozen, then the adapted rows' gradient
-        into ``arena.grad``.  -> the loss."""
-        ids = batch.get("speaker_ids")
+        into ``arena.grad``.  spk: the encoder's output e (B, S), with its autograd graph, that ``inner`` passes to the
+        model as speaker_embed; the per-row gradient d(loss)/de (the position-rate part included) then runs
+        ``spk.backward``.  -> the loss."""
         params = list(self.model.parameters())
         flags = [p.requires_grad for p in params]
         prev = ops.speaker_adapt, ops.frozen_weights
@@ -172,8 +183,14 @@ class SpeakerAdapt:
             d_e = torch.empty(B, self.S, device=e.device)
             lib.call("dv3_spk_grad_reduce", _p(self.partials(B)), self.nsites * self.splits, _p(d_e), B, self.S,
                      _stream())
-            lib.call("dv3_spk_rows_grad", _p(d_e), _p(e.grad), _p(ids), self.lo, self.n, _p(self.arena.grad),
+            if spk is None:
+                ids, lo, n, out = batch.get("speaker_ids"), self.lo, self.n, self.arena.grad
+            else:                   # ids = arange(B): each row's own gradient
+                ids, lo, n, out = self.rows(B, e.device), 0, B, torch.empty(B, self.S, device=e.device)
+            lib.call("dv3_spk_rows_grad", _p(d_e), _p(e.grad), _p(ids), lo, n, _p(out),
                      _p(ops._err_flag(e.device)), B, self.S, _stream())
+            if spk is not None:
+                spk.backward(out)
             return loss
         finally:
             ops.speaker_adapt, ops.frozen_weights = prev
@@ -181,12 +198,22 @@ class SpeakerAdapt:
                 p.requires_grad_(f)
             self._reset()
 
+    def rows(self, B, device):
+        """A cached int64 arange(B) on the device (no allocation per pass: graph-capture safe)."""
+        if B not in self._rows:
+            self._rows[B] = torch.arange(B, device=device)
+        return self._rows[B]
+
     # -- hooks called by the model (through ops.speaker_adapt) ----------------------------------------------
     def embed(self, table, speaker_ids):
         """The lookup (range-checked on the device), as the one tensor of the pass that takes a gradient."""
         with torch.no_grad():
             e = table(speaker_ids)
-        e.requires_grad_(True)
+        return self.anchor_of(e)
+
+    def anchor_of(self, e):
+        """e (B, S) cut from its autograd graph, as the one tensor of the pass that takes a gradient."""
+        e = e.detach().requires_grad_(True)
         self.anchor = e
         return e
 

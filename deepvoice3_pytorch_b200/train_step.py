@@ -303,7 +303,8 @@ def gradient_buckets(model, arena):
 
 def arena_parts(model, arena):
     """[lo, hi) arena ranges of ``model.seq2seq``'s and ``model.postnet``'s parameters, plus whatever lies between or
-    after them (the speaker embedding) as parts of their own: the units that keep their own Adam step count."""
+    after them (the speaker embedding, or a speaker encoder's parameters) as parts of their own: the units that keep
+    their own Adam step count."""
     cuts = sorted(r for r in (arena.range_of(list(getattr(model, name).parameters()))
                               for name in ("seq2seq", "postnet") if hasattr(model, name)) if r)
     parts, pos = [], 0
@@ -466,6 +467,22 @@ class FlatAdam:
         self.part_t = [s.pop() if s else 0 for s in steps]
 
 
+def check_speaker_encoder(model, encoder, train_seq2seq, train_postnet, adapt_speakers):
+    """ValueError for a speaker encoder that ``TrainStep`` cannot fine-tune with ``model`` (before any launch)."""
+    if getattr(model, "n_speakers", 1) <= 1 or not hasattr(model, "embed_speakers"):
+        raise ValueError("speaker_encoder needs a multi-speaker model (n_speakers=%d)" % getattr(model, "n_speakers", 1))
+    if encoder.speaker_embed_dim != model.speaker_embed_dim or encoder.mel_dim != model.mel_dim:
+        raise ValueError("encoder speaker_embed_dim=%d mel_dim=%d, model %d and %d" % (
+            encoder.speaker_embed_dim, encoder.mel_dim, model.speaker_embed_dim, model.mel_dim))
+    if not (train_seq2seq and train_postnet):
+        raise ValueError("speaker_encoder trains through the joint forward: train_seq2seq and train_postnet must both "
+                         "be True")
+    if adapt_speakers is not None:
+        raise ValueError("adapt_speakers and speaker_encoder are two ways to train speaker embeddings: pass one")
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError("speaker_encoder training runs in a single process (world size %d)" % dist.get_world_size())
+
+
 def check_train_mode(model, train_seq2seq, train_postnet):
     """ValueError for a training mode the reference would assert on or crash in later (train.py:615, 690, 699)."""
     if not (train_seq2seq or train_postnet):
@@ -505,15 +522,33 @@ class TrainStep:
     frozen weights afterwards is detected from their version counters at the next ``step()``, which refolds them in
     place (``load_state_dict`` refolds too).  A batch row of a speaker not being adapted changes no parameter and sets
     the device error flag that ``ops.check_index_errors()`` raises on (no host sync inside the step).  Single process
-    only; train_seq2seq / train_postnet must both be True.  ValueError otherwise, before any launch."""
+    only; train_seq2seq / train_postnet must both be True.  ValueError otherwise, before any launch.
+
+    speaker_encoder: fine-tune a ``speaker_encoder.SpeakerEncoder`` through the training loss (DESIGN.md section 2.16).
+    Each batch row's speaker embedding is the encoder's output on the row's cloning samples, batch["speaker_mels"]
+    (B, N, T_crop, mel_dim) fp32 (``data.CloningSampleDataset`` + ``collate_cloning``), one shape for the life of the
+    step; batch["speaker_ids"] is not read.  The encoder runs before the model, outside its extent scope.
+    train_model=True: the joint step -- every trainable model parameter but the speaker table, and every encoder
+    parameter (an Adam part of its own), in one arena; one ``loss.backward()`` reaches the encoder through the model's
+    speaker sites.  The table is not read, takes no gradient, has no Adam state and keeps its bits.
+    train_model=False: the encoder-only step -- every model parameter and buffer keeps its bits; the model runs the
+    adaptation passes (frozen folded weights, collapsed site gradients) with the encoder's output as the anchor, and
+    the per-row gradient of that anchor drives the encoder's backward; Adam runs over the encoder's parameters.  The
+    encoder's parameters are moved into the step's arena, so a ``SpeakerEncoderStep`` built earlier no longer trains
+    them.  Single process only; train_seq2seq / train_postnet must both be True, and adapt_speakers None.  ValueError
+    otherwise, or for a single-speaker model or an encoder of another speaker_embed_dim / mel_dim, before any launch."""
 
     def __init__(self, model, init_lr=5e-4, betas=(0.5, 0.9), eps=1e-6, clip_thresh=0.1, r=1, downsample_step=4,
                  masked_loss_weight=0.5, binary_divergence_weight=0.1, guided_attention_sigma=0.2,
                  use_guided_attention=True, priority_freq=3000, priority_freq_weight=0.0, sample_rate=22050,
                  lr_schedule=noam_learning_rate_decay, use_graph=False, fused_loss=True, weight_bank=None,
                  train_seq2seq=True, train_postnet=True, weight_decay=0.0, amsgrad=False, deterministic=None,
-                 adapt_speakers=None):
+                 adapt_speakers=None, speaker_encoder=None, train_model=True):
         self.adapt = None
+        self.encoder, self.train_model = speaker_encoder, bool(train_model)
+        self._spk_shape = None
+        if speaker_encoder is not None:
+            check_speaker_encoder(model, speaker_encoder, train_seq2seq, train_postnet, adapt_speakers)
         if adapt_speakers is not None:
             ids = check_adapt_speakers(model, adapt_speakers)
             if not (train_seq2seq and train_postnet):
@@ -534,6 +569,24 @@ class TrainStep:
             self.adapt = SpeakerAdapt(model, ids)
             self.arena = self.adapt.arena
             self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad)
+        elif speaker_encoder is not None:
+            # optimizer indices: the model's trainable list as the reference numbers it, then the encoder's parameters
+            # (state_dict() files the latter under "speaker_encoder")
+            trainable = list(model.get_trainable_parameters())
+            enc = list(speaker_encoder.parameters())
+            self._n_model = len(trainable)
+            enc_index = [self._n_model + j for j in range(len(enc))]
+            if self.train_model:
+                table = model.embed_speakers.weight
+                index = [i for i, p in enumerate(trainable) if p is not table]
+                self.arena = ParameterArena(model, [trainable[i] for i in index] + enc)
+                self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad,
+                                    arena_parts(model, self.arena), index + enc_index, self._n_model + len(enc))
+            else:
+                self.adapt = SpeakerAdapt(model, arena=ParameterArena(speaker_encoder, enc))
+                self.arena = self.adapt.arena
+                self.opt = FlatAdam(self.arena, init_lr, betas, eps, clip_thresh, weight_decay, amsgrad,
+                                    index=enc_index, n_index=self._n_model + len(enc))
         else:
             trainable = list(model.get_trainable_parameters())
             own = {id(p) for p in self.trained.parameters()}
@@ -582,7 +635,14 @@ class TrainStep:
     def state_dict(self, global_epoch=0):
         """The reference's checkpoint: in a partial mode the trained part's state_dict (model.seq2seq or
         model.postnet), with optimizer state for its parameters only.  Speaker adaptation: the whole model's
-        state_dict, the Adam state of the adapted rows' leaf and the ids under "adapted_speakers"."""
+        state_dict, the Adam state of the adapted rows' leaf and the ids under "adapted_speakers".  With a speaker
+        encoder: the whole model's state_dict and its Adam state in the reference's index layout (none in the
+        encoder-only mode), plus "speaker_encoder" (the encoder's state_dict and its own Adam state) and "train_model"."""
+        if self.encoder is not None:
+            model_opt, enc_opt = self._split_optimizer(self.opt.state_dict())
+            return {"state_dict": self.model.state_dict(), "optimizer": model_opt, "global_step": self.global_step,
+                    "global_epoch": global_epoch, "train_model": self.train_model,
+                    "speaker_encoder": {"state_dict": self.encoder.state_dict(), "optimizer": enc_opt}}
         if self.adapt is not None:
             return {"state_dict": self.model.state_dict(), "optimizer": self.opt.state_dict(),
                     "adapted_speakers": list(self.adapt.ids), "global_step": self.global_step,
@@ -594,6 +654,8 @@ class TrainStep:
         """Resume from ``state_dict()`` or from a reference checkpoint (same keys), of the whole model or of
         model.seq2seq / model.postnet alone, in any mode.  Restores the Adam moments, the bias-correction steps (parts
         without optimizer state start at step 0) and the position in the learning-rate schedule."""
+        if self.encoder is not None:
+            return self._load_encoder(ckpt, load_optimizer)
         if self.adapt is not None:
             return self._load_adapt(ckpt, load_optimizer)
         sd = ckpt["state_dict"]
@@ -603,12 +665,50 @@ class TrainStep:
                 target = part
         target.load_state_dict(sd)      # copies into the arena views in place
         if load_optimizer and ckpt.get("optimizer") is not None:
-            split = self.opt.split_update()
-            self.opt.load_state_dict(ckpt["optimizer"])
-            if self.opt.split_update() != split:       # captured graphs hold the other update plan: capture anew
-                self._graph = self._static = self._loss = self._graph_key = self._pool = None
-                self._buckets = {}
-                self.launches_per_step = None
+            self._load_optimizer(ckpt["optimizer"])
+        self.global_step = int(ckpt.get("global_step", 0))
+        return int(ckpt.get("global_epoch", 0))
+
+    def _load_optimizer(self, sd):
+        split = self.opt.split_update()
+        self.opt.load_state_dict(sd)
+        if self.opt.split_update() != split:       # captured graphs hold the other update plan: capture anew
+            self._graph = self._static = self._loss = self._graph_key = self._pool = None
+            self._buckets = {}
+            self.launches_per_step = None
+
+    def _split_optimizer(self, sd):
+        """FlatAdam state over [model's trainable list, encoder parameters] -> (the model's part in the reference's
+        layout, the encoder's part indexed from 0)."""
+        n, group = self._n_model, sd["param_groups"][0]
+        n_enc = len(group["params"]) - n
+        model = {"state": {i: s for i, s in sd["state"].items() if i < n},
+                 "param_groups": [dict(group, params=list(range(n)))]}
+        enc = {"state": {i - n: s for i, s in sd["state"].items() if i >= n},
+               "param_groups": [dict(group, params=list(range(n_enc)))]}
+        return model, enc
+
+    def _load_encoder(self, ckpt, load_optimizer):
+        """A checkpoint of either encoder mode, or a reference checkpoint of the model alone (the encoder then keeps
+        its weights and its Adam part starts at step 0)."""
+        self.model.load_state_dict(ckpt["state_dict"])      # in place: arena views and folded buffers stay
+        enc = ckpt.get("speaker_encoder") or {}
+        if enc.get("state_dict") is not None:
+            self.encoder.load_state_dict(enc["state_dict"])
+        if self.adapt is not None:
+            self.adapt.frozen.refresh()                     # outside every graph: same buffers, new values
+        if load_optimizer and ckpt.get("optimizer") is not None:
+            model_opt, n_enc = ckpt["optimizer"], len(list(self.encoder.parameters()))
+            enc_opt = enc.get("optimizer") or {"state": {}, "param_groups": [{"params": list(range(n_enc))}]}
+            ids = [i for g in model_opt["param_groups"] for i in g["params"]]
+            eids = [i for g in enc_opt["param_groups"] for i in g["params"]]
+            if len(ids) != self._n_model or len(eids) != n_enc:
+                raise ValueError("optimizer state has %d model and %d encoder parameters, this step %d and %d"
+                                 % (len(ids), len(eids), self._n_model, n_enc))
+            state = {j: model_opt["state"][i] for j, i in enumerate(ids) if i in model_opt["state"]}
+            state.update({self._n_model + j: enc_opt["state"][i] for j, i in enumerate(eids) if i in enc_opt["state"]})
+            group = dict(model_opt["param_groups"][0], params=list(range(self._n_model + n_enc)))
+            self._load_optimizer({"state": state, "param_groups": [group]})
         self.global_step = int(ckpt.get("global_step", 0))
         return int(ckpt.get("global_epoch", 0))
 
@@ -637,9 +737,12 @@ class TrainStep:
         try:
             if self.bank is not None:
                 self.bank.begin_step()
+            # the speaker encoder runs outside the model's extent scope (a bucket's extents would mask its stacks)
+            # and, in the encoder-only mode, before the frozen-weight cache is installed
+            spk = self.encoder(batch["speaker_mels"]) if self.encoder is not None else None
             if self.adapt is not None:
-                return self.adapt.run(batch, self._forward_backward_inner)
-            return self._forward_backward_inner(batch)
+                return self.adapt.run(batch, lambda b: self._forward_backward_inner(b, spk), spk)
+            return self._forward_backward_inner(batch, spk)
         finally:
             ops.deterministic, ops.det_scratch = det_outer
             ops.grad_sink = False
@@ -662,11 +765,11 @@ class TrainStep:
         with torch.cuda.stream(self._comm):
             self.arena.all_reduce_grads([rng])
 
-    def _forward_backward_inner(self, batch):
+    def _forward_backward_inner(self, batch, spk=None):
         ext = batch.get("extents")          # a batch padded to a bucket (data.pad_to_bucket)
         scope = ops.extent_scope(ext, data.batch_extents(batch)) if ext is not None else contextlib.nullcontext()
         with scope:
-            outs = self._forward(batch)
+            outs = self._forward(batch, spk)
             if self.loss_fn is fused_training_loss:
                 self._terms.zero_()
                 loss = self.loss_fn(outs, batch, terms=self._terms, **self.loss_kw)
@@ -677,9 +780,13 @@ class TrainStep:
             self.bank.end_backward()
         return loss.detach()
 
-    def _forward(self, batch):
-        """-> (mel, linear, attention, done) predictions; the parts this mode does not run are None."""
+    def _forward(self, batch, spk=None):
+        """-> (mel, linear, attention, done) predictions; the parts this mode does not run are None.  spk: the speaker
+        encoder's embeddings, used instead of batch["speaker_ids"]."""
         m = self.model
+        if spk is not None:
+            return m(batch["x"], batch["mel"], speaker_embed=spk, text_positions=batch["text_positions"],
+                     frame_positions=batch["frame_positions"], input_lengths=batch["input_lengths_dev"])
         if self.train_seq2seq and self.train_postnet:
             return m(batch["x"], batch["mel"], speaker_ids=batch.get("speaker_ids"),
                      text_positions=batch["text_positions"], frame_positions=batch["frame_positions"],
@@ -699,6 +806,22 @@ class TrainStep:
         if self.train_seq2seq:
             return batch
         return {k: (v[:, :0] if k in ("x", "text_positions") and torch.is_tensor(v) else v) for k, v in batch.items()}
+
+    def _check_speaker_mels(self, batch):
+        """ValueError before any launch for a missing or malformed batch["speaker_mels"], or one whose shape differs
+        from the first step's."""
+        m, enc = batch.get("speaker_mels"), self.encoder
+        x = batch["x"]
+        if not torch.is_tensor(m) or m.dim() != 4 or m.dtype != torch.float32 or m.device != x.device or \
+                m.shape[0] != x.shape[0] or not 1 <= m.shape[1] <= enc.max_samples or m.shape[2] < 1 or \
+                m.shape[3] != enc.mel_dim:
+            raise ValueError("batch['speaker_mels'] %s: expected (B=%d, N <= %d, T_crop, %d) float32 on %s" % (
+                "missing" if not torch.is_tensor(m) else "%s %s on %s" % (tuple(m.shape), m.dtype, m.device),
+                x.shape[0], enc.max_samples, enc.mel_dim, x.device))
+        if self._spk_shape is not None and tuple(m.shape) != self._spk_shape:
+            raise ValueError("batch['speaker_mels'] has one shape for the life of a TrainStep: %s, then %s"
+                             % (self._spk_shape, tuple(m.shape)))
+        self._spk_shape = tuple(m.shape)
 
     def loss_terms(self):
         """The per-term losses of the last step under the tags reference train.py logs (:761-776), for the terms this
@@ -750,7 +873,12 @@ class TrainStep:
         if ops.math_mode() != self.math:
             raise ValueError("TrainStep was built with ops.conv_math = %r and cannot step under %r: its weight bank and "
                              "CUDA graphs hold that mode's kernels (build a new TrainStep)" % (self.math, ops.conv_math))
-        if self.adapt is not None:
+        if self.encoder is not None:
+            self._check_speaker_mels(batch)
+            self.encoder.train()
+            if self.adapt is not None and self.adapt.frozen.stale():
+                self.adapt.frozen.refresh()
+        elif self.adapt is not None:
             if batch.get("speaker_ids") is None:
                 raise ValueError("speaker adaptation needs batch['speaker_ids']")
             if self.model.embed_speakers.weight is not self.adapt.table:

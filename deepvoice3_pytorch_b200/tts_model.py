@@ -107,7 +107,16 @@ class MultiSpeakerTTSModel(nn.Module):
         return None
 
     # -- forward ------------------------------------------------------------------------------------------
-    def _speaker_embedding(self, speaker_ids):
+    def _speaker_embedding(self, speaker_ids, speaker_embed=None):
+        if speaker_embed is not None:
+            if speaker_ids is not None:
+                raise ValueError("pass speaker_ids or speaker_embed, not both")
+            if self.n_speakers <= 1 or speaker_embed.dim() != 2 or speaker_embed.shape[1] != self.speaker_embed_dim:
+                raise ValueError("speaker_embed of shape %s: expected (B, %d) on a multi-speaker model (n_speakers=%d)"
+                                 % (tuple(speaker_embed.shape), self.speaker_embed_dim, self.n_speakers))
+            if ops.speaker_adapt is not None:        # frozen model: e is the one tensor with a gradient
+                return ops.speaker_adapt.anchor_of(speaker_embed)
+            return speaker_embed
         if speaker_ids is None:
             return None
         assert self.n_speakers > 1
@@ -116,15 +125,16 @@ class MultiSpeakerTTSModel(nn.Module):
         return self.embed_speakers(speaker_ids)
 
     def forward(self, text_sequences, mel_targets=None, speaker_ids=None, text_positions=None,
-                frame_positions=None, input_lengths=None):
+                frame_positions=None, input_lengths=None, speaker_embed=None):
         """-> mel_outputs (B, T, mel_dim), linear_outputs (B, T*ds, linear_dim), alignments (N, B, T_dec, T_text),
-        done (B, T_dec, 1)."""
+        done (B, T_dec, 1).  speaker_embed (B, speaker_embed_dim): the speakers' embeddings themselves, used instead of
+        looking ``speaker_ids`` up in the table (e.g. a speaker encoder's output, which then takes the gradient)."""
         # dropout: call-site salts restart and (in training) a new step seed is drawn with every forward, so
         # model(...) / loss.backward() / optimizer.step() loops get fresh masks without any TrainStep
         ops.rng.begin_forward(self.training, text_sequences.device)
         try:
             batch = text_sequences.size(0)
-            spk = self._speaker_embedding(speaker_ids)
+            spk = self._speaker_embedding(speaker_ids, speaker_embed)
             mel, alignments, done, states = self.seq2seq(text_sequences, mel_targets, spk, text_positions,
                                                          frame_positions, input_lengths)
             mel = mel.reshape(batch, -1, self.mel_dim)    # un-group the r frames per decoder step
