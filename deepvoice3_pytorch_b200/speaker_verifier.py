@@ -268,9 +268,9 @@ def cloned_voice_mels(model, mel_dim, speaker_ids, sequences, vocoder, batch_siz
     """What the cloned-voice evaluations (``verify_cloned_voices``, ``speaker_classifier.classify_cloned_voices``)
     share.  First the checks, ValueError before any launch: a single-speaker model, an unknown phase method,
     mismatched list lengths, speaker ids outside [0, n_speakers), an evaluation network of ``mel_dim`` mel channels
-    where the audio path makes another count, malformed sequences.  Then every ``sequences[k]`` synthesized in the voice
-    ``speaker_ids[k]`` with ``synthesis.tts_batch`` (stage "synthesis") and turned into normalised mels on ``device``
-    with ``audio.stft_mel_batch`` (stage "mel") -> (speaker ids as ints, list of (T_k, num_mels) mels)."""
+    where the audio path makes another count, malformed sequences.  Then ``synthesis.synthesized_mels``: every
+    ``sequences[k]`` synthesized in the voice ``speaker_ids[k]`` (stage "synthesis") and turned into normalised mels on
+    ``device`` (stage "mel") -> (speaker ids as ints, list of (T_k, num_mels) mels)."""
     from . import synthesis
     _check_model(model)
     audio.check_phase_method(vocoder)
@@ -283,19 +283,8 @@ def cloned_voice_mels(model, mel_dim, speaker_ids, sequences, vocoder, batch_siz
     if mel_dim != audio.hparams.num_mels:
         raise ValueError("the evaluation network takes %d mel channels, the audio path makes %d"
                          % (mel_dim, audio.hparams.num_mels))
-    synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
-    with stage("synthesis"):
-        wavs = [w for w, _, _, _ in synthesis.tts_batch(model, sequences, speaker_ids, batch_size=batch_size,
-                                                        vocoder=vocoder)]
-    with stage("mel"):
-        lens = [len(w) for w in wavs]
-        pad = np.zeros((len(wavs), max(lens)), np.float32)
-        for k, w in enumerate(wavs):
-            pad[k, :lens[k]] = w
-        _, mel = audio.stft_mel_batch(torch.from_numpy(pad).to(device), torch.tensor(lens, dtype=torch.int32),
-                                      want_linear=False)
-        return speaker_ids, [mel[k, :audio.num_frames(n)] for k, n in enumerate(lens)]
+    return speaker_ids, synthesis.synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, device,
+                                                   stage_timer)
 
 
 def verify_cloned_voices(model, verifier, speaker_ids, enrollment, sequences, vocoder="griffin_lim", batch_size=16,

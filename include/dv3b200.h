@@ -656,6 +656,22 @@ int dv3_spkcls_bwd(const float* h, long long ld, const float* w, const float* lo
                    const long long* labels, const float* d_logits, const float* d_loss, float loss_scale, float* d_h,
                    float* d_w, float* d_bias, int* err_flag, int R, int C, int K, void* stream);
 
+/* ---- mel-cepstral distortion after dynamic time warping (mcd.cu) ----
+ * dv3_mel_cepstra: cep[(q*T_max + t)*K + k] = sum_m basis[k*M + m] mels[(q*T_max + t)*M + m] (m in order) for the
+ * n_seq sequences of lengths[q] (int32) frames each; basis (K, M) is the orthonormal DCT-II rows 1..K times
+ * -min_level_db ln10 / 20 (mcd.py).  Frames t >= lengths[q] are not read and give zeros.  2 <= M <= 128,
+ * 1 <= K <= min(M - 1, 64), T_max <= dv3_mcd_max_frames().
+ * dv3_dtw_mcd: for each row (pair, a_row, N, b_row, M, ws_off) of the int64 work list (P, 6), the DTW of the N cepstra
+ * starting at row a_row of cep (K floats a row) against the M starting at b_row: cost[pair] = D(N, M) and
+ * path_len[pair] = L (DESIGN.md section 2.17; ties to the diagonal, then (i-1, j), then (i, j-1)).  workspace: per row
+ * 2 * roundup(M, 32) floats at ws_off (a multiple of 32).  One warp per row, launched in list order.  A pair's result
+ * depends on its own cepstra alone.  No atomics. */
+int dv3_mcd_max_frames(void);
+int dv3_mel_cepstra(const float* mels, const int* lengths, const float* basis, float* cep, int n_seq, int T_max, int M,
+                    int K, void* stream);
+int dv3_dtw_mcd(const float* cep, int K, const long long* work, float* workspace, float* cost, int* path_len, int P,
+                void* stream);
+
 #ifdef __cplusplus
 }
 #endif
