@@ -9,14 +9,16 @@ recording of the same text, in dB (DESIGN.md section 2.17).
 * Frame distance d(i, j) = ||c^a_i - c^b_j||_2, the squares summed over k in index order.
 * DTW: D(0,0) = 0, D(i,0) = D(0,j) = +inf, D(i,j) = d(i,j) + min(D(i-1,j-1), D(i-1,j), D(i,j-1)); ties go to the
   diagonal, then to (i-1, j), then to (i, j-1).  The path length L (cells on the chosen path) rides along with the
-  chosen predecessor: no N x M matrix, no backtrace.
+  chosen predecessor: no N x M matrix, no backtrace.  ``dtw_path`` runs the same recursion and also keeps each cell's
+  predecessor in 2 bits, then backtraces the warping path (DESIGN.md section 2.18).
 * mcd = (10 sqrt(2) / ln10) D(N, M) / L, in dB, formed on the host in fp64.
 
 This is the MFCC-style mel cepstrum of this project's filterbank, not SPTK's ``mcep`` of a WORLD envelope: numbers are
 comparable between runs of this project, and parity with the SPTK-based MCD tools is unpinned.
 
-``mel_cepstra`` and ``dtw`` run the kernels of csrc/mcd.cu; ``mcd_dtw`` compares two ragged lists of mels;
-``evaluate_synthesis`` synthesizes, makes mels of the synthesized and the reference audio, and scores them.
+``mel_cepstra`` and ``dtw`` run the kernels of csrc/mcd.cu, ``dtw_path`` those of csrc/pitch.cu; ``mcd_dtw`` compares
+two ragged lists of mels; ``evaluate_synthesis`` synthesizes, makes mels of the synthesized and the reference audio, and
+scores them.
 """
 import contextlib
 import ctypes
@@ -32,6 +34,7 @@ MAX_FRAMES = 16384            # frames per sequence (csrc/mcd.cu MC_MAX_FRAMES):
 MAX_MELS = 128                # the filterbank's limit (audio.check_geometry)
 MAX_CEPS = 64                 # the DTW kernel holds a frame's cepstrum in registers
 MCD_SCALE = 10.0 * math.sqrt(2.0) / math.log(10.0)
+DIR_BUDGET_BYTES = 1 << 30    # dtw_path: direction words of one launch (a 16 384 x 16 384 pair needs 64 MiB)
 
 _basis_cache = {}
 
@@ -169,12 +172,9 @@ def _result(cost, path):
     return {"mcd": MCD_SCALE * cost / L, "cost": cost, "path_length": L}
 
 
-def dtw(ceps_a, ceps_b):
-    """Two lists of (T, K) fp32 CUDA cepstra (or any feature rows, 1 <= K <= 64), paired by index ->
-    {"mcd": fp64 (P,), "cost": D(N, M) fp64 (P,), "path_length": L int64 (P,)}: the DTW of the module docstring, one
-    warp per pair, longest pairs first.  A pair's result does not depend on the rest of the batch (bit for bit).
-    ValueError before any launch for empty or unequal lists, sequences of 0 or more than ``MAX_FRAMES`` frames, mixed
-    widths or K outside [1, 64], tensors that are not fp32 CUDA."""
+def _feature_pairs(ceps_a, ceps_b):
+    """The checks of ``dtw`` and ``dtw_path`` (host values only), then both sides' rows in one contiguous tensor ->
+    (flat (rows, K), K, first row of each sequence, lengths, P); sequences a_0 .. a_{P-1}, then b_0 .. b_{P-1}."""
     _check_pairs(ceps_a, ceps_b)
     K = _check_frames(list(ceps_a) + list(ceps_b), "cepstra")
     if not 1 <= K <= MAX_CEPS:
@@ -183,8 +183,91 @@ def dtw(ceps_a, ceps_b):
     lens = [int(c.shape[0]) for c in seqs]
     rows = np.concatenate([[0], np.cumsum(lens)[:-1]]).tolist()
     flat = torch.cat([c.contiguous() for c in seqs]).contiguous()
-    P = len(ceps_a)
+    return flat, K, rows, lens, len(ceps_a)
+
+
+def dtw(ceps_a, ceps_b):
+    """Two lists of (T, K) fp32 CUDA cepstra (or any feature rows, 1 <= K <= 64), paired by index ->
+    {"mcd": fp64 (P,), "cost": D(N, M) fp64 (P,), "path_length": L int64 (P,)}: the DTW of the module docstring, one
+    warp per pair, longest pairs first.  A pair's result does not depend on the rest of the batch (bit for bit).
+    ValueError before any launch for empty or unequal lists, sequences of 0 or more than ``MAX_FRAMES`` frames, mixed
+    widths or K outside [1, 64], tensors that are not fp32 CUDA."""
+    flat, K, rows, lens, P = _feature_pairs(ceps_a, ceps_b)
     return _result(*_dtw_rows(flat, K, rows[:P], lens[:P], rows[P:], lens[P:]))
+
+
+def _dir_words(N, M):
+    """Direction words of one pair's warping path: N rows of ceil(M / 16) 32-bit words."""
+    return N * (-(-M // 16))
+
+
+def _path_chunks(work, budget=None):
+    """Split the work rows (in list order) into runs [r0, r1) whose direction buffers, 4 bytes a word, total at most
+    ``budget`` bytes (``DIR_BUDGET_BYTES``); a run always takes at least one row.  -> list of (r0, r1)."""
+    budget = DIR_BUDGET_BYTES if budget is None else budget
+    chunks, r0, used = [], 0, 0
+    for r in range(work.shape[0]):
+        b = 4 * _dir_words(int(work[r, 2]), int(work[r, 4]))
+        if r > r0 and used + b > budget:
+            chunks.append((r0, r))
+            r0, used = r, 0
+        used += b
+    chunks.append((r0, work.shape[0]))
+    return chunks
+
+
+def _dtw_path_rows(cep, K, a_rows, a_lens, b_rows, b_lens):
+    """``_dtw_rows`` that also returns the warping paths: per budget chunk of the work list one ``dv3_dtw_path`` and one
+    ``dv3_dtw_backtrace`` launch, reusing one direction buffer.  -> (cost fp32 (P,), L int32 (P,), list of (rows_p, 2)
+    int64 host arrays; rows_p = L_p wherever the cost is finite)."""
+    work, ws_floats = _work_list(a_rows, a_lens, b_rows, b_lens)
+    dev = cep.device
+    P = len(a_lens)
+    chunks = _path_chunks(work)
+    path_work = np.zeros((P, 2), np.int64)
+    slot = np.zeros(P, np.int64)                    # pair -> first path row of its slot
+    rows = 0
+    for r0, r1 in chunks:
+        words = 0
+        for r in range(r0, r1):
+            N, M = int(work[r, 2]), int(work[r, 4])
+            path_work[r] = (words, rows)
+            slot[work[r, 0]] = rows
+            words += _dir_words(N, M)
+            rows += N + M - 1
+    dir_words = max(sum(_dir_words(int(work[r, 2]), int(work[r, 4])) for r in range(r0, r1)) for r0, r1 in chunks)
+    work_d = torch.from_numpy(work).to(dev)
+    path_work_d = torch.from_numpy(path_work).to(dev)
+    ws = torch.empty(ws_floats, device=dev)
+    dirs = torch.empty(dir_words, dtype=torch.int32, device=dev)
+    cost = torch.empty(P, device=dev)
+    length = torch.empty(P, dtype=torch.int32, device=dev)
+    path = torch.empty(rows, 2, dtype=torch.int32, device=dev)
+    path_rows = torch.empty(P, dtype=torch.int32, device=dev)
+    for r0, r1 in chunks:
+        w = ctypes.c_void_p(work_d.data_ptr() + 48 * r0)
+        pw = ctypes.c_void_p(path_work_d.data_ptr() + 16 * r0)
+        lib.call("dv3_dtw_path", _p(cep), K, w, pw, _p(ws), _p(dirs), _p(cost), _p(length), r1 - r0, _stream())
+        lib.call("dv3_dtw_backtrace", w, pw, _p(dirs), _p(path), _p(path_rows), r1 - r0, _stream())
+    n = path_rows.cpu().numpy()
+    path = path.cpu().numpy().astype(np.int64)
+    paths = [np.ascontiguousarray(path[slot[p]:slot[p] + n[p]][::-1]) for p in range(P)]
+    return cost, length, paths
+
+
+def dtw_path(ceps_a, ceps_b):
+    """``dtw`` that also returns the warping paths: -> {"mcd", "cost", "path_length"} bit for bit as ``dtw`` gives them
+    (the same recursion), plus "path": list of (L_p, 2) int64 arrays of 0-based frame pairs (i, j), from (0, 0) to
+    (N - 1, M - 1), monotone with unit steps, the cells the tie rule chose.  Each cell's predecessor is kept as 2 bits,
+    so a pair needs N ceil(M / 16) 4-byte words of device memory (64 MiB at 16 384 x 16 384); the work list is split into
+    launches whose direction buffers stay within ``DIR_BUDGET_BYTES``.  Where the cost is not finite (NaN or overflowing
+    features), the path is still monotone, in the grid and from corner to corner, but its length need not equal
+    "path_length".  ValueError before any launch as ``dtw``."""
+    flat, K, rows, lens, P = _feature_pairs(ceps_a, ceps_b)
+    cost, length, paths = _dtw_path_rows(flat, K, rows[:P], lens[:P], rows[P:], lens[P:])
+    res = _result(cost, length)
+    res["path"] = paths
+    return res
 
 
 def mcd_dtw(mels_a, mels_b, n_ceps=24):
@@ -202,24 +285,9 @@ def mcd_dtw(mels_a, mels_b, n_ceps=24):
     return _result(*_dtw_rows(cep.view(-1, K), K, rows[:P], lengths[:P], rows[P:], lengths[P:]))
 
 
-def evaluate_synthesis(model, sequences, reference_wavs, speaker_ids=None, vocoder="griffin_lim", batch_size=16,
-                       n_ceps=24, stage_timer=None):
-    """MCD-DTW of synthesized speech against recordings of the same text, in one call:
-
-    1. synthesize every ``sequences[k]`` (in voice ``speaker_ids[k]`` for a multi-speaker model) with
-       ``synthesis.tts_batch``;
-    2. turn the synthesized and the reference waveforms into normalised mels with ``audio.stft_mel_batch``, on the GPU,
-       at the same STFT frame;
-    3. ``mcd_dtw`` of each synthesized utterance against its reference;
-    4. -> {"mcd": fp64 (n,), "path_length": int64 (n,), "frames": int64 (n, 2) (synthesized, reference),
-       "frame_ratio": fp64 (n,) synthesized / reference frames, "mean_mcd": float, "median_mcd": float}.
-
-    reference_wavs: fp32 numpy waveforms at ``hparams.sample_rate``.  Trimming silence is the caller's choice
-    (``audio.trim_bounds_batch``): leading and trailing silence in a reference raises its MCD, because the warping path
-    must still cover it.  A frame ratio far above 1 is the cheap sign of an attention failure that ran to
-    ``max_decoder_steps``.  stage_timer: optional ``name -> context manager`` around "synthesis", "mel" (entered for the
-    synthesized, then for the reference audio) and "mcd".  ValueError before any launch for an unknown phase method,
-    mismatched list lengths, malformed sequences or speaker ids (as ``tts_batch``), n_ceps outside
+def check_evaluation(model, sequences, reference_wavs, speaker_ids, vocoder, batch_size, n_ceps):
+    """The checks of ``evaluate_synthesis`` (host values only, nothing allocated or launched) -> K.  ValueError for an
+    unknown phase method, mismatched list lengths, malformed sequences or speaker ids (as ``tts_batch``), n_ceps outside
     [1, min(num_mels - 1, 64)], reference waveforms that are not non-empty 1-D fp32 arrays or give more than
     ``MAX_FRAMES`` frames."""
     audio.check_phase_method(vocoder)
@@ -242,6 +310,30 @@ def evaluate_synthesis(model, sequences, reference_wavs, speaker_ids=None, vocod
         if bad:
             raise ValueError("speaker ids %s outside [0, %d)" % (bad, model.n_speakers))
     synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
+    return K
+
+
+def evaluate_synthesis(model, sequences, reference_wavs, speaker_ids=None, vocoder="griffin_lim", batch_size=16,
+                       n_ceps=24, stage_timer=None):
+    """MCD-DTW of synthesized speech against recordings of the same text, in one call:
+
+    1. synthesize every ``sequences[k]`` (in voice ``speaker_ids[k]`` for a multi-speaker model) with
+       ``synthesis.tts_batch``;
+    2. turn the synthesized and the reference waveforms into normalised mels with ``audio.stft_mel_batch``, on the GPU,
+       at the same STFT frame;
+    3. ``mcd_dtw`` of each synthesized utterance against its reference;
+    4. -> {"mcd": fp64 (n,), "path_length": int64 (n,), "frames": int64 (n, 2) (synthesized, reference),
+       "frame_ratio": fp64 (n,) synthesized / reference frames, "mean_mcd": float, "median_mcd": float}.
+
+    reference_wavs: fp32 numpy waveforms at ``hparams.sample_rate``.  Trimming silence is the caller's choice
+    (``audio.trim_bounds_batch``): leading and trailing silence in a reference raises its MCD, because the warping path
+    must still cover it.  A frame ratio far above 1 is the cheap sign of an attention failure that ran to
+    ``max_decoder_steps``.  stage_timer: optional ``name -> context manager`` around "synthesis", "mel" (entered for the
+    synthesized, then for the reference audio) and "mcd".  ValueError before any launch for an unknown phase method,
+    mismatched list lengths, malformed sequences or speaker ids (as ``tts_batch``), n_ceps outside
+    [1, min(num_mels - 1, 64)], reference waveforms that are not non-empty 1-D fp32 arrays or give more than
+    ``MAX_FRAMES`` frames."""
+    K = check_evaluation(model, sequences, reference_wavs, speaker_ids, vocoder, batch_size, n_ceps)
     device = next(model.parameters()).device
     stage = stage_timer or (lambda name: contextlib.nullcontext())
     synth = synthesis.synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer)

@@ -146,28 +146,40 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
 def wav_mels(wavs, device):
     """fp32 host waveforms -> list of their (T_k, num_mels) normalised mels on ``device``: one padded batch through
     ``audio.stft_mel_batch``, each clip cut to its own ``audio.num_frames``."""
+    return wav_clips_and_mels(wavs, device)[1]
+
+
+def wav_clips_and_mels(wavs, device):
+    """``wav_mels`` that also returns the waveforms as they were copied to ``device``: -> (list of 1-D fp32 views of
+    the padded device batch, one per clip at its own length, list of mels)."""
     lens = [len(w) for w in wavs]
     pad = np.zeros((len(wavs), max(lens)), np.float32)
     for k, w in enumerate(wavs):
         pad[k, :lens[k]] = w
-    _, mel = audio.stft_mel_batch(torch.from_numpy(pad).to(device), torch.tensor(lens, dtype=torch.int32),
-                                  want_linear=False)
-    return [mel[k, :audio.num_frames(n)] for k, n in enumerate(lens)]
+    pad = torch.from_numpy(pad).to(device)
+    _, mel = audio.stft_mel_batch(pad, torch.tensor(lens, dtype=torch.int32), want_linear=False)
+    return [pad[k, :n] for k, n in enumerate(lens)], [mel[k, :audio.num_frames(n)] for k, n in enumerate(lens)]
 
 
-def synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer=None):
-    """What the evaluations of synthesized speech share (``mcd.evaluate_synthesis``, ``speaker_verifier``'s and
-    ``speaker_classifier``'s cloned-voice evaluations): every ``sequences[k]`` synthesized with ``tts_batch`` (in voice
-    ``speaker_ids[k]`` for a multi-speaker model, None for a single-speaker one; stage "synthesis") and turned into
-    normalised mels on ``device`` with ``wav_mels`` (stage "mel") -> list of (T_k, num_mels) mels.  ValueError before
-    any launch for an unknown phase method or malformed inputs (as ``tts_batch``)."""
+def synthesized_audio(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer=None):
+    """What the evaluations of synthesized speech share (``mcd.evaluate_synthesis``, ``pitch.evaluate_pitch``,
+    ``speaker_verifier``'s and ``speaker_classifier``'s cloned-voice evaluations): every ``sequences[k]`` synthesized
+    with ``tts_batch`` (in voice ``speaker_ids[k]`` for a multi-speaker model, None for a single-speaker one; stage
+    "synthesis") and turned into normalised mels on ``device`` with ``wav_clips_and_mels`` (stage "mel") -> (list of
+    the waveforms on ``device``, list of their (T_k, num_mels) mels).  ValueError before any launch for an unknown phase
+    method or malformed inputs (as ``tts_batch``)."""
     audio.check_phase_method(vocoder)
     _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
     with stage("synthesis"):
         wavs = [w for w, _, _, _ in tts_batch(model, sequences, speaker_ids, batch_size=batch_size, vocoder=vocoder)]
     with stage("mel"):
-        return wav_mels(wavs, device)
+        return wav_clips_and_mels(wavs, device)
+
+
+def synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer=None):
+    """``synthesized_audio`` without the waveforms -> list of (T_k, num_mels) mels."""
+    return synthesized_audio(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer)[1]
 
 
 def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stage_timer=None, stats=None,

@@ -672,6 +672,33 @@ int dv3_mel_cepstra(const float* mels, const int* lengths, const float* basis, f
 int dv3_dtw_mcd(const float* cep, int K, const long long* work, float* workspace, float* cost, int* path_len, int P,
                 void* stream);
 
+/* ---- pitch of synthesized speech: YIN F0 and the DTW warping path (pitch.cu) ----
+ * dv3_yin_frames_per_cta: the frames one CTA of dv3_yin_f0 handles at this tau_max (0 outside [1, 1024]).
+ * dv3_yin_f0: YIN F0 (DESIGN.md section 2.18) of frames of several clips in two launches.  blocks: int64 rows
+ * (sample_off, n_samples, out0, t0, nf), one per CTA: frames t0 .. t0 + nf - 1 (nf <= dv3_yin_frames_per_cta) of the clip
+ * of n_samples samples at wav + sample_off, written at rows out0 .. of f0, aperiodicity and energy.  Frame t reads
+ * samples t R + R - W/2 - floor((W + tau_max)/2) + m, m < W + tau_max, zero outside [0, n_samples).  f0 in Hz (0:
+ * unvoiced or below the gate), aperiodicity = d'(tau*), energy = sum of the W squared samples.  clips: int64 rows
+ * (out_off, n_frames), one per clip: the second launch sets f0 = 0 where energy < gate * the clip's largest energy.
+ * diff: null, or (rows, 2, tau_max) floats that receive d(tau) and d'(tau), tau = 1 .. tau_max, of every frame.
+ * 2 <= W <= 4096, 1 <= R <= W, 2 <= tau_min <= tau_max <= 1024, threshold in (0, 1], gate in [0, 1].  A clip's results
+ * depend on its own samples alone.  No atomics.
+ * dv3_dtw_path: dv3_dtw_mcd (the same work rows, workspace, cost and path_len, bit for bit) that also stores each cell's
+ * predecessor, 2 bits (0 diagonal, 1 (i-1, j), 2 (i, j-1)), 16 columns a word: row r's N * ceil(M/16) words start at
+ * dirs + path_work[2r] (path_work: int64 (P, 2)).
+ * dv3_dtw_backtrace: one thread per work row walks those words from (N, M) to (1, 1) and writes the cells of the path
+ * as 0-based int32 (i, j) pairs, last cell first, at path + 2 * path_work[2r + 1] (a slot of N + M - 1 pairs), and their
+ * count at path_rows[pair] (L for a finite cost).  On row 1 it moves left and on column 1 up, so the walk stays in the
+ * grid even where a non-finite D left codes that point outside it. */
+int dv3_yin_frames_per_cta(int tau_max);
+int dv3_yin_f0(const float* wav, const long long* blocks, int n_blocks, const long long* clips, int n_clips, float* f0,
+               float* aperiodicity, float* energy, float* diff, int W, int R, int tau_min, int tau_max, float threshold,
+               float gate, float sample_rate, void* stream);
+int dv3_dtw_path(const float* cep, int K, const long long* work, const long long* path_work, float* workspace,
+                 unsigned* dirs, float* cost, int* path_len, int P, void* stream);
+int dv3_dtw_backtrace(const long long* work, const long long* path_work, const unsigned* dirs, int* path, int* path_rows,
+                      int P, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
