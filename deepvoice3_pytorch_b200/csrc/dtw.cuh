@@ -36,6 +36,8 @@ static __device__ __forceinline__ void cp_async16(void* dst, const void* src) {
 static __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
 static __device__ __forceinline__ void cp_async_wait_1() { asm volatile("cp.async.wait_group 1;\n" ::: "memory"); }
 static __device__ __forceinline__ void cp_async_wait_0() { asm volatile("cp.async.wait_group 0;\n" ::: "memory"); }
+template <int N>
+static __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 
 // One warp per work row (pair, a_row, N, b_row, M, ws_off); ws holds per pair roundup(M, 32) boundary costs, then as
 // many path lengths (int bits), 32-float aligned.  KP: K rounded up to a multiple of 8.  PATH: path_work[2 * row] is

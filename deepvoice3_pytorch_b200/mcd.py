@@ -204,15 +204,20 @@ def _dir_words(N, M):
 def _path_chunks(work, budget=None):
     """Split the work rows (in list order) into runs [r0, r1) whose direction buffers, 4 bytes a word, total at most
     ``budget`` bytes (``DIR_BUDGET_BYTES``); a run always takes at least one row.  -> list of (r0, r1)."""
+    return budget_chunks([4 * _dir_words(int(w[2]), int(w[4])) for w in work], budget)
+
+
+def budget_chunks(sizes, budget=None):
+    """Split rows of ``sizes`` bytes each (in order) into runs [r0, r1) of at most ``budget`` bytes
+    (``DIR_BUDGET_BYTES``) in all; a run always takes at least one row.  -> list of (r0, r1)."""
     budget = DIR_BUDGET_BYTES if budget is None else budget
     chunks, r0, used = [], 0, 0
-    for r in range(work.shape[0]):
-        b = 4 * _dir_words(int(work[r, 2]), int(work[r, 4]))
+    for r, b in enumerate(sizes):
         if r > r0 and used + b > budget:
             chunks.append((r0, r))
             r0, used = r, 0
         used += b
-    chunks.append((r0, work.shape[0]))
+    chunks.append((r0, len(sizes)))
     return chunks
 
 

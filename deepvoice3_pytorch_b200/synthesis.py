@@ -63,6 +63,17 @@ def _check_inputs(model, sequences, speaker_ids, **counts):
 @torch.no_grad()
 def _synthesize_chunk(model, seqs, speaker_ids, stage, vocoder):
     """seqs: list of int64 arrays -> [(waveform, alignment, spectrogram, mel)] for one padded batch."""
+    outputs, aligns, states, steps, spk = _decode_chunk(model, seqs, speaker_ids, stage)
+    aligns = aligns.cpu().numpy()
+    post = _postnet_vocode(model, outputs, states, steps, spk, stage, vocoder)
+    return [(w, aligns[b, :steps[b], :s.size], lin, mel) for b, (s, (w, lin, mel)) in enumerate(zip(seqs, post))]
+
+
+@torch.no_grad()
+def _decode_chunk(model, seqs, speaker_ids, stage):
+    """The encoder and ``incremental.decode_ragged`` of ``tts_batch`` on one padded batch (stages "encoder" and
+    "decoder"): seqs: list of int64 arrays -> (outputs (B, N, in_dim*r), alignments (B, N, T_text) on the device,
+    decoder states (B, N, C), steps [B], speaker embeddings (B, D) or None)."""
     dev = next(model.parameters()).device
     B = len(seqs)
     lens = [s.size for s in seqs]
@@ -82,11 +93,9 @@ def _synthesize_chunk(model, seqs, speaker_ids, stage, vocoder):
             keys, values = model.seq2seq.encoder(text, speaker_embed=spk)
         with stage("decoder"):
             outputs, aligns, _, states, steps = incremental.decode_ragged(dec, (keys, values), tpos, text_len, spk)
-        aligns = aligns.cpu().numpy()
     finally:
         ops.rng.end_forward()
-    post = _postnet_vocode(model, outputs, states, steps, spk, stage, vocoder)
-    return [(w, aligns[b, :steps[b], :lens[b]], lin, mel) for b, (w, lin, mel) in enumerate(post)]
+    return outputs, aligns, states, steps, spk
 
 
 @torch.no_grad()

@@ -699,6 +699,31 @@ int dv3_dtw_path(const float* cep, int K, const long long* work, const long long
 int dv3_dtw_backtrace(const long long* work, const long long* path_work, const unsigned* dirs, int* path, int* path_rows,
                       int P, void* stream);
 
+/* ---- attention alignments: monotonic alignment search and per-step statistics (align.cu) ----
+ * Row b (b < B) is the alignment A[b*stride_b + t*stride_t + j] of steps[b] decoder steps t by tokens[b] tokens j (int32,
+ * 1 <= steps[b] <= N_max, 1 <= tokens[b] <= L_max); lp(t, j) = logf(fmaxf(A, 1e-8f)), so a NaN cell counts as the floor.
+ * dv3_mas_max_tokens: the largest L_max (1024).
+ * dv3_mas_dir_words: the 32-bit direction words of one row, steps * ceil(tokens / 32) (0 for arguments out of range).
+ * dv3_mas_forward: Q(0, 0) = lp(0, 0), Q(t, j) = lp(t, j) + max(Q(t-1, j), Q(t-1, j-1)), -inf at every cell off all paths
+ * from (0, 0) to (steps - 1, tokens - 1) (j > t or tokens - 1 - j > steps - 1 - t).  Tie rule: where
+ * Q(t-1, j) == Q(t-1, j-1) the path stays on token j.  Bit j % 32 of word dirs[dir_off[b] + t*ceil(tokens/32) + j/32] is 1
+ * where Q(t, j) is on a path and came from (t-1, j-1).  score[b] = Q(steps - 1, tokens - 1) (-inf when steps < tokens).
+ * In the same pass: argmax[b*N_max + t] = the lowest j < tokens with the largest A (NaN cells count as -inf), maxv[b*N_max
+ * + t] = that A, coverage[b*L_max + j] = sum_t A (t in increasing order); entries past a row's steps or tokens are not
+ * written.  One CTA of roundup(L_max, 32) threads per row, one barrier per step.  stride_t >= L_max; the alignment extent,
+ * B*N_max and B*L_max must stay below 2^31.
+ * dv3_mas_backtrace: durations[b*L_max + j] = the steps the path of row b spends on token j: >= 1 and summing to steps[b]
+ * for j < tokens[b] (also where non-finite cells left bits off the grid), 0 past tokens[b], and all 0 when steps[b] <
+ * tokens[b] (no path).  One warp per row.  Both kernels: a row's results depend on its own cells and lengths alone; no
+ * atomics. */
+int dv3_mas_max_tokens(void);
+long long dv3_mas_dir_words(int steps, int tokens);
+int dv3_mas_forward(const float* A, long long stride_b, long long stride_t, const int* steps, const int* tokens, int B,
+                    int N_max, int L_max, const long long* dir_off, unsigned* dirs, int* argmax, float* maxv,
+                    float* coverage, float* score, void* stream);
+int dv3_mas_backtrace(const int* steps, const int* tokens, int B, int L_max, const long long* dir_off,
+                      const unsigned* dirs, int* durations, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
