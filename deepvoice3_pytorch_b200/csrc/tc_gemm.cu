@@ -26,12 +26,14 @@
 // setmaxnreg budget per warpgroup:
 //   * warpgroup 2 = producer (24 registers): one thread issues the TMA loads of each K-iteration into the next stage of
 //     a STAGES-deep ring (full[s]: one arrival plus the stage's transaction bytes; empty[s]: one arrival per consumer
-//     warpgroup);
-//   * warpgroups 0 and 1 = consumers (176 registers): each accumulates 64 of the 128 tile rows in registers (wgmma),
+//     warpgroup).  Each configuration names its measured depth in tc_ring.cuh: 4 stages of 32 KB for the gated
+//     forward and the 128-column conv, 4 of 48 KB for the 64-column conv at BK = 64, 5 of 32 KB for the two-plane
+//     weight gradient, 6 for the smaller stages;
+//   * warpgroups 0 and 1 = consumers (168 registers): each accumulates 64 of the 128 tile rows in registers (wgmma),
 //     keeping one stage of MMAs in flight (wait_group 1, then release the previous stage), then writes
 //     main * gmain + cross * 2^-11 into a full-tile fp32 shared-memory hand-off tile (acc_tile) and goes straight on
 //     to the next unit's MMAs;
-//   * warpgroup 3 = epilogue (136 registers): reads acc_tile and stores the unit's output.
+//   * warpgroup 3 = epilogue (152 registers): reads acc_tile and stores the unit's output.
 // Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (all
 // 128 epilogue threads have read it).  So the epilogue of unit n runs while the consumers issue the MMAs of unit n+1.
 // A kernel supplies only its unit list, the TMA loads of one K-iteration, the MMAs of one stage, its gmain and its
@@ -47,6 +49,7 @@
 //
 // tc_wgrad_mn_kernel (WGRAD): MN-major operands and batch-range work units, see the comment at the kernel.
 #include "tc_common.cuh"
+#include "tc_ring.cuh"
 #include "../../include/dv3b200.h"
 
 namespace dv3 {
@@ -55,36 +58,13 @@ using namespace tc;
 
 constexpr int TC_CONV_THREADS = 512;        // tc_conv_kernel, tc_wgrad_mn_kernel: consumers 0-1, producer 2,
                                             // epilogue 3 (warpgroups)
-constexpr int TC_PRODUCER_REGS = 24;        // setmaxnreg budgets: 128 x 24 + 256 x 176 + 128 x 136 = 65 536 registers
-constexpr int TC_CONSUMER_REGS = 176;
-constexpr int TC_EPILOGUE_REGS = 136;       // > 65 536 / 512: claimed with setmaxnreg.inc (.dec may not raise it)
+constexpr int TC_PRODUCER_REGS = 24;        // setmaxnreg budgets: 128 x 24 + 256 x 168 + 128 x 152 = 65 536 registers
+constexpr int TC_CONSUMER_REGS = 168;
+constexpr int TC_EPILOGUE_REGS = 152;       // > 65 536 / 512: claimed with setmaxnreg.inc (.dec may not raise it)
 static_assert(TC_PRODUCER_REGS <= 65536 / TC_CONV_THREADS && TC_CONSUMER_REGS >= 65536 / TC_CONV_THREADS &&
               TC_EPILOGUE_REGS >= 65536 / TC_CONV_THREADS, "setmaxnreg direction of each warpgroup");
 static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS + 128 * TC_EPILOGUE_REGS <= 65536, "register file");
 constexpr int MAX_TAPS_TC = 8;
-constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in dynamic shared memory per CTA
-// Shared memory tc_conv_kernel leaves unused, so that every configuration keeps the ring depth it was measured with
-// (static_asserts after TcCfg).  Claiming it for a deeper ring is a performance change of its own.
-constexpr int RING_RESERVE = 32768;
-
-// Shared-memory layout of the pipeline: STAGES ring stages of STAGE bytes, the consumer -> epilogue hand-off tile (the
-// whole fp32 output tile, [128 rows][NCOLS + 1]), then the barriers full[STAGES], empty[STAGES], acc_full, acc_empty.
-// The ring gets what is left of the 227 KB after 2 KB (alignment slack + barriers), RESERVE and the hand-off tile, at
-// most 6 stages.  The odd pitch keeps the epilogue's column reads (a warp reads one column of 32 consecutive rows)
-// conflict-free; every access is a row base plus an immediate offset, which the register budgets of both sides need
-// (an XOR swizzle that also makes the consumers' fragment-order writes 2-way instead of 4-way conflicted spilled in
-// both warpgroups).
-template <int STAGE_BYTES, int TILE_COLS, int RESERVE>
-struct RingCfg {
-    static constexpr int STAGE = STAGE_BYTES;
-    static constexpr int NCOLS = TILE_COLS;              // columns of the output tile and of each accumulator
-    static constexpr int ACC_PITCH = NCOLS + 1;
-    static constexpr int ACC_TILE = 128 * ACC_PITCH * 4;
-    static constexpr int STAGES_RAW = (SMEM_LIMIT - 2048 - RESERVE - ACC_TILE) / STAGE;
-    static constexpr int STAGES = STAGES_RAW > 6 ? 6 : STAGES_RAW;
-    static constexpr int SMEM = STAGES * STAGE + ACC_TILE + 1024 + 512;   // + alignment slack + barriers
-};
-
 enum { TC_GATED = 0, TC_CONV = 1 };
 
 struct TcMaps { CUtensorMap a[2]; CUtensorMap b[2]; };
@@ -120,32 +100,18 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
     return make_wgmma_desc(saddr, 16, SwizzleOf<BK>::sbo, SwizzleOf<BK>::layout);
 }
 
-// Conv ring: a stage holds NPL planes of one 128-row A tile and NBOX B boxes of BR rows, each BK 16-bit channels wide.
-// BR = rows of one B-operand box (128, or 64 for problems too small to fill the machine with 128-wide tiles); NPL =
-// operand planes per stage (2: hi / lo pairs, 1: single pass)
-template <int NBOX, int BK, int BR, int NPL = 2>
-using TcCfg = RingCfg<NPL * (128 + NBOX * BR) * BK * 2, BR * NBOX, RING_RESERVE>;
-static_assert(TcCfg<2, 32, 64>::STAGES == 4, "gated forward: 4-stage ring");
-static_assert(TcCfg<1, 32, 128>::STAGES == 4, "128-column conv: 4-stage ring");
-static_assert(TcCfg<1, 64, 64>::STAGES == 3, "64-column conv at BK = 64: 3-stage ring");
-static_assert(TcCfg<1, 32, 64>::STAGES == 6, "64-column conv at BK = 32: 6-stage ring");
-// Single pass: BK = 64 wherever the contraction is a multiple of 64 channels, so a one-plane stage carries 32 KB
-// (4 stages) or 24 KB (6 stages) and feeds the MMA 4 K-steps per barrier round trip (a one-plane BK = 32 stage would
-// carry 12-16 KB for 2).  Chosen from the bytes per stage, not from an A/B of the two BK values (DESIGN.md §2.7).
-static_assert(TcCfg<2, 64, 64, 1>::STAGES == 4, "single-pass gated forward: 4-stage ring");
-static_assert(TcCfg<1, 64, 128, 1>::STAGES == 4, "single-pass 128-column conv at BK = 64: 4-stage ring");
-static_assert(TcCfg<1, 32, 128, 1>::STAGES == 6, "single-pass 128-column conv at BK = 32: 6-stage ring");
-static_assert(TcCfg<1, 64, 64, 1>::STAGES == 6, "single-pass 64-column conv at BK = 64: 6-stage ring");
-static_assert(TcCfg<1, 32, 64, 1>::STAGES == 6, "single-pass 64-column conv at BK = 32: 6-stage ring");
-
 // ---- epilogues -----------------------------------------------------------------------------------------------
 // NOTE on the epilogue loads: residual / addend / bias reads go through __ldg (ld.global.nc) and are issued as a
 // batch of 32 independent loads BEFORE the dependent math and stores of the chunk.  With plain loads the compiler
 // must order every load after the previous iteration's stores (possible aliasing), which serialised 128
 // global-memory round trips per thread (ncu: 40 % of the stall samples sat on the first use of these loads).
-// The accumulator values are read from the hand-off tile where they are used rather than staged in registers: the
-// epilogue warpgroup runs on TC_EPILOGUE_REGS.  Both arrive on acc_empty at the end of their last 32-column chunk,
-// while its stores are still under way (the epilogue contract of tc_pipeline).
+// epilogue_conv reads each 32-column chunk's accumulator values into registers before the chunk's loads and arrives
+// on acc_empty as soon as it has read the last chunk, so the consumers can write the next unit's tile while the
+// epilogue's last loads and stores are under way: the 1x1 convs and data gradients, whose short contractions leave
+// the epilogue as the longer side of the pipeline, run 12-24 % faster (DESIGN.md section 2.4).  That holds 96 live
+// floats, which needs the 152 registers of TC_EPILOGUE_REGS (at 136 it spilled).  epilogue_gated reads the tile where
+// it uses it, after the chunk's loads (both halves of a chunk and its residual / speaker addends would be 128 live
+// floats), and arrives at the end of its last chunk.
 template <int BR>
 __device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
                                                int a_z, int b_row0) {
@@ -206,7 +172,10 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
     float* __restrict__ out = p.out;
 #pragma unroll 1
     for (int c32 = 0; c32 < NCOLS; c32 += 32) {             // not unrolled: interleaving the chunks spilled
-        float v[32], x2[32];                                // addends e1, e2
+        float d[32], v[32], x2[32];                         // accumulator values; addends e1, e2
+#pragma unroll
+        for (int i = 0; i < 32; ++i) d[i] = arow[c32 + i];
+        if (c32 + 32 == NCOLS) mbar_arrive(acc_empty);      // last read of the tile: release it before the loads
         const int n0 = b_row0 + c32;
         const size_t cb = ((size_t)b * p.Nc + n0) * p.T + (tv ? t : 0);
         if (tv) {
@@ -221,7 +190,7 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
                 const int n = n0 + i;
                 if (n < p.Nc) {
                     const size_t idx = cb + (size_t)i * p.T;
-                    float g = arow[c32 + i] * drop_scale(drop, (uint32_t)idx);
+                    float g = d[i] * drop_scale(drop, (uint32_t)idx);
                     if (bias) g += __ldg(&bias[n]);
                     if (p.addmode == 1) g += p.alpha * v[i];
                     else if (p.addmode == 2) g += v[i] * (1.f - x2[i]);
@@ -230,7 +199,6 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
                 }
             }
         }
-        if (c32 + 32 == NCOLS) mbar_arrive(acc_empty);
     }
 }
 
@@ -423,15 +391,6 @@ struct TcMnParams {
     int msplit; long long s_m, s_mh, s_n, s_j;
     float gcoef;                              // see TcParams::gmain (n_mma = 2 per 32-row time chunk)
 };
-
-constexpr int WG_BOX = 64 * 32 * 2;                      // 64 channels x 32 time steps of bf16 = 4 KB
-// Per plane: 128 channels of m, 128 channels of n.  The hand-off tile [128 m][128 n + 1] fp32 (66 KB; the odd pitch
-// keeps both epilogue access patterns conflict-free) leaves room for five 32 KB two-plane stages.
-template <int NPL>
-using WgCfg = RingCfg<NPL * 4 * WG_BOX, 128, 0>;
-static_assert(WgCfg<2>::STAGES == 5, "two-plane weight gradient: 5-stage ring");
-static_assert(WgCfg<1>::STAGES == 6, "single-pass weight gradient: 6-stage ring");
-static_assert(WgCfg<2>::SMEM <= SMEM_LIMIT && WgCfg<1>::SMEM <= SMEM_LIMIT, "weight gradient shared memory");
 
 template <int NPL>
 __global__ void __launch_bounds__(TC_CONV_THREADS, 1)
