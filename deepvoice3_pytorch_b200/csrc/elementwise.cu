@@ -1,6 +1,7 @@
 // Memory-bound glue kernels of the hot path: layout changes, lookups, position encodings, dropout,
 // masked softmax.  All are coalesced along the fastest axis and vectorised where alignment allows.
 #include "common.cuh"
+#include <climits>
 
 namespace dv3 {
 
@@ -371,14 +372,26 @@ int dv3_dropout(const float* x, float* y, long long n, float p, const unsigned l
     return check_launch("dropout");
 }
 
+// One warp per row: rows * 32 threads must stay an int.
+static int softmax_args(const char* what, int rows, int L) {
+    DV3_REQUIRE(rows >= 1 && L >= 1, "%s: rows %d and L %d must be >= 1", what, rows, L);
+    DV3_REQUIRE(rows <= INT_MAX / 32, "%s: %d rows exceed one warp each in int", what, rows);
+    return 0;
+}
+
 int dv3_softmax_fwd(const float* s, const unsigned char* mask, float* probs, float* pd, int rows, int L,
                     int rows_per_b, float p, const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+    if (int e = softmax_args("softmax_fwd", rows, L)) return e;
+    DV3_REQUIRE(rows_per_b >= 1, "softmax_fwd: rows_per_b %d must be >= 1", rows_per_b);
+    DV3_REQUIRE(!mask || rows % rows_per_b == 0, "softmax_fwd: %d rows are not whole batches of %d", rows,
+                rows_per_b);
     launch_k(softmax_fwd_kernel, ceil_div(rows * 32, 256), 256, 0, (cudaStream_t)stream, s, mask, probs, pd, rows, L,
                                                                                   rows_per_b, p, seed_ptr, salt);
     return check_launch("softmax_fwd");
 }
 int dv3_softmax_bwd(const float* probs, const float* dpd, const float* dprobs_ext, float* ds, int rows, int L,
                     float p, const unsigned long long* seed_ptr, unsigned salt, void* stream) {
+    if (int e = softmax_args("softmax_bwd", rows, L)) return e;
     launch_k(softmax_bwd_kernel, ceil_div(rows * 32, 256), 256, 0, (cudaStream_t)stream, probs, dpd, dprobs_ext, ds,
                                                                                   rows, L, p, seed_ptr, salt);
     return check_launch("softmax_bwd");

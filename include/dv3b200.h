@@ -105,7 +105,9 @@ int dv3_dropout(const float* x, float* y, long long n, float p, const unsigned l
 
 /* ---- masked row softmax + dropout: reference deepvoice3.py:145-148,161-165.
  * s (rows,L); mask (rows/rows_per_b, L) bytes, 1 = padding (-inf), or NULL; probs = softmax (the returned
- * alignment); pd = dropout(probs) (may be NULL).  bwd: ds = P*(g - <g,P>), g = dpd*dropmask + dprobs_ext. */
+ * alignment); pd = dropout(probs) (may be NULL).  bwd: ds = P*(g - <g,P>), g = dpd*dropmask + dprobs_ext.
+ * One warp per row.  Refused before any launch (return 1): rows < 1, L < 1, rows > INT_MAX / 32, rows_per_b < 1,
+ * and, with a mask, rows % rows_per_b != 0.  A row whose keys are all masked is outside the contract. */
 int dv3_softmax_fwd(const float* s, const unsigned char* mask, float* probs, float* pd, int rows, int L,
                     int rows_per_b, float p, const unsigned long long* seed_ptr, unsigned salt, void* stream);
 int dv3_softmax_bwd(const float* probs, const float* dpd, const float* dprobs_ext, float* ds, int rows, int L,
