@@ -52,6 +52,27 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+// ---- TMA: 3-D tiled store from shared memory, tracked by the issuing thread's bulk groups ----------------------------
+// Elements of the box outside the tensor's extent are not written.  Generic-proxy writes of the source must be made
+// visible to the async proxy first (fence_proxy_async by every writing thread, then a barrier).
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(map), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// every committed store has finished reading its shared-memory source (the source may be overwritten)
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+// every committed store has completed
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// `count` arrivals at once (sm_90)
+__device__ __forceinline__ void mbar_arrive_cnt(uint64_t* bar, uint32_t count) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+}
+// named barrier `id` over `threads` threads (whole warps)
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // ---- per-warpgroup register budget ---------------------------------------------------------------
 // Executed by every thread of a warpgroup: hand registers back to the SM (producer) or claim them (consumers) so that

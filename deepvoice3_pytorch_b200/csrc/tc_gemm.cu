@@ -31,21 +31,23 @@
 //     weight gradient, 6 for the smaller stages;
 //   * warpgroups 0 and 1 = consumers (168 registers): each accumulates 64 of the 128 tile rows in registers (wgmma),
 //     keeping one stage of MMAs in flight (wait_group 1, then release the previous stage), then writes
-//     main * gmain + cross * 2^-11 into a full-tile fp32 shared-memory hand-off tile (acc_tile) and goes straight on
-//     to the next unit's MMAs;
+//     main * gmain + cross * 2^-11 into a full-tile fp32 shared-memory hand-off tile (acc_tile, layout in
+//     tc_ring.cuh) and goes straight on to the next unit's MMAs;
 //   * warpgroup 3 = epilogue (152 registers): reads acc_tile and stores the unit's output.
-// Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (all
-// 128 epilogue threads have read it).  So the epilogue of unit n runs while the consumers issue the MMAs of unit n+1.
-// A kernel supplies only its unit list, the TMA loads of one K-iteration, the MMAs of one stage, its gmain and its
-// epilogue.
+// Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (128
+// arrivals: the epilogue is done with it).  So the epilogue of unit n runs while the consumers issue the MMAs of unit
+// n+1.  A kernel supplies only its unit list, the TMA loads of one K-iteration, the MMAs of one stage, its gmain, its
+// epilogue and the loads of its epilogue's staged inputs.
 //
 // tc_conv_kernel (GATED, CONV): a unit is one 128-step x NCOLS output tile of one utterance.  Operands are 16-bit
 // (B,T,C) planes fetched by TMA as K-major tiles of 128 rows x BK (BK = 64: 128-byte rows, SWIZZLE_128B; BK = 32:
 // 64-byte rows, SWIZZLE_64B; the host launchers pick BK per configuration); the conv's zero padding, the causal shift,
-// ragged T / channel tails are TMA out-of-bounds zero fill.  Epilogue thread r owns row r (time step) of acc_tile and
-// fuses the launch's own math only (gate, bias, speaker bias, residual, dropout mask, addend, ReLU), storing fp32
-// (B,C,T) outputs coalesced along T.  The operand planes of the next GEMM come from the split kernels of tc_split.cu,
-// which run at full occupancy rather than on one warpgroup per SM.
+// ragged T / channel tails are TMA out-of-bounds zero fill.  Its hand-off tile is the dense image of the output's
+// TMA boxes: epilogue thread r owns time step r and fuses the launch's own math only (gate, bias, speaker bias,
+// residual, dropout mask, addend, ReLU) in place in the tile, and the fp32 (B,C,T) outputs leave as TMA bulk tensor
+// stores clipped at T and C; the gated forward's residual tile arrives by TMA into a staging buffer (see the epilogues).
+// The operand planes of the next GEMM come from the split kernels of tc_split.cu, which run at full occupancy rather
+// than on one warpgroup per SM.
 //
 // tc_wgrad_mn_kernel (WGRAD): MN-major operands and batch-range work units, see the comment at the kernel.
 #include "tc_common.cuh"
@@ -89,6 +91,7 @@ struct TcParams {
     // smaller in effect: their loss is below fp32 resolution).
     float gmain;
     int operand_bf16;          // operand format of the MMAs: 0 = fp16 planes (forward), 1 = bf16 planes (gradients)
+    int tma_out;               // 1: outputs (and the gated residual) through the TcOutMaps; 0: per-thread accesses
 };
 
 template <int BK> struct SwizzleOf;
@@ -101,105 +104,185 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
 }
 
 // ---- epilogues -----------------------------------------------------------------------------------------------
-// NOTE on the epilogue loads: residual / addend / bias reads go through __ldg (ld.global.nc) and are issued as a
-// batch of 32 independent loads BEFORE the dependent math and stores of the chunk.  With plain loads the compiler
-// must order every load after the previous iteration's stores (possible aliasing), which serialised 128
-// global-memory round trips per thread (ncu: 40 % of the stall samples sat on the first use of these loads).
-// epilogue_conv reads each 32-column chunk's accumulator values into registers before the chunk's loads and arrives
-// on acc_empty as soon as it has read the last chunk, so the consumers can write the next unit's tile while the
-// epilogue's last loads and stores are under way: the 1x1 convs and data gradients, whose short contractions leave
-// the epilogue as the longer side of the pipeline, run 12-24 % faster (DESIGN.md section 2.4).  That holds 96 live
-// floats, which needs the 152 registers of TC_EPILOGUE_REGS (at 136 it spilled).  epilogue_gated reads the tile where
-// it uses it, after the chunk's loads (both halves of a chunk and its residual / speaker addends would be 128 live
-// floats), and arrives at the end of its last chunk.
+// Both conv epilogues compute in place in the dense hand-off tile (tc_ring.cuh): epilogue thread r owns time step r of
+// the unit and reads / writes its column entries (a warp covers one 128-byte row of a box: conflict-free), then the
+// tile goes out as TMA bulk tensor stores, four 32-step boxes per output, issued by one elected thread after a
+// proxy fence and a named barrier of the epilogue warpgroup.  The tensor maps carry the logical (B, Nc, T) extent, so
+// TMA clipping drops the time steps past T and the channels past Nc; the thread that issued the stores waits until
+// they have read shared memory (not until they have landed) and then releases the tile for all 128 threads.  Global
+// fp32 rows must be 16-byte aligned for a TMA map (T % 4 == 0, aligned pointers); otherwise (p.tma_out == 0) every
+// thread stores its own time step from the tile, coalesced along T, as the per-thread epilogue always did.  The math
+// per element is that of the per-thread epilogue, in the same order.
+// Addend / speaker-bias reads go through __ldg (ld.global.nc) in batches of 32 independent loads BEFORE the dependent
+// math of the chunk: with plain loads the compiler must order every load after the previous iteration's stores.
+
+// float offset of channel c, time step (threadIdx.x % 128) in a dense tile of NC channels
+template <int NC>
+__device__ __forceinline__ int dense_at(int c) {
+    const int r = threadIdx.x & 127;
+    return (r >> 5) * NC * 32 + c * 32 + ((((r >> 2) & 7) ^ (c & 7)) << 2) + (r & 3);
+}
+
+struct TcOutMaps { CUtensorMap out[3]; CUtensorMap res; };   // y | a | s (GATED) or out (CONV); the residual input
+
+// Where an epilogue finds its shared memory: the hand-off tile, the staging buffer, the barriers.
+struct Handoff { float* tile; float* staging; uint64_t* acc_empty; uint64_t* in_full; };
+
+// Release the hand-off tile after the bulk stores of this unit, or, with per-thread stores, after this thread's.
+__device__ __forceinline__ void release_tile(const Handoff& h, bool tma) {
+    if (!tma) mbar_arrive(h.acc_empty);
+    else if ((threadIdx.x & 127) == 0) {
+        bulk_commit();
+        bulk_wait_read();
+        mbar_arrive_cnt(h.acc_empty, 128);
+    }
+}
+
+// The gated forward's residual tile (128 steps x BR channels) into the staging buffer by TMA: issued for the next
+// unit as soon as the current unit's y stores have read the buffer, so it lands under the next unit's MMAs.
 template <int BR>
-__device__ __forceinline__ void epilogue_gated(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
+__device__ __forceinline__ void stage_residual(const TcParams& p, const TcOutMaps& om, const Handoff& h, int a_row0,
                                                int a_z, int b_row0) {
+    if (!p.tma_out || !((p.gate_mode != 0) || p.residual) || (threadIdx.x & 127) != 0) return;
+    mbar_arrive_expect_tx(h.in_full, 128 * BR * 4);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) tma_load_3d(h.staging + q * BR * 32, &om.res, h.in_full, a_row0 + 32 * q, b_row0, a_z);
+}
+
+// Gated: a = acc_a (+ speaker) + bias_a, s = sigmoid(acc_b + bias_b), y from a, s and the residual.  y replaces the
+// residual in the staging buffer, a and s replace the two accumulator halves; the speaker bias (multi-speaker presets
+// only) stays on __ldg.
+template <int BR>
+__device__ __forceinline__ void epilogue_gated(const TcParams& p, const TcOutMaps& om, const Handoff& h, int n,
+                                               int a_row0, int a_z, int b_row0) {
+    constexpr int NC = 2 * BR;                             // a | b halves of the tile
     const int t = a_row0 + (threadIdx.x & 127), b = a_z, C = p.Nc;
-    const bool tv = t < p.T;
+    const bool tv = t < p.T, tma = p.tma_out != 0;
     const float* __restrict__ bias = p.bias;
     const float* __restrict__ res = p.res;
     const float* __restrict__ spk = p.spk;
     float* __restrict__ yo = p.y;
     float* __restrict__ ao = p.save_a;
     float* __restrict__ so = p.save_s;
+    float* tile = h.tile;
+    float* st = h.staging;
     const bool need_res = (p.gate_mode != 0) || p.residual;
     const size_t base = ((size_t)b * C + b_row0) * p.T + (tv ? t : 0);
-#pragma unroll
+    if (need_res) {
+        if (tma) mbar_wait(h.in_full, n & 1);
+        else {
+#pragma unroll 8
+            for (int c = 0; c < BR; ++c) st[dense_at<BR>(c)] = tv ? __ldg(&res[base + (size_t)c * p.T]) : 0.f;
+        }
+    }
+#pragma unroll 1
     for (int c32 = 0; c32 < BR; c32 += 32) {
-        float rr[32], sp[32];                               // rr: residual
-        if (tv) {
-            const size_t cb = base + (size_t)c32 * p.T;
+        float sp[32], ba[32], bb[32];                      // speaker bias; bias of the a and b halves
+        const size_t cb = base + (size_t)c32 * p.T;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) rr[i] = need_res ? __ldg(&res[cb + (size_t)i * p.T]) : 0.f;
-            if (spk) {
+        for (int i = 0; i < 32; ++i) {
+            ba[i] = __ldg(&bias[b_row0 + c32 + i]);
+            bb[i] = __ldg(&bias[C + b_row0 + c32 + i]);
+            if (spk) sp[i] = tv ? __ldg(&spk[cb + (size_t)i * p.T]) : 0.f;
+        }
 #pragma unroll
-                for (int i = 0; i < 32; ++i) sp[i] = __ldg(&spk[cb + (size_t)i * p.T]);
+        for (int i = 0; i < 32; ++i) {
+            const int cl = c32 + i;
+            float va = tile[dense_at<NC>(cl)];
+            if (spk) va += sp[i];
+            const float a = va + ba[i];
+            const float s = sigmoidf_(tile[dense_at<NC>(BR + cl)] + bb[i]);
+            const float rr = need_res ? st[dense_at<BR>(cl)] : 0.f;
+            float y;
+            if (p.gate_mode == 0) {
+                y = a * s;
+                if (p.residual) y = (y + rr) * 0.70710678118654752f;
+            } else {
+                y = s * a + (1.f - s) * rr;
             }
+            st[dense_at<BR>(cl)] = y;
+            tile[dense_at<NC>(cl)] = a;
+            tile[dense_at<NC>(BR + cl)] = s;
+        }
+    }
+    if (tma) {
+        fence_proxy_async();
+        named_bar_sync(1, 128);
+        if ((threadIdx.x & 127) == 0) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                const int c = b_row0 + c32 + i;
-                const size_t idx = cb + (size_t)i * p.T;
-                float va = arow[c32 + i];
-                if (spk) va += sp[i];
-                const float a = va + __ldg(&bias[c]);
-                const float s = sigmoidf_(arow[BR + c32 + i] + __ldg(&bias[C + c]));
-                float y;
-                if (p.gate_mode == 0) {
-                    y = a * s;
-                    if (p.residual) y = (y + rr[i]) * 0.70710678118654752f;
-                } else {
-                    y = s * a + (1.f - s) * rr[i];
-                }
-                yo[idx] = y;
-                if (ao) ao[idx] = a;
-                if (so) so[idx] = s;
+            for (int q = 0; q < 4; ++q) {
+                const int t0 = a_row0 + 32 * q;
+                if (t0 >= p.T) break;
+                tma_store_3d(&om.out[0], st + q * BR * 32, t0, b_row0, b);
+                if (ao) tma_store_3d(&om.out[1], tile + q * NC * 32, t0, b_row0, b);
+                if (so) tma_store_3d(&om.out[2], tile + q * NC * 32 + BR * 32, t0, b_row0, b);
             }
         }
-        if (c32 + 32 == BR) mbar_arrive(acc_empty);
+    } else if (tv) {
+#pragma unroll 8
+        for (int c = 0; c < BR; ++c) {
+            const size_t idx = base + (size_t)c * p.T;
+            yo[idx] = st[dense_at<BR>(c)];
+            if (ao) ao[idx] = tile[dense_at<NC>(c)];
+            if (so) so[idx] = tile[dense_at<NC>(BR + c)];
+        }
     }
+    release_tile(h, tma);
 }
 
+// Conv: out = acc * dropmask + bias + addend, then ReLU.
 template <int NCOLS>
-__device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* arow, uint64_t* acc_empty, int a_row0,
+__device__ __forceinline__ void epilogue_conv(const TcParams& p, const TcOutMaps& om, const Handoff& h, int a_row0,
                                               int a_z, int b_row0) {
     const int t = a_row0 + (threadIdx.x & 127), b = a_z;
-    const bool tv = t < p.T;
+    const bool tv = t < p.T, tma = p.tma_out != 0;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
     const float* __restrict__ bias = p.bias;
     const float* __restrict__ e1 = p.e1;
     const float* __restrict__ e2 = p.e2;
     float* __restrict__ out = p.out;
+    float* tile = h.tile;
+    const size_t base = ((size_t)b * p.Nc + b_row0) * p.T + (tv ? t : 0);
 #pragma unroll 1
     for (int c32 = 0; c32 < NCOLS; c32 += 32) {             // not unrolled: interleaving the chunks spilled
-        float d[32], v[32], x2[32];                         // accumulator values; addends e1, e2
-#pragma unroll
-        for (int i = 0; i < 32; ++i) d[i] = arow[c32 + i];
-        if (c32 + 32 == NCOLS) mbar_arrive(acc_empty);      // last read of the tile: release it before the loads
+        float bz[32], v[32], x2[32];                        // bias; addends e1, e2
         const int n0 = b_row0 + c32;
-        const size_t cb = ((size_t)b * p.Nc + n0) * p.T + (tv ? t : 0);
-        if (tv) {
+        const size_t cb = base + (size_t)c32 * p.T;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                const bool ok = n0 + i < p.Nc;
-                v[i] = (p.addmode != 0 && ok) ? __ldg(&e1[cb + (size_t)i * p.T]) : 0.f;
-                x2[i] = (p.addmode == 2 && ok) ? __ldg(&e2[cb + (size_t)i * p.T]) : 0.f;
-            }
+        for (int i = 0; i < 32; ++i) {
+            const bool ok = tv && n0 + i < p.Nc;
+            bz[i] = (bias && n0 + i < p.Nc) ? __ldg(&bias[n0 + i]) : 0.f;
+            v[i] = (p.addmode != 0 && ok) ? __ldg(&e1[cb + (size_t)i * p.T]) : 0.f;
+            x2[i] = (p.addmode == 2 && ok) ? __ldg(&e2[cb + (size_t)i * p.T]) : 0.f;
+        }
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {
-                const int n = n0 + i;
-                if (n < p.Nc) {
-                    const size_t idx = cb + (size_t)i * p.T;
-                    float g = d[i] * drop_scale(drop, (uint32_t)idx);
-                    if (bias) g += __ldg(&bias[n]);
-                    if (p.addmode == 1) g += p.alpha * v[i];
-                    else if (p.addmode == 2) g += v[i] * (1.f - x2[i]);
-                    if (p.relu) g = fmaxf(g, 0.f);
-                    out[idx] = g;
-                }
-            }
+        for (int i = 0; i < 32; ++i) {
+            float& d = tile[dense_at<NCOLS>(c32 + i)];
+            float g = d * drop_scale(drop, (uint32_t)(cb + (size_t)i * p.T));
+            if (bias) g += bz[i];
+            if (p.addmode == 1) g += p.alpha * v[i];
+            else if (p.addmode == 2) g += v[i] * (1.f - x2[i]);
+            if (p.relu) g = fmaxf(g, 0.f);
+            d = g;
         }
     }
+    if (tma) {
+        fence_proxy_async();
+        named_bar_sync(1, 128);
+        if ((threadIdx.x & 127) == 0) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const int t0 = a_row0 + 32 * q;
+                if (t0 >= p.T) break;
+                tma_store_3d(&om.out[0], tile + q * NCOLS * 32, t0, b_row0, b);
+            }
+        }
+    } else if (tv) {
+#pragma unroll 8
+        for (int c = 0; c < NCOLS; ++c)
+            if (b_row0 + c < p.Nc) out[base + (size_t)c * p.T] = tile[dense_at<NCOLS>(c)];
+    }
+    release_tile(h, tma);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -211,14 +294,18 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const float* ar
 //   mma(stage, wg, acc, xacc)     consumer warpgroup wg's MMAs of one stage: p0 x p0 into acc and, with two planes,
 //                                 p0 x p1 + p1 x p0 into xacc (64 rows x NCOLS columns, NCOLS / 2 registers each)
 //   gmain(w)                      the factor of w's main accumulator (TcParams::gmain)
-//   epilogue(w, acc_tile, acc_empty)   stores w's output from the hand-off tile [128][Cfg::ACC_PITCH].  Contract:
-//                                 every epilogue thread arrives on acc_empty exactly once per unit, right after its
-//                                 last read of acc_tile, so the consumers can overwrite the tile while the epilogue's
-//                                 last stores are still under way.
+//   epilogue(w, n, h)             stores w, this CTA's n-th unit, from the hand-off tile h.tile (layout: Cfg::DENSE,
+//                                 tc_ring.cuh).  Contract: the epilogue warpgroup arrives on h.acc_empty 128 times
+//                                 per unit, once its last access of the tile is done (by a thread or by the bulk
+//                                 stores it issued), so the consumers can overwrite the tile while the epilogue's
+//                                 last global stores are still under way.
+//   stage(w, h)                   issues the loads of unit w's epilogue inputs into h.staging, completing on
+//                                 h.in_full (phase n for the n-th unit): called by every epilogue thread for the
+//                                 first unit up front and for each next unit right after the current epilogue.
 // ------------------------------------------------------------------------------------------------
-template <class Cfg, int NPL, class Decode, class Load, class Mma, class Gmain, class Epilogue>
+template <class Cfg, int NPL, class Decode, class Load, class Mma, class Gmain, class Epilogue, class Stage>
 __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, Decode decode, Load load, Mma mma,
-                                            Gmain gmain, Epilogue epilogue) {
+                                            Gmain gmain, Epilogue epilogue, Stage stage) {
     static_assert(NPL == 1 || NPL == 2, "one or two operand planes");
     static_assert(Cfg::NCOLS <= 128, "main + cross accumulators must fit in the registers of a consumer thread");
     static_assert(Cfg::STAGES >= 2, "pipeline needs at least two stages");
@@ -226,12 +313,16 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
     constexpr int NR = Cfg::NCOLS / 2;                       // registers per accumulator per thread
     pdl_trigger();
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    // 1 KB aligned by pointer arithmetic on the __shared__ array (not through an integer), so that the compiler keeps
+    // knowing the address space: shared loads / stores (LDS / STS) instead of generic ones, which it may not reorder
+    // with the epilogue's global loads.
+    uint8_t* smem = smem_raw + ((1024 - (smem_u32(smem_raw) & 1023)) & 1023);
     float* acc_tile = reinterpret_cast<float*>(smem + STAGES * STAGE);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE + Cfg::ACC_TILE);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE + Cfg::ACC_TILE + Cfg::STAGING);
     uint64_t* empty = full + STAGES;
     uint64_t* acc_full = empty + STAGES;                     // the consumers have written acc_tile (256 arrivals)
-    uint64_t* acc_empty = acc_full + 1;                      // the epilogue has read acc_tile (128 arrivals)
+    uint64_t* acc_empty = acc_full + 1;                      // the epilogue is done with acc_tile (128 arrivals)
+    uint64_t* in_full = acc_empty + 1;                       // the staged epilogue inputs have landed
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
     if (threadIdx.x == 0) {
@@ -242,6 +333,7 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
         mbar_init(acc_full, 256);
         mbar_init(acc_empty, 128);
+        mbar_init(in_full, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -249,12 +341,16 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
 
     if (warp >= 12) {
         setmaxnreg_inc<TC_EPILOGUE_REGS>();                  // up from the launch's 65 536 / 512 = 128 per thread
+        const Handoff h = {acc_tile, acc_tile + Cfg::ACC_TILE / 4, acc_empty, in_full};
+        if (blockIdx.x < num_units) stage(decode(blockIdx.x), h);
         int n = 0;
         for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++n) {
             const auto w = decode(u);
             mbar_wait(acc_full, n & 1);
-            epilogue(w, acc_tile, acc_empty);
+            epilogue(w, n, h);
+            if (u + gridDim.x < num_units) stage(decode(u + gridDim.x), h);
         }
+        if ((threadIdx.x & 127) == 0) bulk_wait();            // the last unit's bulk stores have completed
     } else if (warp >= 8) {
         setmaxnreg_dec<TC_PRODUCER_REGS>();
         if (warp == 8 && lane == 0) {
@@ -295,10 +391,20 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
             wgmma_wait<0>();
             if (w.n_iters > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty[(it - 1) % STAGES]);
             const float gm = gmain(w);
-            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue has read the previous unit
+            mbar_wait(acc_empty, (n & 1) ^ 1);                        // the epilogue is done with the previous unit
+            // Dense tile: register i sits at time step 64 wg + 16 wq + lane / 4 + 8 ((i >> 1) & 1), i.e. in box
+            // 2 wg + wq / 2, chunk 4 (wq & 1) + lane / 16 + 2 ((i >> 1) & 1), and at channel 8 (i >> 2) + 2 (lane & 3)
+            // + (i & 1), so its swizzled chunk is sw ^ (i & 3) with a per-thread sw: four per-thread bases, each
+            // plus an immediate offset per register.
+            const int sw = (((wq & 1) << 2) | (lane >> 4)) ^ ((lane & 3) << 1);
+            float* const frag0 = Cfg::DENSE ? acc_tile + (2 * wg + (wq >> 1)) * Cfg::NCOLS * 32 + (lane & 3) * 64 +
+                                                  ((lane >> 2) & 3)
+                                            : acc_tile;
 #pragma unroll
             for (int i = 0; i < NR; ++i) {                            // lo planes carry 2^11
-                float* dst = &acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)];
+                float* dst = Cfg::DENSE
+                    ? frag0 + (i >> 2) * 256 + (i & 1) * 32 + ((sw ^ (i & 3)) << 2)
+                    : &acc_tile[(64 * wg + frag_row(i, wq, lane)) * Cfg::ACC_PITCH + frag_col(i, lane)];
                 if constexpr (NPL == 2) *dst = fmaf(xacc[i], LO_INV, acc[i] * gm);
                 else *dst = acc[i] * gm;
             }
@@ -313,8 +419,8 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
 // ------------------------------------------------------------------------------------------------
 template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
 __global__ void __launch_bounds__(TC_CONV_THREADS, 1)
-tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcParams p, int tiles_x, int tiles_y,
-               int num_tiles) {
+tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcOutMaps om,
+               const __grid_constant__ TcParams p, int tiles_x, int tiles_y, int num_tiles) {
     using Cfg = TcCfg<NBOX, BK, BR, NPL>;
     constexpr int NCOLS = Cfg::NCOLS;
     constexpr int TILE = 128 * BK * 2, TILE_B = BR * BK * 2;   // one plane of the A tile (128 rows), one B box
@@ -360,12 +466,14 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcPa
         }
     };
     auto gmain = [&](const Tile&) { return p.gmain; };
-    auto epilogue = [&](const Tile& w, const float* acc_tile, uint64_t* acc_empty) {
-        const float* arow = acc_tile + (threadIdx.x & 127) * Cfg::ACC_PITCH;   // this thread's time step
-        if (MODE == TC_GATED) epilogue_gated<BR>(p, arow, acc_empty, w.a_row0, w.a_z, w.b_row0);
-        else epilogue_conv<NCOLS>(p, arow, acc_empty, w.a_row0, w.a_z, w.b_row0);
+    auto epilogue = [&](const Tile& w, int n, const Handoff& h) {
+        if (MODE == TC_GATED) epilogue_gated<BR>(p, om, h, n, w.a_row0, w.a_z, w.b_row0);
+        else epilogue_conv<NCOLS>(p, om, h, w.a_row0, w.a_z, w.b_row0);
     };
-    tc_pipeline<Cfg, NPL>(maps, num_tiles, decode, load, mma, gmain, epilogue);
+    auto stage = [&](const Tile& w, const Handoff& h) {
+        if (MODE == TC_GATED) stage_residual<BR>(p, om, h, w.a_row0, w.a_z, w.b_row0);
+    };
+    tc_pipeline<Cfg, NPL>(maps, num_tiles, decode, load, mma, gmain, epilogue, stage);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -449,7 +557,8 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
     // Tap-major layout (s_n == 1): thread r owns column n0 + r and walks the rows, a warp storing 32 consecutive floats
     // of one row.  Otherwise (ConvTranspose layout, consecutive m two floats apart): thread r owns row m0 + r and walks
     // the columns.
-    auto epilogue = [&](const Unit& w, const float* acc_tile, uint64_t* acc_empty) {
+    auto epilogue = [&](const Unit& w, int, const Handoff& h) {
+        const float* acc_tile = h.tile;
         const int r = threadIdx.x & 127;
         float* __restrict__ out = p.dw + (size_t)w.s * p.split_stride + (size_t)w.j * p.s_j;
         const int rows = min(128, p.Mw - w.m0), cols = min(128, p.Nw - w.n0);
@@ -470,9 +579,9 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
 #pragma unroll 4
             for (int c = 0; c < cols; ++c) o[(size_t)c * p.s_n] = arow[c];
         }
-        mbar_arrive(acc_empty);
+        mbar_arrive(h.acc_empty);
     };
-    tc_pipeline<Cfg, NPL>(maps, p.num_units, decode, load, mma, gmain, epilogue);
+    tc_pipeline<Cfg, NPL>(maps, p.num_units, decode, load, mma, gmain, epilogue, [](const Unit&, const Handoff&) {});
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -514,6 +623,28 @@ int encode_tmap_bf16_3d(CUtensorMap* map, const void* base, uint64_t d0, uint64_
     return 0;
 }
 
+// fp32 (B, Nc, T) tensor as TMA boxes of 32 time steps x box_c channels, SWIZZLE_128B: the boxes of the dense
+// hand-off tile (tc_ring.cuh).  The extent is the logical one, so TMA clips every box at T and at Nc.
+static int encode_tmap_f32_bct(CUtensorMap* map, const float* base, int B, int Nc, int T, int box_c) {
+    const EncodeTiledFn enc = encode_fn();
+    if (!enc) { set_error("cuTensorMapEncodeTiled entry point unavailable"); return 1; }
+    cuuint64_t dims[3] = {(cuuint64_t)T, (cuuint64_t)Nc, (cuuint64_t)B};
+    cuuint64_t strides[2] = {(cuuint64_t)T * 4, (cuuint64_t)Nc * T * 4};
+    cuuint32_t box[3] = {32, (cuuint32_t)box_c, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled failed (%d): fp32 (B,C,T) = (%d,%d,%d) box=(32,%d)", (int)r, B, Nc, T, box_c);
+        return 1;
+    }
+    return 0;
+}
+
+// A TMA map needs 16-byte aligned rows: T % 4 == 0 and a 16-byte aligned base (or no tensor at all).
+static bool tma_rows(const float* base, int T) { return T % 4 == 0 && ((uintptr_t)base & 15) == 0; }
+
 template <typename K>
 static int ensure_smem(K kern, int bytes, const char* what) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
@@ -533,19 +664,19 @@ static int launch_persistent(int units, cudaStream_t st, const char* what, const
 }
 
 template <int MODE, int NBOX, int BR, int BK, bool BF16, int NPL>
-static int launch_conv_fmt(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
-                           const char* what) {
+static int launch_conv_fmt(const TcMaps& maps, const TcOutMaps& om, const TcParams& p, int tiles_x, int tiles_y,
+                           int batch, cudaStream_t st, const char* what) {
     const int num_tiles = tiles_x * tiles_y * batch;
     return launch_persistent<TcCfg<NBOX, BK, BR, NPL>, tc_conv_kernel<MODE, NBOX, BR, BK, BF16, NPL>>(
-        num_tiles, st, what, maps, p, tiles_x, tiles_y, num_tiles);
+        num_tiles, st, what, maps, om, p, tiles_x, tiles_y, num_tiles);
 }
 
 template <int MODE, int NBOX, int BR, int BK, int NPL = 2>
-static int launch_conv(const TcMaps& maps, const TcParams& p, int tiles_x, int tiles_y, int batch, cudaStream_t st,
-                       const char* what) {
+static int launch_conv(const TcMaps& maps, const TcOutMaps& om, const TcParams& p, int tiles_x, int tiles_y, int batch,
+                       cudaStream_t st, const char* what) {
     if (p.operand_bf16)
-        return launch_conv_fmt<MODE, NBOX, BR, BK, true, NPL>(maps, p, tiles_x, tiles_y, batch, st, what);
-    return launch_conv_fmt<MODE, NBOX, BR, BK, false, NPL>(maps, p, tiles_x, tiles_y, batch, st, what);
+        return launch_conv_fmt<MODE, NBOX, BR, BK, true, NPL>(maps, om, p, tiles_x, tiles_y, batch, st, what);
+    return launch_conv_fmt<MODE, NBOX, BR, BK, false, NPL>(maps, om, p, tiles_x, tiles_y, batch, st, what);
 }
 
 static void fill_taps_tc(int* tap_off, int k, int dilation, int causal, bool transpose) {
@@ -601,11 +732,21 @@ int dv3_tc_convblock_fwd(const void* xd, const void* w, int npl, const float* bi
     p.bias = bias; p.spk = spk; p.res = res; p.y = y; p.save_a = save_a; p.save_s = save_s;
     p.gate_mode = mode; p.residual = residual;
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (BK / 16));
+    const bool need_res = mode != 0 || residual;
+    TcOutMaps om = {};
+    p.tma_out = tma_rows(y, T) && (!save_a || tma_rows(save_a, T)) && (!save_s || tma_rows(save_s, T)) &&
+                (!need_res || tma_rows(res, T));
+    if (p.tma_out) {
+        const float* outs[3] = {y, save_a, save_s};
+        for (int i = 0; i < 3; ++i)
+            if (outs[i] && encode_tmap_f32_bct(&om.out[i], outs[i], B, C, T, 64)) return 1;
+        if (need_res && encode_tmap_f32_bct(&om.res, res, B, C, T, 64)) return 1;
+    }
     cudaStream_t st = (cudaStream_t)stream;
     // forward operands: fp16 planes (BF16 = false)
     if (npl == 1)
-        return launch_conv_fmt<TC_GATED, 2, 64, 64, false, 1>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
-    return launch_conv_fmt<TC_GATED, 2, 64, 32, false, 2>(maps, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
+        return launch_conv_fmt<TC_GATED, 2, 64, 64, false, 1>(maps, om, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
+    return launch_conv_fmt<TC_GATED, 2, 64, 32, false, 2>(maps, om, p, t_tiles, C / 64, B, st, "tc_convblock_fwd");
 }
 
 // Generic conv / data-gradient:  out (B, Nc, T) fp32 = sum_j A[b, t+off_j, :] . W[j, n, :]  (+ epilogue)
@@ -645,20 +786,23 @@ int dv3_tc_conv(const void* a, const void* w, int npl, float* out, int B, int Kc
     p.gmain = 1.f + config().tc_gamma * (float)(p.k * p.kb_n * (bk / 16));
     // forward conv: fp16 activation x fp16 weight planes; data gradient: bf16 gradient x bf16 weight planes
     p.operand_bf16 = transpose_taps ? 1 : 0;
+    TcOutMaps om = {};
+    p.tma_out = tma_rows(out, T);
+    if (p.tma_out && encode_tmap_f32_bct(&om.out[0], out, B, Nc, T, br)) return 1;
     const int tiles_y = (Nc + br - 1) / br;
     if (npl == 1) {
         if (narrow) {
-            if (k64) return launch_conv<TC_CONV, 1, 64, 64, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
-            return launch_conv<TC_CONV, 1, 64, 32, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
+            if (k64) return launch_conv<TC_CONV, 1, 64, 64, 1>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
+            return launch_conv<TC_CONV, 1, 64, 32, 1>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
         }
-        if (k64) return launch_conv<TC_CONV, 1, 128, 64, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128,bk64)");
-        return launch_conv<TC_CONV, 1, 128, 32, 1>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
+        if (k64) return launch_conv<TC_CONV, 1, 128, 64, 1>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(128,bk64)");
+        return launch_conv<TC_CONV, 1, 128, 32, 1>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
     }
     if (narrow) {
-        if (k64) return launch_conv<TC_CONV, 1, 64, 64>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
-        return launch_conv<TC_CONV, 1, 64, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
+        if (k64) return launch_conv<TC_CONV, 1, 64, 64>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(64)");
+        return launch_conv<TC_CONV, 1, 64, 32>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(64,bk32)");
     }
-    return launch_conv<TC_CONV, 1, 128, 32>(maps, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
+    return launch_conv<TC_CONV, 1, 128, 32>(maps, om, p, t_tiles, tiles_y, B, st, "tc_conv(128)");
 }
 
 // Split count of the weight gradient, chosen for the persistent grid.  A candidate is a batch range of
