@@ -361,18 +361,18 @@ def _host_ints(values, n, name, what):
     return values
 
 
-def resample_batch(wav, lengths, sr_from):
-    """Resample a ragged batch from ``sr_from`` to ``hparams.sample_rate`` in one launch: wav (nclips, pitch) int16 PCM
-    (read as x / 32768, like ``load_wav``) or fp32 CUDA tensor, clip c valid for its first lengths[c] samples (host
-    sequence).  -> (out (nclips, pitch_out) fp32 with clip c's ``resampled_length`` samples and zeros after them, the
-    output lengths as a list).  Each output sample is scipy's ``resample_poly`` of the fp64 clip rounded to fp32
-    (csrc/resample.cu), bit-identical whatever else is in the batch."""
+def resample_batch(wav, lengths, sr_from, sr_to=None):
+    """Resample a ragged batch from ``sr_from`` to ``sr_to`` (``hparams.sample_rate`` by default) in one launch: wav
+    (nclips, pitch) int16 PCM (read as x / 32768, like ``load_wav``) or fp32 CUDA tensor, clip c valid for its first
+    lengths[c] samples (host sequence).  -> (out (nclips, pitch_out) fp32 with clip c's ``resampled_length`` samples and
+    zeros after them, the output lengths as a list).  Each output sample is scipy's ``resample_poly`` of the fp64 clip
+    rounded to fp32 (csrc/resample.cu), bit-identical whatever else is in the batch."""
     wav = _pcm_batch(wav, "resample_batch")
     nclips, pitch = wav.shape
     lengths = _host_ints(lengths, nclips, "resample_batch", "lengths")
     if not all(0 <= n <= pitch for n in lengths):
         raise Dv3Error("resample_batch: lengths must lie in 0..%d" % pitch)
-    up, down = resample_ratio(sr_from)
+    up, down = resample_ratio(sr_from, sr_to)
     out_lens = [resampled_length(n, up, down) for n in lengths]
     pitch_out = max(4, (max(out_lens) + 3) // 4 * 4)
     if pitch_out >= 2 ** 31:

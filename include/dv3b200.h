@@ -726,6 +726,38 @@ int dv3_mas_forward(const float* A, long long stride_b, long long stride_t, cons
 int dv3_mas_backtrace(const int* steps, const int* tokens, int B, int L_max, const long long* dir_off,
                       const unsigned* dirs, int* durations, void* stream);
 
+/* ---- intelligibility: STOI and ESTOI of clips at 10 kHz (stoi.cu, DESIGN.md section 2.20) ----
+ * clips: int64 rows (wav_off, n, frame_off, ola_off, mask_clip), one per clip: n samples at wav + wav_off, with
+ * F0 = len(range(0, n - 256, 128)) frames whose per-frame slots start at frame_off (energy, keep, kept_idx; the band
+ * envelopes at env + 15 frame_off, band i frame t at i F0 + t; the features at feat + 15 frame_off, frame t band i at
+ * 15 t + i); its compacted signal takes (F0 - 1) 128 + 256 floats (0 when F0 = 0) from ola + ola_off on; it uses the
+ * keep mask of clip mask_clip, which must have the same n.
+ * dv3_stoi_frames: one CTA per clip: energy (fp64 dB) and keep (0 / 1) of every frame, kept_idx = the kept frames in
+ * order, kept[c] = their count.  win: the 256 fp64 window values.  n_clips <= 65535.
+ * dv3_stoi_overlap_add: the mask clip's kept frames of each clip, windowed by the first 256 floats of table and
+ * overlap-added at hop 128 into its compacted signal; frames[c] = max(kept[mask_clip] - 1, 0).  max_samples: the
+ * largest compacted capacity of any clip.
+ * dv3_stoi_bands: blocks: int32 (clip, t0) rows, one per CTA of 8 frames t0 .. t0 + 7 (those < frames[clip] are done).
+ * table: the fft_any.cuh table of N = 512 (3 * 512 + 2 floats) whose window is the 256-point one followed by 256 zeros;
+ * bands: int32 lo[15] then hi[15], band i summing bins [lo_i, hi_i) < 256.  env: X[i, t]; feat: null, or
+ * 10 log10(max(X^2, 1e-10)).  n_blocks = 0 launches nothing.
+ * dv3_stoi_segments: pairs: int64 rows (clean clip, processed clip, path_off, seg_off); pair p has steps[p] path
+ * steps, int32 (i, j) frame pairs at path + 2 path_off, and max(steps[p] - 29, 0) segments whose (stoi band sum,
+ * estoi) fp64 values go to seg + 2 seg_off.  blocks: int32 (pair, s0) rows, one per CTA of 4 segments s0 .. s0 + 3.
+ * Then result[2p] = STOI, result[2p + 1] = ESTOI (NaN without segments), counts[2p] = segments, counts[2p + 1] =
+ * kept[clean clip].  n_blocks = 0 runs the second launch alone.
+ * Every sum has a fixed order and there are no atomics: a pair's results depend on its own clips alone. */
+int dv3_stoi_frames(const float* wav, const long long* clips, int n_clips, const double* win, double* energy, int* keep,
+                    int* kept_idx, int* kept, void* stream);
+int dv3_stoi_overlap_add(const float* wav, const long long* clips, int n_clips, long long max_samples,
+                         const float* table, const int* kept_idx, const int* kept, float* ola, int* frames,
+                         void* stream);
+int dv3_stoi_bands(const float* ola, const long long* clips, const int* blocks, int n_blocks, const float* table,
+                   const int* bands, const int* frames, float* env, float* feat, void* stream);
+int dv3_stoi_segments(const float* env, const long long* clips, const long long* pairs, int n_pairs, const int* blocks,
+                      int n_blocks, const int* path, const int* steps, const int* kept, double* seg, double* result,
+                      int* counts, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
