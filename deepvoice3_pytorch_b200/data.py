@@ -694,3 +694,64 @@ class SpeakerSampleBatches:
                     mels[b, j] = mel[o:o + self.T_crop]
             yield {"mels": torch.from_numpy(mels), "speaker_ids": torch.tensor(spk, dtype=torch.int64),
                    "items": torch.from_numpy(items.astype(np.int64)), "offsets": torch.from_numpy(offsets)}
+
+
+class RecognizerBatches:
+    """Training batches of the token recognizer (recognition.TokenRecognizerStep) over any dataset whose items are
+    (tokens, mel (T, num_mels), ...), such as ``TrainTxtDataset``: utterances with at most T_max frames and L_max
+    tokens, drawn without replacement, each batch padded with zeros to the one shape (B, T_max) / (B, L_max) that the
+    step's CUDA graph takes.  Iterating yields {"mels": (B, T_max, num_mels) float32, "mel_lengths": (B,) int32,
+    "tokens": (B, L_max) int64, "token_lengths": (B,) int32, "items": (B,) dataset indices}, len(self) batches per
+    epoch.  The draws are a function of (seed, epoch) alone; ``set_epoch`` moves to another epoch.  Lengths come from
+    ``frame_lengths`` and the text column of a ``TrainTxtDataset`` without loading its mels, from the items otherwise.
+    ValueError when fewer than B utterances qualify.
+
+    The batches carry no length scope: in training, a row's last few frames see the padded neighbour activations of
+    the deeper layers within the receptive field (DESIGN.md section 2.21)."""
+
+    def __init__(self, dataset, B, T_max, L_max, seed=0):
+        if B < 1 or T_max < 1 or L_max < 1:
+            raise ValueError("B=%d, T_max=%d, L_max=%d must be >= 1" % (B, T_max, L_max))
+        self.dataset, self.B, self.T_max, self.L_max, self.seed = dataset, int(B), int(T_max), int(L_max), int(seed)
+        self.eligible = [i for i in range(len(dataset)) if self._frames(i) <= T_max and self._tokens(i) <= L_max]
+        if len(self.eligible) < B:
+            raise ValueError("%d utterances have <= %d frames and <= %d tokens; a batch needs %d"
+                             % (len(self.eligible), T_max, L_max, B))
+        self.epoch = 0
+
+    def _frames(self, i):
+        fl = getattr(self.dataset, "frame_lengths", None)
+        return int(fl[i]) if fl is not None else int(np.asarray(self.dataset[i][1]).shape[0])
+
+    def _tokens(self, i):
+        ds = self.dataset
+        if hasattr(ds, "rows") and hasattr(ds, "text_to_sequence"):
+            return len(ds.text_to_sequence(ds.rows[i][3]))
+        return int(np.asarray(ds[i][0]).size)
+
+    def set_epoch(self, epoch):
+        self.epoch = int(epoch)
+
+    def __len__(self):
+        return len(self.eligible) // self.B
+
+    def __iter__(self):
+        rng = np.random.default_rng([self.seed, self.epoch])
+        order = rng.permutation(len(self.eligible))
+        for k in range(len(self)):
+            items = [self.eligible[j] for j in order[k * self.B:(k + 1) * self.B]]
+            mels, toks = None, np.zeros((self.B, self.L_max), np.int64)
+            ml, tl = np.zeros(self.B, np.int32), np.zeros(self.B, np.int32)
+            for b, i in enumerate(items):
+                item = self.dataset[i]
+                tok, mel = np.asarray(item[0]), np.asarray(item[1], np.float32)
+                if mel.ndim != 2 or mel.shape[0] > self.T_max or tok.size > self.L_max:
+                    raise ValueError("item %d: mel %s and %d tokens, expected (<= %d, num_mels) and <= %d"
+                                     % (i, mel.shape, tok.size, self.T_max, self.L_max))
+                if mels is None:
+                    mels = np.zeros((self.B, self.T_max, mel.shape[1]), np.float32)
+                mels[b, :mel.shape[0]] = mel
+                toks[b, :tok.size] = tok
+                ml[b], tl[b] = mel.shape[0], tok.size
+            yield {"mels": torch.from_numpy(mels), "mel_lengths": torch.from_numpy(ml), "tokens": torch.from_numpy(toks),
+                   "token_lengths": torch.from_numpy(tl), "items": torch.tensor(items, dtype=torch.int64)}

@@ -319,9 +319,11 @@ class ArenaGraphStep:
     ``ops.deterministic`` modes current at construction, one batch shape, checkpoints of copies that resume bit-exactly,
     and with use_graph one CUDA graph for forward, backward and update.  A subclass defines ``_objective(batch)`` (the
     loss to minimise, on device tensors), ``_check_batch(batch)`` (ValueError before any launch) and may define
-    ``_graph_key()`` (when it changes, the next step captures a new graph)."""
+    ``_graph_key()`` (when it changes, the next step captures a new graph).  ``step`` reads the batch keys
+    ``_batch_keys``."""
 
     _net_key = "net"
+    _batch_keys = ("mels", "speaker_ids")
 
     def __init__(self, net, lr, betas, eps, clip_thresh, use_graph):
         from .train_step import FlatAdam, ParameterArena
@@ -373,7 +375,7 @@ class ArenaGraphStep:
             raise ValueError("%s was built with ops.conv_math = %r and cannot step under %r"
                              % (name, self.math, ops.conv_math))
         dev = self.arena.flat.device
-        batch = {k: batch[k] for k in ("mels", "speaker_ids")}
+        batch = {k: batch[k] for k in self._batch_keys}
         self._check_batch(batch)
         shape = tuple(tuple(v.shape) for v in batch.values())
         if self._shape is not None and shape != self._shape:

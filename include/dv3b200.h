@@ -758,6 +758,40 @@ int dv3_stoi_segments(const float* env, const long long* clips, const long long*
                       int n_blocks, const int* path, const int* steps, const int* kept, double* seg, double* result,
                       int* counts, void* stream);
 
+/* ---- token recognition: CTC loss and gradient, greedy CTC decoding, edit distance (ctc.cu, DESIGN.md section 2.21) ----
+ * Logits z[b*stride_b + v*stride_v + t] of B rows, V classes (2 <= V <= dv3_ctc_max_vocab() = 1024) and T frames
+ * (stride_v >= T; rows do not overlap).  Class 0 is the CTC blank.  Row b has frames[b] in [1, T] frames and
+ * target_lengths[b] in [0, L] int32 targets in [1, V) at targets[b*tgt_stride + k]; 1 <= L <= 1024; B*V*T < 2^31.
+ * dv3_ctc_ws_bytes: the workspace of dv3_ctc_fwd / dv3_ctc_bwd (0 for arguments out of range).
+ * dv3_ctc_fwd: lse[b, t] = the fp64 log-sum-exp of z over V, then the fp64 alpha recursion (one CTA per row, one
+ * barrier per frame) -> nll[b] = -log p_b and partials[b] = -log p_b / max(L_b, 1) (fp32).  A row without a feasible
+ * path (frames < L_b + repeated adjacent labels, or log p = -inf) gets nll = partials = 0 and infeasible[b] = 1
+ * (0 otherwise).  A length or target id out of range sets *err_flag = 1 and leaves the row out the same way.
+ * dv3_ctc_bwd: dz (B, V, T) dense = d_loss[0] * scale / max(L_b, 1) * (softmax(z[b, :, t]) - the state occupancies
+ * of class v) for t < frames[b], 0 past it and for every row the forward left out; ws as dv3_ctc_fwd left it.
+ * dv3_ctc_greedy: hyps (B, T) int32 dense: row b's first hyp_lengths[b] entries are the per-frame argmax classes (ties
+ * to the lowest index) over t < frames[b] with repeats collapsed and blanks dropped.
+ * dv3_edit_ws_ints: the int32 workspace of dv3_edit_distance for P pairs of hypotheses up to M_max tokens.
+ * dv3_edit_distance: pair p compares hyp[p*hyp_stride + j], j < hyp_len[p] <= M_max <= 65535, with reference
+ * ref[p*ref_stride + i], i < ref_len[p] <= N_max <= 1024 -> out[4p..4p+3] = (Levenshtein distance, substitutions,
+ * deletions, insertions) along the path whose ties prefer the diagonal, then the deletion, then the insertion.
+ * One warp per pair.  Every entry point: no atomics, fixed summation orders, a row's or pair's results depend on its
+ * own data alone. */
+int dv3_ctc_max_vocab(void);
+long long dv3_ctc_ws_bytes(int B, int T, int L);
+int dv3_ctc_fwd(const float* z, long long stride_b, long long stride_v, const int* frames, const int* targets,
+                long long tgt_stride, const int* target_lengths, int B, int V, int T, int L, void* ws, float* nll,
+                float* partials, int* infeasible, int* err_flag, void* stream);
+int dv3_ctc_bwd(const float* z, long long stride_b, long long stride_v, const int* frames, const int* targets,
+                long long tgt_stride, const int* target_lengths, int B, int V, int T, int L, const void* ws,
+                const float* d_loss, float scale, float* dz, void* stream);
+int dv3_ctc_greedy(const float* z, long long stride_b, long long stride_v, const int* frames, int B, int V, int T,
+                   int* hyps, int* hyp_lengths, int* err_flag, void* stream);
+long long dv3_edit_ws_ints(int P, int M_max);
+int dv3_edit_distance(const int* hyp, long long hyp_stride, const int* hyp_len, const int* ref, long long ref_stride,
+                      const int* ref_len, int P, int M_max, int N_max, int* ws, int* out, int* err_flag,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
