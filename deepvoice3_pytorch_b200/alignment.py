@@ -191,7 +191,8 @@ def attention_errors(argmax, max, coverage, steps, max_decoder_steps, skip_cover
 _THRESHOLDS = ("skip_coverage", "repeat_margin")
 
 
-def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None, **thresholds):
+def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None, durations=None, speed=1.0,
+                       **thresholds):
     """Attention errors of a model's synthesis, in one call:
 
     1. encode and decode every ``sequences[k]`` (in voice ``speaker_ids[k]`` for a multi-speaker model) in padded
@@ -206,7 +207,10 @@ def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_
 
     Every row's alignment is the one ``tts_batch`` returns for it.  Inputs are checked as ``tts_batch`` checks them
     (ValueError before any launch for malformed sequences or speaker ids, batch_size < 1, sequences longer than 1024
-    tokens, unknown or malformed thresholds)."""
+    tokens, unknown or malformed thresholds).  durations, speed: score duration-guided synthesis, as ``tts_batch``
+    runs it; "steps" are then the durations' totals and no utterance counts as a stop failure (each stops at its
+    prescribed total by construction)."""
+    from .duration import guided_durations
     unknown = sorted(set(thresholds) - set(_THRESHOLDS))
     if unknown:
         raise ValueError("unknown thresholds %s (known: %s)" % (unknown, ", ".join(_THRESHOLDS)))
@@ -216,6 +220,7 @@ def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_
             raise ValueError("speaker ids %s outside [0, %d)" % (bad, model.n_speakers))
     max_steps = model.seq2seq.decoder.max_decoder_steps
     attention_errors([np.zeros(1, np.int64)], [np.zeros(1)], [np.zeros(1)], [1], max_steps, **thresholds)   # checks
+    durs = guided_durations(model, sequences, durations, speed)
     seqs, speaker_ids = synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     if max(s.size for s in seqs) > MAX_TOKENS:
         raise ValueError("a sequence has %d tokens, more than %d" % (max(s.size for s in seqs), MAX_TOKENS))
@@ -225,7 +230,8 @@ def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_
     for c in range(0, len(order), int(batch_size)):
         idx = order[c:c + int(batch_size)]
         ids = None if speaker_ids is None else [speaker_ids[i] for i in idx]
-        _, aligns, _, steps, _ = synthesis._decode_chunk(model, [seqs[i] for i in idx], ids, stage)
+        _, aligns, _, steps, _ = synthesis._decode_chunk(model, [seqs[i] for i in idx], ids, stage,
+                                                         None if durs is None else [durs[i] for i in idx])
         tokens = [seqs[i].size for i in idx]
         with stage("mas"):
             out = _mas_result(_mas(aligns, steps, tokens), steps, tokens)
@@ -235,6 +241,8 @@ def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_
     steps = np.array([r[0] for r in res], np.int64)
     err = attention_errors([r[3] for r in res], [r[4] for r in res], [r[5] for r in res], steps, max_steps,
                            **thresholds)
+    if durs is not None:
+        err["stop_failed"][:] = False
     err.update({"steps": steps, "durations": [r[1] for r in res], "score_per_step": np.array([r[2] for r in res]),
                 "total_skips": int(err["skips"].sum()), "total_repeats": int(err["repeats"].sum()),
                 "total_unreached": int(err["unreached"].sum()), "stop_failures": int(err["stop_failed"].sum()),

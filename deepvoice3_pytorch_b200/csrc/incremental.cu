@@ -169,8 +169,11 @@ __global__ void __launch_bounds__(256) inc_conv_step_kernel(const __grid_constan
 // ROWS (ragged batch): row b sees only its own Ts = text_len[b] keys (the key pitch stays p.Ts) and keeps its own
 // cursor; with Ts substituted, the arithmetic is that of the single-row launch, so each row matches it bit for bit.
 // SLOTS (with ROWS): row b runs at its own step t_ptr[b] -- alignment row and cursor parity follow it.
-template <bool ROWS, bool SLOTS>
-__global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constant__ Dv3IncAttn p, const int* text_len) {
+// PATH (with ROWS): guided attention -- the window's centre is the prescribed token path[b*path_ld + t] instead of the
+// previous step's argmax, and no cursor is written; everything else is the ROWS arithmetic.
+template <bool ROWS, bool SLOTS, bool PATH>
+__global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constant__ Dv3IncAttn p, const int* text_len,
+                                                            const int* path, long long path_ld) {
     pdl_trigger(); pdl_wait();     // programmatic dependent launch: see common.cuh
     extern __shared__ float sm[];  // all of it dynamic, so the host's size check is the whole budget
     float* red = sm;               // [kAttnScratch]: 8 per-warp partials + the broadcast slot red[8]
@@ -186,8 +189,8 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
     for (int e = tid; e < p.E; e += 256) q[e] = p.q[b * p.q_ld + e];
     __syncthreads();
     int lo = 0, hi = Ts;                                    // unmasked key range
-    if (p.last_attended) {
-        const int la = p.last_attended[cur_rd];
+    if (PATH || p.last_attended) {
+        const int la = PATH ? path[b * path_ld + t] : p.last_attended[cur_rd];
         const int backward = la - p.window_backward;
         if (backward > 0) lo = backward;
         const int ahead = la + p.window_ahead;
@@ -226,7 +229,7 @@ __global__ void __launch_bounds__(256) inc_attn_step_kernel(const __grid_constan
     if (ROWS && p.align)
         for (int s = Ts + tid; s < p.Ts; s += 256) p.align[b * p.align_ld + t * p.align_t + s] = 0.f;
     __syncthreads();
-    if (p.last_attended && (ROWS || b == 0) && tid == 0) {  // reference: alignment.max(-1)[1] of batch row 0
+    if (!PATH && p.last_attended && (ROWS || b == 0) && tid == 0) {  // reference: alignment.max(-1)[1] of batch row 0
         int best = 0; float bv = sc[0];
         for (int s = 1; s < Ts; ++s) if (sc[s] > bv) { bv = sc[s]; best = s; }
         p.last_attended[cur_wr] = best;
@@ -261,6 +264,14 @@ __global__ void inc_stop_rows_kernel(const float* done, long long done_ld, const
         const int n = t[b] + 1;
         if ((done[b * done_ld + t[b]] > 0.5f && n > min_steps) || n > max_steps) stop[b] = n;
     }
+}
+
+// guided decoding: row b stops once t[b] + 1 reaches its prescribed step count total[b]; the done flag plays no part.
+// Rows that are idle (stop[b] = -1) or stopped keep their value.  Written once.
+__global__ void inc_stop_rows_total_kernel(const int* t, int* stop, const int* total, int B) {
+    pdl_trigger(); pdl_wait();
+    for (int b = threadIdx.x; b < B; b += blockDim.x)
+        if (stop[b] == 0 && t[b] + 1 >= total[b]) stop[b] = t[b] + 1;
 }
 
 // entry e, slot list index i: row slots[i] of e.dst <- row i of e.src (zeros when e.src is NULL), in 4-byte words
@@ -320,7 +331,8 @@ int dv3_inc_attn_step(const Dv3IncAttn* p, void* stream) {
     const size_t smem = attn_smem(p);
     DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
                 p->E + p->Ts, kAttnMaxKeys);
-    launch_k(inc_attn_step_kernel<false, false>, p->B, 256, smem, (cudaStream_t)stream, *p, (const int*)nullptr);
+    launch_k(inc_attn_step_kernel<false, false, false>, p->B, 256, smem, (cudaStream_t)stream, *p, (const int*)nullptr,
+             (const int*)nullptr, 0LL);
     return check_launch("inc_attn_step");
 }
 
@@ -329,7 +341,8 @@ int dv3_inc_attn_step_rows(const Dv3IncAttn* p, const int* text_len, void* strea
     const size_t smem = attn_smem(p);
     DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_rows: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
                 p->E + p->Ts, kAttnMaxKeys);
-    launch_k(inc_attn_step_kernel<true, false>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
+    launch_k(inc_attn_step_kernel<true, false, false>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len,
+             (const int*)nullptr, 0LL);
     return check_launch("inc_attn_step_rows");
 }
 
@@ -338,8 +351,34 @@ int dv3_inc_attn_step_slots(const Dv3IncAttn* p, const int* text_len, void* stre
     const size_t smem = attn_smem(p);
     DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_slots: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
                 p->E + p->Ts, kAttnMaxKeys);
-    launch_k(inc_attn_step_kernel<true, true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len);
+    launch_k(inc_attn_step_kernel<true, true, false>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len,
+             (const int*)nullptr, 0LL);
     return check_launch("inc_attn_step_slots");
+}
+
+int dv3_inc_attn_step_path(const Dv3IncAttn* p, const int* text_len, const int* path, long long path_ld,
+                           void* stream) {
+    DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0 && text_len && path && path_ld >= 1,
+                "inc_attn_step_path: bad shape");
+    const size_t smem = attn_smem(p);
+    DV3_REQUIRE(smem <= 48 * 1024, "inc_attn_step_path: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
+                p->E + p->Ts, kAttnMaxKeys);
+    launch_k(inc_attn_step_kernel<true, false, true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len, path,
+             path_ld);
+    return check_launch("inc_attn_step_path");
+}
+
+int dv3_inc_attn_step_slots_path(const Dv3IncAttn* p, const int* text_len, const int* path, long long path_ld,
+                                 void* stream) {
+    DV3_REQUIRE(p && p->B > 0 && p->E > 0 && p->Ts > 0 && text_len && p->t_ptr && path && path_ld >= 1,
+                "inc_attn_step_slots_path: bad shape");
+    const size_t smem = attn_smem(p);
+    DV3_REQUIRE(smem <= 48 * 1024,
+                "inc_attn_step_slots_path: E + Ts = %d floats exceed the %d that fit in 48 KB of shared memory",
+                p->E + p->Ts, kAttnMaxKeys);
+    launch_k(inc_attn_step_kernel<true, true, true>, p->B, 256, smem, (cudaStream_t)stream, *p, text_len, path,
+             path_ld);
+    return check_launch("inc_attn_step_slots_path");
 }
 
 int dv3_inc_advance(int* t_ptr, void* stream) {
@@ -358,6 +397,12 @@ int dv3_inc_stop_rows(const float* done, long long done_ld, const int* t, int* s
     DV3_REQUIRE(done && t && stop && B > 0 && B <= 1024 && done_ld > max_steps, "inc_stop_rows: bad shape");
     launch_k(inc_stop_rows_kernel, 1, B, 0, (cudaStream_t)stream, done, done_ld, t, stop, B, min_steps, max_steps);
     return check_launch("inc_stop_rows");
+}
+
+int dv3_inc_stop_rows_total(const int* t, int* stop, const int* total, int B, void* stream) {
+    DV3_REQUIRE(t && stop && total && B > 0 && B <= 1024, "inc_stop_rows_total: bad shape (B = %d)", B);
+    launch_k(inc_stop_rows_total_kernel, 1, B, 0, (cudaStream_t)stream, t, stop, total, B);
+    return check_launch("inc_stop_rows_total");
 }
 
 int dv3_inc_refill(const Dv3IncRefill* table, int n_entries, const int* slots, int n_slots, void* stream) {

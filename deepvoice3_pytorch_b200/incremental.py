@@ -20,11 +20,16 @@ every row gets what ``decode`` gives for that row on its own, bit for bit (every
 ``decode_stream`` is continuous batching (``synthesis.tts_stream``): a fixed set of decoder slots, each with its own
 step counter; when a slot's utterance stops (the stop rule runs on the device, per row), the host gathers it at the next
 check and one ``dv3_inc_refill`` launch resets the slot and loads the next waiting utterance into it.
+
+Both take per-token durations (DESIGN.md section 2.22): guided decoding centres every attention layer's window on a
+prescribed token path (token j for steps S_j <= t < S_{j+1}, S_j the sum of the first j durations) instead of on the
+previous argmax, and stops each row after exactly its total of steps.
 """
 import contextlib
 import ctypes
 import os
 
+import numpy as np
 import torch
 from torch import nn
 
@@ -97,6 +102,7 @@ class StepProgram:
         self.t = torch.zeros(B if slots else 1, dtype=torch.int32, device=device)
         self.rings, self.cursors = [], []   # the per-row history a new utterance starts from zero
         self.stop = None                    # slots: int32 (B,) stop steps, 0 while the row runs
+        self.total = None                   # guided slots: int32 (B,) prescribed step counts (the stop rule)
         self.graph = None
 
     def buf(self, *shape):
@@ -149,8 +155,9 @@ class StepProgram:
         return la
 
     def attention(self, q, keys_bet, values_bte, ctx, align, align_scale, last_attended, window_backward, window_ahead,
-                  text_len=None):
-        """text_len: int32 (B,) device tensor -> the per-row (ragged) step, last_attended then holds [2][B] cursors."""
+                  text_len=None, path=None):
+        """text_len: int32 (B,) device tensor -> the per-row (ragged) step, last_attended then holds [2][B] cursors.
+        path: int32 (B, n) device tensor -> the guided step: row b's window centre at step t is path[b, t]."""
         a = Dv3IncAttn()
         B, E, Ts = keys_bet.shape
         a.q, a.q_ld = q.ptr, q.ld
@@ -164,7 +171,13 @@ class StepProgram:
         a.align_scale = align_scale
         a.B, a.E, a.Ts, a.window_backward, a.window_ahead = B, E, Ts, window_backward, window_ahead
         self.keep += [keys_bet, values_bte]
-        if text_len is None:
+        if path is not None:
+            assert text_len is not None and last_attended is None and path.dtype == torch.int32
+            self.keep += [text_len, path]
+            name = "dv3_inc_attn_step_slots_path" if self.slots else "dv3_inc_attn_step_path"
+            self.calls.append((name, a, (ctypes.c_void_p(text_len.data_ptr()), ctypes.c_void_p(path.data_ptr()),
+                                         path.stride(0))))
+        elif text_len is None:
             assert not self.slots, "the slot program attends per row: it needs text_len"
             self.calls.append(("dv3_inc_attn_step", a, ()))
         else:
@@ -180,13 +193,24 @@ class StepProgram:
         self._stop_args = (ctypes.c_void_p(dones.data_ptr()), dones.size(1), ctypes.c_void_p(self.t.data_ptr()),
                            ctypes.c_void_p(self.stop.data_ptr()), self.B, min_steps, max_steps)
 
+    def stop_rule_total(self, total):
+        """guided slots: stop row b once it has run total[b] (int32 (B,) device) steps; rows start idle as with
+        ``stop_rule``."""
+        assert self.slots and total.dtype == torch.int32
+        self.stop = torch.full((self.B,), -1, dtype=torch.int32, device=self.dev)
+        self.total = total
+
     # -- execution --------------------------------------------------------------------------------
     def _launch_step(self):
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         for name, s, extra in self.calls:
             lib.call(name, ctypes.byref(s), *extra, st)
         if self.slots:
-            lib.call("dv3_inc_stop_rows", *self._stop_args, st)
+            if self.total is not None:
+                lib.call("dv3_inc_stop_rows_total", ctypes.c_void_p(self.t.data_ptr()),
+                         ctypes.c_void_p(self.stop.data_ptr()), ctypes.c_void_p(self.total.data_ptr()), self.B, st)
+            else:
+                lib.call("dv3_inc_stop_rows", *self._stop_args, st)
             lib.call("dv3_inc_advance_rows", ctypes.c_void_p(self.t.data_ptr()),
                      ctypes.c_void_p(self.stop.data_ptr()), self.B, st)
         else:
@@ -295,18 +319,71 @@ def decode(decoder, encoder_out, text_positions, speaker_embed=None, initial_inp
     return _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph)
 
 
+def check_durations(durations, lengths):
+    """durations: one 1-D integer array (sequence or tensor) per row, of lengths[b] entries each >= 1 -> list of int64
+    arrays.  ValueError otherwise (host values only)."""
+    if not isinstance(durations, (list, tuple)) or len(durations) != len(lengths):
+        raise ValueError("durations must be a list of %d arrays, one per sequence" % len(lengths))
+    out = []
+    for b, (d, n) in enumerate(zip(durations, lengths)):
+        d = np.asarray(d.detach().cpu() if torch.is_tensor(d) else d)
+        if d.ndim != 1 or (d.size and not np.issubdtype(d.dtype, np.integer)):
+            raise ValueError("durations[%d] must be a 1-D integer array, got %s of shape %s" % (b, d.dtype, d.shape))
+        if d.size != int(n):
+            raise ValueError("durations[%d] has %d entries for a sequence of %d tokens" % (b, d.size, int(n)))
+        if d.size and d.min() < 1:
+            raise ValueError("durations[%d] holds a duration below 1 step: %d" % (b, int(d.min())))
+        out.append(d.astype(np.int64))
+    return out
+
+
+def path_table(durations, steps=None):
+    """Per-row durations (int64 arrays, each >= 1) -> (path int64 (B, steps), totals [B]): row b attends token j at
+    steps S_j <= t < S_{j+1} (S_j the sum of its first j durations); past its total S_{L_b} it holds its last token,
+    the step a row that has stopped keeps recomputing.  steps defaults to the largest total."""
+    totals = [int(d.sum()) for d in durations]
+    T = max(totals) if steps is None else int(steps)
+    path = np.empty((len(durations), T), np.int64)
+    for b, d in enumerate(durations):
+        row = np.repeat(np.arange(d.size, dtype=np.int64), d)[:T]
+        path[b, :row.size] = row
+        path[b, row.size:] = d.size - 1
+    return path, totals
+
+
+def query_steps(decoder):
+    """The most decoder steps the query-position table holds: steps t = 0.. read positions t + 1."""
+    return decoder.embed_query_positions.num_embeddings - 1
+
+
 @torch.no_grad()
 def decode_ragged(decoder, encoder_out, text_positions, text_lengths, speaker_embed=None, initial_input=None,
-                  test_inputs=None, use_graph=None):
+                  test_inputs=None, use_graph=None, durations=None):
     """Batched decode of rows with text_lengths (B,) valid keys each (encoder outputs padded to T_text).
     -> outputs (B, N, in_dim*r), alignments (B, N, T_text), dones (B, N), decoder_states (B, N, C), steps [B]:
     row b is valid for its first steps[b] decoder steps (and its first text_lengths[b] alignment columns; the rest are
     0) and there equals ``decode`` run on that row alone with its encoder outputs cut to text_lengths[b].  Free-running,
     row b stops by the reference rule applied to its own done flags; rows that stopped keep computing until the last
     one does, their extra frames are not part of the result.  Teacher-forced (test_inputs (B, N, in_dim*r)), every row
-    runs N steps."""
+    runs N steps.
+
+    durations: guided decoding -- one integer array per row, durations[b] of text_lengths[b] entries >= 1 (in decoder
+    steps).  Every attention layer centres its window on token j of row b for steps S_j <= t < S_{j+1}, and row b runs
+    exactly steps[b] = S_{L_b} steps (the sum of its durations): the done flags are computed and returned but do not
+    stop it, and min / max_decoder_steps do not apply.  ValueError before any launch for malformed durations, a total
+    above the query-position table (``query_steps``) or teacher-forced inputs."""
+    guide = None
+    if durations is not None:
+        if test_inputs is not None:
+            raise ValueError("durations guide a free-running decode; teacher-forced inputs take none")
+        lens = np.asarray(text_lengths.cpu() if torch.is_tensor(text_lengths) else text_lengths).reshape(-1)
+        path, totals = path_table(check_durations(durations, lens))
+        if max(totals) > query_steps(decoder):
+            raise ValueError("durations total %d decoder steps; the query-position table holds %d"
+                             % (max(totals), query_steps(decoder)))
+        guide = (path, totals)
     return _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph,
-                   text_lengths=text_lengths)
+                   text_lengths=text_lengths, guide=guide)
 
 
 def _constants(decoder, keys, values, text_positions, speaker_embed, Tmax):
@@ -342,10 +419,11 @@ def _constants(decoder, keys, values, text_positions, speaker_embed, Tmax):
     return kv, pos_table, addend
 
 
-def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, frames, test_inputs=None):
+def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, frames, test_inputs=None, path=None):
     """Record one decoder step into prog (B rows): input frame t of ``frames`` (B, Tmax + 1, Fr) -- or of test_inputs
     (B, Tmax, Fr) -- to output frame t + 1.  spk_of(f) -> _Rows of GLU block f's speaker addend, or None; text_len:
-    int32 (B,) per-row attention lengths, or None (``decode``).  -> states (B, Tmax, Cs), aligns (B, Tmax, Ts),
+    int32 (B,) per-row attention lengths, or None (``decode``); path: int32 (B, Tmax) guided window centres, or None.
+    -> states (B, Tmax, Cs), aligns (B, Tmax, Ts),
     dones (B, Tmax)."""
     nyanko = hasattr(decoder, "audio_encoder_modules")
     B, Ts = prog.B, kv[0][0].size(2)
@@ -366,7 +444,7 @@ def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, fram
     align_rows = _Rows(aligns, Ts, ld=Tmax * Ts, t=Ts)
 
     def cursor(force):
-        return prog.cursor(text_len is not None) if force else None
+        return prog.cursor(text_len is not None) if force and path is None else None
 
     if nyanko:
         D = C
@@ -378,7 +456,7 @@ def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, fram
         q = prog.conv(q_in, att.query_projection)
         ctx = _Rows(prog.buf(B, E), E)
         prog.attention(q, kv[0][0], kv[0][1], ctx, align_rows, 1.0, cursor(decoder.force_monotonic_attention),
-                       att.window_backward, att.window_ahead, text_len)
+                       att.window_backward, att.window_ahead, text_len, path)
         prog.conv(ctx, att.out_projection, res1=q_in, y=_Rows(cat, D, ld=2 * D))
         cur = _run_stack(prog, decoder.audio_decoder_modules, _Rows(cat, 2 * D), last_y=states_rows)
     else:
@@ -399,7 +477,7 @@ def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, fram
             first = ai == 0
             prog.attention(q, kv[ai][0], kv[ai][1], ctx, align_rows if first else None,
                            float(2 ** (n_att - 1)) / n_att, cursor(decoder.force_monotonic_attention[idx]),
-                           att.window_backward, att.window_ahead, text_len)
+                           att.window_backward, att.window_ahead, text_len, path)
             cur = prog.conv(ctx, att.out_projection, res1=q_in, res2=residual, y=dst)
             ai += 1
     xraw = _Rows(prog.buf(B, Fr), Fr)
@@ -410,7 +488,9 @@ def _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, fram
 
 
 def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, test_inputs, use_graph,
-            text_lengths=None):
+            text_lengths=None, guide=None):
+    """guide: (path int (B, n), steps [B]) -- the guided decode of ``decode_ragged``: the window centres of every step
+    t < n and each row's step count."""
     if decoder.training:
         raise RuntimeError("incremental_forward only supports eval mode")     # reference conv.py:19-20
     if use_graph is None:
@@ -432,10 +512,15 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
     old_math = ops.conv_math
     ops.conv_math = "fp32"                       # one-off set-up GEMMs (projections) in exact fp32
     try:
+        path = None
         if test_inputs is not None:
             test_inputs = test_inputs.to(torch.float32).contiguous()
             assert test_inputs.size(-1) == Fr
             Tmax = test_inputs.size(1)
+        elif guide is not None:
+            assert ragged
+            path = torch.from_numpy(np.ascontiguousarray(guide[0], np.int32)).to(dev)
+            Tmax = path.size(1)
         else:
             Tmax = decoder.max_decoder_steps + 1
         kv, pos_table, addend = _constants(decoder, keys, values, text_positions, speaker_embed, Tmax)
@@ -452,7 +537,7 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
         if initial_input is not None:
             frames[:, 0] = initial_input.reshape(B, Fr)
         states, aligns, dones = _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, frames,
-                                               test_inputs)
+                                               test_inputs, path)
     finally:
         ops.conv_math = old_math
 
@@ -468,6 +553,9 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
     if test_inputs is not None:
         prog.run(Tmax, use_graph)
         steps = [Tmax] * B
+    elif guide is not None:
+        prog.run(Tmax, use_graph)
+        steps = [int(n) for n in guide[1]]
     else:
         steps, done_steps = None, 0
         while steps is None:
@@ -509,7 +597,7 @@ def _reset_entries(prog, frames):
 
 
 @torch.no_grad()
-def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_timer=None):
+def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_timer=None, guided_steps=None):
     """Continuous batching: decode many utterances on a fixed set of ``slots`` decoder rows, refilling a row with the
     next waiting utterance as soon as its own one stops.
 
@@ -524,7 +612,15 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
     device by the reference stop rule), gathers the finished utterances and reloads their slots in one launch.
     stats: optional dict, filled with "replays" (steps of the program), "useful_steps" (sum of N), "slots" and
     "refills" [(replays so far, slots reloaded, slots mid-decode)].  stage_timer: optional ``name -> context
-    manager`` around the decoder work ("decoder"); pulling requests happens outside it."""
+    manager`` around the decoder work ("decoder"); pulling requests happens outside it.
+
+    Guided decoding: requests of six entries, the last one the utterance's durations ((T,) integers >= 1, every
+    request or none).  Each slot then carries its path row and step total (loaded by the same refill), attends as
+    ``decode_ragged(..., durations=...)`` does and stops after exactly N = sum(durations) steps (``dv3_inc_stop_rows_total``);
+    each utterance is what ``decode_ragged`` gives it with those durations.  The program is then sized for
+    ``guided_steps`` steps -- the largest total, when the caller knows it -- or, by default, for the query-position
+    table (``query_steps``); a request whose total exceeds that raises ValueError when it is loaded, and so does a
+    guided_steps outside [1, query_steps]."""
     if decoder.training:
         raise RuntimeError("incremental_forward only supports eval mode")     # reference conv.py:19-20
     S = int(slots)
@@ -554,8 +650,12 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
         raise RuntimeError("incremental decoding runs on the GPU only (no CPU fallback)")
     dev, E = keys0.device, keys0.size(-1)
     multi = first[0][4] is not None
+    guided = len(first[0]) > 5 and first[0][5] is not None
     Tp = decoder.embed_keys_positions.num_embeddings - 1      # the longest text: positions 1..Tp index the table
-    Tmax = decoder.max_decoder_steps + 1
+    if guided and guided_steps is not None and not 1 <= int(guided_steps) <= query_steps(decoder):
+        raise ValueError("guided_steps=%r outside [1, %d]" % (guided_steps, query_steps(decoder)))
+    Tmax = decoder.max_decoder_steps + 1 if not guided else \
+        query_steps(decoder) if guided_steps is None else int(guided_steps)
     Fr = decoder.in_dim * decoder.r
     if stats is not None:
         stats.update(replays=0, useful_steps=0, slots=S, refills=[])
@@ -566,11 +666,12 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
         keys = torch.zeros(G, L, E, device=dev)
         values = torch.zeros(G, L, E, device=dev)
         tpos = torch.zeros(G, L, dtype=torch.long, device=dev)
-        for g, (_, k, v, p, _) in enumerate(reqs):
-            if (k.size(0) > Tp or (reqs[g][4] is not None) != multi or k.shape != v.shape
-                    or p.shape != k.shape[:1]):
-                raise ValueError("request %r: keys / values (T, %d), T <= %d, text_positions (T,) and a speaker "
-                                 "embedding for every request or for none" % (reqs[g][0], E, Tp))
+        for g, r in enumerate(reqs):
+            k, v, p = r[1:4]
+            if (k.size(0) > Tp or (r[4] is not None) != multi or k.shape != v.shape
+                    or p.shape != k.shape[:1] or (len(r) > 5 and r[5] is not None) != guided):
+                raise ValueError("request %r: keys / values (T, %d), T <= %d, text_positions (T,), and a speaker "
+                                 "embedding and durations for every request or for none" % (r[0], E, Tp))
             keys[g, :k.size(0)], values[g, :k.size(0)], tpos[g, :k.size(0)] = k, v, p
         spk = torch.stack([r[4] for r in reqs]) if multi else None
         old_math = ops.conv_math
@@ -590,6 +691,9 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
         kv_slot = [(torch.zeros(S, k.size(1), Tp, device=dev), torch.zeros(S, Tp, v.size(2), device=dev))
                    for k, v in kv0]
         pos_slot = torch.zeros(S, Tmax, pos0.size(-1), device=dev)
+        # guided: each slot's window centres and step total (idle slots: token 0, held at step 0)
+        path_slot = torch.zeros(S, Tmax, dtype=torch.int32, device=dev) if guided else None
+        total_slot = torch.ones(S, dtype=torch.int32, device=dev) if guided else None
 
         def spk_of(f):
             if f.speaker_proj is None or not multi:
@@ -604,11 +708,14 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
         try:
             frames = prog.buf(S, Tmax + 1, Fr)
             states, aligns, dones = _build_program(decoder, prog, Tmax, E, kv_slot, pos_slot, spk_of, text_len,
-                                                   frames)
+                                                   frames, path=path_slot)
         finally:
             ops.conv_math = old_math
         prog.keep += spk_slot
-        prog.stop_rule(dones, decoder.min_decoder_steps, decoder.max_decoder_steps)
+        if guided:
+            prog.stop_rule_total(total_slot)
+        else:
+            prog.stop_rule(dones, decoder.min_decoder_steps, decoder.max_decoder_steps)
 
         # staging: row i holds the constants of the i-th slot of the next refill
         kv_stage = [(torch.zeros_like(k), torch.zeros_like(v)) for k, v in kv_slot]
@@ -620,6 +727,10 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
         for (k, v), (ks, vs) in zip(kv_slot, kv_stage):
             entries += [(k, ks, k[0].numel() * 4, 0), (v, vs, v[0].numel() * 4, 0)]
         entries += [(b, bs, b[0].numel() * 4, 0) for b, bs in zip(spk_slot, spk_stage)]
+        if guided:
+            path_stage, total_stage = torch.zeros_like(path_slot), torch.ones_like(total_slot)
+            entries += [(path_slot, path_stage, Tmax * 4, 0), (total_slot, total_stage, 4, 0)]
+            prog.keep += [path_stage, total_stage]
         table = _refill_table(entries, dev)
         prog.keep += [table, slot_list, kv_stage, pos_stage, len_stage, spk_stage]
 
@@ -631,6 +742,12 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
         reqs = take(len(free))
         if not reqs:
             return []
+        if guided:
+            durs = check_durations([r[5] if len(r) > 5 else None for r in reqs], [r[1].size(0) for r in reqs])
+            path, totals = path_table(durs, Tmax)
+            if max(totals) > Tmax:
+                raise ValueError("request %r: durations total %d decoder steps; the program holds %d"
+                                 % (reqs[int(np.argmax(totals))][0], max(totals), Tmax))
         with stage("decoder"):
             kv, pos, spk = constants(reqs)
             G = len(reqs)
@@ -642,6 +759,9 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
                 ss[:G] = s
             lens = [r[1].size(0) for r in reqs]
             len_stage[:G] = torch.tensor(lens, dtype=torch.int32)
+            if guided:
+                path_stage[:G] = torch.from_numpy(path.astype(np.int32))
+                total_stage[:G] = torch.tensor(totals, dtype=torch.int32)
             slot_list[:G] = torch.tensor(free[:G], dtype=torch.int32)
             st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
             lib.call("dv3_inc_refill", ctypes.c_void_p(table.data_ptr()), len(entries),

@@ -14,6 +14,10 @@ slots, each refilled with the next waiting utterance as soon as its own one stop
 utterance of a chunk is done.  Finished utterances go through the post-net and vocoder in groups and are yielded as
 they complete.
 
+Both take ``durations`` (one integer array per sequence, in decoder steps) and ``speed`` for duration-guided synthesis
+(DESIGN.md section 2.22): every attention layer's window follows the prescribed token path and each utterance runs
+exactly sum(durations) decoder steps; ``speed`` rescales the durations (``duration.scale_durations``).
+
 Every kernel on this path computes a row from that row's data alone, in an order that does not depend on the batch,
 so with ``ops.conv_math = "fp32"`` each result is bit-identical to the one-utterance path.  In the default tensor-core
 mode the batch's larger GEMMs may take the tensor-core kernels where a short single sentence runs on the exact-fp32 ones
@@ -61,18 +65,18 @@ def _check_inputs(model, sequences, speaker_ids, **counts):
 
 
 @torch.no_grad()
-def _synthesize_chunk(model, seqs, speaker_ids, stage, vocoder):
+def _synthesize_chunk(model, seqs, speaker_ids, stage, vocoder, durations=None):
     """seqs: list of int64 arrays -> [(waveform, alignment, spectrogram, mel)] for one padded batch."""
-    outputs, aligns, states, steps, spk = _decode_chunk(model, seqs, speaker_ids, stage)
+    outputs, aligns, states, steps, spk = _decode_chunk(model, seqs, speaker_ids, stage, durations)
     aligns = aligns.cpu().numpy()
     post = _postnet_vocode(model, outputs, states, steps, spk, stage, vocoder)
     return [(w, aligns[b, :steps[b], :s.size], lin, mel) for b, (s, (w, lin, mel)) in enumerate(zip(seqs, post))]
 
 
 @torch.no_grad()
-def _decode_chunk(model, seqs, speaker_ids, stage):
+def _decode_chunk(model, seqs, speaker_ids, stage, durations=None):
     """The encoder and ``incremental.decode_ragged`` of ``tts_batch`` on one padded batch (stages "encoder" and
-    "decoder"): seqs: list of int64 arrays -> (outputs (B, N, in_dim*r), alignments (B, N, T_text) on the device,
+    "decoder"), guided by ``durations`` (one int64 array per row) when given: seqs: list of int64 arrays -> (outputs (B, N, in_dim*r), alignments (B, N, T_text) on the device,
     decoder states (B, N, C), steps [B], speaker embeddings (B, D) or None)."""
     dev = next(model.parameters()).device
     B = len(seqs)
@@ -92,7 +96,8 @@ def _decode_chunk(model, seqs, speaker_ids, stage):
         with stage("encoder"), ops.length_scope(text_len, L):
             keys, values = model.seq2seq.encoder(text, speaker_embed=spk)
         with stage("decoder"):
-            outputs, aligns, _, states, steps = incremental.decode_ragged(dec, (keys, values), tpos, text_len, spk)
+            outputs, aligns, _, states, steps = incremental.decode_ragged(dec, (keys, values), tpos, text_len, spk,
+                                                                          durations=durations)
     finally:
         ops.rng.end_forward()
     return outputs, aligns, states, steps, spk
@@ -123,7 +128,8 @@ def _postnet_vocode(model, outputs, states, steps, spk, stage, vocoder="griffin_
     return [(wavs[b], audio._denormalize(lin_rows[b]), audio._denormalize(mel[b, :steps[b] * r])) for b in range(B)]
 
 
-def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None, vocoder="griffin_lim"):
+def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=None, vocoder="griffin_lim",
+              durations=None, speed=1.0):
     """Synthesize many utterances at once.
 
     model: a ``MultiSpeakerTTSModel`` in eval mode on CUDA.  sequences: list of 1-D token-id arrays (what a text
@@ -138,8 +144,17 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
     stage_timer: optional callable ``name -> context manager`` wrapped around each stage ("encoder", "decoder",
     "converter", "vocoder") of every batch, e.g. to time them.  vocoder: the phase recovery of
     ``audio.inv_spectrogram``, "griffin_lim" (the default), "lws" (the reference's algorithm) or "fast_griffin_lim"
-    (Griffin-Lim with momentum); checked first."""
+    (Griffin-Lim with momentum); checked first.
+
+    durations: duration-guided synthesis -- one integer array per sequence, one entry >= 1 per token, in decoder steps
+    (from ``duration.predict_durations``, from ``alignment.teacher_forced_alignment`` of a recording, or the
+    "durations" of ``alignment.evaluate_attention``); sequence k then runs exactly sum(durations[k]) decoder steps with
+    every attention window on the prescribed token (``incremental.decode_ragged``).  speed: speaking rate, applied to
+    the durations with ``duration.scale_durations``; a speed other than 1 needs durations.  ValueError before any
+    launch for malformed durations or speed, or a total above the query-position table."""
+    from .duration import guided_durations
     audio.check_phase_method(vocoder)
+    durs = guided_durations(model, sequences, durations, speed)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
     order = sorted(range(len(seqs)), key=lambda i: -seqs[i].size)
@@ -147,7 +162,9 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
     for c in range(0, len(order), int(batch_size)):
         idx = order[c:c + int(batch_size)]
         ids = None if speaker_ids is None else [speaker_ids[i] for i in idx]
-        for i, res in zip(idx, _synthesize_chunk(model, [seqs[i] for i in idx], ids, stage, vocoder)):
+        chunk = _synthesize_chunk(model, [seqs[i] for i in idx], ids, stage, vocoder,
+                                  None if durs is None else [durs[i] for i in idx])
+        for i, res in zip(idx, chunk):
             out[i] = res
     return out
 
@@ -192,7 +209,7 @@ def synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, device,
 
 
 def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stage_timer=None, stats=None,
-               vocoder="griffin_lim"):
+               vocoder="griffin_lim", durations=None, speed=1.0):
     """Synthesize many utterances with continuous batching; a generator of (index, (waveform, alignment, spectrogram,
     mel)) in completion order, each item what ``tts_batch`` gives for that sequence (bit for bit in exact-fp32 mode).
 
@@ -200,11 +217,14 @@ def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stag
     decoder is ``incremental.decode_stream`` on ``slots`` rows; finished utterances go through the post-net (inside a
     length scope on their frames) and the vocoder in groups of ``post_batch``, the last partial group when the decoder
     is done.  Inputs are checked as ``tts_batch`` checks them, before the first item.  stage_timer, vocoder: as for
-    ``tts_batch``; stats: a dict ``decode_stream`` fills (decoder occupancy)."""
+    ``tts_batch``; stats: a dict ``decode_stream`` fills (decoder occupancy); durations, speed: duration-guided
+    synthesis as for ``tts_batch`` (each slot then stops after its utterance's total of steps)."""
+    from .duration import guided_durations
     audio.check_phase_method(vocoder)
+    durs = guided_durations(model, sequences, durations, speed)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, slots=slots, post_batch=post_batch)
     stage = stage_timer or (lambda name: contextlib.nullcontext())
-    return _stream(model, seqs, speaker_ids, int(slots), int(post_batch), stage, stats, vocoder)
+    return _stream(model, seqs, speaker_ids, int(slots), int(post_batch), stage, stats, vocoder, durs)
 
 
 @torch.no_grad()
@@ -229,12 +249,13 @@ def _encode(model, idx, seqs, speaker_ids, stage):
             for b, (i, n) in enumerate(zip(idx, lens))]
 
 
-def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats, vocoder="griffin_lim"):
+def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats, vocoder="griffin_lim", durations=None):
     def requests():
         for g in range(0, len(seqs), slots):
             idx = list(range(g, min(g + slots, len(seqs))))
-            yield from _encode(model, idx, [seqs[i] for i in idx],
-                               None if speaker_ids is None else [speaker_ids[i] for i in idx], stage)
+            reqs = _encode(model, idx, [seqs[i] for i in idx],
+                           None if speaker_ids is None else [speaker_ids[i] for i in idx], stage)
+            yield from reqs if durations is None else (r + (durations[r[0]],) for r in reqs)
 
     def flush(group):
         N = max(r[5] for r in group)
@@ -251,7 +272,10 @@ def _stream(model, seqs, speaker_ids, slots, post_batch, stage, stats, vocoder="
 
     vocoder_kw = {} if vocoder == "griffin_lim" else {"vocoder": vocoder}     # the default: the six-argument call
     group = []
-    for r in incremental.decode_stream(model.seq2seq.decoder, slots, requests(), stats=stats, stage_timer=stage):
+    # guided: the program holds the longest total, not the whole query-position table
+    guided_kw = {} if durations is None else {"guided_steps": max(int(d.sum()) for d in durations)}
+    for r in incremental.decode_stream(model.seq2seq.decoder, slots, requests(), stats=stats, stage_timer=stage,
+                                       **guided_kw):
         group.append(r)
         if len(group) == post_batch:
             yield from flush(group)

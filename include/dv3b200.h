@@ -533,6 +533,18 @@ int dv3_inc_attn_step_slots(const Dv3IncAttn* attn, const int* text_len, void* s
  * stop[b] == 0 and (done > 0.5 and n > min_steps, or n > max_steps), stop[b] = n.  done_ld > max_steps. */
 int dv3_inc_stop_rows(const float* done, long long done_ld, const int* t, int* stop, int B, int min_steps,
                       int max_steps, void* stream);
+/* ---- guided decoding (DESIGN.md section 2.22): the attention window's centre follows a prescribed token path ----
+ * The _path variants are dv3_inc_attn_step_rows / dv3_inc_attn_step_slots with the cursor of row b at step t read as
+ * path[b*path_ld + t] (int32, device) instead of from last_attended, which they neither read nor write; the window
+ * [c - window_backward, c + window_ahead) clamped to [0, text_len[b]), the softmax, alignment and context are those
+ * of the _rows step.  path_ld >= the steps the program runs. */
+int dv3_inc_attn_step_path(const Dv3IncAttn* attn, const int* text_len, const int* path, long long path_ld,
+                           void* stream);
+int dv3_inc_attn_step_slots_path(const Dv3IncAttn* attn, const int* text_len, const int* path, long long path_ld,
+                                 void* stream);
+/* The guided stop rule: if stop[b] == 0 and t[b] + 1 >= total[b], stop[b] = t[b] + 1 (total[b] >= 1 steps, set per
+ * utterance); the done flags play no part. */
+int dv3_inc_stop_rows_total(const int* t, int* stop, const int* total, int B, void* stream);
 /* t[b] += 1 for every row with stop[b] == 0 (every row when stop is NULL).  A stopped row keeps its step and so
  * recomputes it bit for bit; the host gathers it and refills the slot. */
 int dv3_inc_advance_rows(int* t, const int* stop, int B, void* stream);
@@ -545,6 +557,20 @@ typedef struct Dv3IncRefill {
 /* table: n_entries Dv3IncRefill in device memory; slots: n_slots slot indices (int32, device).  One launch resets the
  * listed slots (ring rows, cursors, counters, go frame) and loads their next utterances' constants from staging. */
 int dv3_inc_refill(const Dv3IncRefill* table, int n_entries, const int* slots, int n_slots, void* stream);
+
+/* ---- duration predictor loss (duration.cu, DESIGN.md section 2.22) ----
+ * y (B, L) predicted log-durations with row stride y_ld, durations (B, L) int32 target steps with row stride d_ld,
+ * lengths int32 [B]: row b's tokens j < lengths[b] count.  1 <= L <= dv3_duration_max_tokens() = 1024, B <= 65535.
+ * dv3_duration_loss_fwd: row_loss[b] = (1/n_b) sum_j (y - log d)^2 summed in fp64 in token order, then
+ * *loss = fp32((1/B) sum_b row_loss[b]) summed in row order; no atomics.  A row with lengths[b] outside [1, L] or a
+ * duration < 1 among its tokens sets *err_flag and counts 0.
+ * dv3_duration_loss_bwd: dy (B, L) dense = fp32(d_loss[0] * 2 (y - log d) / (n_b B)) for j < n_b, 0 past it and for
+ * the rows the forward counts 0. */
+int dv3_duration_max_tokens(void);
+int dv3_duration_loss_fwd(const float* y, long long y_ld, const int* durations, long long d_ld, const int* lengths,
+                          int B, int L, double* row_loss, float* loss, int* err_flag, void* stream);
+int dv3_duration_loss_bwd(const float* y, long long y_ld, const int* durations, long long d_ld, const int* lengths,
+                          int B, int L, const float* d_loss, float* dy, void* stream);
 
 /* ---- speaker adaptation: embedding gradient of a speaker-conditioned site with its weights frozen (spk_adapt.cu) ----
  * The site's share of d_e[b*S + s] = sum_{t < T_b} m(b,t,s)/(1-p) * sum_c w[c*S + s] * G(b,c,t) * (1 - |y(b,c,t)|)^2
