@@ -62,7 +62,18 @@ def check_geometry(mel=True):
     point calls it before anything is allocated or launched.  ``default`` (1024 / 256) selects the specialised forward
     and LWS kernels (csrc/stft.cu, csrc/lws.cu); Griffin-Lim and the inverse STFT are the same at every frame."""
     hp = hparams
-    N, R = hp.fft_size, hp.hop_size
+    N, R = check_frame(hp.fft_size, hp.hop_size)
+    if mel:
+        if not 0 <= hp.num_mels <= 128:
+            raise Dv3Error("num_mels must lie in [0, 128], got %r" % (hp.num_mels,))
+        if hp.fmax is not None and hp.fmax > hp.sample_rate / 2:
+            raise Dv3Error("fmax %r lies above the Nyquist frequency %r" % (hp.fmax, hp.sample_rate / 2))
+    return Geometry(N, R, N // 2 + 1, N // R, (N, R) == (1024, 256))
+
+
+def check_frame(N, R):
+    """The frame rules of ``check_geometry`` for one (fft_size N, hop_size R) -> (N, R) as ints, or Dv3Error naming the
+    rule it breaks.  Host values only."""
     if int(N) != N or int(R) != R:
         raise Dv3Error("fft_size and hop_size must be integers, got %r / %r" % (N, R))
     N, R = int(N), int(R)
@@ -77,12 +88,7 @@ def check_geometry(mel=True):
     if R < 1 or N % R or not 2 <= N // R <= 8:
         raise Dv3Error("hop_size must divide fft_size with fft_size / hop_size in [2, 8] (an integer overlap: only then "
                        "do the squared windows sum to 1), got %d / %d" % (N, R))
-    if mel:
-        if not 0 <= hp.num_mels <= 128:
-            raise Dv3Error("num_mels must lie in [0, 128], got %r" % (hp.num_mels,))
-        if hp.fmax is not None and hp.fmax > hp.sample_rate / 2:
-            raise Dv3Error("fmax %r lies above the Nyquist frequency %r" % (hp.fmax, hp.sample_rate / 2))
-    return Geometry(N, R, N // 2 + 1, N // R, (N, R) == (1024, 256))
+    return N, R
 
 
 _table_cache = {}
@@ -725,9 +731,22 @@ def lws_batch(mag, n_frames, n_iter=None, init_iters=1):
 PHASE_METHODS = ("griffin_lim", "lws", "fast_griffin_lim")
 
 
+def _is_neural(method):
+    """Whether method is a ``vocoder.NeuralVocoder`` instance; a string never imports the vocoder module."""
+    if isinstance(method, str):
+        return False
+    from .vocoder import NeuralVocoder
+    return isinstance(method, NeuralVocoder)
+
+
 def check_phase_method(method):
-    if method not in PHASE_METHODS:
-        raise ValueError("method must be one of %s, got %r" % (", ".join(PHASE_METHODS), method))
+    """method: one of ``PHASE_METHODS`` or a ``vocoder.NeuralVocoder`` instance, else ValueError."""
+    if isinstance(method, str):
+        if method not in PHASE_METHODS:
+            raise ValueError("method must be one of %s or a NeuralVocoder, got %r" % (", ".join(PHASE_METHODS), method))
+        return method
+    if not _is_neural(method):
+        raise ValueError("method must be one of %s or a NeuralVocoder, got %r" % (", ".join(PHASE_METHODS), method))
     return method
 
 
@@ -759,8 +778,15 @@ def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
     (``method="griffin_lim"``, ``hparams.griffin_lim_iters`` iterations when n_iter is None), ``lws_batch``
     (``method="lws"``, ``hparams.lws_iters``) or ``griffin_lim_batch`` with ``momentum=hparams.griffin_lim_momentum``
     (``method="fast_griffin_lim"``, ``hparams.fast_griffin_lim_iters``).  An unknown method, a negative LWS or fast
-    Griffin-Lim iteration count, or a momentum outside [0, 1) raises ValueError before anything runs."""
+    Griffin-Lim iteration count, or a momentum outside [0, 1) raises ValueError before anything runs.
+
+    A ``vocoder.NeuralVocoder`` instance as ``method`` vocodes the batch with ``method.vocode`` instead (no phase
+    recovery, so passing n_iter with it raises ValueError)."""
     check_phase_method(method)
+    if _is_neural(method):
+        if n_iter is not None:
+            raise ValueError("n_iter is an iteration count of phase recovery; a NeuralVocoder takes none")
+        return method.vocode(spectrograms)
     if method in ("lws", "fast_griffin_lim") and n_iter is not None:
         _check_count("n_iter", n_iter)
     if method == "fast_griffin_lim":

@@ -76,22 +76,27 @@ class Conv1d(_WeightNormed):
 
 
 class ConvTranspose1d(_WeightNormed):
-    """kernel_size=2, stride=2 time upsampler, (B, Cin, T) -> (B, Cout, 2T); weight_v (Cin, Cout, 2),
-    normalised over dim 0 = Cin exactly like weight_norm on nn.ConvTranspose1d (reference modules.py:103-109)."""
+    """Time upsampler with kernel_size == stride = s in [2, 8] and padding 0, (B, Cin, T) -> (B, Cout, s*T); weight_v
+    (Cin, Cout, s), normalised over dim 0 = Cin exactly like weight_norm on nn.ConvTranspose1d (reference
+    modules.py:103-109).  The reference builders use s = 2; the neural vocoder's upsamplers use larger strides."""
 
     def __init__(self, in_channels, out_channels, kernel_size, padding=0, stride=2, init_weight=None,
                  init_bias=None):
         super().__init__()
-        if not (kernel_size == 2 and stride == 2 and padding == 0):
-            raise ValueError("only kernel_size=2, stride=2, padding=0 is supported (all the builders use)")
+        if not (kernel_size == stride and 2 <= stride <= 8 and padding == 0):
+            raise ValueError("only kernel_size == stride in [2, 8] with padding=0 is supported, got kernel_size=%r, "
+                             "stride=%r, padding=%r" % (kernel_size, stride, padding))
         self.in_channels, self.out_channels = in_channels, out_channels
-        self.kernel_size, self.stride, self.padding = (2,), (2,), (0,)
-        w = init_weight if init_weight is not None else torch.zeros(in_channels, out_channels, 2)
+        s = int(stride)
+        self.kernel_size, self.stride, self.padding = (s,), (s,), (0,)
+        w = init_weight if init_weight is not None else torch.zeros(in_channels, out_channels, s)
         b = init_bias if init_bias is not None else torch.zeros(out_channels)
         self._set_params(w, b)
 
     def forward(self, x, extent=None):
-        return ops.conv_transpose1d_k2s2(x, self.weight_v, self.weight_g, self.bias, extent=extent)
+        if self.stride[0] == 2:
+            return ops.conv_transpose1d_k2s2(x, self.weight_v, self.weight_g, self.bias, extent=extent)
+        return ops.conv_transpose1d(x, self.weight_v, self.weight_g, self.bias, self.stride[0], extent=extent)
 
 
 class WNLinear(_WeightNormed):

@@ -105,4 +105,17 @@ int dv3_tc_weightnorm_convt_fwd(const float* v, const float* g, float* inv_norm,
                   "tc_weightnorm_convt_fwd");
 }
 
+// ConvTranspose1d(k=s, stride=s) weight v (Cin, Cout, s), g [Cin], s in [2, 8], as a 1x1 conv with s*Cout rows ordered
+// (j, co): the layouts of dv3_tc_weightnorm_convt_fwd with s taps.
+int dv3_tc_weightnorm_convt_s_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
+                                  void* wbwd, int Cin, int Cout, int stride, void* stream) {
+    DV3_REQUIRE(npl == 1 || npl == 2, "tc_weightnorm_convt_s_fwd: npl must be 1 or 2");
+    DV3_REQUIRE(stride >= 2 && stride <= 8, "tc_weightnorm_convt_s_fwd: stride %d outside [2, 8]", stride);
+    const long long Cinp = (Cin + 7) / 8 * 8, Ksp = ((long long)stride * Cout + 7) / 8 * 8;
+    auto launch = npl == 1 ? weightnorm_launch<FMT_BF16, FMT_F16, 1> : weightnorm_launch<FMT_BF16, FMT_F16, 2>;
+    return launch(v, g, inv_norm, scale, wbwd, Ksp, 1, (long long)Cout, (long long)Cin * Ksp, wfwd, 1, Cinp,
+                  (long long)Cout * Cinp, (long long)stride * Cout * Cinp, Cin, Cout, stride, (cudaStream_t)stream,
+                  "tc_weightnorm_convt_s_fwd");
+}
+
 }  // extern "C"

@@ -755,3 +755,63 @@ class RecognizerBatches:
                 ml[b], tl[b] = mel.shape[0], tok.size
             yield {"mels": torch.from_numpy(mels), "mel_lengths": torch.from_numpy(ml), "tokens": torch.from_numpy(toks),
                    "token_lengths": torch.from_numpy(tl), "items": torch.tensor(items, dtype=torch.int64)}
+
+
+class VocoderBatches:
+    """Training batches of the neural vocoder (``vocoder.NeuralVocoderStep`` through ``vocoder.vocoder_batch``).
+    source: a ``WavDataset`` or a list of 1-D float32 waveforms at ``hparams.sample_rate``.  Each batch draws B
+    utterances with at least ``seg_frames`` frames without replacement, and for each a start frame uniform over the
+    segments of seg_frames frames that fit it.  A ``WavDataset`` must hold whole utterances at ``hparams.sample_rate``
+    (``WavDataset(items)`` / ``from_ljspeech``, whose items are resampled on load): the segment items of
+    ``WavDataset.from_vctk`` carry raw input spans at the file's rate, which this class does not resample, and are
+    refused.  Iterating yields {"pcm": (B, pitch) float32 (int16 PCM read as
+    x / 32768), "lengths": (B,) int32, "starts": (B,) int32, "items": (B,) source indices}, len(self) batches per epoch.
+    The draws are a function of (seed, epoch) alone; ``set_epoch`` moves to another epoch.  ValueError when
+    seg_frames < 1, fewer than B utterances qualify or the source is a segmented WavDataset."""
+
+    def __init__(self, source, B, seg_frames=32, seed=0):
+        from .audio import num_frames_host
+        if int(B) < 1 or int(seg_frames) < 1:
+            raise ValueError("B=%r and seg_frames=%r must be >= 1" % (B, seg_frames))
+        self.source, self.B, self.seg_frames, self.seed = source, int(B), int(seg_frames), int(seed)
+        if isinstance(source, WavDataset):
+            if source._segments is not None:
+                raise ValueError("VocoderBatches takes whole utterances at the training rate; a segmented WavDataset "
+                                 "(WavDataset.from_vctk) holds raw input spans at the file's rate")
+            frames = [int(f) for f in source.frame_lengths]
+        else:
+            frames = [num_frames_host(np.asarray(w).reshape(-1).size) for w in source]
+        self.frames = frames
+        self.eligible = [i for i, f in enumerate(frames) if f >= self.seg_frames]
+        if len(self.eligible) < self.B:
+            raise ValueError("%d utterances have >= %d frames; a batch needs %d"
+                             % (len(self.eligible), self.seg_frames, self.B))
+        self.epoch = 0
+
+    def set_epoch(self, epoch):
+        self.epoch = int(epoch)
+
+    def __len__(self):
+        return len(self.eligible) // self.B
+
+    def _pcm(self, i):
+        if isinstance(self.source, WavDataset):
+            x = np.asarray(self.source[i][1])
+        else:
+            x = np.asarray(self.source[i]).reshape(-1)
+        if x.dtype == np.int16:
+            return x.astype(np.float32) * np.float32(3.0517578125e-05)        # x / 32768, exactly
+        return np.ascontiguousarray(x, dtype=np.float32)
+
+    def __iter__(self):
+        rng = np.random.default_rng([self.seed, self.epoch])
+        order = rng.permutation(len(self.eligible))
+        for k in range(len(self)):
+            items = [self.eligible[j] for j in order[k * self.B:(k + 1) * self.B]]
+            starts = np.array([rng.integers(0, self.frames[i] - self.seg_frames + 1) for i in items], np.int32)
+            wavs = [self._pcm(i) for i in items]
+            pcm = np.zeros((self.B, max(w.size for w in wavs)), np.float32)
+            for b, w in enumerate(wavs):
+                pcm[b, :w.size] = w
+            yield {"pcm": torch.from_numpy(pcm), "lengths": torch.tensor([w.size for w in wavs], dtype=torch.int32),
+                   "starts": torch.from_numpy(starts), "items": torch.tensor(items, dtype=torch.int64)}

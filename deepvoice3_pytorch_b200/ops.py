@@ -219,10 +219,30 @@ _CONV = _Layout(lambda v: tuple(v.shape), "fp32", "tc",
                 lambda M, N, k, tc: (M, N, 0, 1, M * N, k) if tc else (M, N * k, 0, k, 1, 0),
                 lambda b: b, lambda db: db, True)
 # v (Cin, Cout, 2) normalised over Cin; GEMM element (m = (j, co), ci) is v[ci, co, j] on both paths
-_CONVT = _Layout(lambda v: (2 * v.shape[1], v.shape[0], 1), "convt_fp32", "convt_tc",
+_CONVT = _Layout(lambda v: (v.shape[2] * v.shape[1], v.shape[0], 1), "convt_fp32", "convt_tc",
                  lambda M, N, k, tc: (M // 2, 2, 1, M, 0, 0),
                  lambda b: b.repeat(2), lambda db: db if db is None else db[:db.numel() // 2] + db[db.numel() // 2:],
                  False)
+_CONVT_S = {}
+
+
+def _convt_layout(s):
+    """The _CONVT record of a ConvTranspose1d(k = s, stride = s), v (Cin, Cout, s): s*Cout GEMM rows ordered (j, co);
+    the bias gradient adds the s row blocks in j order."""
+    if s == 2:
+        return _CONVT
+    if s not in _CONVT_S:
+        def dbias(db):
+            if db is None:
+                return db
+            parts = db.view(s, -1)
+            out = parts[0].clone()
+            for j in range(1, s):
+                out += parts[j]
+            return out
+        _CONVT_S[s] = _Layout(_CONVT.dims, "convt_fp32", "convt_s_tc", lambda M, N, k, tc: (M // s, s, 1, M, 0, 0),
+                              lambda b: b.repeat(s), dbias, False)
+    return _CONVT_S[s]
 
 
 def _wn_buffers(lay, v, npl):
@@ -248,9 +268,9 @@ def _fold_fp32(v, g, npl, out):
 
 def _fold_convt_fp32(v, g, npl, out):
     w_f, w_b, inv, scale = out
-    Cin, Cout = v.shape[0], v.shape[1]
-    lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cin, Cout, 2,
-             2 * Cout, 1, Cout, 1, Cin, Cout * Cin, _stream())
+    Cin, Cout, s = v.shape
+    lib.call("dv3_weightnorm_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(w_f), _p(w_b), Cin, Cout, s,
+             s * Cout, 1, Cout, 1, Cin, Cout * Cin, _stream())
 
 
 def _fold_tc(v, g, npl, out):
@@ -266,8 +286,15 @@ def _fold_convt_tc(v, g, npl, out):
              v.shape[1], _stream())
 
 
+def _fold_convt_s_tc(v, g, npl, out):
+    inv, wfwd, wbwd, scale = out
+    lib.call("dv3_tc_weightnorm_convt_s_fwd", _p(v), _p(g), _p(inv), _p(scale), _p(wfwd), npl, _p(wbwd), v.shape[0],
+             v.shape[1], v.shape[2], _stream())
+
+
 _FOLDS = {"fp32": (_CONV, _fold_fp32), "tc": (_CONV, _fold_tc),
-          "convt_fp32": (_CONVT, _fold_convt_fp32), "convt_tc": (_CONVT, _fold_convt_tc)}
+          "convt_fp32": (_CONVT, _fold_convt_fp32), "convt_tc": (_CONVT, _fold_convt_tc),
+          "convt_s_tc": (_CONVT, _fold_convt_s_tc)}
 
 
 def _fold(kind, v, g, npl=0, out=None):
@@ -990,6 +1017,44 @@ def conv_transpose1d_k2s2(x, v, g, bias, extent=None):
     by the time interleave.  extent: of x's time axis; the incoming gradient past it (2x in output frames) is taken
     as 0."""
     return _Interleave2Fn.apply(_conv1d(_CONVT, x, v, g, bias, 1, 1, False, False, extent))
+
+
+class _InterleaveFn(torch.autograd.Function):
+    """x (B, s*C, T) with rows ordered (j, c) -> y (B, C, s*T), y[b, c, s*t + j] = x[b, j*C + c, t], s in [3, 8]: the
+    time interleave after the 1x1 conv of a ConvTranspose1d(k=s, stride=s) (s = 2 keeps _Interleave2Fn).  A
+    permutation: its adjoint is its inverse."""
+
+    @staticmethod
+    def forward(ctx, x, s):
+        ctx.s = s
+        return interleave(x, s, 0)
+
+    @staticmethod
+    def backward(ctx, dy):
+        return interleave(_c(dy), ctx.s, 1), None
+
+
+def interleave(x, s, inverse=0):
+    """The stride-s time interleave (B, s*C, T) -> (B, C, s*T) (dv3_interleave), or its inverse with inverse=1."""
+    _chk(x)
+    B, R, T = x.shape
+    C, T = (R, T // s) if inverse else (R // s, T)
+    y = torch.empty((B, s * C, T) if inverse else (B, C, s * T), device=x.device)
+    lib.call("dv3_interleave", _p(x), _p(y), B, C, T, s, inverse, _stream())
+    return y
+
+
+def conv_transpose1d(x, v, g, bias, stride, extent=None):
+    """Weight-normed ConvTranspose1d(k = stride = s), s in [2, 8], v (Cin, Cout, s):
+    y[b,co,s*t+j] = bias[co] + sum_ci x[b,ci,t] w[ci,co,j], w = g*v/||v|| over dim 0 (= Cin).  The 1x1 conv with s*Cout
+    output rows ordered (j,co) followed by the stride-s time interleave; s = 2 is ``conv_transpose1d_k2s2``."""
+    s = int(stride)
+    if s == 2:
+        return conv_transpose1d_k2s2(x, v, g, bias, extent=extent)
+    if not 2 <= s <= 8 or v.dim() != 3 or v.shape[2] != s:
+        raise Dv3Error("conv_transpose1d: stride %d must lie in [2, 8] and equal the kernel size of v %s"
+                       % (s, tuple(v.shape)))
+    return _InterleaveFn.apply(_conv1d(_convt_layout(s), x, v, g, bias, 1, 1, False, False, extent), s)
 
 
 def linear(x, v, g, bias):

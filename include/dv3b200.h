@@ -359,6 +359,10 @@ int dv3_tc_weightnorm_fwd(const float* v, const float* g, float* inv_norm, float
  * wfwd: [npl][2*Cout][Cinp], wbwd: [npl][Cin][pad8(2*Cout)]; npl in {1, 2}. */
 int dv3_tc_weightnorm_convt_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
                                 void* wbwd, int Cin, int Cout, void* stream);
+/* ConvTranspose1d(k=s, stride=s), s in [2, 8]: v (Cin,Cout,s), g [Cin] as a 1x1 conv with s*Cout rows ordered (j,co):
+ * wfwd: [npl][s*Cout][Cinp], wbwd: [npl][Cin][pad8(s*Cout)] (the k = 2 layer keeps dv3_tc_weightnorm_convt_fwd). */
+int dv3_tc_weightnorm_convt_s_fwd(const float* v, const float* g, float* inv_norm, float* scale, void* wfwd, int npl,
+                                  void* wbwd, int Cin, int Cout, int stride, void* stream);
 /* Batched weight norm (csrc/wn_batched.cu): one record per weight-normed conv (v (Cout,Cin,k), g [Cout]); the table
  * lives in DEVICE memory, blk_* are the first block of the record in the batched norm / pack / backward launches
  * (ascending over the table), pack_gx = ceil(Cin*k / 32).  Layouts as dv3_tc_weightnorm_fwd with npl = 2; the
@@ -817,6 +821,37 @@ long long dv3_edit_ws_ints(int P, int M_max);
 int dv3_edit_distance(const int* hyp, long long hyp_stride, const int* hyp_len, const int* ref, long long ref_stride,
                       const int* ref_len, int P, int M_max, int N_max, int* ws, int* out, int* err_flag,
                       void* stream);
+
+/* ---- neural vocoder (vocoder.cu, DESIGN.md section 2.23) ----
+ * Multi-resolution STFT loss, one resolution (n_fft, hop) per dv3_mrstft_loss_fwd call.  spec_y / spec_x: the
+ * (B, max_frames, n_fft/2 + 1) complex half spectra (float2) of the generated and the target waveform, as
+ * dv3_stft_complex_geom writes them; clip c has lengths[c] in [1, n] samples and its first num_frames(lengths[c])
+ * frames count.  ws: dv3_mrstft_ws_doubles(B, max_frames) doubles.  stats (B, 4) fp64 = (sum (A_x - A_y)^2,
+ * sum A_x^2, sum |log A_x - log A_y|, frames * bins) over the clip's frames and bins (x the target), with
+ * A = sqrt(max(re^2 + im^2, 1e-7)), summed in a fixed order without atomics; an invalid length or a non-finite sum
+ * sets *err_flag and stores zeros (the clip then counts 0 in the loss and the gradient).
+ * dv3_mrstft_loss_total: stats (M, B, 4) of M resolutions -> clip_loss[c] (fp64, may be NULL) = (1/M) sum_m
+ * (sqrt(num/den) + lg/count) and *loss = fp32((1/B) sum_c clip_loss[c]).
+ * dv3_mrstft_loss_bwd: dspec (B, max_frames, K) float2 = dL/dX of the generated spectrum for d_loss[0] = dL, every
+ * bin written (0 past a clip's frames); adjoint = 1 writes instead the spectrum whose dv3_istft_geom is dL/dy:
+ * N dL/dX / 2 at 0 < k < N/2, N Re(dL/dX) at k = 0 and N/2.
+ * dv3_vocoder_gather: for each of B rows, cond[b, k, s] = lin[b, starts[b] + s, k] (lin (B, lin_rows, K) as
+ * dv3_stft_mel_geom writes it, frames[b] valid rows) and target[b, u] = fp32(x[p] - preemph x[p-1]) (fp64 arithmetic)
+ * at p = starts[b] hop - (n_fft - hop)/2 + u, u < S hop, x = wav row b (pitch samples, lengths[b] valid), zero outside
+ * the clip.  A start outside [0, frames[b] - S] sets *err_flag and writes zeros for the row.  The spectrogram is
+ * transposed through shared-memory tiles: reads and writes are coalesced.
+ * dv3_interleave: in (B, s*C, T) rows ordered (j, c) -> out (B, C, s*T), out[b,c,s*t+j] = in[b,j*C+c,t], s in
+ * [2, 8]; inverse = 1 undoes it. */
+long long dv3_mrstft_ws_doubles(int B, int max_frames);
+int dv3_mrstft_loss_fwd(const float* spec_y, const float* spec_x, const int* lengths, int n, int B, int max_frames,
+                        int n_fft, int hop, double* ws, double* stats, int* err_flag, void* stream);
+int dv3_mrstft_loss_total(const double* stats, int M, int B, double* clip_loss, float* loss, void* stream);
+int dv3_mrstft_loss_bwd(const float* spec_y, const float* spec_x, const double* stats, int B, int max_frames,
+                        int n_fft, int hop, int M, const float* d_loss, int adjoint, float* dspec, void* stream);
+int dv3_vocoder_gather(const float* lin, int lin_rows, const int* frames, const float* wav, long long pitch,
+                       const int* lengths, const int* starts, int B, int S, int n_fft, int hop, double preemph,
+                       float* cond, float* target, int* err_flag, void* stream);
+int dv3_interleave(const float* in, float* out, int B, int C, int T, int stride, int inverse, void* stream);
 
 #ifdef __cplusplus
 }
