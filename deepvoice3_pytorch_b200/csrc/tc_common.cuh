@@ -52,6 +52,10 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
+// the line holding p into L2 (no register, no shared memory; a hint that never faults on a valid address)
+__device__ __forceinline__ void prefetch_l2(const void* p) {
+    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
+}
 // ---- TMA: 3-D tiled store from shared memory, tracked by the issuing thread's bulk groups ----------------------------
 // Elements of the box outside the tensor's extent are not written.  Generic-proxy writes of the source must be made
 // visible to the async proxy first (fence_proxy_async by every writing thread, then a barrier).

@@ -36,7 +36,9 @@
 //   * warpgroup 3 = epilogue (152 registers): reads acc_tile and stores the unit's output.
 // Two mbarriers pass acc_tile back and forth: acc_full (all 256 consumer threads have written it) and acc_empty (128
 // arrivals: the epilogue is done with it).  So the epilogue of unit n runs while the consumers issue the MMAs of unit
-// n+1.  A kernel supplies only its unit list, the TMA loads of one K-iteration, the MMAs of one stage, its gmain, its
+// n+1.  A CTA's last unit has nothing to overlap with: the consumers, which have no next unit, join its epilogue and
+// the three warpgroups split it (a one-wave launch is all last units).  While the MMAs run, the epilogue warpgroup
+// prefetches the unit's global epilogue inputs into L2.  A kernel supplies only its unit list, the TMA loads of one K-iteration, the MMAs of one stage, its gmain, its
 // epilogue and the loads of its epilogue's staged inputs.
 //
 // tc_conv_kernel (GATED, CONV): a unit is one 128-step x NCOLS output tile of one utterance.  Operands are 16-bit
@@ -66,6 +68,8 @@ constexpr int TC_EPILOGUE_REGS = 152;       // > 65 536 / 512: claimed with setm
 static_assert(TC_PRODUCER_REGS <= 65536 / TC_CONV_THREADS && TC_CONSUMER_REGS >= 65536 / TC_CONV_THREADS &&
               TC_EPILOGUE_REGS >= 65536 / TC_CONV_THREADS, "setmaxnreg direction of each warpgroup");
 static_assert(128 * TC_PRODUCER_REGS + 256 * TC_CONSUMER_REGS + 128 * TC_EPILOGUE_REGS <= 65536, "register file");
+constexpr int TC_EPILOGUE_LEAD = 3 * 128;   // thread 0 of the epilogue warpgroup: issues its bulk stores
+constexpr int TC_LAST_PARTS = 3;            // warpgroups sharing a CTA's last epilogue: consumers 0, 1 and epilogue 3
 constexpr int MAX_TAPS_TC = 8;
 enum { TC_GATED = 0, TC_CONV = 1 };
 
@@ -128,13 +132,31 @@ struct TcOutMaps { CUtensorMap out[3]; CUtensorMap res; };   // y | a | s (GATED
 // Where an epilogue finds its shared memory: the hand-off tile, the staging buffer, the barriers.
 struct Handoff { float* tile; float* staging; uint64_t* acc_empty; uint64_t* in_full; };
 
-// Release the hand-off tile after the bulk stores of this unit, or, with per-thread stores, after this thread's.
+// Release the hand-off tile after the bulk stores of this unit, or, with per-thread stores, after this thread's.  Only
+// the epilogue warpgroup releases it: the consumers that join a CTA's last epilogue have no next unit to hand off.
+// The wait is for the stores to have READ the tile, also after the last unit: the global writes of bulk stores still
+// in flight when the CTA exits complete before the grid does.
 __device__ __forceinline__ void release_tile(const Handoff& h, bool tma) {
+    if (threadIdx.x < TC_EPILOGUE_LEAD) return;
     if (!tma) mbar_arrive(h.acc_empty);
-    else if ((threadIdx.x & 127) == 0) {
+    else if (threadIdx.x == TC_EPILOGUE_LEAD) {
         bulk_commit();
         bulk_wait_read();
         mbar_arrive_cnt(h.acc_empty, 128);
+    }
+}
+
+// L2 prefetch of the part of a (B, C, T) fp32 epilogue input that unit (t0, b, channels [c0, c0 + nc)) reads, issued
+// by the epilogue warpgroup while the unit's MMAs run: warp q covers time steps [t0 + 32 q, t0 + 32 q + 32), lane l
+// channels l, l + 32, ..., both ends of each 128-byte row segment (which may straddle two lines).
+__device__ __forceinline__ void prefetch_bct(const float* x, int T, int C, int b, int c0, int nc, int t0) {
+    const int ta = t0 + 32 * ((threadIdx.x >> 5) & 3), lane = threadIdx.x & 31;
+    if (ta >= T) return;
+    const int tb = min(ta + 31, T - 1);
+    for (int c = lane; c < nc && c0 + c < C; c += 32) {
+        const float* row = x + ((size_t)b * C + c0 + c) * T;
+        prefetch_l2(row + ta);
+        prefetch_l2(row + tb);
     }
 }
 
@@ -152,10 +174,11 @@ __device__ __forceinline__ void stage_residual(const TcParams& p, const TcOutMap
 // Gated: a = acc_a (+ speaker) + bias_a, s = sigmoid(acc_b + bias_b), y from a, s and the residual.  y replaces the
 // residual in the staging buffer, a and s replace the two accumulator halves; the speaker bias (multi-speaker presets
 // only) stays on __ldg.
-template <int BR>
+template <int BR, int CW>
 __device__ __forceinline__ void epilogue_gated(const TcParams& p, const TcOutMaps& om, const Handoff& h, int n,
-                                               int a_row0, int a_z, int b_row0) {
+                                               int a_row0, int a_z, int b_row0, int part, int nparts) {
     constexpr int NC = 2 * BR;                             // a | b halves of the tile
+    static_assert(BR % CW == 0, "whole channel chunks");
     const int t = a_row0 + (threadIdx.x & 127), b = a_z, C = p.Nc;
     const bool tv = t < p.T, tma = p.tma_out != 0;
     const float* __restrict__ bias = p.bias;
@@ -168,25 +191,23 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const TcOutMap
     float* st = h.staging;
     const bool need_res = (p.gate_mode != 0) || p.residual;
     const size_t base = ((size_t)b * C + b_row0) * p.T + (tv ? t : 0);
-    if (need_res) {
-        if (tma) mbar_wait(h.in_full, n & 1);
-        else {
-#pragma unroll 8
-            for (int c = 0; c < BR; ++c) st[dense_at<BR>(c)] = tv ? __ldg(&res[base + (size_t)c * p.T]) : 0.f;
-        }
-    }
+    if (need_res && tma) mbar_wait(h.in_full, n & 1);
 #pragma unroll 1
-    for (int c32 = 0; c32 < BR; c32 += 32) {
-        float sp[32], ba[32], bb[32];                      // speaker bias; bias of the a and b halves
+    for (int c32 = part * CW; c32 < BR; c32 += nparts * CW) {   // this warpgroup's chunks of CW channels
+        float sp[CW], ba[CW], bb[CW];                      // speaker bias; bias of the a and b halves
         const size_t cb = base + (size_t)c32 * p.T;
+        if (need_res && !tma) {
+#pragma unroll 8
+            for (int i = 0; i < CW; ++i) st[dense_at<BR>(c32 + i)] = tv ? __ldg(&res[cb + (size_t)i * p.T]) : 0.f;
+        }
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
+        for (int i = 0; i < CW; ++i) {
             ba[i] = __ldg(&bias[b_row0 + c32 + i]);
             bb[i] = __ldg(&bias[C + b_row0 + c32 + i]);
             if (spk) sp[i] = tv ? __ldg(&spk[cb + (size_t)i * p.T]) : 0.f;
         }
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
+        for (int i = 0; i < CW; ++i) {
             const int cl = c32 + i;
             float va = tile[dense_at<NC>(cl)];
             if (spk) va += sp[i];
@@ -207,8 +228,8 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const TcOutMap
     }
     if (tma) {
         fence_proxy_async();
-        named_bar_sync(1, 128);
-        if ((threadIdx.x & 127) == 0) {
+        named_bar_sync(1, 128 * nparts);
+        if (threadIdx.x == TC_EPILOGUE_LEAD) {
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int t0 = a_row0 + 32 * q;
@@ -219,21 +240,25 @@ __device__ __forceinline__ void epilogue_gated(const TcParams& p, const TcOutMap
             }
         }
     } else if (tv) {
+#pragma unroll 1
+        for (int c32 = part * CW; c32 < BR; c32 += nparts * CW) {
 #pragma unroll 8
-        for (int c = 0; c < BR; ++c) {
-            const size_t idx = base + (size_t)c * p.T;
-            yo[idx] = st[dense_at<BR>(c)];
-            if (ao) ao[idx] = tile[dense_at<NC>(c)];
-            if (so) so[idx] = tile[dense_at<NC>(BR + c)];
+            for (int c = c32; c < c32 + CW; ++c) {
+                const size_t idx = base + (size_t)c * p.T;
+                yo[idx] = st[dense_at<BR>(c)];
+                if (ao) ao[idx] = tile[dense_at<NC>(c)];
+                if (so) so[idx] = tile[dense_at<NC>(BR + c)];
+            }
         }
     }
     release_tile(h, tma);
 }
 
 // Conv: out = acc * dropmask + bias + addend, then ReLU.
-template <int NCOLS>
+template <int NCOLS, int CW>
 __device__ __forceinline__ void epilogue_conv(const TcParams& p, const TcOutMaps& om, const Handoff& h, int a_row0,
-                                              int a_z, int b_row0) {
+                                              int a_z, int b_row0, int part, int nparts) {
+    static_assert(NCOLS % CW == 0, "whole channel chunks");
     const int t = a_row0 + (threadIdx.x & 127), b = a_z;
     const bool tv = t < p.T, tma = p.tma_out != 0;
     const DropCfg drop = make_drop(p.p_drop, p.seed_ptr, p.salt);
@@ -244,19 +269,19 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const TcOutMaps
     float* tile = h.tile;
     const size_t base = ((size_t)b * p.Nc + b_row0) * p.T + (tv ? t : 0);
 #pragma unroll 1
-    for (int c32 = 0; c32 < NCOLS; c32 += 32) {             // not unrolled: interleaving the chunks spilled
-        float bz[32], v[32], x2[32];                        // bias; addends e1, e2
+    for (int c32 = part * CW; c32 < NCOLS; c32 += nparts * CW) {   // not unrolled: interleaving the chunks spilled
+        float bz[CW], v[CW], x2[CW];                        // bias; addends e1, e2
         const int n0 = b_row0 + c32;
         const size_t cb = base + (size_t)c32 * p.T;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
+        for (int i = 0; i < CW; ++i) {
             const bool ok = tv && n0 + i < p.Nc;
             bz[i] = (bias && n0 + i < p.Nc) ? __ldg(&bias[n0 + i]) : 0.f;
             v[i] = (p.addmode != 0 && ok) ? __ldg(&e1[cb + (size_t)i * p.T]) : 0.f;
             x2[i] = (p.addmode == 2 && ok) ? __ldg(&e2[cb + (size_t)i * p.T]) : 0.f;
         }
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
+        for (int i = 0; i < CW; ++i) {
             float& d = tile[dense_at<NCOLS>(c32 + i)];
             float g = d * drop_scale(drop, (uint32_t)(cb + (size_t)i * p.T));
             if (bias) g += bz[i];
@@ -268,8 +293,8 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const TcOutMaps
     }
     if (tma) {
         fence_proxy_async();
-        named_bar_sync(1, 128);
-        if ((threadIdx.x & 127) == 0) {
+        named_bar_sync(1, 128 * nparts);
+        if (threadIdx.x == TC_EPILOGUE_LEAD) {
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
                 const int t0 = a_row0 + 32 * q;
@@ -278,9 +303,12 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const TcOutMaps
             }
         }
     } else if (tv) {
+#pragma unroll 1
+        for (int c32 = part * CW; c32 < NCOLS; c32 += nparts * CW) {
 #pragma unroll 8
-        for (int c = 0; c < NCOLS; ++c)
-            if (b_row0 + c < p.Nc) out[base + (size_t)c * p.T] = tile[dense_at<NCOLS>(c)];
+            for (int c = c32; c < c32 + CW; ++c)
+                if (b_row0 + c < p.Nc) out[base + (size_t)c * p.T] = tile[dense_at<NCOLS>(c)];
+        }
     }
     release_tile(h, tma);
 }
@@ -294,14 +322,19 @@ __device__ __forceinline__ void epilogue_conv(const TcParams& p, const TcOutMaps
 //   mma(stage, wg, acc, xacc)     consumer warpgroup wg's MMAs of one stage: p0 x p0 into acc and, with two planes,
 //                                 p0 x p1 + p1 x p0 into xacc (64 rows x NCOLS columns, NCOLS / 2 registers each)
 //   gmain(w)                      the factor of w's main accumulator (TcParams::gmain)
-//   epilogue(w, n, h)             stores w, this CTA's n-th unit, from the hand-off tile h.tile (layout: Cfg::DENSE,
-//                                 tc_ring.cuh).  Contract: the epilogue warpgroup arrives on h.acc_empty 128 times
-//                                 per unit, once its last access of the tile is done (by a thread or by the bulk
-//                                 stores it issued), so the consumers can overwrite the tile while the epilogue's
-//                                 last global stores are still under way.
+//   epilogue(w, n, h, part, nparts)  stores w, this CTA's n-th unit, from the hand-off tile h.tile (layout:
+//                                 Cfg::DENSE, tc_ring.cuh).  nparts = 1: the epilogue warpgroup alone (part 0).
+//                                 nparts = TC_LAST_PARTS, for the CTA's last unit only: consumer warpgroups 0 and 1
+//                                 (parts 0, 1) have no next unit and share it with the epilogue warpgroup (part 2),
+//                                 each taking its own slices of the tile; every output element keeps the expression
+//                                 (and the thread's time step or column) it has with one part.  Contract: the epilogue
+//                                 warpgroup arrives on h.acc_empty 128 times per unit, once its last access of the
+//                                 tile is done (by a thread or by the bulk stores it issued), so the consumers can
+//                                 overwrite the tile while the epilogue's last global stores are still under way.
 //   stage(w, h)                   issues the loads of unit w's epilogue inputs into h.staging, completing on
-//                                 h.in_full (phase n for the n-th unit): called by every epilogue thread for the
-//                                 first unit up front and for each next unit right after the current epilogue.
+//                                 h.in_full (phase n for the n-th unit), and L2 prefetches of those it reads from
+//                                 global memory: called by every epilogue thread for the first unit up front and for
+//                                 each next unit right after the current epilogue, so both run under w's MMAs.
 // ------------------------------------------------------------------------------------------------
 template <class Cfg, int NPL, class Decode, class Load, class Mma, class Gmain, class Epilogue, class Stage>
 __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, Decode decode, Load load, Mma mma,
@@ -346,11 +379,14 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
         int n = 0;
         for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++n) {
             const auto w = decode(u);
+            const bool last = u + gridDim.x >= num_units;
             mbar_wait(acc_full, n & 1);
-            epilogue(w, n, h);
-            if (u + gridDim.x < num_units) stage(decode(u + gridDim.x), h);
+            if (last) epilogue(w, n, h, TC_LAST_PARTS - 1, TC_LAST_PARTS);
+            else {
+                epilogue(w, n, h, 0, 1);
+                stage(decode(u + gridDim.x), h);
+            }
         }
-        if ((threadIdx.x & 127) == 0) bulk_wait();            // the last unit's bulk stores have completed
     } else if (warp >= 8) {
         setmaxnreg_dec<TC_PRODUCER_REGS>();
         if (warp == 8 && lane == 0) {
@@ -409,6 +445,11 @@ __device__ __forceinline__ void tc_pipeline(const TcMaps& maps, int num_units, D
                 else *dst = acc[i] * gm;
             }
             mbar_arrive(acc_full);
+            if (u + gridDim.x >= num_units) {                       // no next unit: join the last epilogue
+                const Handoff h = {acc_tile, acc_tile + Cfg::ACC_TILE / 4, acc_empty, in_full};
+                mbar_wait(acc_full, n & 1);
+                epilogue(w, n, h, wg, TC_LAST_PARTS);
+            }
         }
     }
 }
@@ -466,12 +507,25 @@ tc_conv_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ TcOu
         }
     };
     auto gmain = [&](const Tile&) { return p.gmain; };
-    auto epilogue = [&](const Tile& w, int n, const Handoff& h) {
-        if (MODE == TC_GATED) epilogue_gated<BR>(p, om, h, n, w.a_row0, w.a_z, w.b_row0);
-        else epilogue_conv<NCOLS>(p, om, h, w.a_row0, w.a_z, w.b_row0);
+    // 32-channel chunks for the epilogue warpgroup alone; eight chunks of the tile's channels when three warpgroups
+    // share the last unit (3 + 3 + 2, the epilogue warpgroup, which also issues the stores, taking 2)
+    auto epilogue = [&](const Tile& w, int n, const Handoff& h, int part, int nparts) {
+        if (MODE == TC_GATED) {
+            if (nparts == 1) epilogue_gated<BR, 32>(p, om, h, n, w.a_row0, w.a_z, w.b_row0, 0, 1);
+            else epilogue_gated<BR, BR / 8>(p, om, h, n, w.a_row0, w.a_z, w.b_row0, part, nparts);
+        } else {
+            if (nparts == 1) epilogue_conv<NCOLS, 32>(p, om, h, w.a_row0, w.a_z, w.b_row0, 0, 1);
+            else epilogue_conv<NCOLS, NCOLS / 8>(p, om, h, w.a_row0, w.a_z, w.b_row0, part, nparts);
+        }
     };
     auto stage = [&](const Tile& w, const Handoff& h) {
-        if (MODE == TC_GATED) stage_residual<BR>(p, om, h, w.a_row0, w.a_z, w.b_row0);
+        if (MODE == TC_GATED) {
+            stage_residual<BR>(p, om, h, w.a_row0, w.a_z, w.b_row0);
+            if (p.spk) prefetch_bct(p.spk, p.T, p.Nc, w.a_z, w.b_row0, BR, w.a_row0);
+        } else {
+            if (p.addmode != 0) prefetch_bct(p.e1, p.T, p.Nc, w.a_z, w.b_row0, NCOLS, w.a_row0);
+            if (p.addmode == 2) prefetch_bct(p.e2, p.T, p.Nc, w.a_z, w.b_row0, NCOLS, w.a_row0);
+        }
     };
     tc_pipeline<Cfg, NPL>(maps, num_tiles, decode, load, mma, gmain, epilogue, stage);
 }
@@ -556,19 +610,27 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
     auto gmain = [&](const Unit& w) { return 1.f + p.gcoef * (float)(2 * w.n_iters); };
     // Tap-major layout (s_n == 1): thread r owns column n0 + r and walks the rows, a warp storing 32 consecutive floats
     // of one row.  Otherwise (ConvTranspose layout, consecutive m two floats apart): thread r owns row m0 + r and walks
-    // the columns.
-    auto epilogue = [&](const Unit& w, int, const Handoff& h) {
+    // the columns.  The warpgroups sharing a last unit walk interleaved 16-row (16-column) slices of the tile.
+    auto epilogue = [&](const Unit& w, int, const Handoff& h, int part, int nparts) {
         const float* acc_tile = h.tile;
         const int r = threadIdx.x & 127;
+        const int cw = nparts == 1 ? 128 : 16;
         float* __restrict__ out = p.dw + (size_t)w.s * p.split_stride + (size_t)w.j * p.s_j;
         const int rows = min(128, p.Mw - w.m0), cols = min(128, p.Nw - w.n0);
         if (p.s_n == 1) {
             if (r < cols) {
                 float* __restrict__ o = out + w.n0 + r;
+#pragma unroll 1
+                for (int i0 = part * cw; i0 < rows; i0 += nparts * cw) {
+                    const int i1 = min(i0 + cw, rows);
+                    // row m = m0 + i at (m % msplit) * s_m + (m / msplit) * s_mh: one division per slice, then the
+                    // remainder and quotient stepped along the rows
+                    int mr = (w.m0 + i0) % p.msplit, mq = (w.m0 + i0) / p.msplit;
 #pragma unroll 4
-                for (int i = 0; i < rows; ++i) {
-                    const int m = w.m0 + i;
-                    o[(size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh] = acc_tile[i * Cfg::ACC_PITCH + r];
+                    for (int i = i0; i < i1; ++i) {
+                        o[(size_t)mr * p.s_m + (size_t)mq * p.s_mh] = acc_tile[i * Cfg::ACC_PITCH + r];
+                        if (++mr == p.msplit) { mr = 0; ++mq; }
+                    }
                 }
             }
         } else if (r < rows) {
@@ -576,10 +638,14 @@ tc_wgrad_mn_kernel(const __grid_constant__ TcMaps maps, const __grid_constant__ 
             float* __restrict__ o = out + (size_t)(m % p.msplit) * p.s_m + (size_t)(m / p.msplit) * p.s_mh +
                                     (size_t)w.n0 * p.s_n;
             const float* arow = acc_tile + r * Cfg::ACC_PITCH;
+#pragma unroll 1
+            for (int c0 = part * cw; c0 < cols; c0 += nparts * cw) {
+                const int c1 = min(c0 + cw, cols);
 #pragma unroll 4
-            for (int c = 0; c < cols; ++c) o[(size_t)c * p.s_n] = arow[c];
+                for (int c = c0; c < c1; ++c) o[(size_t)c * p.s_n] = arow[c];
+            }
         }
-        mbar_arrive(h.acc_empty);
+        if (threadIdx.x >= TC_EPILOGUE_LEAD) mbar_arrive(h.acc_empty);
     };
     tc_pipeline<Cfg, NPL>(maps, p.num_units, decode, load, mma, gmain, epilogue, [](const Unit&, const Handoff&) {});
 }
