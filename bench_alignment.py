@@ -27,7 +27,7 @@ import torch
 from bench import PRESETS
 from bench_mcd import _cpu_name, _events
 from bench_speaker_adapt import card
-from deepvoice3_pytorch_b200 import alignment, builder, data, mcd
+from deepvoice3_pytorch_b200 import alignment, builder, data, mcd, ops
 from deepvoice3_pytorch_b200._lib import lib
 from deepvoice3_pytorch_b200.train_step import TrainStep, to_device
 
@@ -67,7 +67,7 @@ def kernels(A_np, steps, tokens, iters, warmup):
     argmax, maxv = torch.empty(B, N, dtype=torch.int32, device=dev), torch.empty(B, N, device=dev)
     cov, score = torch.empty(B, L, device=dev), torch.empty(B, device=dev)
     dur = torch.empty(B, L, dtype=torch.int32, device=dev)
-    p, st = mcd._p, mcd._stream
+    p, st = ops._p, ops._stream
     fwd = lambda: lib.call("dv3_mas_forward", p(A), A.stride(0), A.stride(1), p(s_d), p(l_d), B, N, L, p(dir_off),
                            p(dirs), p(argmax), p(maxv), p(cov), p(score), st())
     bt = lambda: lib.call("dv3_mas_backtrace", p(s_d), p(l_d), B, L, p(dir_off), p(dirs), p(dur), st())

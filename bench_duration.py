@@ -159,7 +159,7 @@ def bench_loss():
     one = torch.ones((), device="cuda")
     dy = torch.empty(B, L, device="cuda")
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    p = D._p
+    p = ops._p
     fwd = _time_us(lambda: lib.call("dv3_duration_loss_fwd", p(y), L, p(d), L, p(n), B, L, p(row), p(loss),
                                     p(ops._err_flag(y.device)), st))
     bwd = _time_us(lambda: lib.call("dv3_duration_loss_bwd", p(y), L, p(d), L, p(n), B, L, p(one), p(dy), st))

@@ -26,6 +26,7 @@ from bench import PRESETS
 from bench_speaker_adapt import card
 from deepvoice3_pytorch_b200 import builder, mcd
 from deepvoice3_pytorch_b200._lib import lib
+from deepvoice3_pytorch_b200.ops import _p, _stream
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "tests"))
 import mcd_oracle as MO  # noqa: E402
@@ -64,8 +65,8 @@ def kernels(a_np, b_np, iters, warmup):
     cep = torch.empty(n, T_max, K, device=dev)
 
     def cepstra():
-        lib.call("dv3_mel_cepstra", mcd._p(padded), mcd._p(lens), mcd._p(basis), mcd._p(cep), n, T_max, M, K,
-                 mcd._stream())
+        lib.call("dv3_mel_cepstra", _p(padded), _p(lens), _p(basis), _p(cep), n, T_max, M, K,
+                 _stream())
     cepstra()
     rows = [q * T_max for q in range(n)]
     work, ws_floats = mcd._work_list(rows[:P], la, rows[P:], lb)
@@ -75,8 +76,8 @@ def kernels(a_np, b_np, iters, warmup):
     path = torch.empty(P, dtype=torch.int32, device=dev)
 
     def dtw():
-        lib.call("dv3_dtw_mcd", mcd._p(cep), K, mcd._p(work_d), mcd._p(ws), mcd._p(cost), mcd._p(path), P,
-                 mcd._stream())
+        lib.call("dv3_dtw_mcd", _p(cep), K, _p(work_d), _p(ws), _p(cost), _p(path), P,
+                 _stream())
     t_cep = _events(cepstra, iters, warmup)
     t_dtw = _events(dtw, iters, warmup)
     res = mcd.mcd_dtw(mels[:P], mels[P:], K)                       # the public call, checked against the raw one

@@ -26,7 +26,7 @@ import torch
 from bench import PRESETS
 from bench_mcd import K, _cpu_name, _events, _pairs
 from bench_speaker_adapt import card
-from deepvoice3_pytorch_b200 import audio, builder, mcd, pitch
+from deepvoice3_pytorch_b200 import audio, builder, mcd, ops, pitch
 from deepvoice3_pytorch_b200._lib import lib
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "tests"))
@@ -92,7 +92,7 @@ def dtw_kernels(iters, warmup):
     cost, length = torch.empty(P, device=dev), torch.empty(P, dtype=torch.int32, device=dev)
     path = torch.empty(int(sum(la) + sum(lb)), 2, dtype=torch.int32, device=dev)
     path_rows = torch.empty(P, dtype=torch.int32, device=dev)
-    p, st = mcd._p, mcd._stream
+    p, st = ops._p, ops._stream
     t_rec_path = _events(lambda: lib.call("dv3_dtw_path", p(flat), K, p(work_d), p(pw_d), p(ws), p(dirs), p(cost),
                                           p(length), P, st()), iters, warmup)
     t_rec = _events(lambda: lib.call("dv3_dtw_mcd", p(flat), K, p(work_d), p(ws), p(cost), p(length), P, st()),

@@ -126,7 +126,7 @@ def ctc_kernels(iters=20):
     inf = torch.empty(n, dtype=torch.int32, device=dev)
     one = torch.ones(1, device=dev)
     dz = torch.empty(n, Vk, Tm, device=dev)
-    p, s = R._p, R._stream
+    p, s = ops._p, ops._stream
 
     def fwd():
         lib.call("dv3_ctc_fwd", p(z), z.stride(0), z.stride(1), p(frd), p(tgd), Lm, p(tld), n, Vk, Tm, Lm, p(ws),

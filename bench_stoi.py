@@ -27,7 +27,7 @@ import torch
 from bench import PRESETS
 from bench_mcd import _cpu_name, _events
 from bench_speaker_adapt import card
-from deepvoice3_pytorch_b200 import audio, builder, intelligibility as I
+from deepvoice3_pytorch_b200 import audio, builder, intelligibility as I, ops
 from deepvoice3_pytorch_b200._lib import lib
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "tests"))
@@ -71,8 +71,8 @@ def kernels(clean, proc, iters, warmup):
     an = I._Analysis(wavs, list(range(P)) * 2)
     x10, n10 = audio.resample_batch(pad, lens, audio.hparams.sample_rate, sr_to=I.FS)
     table, win64, bands = I._tables(dev)
-    st = I._stream()
-    p = I._p
+    st = ops._stream()
+    p = ops._p
     n = 2 * P
     F0 = an.F0
     cap = [(f - 1) * I.HOP + I.FRAME if f else 0 for f in F0]

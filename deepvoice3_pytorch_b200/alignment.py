@@ -12,7 +12,6 @@
   every utterance.  ``teacher_forced_alignment``: durations and alignment confidence of a training batch under teacher
   forcing (to distil a duration model, or to find mislabelled or badly trimmed clips).
 """
-import contextlib
 import ctypes
 import math
 
@@ -21,6 +20,7 @@ import torch
 
 from . import mcd, synthesis
 from ._lib import lib
+from .ops import _p, _stream
 
 MAX_TOKENS = 1024             # csrc/align.cu MAS_MAX_TOKENS: one column per thread
 
@@ -87,10 +87,10 @@ def _mas(aligns, steps, tokens):
     for r0, r1 in chunks:
         n = r1 - r0
         lib.call("dv3_mas_forward", at(aligns, r0, sb), sb, st, at(steps_d, r0, 1), at(tokens_d, r0, 1), n, N, L,
-                 at(dir_off_d, r0, 1), mcd._p(dirs), at(argmax, r0, N), at(maxv, r0, N), at(coverage, r0, L),
-                 at(score, r0, 1), mcd._stream())
+                 at(dir_off_d, r0, 1), _p(dirs), at(argmax, r0, N), at(maxv, r0, N), at(coverage, r0, L),
+                 at(score, r0, 1), _stream())
         lib.call("dv3_mas_backtrace", at(steps_d, r0, 1), at(tokens_d, r0, 1), n, L, at(dir_off_d, r0, 1),
-                 mcd._p(dirs), at(durations, r0, L), mcd._stream())
+                 _p(dirs), at(durations, r0, L), _stream())
     return durations, score, argmax, maxv, coverage
 
 
@@ -224,7 +224,7 @@ def evaluate_attention(model, sequences, speaker_ids=None, batch_size=16, stage_
     seqs, speaker_ids = synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     if max(s.size for s in seqs) > MAX_TOKENS:
         raise ValueError("a sequence has %d tokens, more than %d" % (max(s.size for s in seqs), MAX_TOKENS))
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     order = sorted(range(len(seqs)), key=lambda i: -seqs[i].size)
     res = [None] * len(seqs)
     for c in range(0, len(order), int(batch_size)):

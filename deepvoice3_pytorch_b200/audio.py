@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from ._lib import lib, Dv3Error
+from .ops import _p
 
 
 class _HP:
@@ -261,14 +262,14 @@ def stft_mel_targets(wav, lengths, T_lin, r, downsample_step, lengths_dev=None):
     peak = None
     if hparams.rescaling:
         peak = torch.empty(B, device=dev)
-        lib.call("dv3_peak_abs_batched", _cp(wav), is16, _cp(lengths_dev), pitch, B, _cp(peak), st)
+        lib.call("dv3_peak_abs_batched", _p(wav), is16, _p(lengths_dev), pitch, B, _p(peak), st)
     if g.default:
-        lib.call("dv3_stft_mel_targets", _cp(wav), is16, _cp(lengths_dev), _cp(peak), float(hparams.rescaling_max),
-                 _cp(basis), _cp(start), _cp(length), _cp(y), _cp(mel), B, pitch, T_lin, r, ds, hparams.num_mels,
+        lib.call("dv3_stft_mel_targets", _p(wav), is16, _p(lengths_dev), _p(peak), float(hparams.rescaling_max),
+                 _p(basis), _p(start), _p(length), _p(y), _p(mel), B, pitch, T_lin, r, ds, hparams.num_mels,
                  float(hparams.preemphasis), float(hparams.min_level_db), float(hparams.ref_level_db), st)
     else:
-        lib.call("dv3_stft_mel_geom", _cp(wav), is16, _cp(lengths_dev), _cp(peak), float(hparams.rescaling_max),
-                 _cp(_geometry_table(dev, g.n_fft, g.hop)), _cp(basis), _cp(start), _cp(length), _cp(y), _cp(mel), B,
+        lib.call("dv3_stft_mel_geom", _p(wav), is16, _p(lengths_dev), _p(peak), float(hparams.rescaling_max),
+                 _p(_geometry_table(dev, g.n_fft, g.hop)), _p(basis), _p(start), _p(length), _p(y), _p(mel), B,
                  pitch, T_lin, r, ds, hparams.num_mels, g.n_fft, g.hop, float(hparams.preemphasis),
                  float(hparams.min_level_db), float(hparams.ref_level_db), st)
     return y, mel
@@ -387,8 +388,8 @@ def resample_batch(wav, lengths, sr_from, sr_to=None):
     bank, ntaps, pre_remove = _device_bank(dev, up, down)
     lengths_dev = torch.tensor(lengths, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
     out = torch.empty(nclips, pitch_out, device=dev)                   # the kernel writes every sample
-    lib.call("dv3_resample_poly_batched", _cp(wav), int(wav.dtype == torch.int16), _cp(lengths_dev), pitch, _cp(out),
-             pitch_out, nclips, _cp(bank), up, down, ntaps, pre_remove,
+    lib.call("dv3_resample_poly_batched", _p(wav), int(wav.dtype == torch.int16), _p(lengths_dev), pitch, _p(out),
+             pitch_out, nclips, _p(bank), up, down, ntaps, pre_remove,
              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     return out, out_lens
 
@@ -450,8 +451,8 @@ def resample_segments(wav, seg, sr_from, out, seg_dev=None):
               and tuple(seg_dev.shape) == (len(seg), len(SEG_FIELDS))):
         raise Dv3Error("resample_segments: seg_dev must be a contiguous int32 (%d, %d) tensor on %s"
                        % (len(seg), len(SEG_FIELDS), out.device))
-    lib.call("dv3_resample_segments_batched", _cp(wav), int(wav.dtype == torch.int16), pitch_in, _cp(seg_dev),
-             len(seg), _cp(out), pitch_out, _cp(bank), up, down, ntaps, pre_remove,
+    lib.call("dv3_resample_segments_batched", _p(wav), int(wav.dtype == torch.int16), pitch_in, _p(seg_dev),
+             len(seg), _p(out), pitch_out, _p(bank), up, down, ntaps, pre_remove,
              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     return out
 
@@ -475,8 +476,8 @@ def trim_bounds_batch(wav, lengths, top_db, offsets=None):
     ints = torch.tensor(lengths + offs, dtype=torch.int32).pin_memory().to(dev, non_blocking=True)
     dbs = torch.tensor(dbs, dtype=torch.float64).pin_memory().to(dev, non_blocking=True)
     bounds = torch.empty(nclips, 2, dtype=torch.int32, device=dev)
-    lib.call("dv3_trim_bounds_batched", _cp(wav), int(wav.dtype == torch.int16), _cp(ints),
-             None if offsets is None else _cp(ints[nclips:]), pitch, nclips, _cp(dbs), _cp(bounds),
+    lib.call("dv3_trim_bounds_batched", _p(wav), int(wav.dtype == torch.int16), _p(ints),
+             None if offsets is None else _p(ints[nclips:]), pitch, nclips, _p(dbs), _p(bounds),
              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     return bounds
 
@@ -543,10 +544,6 @@ def _normalize(S):
 
 def _denormalize(S):
     return (np.clip(S, 0, 1) * -hparams.min_level_db) + hparams.min_level_db
-
-
-def _cp(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
 def inv_num_samples(n_frames):
@@ -620,12 +617,12 @@ def griffin_lim_batch(mag, n_frames, n_iter=None, momentum=0.0):
         beta = momentum / (1.0 + momentum)               # fp64 here, rounded to fp32 once by the call
 
         def stft(x, spec):
-            lib.call("dv3_stft_complex_momentum_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(prev),
-                     _cp(spec), _cp(frames_d), T_max, nclips, beta, _cp(tab), g.n_fft, g.hop, st)
+            lib.call("dv3_stft_complex_momentum_geom", _p(x), _p(samples_d), n_max, _p(mag), _p(prev),
+                     _p(spec), _p(frames_d), T_max, nclips, beta, _p(tab), g.n_fft, g.hop, st)
     else:
         def stft(x, spec):
-            lib.call("dv3_stft_complex_geom", _cp(x), _cp(samples_d), n_max, _cp(mag), _cp(spec), _cp(frames_d),
-                     T_max, nclips, _cp(tab), g.n_fft, g.hop, st)
+            lib.call("dv3_stft_complex_geom", _p(x), _p(samples_d), n_max, _p(mag), _p(spec), _p(frames_d),
+                     T_max, nclips, _p(tab), g.n_fft, g.hop, st)
     _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g, tab)
     for _ in range(hparams.griffin_lim_iters if n_iter is None else n_iter):
         stft(x, spec)
@@ -635,7 +632,7 @@ def griffin_lim_batch(mag, n_frames, n_iter=None, momentum=0.0):
 
 
 def _istft(spec, x, samples_d, n_max, frames_d, T_max, nclips, st, g, tab):
-    lib.call("dv3_istft_geom", _cp(spec), _cp(x), _cp(samples_d), n_max, _cp(frames_d), T_max, nclips, _cp(tab), g.n_fft,
+    lib.call("dv3_istft_geom", _p(spec), _p(x), _p(samples_d), n_max, _p(frames_d), T_max, nclips, _p(tab), g.n_fft,
              g.hop, st)
 
 
@@ -711,16 +708,16 @@ def lws_batch(mag, n_frames, n_iter=None, init_iters=1):
     spec = torch.empty(nclips, T_max, g.bins, 2, device=dev)
     other = torch.empty_like(spec) if n_iter else None
     if g.default:
-        lib.call("dv3_lws_nofuture_batched", _cp(mag), _cp(spec), _cp(w), _cp(frames_d), T_max, nclips, init_iters, st)
+        lib.call("dv3_lws_nofuture_batched", _p(mag), _p(spec), _p(w), _p(frames_d), T_max, nclips, init_iters, st)
     else:
-        lib.call("dv3_lws_nofuture_geom", _cp(mag), _cp(spec), _cp(w), _cp(frames_d), T_max, nclips, init_iters,
+        lib.call("dv3_lws_nofuture_geom", _p(mag), _p(spec), _p(w), _p(frames_d), T_max, nclips, init_iters,
                  g.n_fft, g.hop, st)
     for _ in range(n_iter):
         if g.default:
-            lib.call("dv3_lws_iterate_batched", _cp(mag), _cp(spec), _cp(other), _cp(w), _cp(frames_d), T_max, nclips,
+            lib.call("dv3_lws_iterate_batched", _p(mag), _p(spec), _p(other), _p(w), _p(frames_d), T_max, nclips,
                      st)
         else:
-            lib.call("dv3_lws_iterate_geom", _cp(mag), _cp(spec), _cp(other), _cp(w), _cp(frames_d), T_max, nclips,
+            lib.call("dv3_lws_iterate_geom", _p(mag), _p(spec), _p(other), _p(w), _p(frames_d), T_max, nclips,
                      g.n_fft, g.hop, st)
         spec, other = other, spec
     x = torch.zeros(nclips, n_max, device=dev)
@@ -758,7 +755,7 @@ def inv_preemphasis(x):
     x2 = x.view(1, -1) if x.dim() == 1 else x
     x2 = x2.contiguous()
     y = torch.empty_like(x2)
-    lib.call("dv3_deemphasis", _cp(x2), _cp(y), x2.shape[0], x2.shape[1], x2.shape[1], float(hparams.preemphasis),
+    lib.call("dv3_deemphasis", _p(x2), _p(y), x2.shape[0], x2.shape[1], x2.shape[1], float(hparams.preemphasis),
              ctypes.c_void_p(torch.cuda.current_stream().cuda_stream))
     return y.view_as(x)
 
@@ -806,7 +803,7 @@ def inv_spectrogram_batch(spectrograms, n_iter=None, method="griffin_lim"):
     S = torch.from_numpy(S).cuda()
     amp = torch.empty_like(S)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    lib.call("dv3_spec_to_amp", _cp(S), _cp(amp), S.numel(), float(hparams.min_level_db), float(hparams.ref_level_db),
+    lib.call("dv3_spec_to_amp", _p(S), _p(amp), S.numel(), float(hparams.min_level_db), float(hparams.ref_level_db),
              float(hparams.power), st)
     if method == "fast_griffin_lim":
         wav = griffin_lim_batch(amp, n_frames, n_iter, momentum)

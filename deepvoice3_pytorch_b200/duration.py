@@ -11,7 +11,6 @@ speaking-rate rule, and the guided decoding they drive.
   attention layer's window then follows the prescribed token path and each utterance runs exactly sum(durations)
   decoder steps (``incremental.decode_ragged``).
 """
-import ctypes
 import math
 
 import numpy as np
@@ -21,17 +20,10 @@ from torch import nn
 from . import modules, ops, synthesis
 from ._lib import lib
 from .incremental import check_durations, query_steps
-from .speaker_encoder import ArenaGraphStep, check_single_process
+from .ops import _device_i32, _p, _stream
+from .train_step import ArenaGraphStep, check_single_process
 
 MAX_TOKENS = 1024             # csrc/duration.cu DUR_MAX_TOKENS
-
-
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 # ---- speaking rate ----------------------------------------------------------------------------------------------------
@@ -102,12 +94,6 @@ class _DurationLossFn(torch.autograd.Function):
         lib.call("dv3_duration_loss_bwd", _p(y), y.stride(0), _p(dur), dur.stride(0), _p(lens), B, L,
                  _p(ops._c(d_loss)), _p(dy), _stream())
         return dy, None, None
-
-
-def _device_i32(x, dev):
-    if torch.is_tensor(x):
-        return x.to(dev, torch.int32).contiguous()
-    return torch.from_numpy(np.ascontiguousarray(x, np.int32)).to(dev)
 
 
 def _check_loss_inputs(y, durations, lengths):

@@ -509,9 +509,7 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
     else:
         text_len = None
     Fr = decoder.in_dim * decoder.r
-    old_math = ops.conv_math
-    ops.conv_math = "fp32"                       # one-off set-up GEMMs (projections) in exact fp32
-    try:
+    with ops.overrides(conv_math="fp32"):       # one-off set-up GEMMs (projections) in exact fp32
         path = None
         if test_inputs is not None:
             test_inputs = test_inputs.to(torch.float32).contiguous()
@@ -538,8 +536,6 @@ def _decode(decoder, encoder_out, text_positions, speaker_embed, initial_input, 
             frames[:, 0] = initial_input.reshape(B, Fr)
         states, aligns, dones = _build_program(decoder, prog, Tmax, E, kv, pos_table, spk_of, text_len, frames,
                                                test_inputs, path)
-    finally:
-        ops.conv_math = old_math
 
     # ---- run ---------------------------------------------------------------------------------------
     def stop_steps(done):
@@ -674,13 +670,9 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
                                  "embedding and durations for every request or for none" % (r[0], E, Tp))
             keys[g, :k.size(0)], values[g, :k.size(0)], tpos[g, :k.size(0)] = k, v, p
         spk = torch.stack([r[4] for r in reqs]) if multi else None
-        old_math = ops.conv_math
-        ops.conv_math = "fp32"
-        try:
+        with ops.overrides(conv_math="fp32"):
             kv, pos_table, addend = _constants(decoder, keys, values, tpos, spk, Tmax)
             return kv, pos_table, [addend(f) for f in spk_layers] if spk_layers else []
-        finally:
-            ops.conv_math = old_math
 
     # ---- the slot program: per-request constants live in slot buffers, loaded from staging by dv3_inc_refill ----
     spk_layers, spk_slot = [], []
@@ -703,14 +695,10 @@ def decode_stream(decoder, slots, requests, use_graph=None, stats=None, stage_ti
             spk_slot.append(buf)
             return _Rows(buf, buf.size(-1))
 
-        old_math = ops.conv_math
-        ops.conv_math = "fp32"
-        try:
+        with ops.overrides(conv_math="fp32"):
             frames = prog.buf(S, Tmax + 1, Fr)
             states, aligns, dones = _build_program(decoder, prog, Tmax, E, kv_slot, pos_slot, spk_of, text_len,
                                                    frames, path=path_slot)
-        finally:
-            ops.conv_math = old_math
         prog.keep += spk_slot
         if guided:
             prog.stop_rule_total(total_slot)

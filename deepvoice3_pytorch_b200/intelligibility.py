@@ -27,13 +27,13 @@ Differences from pystoi and the MATLAB reference, whose parity is unpinned (neit
 ``stoi`` is the standard time-aligned measure; ``stoi_dtw`` warps two signals of different length along a DTW path,
 ``evaluate_vocoder`` scores copy synthesis, ``evaluate_intelligibility`` scores a TTS model against recordings.
 """
-import contextlib
 
 import numpy as np
 import torch
 
 from . import audio, mcd, synthesis
 from ._lib import lib
+from .ops import _p, _stream
 from .pitch import _nanmean
 
 FS = 10000
@@ -42,7 +42,6 @@ BANDS, MIN_FREQ = 15, 150.0
 N_SEG = 30
 BAND_WARPS, SEG_WARPS = 8, 4      # frames per dv3_stoi_bands CTA, segments per dv3_stoi_segments CTA
 
-_p, _stream = mcd._p, mcd._stream
 _table_cache = {}
 
 
@@ -244,7 +243,7 @@ def stoi_dtw(clean, processed):
     the envelope frames of (clean, processed).  A pair where either side has fewer than 30 envelope frames gets NaN and
     0 segments.  ValueError before any launch as ``stoi``, except that lengths may differ."""
     _check_pair_lists(clean, processed)
-    return _warped(clean, processed, lambda name: contextlib.nullcontext())
+    return _warped(clean, processed, synthesis.stages(None))
 
 
 def evaluate_vocoder(wavs, method="griffin_lim"):
@@ -288,7 +287,7 @@ def evaluate_intelligibility(model, sequences, reference_wavs, speaker_ids=None,
         if num_frames(audio.resampled_length(w.size, up, down)) > mcd.MAX_FRAMES:
             raise ValueError("reference_wavs[%d] gives more than %d frames at 10 kHz" % (k, mcd.MAX_FRAMES))
     device = next(model.parameters()).device
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     wavs, _ = synthesis.synthesized_audio(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer)
     with stage("stoi"):
         refs = [torch.from_numpy(np.ascontiguousarray(w)).to(device) for w in reference_wavs]

@@ -20,7 +20,6 @@ comparable between runs of this project, and parity with the SPTK-based MCD tool
 two ragged lists of mels; ``evaluate_synthesis`` synthesizes, makes mels of the synthesized and the reference audio, and
 scores them.
 """
-import contextlib
 import ctypes
 import math
 
@@ -29,6 +28,7 @@ import torch
 
 from . import audio, synthesis
 from ._lib import lib
+from .ops import _p, _stream
 
 MAX_FRAMES = 16384            # frames per sequence (csrc/mcd.cu MC_MAX_FRAMES): about 190 s at 22 050 Hz / hop 256
 MAX_MELS = 128                # the filterbank's limit (audio.check_geometry)
@@ -37,14 +37,6 @@ MCD_SCALE = 10.0 * math.sqrt(2.0) / math.log(10.0)
 DIR_BUDGET_BYTES = 1 << 30    # dtw_path: direction words of one launch (a 16 384 x 16 384 pair needs 64 MiB)
 
 _basis_cache = {}
-
-
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def dct_basis_fp64(M, K, min_level_db=None):
@@ -340,7 +332,7 @@ def evaluate_synthesis(model, sequences, reference_wavs, speaker_ids=None, vocod
     ``MAX_FRAMES`` frames."""
     K = check_evaluation(model, sequences, reference_wavs, speaker_ids, vocoder, batch_size, n_ceps)
     device = next(model.parameters()).device
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     synth = synthesis.synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer)
     with stage("mel"):
         ref = synthesis.wav_mels(list(reference_wavs), device)

@@ -5,9 +5,11 @@ arithmetic happens in csrc/*.cu.  Every function requires CUDA fp32 tensors and 
 there is no CPU fallback.
 """
 import collections
+import contextlib
 import ctypes
 import os
 
+import numpy as np
 import torch
 
 from ._lib import lib, Dv3Error
@@ -46,6 +48,27 @@ def is_deterministic():
     raise Dv3Error("unknown ops.deterministic %r (DV3_DETERMINISTIC is \"0\" or \"1\")" % (deterministic,))
 
 
+# The module attributes that select how the Functions run (each is described where it is defined below).
+_STATE = ("conv_math", "deterministic", "det_scratch", "grad_sink", "weight_bank", "grad_boundary_cb",
+          "frozen_weights", "speaker_adapt")
+
+
+@contextlib.contextmanager
+def overrides(**state):
+    """Set some of the execution-state attributes (``_STATE``) for the body of a ``with`` block and restore each to
+    the value it had on entry, on exit or exception.  An unknown name raises ValueError before anything is set."""
+    unknown = sorted(set(state) - set(_STATE))
+    if unknown:
+        raise ValueError("ops.overrides: unknown execution state %s (one of %s)" % (unknown, ", ".join(_STATE)))
+    scope = globals()
+    outer = {k: scope[k] for k in state}
+    scope.update(state)
+    try:
+        yield
+    finally:
+        scope.update(outer)
+
+
 # ----------------------------------------------------------------------------------------------
 # plumbing
 # ----------------------------------------------------------------------------------------------
@@ -61,12 +84,20 @@ def _chk(*tensors):
             raise Dv3Error("dv3b200 ops need contiguous tensors")
 
 
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
+def _p(t, offset=0):
+    """Device address of t's data, ``offset`` fp32 elements in (None for None)."""
+    return None if t is None else ctypes.c_void_p(t.data_ptr() + 4 * offset)
 
 
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def _device_i32(x, dev):
+    """An integer array, sequence or tensor as a contiguous int32 tensor on ``dev``."""
+    if torch.is_tensor(x):
+        return x.to(dev, torch.int32).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(x, np.int32)).to(dev)
 
 
 def _c(t):

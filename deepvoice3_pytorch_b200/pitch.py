@@ -25,7 +25,6 @@
 
 Parity with WORLD (DIO / Harvest), pYIN or librosa's ``yin`` is unpinned: none of them is installed.
 """
-import contextlib
 import ctypes
 import math
 import warnings
@@ -35,6 +34,7 @@ import torch
 
 from . import audio, mcd, synthesis
 from ._lib import lib
+from .ops import _p, _stream
 
 MAX_TAU = 1024                # the kernel's shared-memory span is sized for lags up to this
 GROSS_ERROR = 0.2             # GPE: |f0_a / f0_b - 1| above this is a gross error
@@ -114,10 +114,9 @@ def _yin(wavs, frames, tau_min, tau_max, threshold, gate, want_diff=False):
     ap = torch.empty(foff, device=dev)
     energy = torch.empty(foff, device=dev)
     diff = torch.empty(foff, 2, tau_max, device=dev) if want_diff else None
-    p = mcd._p
-    lib.call("dv3_yin_f0", p(flat), p(blocks_d), len(blocks), p(clips_d), len(clips), p(f0), p(ap), p(energy), p(diff),
-             g.n_fft, g.hop, int(tau_min), int(tau_max), ctypes.c_float(threshold), ctypes.c_float(gate),
-             ctypes.c_float(audio.hparams.sample_rate), mcd._stream())
+    lib.call("dv3_yin_f0", _p(flat), _p(blocks_d), len(blocks), _p(clips_d), len(clips), _p(f0), _p(ap), _p(energy),
+             _p(diff), g.n_fft, g.hop, int(tau_min), int(tau_max), ctypes.c_float(threshold), ctypes.c_float(gate),
+             ctypes.c_float(audio.hparams.sample_rate), _stream())
     return f0, ap, energy, diff
 
 
@@ -205,7 +204,7 @@ def evaluate_pitch(model, sequences, reference_wavs, speaker_ids=None, vocoder="
     tau_min, tau_max, gate = yin_params(f0_min, f0_max, threshold, silence_db)
     K = mcd.check_evaluation(model, sequences, reference_wavs, speaker_ids, vocoder, batch_size, n_ceps)
     device = next(model.parameters()).device
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     wavs, synth = synthesis.synthesized_audio(model, sequences, speaker_ids, vocoder, batch_size, device, stage_timer)
     with stage("mel"):
         ref_wavs, ref = synthesis.wav_clips_and_mels(list(reference_wavs), device)

@@ -18,8 +18,6 @@ The recognizer's floor on real recordings is the same call on their mels::
 
     token_error_rates(recognizer, synthesis.wav_mels(wavs, device), sequences)
 """
-import contextlib
-import ctypes
 
 import numpy as np
 import torch
@@ -27,22 +25,15 @@ from torch import nn
 
 from . import audio, modules, ops, synthesis
 from ._lib import lib
+from .ops import _device_i32, _p, _stream
 from .speaker_classifier import mean_loss
-from .speaker_encoder import ArenaGraphStep, check_single_process
+from .train_step import ArenaGraphStep, check_single_process
 
 MAX_VOCAB = 1024              # csrc/ctc.cu CTC_MAX_VOCAB
 MAX_TARGET = 1024             # target and reference tokens per row: the largest max_positions
 MAX_HYP = 65535               # hypothesis tokens per edit-distance pair
 WS_LIMIT = 2 << 30            # bytes of one CTC workspace
 EDIT_BUDGET = 1 << 28         # bytes of packed rows and workspace per edit-distance launch
-
-
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def ctc_ws_bytes(B, T, L):
@@ -76,12 +67,6 @@ def _host_ints(x, name):
     if x.ndim != 1 or not np.issubdtype(x.dtype, np.integer):
         raise ValueError("%s must be a 1-D integer array, got %s of shape %s" % (name, x.dtype, x.shape))
     return x.astype(np.int64)
-
-
-def _device_i32(x, dev):
-    if torch.is_tensor(x):
-        return x.to(dev, torch.int32) if x.dtype != torch.int32 or x.device != dev else x
-    return torch.from_numpy(np.ascontiguousarray(x, np.int32)).to(dev)
 
 
 def _check_logits(logits):
@@ -188,8 +173,6 @@ def ctc_loss(logits, frame_lengths, targets, target_lengths):
     tlen = _device_i32(_host_ints(target_lengths, "target_lengths") if not torch.is_tensor(target_lengths)
                        else target_lengths, dev)
     tgt = _device_i32(targets if torch.is_tensor(targets) else np.asarray(targets), dev)
-    if tgt.stride(1) != 1:
-        tgt = tgt.contiguous()
     return _CTCLossFn.apply(logits, frames, tgt, tlen)
 
 
@@ -478,7 +461,7 @@ def evaluate_recognition(model, recognizer, sequences, speaker_ids=None, vocoder
     synthesis._check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
     dev = recognizer.out[0].weight_v.device
     mels = synthesis.synthesized_mels(model, sequences, speaker_ids, vocoder, batch_size, dev, stage_timer)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     with stage("recognition"):
         return token_error_rates(recognizer, mels, sequences, word_sep)
 

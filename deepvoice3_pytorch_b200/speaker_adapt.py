@@ -23,14 +23,7 @@ import torch.nn.functional as F
 
 from . import ops
 from ._lib import lib, Dv3Error
-
-
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+from .ops import _p, _stream
 
 
 def check_adapt_speakers(model, ids):
@@ -172,28 +165,26 @@ class SpeakerAdapt:
         ``spk.backward``.  -> the loss."""
         params = list(self.model.parameters())
         flags = [p.requires_grad for p in params]
-        prev = ops.speaker_adapt, ops.frozen_weights
         for p in params:
             p.requires_grad_(False)
-        ops.speaker_adapt, ops.frozen_weights = self, self.frozen
         try:
-            loss = inner(batch)
-            e = self.anchor
-            B = e.shape[0]
-            d_e = torch.empty(B, self.S, device=e.device)
-            lib.call("dv3_spk_grad_reduce", _p(self.partials(B)), self.nsites * self.splits, _p(d_e), B, self.S,
-                     _stream())
-            if spk is None:
-                ids, lo, n, out = batch.get("speaker_ids"), self.lo, self.n, self.arena.grad
-            else:                   # ids = arange(B): each row's own gradient
-                ids, lo, n, out = self.rows(B, e.device), 0, B, torch.empty(B, self.S, device=e.device)
-            lib.call("dv3_spk_rows_grad", _p(d_e), _p(e.grad), _p(ids), lo, n, _p(out),
-                     _p(ops._err_flag(e.device)), B, self.S, _stream())
-            if spk is not None:
-                spk.backward(out)
-            return loss
+            with ops.overrides(speaker_adapt=self, frozen_weights=self.frozen):
+                loss = inner(batch)
+                e = self.anchor
+                B = e.shape[0]
+                d_e = torch.empty(B, self.S, device=e.device)
+                lib.call("dv3_spk_grad_reduce", _p(self.partials(B)), self.nsites * self.splits, _p(d_e), B, self.S,
+                         _stream())
+                if spk is None:
+                    ids, lo, n, out = batch.get("speaker_ids"), self.lo, self.n, self.arena.grad
+                else:                   # ids = arange(B): each row's own gradient
+                    ids, lo, n, out = self.rows(B, e.device), 0, B, torch.empty(B, self.S, device=e.device)
+                lib.call("dv3_spk_rows_grad", _p(d_e), _p(e.grad), _p(ids), lo, n, _p(out),
+                         _p(ops._err_flag(e.device)), B, self.S, _stream())
+                if spk is not None:
+                    spk.backward(out)
+                return loss
         finally:
-            ops.speaker_adapt, ops.frozen_weights = prev
             for p, f in zip(params, flags):
                 p.requires_grad_(f)
             self._reset()

@@ -11,29 +11,21 @@ frames.  Then, with W (K, C) and c (K) plain parameters:
 * training loss: the mean softmax cross-entropy over the rows, its partials fused into the row pass and summed in index
   order by ``dv3_spkenc_reduce``; the gradients (``dv3_spkcls_bwd``) are written directly, with no float atomics.
 """
-import contextlib
-import ctypes
 import math
 
 import numpy as np
 import torch
 from torch import nn
 
-from . import ops
+from . import ops, synthesis
 from ._lib import Dv3Error, lib
-from .speaker_encoder import (MAX_CHANNELS, ArenaGraphStep, SpeakerEncoder, check_samples, check_single_process,
-                              pad_samples, pooled_features, trunk_layers)
+from .ops import _p, _stream
+from .speaker_encoder import (MAX_CHANNELS, SpeakerEncoder, check_samples, pad_samples, pooled_features,
+                              trunk_layers)
 from .speaker_verifier import cloned_voice_mels
+from .train_step import ArenaGraphStep, check_single_process
 
 MIN_CLASSES, MAX_CLASSES = 2, 8192
-
-
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def check_head(R, C, K):
@@ -246,7 +238,7 @@ def classify_cloned_voices(model, classifier, speaker_ids, sequences, targets=No
     check_head(len(sequences), classifier.channels, classifier.n_classes)
     _, tests = cloned_voice_mels(model, classifier.mel_dim, speaker_ids, sequences, vocoder, batch_size,
                                  classifier.w.device, stage_timer)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     with stage("classification"):
         logits, pred = classifier.classify(tests)
     return {"logits": logits, "predicted": pred, "targets": targets,
@@ -256,7 +248,7 @@ def classify_cloned_voices(model, classifier, speaker_ids, sequences, targets=No
 # ---- training -------------------------------------------------------------------------------------------------------
 class SpeakerClassifierStep(ArenaGraphStep):
     """One training step of a SpeakerClassifier: the mean softmax cross-entropy over the B*N utterances of a batch,
-    then clip + Adam (``speaker_encoder.ArenaGraphStep``: ParameterArena + FlatAdam, the conv_math and deterministic
+    then clip + Adam (``train_step.ArenaGraphStep``: ParameterArena + FlatAdam, the conv_math and deterministic
     modes of construction, one batch shape, bit-exact checkpoints, one CUDA graph with use_graph).
 
     ``step(batch)`` takes {"mels": (B, N, T, mel_dim) fp32, "speaker_ids": (B,) int64 in [0, n_classes)}, as

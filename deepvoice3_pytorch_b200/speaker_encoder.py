@@ -15,29 +15,20 @@ Layers, on B speakers x N cloning samples of (T, mel_dim) normalised mel frames:
   rows in index order).
 """
 import contextlib
-import ctypes
 import math
-import time
 
 import torch
-import torch.distributed as dist
 from torch import nn
 
 from . import modules, ops
 from ._lib import lib, Dv3Error
+from .ops import _p, _stream
+from .train_step import ArenaGraphStep, check_single_process
 
 MAX_SAMPLES, MAX_CHANNELS, MAX_EMBED, MAX_HEADS = 32, 256, 64, 8
 _ATTN_PARAMS = ("w_q", "b_q", "w_k", "b_k", "w_v", "b_v", "w_s", "b_s", "w_e", "b_e")
 # order of the parameter gradients in a partial row of dv3_spkenc_attn_bwd
 _GRAD_ORDER = ("w_q", "w_k", "w_v", "b_q", "b_k", "b_v", "w_s", "b_s", "w_e", "b_e")
-
-
-def _p(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _chk_index(t, what):
@@ -306,118 +297,6 @@ def clone_voices(model, encoder, samples):
                                                                      model.speaker_embed_dim))
     encoder.check_samples(samples)
     return model.add_speakers(len(samples), init=encoder.embed_batch(samples))
-
-
-def check_single_process(name):
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-        raise ValueError("%s runs in a single process (world size %d)" % (name, dist.get_world_size()))
-
-
-class ArenaGraphStep:
-    """What the speaker encoder's and the speaker verifier's training steps share: clip + Adam (``train_step.FlatAdam``
-    over a ``ParameterArena`` of ``net``'s parameters; clip_thresh None: no clipping), the ``ops.conv_math`` and
-    ``ops.deterministic`` modes current at construction, one batch shape, checkpoints of copies that resume bit-exactly,
-    and with use_graph one CUDA graph for forward, backward and update.  A subclass defines ``_objective(batch)`` (the
-    loss to minimise, on device tensors), ``_check_batch(batch)`` (ValueError before any launch) and may define
-    ``_graph_key()`` (when it changes, the next step captures a new graph).  ``step`` reads the batch keys
-    ``_batch_keys``."""
-
-    _net_key = "net"
-    _batch_keys = ("mels", "speaker_ids")
-
-    def __init__(self, net, lr, betas, eps, clip_thresh, use_graph):
-        from .train_step import FlatAdam, ParameterArena
-        self.math = ops.math_mode()
-        self.deterministic = ops.is_deterministic()
-        self._det_scratch = ops.DetScratch() if self.deterministic else None
-        self.net, self.lr = net, lr
-        self.arena = ParameterArena(net, list(net.parameters()))
-        self.opt = FlatAdam(self.arena, lr, betas, eps, 0.0 if clip_thresh is None else float(clip_thresh))
-        self.use_graph = use_graph
-        self.global_step = 0
-        self._graph = self._static = self._loss = self._shape = self._captured_key = None
-        self.launches_per_step = None
-        self.graphs_captured = 0
-        self.capture_seconds = 0.0
-
-    def state_dict(self):
-        """A checkpoint of copies (the network's own state_dict holds views of the live parameter arena)."""
-        return {self._net_key: {k: v.clone() for k, v in self.net.state_dict().items()},
-                "optimizer": self.opt.state_dict(), "global_step": self.global_step}
-
-    def load_state_dict(self, ckpt):
-        """Resume bit-exactly from ``state_dict()``: parameters (in place, so captured graphs stay valid), Adam moments
-        and step count."""
-        self.net.load_state_dict(ckpt[self._net_key])
-        self.opt.load_state_dict(ckpt["optimizer"])
-        self.global_step = int(ckpt.get("global_step", 0))
-
-    def _graph_key(self):
-        return None
-
-    def _forward_backward(self, batch):
-        self.arena.zero_grad()
-        outer = (ops.deterministic, ops.det_scratch)
-        ops.deterministic = self.deterministic
-        if self.deterministic:
-            ops.det_scratch = self._det_scratch
-        try:
-            loss = self._objective(batch)
-            loss.backward()
-            return loss.detach()
-        finally:
-            ops.deterministic, ops.det_scratch = outer
-
-    def step(self, batch):
-        """-> the batch's loss (a device scalar, valid until the next step)."""
-        name = type(self).__name__
-        if ops.math_mode() != self.math:
-            raise ValueError("%s was built with ops.conv_math = %r and cannot step under %r"
-                             % (name, self.math, ops.conv_math))
-        dev = self.arena.flat.device
-        batch = {k: batch[k] for k in self._batch_keys}
-        self._check_batch(batch)
-        shape = tuple(tuple(v.shape) for v in batch.values())
-        if self._shape is not None and shape != self._shape:
-            raise ValueError("%s batches have one shape: %s, then %s" % (name, self._shape, shape))
-        self._shape = shape
-        self.net.train()
-        self.opt.set_hyper(self.lr)
-        if not self.use_graph:
-            loss = self._forward_backward({k: v.to(dev, non_blocking=True) for k, v in batch.items()})
-            self.opt.apply()
-        else:
-            loss = self._graph_step(batch)
-        self.global_step += 1
-        return loss
-
-    def _graph_step(self, batch):
-        if self._graph is not None and self._graph_key() != self._captured_key:
-            self._graph = self._static = self._loss = None     # the captured step reads stale addresses: capture anew
-        if self._graph is None:
-            t0 = time.perf_counter()
-            dev = self.arena.flat.device
-            self._static = {k: v.to(dev).clone() for k, v in batch.items()}
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):              # allocator, weight-norm buffers, deterministic scratch
-                for _ in range(2):
-                    self._forward_backward(self._static)
-            torch.cuda.current_stream().wait_stream(s)
-            self._graph = torch.cuda.CUDAGraph()
-            self._captured_key = self._graph_key()
-            n0 = lib.raw("dv3_launch_count")()
-            with torch.cuda.graph(self._graph):
-                self._loss = self._forward_backward(self._static)
-                self.opt.apply()
-            self.launches_per_step = int(lib.raw("dv3_launch_count")() - n0)
-            self.graphs_captured += 1
-            torch.cuda.synchronize(dev)
-            self.capture_seconds += time.perf_counter() - t0
-        for k, v in batch.items():
-            self._static[k].copy_(v, non_blocking=True)
-        self._graph.replay()
-        return self._loss
 
 
 class SpeakerEncoderStep(ArenaGraphStep):

@@ -15,28 +15,20 @@ frames.  Then, with W (D, C), c, S (D, D) and b plain parameters:
   softplus(L), over every (enrollment, test) pair of a batch, fused into the score kernels; ``dv3_spkenc_reduce`` sums
   every partial in index order, so there are no float atomics.
 """
-import contextlib
-import ctypes
 import math
 
 import numpy as np
 import torch
 from torch import nn
 
-from . import audio, ops
+from . import audio, ops, synthesis
 from ._lib import lib
-from .speaker_encoder import (ArenaGraphStep, SpeakerEncoder, _check_model, _chk_index, check_samples,
-                              check_single_process, pad_samples, pooled_features, trunk_layers)
+from .ops import _p, _stream
+from .speaker_encoder import (SpeakerEncoder, _check_model, _chk_index, check_samples, pad_samples, pooled_features,
+                              trunk_layers)
+from .train_step import ArenaGraphStep, check_single_process
 
 MAX_ENROLL, MAX_CHANNELS, MAX_EMBED = 32, 256, 128
-
-
-def _p(t, offset=0):
-    return None if t is None else ctypes.c_void_p(t.data_ptr() + 4 * offset)
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 # ---- launches -----------------------------------------------------------------------------------------------------
@@ -271,7 +263,6 @@ def cloned_voice_mels(model, mel_dim, speaker_ids, sequences, vocoder, batch_siz
     where the audio path makes another count, malformed sequences.  Then ``synthesis.synthesized_mels``: every
     ``sequences[k]`` synthesized in the voice ``speaker_ids[k]`` (stage "synthesis") and turned into normalised mels on
     ``device`` (stage "mel") -> (speaker ids as ints, list of (T_k, num_mels) mels)."""
-    from . import synthesis
     _check_model(model)
     audio.check_phase_method(vocoder)
     speaker_ids = [int(s) for s in speaker_ids]
@@ -311,7 +302,7 @@ def verify_cloned_voices(model, verifier, speaker_ids, enrollment, sequences, vo
     samples = check_samples([enrollment[k] for k in enrolled], verifier.mel_dim, verifier.max_enroll)
     speaker_ids, tests = cloned_voice_mels(model, verifier.mel_dim, speaker_ids, sequences, vocoder, batch_size,
                                            verifier.w.device, stage_timer)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = synthesis.stages(stage_timer)
     with stage("scoring"):
         scores = verifier.score(verifier.embed_enrollment(samples), verifier.embed_tests(tests))
         scores = scores.double().cpu().numpy()
@@ -323,7 +314,7 @@ def verify_cloned_voices(model, verifier, speaker_ids, enrollment, sequences, vo
 # ---- training -------------------------------------------------------------------------------------------------------
 class SpeakerVerifierStep(ArenaGraphStep):
     """One training step of a SpeakerVerifier: the balanced binary cross-entropy over the B x B (enrollment, test)
-    pairs of a batch, then clip + Adam (``speaker_encoder.ArenaGraphStep``: ParameterArena + FlatAdam, the conv_math
+    pairs of a batch, then clip + Adam (``train_step.ArenaGraphStep``: ParameterArena + FlatAdam, the conv_math
     and deterministic modes of construction, one batch shape, bit-exact checkpoints, one CUDA graph with use_graph).
 
     ``step(batch)`` takes {"mels": (B, N, T, mel_dim) fp32, "speaker_ids": (B,) int64}, as

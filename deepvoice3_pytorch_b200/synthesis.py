@@ -31,6 +31,12 @@ import torch
 from . import audio, incremental, ops
 
 
+def stages(stage_timer):
+    """The ``stage_timer`` argument of the synthesis and evaluation calls as a callable ``name -> context manager``
+    (None: no timing)."""
+    return stage_timer or (lambda name: contextlib.nullcontext())
+
+
 def _check_inputs(model, sequences, speaker_ids, **counts):
     """-> int64 token arrays, int speaker ids; counts: name=value arguments that must be >= 1 (batch_size, slots)."""
     if len(sequences) == 0:
@@ -156,7 +162,7 @@ def tts_batch(model, sequences, speaker_ids=None, batch_size=16, stage_timer=Non
     audio.check_phase_method(vocoder)
     durs = guided_durations(model, sequences, durations, speed)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = stages(stage_timer)
     order = sorted(range(len(seqs)), key=lambda i: -seqs[i].size)
     out = [None] * len(seqs)
     for c in range(0, len(order), int(batch_size)):
@@ -196,7 +202,7 @@ def synthesized_audio(model, sequences, speaker_ids, vocoder, batch_size, device
     method or malformed inputs (as ``tts_batch``)."""
     audio.check_phase_method(vocoder)
     _check_inputs(model, sequences, speaker_ids, batch_size=batch_size)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = stages(stage_timer)
     with stage("synthesis"):
         wavs = [w for w, _, _, _ in tts_batch(model, sequences, speaker_ids, batch_size=batch_size, vocoder=vocoder)]
     with stage("mel"):
@@ -223,7 +229,7 @@ def tts_stream(model, sequences, speaker_ids=None, slots=16, post_batch=16, stag
     audio.check_phase_method(vocoder)
     durs = guided_durations(model, sequences, durations, speed)
     seqs, speaker_ids = _check_inputs(model, sequences, speaker_ids, slots=slots, post_batch=post_batch)
-    stage = stage_timer or (lambda name: contextlib.nullcontext())
+    stage = stages(stage_timer)
     return _stream(model, seqs, speaker_ids, int(slots), int(post_batch), stage, stats, vocoder, durs)
 
 

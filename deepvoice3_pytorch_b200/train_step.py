@@ -479,8 +479,7 @@ def check_speaker_encoder(model, encoder, train_seq2seq, train_postnet, adapt_sp
                          "be True")
     if adapt_speakers is not None:
         raise ValueError("adapt_speakers and speaker_encoder are two ways to train speaker embeddings: pass one")
-    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-        raise ValueError("speaker_encoder training runs in a single process (world size %d)" % dist.get_world_size())
+    check_single_process("speaker_encoder training")
 
 
 def check_train_mode(model, train_seq2seq, train_postnet):
@@ -495,6 +494,30 @@ def check_train_mode(model, train_seq2seq, train_postnet):
     if train_postnet and getattr(model, "use_decoder_state_for_postnet_input", False):
         raise ValueError("postnet-only training feeds the converter ground-truth mels, but this model was built with "
                          "use_decoder_state_for_postnet_input=True (its converter reads decoder states)")
+
+
+def check_single_process(name):
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        raise ValueError("%s runs in a single process (world size %d)" % (name, dist.get_world_size()))
+
+
+def capture_step(warm_up, body, pool=None):
+    """Capture a training step in a new CUDA graph: ``warm_up()`` runs eagerly on a side stream first (its passes
+    allocate the buffers, tables and scratch the captured kernels address), then ``body()`` is captured, into the
+    memory pool ``pool`` when given.  -> (graph, dv3 kernel launches recorded in it, wall seconds of both)."""
+    t0 = time.perf_counter()
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        warm_up()
+    torch.cuda.current_stream().wait_stream(s)
+    graph = torch.cuda.CUDAGraph()
+    n0 = lib.raw("dv3_launch_count")()
+    with torch.cuda.graph(graph, pool=pool):
+        body()
+    launches = int(lib.raw("dv3_launch_count")() - n0)
+    torch.cuda.synchronize()
+    return graph, launches, time.perf_counter() - t0
 
 
 class TrainStep:
@@ -554,8 +577,7 @@ class TrainStep:
             if not (train_seq2seq and train_postnet):
                 raise ValueError("speaker adaptation trains through the joint forward: train_seq2seq and train_postnet "
                                  "must both be True")
-            if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
-                raise ValueError("speaker adaptation runs in a single process (world size %d)" % dist.get_world_size())
+            check_single_process("speaker adaptation")
         check_train_mode(model, train_seq2seq, train_postnet)
         self.math = ops.math_mode()
         self.deterministic = ops.is_deterministic() if deterministic is None else bool(deterministic)
@@ -726,30 +748,27 @@ class TrainStep:
     # -- pieces -------------------------------------------------------------------------------
     def _forward_backward(self, batch):
         self.arena.zero_grad()
-        ops.grad_sink = self.adapt is None  # kernels accumulate parameter gradients straight into the arena
-        ops.weight_bank = self.bank   # weight norm of all layers: 2 launches up front, 1 per bucket in the backward
-        ops.grad_boundary_cb = self._bucket_ready if self.overlap_comm else None
         self._reduced = set()
-        det_outer = (ops.deterministic, ops.det_scratch)
-        ops.deterministic = self.deterministic
+        # grad_sink: kernels accumulate parameter gradients straight into the arena; weight_bank: weight norm of all
+        # layers, 2 launches up front, 1 per bucket in the backward
+        state = dict(grad_sink=self.adapt is None, weight_bank=self.bank,
+                     grad_boundary_cb=self._bucket_ready if self.overlap_comm else None,
+                     deterministic=self.deterministic)
         if self.deterministic:
-            ops.det_scratch = self._det_scratch
-        try:
-            if self.bank is not None:
-                self.bank.begin_step()
-            # the speaker encoder runs outside the model's extent scope (a bucket's extents would mask its stacks)
-            # and, in the encoder-only mode, before the frozen-weight cache is installed
-            spk = self.encoder(batch["speaker_mels"]) if self.encoder is not None else None
-            if self.adapt is not None:
-                return self.adapt.run(batch, lambda b: self._forward_backward_inner(b, spk), spk)
-            return self._forward_backward_inner(batch, spk)
-        finally:
-            ops.deterministic, ops.det_scratch = det_outer
-            ops.grad_sink = False
-            ops.weight_bank = None
-            ops.grad_boundary_cb = None
-            if self.bank is not None:
-                self.bank.end_step()
+            state["det_scratch"] = self._det_scratch
+        with ops.overrides(**state):
+            try:
+                if self.bank is not None:
+                    self.bank.begin_step()
+                # the speaker encoder runs outside the model's extent scope (a bucket's extents would mask its stacks)
+                # and, in the encoder-only mode, before the frozen-weight cache is installed
+                spk = self.encoder(batch["speaker_mels"]) if self.encoder is not None else None
+                if self.adapt is not None:
+                    return self.adapt.run(batch, lambda b: self._forward_backward_inner(b, spk), spk)
+                return self._forward_backward_inner(batch, spk)
+            finally:
+                if self.bank is not None:
+                    self.bank.end_step()
 
     def _bucket_ready(self, tag):
         """Called from the backward pass (ops.grad_boundary hook): the parameter gradients of bucket ``tag`` are final
@@ -902,24 +921,20 @@ class TrainStep:
         return tuple((k, tuple(v.shape)) for k, v in sorted(batch.items()) if torch.is_tensor(v))
 
     def _warm_up(self, static):
-        """Two eager passes on a side stream before a capture (allocator, NCCL, weight-bank tables); they do not
-        consume dropout seeds."""
-        s = torch.cuda.Stream()
-        s.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(s):
-            dev = self.arena.flat.device
-            ops.rng.seed_tensor(dev)
-            seed0 = ops.rng.base.clone()
-            for _ in range(2):
-                self._forward_backward(static)
-                if self.world > 1 and self.overlap_comm:    # NCCL communicators / bucket tables exist before capture
-                    pend = [r for t, r in self.buckets.items() if t not in self._reduced]
-                    with torch.cuda.stream(self._comm):
-                        self._comm.wait_stream(s)
-                        self.arena.all_reduce_grads(pend + self.rest_ranges)
-                    s.wait_stream(self._comm)
-            ops.rng.base.copy_(seed0)           # the warm-up passes do not consume dropout seeds
-        torch.cuda.current_stream().wait_stream(s)
+        """Two eager passes before a capture (allocator, NCCL, weight-bank tables), on ``capture_step``'s side stream;
+        they do not consume dropout seeds."""
+        s = torch.cuda.current_stream()
+        ops.rng.seed_tensor(self.arena.flat.device)
+        seed0 = ops.rng.base.clone()
+        for _ in range(2):
+            self._forward_backward(static)
+            if self.world > 1 and self.overlap_comm:    # NCCL communicators / bucket tables exist before capture
+                pend = [r for t, r in self.buckets.items() if t not in self._reduced]
+                with torch.cuda.stream(self._comm):
+                    self._comm.wait_stream(s)
+                    self.arena.all_reduce_grads(pend + self.rest_ranges)
+                s.wait_stream(self._comm)
+        ops.rng.base.copy_(seed0)           # the warm-up passes do not consume dropout seeds
 
     def _bucket_step(self, batch):
         """A batch of another shape than the first graph's: pad it to its bucket and replay (capturing on first use)
@@ -940,21 +955,18 @@ class TrainStep:
             key = ("bucket", shape, int(batch["x"].shape[0]), "speaker_ids" in batch)
         rec = self._buckets.get(key)
         if rec is None:
-            t0 = time.perf_counter()
             if shape is None:
                 static = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in batch.items()}
             else:
                 static = data.pad_to_bucket(batch, shape[0], shape[1], r, ds)
             out = torch.zeros((), device=self.arena.flat.device)   # outside the graph pool: read after the replay
-            self._warm_up(static)
-            graph = torch.cuda.CUDAGraph()
-            n0 = lib.raw("dv3_launch_count")()
-            with torch.cuda.graph(graph, pool=self._pool):
+
+            def body():
                 out.copy_(self._forward_backward(static))
                 self._exchange_and_update()
-            rec = self._buckets[key] = (graph, static, out, int(lib.raw("dv3_launch_count")() - n0))
-            torch.cuda.synchronize()
-            self.capture_seconds += time.perf_counter() - t0
+            graph, launches, seconds = capture_step(lambda: self._warm_up(static), body, self._pool)
+            rec = self._buckets[key] = (graph, static, out, launches)
+            self.capture_seconds += seconds
         graph, static, out, _ = rec
         if shape is None:
             for k, v in batch.items():
@@ -969,29 +981,124 @@ class TrainStep:
         if self._graph is not None and self._shape_key(batch) != self._graph_key:
             return self._bucket_step(batch)
         if self._graph is None:
-            t0 = time.perf_counter()
             self._pool = torch.cuda.graph_pool_handle()
             self._graph_key = self._shape_key(batch)
-            # static input buffers; warm up on a side stream, then capture forward+loss+backward (+update when
-            # there is no collective to run in between)
+            # static input buffers; capture forward+loss+backward (+update when there is no collective to run in
+            # between)
             self._static = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in batch.items()}
-            self._warm_up(self._static)
-            self._graph = torch.cuda.CUDAGraph()
-            n0 = lib.raw("dv3_launch_count")()
             capture_all = self.world == 1 or self.graph_comm
-            with torch.cuda.graph(self._graph, pool=self._pool):
+
+            def body():
                 self._loss = self._forward_backward(self._static)
                 if capture_all:                     # NCCL all-reduces are captured as graph nodes on the comm stream
                     self._exchange_and_update()
-            self.launches_per_step = int(lib.raw("dv3_launch_count")() - n0) + (0 if capture_all else 2)
-            torch.cuda.synchronize()
-            self.capture_seconds += time.perf_counter() - t0
+            self._graph, launches, seconds = capture_step(lambda: self._warm_up(self._static), body, self._pool)
+            self.launches_per_step = launches + (0 if capture_all else 2)
+            self.capture_seconds += seconds
         for k, v in batch.items():
             if torch.is_tensor(v):
                 self._static[k].copy_(v, non_blocking=True)
         self._graph.replay()
         if self.world > 1 and not self.graph_comm:
             self._exchange_and_update()
+        return self._loss
+
+
+class ArenaGraphStep:
+    """What the training steps of the small networks (speaker encoder, verifier and classifier, recognizer, duration
+    predictor, neural vocoder) share: clip + Adam (``FlatAdam`` over a ``ParameterArena`` of ``net``'s parameters;
+    clip_thresh None: no clipping), the ``ops.conv_math`` and ``ops.deterministic`` modes current at construction, one
+    batch shape, checkpoints of copies that resume bit-exactly, and with use_graph one CUDA graph for forward, backward
+    and update.  A subclass defines ``_objective(batch)`` (the loss to minimise, on device tensors),
+    ``_check_batch(batch)`` (ValueError before any launch) and may define ``_graph_key()`` (when it changes, the next
+    step captures a new graph).  ``step`` reads the batch keys ``_batch_keys``."""
+
+    _net_key = "net"
+    _batch_keys = ("mels", "speaker_ids")
+
+    def __init__(self, net, lr, betas, eps, clip_thresh, use_graph):
+        self.math = ops.math_mode()
+        self.deterministic = ops.is_deterministic()
+        self._det_scratch = ops.DetScratch() if self.deterministic else None
+        self.net, self.lr = net, lr
+        self.arena = ParameterArena(net, list(net.parameters()))
+        self.opt = FlatAdam(self.arena, lr, betas, eps, 0.0 if clip_thresh is None else float(clip_thresh))
+        self.use_graph = use_graph
+        self.global_step = 0
+        self._graph = self._static = self._loss = self._shape = self._captured_key = None
+        self.launches_per_step = None
+        self.graphs_captured = 0
+        self.capture_seconds = 0.0
+
+    def state_dict(self):
+        """A checkpoint of copies (the network's own state_dict holds views of the live parameter arena)."""
+        return {self._net_key: {k: v.clone() for k, v in self.net.state_dict().items()},
+                "optimizer": self.opt.state_dict(), "global_step": self.global_step}
+
+    def load_state_dict(self, ckpt):
+        """Resume bit-exactly from ``state_dict()``: parameters (in place, so captured graphs stay valid), Adam moments
+        and step count."""
+        self.net.load_state_dict(ckpt[self._net_key])
+        self.opt.load_state_dict(ckpt["optimizer"])
+        self.global_step = int(ckpt.get("global_step", 0))
+
+    def _graph_key(self):
+        return None
+
+    def _forward_backward(self, batch):
+        self.arena.zero_grad()
+        state = dict(deterministic=self.deterministic)
+        if self.deterministic:
+            state["det_scratch"] = self._det_scratch
+        with ops.overrides(**state):
+            loss = self._objective(batch)
+            loss.backward()
+            return loss.detach()
+
+    def step(self, batch):
+        """-> the batch's loss (a device scalar, valid until the next step)."""
+        name = type(self).__name__
+        if ops.math_mode() != self.math:
+            raise ValueError("%s was built with ops.conv_math = %r and cannot step under %r"
+                             % (name, self.math, ops.conv_math))
+        dev = self.arena.flat.device
+        batch = {k: batch[k] for k in self._batch_keys}
+        self._check_batch(batch)
+        shape = tuple(tuple(v.shape) for v in batch.values())
+        if self._shape is not None and shape != self._shape:
+            raise ValueError("%s batches have one shape: %s, then %s" % (name, self._shape, shape))
+        self._shape = shape
+        self.net.train()
+        self.opt.set_hyper(self.lr)
+        if not self.use_graph:
+            loss = self._forward_backward({k: v.to(dev, non_blocking=True) for k, v in batch.items()})
+            self.opt.apply()
+        else:
+            loss = self._graph_step(batch)
+        self.global_step += 1
+        return loss
+
+    def _graph_step(self, batch):
+        if self._graph is not None and self._graph_key() != self._captured_key:
+            self._graph = self._static = self._loss = None     # the captured step reads stale addresses: capture anew
+        if self._graph is None:
+            dev = self.arena.flat.device
+            self._static = {k: v.to(dev).clone() for k, v in batch.items()}
+            self._captured_key = self._graph_key()
+
+            def warm_up():                          # allocator, weight-norm buffers, deterministic scratch
+                for _ in range(2):
+                    self._forward_backward(self._static)
+
+            def body():
+                self._loss = self._forward_backward(self._static)
+                self.opt.apply()
+            self._graph, self.launches_per_step, seconds = capture_step(warm_up, body)
+            self.graphs_captured += 1
+            self.capture_seconds += seconds
+        for k, v in batch.items():
+            self._static[k].copy_(v, non_blocking=True)
+        self._graph.replay()
         return self._loss
 
 

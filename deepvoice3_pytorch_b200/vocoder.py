@@ -9,25 +9,16 @@ Griffin-Lim are (``audio.inv_spectrogram_batch(..., method=<NeuralVocoder>)`` an
 * ``vocoder_batch``: a ``data.VocoderBatches`` batch -> conditioning segments and pre-emphasised targets on the GPU.
 * ``NeuralVocoderStep``: clip + Adam over a parameter arena, one CUDA graph per batch shape, bit-exact checkpoints.
 """
-import ctypes
-
 import numpy as np
 import torch
 from torch import nn
 
 from . import audio, modules, ops
 from ._lib import lib, Dv3Error
-from .speaker_encoder import ArenaGraphStep, check_single_process
+from .ops import _p, _stream
+from .train_step import ArenaGraphStep, check_single_process
 
 DEFAULT_RESOLUTIONS = ((512, 128), (1024, 256), (2048, 512))
-
-
-def _cp(t):
-    return None if t is None else ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def check_resolutions(resolutions):
@@ -88,8 +79,8 @@ def _check_pair(y, target, lengths):
 
 def _spectra(wav, lens_d, frames_d, F, N, R, B):
     spec = torch.empty(B, F, N // 2 + 1, 2, device=wav.device)
-    lib.call("dv3_stft_complex_geom", _cp(wav), _cp(lens_d), wav.shape[1], None, _cp(spec), _cp(frames_d), F, B,
-             _cp(audio._geometry_table(wav.device, N, R)), N, R, _stream())
+    lib.call("dv3_stft_complex_geom", _p(wav), _p(lens_d), wav.shape[1], None, _p(spec), _p(frames_d), F, B,
+             _p(audio._geometry_table(wav.device, N, R)), N, R, _stream())
     return spec
 
 
@@ -107,12 +98,12 @@ def _mrstft_forward(y, target, resolutions, lengths):
         sy = _spectra(y, lens_d, frames_d, F, N, R, B)
         sx = _spectra(target, lens_d, frames_d, F, N, R, B)
         ws = torch.empty(lib.raw("dv3_mrstft_ws_doubles")(B, F), dtype=torch.float64, device=dev)
-        lib.call("dv3_mrstft_loss_fwd", _cp(sy), _cp(sx), _cp(lens_d), n, B, F, N, R, _cp(ws), _cp(stats[m]),
-                 _cp(ops._err_flag(dev)), _stream())
+        lib.call("dv3_mrstft_loss_fwd", _p(sy), _p(sx), _p(lens_d), n, B, F, N, R, _p(ws), _p(stats[m]),
+                 _p(ops._err_flag(dev)), _stream())
         saved.append((sy, sx, frames_d, F, N, R))
     loss = torch.empty((), device=dev)
     clip = torch.empty(B, dtype=torch.float64, device=dev)
-    lib.call("dv3_mrstft_loss_total", _cp(stats), M, B, _cp(clip), _cp(loss), _stream())
+    lib.call("dv3_mrstft_loss_total", _p(stats), M, B, _p(clip), _p(loss), _stream())
     return loss, clip, (stats, lens_d, saved)
 
 
@@ -123,10 +114,10 @@ def _mrstft_backward(d_loss, state, B, n, dev, adjoint=1):
     dy = torch.zeros(B, n, device=dev)
     for m, (sy, sx, frames_d, F, N, R) in enumerate(saved):
         dspec = torch.empty_like(sy)
-        lib.call("dv3_mrstft_loss_bwd", _cp(sy), _cp(sx), _cp(stats[m]), B, F, N, R, M, _cp(d_loss), adjoint,
-                 _cp(dspec), _stream())
-        lib.call("dv3_istft_geom", _cp(dspec), _cp(dy), _cp(lens_d), n, _cp(frames_d), F, B,
-                 _cp(audio._geometry_table(dev, N, R)), N, R, _stream())
+        lib.call("dv3_mrstft_loss_bwd", _p(sy), _p(sx), _p(stats[m]), B, F, N, R, M, _p(d_loss), adjoint,
+                 _p(dspec), _stream())
+        lib.call("dv3_istft_geom", _p(dspec), _p(dy), _p(lens_d), n, _p(frames_d), F, B,
+                 _p(audio._geometry_table(dev, N, R)), N, R, _stream())
     return dy
 
 
@@ -287,15 +278,15 @@ def vocoder_batch(batch, seg_frames, device="cuda"):
     lin, _ = audio.stft_mel_batch(wav, ints[:B], want_linear=True, want_mel=False)
     cond = torch.empty(B, g.bins, S, device=dev)
     target = torch.empty(B, S * g.hop, device=dev)
-    lib.call("dv3_vocoder_gather", _cp(lin), lin.shape[1], _cp(ints[B:2 * B]), _cp(wav), pitch, _cp(ints[:B]),
-             _cp(ints[2 * B:]), B, S, g.n_fft, g.hop, float(audio.hparams.preemphasis), _cp(cond), _cp(target),
-             _cp(ops._err_flag(dev)), _stream())
+    lib.call("dv3_vocoder_gather", _p(lin), lin.shape[1], _p(ints[B:2 * B]), _p(wav), pitch, _p(ints[:B]),
+             _p(ints[2 * B:]), B, S, g.n_fft, g.hop, float(audio.hparams.preemphasis), _p(cond), _p(target),
+             _p(ops._err_flag(dev)), _stream())
     return {"cond": cond, "target": target}
 
 
 class NeuralVocoderStep(ArenaGraphStep):
     """One training step of a NeuralVocoder: ``stft_loss(vocoder(cond), target, resolutions)``, then clip + Adam
-    (``speaker_encoder.ArenaGraphStep``: the conv_math and deterministic modes of construction, one batch shape,
+    (``train_step.ArenaGraphStep``: the conv_math and deterministic modes of construction, one batch shape,
     checkpoints that resume bit-exactly, and with use_graph one CUDA graph for forward, backward and update).
     ``step(batch)`` takes ``vocoder_batch``'s {"cond" (B, K, S), "target" (B, S * R)}.  Single process only.
     ValueError before any launch for a world size above 1, bad resolutions or a malformed batch."""

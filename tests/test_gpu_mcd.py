@@ -48,6 +48,7 @@ def test_cepstra_against_the_fp64_oracle(M, K):
 def test_cepstra_read_no_frame_past_a_count_and_write_zeros_there():
     from deepvoice3_pytorch_b200 import mcd
     from deepvoice3_pytorch_b200._lib import lib
+    from deepvoice3_pytorch_b200.ops import _p, _stream
     M, K, T = 80, 24, 40
     rng = np.random.RandomState(2)
     mels = torch.from_numpy(rng.rand(3, T, M).astype(np.float32)).cuda()
@@ -56,8 +57,8 @@ def test_cepstra_read_no_frame_past_a_count_and_write_zeros_there():
         mels[q, n:] = float("nan")
     cep = torch.full((3, T, K), 7.0, device="cuda")
     lens = torch.tensor(lengths, dtype=torch.int32, device="cuda")
-    lib.call("dv3_mel_cepstra", mcd._p(mels), mcd._p(lens), mcd._p(mcd._device_basis(mels.device, M, K)), mcd._p(cep),
-             3, T, M, K, mcd._stream())
+    lib.call("dv3_mel_cepstra", _p(mels), _p(lens), _p(mcd._device_basis(mels.device, M, K)), _p(cep),
+             3, T, M, K, _stream())
     alone = mcd.mel_cepstra([mels[q, :n] for q, n in enumerate(lengths)], K)
     for q, n in enumerate(lengths):
         assert torch.equal(cep[q, :n], alone[q])

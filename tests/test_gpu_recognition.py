@@ -58,7 +58,7 @@ def _ctc_abi(z, frames, targets, tlen, scale=None):
     """nll, partials, infeasible and dz of one fwd + bwd through the C ABI (d_loss = 1, scale default 1 / B)."""
     from deepvoice3_pytorch_b200 import ops
     from deepvoice3_pytorch_b200._lib import lib
-    from deepvoice3_pytorch_b200.recognition import _p, _stream
+    from deepvoice3_pytorch_b200.ops import _p, _stream
     B, V, T = z.shape
     L = targets.shape[1]
     dev = z.device

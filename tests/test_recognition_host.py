@@ -167,7 +167,8 @@ def test_ptxas_no_spills_zero_stack():
 def test_arena_graph_steps_read_their_keys():
     from deepvoice3_pytorch_b200.recognition import TokenRecognizerStep
     from deepvoice3_pytorch_b200.speaker_classifier import SpeakerClassifierStep
-    from deepvoice3_pytorch_b200.speaker_encoder import ArenaGraphStep, SpeakerEncoderStep
+    from deepvoice3_pytorch_b200.speaker_encoder import SpeakerEncoderStep
+    from deepvoice3_pytorch_b200.train_step import ArenaGraphStep
     from deepvoice3_pytorch_b200.speaker_verifier import SpeakerVerifierStep
     assert ArenaGraphStep._batch_keys == ("mels", "speaker_ids")
     for cls in (SpeakerEncoderStep, SpeakerVerifierStep, SpeakerClassifierStep):

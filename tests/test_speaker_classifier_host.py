@@ -208,8 +208,8 @@ def test_step_refusals(no_lib, monkeypatch):
                     (torch.zeros(2, 0, 10, 8), ids)):
         with pytest.raises(ValueError):
             step.step({"mels": mels, "speaker_ids": i})
-    monkeypatch.setattr(SE.dist, "is_initialized", lambda: True)
-    monkeypatch.setattr(SE.dist, "get_world_size", lambda: 2)
+    monkeypatch.setattr(torch.distributed, "is_initialized", lambda: True)
+    monkeypatch.setattr(torch.distributed, "get_world_size", lambda: 2)
     with pytest.raises(ValueError):
         SpeakerClassifierStep(cl)
     assert no_lib == []

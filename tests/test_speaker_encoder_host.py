@@ -233,8 +233,8 @@ def test_encoder_step_refusals(no_lib, monkeypatch):
                                 max_positions=64)
     with pytest.raises(ValueError):
         SE.SpeakerEncoderStep(enc, single)
-    monkeypatch.setattr(SE.dist, "is_initialized", lambda: True)
-    monkeypatch.setattr(SE.dist, "get_world_size", lambda: 2)
+    monkeypatch.setattr(torch.distributed, "is_initialized", lambda: True)
+    monkeypatch.setattr(torch.distributed, "get_world_size", lambda: 2)
     with pytest.raises(ValueError):
         SE.SpeakerEncoderStep(enc, _ms_model())
     assert no_lib == []
